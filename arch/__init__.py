@@ -1,1 +1,1 @@
-"""Reference package name (arch/) -> B200 implementations."""
+"""Reference package name (arch/) -> CUDA implementations."""

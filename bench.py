@@ -9,8 +9,8 @@ the metric is quoted on at one GPU:
   c1  Llama 2M    AdamW    fp32   B16 x S1024                     (plumbing / loss parity config)
   c2  Llama "80M" Muon     bf16   B16 x S1024   V = 32003         <- default, `value`
   c3  Llama 400M  Muon     bf16   B16 x S2048 x 8 accumulation micro-batches, clip 1.0
-  c4  Llama 256M  Shampoo  bf16   B64 x S2048   roots every 100 steps (the timed region contains one recompute)
-  c5  Llama 1B    AdamW    bf16   B32 x S2048   D = 128
+  c4  Llama 256M  Shampoo  bf16   B16 x S2048 x 4 micro-batches, roots every 100 steps (the timed region contains one recompute)
+  c5  Llama 1B    AdamW    bf16   B16 x S2048 x 2 micro-batches, D = 128
 A "step" = ONE OPTIMIZER UPDATE: `gradient_accumulation_steps` x (fwd + bwd + clamp/accumulate) + gradient
 all-reduce (N > 1) + the full optimizer update.  Weak scaling: per-GPU batch fixed.  One JSON line (rank 0).
 
@@ -26,15 +26,18 @@ Keys beyond the base contract:
   dp_check      (N > 1) replicas bit-identical after the timed loop; one update through every exchange
                 implementation (peer-store unicast / NVSwitch multicast / NCCL all-gather) compared
 --impl reference times the reference's CPU path (the oracle port: MLX is not installable here).
+--dump-outputs DIR writes, after the timed steps, what the last timed step produced (see dump_outputs).
 """
 from __future__ import annotations
 
 import argparse
 import json
 import os
+import shutil
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 from pathlib import Path
@@ -113,7 +116,7 @@ def attn_bytes_per_step(c: dict):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
 
     def __init__(self, gpu_index: int):
         self.rows = []
@@ -162,14 +165,17 @@ class ClockSampler:
                 "power_w_max": max(pw) if pw else None, "samples": len(sm), "reasons": sorted(reasons)}
 
 
+# NVIDIA H100 SXM data sheet (700 W): dense bf16 989 TFLOP/s, HBM3 3.35 TB/s.  Not reached figures, only the
+# denominators of the frac_* keys; a card set to a lower power limit clocks lower under sustained load.
+H100_DATASHEET = {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0}
+
+
 def load_peaks() -> dict:
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
         d = json.loads(p.read_text())
-        return {"bf16_tflops": d.get("bf16_tflops", 1590.0), "bf16_tflops_sustained": d.get("bf16_tflops_sustained", 1400.0),
-                "hbm_gbs": d.get("hbm_gbs", 6650.0), "source": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "fallback (B200_PROFILING.md)"}
+        return {**{k: d.get(k, v) for k, v in H100_DATASHEET.items()}, "source": "measured (MEASURED_PEAKS.json)"}
+    return {**H100_DATASHEET, "source": "NVIDIA H100 SXM data sheet, dense bf16 at 700 W (not measured)"}
 
 
 # ------------------------------------------------------------------------------------------------
@@ -178,9 +184,8 @@ def load_peaks() -> dict:
 def pick_cpu_threads(c: dict) -> int:
     """Thread count for the CPU arm: the fastest of n, n/2, n/4, n/8 host threads on a probe of the workload itself
     -- fwd+bwd of ONE sequence through a 2-layer cut of the config's model (same widths, seq <= 1024) -- because the
-    oracle's step mixes GEMMs with memory-bound elementwise work and a plain matmul probe picked 64 threads on a box
-    where 32 ran the real step 1.4x faster (profiles/r03_bench_c2.json vs r03_bench_reference.json).  The choice is
-    reported in cpu_baseline.cores."""
+    oracle's step mixes GEMMs with memory-bound elementwise work, and a plain matmul probe can pick a thread count
+    that runs the real step slower.  The choice is reported in cpu_baseline.cores."""
     from oracle import reference_math as R
     n = os.cpu_count() or 1
     cand = sorted({n, max(1, n // 2), max(1, n // 4), max(1, n // 8)}, reverse=True)
@@ -297,14 +302,37 @@ def run_reference(args) -> None:
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------
 def master_fingerprint(store) -> torch.Tensor:
     """Order-independent but bit-sensitive checksum of the fp32 masters: sum of the raw bit patterns (int64)."""
     return store.master.view(torch.int32).to(torch.int64).sum().reshape(1)
 
 
-def run_workload(tag: str, K: int, W: int, with_e2e: bool = True, with_dp_check: bool = True) -> dict:
+DUMP_SAMPLE = 4 << 20  # parameters sampled into params_sample.npy (16 MB of float32)
+
+
+def dump_outputs(out_dir: str, tr, loss) -> None:
+    """What a caller of the timed step receives: the loss of the last update and the updated fp32 parameters.  The
+    parameters are a fixed, seeded sample of DUMP_SAMPLE positions of the flat master buffer (the same positions on
+    every run of the same config), so two builds can be compared output for output within 64 MB."""
+    import numpy as np
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    master = tr.store.master.detach()
+    n = master.numel()
+    if n > DUMP_SAMPLE:
+        idx = torch.randint(0, n, (DUMP_SAMPLE,), generator=torch.Generator().manual_seed(1234)).sort().values
+        np.save(d / "params_sample_index.npy", idx.numpy().astype(np.float64))
+        sample = master[idx.to(master.device)]
+    else:
+        sample = master
+    np.save(d / "params_sample.npy", sample.float().cpu().numpy())
+    np.save(d / "loss.npy", np.asarray([float(loss.item())], dtype=np.float32))
+
+
+def run_workload(tag: str, K: int, W: int, with_e2e: bool = True, with_dp_check: bool = True,
+                 dump_dir: str | None = None) -> dict:
     from mlx_cuda_distributed_pretraining_b200 import ops
     from mlx_cuda_distributed_pretraining_b200._lib import lib
     from mlx_cuda_distributed_pretraining_b200.core.training import Config, Trainer
@@ -315,7 +343,8 @@ def run_workload(tag: str, K: int, W: int, with_e2e: bool = True, with_dp_check:
     c = dims_of(d)
     k = c["accum"]
     d["training"]["hyperparameters"]["iters"] = max(d["training"]["hyperparameters"].get("iters", 0), (2 * (K + W) + 8) * k)
-    tr = Trainer(Config.from_dict(d), synthetic=True, quiet=True, run_root=str(ROOT / "gpurun_out" / "bench_runs"))
+    run_root = tempfile.mkdtemp(prefix="bench_runs_")   # the tree may be read-only: run files go to a temp dir
+    tr = Trainer(Config.from_dict(d), synthetic=True, quiet=True, run_root=run_root)
     tr._accum_step, tr._accum_tokens = 0, 0
     dev = tr.device
     tokens_per_step = c["batch"] * c["seq"] * k * world
@@ -375,6 +404,8 @@ def run_workload(tag: str, K: int, W: int, with_e2e: bool = True, with_dp_check:
     ops.TIMER = None
     clocks = sampler.stop() if rank == 0 else {}
     final_loss = float(loss.item())
+    if dump_dir is not None and rank == 0:
+        dump_outputs(dump_dir, tr, loss)
     ms_per_step = ms_total / K
     value = tokens_per_step / (ms_per_step / 1e3)
 
@@ -506,8 +537,8 @@ def run_workload(tag: str, K: int, W: int, with_e2e: bool = True, with_dp_check:
                    "of every rank's updates (2 bytes x all matrix parameters into each rank per step)")
             if tf_r[slow] > 1.15 * share:
                 why = (f"this rank's largest matrix is one indivisible chain above the per-rank share of {share:.2f} TFLOP "
-                       "(C2 at 8 ranks: the 32003 x 1024 embedding, 0.68 TFLOP, 0.65 ms when timed alone on an idle GPU: "
-                       "tools/ns_single_probe.py), and its last GEMM's peer stores share NVLink with the all-gather of "
+                       "(C2 at 8 ranks: the 32003 x 1024 embedding, 0.68 TFLOP), and its last GEMM's peer stores share "
+                       "NVLink with the all-gather of "
                        "every rank's updates (2 bytes x all matrix parameters into each rank per step)")
             out["ns_ranks"] = {
                 "ns_ms_per_rank": [round(x, 3) for x in ms_r], "ns_tflop_per_rank": [round(x, 3) for x in tf_r],
@@ -516,6 +547,7 @@ def run_workload(tag: str, K: int, W: int, with_e2e: bool = True, with_dp_check:
                             f"{(sum(ms_r) - ms_r[slow]) / max(1, world - 1):.2f} ms); " + why)}
     del tr
     torch.cuda.empty_cache()
+    shutil.rmtree(run_root, ignore_errors=True)
     return out
 
 
@@ -543,16 +575,9 @@ def summarize(r: dict, peaks: dict) -> dict:
     if ns_ms > 0 and "ns_flops_rank" in r:
         ns_step = ns_ms / K
         tf = r["ns_flops_rank"] / (ns_step * 1e-3) / 1e12
-        traffic, traffic_src = None, None
-        for tf_path in sorted(ROOT.glob("profiles/*_gemm_traffic.json")):   # written by tools/summarize_profiles.py
-            try:
-                traffic = float(json.loads(tf_path.read_text())["mean_dram_bytes_per_launch"])
-                traffic_src = f"{tf_path.relative_to(ROOT)} (ncu --set full, mean DRAM read+write bytes per launch)"
-            except Exception:  # noqa: BLE001
-                pass
-        roofline = {"kernel": "gemm2_bf16_tc_kernel (Newton-Schulz chain: batched tcgen05 cta_group::2 GEMMs)",
+        roofline = {"kernel": "gemm_wgmma_kernel (Newton-Schulz chain: batched wgmma GEMMs)",
                     "bound": "tensor", "achieved": tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": tf / peak_tf,
-                    "traffic": traffic, "traffic_source": traffic_src,
+                    "traffic": None,
                     "peak_source": peaks["source"] + ", sustained bf16 (kernel timed inside a long step)",
                     "frac_of_burst": tf / peak_burst, "algorithmic_flops_per_step": r["ns_flops_rank"],
                     "algorithmic_flops_all_ranks": ns_flops_per_step(c), "ns_sharded_over_ranks": r["ns_sharded"],
@@ -561,7 +586,7 @@ def summarize(r: dict, peaks: dict) -> dict:
             roofline.update(r["ns_ranks"])
     elif "attn_bwd" in kernels:
         kb = kernels["attn_bwd"]
-        roofline = {"kernel": "attn_bwd (fused causal/GQA attention backward, tcgen05; 2.5 x 4BHS^2D flops, full count)",
+        roofline = {"kernel": "attn_bwd (fused causal/GQA attention backward, mma.sync; 2.5 x 4BHS^2D flops, full count)",
                     "bound": "tensor", "achieved": kb["tflops_full_count"], "peak": peak_tf, "unit": "TFLOP/s",
                     "frac": kb["frac_of_tensor_peak"], "frac_of_burst": kb["frac_of_tensor_peak_burst"], "traffic": None,
                     "peak_source": peaks["source"] + ", sustained bf16 (kernel timed inside a long step)",
@@ -580,6 +605,9 @@ def main() -> None:
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs-block", action="store_true", help="skip the extra C3 single-GPU leg of the default run")
     ap.add_argument("--no-e2e", action="store_true", help="profiling runs: only the device-resident leg")
+    ap.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                    help="after the timed steps, write the last step's loss and a seeded sample of the updated "
+                         "parameters as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)
@@ -591,7 +619,7 @@ def main() -> None:
     if world != args.gpus and world > 1:
         raise SystemExit(f"--gpus {args.gpus} but WORLD_SIZE={world}")
     tag = args.config
-    r = run_workload(tag, args.steps, args.warmup, with_e2e=not args.no_e2e)
+    r = run_workload(tag, args.steps, args.warmup, with_e2e=not args.no_e2e, dump_dir=args.dump_outputs)
     extra = None
     if world == 1 and tag == "c2" and not args.no_configs_block:
         extra = run_workload("c3", max(2, min(args.steps, 4)), 3, with_e2e=False)
@@ -608,7 +636,7 @@ def main() -> None:
         "scaling": "weak", "vs_baseline": None, "dtype": "bf16" if c["mixed"] else "f32", "data": "synthetic",
         "config": {"workload": workload_name(tag, c), "global_batch": c["batch"] * world, "seq_len": c["seq"],
                    "micro_batches_per_step": c["accum"], "parallelism": f"dp{world}",
-                   "l2": "working set (params+grads+activations, GBs) >> 126 MB L2"},
+                   "l2": "working set (params+grads+activations, GBs) >> 50 MB L2"},
         "e2e": r["e2e"], "gpu_launches": r["launches"], "host_issue_ms_per_step": r["host_issue_ms"], "clocks": r["clocks"], "roofline": s["roofline"],
         "kernels": s["kernels"], "final_loss": r["final_loss"],
     }

@@ -1,1 +1,1 @@
-"""Drop-in shim: `python -m core.training --config <yaml>` resolves to the B200 hot path."""
+"""Drop-in shim: `python -m core.training --config <yaml>` resolves to the CUDA hot path."""

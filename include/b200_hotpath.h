@@ -1,5 +1,5 @@
 /*
- * b200_hotpath.h -- C ABI of the B200-native training-step hot path.
+ * b200_hotpath.h -- C ABI of the CUDA-native (H100, sm_90a) training-step hot path.
  *
  * The reference (arthurcolle/mlx-cuda-distributed-pretraining) has no native code and no FFI: its
  * hot path is Python over mlx.core ops.  This header is therefore the boundary a maintainer would
@@ -30,19 +30,19 @@ extern "C" {
 /* ---- library / device ---------------------------------------------------------------------- */
 int b200_version(void);                 /* ABI version (monotonic integer) */
 const char* b200_last_error(void);      /* thread-local message of the last failing call */
-int b200_device_ok(void);               /* 1 if the current device is compute capability 10.x */
+int b200_device_ok(void);               /* 1 if the current device is compute capability 9.0 */
 unsigned long long b200_launch_count(void); /* kernels launched by this library so far (process-wide) */
 /* TMA descriptors are cached per (address, shape, strides, box): calls answered from the cache / encoded by the driver */
 void b200_tensor_map_cache_stats(unsigned long long* hits, unsigned long long* misses);
 
-/* ---- dense contraction engine (tcgen05 + TMA) ----------------------------------------------
+/* ---- dense contraction engine (wgmma + TMA) ----------------------------------------------
  * D[b] = alpha*alpha_vec[b] * op(A[b]) op(B[b]) + beta*beta_vec[b] * C[b],  b in [0,batch)
  * replaces: `@` / mx.matmul in optimizers/muon.py:76-78, optimizers/shampoo.py:121,250,254,287-290
  * a_mn=0: A is [M,K] row-major (K-major);  a_mn=1: A is stored [K,M] row-major (MN-major)
  * b_mn=0: B is [N,K] row-major (K-major);  b_mn=1: B is stored [K,N] row-major (MN-major)
- * A,B bf16; C,D bf16 (out_f32=0) or f32 (out_f32=1); accumulate fp32 in TMEM.
+ * A,B bf16; C,D bf16 (out_f32=0) or f32 (out_f32=1); accumulate fp32.
  * alpha_vec/beta_vec: optional per-batch device scalars (NULL = 1).
- * force_bn: 0 auto | 128 | 256 tile width | 1256 = 256-wide tiles and the caller asserts D == D^T
+ * force_bn: 0 | 128 | 256 (tile-width hints; tiles are 128 x 128) | 1256 = the caller asserts D == D^T
  * (M == N, bf16 out): only tiles on/above the diagonal are computed, the rest mirror-written.
  * lda/ldb/ldd/ldc multiples of 8 (bf16) / 4 (f32 C,D).  M, K arbitrary (TMA zero-fills); N arbitrary too if
  * ldd/ldc >= round_up(N, 16 bytes): the padded tail columns of D are then written with alpha*0 + beta*C.
@@ -81,7 +81,7 @@ int b200_newton_schulz_allgather(const void* x_in, void* x_out, int batch, int r
  * replicas that hold identical gradients compute bit-identical norms and stay bit-identical. */
 size_t b200_reduce_workspace_bytes(int batch);
 /* Whole-model chain: all shape groups of the optimizer advance through the iteration together and every stage
- * (A = X X^T | B = bA + cAA | X' = aX + BX) is ONE grouped tcgen05 launch over all groups -- 3 launches per
+ * (A = X X^T | B = bA + cAA | X' = aX + BX) is ONE grouped wgmma launch over all groups -- 3 launches per
  * iteration instead of 3 per group (muon.py:91 loops over parameters).  Per group the arguments mean what they
  * mean in b200_newton_schulz / _allgather; n_groups <= 6 takes the grouped path (each group min(rows, cols) > 128),
  * anything else falls back to per-group chains.  Results are identical to per-group calls up to the fp32
@@ -221,7 +221,7 @@ int b200_rope(const void* x, void* y, const float* cos_t, const float* sin_t, in
  * arch/llama.py:142-151: down( gate(x) * sigmoid(up(x)) * 2 ).  gate_proj.weight and up_proj.weight must be
  * adjacent in memory (W2 = [Wg ; Wu], [2I, K] row-major; flat.ParamStore lays them out that way).
  * b200_mlp_gateup_glu_fwd:  gu[M, 2I] = x[M, K] W2^T  (columns [0, I) = gate(x), [I, 2I) = up(x)),
- *                           y[M, I] = gate * sigmoid(up) * 2 from the fp32 accumulators -- one tcgen05 kernel,
+ *                           y[M, I] = gate * sigmoid(up) * 2 from the fp32 accumulators -- one wgmma kernel,
  *                           no separate activation pass.  K % 8 == 0, I % 128 == 0.
  * b200_mlp_down_glu_bwd:    d = dy[M, H] Wd (dgrad of down_proj, Wd = down_proj.weight [H, I]) never leaves the
  *                           chip: dgu[M, 2I] = [ d * sigmoid(u) * 2 | d * g * sigmoid(u) * (1 - sigmoid(u)) * 2 ]

@@ -1,4 +1,4 @@
-"""B200-native hot path of arthurcolle/mlx-cuda-distributed-pretraining (see DESIGN.md).
+"""H100-native (sm_90a) hot path of arthurcolle/mlx-cuda-distributed-pretraining (see DESIGN.md).
 
 Importing the package is cheap and GPU-free; the C-ABI library is loaded on first use
 (`_lib.lib()`), and every op raises if it is missing -- there is no CPU fallback.

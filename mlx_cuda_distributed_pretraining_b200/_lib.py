@@ -101,7 +101,7 @@ def lib() -> C.CDLL:
         path = Path(os.environ.get("B200_HOTPATH_LIB", LIB_PATH))
         if not path.exists():
             raise B200Error(
-                f"{path} not found: run `python __graft_entry__.py` (nvcc, sm_100a) first. "
+                f"{path} not found: run `python __graft_entry__.py` (nvcc, sm_90a) first. "
                 "There is no CPU fallback for the hot path.")
         handle = C.CDLL(str(path))
         for name, (res, args) in SIGNATURES.items():
@@ -119,9 +119,9 @@ def check(rc: int, what: str) -> None:
 
 
 def require_device() -> None:
-    """Fail loudly when the CUDA path cannot run (no GPU / not an sm_100 part)."""
+    """Fail loudly when the CUDA path cannot run (no GPU / not an sm_90 part)."""
     import torch
     if not torch.cuda.is_available():
-        raise B200Error("CUDA device required: the B200 hot path has no CPU fallback")
+        raise B200Error("CUDA device required: the hot path has no CPU fallback")
     if not lib().b200_device_ok():
-        raise B200Error("the current CUDA device is not compute capability 10.x (B200)")
+        raise B200Error("the current CUDA device is not compute capability 9.0 (H100)")

@@ -1,8 +1,8 @@
 """FlashAttention module with the reference's constructor and call surface
-(arch/flash_attention.py:32-41,158-194), running the fused sm_100a kernels.
+(arch/flash_attention.py:32-41,158-194), running the fused sm_90a kernels.
 
 The reference materialises softmax(QK^T*scale + mask)V un-tiled (:97-156); here the same result
-comes from `ops.attention` (tcgen05 forward + backward, online softmax, GQA head sharing).
+comes from `ops.attention` (tensor-core forward + backward, online softmax, GQA head sharing).
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 """Llama-style decoder with the reference's structure and parameter names (arch/llama.py), hosted
-on PyTorch modules whose hot ops are the sm_100a kernels:
+on PyTorch modules whose hot ops are the sm_90a kernels:
 
   RMSNorm            arch/llama.py:44-56   -> ops.rmsnorm (fused fwd/bwd)
   MLP                arch/llama.py:142-151 -> down(gate(x) * sigmoid(up(x)) * 2)  (sic, SURVEY D7)

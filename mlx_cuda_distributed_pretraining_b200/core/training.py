@@ -1,5 +1,5 @@
 """`python -m core.training --config <yaml>` -- the reference's entry point (core/training.py),
-re-hosted on the B200 hot path.
+re-hosted on the CUDA hot path (H100).
 
 Kept from the reference: the YAML schema (dataclasses core/training.py:52-138), `Config.from_yaml`
 (:141-167), the byte-level / tokenizers-JSON `TokenizerManager` (:324-440), JSONL chunking
@@ -8,7 +8,7 @@ factory names (:787-896), `compute_loss` (:1195-1234), the hot loop's order of o
 (:1637-1768: fwd/bwd -> fp32 grads -> elementwise clip -> accumulate -> optimizer.update),
 the `Step n: k=v | ...` log line (:257-271) and the three-file checkpoint layout (:1347-1394).
 
-Replaced: mlx arrays/autograd -> PyTorch autograd over the sm_100a kernels; the thread-queue
+Replaced: mlx arrays/autograd -> PyTorch autograd over the sm_90a kernels; the thread-queue
 "devices" (distributed/utils.py) -> one process per GPU with an NCCL all-reduce of the flat
 gradient buffer, engaged only when `system.distributed: true` and the job runs under torchrun.
 
@@ -854,7 +854,7 @@ def train(config, **trainer_kwargs) -> Dict[str, Any]:
 
 
 def main(argv: Optional[List[str]] = None) -> None:
-    ap = argparse.ArgumentParser(description="Train a language model on the B200 hot path")
+    ap = argparse.ArgumentParser(description="Train a language model on the CUDA hot path")
     ap.add_argument("--config", type=str, required=True, help="Path to YAML config file")
     ap.add_argument("--mixed-precision", action="store_true")
     ap.add_argument("--precision", type=str, default=None, choices=["float16", "bfloat16"])

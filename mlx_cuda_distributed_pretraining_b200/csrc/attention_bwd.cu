@@ -1,381 +1,240 @@
-// Fused causal / GQA attention backward on tcgen05 (sm_100a): the adjoint the reference obtains
-// from MLX autograd of arch/flash_attention.py:123-151 (core/training.py:1580,1650), including
-// the sum of dK/dV over the query heads that share a kv head (adjoint of mx.repeat, :107-120).
+// Fused causal / GQA attention backward on Hopper warpgroup MMA (wgmma) fed by TMA through mbarriers: the adjoint
+// the reference obtains from MLX autograd of arch/flash_attention.py:123-151 (core/training.py:1580,1650),
+// including the sum of dK/dV over the query heads that share a kv head (adjoint of mx.repeat, :107-120).
 //
-//   delta = rowsum(dO * O)                                  (pre-pass kernel)
-//   per (kv tile, kv head, batch) CTA, looping over the group's query heads and query tiles:
-//     S^T  = K Q^T          P^T  = exp2(S^T * scale*log2e - LSE*log2e)         (keys on TMEM lanes)
-//     dP^T = V dO^T         dS^T = P^T * (dP^T - delta) * scale
-//     dV  += P^T dO         dK  += dS^T Q          dQ_tile = dS K  -> fp32 red.global into dq_acc
-//   dq_acc (fp32) -> dq (bf16)                               (post-pass kernel)
-//
-// Working transposed puts keys on the 128 TMEM lanes, so P^T / dS^T rows are written by their
-// owning thread straight into K-major swizzled smem tiles that feed the dV / dK MMAs, and the
-// same dS^T tile is read as an MN-major A operand for dQ -- no smem transposes anywhere.
-// Warp roles: warp 0 TMA, warp 1 MMA issue, warps 2-9 (two warpgroups, half the columns each)
-// softmax / dQ drain / dK,dV epilogue.
-#include <stdlib.h>
-
+//   delta = rowsum(dO * O)                                  (pre-pass kernel, also zeroes the dQ accumulator)
+//   per (128-key tile, kv head, batch) CTA, 256 threads: thread 0 loads K / V once by TMA and prefetches the Q / dO tiles
+//   (64 queries) of every query head of the GQA group one item ahead through a 2-stage ring; warpgroups 0-1 own 64 keys
+//   each (a separate producer warp would cap the MMA warpgroups at 168 registers and make them spill):
+//     S^T  = K Q^T , dP^T = V dO^T          wgmma, both operands K-major in shared memory
+//     P^T  = exp2(S^T * scale*log2e - LSE*log2e),  dS^T = P^T * (dP^T - delta)      (registers)
+//     dV  += P^T dO , dK += dS^T Q          wgmma with P^T / dS^T as register A operands, dO / Q MN-major in smem
+//     dS^T -> shared memory (the 128B-swizzled MN-major layout wgmma reads), then dQ_tile = dS K as wgmma with
+//     both operands MN-major, added into the fp32 dq_acc with atomics
+//   dq_acc (fp32) * scale -> dq (bf16)                       (post-pass kernel)
+// dK and dQ leave the softmax scale out of dS and apply it once at the end.
 #include "common.cuh"
 #include "host.h"
 
 namespace b200 {
 
-int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, int D, int box_rows,
-                  bool f32);
-int launch_attn_bwd64(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                      const CUtensorMap& tmDO, const float* lse, const float* delta, float* dq_acc, void* dk,
-                      void* dv, int B, int S, int H, int Hk, int dkv_row_heads, float scale, int causal,
-                      cudaStream_t stream);
-
-int launch_attn_bwd128(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                       const CUtensorMap& tmDO, const float* lse, const float* delta, float* dq_acc, void* dk,
-                       void* dv, int B, int S, int H, int Hk, int dkv_row_heads, float scale, int causal,
-                       cudaStream_t stream);
+int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, int D, int box_rows);
 
 namespace {
 
-constexpr int BWD_THREADS = 320;  // warp 0 TMA, warp 1 MMA, warps 2-9: two softmax warpgroups
-constexpr int BT = 128;  // tile size along both queries and keys
+constexpr int BWD_THREADS = 256;  // two MMA warpgroups; thread 0 also issues the TMA loads
+constexpr int BKV = 128;          // keys per CTA (64 per warpgroup)
+constexpr int BQ = 64;            // queries per inner tile
+constexpr float kLog2e = 1.4426950408889634f;
 
 template <int D>
 struct BwdCfg {
-  static constexpr int ST = (D == 64) ? 2 : 1;      // Q/dO stages
-  static constexpr bool ALIAS_DQ = (D == 128);      // dQ accumulator reuses the S^T columns
-  static constexpr int TILE_BYTES = 128 * D * 2;
-  static constexpr int PT_BYTES = 128 * 128 * 2;
+  static constexpr int NB = D / 64;                // 64-column (128-byte) blocks per row
+  static constexpr int KV_BYTES = BKV * D * 2;     // K or V
+  static constexpr int QS_BYTES = BQ * D * 2;      // one Q or dO stage
   static constexpr int OFF_K = 0;
-  static constexpr int OFF_V = OFF_K + TILE_BYTES;
-  static constexpr int OFF_Q = OFF_V + TILE_BYTES;
-  static constexpr int OFF_DO = OFF_Q + ST * TILE_BYTES;
-  static constexpr int OFF_PT = OFF_DO + ST * TILE_BYTES;
-  static constexpr int OFF_DS = OFF_PT + PT_BYTES;
-  static constexpr int OFF_LSE = OFF_DS + PT_BYTES;  // 2 slots x (128 lse + 128 delta) floats
-  static constexpr int OFF_BAR = OFF_LSE + 2 * 2 * 128 * 4;
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static constexpr int TM_S = 0, TM_DP = 128, TM_DV = 256, TM_DK = 256 + D;
-  static constexpr int TM_DQ = ALIAS_DQ ? 0 : 256 + 2 * D;
-  static constexpr int TMEM_COLS = 512;
+  static constexpr int OFF_V = OFF_K + KV_BYTES;
+  static constexpr int OFF_Q = OFF_V + KV_BYTES;        // 2 stages
+  static constexpr int OFF_DO = OFF_Q + 2 * QS_BYTES;   // 2 stages
+  static constexpr int OFF_DS = OFF_DO + 2 * QS_BYTES;  // dS^T [128 keys][64 queries] bf16
+  static constexpr int OFF_BAR = OFF_DS + BKV * BQ * 2;
+  static constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;
 };
 
 struct BwdArgs {
   const float* lse;    // [B,H,S]
   const float* delta;  // [B,H,S]
   float* dq_acc;       // [B,S,H,D] fp32
-  __nv_bfloat16* dk;   // [B,S,Hk,D] rows of dkv_rh heads
+  __nv_bfloat16* dk;   // [B,S,dkv_rh,D]-strided rows
   __nv_bfloat16* dv;
   int B, S, H, Hk;
   int dkv_rh;          // heads per dk/dv token row (>= Hk)
   float scale;
   int causal;
-  long long* trace;  // optional clock64 trace of CTA 0 (debug; nullptr in production)
 };
 
-#define BWD_TRACE(slot)                                                                   \
-  do {                                                                                    \
-    if (p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && it < 16) \
-      p.trace[it * 16 + (slot)] = clock64();                                              \
-  } while (0)
-
-__device__ __forceinline__ float ex2(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c),
-               "f"(d)
-               : "memory");
-}
-
-// store 8 bf16 (one 16-byte chunk) of row `row`, logical column chunk `chunk` (0..15) of a
-// [128 x 128] K-major tile made of two 64-column blocks with 128-byte swizzle
-__device__ __forceinline__ void st_tile_chunk(uint32_t tile, int row, int chunk, const float* f) {
-  const uint32_t addr = tile + (chunk >> 3) * 16384 + row * 128 + (((chunk & 7) ^ (row & 7)) << 4);
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pack_bf16x2(f[0], f[1])),
-               "r"(pack_bf16x2(f[2], f[3])), "r"(pack_bf16x2(f[4], f[5])),
-               "r"(pack_bf16x2(f[6], f[7]))
-               : "memory");
+template <int D>
+__device__ __forceinline__ void rs_mma(float* acc, const uint32_t* a, uint64_t db) {
+  if constexpr (D == 128) wgmma_m64n128k16_rs<1>(acc, a, db);
+  else wgmma_m64n64k16_rs<1>(acc, a, db);
 }
 
 template <int D>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
-                const BwdArgs p) {
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO, const BwdArgs p) {
   using Cfg = BwdCfg<D>;
-  constexpr int ST = Cfg::ST;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* sgen = smem_raw + (sbase - smem_u32(smem_raw));  // generic pointer to the aligned base
-  const uint32_t sK = sbase + Cfg::OFF_K, sV = sbase + Cfg::OFF_V;
-  auto sQ = [&](int st) { return sbase + Cfg::OFF_Q + st * Cfg::TILE_BYTES; };
-  auto sDO = [&](int st) { return sbase + Cfg::OFF_DO + st * Cfg::TILE_BYTES; };
-  const uint32_t sPT = sbase + Cfg::OFF_PT, sDS = sbase + Cfg::OFF_DS;
-  float* lse_s = reinterpret_cast<float*>(sgen + Cfg::OFF_LSE);  // [2][2][128]
-  const uint32_t bar = sbase + Cfg::OFF_BAR;
-  const uint32_t kv_full = bar;
-  auto q_full = [&](int s) { return bar + 8u * (1 + s); };
-  auto q_empty = [&](int s) { return bar + 8u * (3 + s); };
-  const uint32_t s_full = bar + 8u * 5;
-  const uint32_t pds_full = bar + 8u * 6;
-  const uint32_t dq_full = bar + 8u * 7;
-  const uint32_t dq_empty = bar + 8u * 8;
-  const uint32_t tmem_slot = bar + 8u * 9;
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t s0 = smem_u32(smem);
+  const uint32_t sK = s0 + Cfg::OFF_K, sV = s0 + Cfg::OFF_V, sQ = s0 + Cfg::OFF_Q, sDO = s0 + Cfg::OFF_DO;
+  const uint32_t sDS = s0 + Cfg::OFF_DS;
+  const uint32_t kv_full = s0 + Cfg::OFF_BAR, q_full0 = kv_full + 8, q_empty0 = kv_full + 24;
+  const int kt = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
+  const int k0 = kt * BKV;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int group = p.H / p.Hk;
+  const int n_qt = (p.S + BQ - 1) / BQ;
+  const int qt_first = p.causal ? k0 / BQ : 0;
+  const int per_head = n_qt - qt_first;
+  const int n_items = group * per_head;
 
-  const int warp = warp_idx_uniform();
-  const int lane = threadIdx.x & 31;
-
-  const int kt = blockIdx.x;  // kv tile (tile 0 sees every query tile under the causal mask)
-  const int hk = blockIdx.y;
-  const int b = blockIdx.z;
-  const int G = p.H / p.Hk;
-  const int k0 = kt * BT;
-  const int n_qt_all = (p.S + BT - 1) / BT;
-  const int qt_first = p.causal ? kt : 0;
-  const int n_qt = n_qt_all - qt_first;
-  const int n_it = G * n_qt;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    tma_prefetch_desc(&tmDO);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
     for (int s = 0; s < 2; ++s) {
-      mbar_init(q_full(s), 1);
-      mbar_init(q_empty(s), 1);
+      mbar_init(q_full0 + 8 * s, 1);
+      mbar_init(q_empty0 + 8 * s, 2);  // one arrival per consumer warpgroup
     }
-    mbar_init(s_full, 1);
-    mbar_init(pds_full, 8);
-    mbar_init(dq_full, 1);
-    mbar_init(dq_empty, 8);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // ---------------------------------- TMA producer ------------------------------------
-      mbar_arrive_expect_tx(kv_full, 2 * Cfg::TILE_BYTES);
-#pragma unroll
-      for (int db = 0; db < D / 64; ++db) {
-        tma_load_4d(sK + db * 16384, &tmK, kv_full, db * 64, hk, k0, b);
-        tma_load_4d(sV + db * 16384, &tmV, kv_full, db * 64, hk, k0, b);
-      }
-      for (int it = 0; it < n_it; ++it) {
-        const int st = it % ST;
-        const uint32_t ph = (it / ST) & 1u;
-        const int h = hk * G + it / n_qt;
-        const int q0 = (qt_first + it % n_qt) * BT;
-        BWD_TRACE(6);
-        mbar_wait(q_empty(st), ph ^ 1u);
-        BWD_TRACE(7);
-        mbar_arrive_expect_tx(q_full(st), 2 * Cfg::TILE_BYTES);
-#pragma unroll
-        for (int db = 0; db < D / 64; ++db) {
-          tma_load_4d(sQ(st) + db * 16384, &tmQ, q_full(st), db * 64, h, q0, b);
-          tma_load_4d(sDO(st) + db * 16384, &tmDO, q_full(st), db * 64, h, q0, b);
-        }
-      }
+  // one elected thread: K / V once, then the Q / dO tiles of item `it` into stage it % 2 once both warpgroups
+  // have released that stage (item it - 2)
+  auto issue_item = [&](int it) {
+    const int s = it & 1;
+    const int h = hk * group + it / per_head;
+    const int q0 = (qt_first + it % per_head) * BQ;
+    mbar_wait(q_empty0 + 8 * s, ((it >> 1) & 1) ^ 1u);
+    const uint32_t full = q_full0 + 8 * s;
+    mbar_arrive_expect_tx(full, 2 * Cfg::QS_BYTES);
+    for (int nb = 0; nb < Cfg::NB; ++nb) {
+      tma_load_4d(sQ + s * Cfg::QS_BYTES + nb * BQ * 128, &tmQ, full, nb * 64, h, q0, b);
+      tma_load_4d(sDO + s * Cfg::QS_BYTES + nb * BQ * 128, &tmDO, full, nb * 64, h, q0, b);
     }
-  } else if (warp == 1) {
-    {
-      // ---------------- MMA issuer: the whole warp runs the control flow (uniform), -------------
-      // ---------------- one elected lane issues tcgen05.mma / commit ---------------------------
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);  // K-major x K-major
-      constexpr uint32_t idesc_kv = make_idesc_bf16(128, D, false, true);    // K-major x MN-major
-      constexpr uint32_t idesc_dq = make_idesc_bf16(128, D, true, true);     // MN-major x MN-major
-      mbar_wait(kv_full, 0);
-      for (int it = 0; it < n_it; ++it) {
-        const int st = it % ST;
-        if (lane == 0) BWD_TRACE(8);
-        mbar_wait(q_full(st), (it / ST) & 1u);
-        if (Cfg::ALIAS_DQ && it > 0) mbar_wait(dq_empty, (it - 1) & 1u);
-        tc_fence_after_sync();
-        if (lane == 0) BWD_TRACE(9);
-        if (elect_one()) {
-          // S^T = K Q^T and dP^T = V dO^T   (M = keys, N = queries, K = head dim)
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-            umma_bf16_ss(tmem_base + Cfg::TM_S, make_smem_desc_sw128(sK + off, 0, 1024),
-                         make_smem_desc_sw128(sQ(st) + off, 0, 1024), idesc_s, kk != 0);
-          }
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-            umma_bf16_ss(tmem_base + Cfg::TM_DP, make_smem_desc_sw128(sV + off, 0, 1024),
-                         make_smem_desc_sw128(sDO(st) + off, 0, 1024), idesc_s, kk != 0);
-          }
-          umma_commit(s_full);
-        }
-        __syncwarp();
-        if (lane == 0) BWD_TRACE(10);
-
-        mbar_wait(pds_full, it & 1u);
-        if (lane == 0) BWD_TRACE(11);
-        if (!Cfg::ALIAS_DQ && it > 0) mbar_wait(dq_empty, (it - 1) & 1u);
-        tc_fence_after_sync();
-        if (lane == 0) BWD_TRACE(12);
-        if (elect_one()) {
-          // dV += P^T dO ; dK += dS^T Q   (M = keys, N = head dim, K = queries)
-#pragma unroll
-          for (int kk = 0; kk < BT / 16; ++kk) {
-            const uint32_t aoff = (kk >> 2) * 16384 + (kk & 3) * 32;
-            umma_bf16_ss(tmem_base + Cfg::TM_DV, make_smem_desc_sw128(sPT + aoff, 0, 1024),
-                         make_smem_desc_sw128(sDO(st) + kk * 2048, 16384, 1024), idesc_kv,
-                         (it | kk) != 0);
-          }
-#pragma unroll
-          for (int kk = 0; kk < BT / 16; ++kk) {
-            const uint32_t aoff = (kk >> 2) * 16384 + (kk & 3) * 32;
-            umma_bf16_ss(tmem_base + Cfg::TM_DK, make_smem_desc_sw128(sDS + aoff, 0, 1024),
-                         make_smem_desc_sw128(sQ(st) + kk * 2048, 16384, 1024), idesc_kv,
-                         (it | kk) != 0);
-          }
-          // dQ = dS K   (M = queries, N = head dim, K = keys): dS^T tile read as an MN-major A
-#pragma unroll
-          for (int kk = 0; kk < BT / 16; ++kk) {
-            umma_bf16_ss(tmem_base + Cfg::TM_DQ, make_smem_desc_sw128(sDS + kk * 2048, 16384, 1024),
-                         make_smem_desc_sw128(sK + kk * 2048, 16384, 1024), idesc_dq, kk != 0);
-          }
-          umma_commit(q_empty(st));
-          umma_commit(dq_full);
-        }
-        __syncwarp();
-        if (lane == 0) BWD_TRACE(13);
-      }
+  };
+  if (threadIdx.x == 0) {
+    mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
+    for (int nb = 0; nb < Cfg::NB; ++nb) {
+      tma_load_4d(sK + nb * BKV * 128, &tmK, kv_full, nb * 64, hk, k0, b);
+      tma_load_4d(sV + nb * BKV * 128, &tmV, kv_full, nb * 64, hk, k0, b);
     }
-  } else {
-    // --------------------------- softmax / dQ drain / dK,dV epilogue ------------------------
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;  // key row inside the tile (S^T) or query row (dQ)
-    const int key = k0 + row;
-    const uint32_t t_lane = tmem_base + (uint32_t(qd * 32) << 16);
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const int tid = threadIdx.x - 64;  // 0..255 (warp-major, not TMEM-lane order)
-    // Two warpgroups share every tile: both see all 128 key rows (TMEM lane quarter = warp % 4) and
-    // each takes half of the columns, so every SM sub-partition holds two softmax warps that hide
-    // each other's TMEM / MUFU latency.
-    const int wg = (warp - 2) >> 2;
-
-    for (int it = 0; it < n_it; ++it) {
-      const int h = hk * G + it / n_qt;
-      const int q0 = (qt_first + it % n_qt) * BT;
-      float* lse2 = lse_s + (it & 1) * 256;
-      float* dlt = lse2 + 128;
-      if (threadIdx.x == 64) BWD_TRACE(0);
-      {
-        const int qi = tid & 127;
-        const int q = q0 + qi;
-        const long long idx = ((long long)b * p.H + h) * p.S + q;
-        if (tid < 128)
-          lse2[qi] = q < p.S ? p.lse[idx] * 1.4426950408889634f : INFINITY;
-        else
-          dlt[qi] = q < p.S ? p.delta[idx] : 0.f;
-      }
-      named_bar_sync(1, 256);
-      if (threadIdx.x == 64) BWD_TRACE(1);
-      mbar_wait(s_full, it & 1u);
-      tc_fence_after_sync();
-      if (threadIdx.x == 64) BWD_TRACE(2);
-      const bool diag = p.causal && q0 == k0;  // tiles are aligned: only the diagonal tile is cut
-#pragma unroll 1
-      for (int c0 = wg * (BT / 2); c0 < (wg + 1) * (BT / 2); c0 += 32) {
-        uint32_t vs[32], vd[32];
-        tmem_ld_32x32b_x32(t_lane + Cfg::TM_S + c0, vs);
-        tmem_ld_32x32b_x32(t_lane + Cfg::TM_DP + c0, vd);
-        tmem_ld_wait();
-        float pr[32], ds[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int qc = c0 + i;
-          float e = ex2(fmaf(__uint_as_float(vs[i]), sl2, -lse2[qc]));
-          if ((diag && (q0 + qc < key)) || key >= p.S) e = 0.f;
-          pr[i] = e;
-          ds[i] = e * (__uint_as_float(vd[i]) - dlt[qc]) * p.scale;
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          st_tile_chunk(sPT, row, (c0 >> 3) + g, pr + g * 8);
-          st_tile_chunk(sDS, row, (c0 >> 3) + g, ds + g * 8);
-        }
-      }
-      tc_fence_before_sync();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_full);
-      if (threadIdx.x == 64) BWD_TRACE(3);
-
-      // drain dQ (TMEM lanes are query rows here) into the fp32 accumulator
-      mbar_wait(dq_full, it & 1u);
-      tc_fence_after_sync();
-      if (threadIdx.x == 64) BWD_TRACE(4);
-      {
-        const int q = q0 + row;
-        float* dst = p.dq_acc + (((long long)b * p.S + q) * p.H + h) * D;
-#pragma unroll 1
-        for (int c0 = wg * (D / 2); c0 < (wg + 1) * (D / 2); c0 += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(t_lane + Cfg::TM_DQ + c0, v);
-          tmem_ld_wait();
-          if (q < p.S) {
-#pragma unroll
-            for (int g = 0; g < 8; ++g)
-              red_add_v4(dst + c0 + g * 4, __uint_as_float(v[g * 4 + 0]), __uint_as_float(v[g * 4 + 1]),
-                         __uint_as_float(v[g * 4 + 2]), __uint_as_float(v[g * 4 + 3]));
-          }
-        }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dq_empty);
-      if (threadIdx.x == 64) BWD_TRACE(5);
-    }
-
-    // dK / dV: the last dq_full commit covers every MMA issued before it
-#pragma unroll 1
-    for (int which = 0; which < 2; ++which) {
-      __nv_bfloat16* out = (which == 0 ? p.dv : p.dk) + (((long long)b * p.S + key) * p.dkv_rh + hk) * D;
-      const uint32_t col = which == 0 ? Cfg::TM_DV : Cfg::TM_DK;
-#pragma unroll 1
-      for (int c0 = wg * (D / 2); c0 < (wg + 1) * (D / 2); c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(t_lane + col + c0, v);
-        tmem_ld_wait();
-        if (key < p.S) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4 o4;
-            if (n_it > 0) {
-              o4.x = pack_bf16x2(__uint_as_float(v[g * 8 + 0]), __uint_as_float(v[g * 8 + 1]));
-              o4.y = pack_bf16x2(__uint_as_float(v[g * 8 + 2]), __uint_as_float(v[g * 8 + 3]));
-              o4.z = pack_bf16x2(__uint_as_float(v[g * 8 + 4]), __uint_as_float(v[g * 8 + 5]));
-              o4.w = pack_bf16x2(__uint_as_float(v[g * 8 + 6]), __uint_as_float(v[g * 8 + 7]));
-            } else {
-              o4 = make_uint4(0, 0, 0, 0);
-            }
-            stg128(out + c0 + g * 8, o4);
-          }
-        }
-      }
-    }
+    if (n_items > 0) issue_item(0);
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  const int wg = warp >> 2, wq = warp & 3;
+  const int g = lane >> 2, cq = (lane & 3) * 2;
+  const int key_a = k0 + wg * 64 + wq * 16 + g;  // this thread's keys: key_a, key_a + 8
+  float dk[D / 2], dv[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
+  const float sl2 = p.scale * kLog2e;
+  mbar_wait(kv_full, 0);
+
+  for (int it = 0; it < n_items; ++it) {
+    const int s = it & 1;
+    const int h = hk * group + it / per_head;
+    const int q0 = (qt_first + it % per_head) * BQ;
+    if (threadIdx.x == 0 && it + 1 < n_items) issue_item(it + 1);
+    mbar_wait(q_full0 + 8 * s, (it >> 1) & 1);
+    const uint32_t tQ = sQ + s * Cfg::QS_BYTES, tDO = sDO + s * Cfg::QS_BYTES;
+
+    // S^T = K Q^T and dP^T = V dO^T: 64 keys x 64 queries per warpgroup
+    float st[32], dpt[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) st[i] = dpt[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk) {
+      const uint32_t ka = (kk >> 2) * BKV * 128 + wg * 64 * 128 + (kk & 3) * 32;
+      const uint32_t qb = (kk >> 2) * BQ * 128 + (kk & 3) * 32;
+      wgmma_m64n64k16_ss<0, 0>(st, make_wgmma_desc_sw128(sK + ka, 16, 1024), make_wgmma_desc_sw128(tQ + qb, 16, 1024));
+      wgmma_m64n64k16_ss<0, 0>(dpt, make_wgmma_desc_sw128(sV + ka, 16, 1024), make_wgmma_desc_sw128(tDO + qb, 16, 1024));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+
+    // P^T and dS^T (unscaled); masked entries are exactly 0.  Chunk nc holds queries 8 nc + cq + {0, 1}.
+    const long long lrow = ((long long)b * p.H + h) * p.S;
+#pragma unroll
+    for (int nc = 0; nc < 8; ++nc) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int qi = q0 + nc * 8 + cq + (e & 1);
+        const int key = key_a + ((e >> 1) << 3);
+        const bool ok = qi < p.S && key < p.S && !(p.causal && key > qi);
+        const float pv = ok ? exp2f(st[4 * nc + e] * sl2 - p.lse[lrow + qi] * kLog2e) : 0.f;
+        st[4 * nc + e] = pv;
+        dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] - p.delta[lrow + qi]) : 0.f;
+      }
+    }
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        pa[kk][i] = pack_bf16x2(st[8 * kk + 2 * i], st[8 * kk + 2 * i + 1]);
+        da[kk][i] = pack_bf16x2(dpt[8 * kk + 2 * i], dpt[8 * kk + 2 * i + 1]);
+      }
+    }
+    // dS^T rows of this thread -> [key][64 queries] tile, 128 B per row, 16-byte chunks XOR (row % 8)
+    {
+      const int r = wg * 64 + wq * 16 + g;
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int row = r + ((i & 1) << 3), chunk = 2 * kk + (i >> 1);
+          *reinterpret_cast<uint32_t*>(smem + Cfg::OFF_DS + row * 128 + ((chunk ^ (row & 7)) << 4) + cq * 2) = da[kk][i];
+        }
+      }
+    }
+    fence_proxy_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads below
+
+    // dV += P^T dO, dK += dS^T Q: k = queries (16 rows of 128 B per step), n = head dim (64-column blocks)
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) rs_mma<D>(dv, pa[kk], make_wgmma_desc_sw128(tDO + kk * 2048, BQ * 128, 1024));
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) rs_mma<D>(dk, da[kk], make_wgmma_desc_sw128(tQ + kk * 2048, BQ * 128, 1024));
+    wgmma_commit();
+    named_bar_sync(1, 256);  // both warpgroups' dS^T rows are in shared memory
+
+    // dQ[64 queries, head-dim block] = dS K over all 128 keys; at D = 64 warpgroup 0 does the whole tile
+    float dq[32];
+    const bool do_dq = (D == 128) || wg == 0;
+    const int nblk = (D == 128) ? wg : 0;
+    if (do_dq) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BKV / 16; ++kk)
+        wgmma_m64n64k16_ss<1, 1>(dq, make_wgmma_desc_sw128(sDS + kk * 2048, 8192, 1024),
+                                 make_wgmma_desc_sw128(sK + nblk * BKV * 128 + kk * 2048, BKV * 128, 1024));
+      wgmma_commit();
+    }
+    wgmma_wait<0>();
+    if ((threadIdx.x & 127) == 0) mbar_arrive(q_empty0 + 8 * s);
+    if (do_dq) {
+      float* dqb = p.dq_acc + ((long long)b * p.S * p.H + h) * D + nblk * 64;
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int qi = q0 + wq * 16 + g + 8 * r;
+        if (qi >= p.S) continue;
+        float* row = dqb + (long long)qi * p.H * D + cq;
+#pragma unroll
+        for (int nc = 0; nc < 8; ++nc) {
+          atomicAdd(row + nc * 8, dq[4 * nc + 2 * r]);
+          atomicAdd(row + nc * 8 + 1, dq[4 * nc + 2 * r + 1]);
+        }
+      }
+    }
+    named_bar_sync(1, 256);  // the dS^T tile is rewritten by the next item
+  }
+
+  // dK (scale applied here), dV -> bf16 rows of dkv_rh heads
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int key = key_a + 8 * r;
+    if (key >= p.S) continue;
+    const long long off = ((long long)b * p.S + key) * p.dkv_rh * D + (long long)hk * D + cq;
+#pragma unroll
+    for (int dc = 0; dc < D / 8; ++dc) {
+      *reinterpret_cast<uint32_t*>(p.dk + off + dc * 8) =
+          pack_bf16x2(dk[4 * dc + 2 * r] * p.scale, dk[4 * dc + 2 * r + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(p.dv + off + dc * 8) = pack_bf16x2(dv[4 * dc + 2 * r], dv[4 * dc + 2 * r + 1]);
+    }
   }
 }
 
@@ -433,8 +292,8 @@ f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ ds
 }
 
 template <int D>
-int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-               const CUtensorMap& tmDO, const BwdArgs& a, cudaStream_t stream) {
+int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmDO,
+               const BwdArgs& a, cudaStream_t stream) {
   using Cfg = BwdCfg<D>;
   auto kern = attn_bwd_kernel<D>;
   static bool attr_set = false;
@@ -442,7 +301,7 @@ int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set = true;
   }
-  dim3 grid((a.S + BT - 1) / BT, a.Hk, a.B);
+  dim3 grid((a.S + BKV - 1) / BKV, a.Hk, a.B);
   kern<<<grid, BWD_THREADS, Cfg::SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmDO, a);
   B200_CHECK_LAUNCH();
   return B200_OK;
@@ -474,6 +333,9 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
     return B200_ERR_WORKSPACE;
   }
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, "attn_bwd: workspace must be 256-byte aligned");
+  B200_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+                   reinterpret_cast<uintptr_t>(o) | reinterpret_cast<uintptr_t>(d_o)) & 15u) == 0,
+                 "attn_bwd: q/k/v/o/do must be 16-byte aligned");
   float* dq_acc = reinterpret_cast<float*>(ws);
   float* delta = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + al256((size_t)B * S * H * D * 4));
   const long long n = (long long)B * S * H * D;
@@ -488,10 +350,10 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
   }
   CUtensorMap tmQ, tmK, tmV, tmDO;
   int rc;
-  if ((rc = make_bshd_map(&tmQ, q, B, S, H, D, BT, false))) return rc;
-  if ((rc = make_bshd_map(&tmK, k, B, S, Hk, D, BT, false))) return rc;
-  if ((rc = make_bshd_map(&tmV, v, B, S, Hk, D, BT, false))) return rc;
-  if ((rc = make_bshd_map(&tmDO, d_o, B, S, H, D, BT, false))) return rc;
+  if ((rc = make_bshd_map(&tmQ, q, B, S, H, D, BQ))) return rc;
+  if ((rc = make_bshd_map(&tmK, k, B, S, Hk, D, BKV))) return rc;
+  if ((rc = make_bshd_map(&tmV, v, B, S, Hk, D, BKV))) return rc;
+  if ((rc = make_bshd_map(&tmDO, d_o, B, S, H, D, BQ))) return rc;
   BwdArgs a;
   a.lse = lse;
   a.delta = delta;
@@ -505,32 +367,14 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
   a.dkv_rh = dkv_row_heads;
   a.scale = scale;
   a.causal = causal;
-  {
-    // debug: B200_ATTN_TRACE=<device pointer, hex> makes CTA 0 record clock64 stamps (tools/attn_trace.py)
-    const char* e = getenv("B200_ATTN_TRACE");
-    a.trace = e ? reinterpret_cast<long long*>(strtoull(e, nullptr, 16)) : nullptr;
-  }
-  static const bool force_v1 = [] {
-    const char* e = getenv("B200_ATTN_BWD_V1");
-    return e != nullptr && e[0] == '1';
-  }();
-  const bool pipelined = !force_v1;   // software-pipelined kernels (attention_bwd64.cu / attention_bwd128.cu)
-  if (pipelined && D == 64)
-    rc = launch_attn_bwd64(tmQ, tmK, tmV, tmDO, lse, delta, dq_acc, dk, dv, B, S, H, Hk, dkv_row_heads, scale, causal,
-                           stream);
-  else if (pipelined)
-    rc = launch_attn_bwd128(tmQ, tmK, tmV, tmDO, lse, delta, dq_acc, dk, dv, B, S, H, Hk, dkv_row_heads, scale, causal,
-                            stream);
-  else
-    rc = D == 64 ? launch_bwd<64>(tmQ, tmK, tmV, tmDO, a, stream) : launch_bwd<128>(tmQ, tmK, tmV, tmDO, a, stream);
+  rc = D == 64 ? launch_bwd<64>(tmQ, tmK, tmV, tmDO, a, stream) : launch_bwd<128>(tmQ, tmK, tmV, tmDO, a, stream);
   if (rc) return rc;
   {
     const long long nvec = n / 8;
     long long blocks = (nvec + 255) / 256;
     if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
-    // the pipelined kernels accumulate dS without the softmax scale (one multiply less per score): applied here
-    f32_to_bf16_kernel<<<(int)blocks, 256, 0, stream>>>(dq_acc, reinterpret_cast<__nv_bfloat16*>(dq), nvec,
-                                                        pipelined ? scale : 1.0f);
+    // the kernel accumulates dS without the softmax scale: applied here
+    f32_to_bf16_kernel<<<(int)blocks, 256, 0, stream>>>(dq_acc, reinterpret_cast<__nv_bfloat16*>(dq), nvec, scale);
     B200_CHECK_LAUNCH();
   }
   return B200_OK;

@@ -1,25 +1,16 @@
-// Fused causal / GQA attention forward on tcgen05 (sm_100a).
+// Fused causal / GQA attention forward on Hopper warpgroup MMA (wgmma) fed by TMA through an mbarrier ring.
 //
 // Computes what FlashAttention._flash_attention (arch/flash_attention.py:97-156 of the reference)
 // computes -- O = softmax(Q K^T * scale + mask) V with q-head h reading kv-head h / (H/Hk) -- but
 // tiled with an online softmax, so the [B,H,S,S] score tensor the reference materialises (:134)
 // never exists.  Also emits LSE = log sum exp(scaled masked scores) for the backward pass.
 //
-// One CTA per (128-query tile, head, batch); 320 threads; at head_dim 64 TWO CTAs share an SM (97 KB smem,
-// 256 TMEM columns, <= 102 registers each) so one CTA's prologue / softmax / epilogue hides behind the
-// other's tensor work -- with S = 1024 a CTA lives for only 1..8 key tiles and its fixed costs matter:
-//   warp 0      TMA producer: Q once, then K / V tiles (128 keys) through 2-stage rings
-//   warp 1      tcgen05.mma issuer: S = Q K^T -> TMEM, O += P V -> TMEM with P as a TMEM A operand
-//   warps 2-9   softmax, two warpgroups: each thread owns one query row (TMEM lane) x 64 of the 128
-//               key columns; scores stay in registers between row max (exchanged through smem) and
-//               exp2; P written back to TMEM as packed bf16 (tcgen05.st); O rescaled in TMEM only when a
-//               row max moved.
-// The S accumulator is handed back as soon as the scores sit in registers, so QK^T(j+1) overlaps the
-// exponentials of tile j even with a single S buffer.
-// Tried in r02 and dropped (commit "attention forward: register-prefetch variant"): one CTA per SM with S double-buffered
-// in TMEM and a second set of 64 score registers per thread, so that tile j+1's scores stream out of tensor memory
-// (asynchronous tcgen05.ld) under tile j's exponentials.  Correct, but slower everywhere: 137 vs 97 us (S=1024, D=64),
-// 397 vs 277 us (S=2048), 1023 vs 863 us (D=128, C5 shape) -- the second resident CTA hides more than the prefetch does.
+// One CTA per (128-query tile, head, batch), 288 threads:
+//   warp 8          TMA producer: the Q tile once, then K / V tiles of 128 keys through a 2-stage ring
+//                   (128B-swizzled boxes of 64 head-dim columns, full / empty mbarriers per stage)
+//   warpgroups 0-1  64 query rows each: S = Q K^T as wgmma.m64n128k16 with both operands in shared memory,
+//                   online softmax on the fp32 accumulators in registers, then O += P V as wgmma with P as the
+//                   register A operand (the accumulator fragment packed to bf16) and V read MN-major from smem.
 #include "common.cuh"
 #include "host.h"
 
@@ -29,29 +20,19 @@ namespace {
 
 constexpr int ATT_BQ = 128;
 constexpr int ATT_BKV = 128;
-constexpr int FWD_THREADS = 320;  // warp 0 TMA, warp 1 MMA, warps 2-9: two softmax warpgroups
-constexpr int KV_STAGES = 2;
-// P = exp(S - max) goes back to TENSOR MEMORY (packed bf16, 64 columns) and feeds O += P V as the A operand
-// of tcgen05.mma (A in TMEM, B = V in smem): no 32 KB smem round trip per key tile, and the MMA reads only V
-// from shared memory.  false = the first version (P as a swizzled K-major smem tile).
-constexpr bool kPInTmem = true;
+constexpr int FWD_THREADS = 288;  // two consumer warpgroups + one producer warp
+constexpr float kLog2e = 1.4426950408889634f;
 
 template <int D>
 struct FwdCfg {
-  static constexpr int TILE_BYTES = 128 * D * 2;  // one Q / K / V tile
-  static constexpr int P_BYTES = kPInTmem ? 0 : 128 * 128 * 2;
-  static constexpr int V_STAGES = kPInTmem ? 2 : 1;  // without the smem P tile both K and V are double-buffered
+  static constexpr int NB = D / 64;                 // 64-column (128-byte) blocks per row
+  static constexpr int Q_BYTES = ATT_BQ * D * 2;
+  static constexpr int KV_BYTES = ATT_BKV * D * 2;  // one K or V stage
   static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = OFF_Q + TILE_BYTES;
-  static constexpr int OFF_V = OFF_K + KV_STAGES * TILE_BYTES;
-  static constexpr int OFF_P = OFF_V + V_STAGES * TILE_BYTES;
-  static constexpr int OFF_BAR = OFF_P + P_BYTES;
-  static constexpr int OFF_RED = OFF_BAR + 256;  // [2][2][128] row-max exchange + [2][128] row-sum exchange
-  static constexpr int SMEM_BYTES = OFF_RED + 3072 + 1024;
-  static constexpr int CTAS_PER_SM = (2 * SMEM_BYTES + 2048 <= 227 * 1024) ? 2 : 1;
-  // S 128 | O D | P 64 (packed bf16): 256 columns at D = 64, so two co-resident CTAs fill the 512
-  static constexpr int TMEM_COLS = (128 + D + 64 <= 256) ? 256 : 512;
-  static constexpr int TM_S = 0, TM_O = 128, TM_P = 128 + D;
+  static constexpr int OFF_K = OFF_Q + Q_BYTES;       // 2 stages
+  static constexpr int OFF_V = OFF_K + 2 * KV_BYTES;  // 2 stages
+  static constexpr int OFF_BAR = OFF_V + 2 * KV_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;
 };
 
 struct FwdArgs {
@@ -62,301 +43,174 @@ struct FwdArgs {
   int causal;
 };
 
-__device__ __forceinline__ float fast_exp2(float x) {
-  float y;
-  asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
+template <int D>
+__device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db) {
+  if constexpr (D == 128) wgmma_m64n128k16_rs<1>(o, a, db);
+  else wgmma_m64n64k16_rs<1>(o, a, db);
 }
 
 template <int D>
-__global__ void __launch_bounds__(FWD_THREADS, FwdCfg<D>::CTAS_PER_SM)
+__global__ void __launch_bounds__(FWD_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdArgs p) {
   using Cfg = FwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = sbase + Cfg::OFF_Q;
-  const uint32_t sP = sbase + Cfg::OFF_P;
-  auto sK = [&](int st) { return sbase + Cfg::OFF_K + st * Cfg::TILE_BYTES; };
-  auto sV = [&](int j) { return sbase + Cfg::OFF_V + (Cfg::V_STAGES == 2 ? (j & 1) : 0) * Cfg::TILE_BYTES; };
-  const uint32_t bar = sbase + Cfg::OFF_BAR;
-  const uint32_t q_full = bar;
-  auto k_full = [&](int s) { return bar + 8u * (1 + s); };
-  auto k_empty = [&](int s) { return bar + 8u * (3 + s); };
-  // V tile j lives in stage j % V_STAGES; its barriers complete once per V_STAGES tiles
-  auto v_full = [&](int j) { return bar + 8u * (5 + (Cfg::V_STAGES == 2 ? (j & 1) : 0)); };
-  auto v_empty = [&](int j) { return bar + 8u * (7 + (Cfg::V_STAGES == 2 ? (j & 1) : 0)); };
-  auto v_par = [&](int j) { return (uint32_t)((Cfg::V_STAGES == 2 ? (j >> 1) : j) & 1); };
-  const uint32_t s_full = bar + 8u * 9;
-  const uint32_t s_empty = bar + 8u * 10;
-  const uint32_t p_full = bar + 8u * 13;
-  const uint32_t pv_done = bar + 8u * 14;
-  const uint32_t tmem_slot = bar + 8u * 15;
-  float* red_s = reinterpret_cast<float*>(smem_raw + (sbase - smem_u32(smem_raw)) + Cfg::OFF_RED);
-
-  const int warp = warp_idx_uniform();
-  const int lane = threadIdx.x & 31;
-
-  const int qt = (int)gridDim.x - 1 - (int)blockIdx.x;  // heaviest (longest causal row) tiles first
-  const int h = blockIdx.y;
-  const int b = blockIdx.z;
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t s0 = smem_u32(smem);
+  const uint32_t sQ = s0 + Cfg::OFF_Q, sK = s0 + Cfg::OFF_K, sV = s0 + Cfg::OFF_V;
+  const uint32_t q_full = s0 + Cfg::OFF_BAR, kv_full0 = q_full + 8, kv_empty0 = q_full + 24;
+  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int hk = h / (p.H / p.Hk);
   const int q0 = qt * ATT_BQ;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_kv_all = (p.S + ATT_BKV - 1) / ATT_BKV;
-  const int n_kv = p.causal ? (qt + 1 < n_kv_all ? qt + 1 : n_kv_all) : n_kv_all;
+  const int n_kv = p.causal ? min(n_kv_all, (q0 + ATT_BQ - 1) / ATT_BKV + 1) : n_kv_all;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
     for (int s = 0; s < 2; ++s) {
-      mbar_init(k_full(s), 1);
-      mbar_init(k_empty(s), 1);
+      mbar_init(kv_full0 + 8 * s, 1);
+      mbar_init(kv_empty0 + 8 * s, 2);  // one arrival per consumer warpgroup
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(v_full(s), 1);
-      mbar_init(v_empty(s), 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, 8);
-    mbar_init(p_full, 8);
-    mbar_init(pv_done, 1);
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
-      // ---------------------------------- TMA producer ------------------------------------
-      mbar_arrive_expect_tx(q_full, Cfg::TILE_BYTES);
-#pragma unroll
-      for (int db = 0; db < D / 64; ++db) tma_load_4d(sQ + db * 16384, &tmQ, q_full, db * 64, h, q0, b);
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmK);
+      tma_prefetch_desc(&tmV);
+      mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
+      for (int nb = 0; nb < Cfg::NB; ++nb) tma_load_4d(sQ + nb * ATT_BQ * 128, &tmQ, q_full, nb * 64, h, q0, b);
       for (int j = 0; j < n_kv; ++j) {
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1u;
-        mbar_wait(k_empty(st), ph ^ 1u);
-        mbar_arrive_expect_tx(k_full(st), Cfg::TILE_BYTES);
-#pragma unroll
-        for (int db = 0; db < D / 64; ++db)
-          tma_load_4d(sK(st) + db * 16384, &tmK, k_full(st), db * 64, hk, j * ATT_BKV, b);
-        mbar_wait(v_empty(j), v_par(j) ^ 1u);
-        mbar_arrive_expect_tx(v_full(j), Cfg::TILE_BYTES);
-#pragma unroll
-        for (int db = 0; db < D / 64; ++db)
-          tma_load_4d(sV(j) + db * 16384, &tmV, v_full(j), db * 64, hk, j * ATT_BKV, b);
-      }
-    }
-  } else if (warp == 1) {
-    {
-      // ------ MMA issuer: whole warp runs the uniform control flow, one elected lane issues ------
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, D, false, true);
-      auto issue_s = [&](int j) {
-        const int st = j & 1;
-        const uint32_t ph = (j >> 1) & 1u;
-        mbar_wait(s_empty, (j & 1u) ^ 1u);
-        mbar_wait(k_full(st), ph);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + Cfg::TM_S;
-        if (elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-            umma_bf16_ss(d_tmem, make_smem_desc_sw128(sQ + off, 0, 1024),
-                         make_smem_desc_sw128(sK(st) + off, 0, 1024), idesc_s, kk != 0);
-          }
-          umma_commit(k_empty(st));
-          umma_commit(s_full);
-        }
-        __syncwarp();
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      for (int j = 0; j < n_kv; ++j) {
-        if (j + 1 < n_kv) issue_s(j + 1);
-        mbar_wait(p_full, j & 1u);
-        mbar_wait(v_full(j), v_par(j));
-        tc_fence_after_sync();
-        if (elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
-            const uint64_t db = make_smem_desc_sw128(sV(j) + kk * 2048, 16384, 1024);
-            if constexpr (kPInTmem) {
-              // A = P[128 x 16] from TMEM: 16 bf16 of K per row = 8 packed columns per K step
-              umma_bf16_ts(tmem_base + Cfg::TM_O, tmem_base + Cfg::TM_P + kk * 8, db, idesc_pv, (j | kk) != 0);
-            } else {
-              const uint64_t da = make_smem_desc_sw128(sP + (kk >> 2) * 16384 + (kk & 3) * 32, 0, 1024);
-              umma_bf16_ss(tmem_base + Cfg::TM_O, da, db, idesc_pv, (j | kk) != 0);
-            }
-          }
-          umma_commit(v_empty(j));
-          umma_commit(pv_done);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ------------------------------------ softmax warps -------------------------------------
-    // Two warpgroups (warps 2-5, 6-9) share every S tile: both cover all 128 query rows (TMEM lane
-    // quarter = warp % 4), each owns 64 of the 128 key columns and half of O's columns.  Each SM
-    // sub-partition therefore runs two softmax warps that hide each other's TMEM / MUFU latency, and a
-    // thread's 64 scores stay in registers between the max and the exp (one TMEM pass).
-    const int qd = warp & 3;
-    const int wg = (warp - 2) >> 2;
-    const int row = qd * 32 + lane;
-    const int q_row = q0 + row;
-    const uint32_t t_lane = tmem_base + (uint32_t(qd * 32) << 16);
-    const float sl2 = p.scale * 1.4426950408889634f;
-    const int cbase = wg * 64;
-    constexpr int OH = D / 2;  // O columns owned by this warpgroup
-    float m = -INFINITY, l = 0.f;
-
-    for (int j = 0; j < n_kv; ++j) {
-      const uint32_t t_s = t_lane + Cfg::TM_S + cbase;
-      const int k0 = j * ATT_BKV + cbase;
-      const bool need_mask = (p.causal && j * ATT_BKV + ATT_BKV - 1 > q0) || (j * ATT_BKV + ATT_BKV > p.S);
-      const int kmax = p.causal ? (q_row < p.S - 1 ? q_row : p.S - 1) : p.S - 1;  // last valid key
-
-      mbar_wait(s_full, j & 1u);
-      tc_fence_after_sync();
-      uint32_t v[64];
-      tmem_ld_32x32b_x32(t_s, v);
-      tmem_ld_32x32b_x32(t_s + 32, v + 32);
-      tmem_ld_wait();
-      // the scores now live in registers: hand the S buffer back to the tensor core right away
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_empty);
-
-      float mx = -INFINITY;
-      if (need_mask) {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) {
-          if (k0 + i > kmax) v[i] = __float_as_uint(-INFINITY);
-          mx = fmaxf(mx, __uint_as_float(v[i]));
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 64; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-      }
-      float* mslot = red_s + (j & 1) * 256;
-      mslot[wg * 128 + row] = mx;
-      named_bar_sync(1, 256);
-      mx = fmaxf(mx, mslot[(wg ^ 1) * 128 + row]);
-      const float m_new = fmaxf(m, mx);
-      const float alpha = fast_exp2((m - m_new) * sl2);
-      const float mb = m_new * sl2;
-
-      // P smem and the O accumulator are free once PV(j-1) has retired
-      if (j > 0) {
-        mbar_wait(pv_done, (j - 1) & 1u);
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, m_new > m)) {
-          // 8 columns at a time: the 64 scores stay live across this loop and the register budget with
-          // two CTAs per SM is 102
-#pragma unroll 1
-          for (int c0 = 0; c0 < OH; c0 += 8) {
-            uint32_t o[8];
-            tmem_ld_32x32b_x8(t_lane + Cfg::TM_O + wg * OH + c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 8; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st_32x32b_x8(t_lane + Cfg::TM_O + wg * OH + c0, o);
-          }
-          tmem_st_wait();
-        }
-      }
-      // probabilities -> bf16 P tile (K-major, 128B swizzle): this warpgroup fills 64-column block `wg`
-      float rs = 0.f;
-      if constexpr (kPInTmem) {
-        // this warpgroup's 64 key columns = packed columns [32 wg, 32 wg + 32) of the P operand
-#pragma unroll
-        for (int hlf = 0; hlf < 2; ++hlf) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float e0 = fast_exp2(fmaf(__uint_as_float(v[hlf * 32 + 2 * i]), sl2, -mb));
-            const float e1 = fast_exp2(fmaf(__uint_as_float(v[hlf * 32 + 2 * i + 1]), sl2, -mb));
-            rs += e0 + e1;
-            pk[i] = pack_bf16x2(e0, e1);
-          }
-          tmem_st_32x32b_x16(t_lane + Cfg::TM_P + wg * 32 + hlf * 16, pk);
-        }
-        tmem_st_wait();
-      } else {
-        const uint32_t blk = sP + wg * 16384 + row * 128;
-#pragma unroll
-        for (int g = 0; g < 8; ++g) {
-          float e[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            e[i] = fast_exp2(fmaf(__uint_as_float(v[g * 8 + i]), sl2, -mb));
-            rs += e[i];
-          }
-          const uint32_t addr = blk + ((g ^ (row & 7)) << 4);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pack_bf16x2(e[0], e[1])),
-                       "r"(pack_bf16x2(e[2], e[3])), "r"(pack_bf16x2(e[4], e[5])), "r"(pack_bf16x2(e[6], e[7]))
-                       : "memory");
-        }
-        fence_proxy_async_smem();
-      }
-      l = l * alpha + rs;
-      m = m_new;
-      // publish: P + rescaled O visible to the tensor core
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-    }
-
-    // --------------------------------------- epilogue ---------------------------------------
-    // each warpgroup holds the row sum of its own 64-column halves: combine them once
-    float* lslot = red_s + 512;
-    lslot[wg * 128 + row] = l;
-    named_bar_sync(1, 256);
-    l += lslot[(wg ^ 1) * 128 + row];
-    mbar_wait(pv_done, (n_kv - 1) & 1u);
-    tc_fence_after_sync();
-    const float inv_l = 1.0f / l;
-    __nv_bfloat16* orow = p.o + (((long long)b * p.S + q_row) * p.H + h) * D + wg * OH;
-#pragma unroll 1
-    for (int c0 = 0; c0 < OH; c0 += 32) {
-      uint32_t o[32];
-      tmem_ld_32x32b_x32(t_lane + Cfg::TM_O + wg * OH + c0, o);
-      tmem_ld_wait();
-      if (q_row < p.S) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 o4;
-          o4.x = pack_bf16x2(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l);
-          o4.y = pack_bf16x2(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l);
-          o4.z = pack_bf16x2(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l);
-          o4.w = pack_bf16x2(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l);
-          stg128(orow + c0 + g * 8, o4);
+        const int s = j & 1;
+        mbar_wait(kv_empty0 + 8 * s, ((j >> 1) & 1) ^ 1u);
+        const uint32_t full = kv_full0 + 8 * s;
+        mbar_arrive_expect_tx(full, 2 * Cfg::KV_BYTES);
+        for (int nb = 0; nb < Cfg::NB; ++nb) {
+          tma_load_4d(sK + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmK, full, nb * 64, hk, j * ATT_BKV, b);
+          tma_load_4d(sV + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmV, full, nb * 64, hk, j * ATT_BKV, b);
         }
       }
     }
-    if (wg == 0 && q_row < p.S) p.lse[((long long)b * p.H + h) * p.S + q_row] = m * p.scale + logf(l);
+    return;
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  const int wg = warp >> 2, wq = warp & 3;
+  float o[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+  float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
+  const float sl2 = p.scale * kLog2e;
+  const int row_a = q0 + wg * 64 + wq * 16 + (lane >> 2);  // this thread's rows: row_a, row_a + 8
+  mbar_wait(q_full, 0);
+
+  for (int j = 0; j < n_kv; ++j) {
+    const int s = j & 1;
+    mbar_wait(kv_full0 + 8 * s, (j >> 1) & 1);
+    const uint32_t tK = sK + s * Cfg::KV_BYTES, tV = sV + s * Cfg::KV_BYTES;
+    const int k0 = j * ATT_BKV;
+
+    // S = Q K^T: 64 rows x 128 keys per warpgroup, both operands K-major (head dim contiguous)
+    float sc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) sc[i] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < D / 16; ++kk) {
+      const uint64_t da = make_wgmma_desc_sw128(sQ + (kk >> 2) * ATT_BQ * 128 + wg * 64 * 128 + (kk & 3) * 32, 16, 1024);
+      const uint64_t db = make_wgmma_desc_sw128(tK + (kk >> 2) * ATT_BKV * 128 + (kk & 3) * 32, 16, 1024);
+      wgmma_m64n128k16_ss<0, 0>(sc, da, db);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+
+    // scale (log2 domain), mask, online softmax; accumulator chunk nc holds keys 8 nc + 2 (lane % 4) + {0, 1}
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
+        const int row = row_a + ((e >> 1) << 3);
+        float x = sc[4 * nc + e] * sl2;
+        if (key >= p.S || (p.causal && key > row)) x = -INFINITY;
+        sc[4 * nc + e] = x;
+        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      }
+    }
+    float alpha[2], m_use[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_new = fmaxf(m_r[r], mx[r]);
+      m_use[r] = (m_new == -INFINITY) ? 0.f : m_new;
+      alpha[r] = exp2f(m_r[r] - m_use[r]);
+      m_r[r] = m_new;
+      l_r[r] *= alpha[r];
+    }
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const float pe = exp2f(sc[4 * nc + e] - m_use[e >> 1]);
+        sc[4 * nc + e] = pe;
+        l_r[e >> 1] += pe;
+      }
+    }
+    // two adjacent key chunks form one k16 A fragment: (row, k 0-7), (row + 8, k 0-7), (row, k 8-15), (row + 8, k 8-15)
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      pa[kk][0] = pack_bf16x2(sc[8 * kk + 0], sc[8 * kk + 1]);
+      pa[kk][1] = pack_bf16x2(sc[8 * kk + 2], sc[8 * kk + 3]);
+      pa[kk][2] = pack_bf16x2(sc[8 * kk + 4], sc[8 * kk + 5]);
+      pa[kk][3] = pack_bf16x2(sc[8 * kk + 6], sc[8 * kk + 7]);
+    }
+#pragma unroll
+    for (int dc = 0; dc < D / 8; ++dc) {
+      o[4 * dc + 0] *= alpha[0];
+      o[4 * dc + 1] *= alpha[0];
+      o[4 * dc + 2] *= alpha[1];
+      o[4 * dc + 3] *= alpha[1];
+    }
+    // O += P V: V is the MN-major B operand (keys = k rows of 128 B, head-dim blocks LBO apart)
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      pv_mma<D>(o, pa[kk], make_wgmma_desc_sw128(tV + kk * 2048, ATT_BKV * 128, 1024));
+    wgmma_commit();
+    wgmma_wait<0>();
+    if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty0 + 8 * s);
+  }
+
+  // normalise, store O and LSE (natural log of the scaled scores' sum-exp)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 1);
+    l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 2);
+  }
+  const float inv[2] = {1.0f / l_r[0], 1.0f / l_r[1]};
+  const long long q_stride = (long long)p.H * D;
+  __nv_bfloat16* ob = p.o + (long long)b * p.S * q_stride + (long long)h * D;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = row_a + 8 * r;
+    if (row >= p.S) continue;
+    __nv_bfloat16* orow = ob + (long long)row * q_stride;
+#pragma unroll
+    for (int dc = 0; dc < D / 8; ++dc)
+      *reinterpret_cast<uint32_t*>(orow + dc * 8 + (lane & 3) * 2) =
+          pack_bf16x2(o[4 * dc + 2 * r] * inv[r], o[4 * dc + 2 * r + 1] * inv[r]);
+    if ((lane & 3) == 0) p.lse[((long long)b * p.H + h) * p.S + row] = (m_r[r] + log2f(l_r[r])) / kLog2e;
   }
 }
 
 template <int D>
-int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-               const FwdArgs& a, cudaStream_t stream) {
+int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
+               cudaStream_t stream) {
   using Cfg = FwdCfg<D>;
   auto kern = attn_fwd_kernel<D>;
   static bool attr_set = false;
@@ -372,15 +226,12 @@ int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap
 
 }  // namespace
 
-// [B, S, heads, D] bf16 tensor -> 4-D tensor map {D, heads, S, B}, box {64, 1, rows, 1}
-int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, int D, int box_rows,
-                  bool f32) {
-  const int es = f32 ? 4 : 2;
+// [B, S, heads, D] bf16 tensor -> 4-D tensor map {D, heads, S, B}, box {64, 1, rows, 1}, 128B swizzle
+int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, int D, int box_rows) {
   const uint64_t dims[4] = {(uint64_t)D, (uint64_t)heads, (uint64_t)S, (uint64_t)B};
-  const uint64_t strides[3] = {(uint64_t)D * es, (uint64_t)heads * D * es, (uint64_t)S * heads * D * es};
-  const uint32_t box[4] = {(uint32_t)(f32 ? 32 : 64), 1, (uint32_t)box_rows, 1};
-  return make_tensor_map(tm, base, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
-                         es, 4, dims, strides, box, true);
+  const uint64_t strides[3] = {(uint64_t)D * 2, (uint64_t)heads * D * 2, (uint64_t)S * heads * D * 2};
+  const uint32_t box[4] = {64, 1, (uint32_t)box_rows, 1};
+  return make_tensor_map(tm, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 4, dims, strides, box, true);
 }
 
 int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int H,
@@ -391,9 +242,9 @@ int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, i
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(o) & 15u) == 0, "attn_fwd: o must be 16-byte aligned");
   CUtensorMap tmQ, tmK, tmV;
   int rc;
-  if ((rc = make_bshd_map(&tmQ, q, B, S, H, D, ATT_BQ, false))) return rc;
-  if ((rc = make_bshd_map(&tmK, k, B, S, Hk, D, ATT_BKV, false))) return rc;
-  if ((rc = make_bshd_map(&tmV, v, B, S, Hk, D, ATT_BKV, false))) return rc;
+  if ((rc = make_bshd_map(&tmQ, q, B, S, H, D, ATT_BQ))) return rc;
+  if ((rc = make_bshd_map(&tmK, k, B, S, Hk, D, ATT_BKV))) return rc;
+  if ((rc = make_bshd_map(&tmV, v, B, S, Hk, D, ATT_BKV))) return rc;
   FwdArgs a;
   a.o = reinterpret_cast<__nv_bfloat16*>(o);
   a.lse = lse;

@@ -25,8 +25,8 @@ struct NsGroup {
 size_t newton_schulz_multi_workspace_bytes(const NsGroup* g, int n, int steps);
 int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, float c, void* ws, size_t ws_bytes,
                         cudaStream_t stream);
-int gemm_glu_fwd_2cta(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, cudaStream_t stream);
-int gemm_glu_bwd_2cta(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
+int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, cudaStream_t stream);
+int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
                       cudaStream_t stream);
 size_t embedding_bwd_workspace_bytes(int V, int H);
 int embedding_bwd(const void* dh, const long long* tokens, void* grad, int grad_is_bf16, long long rows, int V, int H,
@@ -112,10 +112,11 @@ void b200_tensor_map_cache_stats(unsigned long long* hits, unsigned long long* m
 }
 
 int b200_device_ok(void) {
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
-  return major == 10 ? 1 : 0;
+  if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+  return (major == 9 && minor == 0) ? 1 : 0;  // the library holds sm_90a code only
 }
 
 int b200_gemm_bf16(int a_mn, int b_mn, int M, int N, int K, int batch, const void* A,
@@ -154,11 +155,11 @@ int b200_newton_schulz_multi(const b200_ns_group* groups, int n_groups, int step
                                    workspace_bytes, S_(stream));
 }
 int b200_mlp_gateup_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, void* stream) {
-  return b200::gemm_glu_fwd_2cta(x, W2, gu, y, M, K, I, S_(stream));
+  return b200::gemm_glu_fwd(x, W2, gu, y, M, K, I, S_(stream));
 }
 int b200_mlp_down_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
                           void* stream) {
-  return b200::gemm_glu_bwd_2cta(dy, Wd, gu, dgu, M, H, I, S_(stream));
+  return b200::gemm_glu_bwd(dy, Wd, gu, dgu, M, H, I, S_(stream));
 }
 size_t b200_embedding_bwd_workspace_bytes(int V, int H) { return b200::embedding_bwd_workspace_bytes(V, H); }
 int b200_embedding_bwd(const void* dh, const long long* tokens, void* grad, int grad_is_bf16, long long rows,

@@ -1,0 +1,575 @@
+// Batched bf16 GEMM engine on Hopper warpgroup MMA (wgmma) fed by TMA through an mbarrier ring.
+//
+// One CTA computes one 128 x 128 output tile (or one K-split of it):
+//   warpgroup 0   producer: one thread streams A[128 x 64] + B[128 x 64] k-blocks (128B-swizzled TMA boxes)
+//                 into a 6-stage ring (32 KB per stage, 192 KB of the 227 KB a block may use)
+//   warpgroups 1-2  consumers: rows [0, 64) and [64, 128) of the tile, wgmma.m64n128k16 with fp32
+//                 accumulators in registers (64 per thread); a stage is handed back once the wgmma batch
+//                 that read it has retired, so one batch is always in flight behind the next TMA wait
+//   epilogue      straight from the accumulator registers: alpha/beta/C, bf16 or fp32 stores, the
+//                 symmetric-output mirror, split-K partials, peer stores and the two fused MLP epilogues.
+// Operand layouts (K-major or MN-major for A and for B) are per-problem run-time flags: they select the TMA
+// box shape and the transpose bits of the wgmma instruction.  Problems of one launch are concatenated work
+// lists (grouped GEMM), which is how the Newton-Schulz chain runs each stage over all shape groups at once.
+#include "common.cuh"
+#include "host.h"
+
+namespace b200 {
+
+namespace {
+
+constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int STAGES = 6;
+constexpr int THREADS = 384;
+constexpr int A_BYTES = BM * BK * 2;  // 16 KB
+constexpr int B_BYTES = BN * BK * 2;  // 16 KB
+constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
+constexpr int MAX_PROBLEMS = 6;
+constexpr int MAX_PEERS = 7;
+constexpr int GROUP_M = 8;  // tile raster: 8 row blocks sweep the columns together (L2 reuse of B)
+
+struct Problem {
+  int M, N, K, batch;
+  int tiles_m, tiles_n, tiles_per_batch, num_kb;
+  int work_begin;  // first work item of this problem in the concatenated list
+  int a_mn, b_mn, symmetric, k_splits, n_peers, out_f32;
+  int epi;         // 0 plain | 1 gate/up + GLU forward | 2 down dgrad + GLU adjoint
+  int n_store;     // columns written per row: N rounded up to the store vector
+  float alpha, beta;
+  const float* alpha_vec;
+  const float* beta_vec;
+  const void* C;
+  long long ldc, strideC;
+  void* D;
+  long long ldd, strideD;
+  float* ws;  // split-K fp32 slabs [k_splits][batch][M][N]
+  void* peer_D[MAX_PEERS];
+  int glu_I;
+  void* aux;  // epi 1: y [M, I] (written); epi 2: gu [M, 2I] (read)
+  long long ld_aux;
+};
+
+struct Args {
+  int n_problems;
+  Problem p[MAX_PROBLEMS];
+  CUtensorMap tmA[MAX_PROBLEMS];
+  CUtensorMap tmB[MAX_PROBLEMS];
+};
+static_assert(sizeof(Args) <= 4096, "kernel parameter block");
+
+__device__ __forceinline__ void tile_coords(const Problem& p, int r, int& mi, int& ni) {
+  if (p.symmetric) {  // upper triangle, row by row
+    int row = 0, len = p.tiles_n;
+    while (r >= len) {
+      r -= len;
+      ++row;
+      --len;
+    }
+    mi = row;
+    ni = row + r;
+    return;
+  }
+  const int per_group = GROUP_M * p.tiles_n;
+  const int first_m = (r / per_group) * GROUP_M;
+  const int gsize = min(p.tiles_m - first_m, GROUP_M);
+  const int rr = r % per_group;
+  mi = first_m + rr % gsize;
+  ni = rr / gsize;
+}
+
+// sigmoid with one special-function op: sigmoid(x) = 0.5 + 0.5 tanh(x / 2)
+__device__ __forceinline__ float fast_sigmoid(float x) {
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
+  return fmaf(0.5f, t, 0.5f);
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_base, uint32_t b_base) {
+  // per k16 step: K-major operands advance 32 B inside the swizzled row, MN-major ones 16 rows of 128 B
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint64_t da = make_wgmma_desc_sw128(a_base + k * (TA ? 2048 : 32), 8192, 1024);
+    const uint64_t db = make_wgmma_desc_sw128(b_base + k * (TB ? 2048 : 32), 8192, 1024);
+    wgmma_m64n128k16_ss<TA, TB>(acc, da, db);
+  }
+}
+
+__device__ __forceinline__ void store_pair(void* D, bool f32, long long off, float v0, float v1) {
+  if (f32)
+    *reinterpret_cast<float2*>(reinterpret_cast<float*>(D) + off) = make_float2(v0, v1);
+  else
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(D) + off) = pack_bf16x2(v0, v1);
+}
+
+__global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ Args g) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const uint32_t sbase = smem_u32(smem);
+  const uint32_t full0 = sbase + STAGES * STAGE_BYTES;
+  const uint32_t empty0 = full0 + STAGES * 8;
+
+  int pi = 0;
+#pragma unroll
+  for (int i = 1; i < MAX_PROBLEMS; ++i)
+    if (i < g.n_problems && (int)blockIdx.x >= g.p[i].work_begin) pi = i;
+  const Problem& p = g.p[pi];
+  int r = blockIdx.x - p.work_begin;
+  const int split = r % p.k_splits;
+  r /= p.k_splits;
+  const int b = r / p.tiles_per_batch;
+  int mi, ni;
+  tile_coords(p, r - b * p.tiles_per_batch, mi, ni);
+  const int kb_per = (p.num_kb + p.k_splits - 1) / p.k_splits;
+  const int kb_begin = split * kb_per;
+  const int kb_end = min(p.num_kb, kb_begin + kb_per);
+  const int wg = threadIdx.x >> 7;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, 2);  // one arrival per consumer warpgroup
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
+      const CUtensorMap* tmA = &g.tmA[pi];
+      const CUtensorMap* tmB = &g.tmB[pi];
+      tma_prefetch_desc(tmA);
+      tma_prefetch_desc(tmB);
+      for (int kb = kb_begin, i = 0; kb < kb_end; ++kb, ++i) {
+        const int s = i % STAGES;
+        const uint32_t ph = (i / STAGES) & 1;
+        mbar_wait(empty0 + 8 * s, ph ^ 1u);
+        const uint32_t full = full0 + 8 * s;
+        mbar_arrive_expect_tx(full, STAGE_BYTES);
+        const uint32_t sA = sbase + s * STAGE_BYTES, sB = sA + A_BYTES;
+        const int k0 = kb * BK;
+        if (p.a_mn) {  // two [64 k-rows x 64 m] boxes
+          tma_load_3d(sA, tmA, full, mi * BM, k0, b);
+          tma_load_3d(sA + 8192, tmA, full, mi * BM + 64, k0, b);
+        } else {
+          tma_load_3d(sA, tmA, full, k0, mi * BM, b);
+        }
+        if (p.epi == 1) {  // 64 gate rows of W2, then the same 64 up rows
+          tma_load_3d(sB, tmB, full, k0, ni * 64, b);
+          tma_load_3d(sB + 8192, tmB, full, k0, p.glu_I + ni * 64, b);
+        } else if (p.b_mn) {
+          tma_load_3d(sB, tmB, full, ni * BN, k0, b);
+          tma_load_3d(sB + 8192, tmB, full, ni * BN + 64, k0, b);
+        } else {
+          tma_load_3d(sB, tmB, full, k0, ni * BN, b);
+        }
+      }
+    }
+    return;
+  }
+
+  const int c = wg - 1;  // rows [64c, 64c + 64) of the tile
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  int prev = -1;
+  for (int kb = kb_begin, i = 0; kb < kb_end; ++kb, ++i) {
+    const int s = i % STAGES;
+    mbar_wait(full0 + 8 * s, (i / STAGES) & 1);
+    const uint32_t sA = sbase + s * STAGE_BYTES + c * 8192, sB = sbase + s * STAGE_BYTES + A_BYTES;
+    wgmma_fence();
+    if (p.a_mn) {
+      if (p.b_mn) mma_kblock<1, 1>(acc, sA, sB);
+      else mma_kblock<1, 0>(acc, sA, sB);
+    } else {
+      if (p.b_mn) mma_kblock<0, 1>(acc, sA, sB);
+      else mma_kblock<0, 0>(acc, sA, sB);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty0 + 8 * prev);
+    prev = s;
+  }
+  wgmma_wait<0>();
+
+  // ---- epilogue: thread owns rows (r0, r0 + 8) x columns (8j + 2q, +1), j = 0..15 ----
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
+  const int r0 = mi * BM + c * 64 + warp * 16 + (lane >> 2);
+  const int cq = (lane & 3) * 2;
+
+  if (p.k_splits > 1) {  // raw fp32 partial of this K range
+    float* ws = p.ws + ((long long)split * p.batch + b) * p.M * (long long)p.N;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = ni * BN + 8 * j + cq;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (row < p.M && col < p.N)
+          *reinterpret_cast<float2*>(ws + (long long)row * p.N + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    }
+    return;
+  }
+
+  if (p.epi == 1) {  // acc columns [0, 64) = gate, [64, 128) = up of the same 64 output columns
+    __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.D);
+    __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(p.aux);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int col = ni * 64 + 8 * j + cq;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (row >= p.M) continue;
+        const float g0 = acc[4 * j + 2 * h], g1 = acc[4 * j + 2 * h + 1];
+        const float u0 = acc[4 * (j + 8) + 2 * h], u1 = acc[4 * (j + 8) + 2 * h + 1];
+        const long long o = (long long)row * p.ldd + col;
+        *reinterpret_cast<uint32_t*>(gu + o) = pack_bf16x2(g0, g1);
+        *reinterpret_cast<uint32_t*>(gu + o + p.glu_I) = pack_bf16x2(u0, u1);
+        *reinterpret_cast<uint32_t*>(y + (long long)row * p.ld_aux + col) =
+            pack_bf16x2(g0 * fast_sigmoid(u0) * 2.0f, g1 * fast_sigmoid(u1) * 2.0f);
+      }
+    }
+    return;
+  }
+
+  if (p.epi == 2) {  // acc = d = dy Wd; dg = d s 2, du = d g s (1 - s) 2 with g, u from the saved gu
+    const __nv_bfloat16* gu = reinterpret_cast<const __nv_bfloat16*>(p.aux);
+    __nv_bfloat16* dgu = reinterpret_cast<__nv_bfloat16*>(p.D);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int col = ni * BN + 8 * j + cq;
+      if (col >= p.glu_I) continue;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        if (row >= p.M) continue;
+        const long long oa = (long long)row * p.ld_aux + col;
+        const float2 gg = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(gu + oa));
+        const float2 uu = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(gu + oa + p.glu_I));
+        const float d0 = acc[4 * j + 2 * h], d1 = acc[4 * j + 2 * h + 1];
+        const float s0 = fast_sigmoid(uu.x), s1 = fast_sigmoid(uu.y);
+        const long long o = (long long)row * p.ldd + col;
+        *reinterpret_cast<uint32_t*>(dgu + o) = pack_bf16x2(d0 * s0 * 2.0f, d1 * s1 * 2.0f);
+        *reinterpret_cast<uint32_t*>(dgu + o + p.glu_I) =
+            pack_bf16x2(d0 * gg.x * s0 * (1.0f - s0) * 2.0f, d1 * gg.y * s1 * (1.0f - s1) * 2.0f);
+      }
+    }
+    return;
+  }
+
+  const float alpha = p.alpha * (p.alpha_vec ? p.alpha_vec[b] : 1.0f);
+  const float beta = p.beta * (p.beta_vec ? p.beta_vec[b] : 1.0f);
+  const bool f32 = p.out_f32 != 0;
+  const bool mirror = p.symmetric && mi != ni;
+  char* Db = reinterpret_cast<char*>(p.D) + (long long)b * p.strideD * (f32 ? 4 : 2);
+  const char* Cb = p.C ? reinterpret_cast<const char*>(p.C) + (long long)b * p.strideC * (f32 ? 4 : 2) : nullptr;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const int col = ni * BN + 8 * j + cq;
+    if (col >= p.n_store) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      if (row >= p.M) continue;
+      float v0 = alpha * acc[4 * j + 2 * h], v1 = alpha * acc[4 * j + 2 * h + 1];
+      if (Cb) {
+        const long long oc = (long long)row * p.ldc + col;
+        if (f32) {
+          const float2 cv = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(Cb) + oc);
+          v0 += beta * cv.x;
+          v1 += beta * cv.y;
+        } else {
+          const float2 cv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(Cb) + oc));
+          v0 += beta * cv.x;
+          v1 += beta * cv.y;
+        }
+      }
+      const long long od = (long long)row * p.ldd + col;
+      store_pair(Db, f32, od, v0, v1);
+      for (int pe = 0; pe < p.n_peers; ++pe)
+        store_pair(reinterpret_cast<char*>(p.peer_D[pe]) + (long long)b * p.strideD * (f32 ? 4 : 2), f32, od, v0, v1);
+      if (mirror) {  // D == D^T: the tile below the diagonal is this one transposed (bf16 only)
+        __nv_bfloat16* Dm = reinterpret_cast<__nv_bfloat16*>(Db);
+        Dm[(long long)col * p.ldd + row] = __float2bfloat16_rn(v0);
+        if (col + 1 < p.N) Dm[(long long)(col + 1) * p.ldd + row] = __float2bfloat16_rn(v1);
+      }
+    }
+  }
+}
+
+// Split-K epilogue: D = bf16(alpha * sum_s ws[s]) in a fixed summation order (deterministic), with the
+// symmetric mode's mirror writes.
+__global__ void __launch_bounds__(256)
+splitk_finalize_kernel(const float* __restrict__ ws, int splits, int batch, int M, int N, __nv_bfloat16* D,
+                       long long ldd, long long strideD, float alpha, const float* __restrict__ alpha_vec,
+                       int symmetric) {
+  const int b = blockIdx.z;
+  const int i = blockIdx.x * 32 + (threadIdx.x & 31);
+  const int j0 = (blockIdx.y * 8 + (threadIdx.x >> 5)) * 8;
+  if (i >= M || j0 >= N) return;
+  const int ti = i / BM, tj = j0 / BN;
+  if (symmetric && ti > tj) return;
+  float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  for (int s = 0; s < splits; ++s) {
+    const float* src = ws + (((long long)s * batch + b) * M + i) * (long long)N + j0;
+    const float4 v0 = *reinterpret_cast<const float4*>(src);
+    const float4 v1 = *reinterpret_cast<const float4*>(src + 4);
+    acc[0] += v0.x; acc[1] += v0.y; acc[2] += v0.z; acc[3] += v0.w;
+    acc[4] += v1.x; acc[5] += v1.y; acc[6] += v1.z; acc[7] += v1.w;
+  }
+  const float a = alpha * (alpha_vec ? alpha_vec[b] : 1.0f);
+  uint4 o;
+  o.x = pack_bf16x2(a * acc[0], a * acc[1]);
+  o.y = pack_bf16x2(a * acc[2], a * acc[3]);
+  o.z = pack_bf16x2(a * acc[4], a * acc[5]);
+  o.w = pack_bf16x2(a * acc[6], a * acc[7]);
+  __nv_bfloat16* dbase = D + (long long)b * strideD;
+  stg128(dbase + (long long)i * ldd + j0, o);
+  if (symmetric && ti != tj) {
+    const uint32_t w[4] = {o.x, o.y, o.z, o.w};
+#pragma unroll
+    for (int t = 0; t < 8; ++t) {
+      const uint16_t h = (t & 1) ? (uint16_t)(w[t >> 1] >> 16) : (uint16_t)(w[t >> 1] & 0xffffu);
+      *reinterpret_cast<uint16_t*>(dbase + (long long)(j0 + t) * ldd + i) = h;
+    }
+  }
+}
+
+// TMA map of one bf16 operand: K-major -> dims {K, rows, batch}, box {64, box_rows};
+// MN-major -> dims {rows, K, batch}, box {64, 64} (two boxes cover a 128-wide tile).
+int operand_map(CUtensorMap* m, const void* base, bool mn, int rows, int K, int batch, long long ld,
+                long long stride, int box_rows) {
+  const uint64_t dims[3] = {(uint64_t)(mn ? rows : K), (uint64_t)(mn ? K : rows), (uint64_t)batch};
+  const uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)(batch > 1 ? stride : (long long)dims[1] * ld) * 2};
+  const uint32_t box[3] = {64, (uint32_t)(mn ? 64 : box_rows), 1};
+  return make_tensor_map(m, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 3, dims, strides, box, true);
+}
+
+Problem base_problem(int M, int N, int K, int batch, int tiles_n, int epi) {
+  Problem q = {};
+  q.M = M;
+  q.N = N;
+  q.K = K;
+  q.batch = batch;
+  q.tiles_m = (M + BM - 1) / BM;
+  q.tiles_n = tiles_n;
+  q.tiles_per_batch = q.tiles_m * tiles_n;
+  q.num_kb = (K + BK - 1) / BK;
+  q.k_splits = 1;
+  q.epi = epi;
+  q.n_store = N;
+  q.alpha = 1.0f;
+  return q;
+}
+
+int launch(Args& a, int n, cudaStream_t stream) {
+  int work = 0;
+  for (int i = 0; i < n; ++i) {
+    a.p[i].work_begin = work;
+    work += a.p[i].tiles_per_batch * a.p[i].batch * a.p[i].k_splits;
+  }
+  a.n_problems = n;
+  static bool attr_set = false;
+  if (!attr_set) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    attr_set = true;
+  }
+  gemm_wgmma_kernel<<<work, THREADS, SMEM_BYTES, stream>>>(a);
+  B200_CHECK_LAUNCH();
+  for (int i = 0; i < n; ++i) {
+    const Problem& q = a.p[i];
+    if (q.k_splits <= 1) continue;
+    const dim3 grid((q.M + 31) / 32, (q.N + 63) / 64, q.batch);
+    splitk_finalize_kernel<<<grid, 256, 0, stream>>>(q.ws, q.k_splits, q.batch, q.M, q.N,
+                                                     reinterpret_cast<__nv_bfloat16*>(q.D), q.ldd, q.strideD, q.alpha,
+                                                     q.alpha_vec, q.symmetric);
+    B200_CHECK_LAUNCH();
+  }
+  return B200_OK;
+}
+
+}  // namespace
+
+// Same contract as gemm_bf16 plus the engine's extra modes; arguments are assumed validated by the caller.
+// symmetric: D == D^T (M == N, bf16 out): only tiles on/above the diagonal are computed, the rest mirror-written.
+// k_splits > 1: K cut into k_splits ranges with fp32 partials in splitk_ws + a deterministic finalize.
+// peer_D: peer-mapped copies of D (other GPUs' buffers) written by the same epilogue.
+int gemm_bf16_ex(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
+                 long long strideA, const void* B, long long ldb, long long strideB, const void* C,
+                 long long ldc, long long strideC, void* D, long long ldd, long long strideD, bool out_f32,
+                 float alpha, float beta, const float* alpha_vec, const float* beta_vec, int symmetric,
+                 int k_splits, float* splitk_ws, const void* const* peer_D, int n_peers, cudaStream_t stream) {
+  if (symmetric && (M != N || out_f32)) symmetric = 0;
+  B200_CHECK_ARG(n_peers >= 0 && n_peers <= MAX_PEERS, "gemm: n_peers=%d out of range (0..%d)", n_peers, MAX_PEERS);
+  B200_CHECK_ARG(n_peers == 0 || (!out_f32 && !symmetric && k_splits <= 1),
+                 "gemm: peer stores need a bf16, non-symmetric, non-split-K output");
+  // split-K needs a plain alpha-only bf16 epilogue and 16-byte partial rows
+  if (k_splits > 1 && (!splitk_ws || out_f32 || beta != 0.0f || (N & 7) != 0)) k_splits = 1;
+  if (k_splits < 1) k_splits = 1;
+  Args a;
+  int rc;
+  if ((rc = operand_map(&a.tmA[0], A, a_mn, M, K, batch, lda, strideA, BM))) return rc;
+  if ((rc = operand_map(&a.tmB[0], B, b_mn, N, K, batch, ldb, strideB, BN))) return rc;
+  const int tiles_n = (N + BN - 1) / BN;
+  Problem& q = a.p[0];
+  q = base_problem(M, N, K, batch, tiles_n, 0);
+  const int vec = out_f32 ? 4 : 8;
+  q.n_store = (N + vec - 1) / vec * vec;
+  if (symmetric) q.tiles_per_batch = q.tiles_m * (q.tiles_m + 1) / 2;
+  q.a_mn = a_mn;
+  q.b_mn = b_mn;
+  q.symmetric = symmetric;
+  q.k_splits = k_splits;
+  q.out_f32 = out_f32;
+  q.alpha = alpha;
+  q.beta = beta;
+  q.alpha_vec = alpha_vec;
+  q.beta_vec = beta_vec;
+  q.C = (beta != 0.0f) ? C : nullptr;
+  q.ldc = ldc;
+  q.strideC = strideC;
+  q.D = D;
+  q.ldd = ldd;
+  q.strideD = strideD;
+  q.ws = splitk_ws;
+  q.n_peers = n_peers;
+  for (int i = 0; i < n_peers; ++i) q.peer_D[i] = const_cast<void*>(peer_D[i]);
+  return launch(a, 1, stream);
+}
+
+// Internal C++ entry (also used by the Newton-Schulz / Shampoo drivers).
+int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
+              long long strideA, const void* B, long long ldb, long long strideB, const void* C,
+              long long ldc, long long strideC, void* D, long long ldd, long long strideD,
+              bool out_f32, float alpha, float beta, const float* alpha_vec, const float* beta_vec,
+              int force_bn, cudaStream_t stream) {
+  B200_CHECK_ARG(M > 0 && N > 0 && K > 0 && batch > 0, "gemm: empty problem M=%d N=%d K=%d b=%d", M,
+                 N, K, batch);
+  B200_CHECK_ARG(lda % 8 == 0 && ldb % 8 == 0, "gemm: lda=%lld ldb=%lld must be multiples of 8", lda,
+                 ldb);
+  const int out_vec = out_f32 ? 4 : 8;
+  // N need not be a multiple of the store vector as long as the padded row exists: columns
+  // [N, round_up(N, vec)) of D receive alpha*0 + beta*C (B rows >= N are zero-filled by TMA).  Used by
+  // Shampoo's [259, 259] factor of the byte-level embedding (stored with ld = 264).
+  {
+    const long long n_pad = ((long long)N + out_vec - 1) / out_vec * out_vec;
+    B200_CHECK_ARG(N % out_vec == 0 || (ldd >= n_pad && (C == nullptr || ldc >= n_pad) && force_bn != 1256),
+                   "gemm: N=%d is not a multiple of %d and ldd=%lld/ldc=%lld leave no room for the padded vector",
+                   N, out_vec, ldd, ldc);
+  }
+  B200_CHECK_ARG(ldd % out_vec == 0 && (C == nullptr || ldc % out_vec == 0),
+                 "gemm: ldd=%lld ldc=%lld must be multiples of %d", ldd, ldc, out_vec);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(D) & 15u) == 0 &&
+                     (reinterpret_cast<uintptr_t>(C) & 15u) == 0,
+                 "gemm: C/D must be 16-byte aligned");
+  B200_CHECK_ARG(strideA % 8 == 0 && strideB % 8 == 0 && strideD % out_vec == 0 &&
+                     strideC % out_vec == 0,
+                 "gemm: batch strides must keep 16-byte alignment");
+  // force_bn: 0 / 128 / 256 = tile-width hints (the engine's tiles are 128 wide) | 1256 = D == D^T asserted
+  return gemm_bf16_ex(a_mn, b_mn, M, N, K, batch, A, lda, strideA, B, ldb, strideB, C, ldc, strideC, D, ldd, strideD,
+                      out_f32, alpha, beta, alpha_vec, beta_vec, force_bn == 1256 ? 1 : 0, 1, nullptr, nullptr, 0,
+                      stream);
+}
+
+// ---- fused MLP GEMMs (arch/llama.py:142-151: down(gate(x) * sigmoid(up(x)) * 2)) --------------------------
+// gu[M, 2I] = x[M, K] [Wg ; Wu]^T (W2: [2I, K] row-major, gate rows first), y[M, I] = g * sigmoid(u) * 2
+int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, cudaStream_t stream) {
+  B200_CHECK_ARG(M > 0 && K > 0 && I > 0 && K % 8 == 0 && I % 128 == 0,
+                 "mlp_glu_fwd: need K %% 8 == 0 and intermediate size %% 128 == 0 (M=%d K=%d I=%d)", M, K, I);
+  Args a;
+  int rc;
+  if ((rc = operand_map(&a.tmA[0], x, false, M, K, 1, K, 0, BM))) return rc;
+  if ((rc = operand_map(&a.tmB[0], W2, false, 2 * I, K, 1, K, 0, 64))) return rc;
+  Problem& q = a.p[0];
+  q = base_problem(M, I, K, 1, I / 64, 1);
+  q.D = gu;
+  q.ldd = 2LL * I;
+  q.glu_I = I;
+  q.aux = y;
+  q.ld_aux = I;
+  return launch(a, 1, stream);
+}
+
+// dgu[M, 2I] = GLU adjoint of d = dy[M, H] Wd (Wd: [H, I] row-major = down_proj.weight), gu[M, 2I] the saved
+// forward activations: dg = d * sigmoid(u) * 2 ; du = d * g * sigmoid(u) * (1 - sigmoid(u)) * 2
+int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I, cudaStream_t stream) {
+  B200_CHECK_ARG(M > 0 && H > 0 && I > 0 && H % 8 == 0 && I % 8 == 0, "mlp_glu_bwd: bad shape M=%d H=%d I=%d", M, H, I);
+  Args a;
+  int rc;
+  if ((rc = operand_map(&a.tmA[0], dy, false, M, H, 1, H, 0, BM))) return rc;
+  // B[n = i, k = h] = Wd[h, i]: stored [K = H rows][N = I]: MN-major
+  if ((rc = operand_map(&a.tmB[0], Wd, true, I, H, 1, I, 0, BN))) return rc;
+  Problem& q = a.p[0];
+  q = base_problem(M, I, H, 1, (I + BN - 1) / BN, 2);
+  q.b_mn = 1;
+  q.D = dgu;
+  q.ldd = 2LL * I;
+  q.glu_I = I;
+  q.aux = const_cast<void*>(gu);
+  q.ld_aux = 2LL * I;
+  return launch(a, 1, stream);
+}
+
+// ---- grouped launch: up to MAX_PROBLEMS independent batched problems in one grid ----------------------------
+// Problems are bf16-out; `k_splits` > 1 requests split-K into fp32 slabs (splitk_ws) + a finalize pass.  Work
+// items are ordered heaviest K range first, so the tail of the launch is made of the cheapest tiles.
+int gemm_grouped(const GroupedGemm* probs, int n, cudaStream_t stream) {
+  B200_CHECK_ARG(n >= 1 && n <= MAX_PROBLEMS, "grouped gemm: %d problems (1..%d supported)", n, MAX_PROBLEMS);
+  int order[MAX_PROBLEMS];
+  for (int i = 0; i < n; ++i) order[i] = i;
+  auto item_kb = [&](int i) {
+    const int num_kb = (probs[i].K + BK - 1) / BK;
+    const int ks = probs[i].k_splits > 1 ? probs[i].k_splits : 1;
+    return (num_kb + ks - 1) / ks;
+  };
+  for (int i = 1; i < n; ++i)
+    for (int j = i; j > 0 && item_kb(order[j]) > item_kb(order[j - 1]); --j) {
+      const int t = order[j];
+      order[j] = order[j - 1];
+      order[j - 1] = t;
+    }
+  Args a;
+  for (int oi = 0; oi < n; ++oi) {
+    const GroupedGemm& h = probs[order[oi]];
+    B200_CHECK_ARG(h.M > 0 && h.N > 0 && h.K > 0 && h.batch > 0 && h.N % 8 == 0,
+                   "grouped gemm: problem %d has an unsupported shape M=%d N=%d K=%d batch=%d", order[oi], h.M, h.N,
+                   h.K, h.batch);
+    B200_CHECK_ARG(h.lda % 8 == 0 && h.ldb % 8 == 0 && h.ldd % 8 == 0 && (h.C == nullptr || h.ldc % 8 == 0),
+                   "grouped gemm: leading dimensions must be multiples of 8");
+    B200_CHECK_ARG(h.n_peers >= 0 && h.n_peers <= MAX_PEERS, "grouped gemm: n_peers out of range");
+    const int symmetric = (h.symmetric && h.M == h.N) ? 1 : 0;
+    int k_splits = h.k_splits > 1 ? h.k_splits : 1;
+    if (k_splits > 1 && (h.splitk_ws == nullptr || h.beta != 0.0f)) k_splits = 1;
+    B200_CHECK_ARG(h.n_peers == 0 || (!symmetric && k_splits == 1),
+                   "grouped gemm: peer stores need a non-symmetric, non-split-K problem");
+    int rc;
+    if ((rc = operand_map(&a.tmA[oi], h.A, h.a_mn, h.M, h.K, h.batch, h.lda, h.strideA, BM))) return rc;
+    if ((rc = operand_map(&a.tmB[oi], h.B, h.b_mn, h.N, h.K, h.batch, h.ldb, h.strideB, BN))) return rc;
+    Problem& q = a.p[oi];
+    q = base_problem(h.M, h.N, h.K, h.batch, (h.N + BN - 1) / BN, 0);
+    if (symmetric) q.tiles_per_batch = q.tiles_m * (q.tiles_m + 1) / 2;
+    q.a_mn = h.a_mn;
+    q.b_mn = h.b_mn;
+    q.symmetric = symmetric;
+    q.k_splits = k_splits;
+    q.alpha = h.alpha;
+    q.beta = h.beta;
+    q.alpha_vec = h.alpha_vec;
+    q.beta_vec = h.beta_vec;
+    q.C = (h.beta != 0.0f) ? h.C : nullptr;
+    q.ldc = h.ldc;
+    q.strideC = h.strideC;
+    q.D = h.D;
+    q.ldd = h.ldd;
+    q.strideD = h.strideD;
+    q.ws = h.splitk_ws;
+    q.n_peers = h.n_peers;
+    for (int i = 0; i < h.n_peers; ++i) q.peer_D[i] = const_cast<void*>(h.peer_D[i]);
+  }
+  return launch(a, n, stream);
+}
+
+}  // namespace b200

@@ -62,7 +62,7 @@ int make_tensor_map(CUtensorMap* out, const void* base, CUtensorMapDataType dtyp
 
 int num_sms();
 
-// One problem of a grouped CTA-pair GEMM launch (gemm_tc2.cu: gemm_grouped_2cta): D = alpha*av[b]*op(A)op(B) +
+// One problem of a grouped GEMM launch (gemm_wgmma.cu: gemm_grouped): D = alpha*av[b]*op(A)op(B) +
 // beta*bv[b]*C, bf16 in/out, batched; layouts as in b200_gemm_bf16.
 struct GroupedGemm {
   bool a_mn, b_mn;
@@ -84,6 +84,6 @@ struct GroupedGemm {
   const void* const* peer_D;  // GEMM -> all-gather: peer-mapped copies of D (n_peers <= 7)
   int n_peers;
 };
-int gemm_grouped_2cta(const GroupedGemm* probs, int n, cudaStream_t stream);
+int gemm_grouped(const GroupedGemm* probs, int n, cudaStream_t stream);
 
 }  // namespace b200

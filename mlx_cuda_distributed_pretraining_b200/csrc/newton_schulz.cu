@@ -1,7 +1,7 @@
 // Newton-Schulz orthogonalisation driver (reference: Muon.zeropower_via_newtonschulz5,
 // optimizers/muon.py:54-83):   X0 = G/(||G||_F+eps);  repeat: A = X X^T, B = bA + cAA, X = aX + BX
 //
-// B200 formulation: every step is a batched tcgen05 GEMM with a fused epilogue
+// Formulation: every step is a batched wgmma GEMM (gemm_wgmma.cu) with a fused epilogue
 //   G1: A  = X X^T                (wide)   |  A = X^T X   (tall, both operands MN-major)
 //   G2: B  = b*A + c*(A A)        (A symmetric -> A A^T, both operands K-major)
 //   G3: X' = a*X + B X            (wide, X as MN-major B operand) | X' = a*X + X B (tall)
@@ -20,11 +20,10 @@ int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* 
               bool out_f32, float alpha, float beta, const float* alpha_vec, const float* beta_vec,
               int force_bn, cudaStream_t stream);
 
-int gemm_bf16_2cta(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
+int gemm_bf16_ex(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
                    long long strideA, const void* B, long long ldb, long long strideB, const void* C,
                    long long ldc, long long strideC, void* D, long long ldd, long long strideD, bool out_f32,
-                   float alpha, float beta, const float* alpha_vec, const float* beta_vec, int bn,
-                   int symmetric, int k_splits, float* splitk_ws, const void* const* peer_D, int n_peers,
+                   float alpha, float beta, const float* alpha_vec, const float* beta_vec, int symmetric, int k_splits, float* splitk_ws, const void* const* peer_D, int n_peers,
                    cudaStream_t stream);
 
 static inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
@@ -40,16 +39,16 @@ struct NsGroup {
   int n_peers;
 };
 
-// G1 of a lone big matrix (the 32003 x 1024 embedding: 10 symmetric tiles, K = 32003) would occupy a
-// fraction of the CTA pairs for hundreds of microseconds.  Cut K so that every pair gets a work item.
+// G1 of a lone big matrix (the 32003 x 1024 embedding: 36 symmetric 128-tiles, K = 32003) would occupy a
+// fraction of the SMs for hundreds of microseconds.  Cut K so that every SM gets a work item.
 static int g1_k_splits(int batch, int m, int k) {
   if (m <= 128 || (m & 7) != 0) return 1;
-  const int t = (m + 255) / 256;
+  const int t = (m + 127) / 128;
   const long long tiles = (long long)t * (t + 1) / 2 * batch;
-  const int pairs = num_sms() / 2;
-  if (tiles * 2 > pairs) return 1;
+  const int ctas = num_sms();
+  if (tiles * 2 > ctas) return 1;
   const int num_kb = (k + 63) / 64;
-  int s = (int)(pairs / tiles);
+  int s = (int)(ctas / tiles);
   if (s > num_kb / 16) s = num_kb / 16;
   return s < 2 ? 1 : s;
 }
@@ -109,8 +108,8 @@ int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, 
     int rc_;
     // G1
     if (splits > 1)
-      rc_ = gemm_bf16_2cta(tall, tall, m, m, tall ? rows : cols, batch, cur, cols, rc, cur, cols, rc, nullptr,
-                           0, 0, Abuf, m, mm, false, 1.0f, 0.0f, s2, nullptr, 256, 1, splits, splitk_ws,
+      rc_ = gemm_bf16_ex(tall, tall, m, m, tall ? rows : cols, batch, cur, cols, rc, cur, cols, rc, nullptr,
+                           0, 0, Abuf, m, mm, false, 1.0f, 0.0f, s2, nullptr, 1, splits, splitk_ws,
                            nullptr, 0, stream);
     else if (!tall)
       rc_ = gemm_bf16(false, false, m, m, cols, batch, cur, cols, rc, cur, cols, rc, nullptr, 0, 0,
@@ -125,31 +124,14 @@ int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, 
     if (rc_) return rc_;
     // G3 (the last one carries the peer stores)
     const bool last = it == steps - 1;
-    const int g3_m = tall ? rows : m, g3_n = tall ? m : cols;
-    if (last && n_peers > 0 && g3_m > 128) {
-      // CTA-pair kernel directly: tile-N choice as in gemm_bf16
-      const long long t256 = (long long)((g3_m + 255) / 256) * ((g3_n + 255) / 256) * batch;
-      const int bn2 = (g3_n <= 128 || t256 < (num_sms() / 2) * 3 / 4) ? 128 : 256;
-      if (!tall)
-        rc_ = gemm_bf16_2cta(false, true, m, cols, m, batch, Bbuf, m, mm, cur, cols, rc, cur, cols, rc, nxt, cols,
-                             rc, false, 1.0f, a, s1, s1, bn2, 0, 1, nullptr, peer_out, n_peers, stream);
-      else
-        rc_ = gemm_bf16_2cta(false, false, rows, m, m, batch, cur, cols, rc, Bbuf, m, mm, cur, cols, rc, nxt, cols,
-                             rc, false, 1.0f, a, s1, s1, bn2, 0, 1, nullptr, peer_out, n_peers, stream);
-    } else {
-      if (!tall)
-        rc_ = gemm_bf16(false, true, m, cols, m, batch, Bbuf, m, mm, cur, cols, rc, cur, cols, rc,
-                        nxt, cols, rc, false, 1.0f, a, s1, s1, 0, stream);
-      else
-        rc_ = gemm_bf16(false, false, rows, m, m, batch, cur, cols, rc, Bbuf, m, mm, cur, cols, rc,
-                        nxt, cols, rc, false, 1.0f, a, s1, s1, 0, stream);
-      if (rc_ == 0 && last && n_peers > 0) {
-        // small matrices run on the single-CTA kernel, which has no peer epilogue: copy the result out
-        for (int pi = 0; pi < n_peers; ++pi)
-          B200_CHECK_CUDA(cudaMemcpyAsync(const_cast<void*>(peer_out[pi]), nxt, (size_t)batch * rc * 2,
-                                          cudaMemcpyDeviceToDevice, stream));
-      }
-    }
+    const void* const* peers = last ? peer_out : nullptr;
+    const int np = last ? n_peers : 0;
+    if (!tall)
+      rc_ = gemm_bf16_ex(false, true, m, cols, m, batch, Bbuf, m, mm, cur, cols, rc, cur, cols, rc, nxt, cols, rc,
+                         false, 1.0f, a, s1, s1, 0, 1, nullptr, peers, np, stream);
+    else
+      rc_ = gemm_bf16_ex(false, false, rows, m, m, batch, cur, cols, rc, Bbuf, m, mm, cur, cols, rc, nxt, cols, rc,
+                         false, 1.0f, a, s1, s1, 0, 1, nullptr, peers, np, stream);
     if (rc_) return rc_;
     cur = nxt;
   }
@@ -159,11 +141,10 @@ int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, 
 
 // ---------------------------------------------------------------------------------------------------------
 // Whole-model chain: every shape group of the optimizer advances through the SAME iteration together, so each
-// stage (A = X X^T | B = bA + cAA | X' = aX + BX) is ONE grouped launch over all groups (gemm_tc2.cu) instead of
-// one launch per group: 3 launches per iteration (+ one split-K finalize for a lone tall matrix) instead of
-// 3 x groups, and the per-launch wave tail is amortised over all groups' tiles (C2: 682 instead of 240 tiles
-// for the B stage on 74 CTA pairs).  Falls back to the per-group chain when a group is too small for the
-// CTA-pair kernel (min(rows, cols) <= 128) or there are more groups than one launch takes.
+// stage (A = X X^T | B = bA + cAA | X' = aX + BX) is ONE grouped launch over all groups (gemm_wgmma.cu) instead
+// of one launch per group: 3 launches per iteration (+ one split-K finalize for a lone tall matrix) instead of
+// 3 x groups, and the per-launch wave tail is amortised over all groups' tiles.  Falls back to the per-group
+// chain for small groups (min(rows, cols) <= 128) or when there are more groups than one launch takes.
 // ---------------------------------------------------------------------------------------------------------
 static bool multi_grouped_ok(const NsGroup* g, int n) {
   static const bool off = [] {
@@ -276,7 +257,7 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       q.k_splits = lay[i].splits;
       q.splitk_ws = reinterpret_cast<float*>(w + lay[i].splitk);
     }
-    int rc = gemm_grouped_2cta(pr, n, stream);
+    int rc = gemm_grouped(pr, n, stream);
     if (rc) return rc;
     // ---- G2: B = b A + c A A (A symmetric: A A^T with both operands K-major) ----
     for (int i = 0; i < n; ++i) {
@@ -295,7 +276,7 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       q.symmetric = kSym ? 1 : 0;
       q.k_splits = 1;
     }
-    rc = gemm_grouped_2cta(pr, n, stream);
+    rc = gemm_grouped(pr, n, stream);
     if (rc) return rc;
     // ---- G3: X' = a X + B X (wide) / a X + X B (tall); the last one carries the peer stores ----
     for (int i = 0; i < n; ++i) {
@@ -348,7 +329,7 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       }
       cur[i] = nxt;
     }
-    rc = gemm_grouped_2cta(pr, n, stream);
+    rc = gemm_grouped(pr, n, stream);
     if (rc) return rc;
   }
   return B200_OK;

@@ -1,5 +1,5 @@
 // Shampoo's Kronecker-factor path (reference: optimizers/shampoo.py) as C-ABI orchestration over the
-// tcgen05 GEMM engine, batched over the same-shape parameters of a flat.ParamStore group:
+// wgmma GEMM engine, batched over the same-shape parameters of a flat.ParamStore group:
 //
 //   shampoo_stats    :229-255   L = b2 L + (1-b2) G G^T ; R = b2 R + (1-b2) G^T G   on G[:k1,:k2]
 //   shampoo_root     :88-126    MatrixSqrt.matrix_inverse_pth_root, literally:
@@ -8,7 +8,7 @@
 //   shampoo_graft    :297-312 + :365-373   ||upd||, ||graft|| -> rescale -> p = p*decay + upd
 //
 // fp32 matrices enter the tensor cores as bf16 hi+lo pairs (hi*hi + hi*lo + lo*hi: three accumulating
-// GEMMs with fp32 accumulation in TMEM, ~16 mantissa bits), so statistics and roots track the reference's
+// GEMMs with fp32 accumulation, ~16 mantissa bits), so statistics and roots track the reference's
 // fp32 matmuls to ~1e-5 instead of bf16's 4e-3.  Factor matrices are stored [batch, kp, kp] with
 // kp = round_up(k, 8) (16-byte TMA rows) and zero padding; trace / identity use the true k, so the padding
 // stays exactly zero through the iteration (block-diagonal with a zero block).

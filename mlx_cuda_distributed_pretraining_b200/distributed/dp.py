@@ -1,4 +1,4 @@
-"""Data-parallel plumbing: one process per GPU (torchrun), NCCL over NVLink 5 / NVSwitch.
+"""Data-parallel plumbing: one process per GPU (torchrun), NCCL over NVLink 4 / NVSwitch.
 
 Replaces the reference's thread-queue "devices" and Python gradient averaging
 (distributed/utils.py:8-226, distributed/hybrid_distributed.py:303-354,430-452,495-522).  The DP

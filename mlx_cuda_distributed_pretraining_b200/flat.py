@@ -1,6 +1,6 @@
 """Shape-grouped flat storage for parameters, gradients and fp32 masters.
 
-HBM layout (one allocation each, sized for 180 GB parts -- nothing is sharded or offloaded):
+HBM layout (one allocation each, sized for one 80 GB H100 -- nothing is sharded or offloaded):
 
     master  fp32  [ group(r0,c0): batch0 x r0 x c0 | group(r1,c1): ... | all non-2-D params ]
     shadow  bf16  same layout (only with mixed precision): what forward/backward read

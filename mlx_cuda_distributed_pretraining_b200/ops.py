@@ -1,7 +1,7 @@
 """PyTorch-tensor wrappers over the C ABI (include/b200_hotpath.h).
 
 PyTorch is plumbing here: it owns device memory and streams; all arithmetic below runs in the
-hand-written sm_100a kernels.  Every wrapper validates dtype/contiguity and raises on failure --
+hand-written sm_90a kernels.  Every wrapper validates dtype/contiguity and raises on failure --
 there is no eager fallback.
 """
 from __future__ import annotations
@@ -19,7 +19,7 @@ NS_EPS = 1e-7                          # optimizers/muon.py:73
 
 def _stream() -> int:
     # raw handle of torch's current stream on the current device; torch.cuda.current_stream() builds a Stream
-    # object (~17 us per call measured, ~100 calls per C2 step: tools/host_profile.py)
+    # object on every call (~100 calls per C2 step)
     return torch._C._cuda_getCurrentRawStream(torch._C._cuda_getDevice())
 
 
@@ -189,7 +189,7 @@ def zeropower_via_newtonschulz5(g: torch.Tensor, steps: int = 5, eps: float = NS
                                 coeffs: Sequence[float] = NS_COEFFS) -> torch.Tensor:
     """Drop-in for Muon.zeropower_via_newtonschulz5 (optimizers/muon.py:54-83).
 
-    g: [rows, cols] or [batch, rows, cols], fp32 or bf16 on a B200. Returns bf16 of the same shape.
+    g: [rows, cols] or [batch, rows, cols], fp32 or bf16 on an H100. Returns bf16 of the same shape.
     """
     require_device()
     squeeze = g.dim() == 2
@@ -865,10 +865,10 @@ def _adjacent_rows(w_a: torch.Tensor, w_b: torch.Tensor) -> bool:
 class _MlpFn(torch.autograd.Function):
     """down( gate(x) * sigmoid(up(x)) * 2 )  (arch/llama.py:142-151) with the activation inside the GEMM epilogues:
 
-      forward   [g | u], y = b200_mlp_gateup_glu_fwd(x, [Wg ; Wu])      one tcgen05 kernel (in-tree engine)
+      forward   [g | u], y = b200_mlp_gateup_glu_fwd(x, [Wg ; Wu])      one wgmma kernel (in-tree engine)
                 out        = y Wd^T                                      library GEMM
       backward  dWd       += dout^T y                                    library GEMM into the flat gradient
-                [dg | du]  = b200_mlp_down_glu_bwd(dout, Wd, [g | u])    one tcgen05 kernel: dout Wd never leaves the chip
+                [dg | du]  = b200_mlp_down_glu_bwd(dout, Wd, [g | u])    one wgmma kernel: dout Wd never leaves the chip
                 dx         = [dg | du] [Wg ; Wu]                         ONE library GEMM (K = 2I) instead of two
                 d[Wg ; Wu] += [dg | du]^T x                              ONE library GEMM into the flat gradient
 

@@ -1,4 +1,4 @@
-"""Muon with the reference's surface (optimizers/muon.py:7-141), running on the sm_100a kernels.
+"""Muon with the reference's surface (optimizers/muon.py:7-141), running on the sm_90a kernels.
 
     opt = Muon(learning_rate=float|callable, momentum=0.95, nesterov=True, ns_steps=5,
                alternate_optimizer=None, betas=None, eps=None, weight_decay=None)
@@ -8,7 +8,7 @@
 Semantics follow the reference's intended math with its wiring defects fixed (SURVEY D1, D2):
 gradients are matched by flattened name and the update is applied to the model in place.
 Per 2-D shape group the step is: fused momentum+Nesterov+sum-of-squares pass -> batched
-Newton-Schulz on tcgen05 -> fused `p += -lr*max(1,r/c)^0.5 * X` pass (fp32 master + bf16 shadow).
+Newton-Schulz on wgmma -> fused `p += -lr*max(1,r/c)^0.5 * X` pass (fp32 master + bf16 shadow).
 Non-2-D parameters go to `alternate_optimizer` if given, else to the SGD-momentum fallback
 (muon.py:119-138).  `betas/eps/weight_decay` are accepted and ignored, as in the reference (:41-52).
 
@@ -154,7 +154,7 @@ class Muon:
             ops.check(lib.b200_ns_scales(self._ss.data_ptr(), self._inv.data_ptr(), self._inv2.data_ptr(),
                                          self._ss.numel(), ops.NS_EPS, stream), "b200_ns_scales")
             # 2. Newton-Schulz on the matrices this rank owns, all groups advancing together: every stage of the
-            #    iteration is one grouped tcgen05 launch (b200_newton_schulz_multi)
+            #    iteration is one grouped wgmma launch (b200_newton_schulz_multi)
             entries, keep = [], []
             for gi, g in enumerate(groups):
                 rc = g.rows * g.cols
@@ -239,8 +239,8 @@ class Muon:
                 bufs = [symm.empty(n, dtype=torch.bfloat16, device=store.device) for n in sizes]
                 self._xg_handles = [symm.rendezvous(t, group=dist.group.WORLD) for t in bufs]
                 self._xg = bufs
-                # multicast pays off once a unicast exchange would send several copies (measured at 2 ranks:
-                # one unicast copy 27.5 ms/step vs multicast 28.0); B200_NS_MULTICAST=1/0 forces it on/off
+                # multicast pays off once a unicast exchange would send several copies; B200_NS_MULTICAST=1/0 forces
+                # it on/off
                 mc_env = os.environ.get("B200_NS_MULTICAST", "auto")
                 mc_ok = all(int(getattr(h, "multicast_ptr", 0) or 0) != 0 for h in self._xg_handles)
                 self._use_multicast = mc_ok and (mc_env == "1" or (mc_env == "auto" and world >= 4))

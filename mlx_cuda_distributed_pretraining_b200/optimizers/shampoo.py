@@ -1,4 +1,4 @@
-"""Shampoo with the reference's surface (optimizers/shampoo.py:20-45,143-378) on the sm_100a GEMM
+"""Shampoo with the reference's surface (optimizers/shampoo.py:20-45,143-378) on the sm_90a GEMM
 engine, orchestrated through the C ABI's b200_shampoo_* entry points (include/b200_hotpath.h).
 
     opt = Shampoo(learning_rate=float|callable, params=ShampooParams(...))
@@ -17,7 +17,7 @@ Per step (shampoo.py:314-378, with the wiring defects D1/D2/D9 of SURVEY 2.3 fix
                                                                                            b200_shampoo_graft
 
 All matrix products are batched over the same-shape parameters of a flat.ParamStore group and run on
-tcgen05.  fp32 matrices enter the tensor cores as bf16 hi+lo pairs (hi*hi + hi*lo + lo*hi, three
+wgmma.  fp32 matrices enter the tensor cores as bf16 hi+lo pairs (hi*hi + hi*lo + lo*hi, three
 accumulating GEMMs, ~16 mantissa bits) so statistics/roots stay close to the reference's fp32 matmuls;
 bf16 gradients (mixed precision) are used as they are, fp32 gradients are split the same way.
 State per parameter mirrors the reference's (:180-208): momentum, statistics.0/1, preconditioners.0/1

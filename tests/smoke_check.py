@@ -7,6 +7,7 @@ Used by __graft_entry__.smoke(); the oracle is the checker here, never the thing
 from __future__ import annotations
 
 import sys
+import tempfile
 from pathlib import Path
 
 import torch
@@ -77,13 +78,13 @@ def smoke(verbose: bool = True) -> dict:
     out["attn_dq"], out["attn_dk"], out["attn_dv"] = _rel(qc.grad, qr.grad), _rel(kc.grad, kr.grad), _rel(vc.grad, vr.grad)
     assert max(out["attn_o"], out["attn_dq"], out["attn_dk"], out["attn_dv"]) < 2e-2, out
     # 3. one full training step through the Trainer vs the oracle's step
-    tr = Trainer(Config.from_dict(tiny_config()), synthetic=True, quiet=True,
-                 run_root=str(ROOT / "gpurun_out" / "smoke_runs"))
-    tr._accum_step, tr._accum_tokens = 0, 0
-    d = R.LlamaDims(128, 256, 2, 4, 2, 32, 259)
-    params = {n: t.detach().cpu().clone() for n, t in tr.store.named_master().items()}
-    batch = tr.data_manager.generate_batch(0)
-    loss, ntoks, _ = tr.train_step(0, batch)
+    with tempfile.TemporaryDirectory(prefix="smoke_runs_") as run_root:
+        tr = Trainer(Config.from_dict(tiny_config()), synthetic=True, quiet=True, run_root=run_root)
+        tr._accum_step, tr._accum_tokens = 0, 0
+        d = R.LlamaDims(128, 256, 2, 4, 2, 32, 259)
+        params = {n: t.detach().cpu().clone() for n, t in tr.store.named_master().items()}
+        batch = tr.data_manager.generate_batch(0)
+        loss, ntoks, _ = tr.train_step(0, batch)
     loss_ref, _, grads = R.loss_and_grads(params, batch, d, pad_token=256)
     out["loss"], out["loss_ref"] = float(loss), float(loss_ref)
     assert abs(out["loss"] - out["loss_ref"]) < 2e-2, out
@@ -97,7 +98,7 @@ def smoke(verbose: bool = True) -> dict:
         if delta_ref.norm() > 0:
             worst = max(worst, _rel(delta, delta_ref))
     out["worst_param_delta_rel"] = worst
-    assert worst < 0.15, out   # bf16 fwd/bwd gradients through NS5; see DESIGN.md tolerances
+    assert worst < 0.15, out   # bf16 fwd/bwd gradients through NS5; DESIGN.md §5 tolerances
     if verbose:
         print("smoke ok:", {k: (round(v, 5) if isinstance(v, float) else v) for k, v in out.items()})
     return out

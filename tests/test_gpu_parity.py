@@ -168,7 +168,7 @@ def test_muon_momentum_and_scales(ops, gdt):
 
 
 def test_muon_update_golden(ops, golden):
-    """The product's Muon.update(model, gradients) -- momentum, Nesterov, Newton-Schulz on tcgen05, scaled apply,
+    """The product's Muon.update(model, gradients) -- momentum, Nesterov, Newton-Schulz on wgmma, scaled apply,
     SGD-momentum fallback for the 1-D parameter -- against two steps of the REFERENCE's own optimizers/muon.py
     (callable learning rate, explicit gradient dict, as the reference trainer calls it)."""
     from mlx_cuda_distributed_pretraining_b200.optimizers.muon import Muon
@@ -803,7 +803,7 @@ def test_attention_fp32_path_large_logits(ops, B, S, H, Hk, D):
 @pytest.mark.parametrize("M,K,I", [(300, 128, 256), (1024, 1024, 2816), (515, 256, 384)])
 def test_mlp_fused_glu_epilogues(ops, M, K, I):
     """The MLP block on the in-tree GEMM engine (b200_mlp_gateup_glu_fwd / b200_mlp_down_glu_bwd: gate*sigmoid(up)*2 and
-    its adjoint inside the tcgen05 epilogues, arch/llama.py:149-151) against fp32 autograd of the same formula, and
+    its adjoint inside the wgmma epilogues, arch/llama.py:149-151) against fp32 autograd of the same formula, and
     against the unfused path (library GEMMs + glu kernels)."""
     torch.manual_seed(80 + I)
     wflat = (torch.randn(2 * I * K, device="cuda") * K ** -0.5).to(torch.bfloat16)

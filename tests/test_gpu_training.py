@@ -74,7 +74,6 @@ def test_muon_steps_track_oracle(tmp_path):
 def test_adamw_fp32_steps_track_oracle(tmp_path):
     # lr 2e-3: at the tiny config's default 2e-2 this model diverges within three AdamW steps (attention scores
     # reach +-170, loss goes up), and a per-step comparison of a chaotic trajectory measures rounding luck
-    # (tools/attn_debug.py replays it: every attention call stays within bf16 error of the dense reference)
     tr = make_trainer(tmp_path, optimizer="adamw", mixed=False, hp__learning_rate=2e-3)
     for step in range(4):
         batch = tr.data_manager.generate_batch(step)
@@ -382,10 +381,10 @@ def test_c1_loss_curve_matches_oracle(tmp_path, data, lr):
       markov, lr 1e-3  control: same stream with a learning rate that does NOT blow up in the first steps
     With the config's own lr 2e-2 (AdamW without bias correction, no warm-up) the loss explodes to 9-10 around steps
     3-8; that transient is chaotic (the fp32 and fp64 ORACLES differ by 1-2 there, a 1e-6 weight perturbation moves
-    step 6 by 3.9: tools/c1_transient_chaos.py, profiles/r02_c1_transient_chaos.txt), so step-by-step agreement is
+    step 6 by 3.9), so step-by-step agreement is
     asserted before it (steps 0-2) and after it has died out; on the learnable stream the two runs then sit in
     different basins and agree as trajectories (smoothed), not step by step.  The lr-1e-3 control has no such
-    transient and must agree step by step throughout.  Measured values: gpurun_out/c1_curve_*.json -> profiles/."""
+    transient and must agree step by step throughout."""
     import yaml
     from mlx_cuda_distributed_pretraining_b200.core.training import Config, Trainer
     tag = data + (f"_lr{lr:g}" if lr is not None else "")
@@ -413,9 +412,7 @@ def test_c1_loss_curve_matches_oracle(tmp_path, data, lr):
     k = 25
     smooth = lambda t: torch.nn.functional.avg_pool1d(t[None, None], k, 1)[0, 0] if len(t) >= k else t   # noqa: E731
     sdiff = (smooth(got) - smooth(want)).abs()
-    out = ROOT / "gpurun_out"
-    out.mkdir(exist_ok=True)
-    (out / f"c1_curve_{tag}.json").write_text(json.dumps({
+    (tmp_path / f"c1_curve_{tag}.json").write_text(json.dumps({
         "steps": n, "max_abs_diff": float(diff.max()), "argmax": int(diff.argmax()), "mean_abs_diff": float(diff.mean()),
         "head_0_2": float(diff[:3].max()), "max_30_99": float(diff[30:100].max()) if n > 100 else None,
         "max_from_100": float(diff[100:].max()) if n > 100 else None,
@@ -441,8 +438,7 @@ def test_c1_loss_curve_matches_oracle(tmp_path, data, lr):
 
 
 # |loss_gpu - loss_oracle| bounds.  The GPU run is itself not bit-reproducible (dQ is accumulated with fp32 atomics) and
-# the config's chaotic first ~30 steps amplify that, so where the transient ends differs run to run.  Measured on B200
-# over five runs of the uniform stream: head 4e-4 / 1.4e-2 (steps 1 / 2); steps 30-39 up to 0.065 (the transient dying,
-# not asserted), steps 40-99 0.0063 ... 0.012; steps >= 100 single-step 0.0038 ... 0.0073, 25-step running mean
-# 0.0018 ... 0.0053; lr-1e-3 control (no transient): 1.1e-3 over the whole curve, single steps.
+# the config's chaotic first ~30 steps amplify that, so where the transient ends differs run to run.  One run on an
+# H100 80GB HBM3 (700 W): uniform stream head 9.5e-3 (steps 0-2), steps 30-99 up to 0.023, steps >= 100 single-step
+# 0.0048; lr-1e-3 control (no transient): 5.9e-4 over the whole curve, single steps.
 C1_TOL = {"head": 3e-2, "settling": 0.15, "settled": 2e-2, "tail": 1e-2, "control": 1e-2}
