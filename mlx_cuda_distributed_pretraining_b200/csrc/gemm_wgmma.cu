@@ -1,16 +1,22 @@
 // Batched bf16 GEMM engine on Hopper warpgroup MMA (wgmma) fed by TMA through an mbarrier ring.
 //
-// One CTA computes one 128 x 128 output tile (or one K-split of it):
-//   warpgroup 0   producer: one thread streams A[128 x 64] + B[128 x 64] k-blocks (128B-swizzled TMA boxes)
-//                 into a 6-stage ring (32 KB per stage, 192 KB of the 227 KB a block may use)
-//   warpgroups 1-2  consumers: rows [0, 64) and [64, 128) of the tile, wgmma.m64n128k16 with fp32
-//                 accumulators in registers (64 per thread); a stage is handed back once the wgmma batch
-//                 that read it has retired, so one batch is always in flight behind the next TMA wait
-//   epilogue      straight from the accumulator registers: alpha/beta/C, bf16 or fp32 stores, the
-//                 symmetric-output mirror, split-K partials, peer stores and the two fused MLP epilogues.
+// Persistent and warp-specialised: the grid is min(work items, SMs) CTAs and CTA c walks work items
+// c, c + gridDim.x, ... of the concatenated list of every problem of the launch (grouped GEMM).
+//   warpgroup 0     producer: one thread streams A[128 x 64] + B[128 x 64] k-blocks (128B-swizzled TMA boxes)
+//                   into a 5-stage ring (32 KB per stage).  Ring slot and phase run on across work items, so the
+//                   next tile's loads start while the current one is still being multiplied.
+//   warpgroups 1-2  consumers, ping-pong: each owns a whole 128 x 128 tile (two wgmma.m64n128k16 per k16 step,
+//                   128 fp32 accumulators per thread) and they take the CTA's work items in turn.  A pair of
+//                   named barriers orders their mainloops, so one warpgroup's epilogue runs while the other
+//                   keeps the tensor cores busy.  A stage is handed back once the wgmma batch that read it has
+//                   retired, so one batch is always in flight behind the next TMA wait.
+//   epilogue        bf16 outputs go through a 32 KB shared-memory tile per consumer (stmatrix in, 16-byte
+//                   coalesced rows out): alpha/beta/C (C read as 16-byte rows), the symmetric-output mirror
+//                   (stmatrix.trans), peer stores and the two fused MLP epilogues.  fp32 outputs and split-K
+//                   partials are stored straight from the accumulators.
 // Operand layouts (K-major or MN-major for A and for B) are per-problem run-time flags: they select the TMA
-// box shape and the transpose bits of the wgmma instruction.  Problems of one launch are concatenated work
-// lists (grouped GEMM), which is how the Newton-Schulz chain runs each stage over all shape groups at once.
+// box shape and the transpose bits of the wgmma instruction.  Grouped launches are how the Newton-Schulz chain
+// runs each stage over all shape groups at once.
 #include "common.cuh"
 #include "host.h"
 
@@ -19,15 +25,19 @@ namespace b200 {
 namespace {
 
 constexpr int BM = 128, BN = 128, BK = 64;
-constexpr int STAGES = 6;
+constexpr int STAGES = 5;
 constexpr int THREADS = 384;
 constexpr int A_BYTES = BM * BK * 2;  // 16 KB
 constexpr int B_BYTES = BN * BK * 2;  // 16 KB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
+constexpr int OUT_BYTES = BM * BN * 2;  // bf16 staging tile of one consumer warpgroup
+constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * OUT_BYTES + 1024 + 256;
+static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget of one block");
 constexpr int MAX_PROBLEMS = 6;
 constexpr int MAX_PEERS = 7;
 constexpr int GROUP_M = 8;  // tile raster: 8 row blocks sweep the columns together (L2 reuse of B)
+// named barriers: 1 + c = "consumer c may start its mainloop", 3 + c = consumer c's own warpgroup barrier
+constexpr uint32_t BAR_ORDER = 1, BAR_WG = 3;
 
 struct Problem {
   int M, N, K, batch;
@@ -51,7 +61,7 @@ struct Problem {
 };
 
 struct Args {
-  int n_problems;
+  int n_problems, total_work;
   Problem p[MAX_PROBLEMS];
   CUtensorMap tmA[MAX_PROBLEMS];
   CUtensorMap tmB[MAX_PROBLEMS];
@@ -78,6 +88,45 @@ __device__ __forceinline__ void tile_coords(const Problem& p, int r, int& mi, in
   ni = rr / gsize;
 }
 
+struct Item {
+  int pi, split, b, mi, ni, kb_begin, kb_end;
+};
+
+__device__ __forceinline__ int problem_of(const Args& g, int w) {
+  int pi = 0;
+#pragma unroll
+  for (int i = 1; i < MAX_PROBLEMS; ++i)
+    if (i < g.n_problems && w >= g.p[i].work_begin) pi = i;
+  return pi;
+}
+
+// k-block range of work item w (split s of its tile covers [s * kb_per, min(num_kb, (s + 1) * kb_per)))
+__device__ __forceinline__ void kb_range(const Problem& p, int split, int& kb_begin, int& kb_end) {
+  const int kb_per = (p.num_kb + p.k_splits - 1) / p.k_splits;
+  kb_begin = split * kb_per;
+  kb_end = min(p.num_kb, kb_begin + kb_per);
+}
+
+__device__ __forceinline__ Item decode(const Args& g, int w) {
+  Item it;
+  it.pi = problem_of(g, w);
+  const Problem& p = g.p[it.pi];
+  int r = w - p.work_begin;
+  it.split = r % p.k_splits;
+  r /= p.k_splits;
+  it.b = r / p.tiles_per_batch;
+  tile_coords(p, r - it.b * p.tiles_per_batch, it.mi, it.ni);
+  kb_range(p, it.split, it.kb_begin, it.kb_end);
+  return it;
+}
+
+__device__ __forceinline__ int item_kbs(const Args& g, int w) {
+  const Problem& p = g.p[problem_of(g, w)];
+  int kb_begin, kb_end;
+  kb_range(p, (w - p.work_begin) % p.k_splits, kb_begin, kb_end);
+  return max(kb_end - kb_begin, 0);
+}
+
 // sigmoid with one special-function op: sigmoid(x) = 0.5 + 0.5 tanh(x / 2)
 __device__ __forceinline__ float fast_sigmoid(float x) {
   float t;
@@ -85,216 +134,362 @@ __device__ __forceinline__ float fast_sigmoid(float x) {
   return fmaf(0.5f, t, 0.5f);
 }
 
+// One tile's k-blocks [kb_begin, kb_end) from the ring: acc[0, 64) = rows [0, 64), acc[64, 128) = rows [64, 128).
 template <int TA, int TB>
-__device__ __forceinline__ void mma_kblock(float* acc, uint32_t a_base, uint32_t b_base) {
-  // per k16 step: K-major operands advance 32 B inside the swizzled row, MN-major ones 16 rows of 128 B
+__device__ __forceinline__ void mainloop(float* acc, uint32_t sbase, uint32_t full0, uint32_t empty0, int n_kb,
+                                         int& slot, uint32_t& phase, bool leader) {
+  int prev = -1;
+  for (int i = 0; i < n_kb; ++i) {
+    mbar_wait(full0 + 8 * slot, phase);
+    const uint32_t sA = sbase + slot * STAGE_BYTES, sB = sA + A_BYTES;
+    wgmma_fence();
+    // per k16 step: K-major operands advance 32 B inside the swizzled row, MN-major ones 16 rows of 128 B
 #pragma unroll
-  for (int k = 0; k < BK / 16; ++k) {
-    const uint64_t da = make_wgmma_desc_sw128(a_base + k * (TA ? 2048 : 32), 8192, 1024);
-    const uint64_t db = make_wgmma_desc_sw128(b_base + k * (TB ? 2048 : 32), 8192, 1024);
-    wgmma_m64n128k16_ss<TA, TB>(acc, da, db);
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t db = make_wgmma_desc_sw128(sB + k * (TB ? 2048 : 32), 8192, 1024);
+      const uint64_t da0 = make_wgmma_desc_sw128(sA + k * (TA ? 2048 : 32), 8192, 1024);
+      const uint64_t da1 = make_wgmma_desc_sw128(sA + 8192 + k * (TA ? 2048 : 32), 8192, 1024);
+      wgmma_m64n128k16_ss<TA, TB>(acc, da0, db);
+      wgmma_m64n128k16_ss<TA, TB>(acc + 64, da1, db);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && leader) mbar_arrive(empty0 + 8 * prev);
+    prev = slot;
+    if (++slot == STAGES) {
+      slot = 0;
+      phase ^= 1u;
+    }
   }
+  wgmma_wait<0>();
+  if (prev >= 0 && leader) mbar_arrive(empty0 + 8 * prev);
 }
 
-__device__ __forceinline__ void store_pair(void* D, bool f32, long long off, float v0, float v1) {
-  if (f32)
-    *reinterpret_cast<float2*>(reinterpret_cast<float*>(D) + off) = make_float2(v0, v1);
-  else
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(D) + off) = pack_bf16x2(v0, v1);
+// Staging tile: 128 rows of 256 B (16 chunks of 8 bf16); chunk k of row r sits at chunk k ^ (r & 7), so the
+// eight rows of an 8x8 stmatrix / ldmatrix and the eight chunks of a 128-byte row hit distinct banks.
+__device__ __forceinline__ uint32_t stage_off(int row, int chunk) { return row * 256 + ((chunk ^ (row & 7)) << 4); }
+
+// Row addresses of the x4 matrix group (h = 0/1 row halves of 8, column groups j0, j0 + 1) of warp `warp`
+// at tile row offset `row0`; lane 8i + rr addresses row rr of matrix i.
+__device__ __forceinline__ uint32_t frag_addr(uint32_t stg, int row0, int warp, int j0, int lane) {
+  const int mi = lane >> 3, rr = lane & 7;
+  return stg + stage_off(row0 + 16 * warp + 8 * (mi & 1) + rr, j0 + (mi >> 1));
+}
+// The same matrices stored transposed: fragment column 8j + c becomes staging row 8j + c.
+__device__ __forceinline__ uint32_t frag_addr_trans(uint32_t stg, int row0, int warp, int j0, int lane) {
+  const int mi = lane >> 3, rr = lane & 7;
+  return stg + stage_off(8 * (j0 + (mi >> 1)) + rr, (row0 >> 3) + 2 * warp + (mi & 1));
 }
 
 __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ Args g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t full0 = sbase + STAGES * STAGE_BYTES;
+  const uint32_t full0 = sbase + STAGES * STAGE_BYTES + 2 * OUT_BYTES;
   const uint32_t empty0 = full0 + STAGES * 8;
-
-  int pi = 0;
-#pragma unroll
-  for (int i = 1; i < MAX_PROBLEMS; ++i)
-    if (i < g.n_problems && (int)blockIdx.x >= g.p[i].work_begin) pi = i;
-  const Problem& p = g.p[pi];
-  int r = blockIdx.x - p.work_begin;
-  const int split = r % p.k_splits;
-  r /= p.k_splits;
-  const int b = r / p.tiles_per_batch;
-  int mi, ni;
-  tile_coords(p, r - b * p.tiles_per_batch, mi, ni);
-  const int kb_per = (p.num_kb + p.k_splits - 1) / p.k_splits;
-  const int kb_begin = split * kb_per;
-  const int kb_end = min(p.num_kb, kb_begin + kb_per);
   const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 2);  // one arrival per consumer warpgroup
+      mbar_init(empty0 + 8 * s, 1);  // one arrival by the consumer warpgroup that read the stage
     }
     fence_mbar_init();
   }
   __syncthreads();
 
   if (wg == 0) {
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
-      const CUtensorMap* tmA = &g.tmA[pi];
-      const CUtensorMap* tmB = &g.tmB[pi];
-      tma_prefetch_desc(tmA);
-      tma_prefetch_desc(tmB);
-      for (int kb = kb_begin, i = 0; kb < kb_end; ++kb, ++i) {
-        const int s = i % STAGES;
-        const uint32_t ph = (i / STAGES) & 1;
-        mbar_wait(empty0 + 8 * s, ph ^ 1u);
-        const uint32_t full = full0 + 8 * s;
-        mbar_arrive_expect_tx(full, STAGE_BYTES);
-        const uint32_t sA = sbase + s * STAGE_BYTES, sB = sA + A_BYTES;
-        const int k0 = kb * BK;
-        if (p.a_mn) {  // two [64 k-rows x 64 m] boxes
-          tma_load_3d(sA, tmA, full, mi * BM, k0, b);
-          tma_load_3d(sA + 8192, tmA, full, mi * BM + 64, k0, b);
-        } else {
-          tma_load_3d(sA, tmA, full, k0, mi * BM, b);
-        }
-        if (p.epi == 1) {  // 64 gate rows of W2, then the same 64 up rows
-          tma_load_3d(sB, tmB, full, k0, ni * 64, b);
-          tma_load_3d(sB + 8192, tmB, full, k0, p.glu_I + ni * 64, b);
-        } else if (p.b_mn) {
-          tma_load_3d(sB, tmB, full, ni * BN, k0, b);
-          tma_load_3d(sB + 8192, tmB, full, ni * BN + 64, k0, b);
-        } else {
-          tma_load_3d(sB, tmB, full, k0, ni * BN, b);
+      for (int i = 0; i < g.n_problems; ++i) {
+        tma_prefetch_desc(&g.tmA[i]);
+        tma_prefetch_desc(&g.tmB[i]);
+      }
+      int slot = 0;
+      uint32_t phase = 0;
+      for (int w = blockIdx.x; w < g.total_work; w += gridDim.x) {
+        const Item it = decode(g, w);
+        const Problem& p = g.p[it.pi];
+        const CUtensorMap* tmA = &g.tmA[it.pi];
+        const CUtensorMap* tmB = &g.tmB[it.pi];
+        const int mi = it.mi, ni = it.ni, b = it.b;
+        for (int kb = it.kb_begin; kb < it.kb_end; ++kb) {
+          mbar_wait(empty0 + 8 * slot, phase ^ 1u);
+          const uint32_t full = full0 + 8 * slot;
+          mbar_arrive_expect_tx(full, STAGE_BYTES);
+          const uint32_t sA = sbase + slot * STAGE_BYTES, sB = sA + A_BYTES;
+          const int k0 = kb * BK;
+          if (p.a_mn) {  // two [64 k-rows x 64 m] boxes
+            tma_load_3d(sA, tmA, full, mi * BM, k0, b);
+            tma_load_3d(sA + 8192, tmA, full, mi * BM + 64, k0, b);
+          } else {
+            tma_load_3d(sA, tmA, full, k0, mi * BM, b);
+          }
+          if (p.epi == 1) {  // 64 gate rows of W2, then the same 64 up rows
+            tma_load_3d(sB, tmB, full, k0, ni * 64, b);
+            tma_load_3d(sB + 8192, tmB, full, k0, p.glu_I + ni * 64, b);
+          } else if (p.b_mn) {
+            tma_load_3d(sB, tmB, full, ni * BN, k0, b);
+            tma_load_3d(sB + 8192, tmB, full, ni * BN + 64, k0, b);
+          } else {
+            tma_load_3d(sB, tmB, full, k0, ni * BN, b);
+          }
+          if (++slot == STAGES) {
+            slot = 0;
+            phase ^= 1u;
+          }
         }
       }
     }
     return;
   }
 
-  const int c = wg - 1;  // rows [64c, 64c + 64) of the tile
-  float acc[64];
+  setmaxnreg_inc<232>();
+  const int c = wg - 1;
+  const int tid = threadIdx.x & 127, lane = threadIdx.x & 31, warp = tid >> 5;
+  const uint32_t stg = sbase + STAGES * STAGE_BYTES + c * OUT_BYTES;
+  const uint32_t bar_wg = BAR_WG + c;
+  int slot = 0;
+  uint32_t phase = 0;
+  for (int w = blockIdx.x, t = 0; w < g.total_work; w += gridDim.x, ++t) {
+    if ((t & 1) != c) {  // the other warpgroup's tile: step the ring past its k-blocks
+      const int n = slot + item_kbs(g, w);
+      phase ^= (uint32_t)(n / STAGES) & 1u;
+      slot = n % STAGES;
+      continue;
+    }
+    const Item it = decode(g, w);
+    const Problem& p = g.p[it.pi];
+    const int mi = it.mi, ni = it.ni, b = it.b;
+
+    float acc[128];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-  int prev = -1;
-  for (int kb = kb_begin, i = 0; kb < kb_end; ++kb, ++i) {
-    const int s = i % STAGES;
-    mbar_wait(full0 + 8 * s, (i / STAGES) & 1);
-    const uint32_t sA = sbase + s * STAGE_BYTES + c * 8192, sB = sbase + s * STAGE_BYTES + A_BYTES;
-    wgmma_fence();
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    if (t > 0) named_bar_sync(BAR_ORDER + c, 256);  // the other warpgroup's mainloop is done
+    const int n_kb = max(it.kb_end - it.kb_begin, 0);
+    const bool leader = tid == 0;
     if (p.a_mn) {
-      if (p.b_mn) mma_kblock<1, 1>(acc, sA, sB);
-      else mma_kblock<1, 0>(acc, sA, sB);
+      if (p.b_mn) mainloop<1, 1>(acc, sbase, full0, empty0, n_kb, slot, phase, leader);
+      else mainloop<1, 0>(acc, sbase, full0, empty0, n_kb, slot, phase, leader);
     } else {
-      if (p.b_mn) mma_kblock<0, 1>(acc, sA, sB);
-      else mma_kblock<0, 0>(acc, sA, sB);
+      if (p.b_mn) mainloop<0, 1>(acc, sbase, full0, empty0, n_kb, slot, phase, leader);
+      else mainloop<0, 0>(acc, sbase, full0, empty0, n_kb, slot, phase, leader);
     }
-    wgmma_commit();
-    wgmma_wait<1>();
-    if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty0 + 8 * prev);
-    prev = s;
-  }
-  wgmma_wait<0>();
+    if (w + (int)gridDim.x < g.total_work) named_bar_arrive(BAR_ORDER + (c ^ 1), 256);
 
-  // ---- epilogue: thread owns rows (r0, r0 + 8) x columns (8j + 2q, +1), j = 0..15 ----
-  const int lane = threadIdx.x & 31, warp = (threadIdx.x >> 5) & 3;
-  const int r0 = mi * BM + c * 64 + warp * 16 + (lane >> 2);
-  const int cq = (lane & 3) * 2;
+    // accumulator fragment: acc[64 hm + 4 j + 2 h + e] = tile (64 hm + 16 warp + 8 h + lane / 4, 8 j + cq + e)
+    const int cq = (lane & 3) * 2;
+    const int rq = 16 * warp + (lane >> 2);
 
-  if (p.k_splits > 1) {  // raw fp32 partial of this K range
-    float* ws = p.ws + ((long long)split * p.batch + b) * p.M * (long long)p.N;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int col = ni * BN + 8 * j + cq;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
-        if (row < p.M && col < p.N)
-          *reinterpret_cast<float2*>(ws + (long long)row * p.N + col) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+    if (p.k_splits > 1 || p.out_f32) {  // fp32 results straight from the accumulators
+      const float alpha = p.k_splits > 1 ? 1.0f : p.alpha * (p.alpha_vec ? p.alpha_vec[b] : 1.0f);
+      const float beta = p.beta * (p.beta_vec ? p.beta_vec[b] : 1.0f);
+      float* Db;
+      long long ld;
+      const float* Cb = nullptr;
+      int n_cols;
+      if (p.k_splits > 1) {  // raw partial of this K range
+        Db = p.ws + ((long long)it.split * p.batch + b) * p.M * (long long)p.N;
+        ld = p.N;
+        n_cols = p.N;
+      } else {
+        Db = reinterpret_cast<float*>(p.D) + (long long)b * p.strideD;
+        ld = p.ldd;
+        n_cols = p.n_store;
+        if (p.C) Cb = reinterpret_cast<const float*>(p.C) + (long long)b * p.strideC;
       }
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int col = ni * BN + 8 * j + cq;
+          if (col >= n_cols) continue;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = mi * BM + 64 * hm + rq + 8 * h;
+            if (row >= p.M) continue;
+            float v0 = acc[64 * hm + 4 * j + 2 * h], v1 = acc[64 * hm + 4 * j + 2 * h + 1];
+            if (p.k_splits <= 1) {
+              v0 = alpha * v0;
+              v1 = alpha * v1;
+              if (Cb) {
+                const float2 cv = *reinterpret_cast<const float2*>(Cb + (long long)row * p.ldc + col);
+                v0 += beta * cv.x;
+                v1 += beta * cv.y;
+              }
+            }
+            *reinterpret_cast<float2*>(Db + (long long)row * ld + col) = make_float2(v0, v1);
+          }
+        }
+      continue;
     }
-    return;
-  }
 
-  if (p.epi == 1) {  // acc columns [0, 64) = gate, [64, 128) = up of the same 64 output columns
-    __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.D);
-    __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(p.aux);
+    named_bar_sync(bar_wg, 128);  // this warpgroup's previous tile has left the staging buffer
+
+    if (p.epi == 1) {  // acc columns [0, 64) = gate, [64, 128) = up of the same 64 output columns
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int col = ni * 64 + 8 * j + cq;
+      for (int hm = 0; hm < 2; ++hm)
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
-        if (row >= p.M) continue;
-        const float g0 = acc[4 * j + 2 * h], g1 = acc[4 * j + 2 * h + 1];
-        const float u0 = acc[4 * (j + 8) + 2 * h], u1 = acc[4 * (j + 8) + 2 * h + 1];
-        const long long o = (long long)row * p.ldd + col;
-        *reinterpret_cast<uint32_t*>(gu + o) = pack_bf16x2(g0, g1);
-        *reinterpret_cast<uint32_t*>(gu + o + p.glu_I) = pack_bf16x2(u0, u1);
-        *reinterpret_cast<uint32_t*>(y + (long long)row * p.ld_aux + col) =
-            pack_bf16x2(g0 * fast_sigmoid(u0) * 2.0f, g1 * fast_sigmoid(u1) * 2.0f);
+        for (int j = 0; j < 16; j += 2) {
+          const float* a = acc + 64 * hm + 4 * j;
+          stmatrix_x4(frag_addr(stg, 64 * hm, warp, j, lane), pack_bf16x2(a[0], a[1]), pack_bf16x2(a[2], a[3]),
+                      pack_bf16x2(a[4], a[5]), pack_bf16x2(a[6], a[7]));
+        }
+      named_bar_sync(bar_wg, 128);
+      __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.D);
+#pragma unroll 4
+      for (int i = 0; i < 16; ++i) {  // chunk k < 8: gate columns, k >= 8: the up columns I later
+        const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
+        const int row = mi * BM + r;
+        if (row < p.M)
+          stg128(gu + (long long)row * p.ldd + (k >= 8 ? p.glu_I : 0) + ni * 64 + 8 * (k & 7),
+                 lds128(stg + stage_off(r, k)));
       }
-    }
-    return;
-  }
-
-  if (p.epi == 2) {  // acc = d = dy Wd; dg = d s 2, du = d g s (1 - s) 2 with g, u from the saved gu
-    const __nv_bfloat16* gu = reinterpret_cast<const __nv_bfloat16*>(p.aux);
-    __nv_bfloat16* dgu = reinterpret_cast<__nv_bfloat16*>(p.D);
+      named_bar_sync(bar_wg, 128);
 #pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int col = ni * BN + 8 * j + cq;
-      if (col >= p.glu_I) continue;
+      for (int hm = 0; hm < 2; ++hm)
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
-        if (row >= p.M) continue;
-        const long long oa = (long long)row * p.ld_aux + col;
-        const float2 gg = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(gu + oa));
-        const float2 uu = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(gu + oa + p.glu_I));
-        const float d0 = acc[4 * j + 2 * h], d1 = acc[4 * j + 2 * h + 1];
-        const float s0 = fast_sigmoid(uu.x), s1 = fast_sigmoid(uu.y);
-        const long long o = (long long)row * p.ldd + col;
-        *reinterpret_cast<uint32_t*>(dgu + o) = pack_bf16x2(d0 * s0 * 2.0f, d1 * s1 * 2.0f);
-        *reinterpret_cast<uint32_t*>(dgu + o + p.glu_I) =
-            pack_bf16x2(d0 * gg.x * s0 * (1.0f - s0) * 2.0f, d1 * gg.y * s1 * (1.0f - s1) * 2.0f);
+        for (int j = 0; j < 8; j += 2) {  // y = g sigmoid(u) 2 from the fp32 accumulators
+          const float* g = acc + 64 * hm + 4 * j;
+          const float* u = g + 32;
+          uint32_t yv[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q)
+            yv[q] = pack_bf16x2(g[2 * q] * fast_sigmoid(u[2 * q]) * 2.0f, g[2 * q + 1] * fast_sigmoid(u[2 * q + 1]) * 2.0f);
+          stmatrix_x4(frag_addr(stg, 64 * hm, warp, j, lane), yv[0], yv[1], yv[2], yv[3]);
+        }
+      named_bar_sync(bar_wg, 128);
+      __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(p.aux);
+#pragma unroll 4
+      for (int i = 0; i < 8; ++i) {
+        const int idx = i * 128 + tid, r = idx >> 3, k = idx & 7;
+        const int row = mi * BM + r;
+        if (row < p.M) stg128(y + (long long)row * p.ld_aux + ni * 64 + 8 * k, lds128(stg + stage_off(r, k)));
       }
+      continue;
     }
-    return;
-  }
 
-  const float alpha = p.alpha * (p.alpha_vec ? p.alpha_vec[b] : 1.0f);
-  const float beta = p.beta * (p.beta_vec ? p.beta_vec[b] : 1.0f);
-  const bool f32 = p.out_f32 != 0;
-  const bool mirror = p.symmetric && mi != ni;
-  char* Db = reinterpret_cast<char*>(p.D) + (long long)b * p.strideD * (f32 ? 4 : 2);
-  const char* Cb = p.C ? reinterpret_cast<const char*>(p.C) + (long long)b * p.strideC * (f32 ? 4 : 2) : nullptr;
+    if (p.epi == 2) {  // acc = d = dy Wd; dg = d s 2, du = d g s (1 - s) 2 with g, u from the saved gu
+      const __nv_bfloat16* gu = reinterpret_cast<const __nv_bfloat16*>(p.aux);
+      __nv_bfloat16* dgu = reinterpret_cast<__nv_bfloat16*>(p.D);
 #pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    const int col = ni * BN + 8 * j + cq;
-    if (col >= p.n_store) continue;
+      for (int hm = 0; hm < 2; ++hm) {  // staging rows [0, 64): g, [64, 128): u of tile rows [64 hm, 64 hm + 64)
+        if (hm) named_bar_sync(bar_wg, 128);
+#pragma unroll 2
+        for (int i = 0; i < 16; ++i) {
+          const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
+          const int row = mi * BM + 64 * hm + (r & 63), col = ni * BN + 8 * k;
+          uint4 v = make_uint4(0, 0, 0, 0);
+          if (row < p.M && col < p.glu_I) v = ldg128(gu + (long long)row * p.ld_aux + (r >= 64 ? p.glu_I : 0) + col);
+          sts128(stg + stage_off(r, k), v);
+        }
+        named_bar_sync(bar_wg, 128);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r0 + 8 * h;
-      if (row >= p.M) continue;
-      float v0 = alpha * acc[4 * j + 2 * h], v1 = alpha * acc[4 * j + 2 * h + 1];
-      if (Cb) {
-        const long long oc = (long long)row * p.ldc + col;
-        if (f32) {
-          const float2 cv = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(Cb) + oc);
-          v0 += beta * cv.x;
-          v1 += beta * cv.y;
-        } else {
-          const float2 cv = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(Cb) + oc));
-          v0 += beta * cv.x;
-          v1 += beta * cv.y;
+        for (int j = 0; j < 16; j += 2) {  // each warp reads and rewrites only its own 16 rows: in place
+          const uint32_t ga = frag_addr(stg, 0, warp, j, lane), ua = frag_addr(stg, 64, warp, j, lane);
+          uint32_t gq[4], uq[4], dg[4], du[4];
+          ldmatrix_x4(ga, gq);
+          ldmatrix_x4(ua, uq);
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {  // q = (column group j + q / 2, row half q % 2)
+            const float* a = acc + 64 * hm + 4 * (j + (q >> 1)) + 2 * (q & 1);
+            const float2 gg = unpack_bf16x2(gq[q]), uu = unpack_bf16x2(uq[q]);
+            const float d0 = a[0], d1 = a[1];
+            const float s0 = fast_sigmoid(uu.x), s1 = fast_sigmoid(uu.y);
+            dg[q] = pack_bf16x2(d0 * s0 * 2.0f, d1 * s1 * 2.0f);
+            du[q] = pack_bf16x2(d0 * gg.x * s0 * (1.0f - s0) * 2.0f, d1 * gg.y * s1 * (1.0f - s1) * 2.0f);
+          }
+          __syncwarp();
+          stmatrix_x4(ga, dg[0], dg[1], dg[2], dg[3]);
+          stmatrix_x4(ua, du[0], du[1], du[2], du[3]);
+        }
+        named_bar_sync(bar_wg, 128);
+#pragma unroll 1
+        for (int i = 0; i < 16; ++i) {
+          const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
+          const int row = mi * BM + 64 * hm + (r & 63), col = ni * BN + 8 * k;
+          if (row < p.M && col < p.glu_I)
+            stg128(dgu + (long long)row * p.ldd + (r >= 64 ? p.glu_I : 0) + col, lds128(stg + stage_off(r, k)));
         }
       }
+      continue;
+    }
+
+    // ---- plain bf16: D = alpha acc + beta C, optional mirror and peer copies ----
+    const float alpha = p.alpha * (p.alpha_vec ? p.alpha_vec[b] : 1.0f);
+    const float beta = p.beta * (p.beta_vec ? p.beta_vec[b] : 1.0f);
+    __nv_bfloat16* Db = reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)b * p.strideD;
+    const __nv_bfloat16* Cb =
+        p.C ? reinterpret_cast<const __nv_bfloat16*>(p.C) + (long long)b * p.strideC : nullptr;
+    if (Cb) {
+#pragma unroll 4
+      for (int i = 0; i < 16; ++i) {
+        const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
+        const int row = mi * BM + r, col = ni * BN + 8 * k;
+        uint4 v = make_uint4(0, 0, 0, 0);
+        if (row < p.M && col < p.n_store) v = ldg128(Cb + (long long)row * p.ldc + col);
+        sts128(stg + stage_off(r, k), v);
+      }
+      named_bar_sync(bar_wg, 128);
+    }
+    uint32_t dv[2][8][4];  // the tile as packed bf16 pairs, kept for the mirror
+#pragma unroll
+    for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+      for (int jp = 0; jp < 8; ++jp) {  // each warp reads and rewrites only its own 16 rows: in place
+        const uint32_t fa = frag_addr(stg, 64 * hm, warp, 2 * jp, lane);
+        uint32_t cq4[4];
+        if (Cb) ldmatrix_x4(fa, cq4);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float* a = acc + 64 * hm + 4 * (2 * jp + (q >> 1)) + 2 * (q & 1);
+          float v0 = alpha * a[0], v1 = alpha * a[1];
+          if (Cb) {
+            const float2 cv = unpack_bf16x2(cq4[q]);
+            v0 += beta * cv.x;
+            v1 += beta * cv.y;
+          }
+          dv[hm][jp][q] = pack_bf16x2(v0, v1);
+        }
+        __syncwarp();
+        stmatrix_x4(fa, dv[hm][jp][0], dv[hm][jp][1], dv[hm][jp][2], dv[hm][jp][3]);
+      }
+    named_bar_sync(bar_wg, 128);
+#pragma unroll 4
+    for (int i = 0; i < 16; ++i) {
+      const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
+      const int row = mi * BM + r, col = ni * BN + 8 * k;
+      if (row >= p.M || col >= p.n_store) continue;
+      const uint4 v = lds128(stg + stage_off(r, k));
       const long long od = (long long)row * p.ldd + col;
-      store_pair(Db, f32, od, v0, v1);
+      stg128(Db + od, v);
       for (int pe = 0; pe < p.n_peers; ++pe)
-        store_pair(reinterpret_cast<char*>(p.peer_D[pe]) + (long long)b * p.strideD * (f32 ? 4 : 2), f32, od, v0, v1);
-      if (mirror) {  // D == D^T: the tile below the diagonal is this one transposed (bf16 only)
-        __nv_bfloat16* Dm = reinterpret_cast<__nv_bfloat16*>(Db);
-        Dm[(long long)col * p.ldd + row] = __float2bfloat16_rn(v0);
-        if (col + 1 < p.N) Dm[(long long)(col + 1) * p.ldd + row] = __float2bfloat16_rn(v1);
+        stg128(reinterpret_cast<__nv_bfloat16*>(p.peer_D[pe]) + (long long)b * p.strideD + od, v);
+    }
+    if (p.symmetric && mi != ni) {  // D == D^T: block (ni, mi) is this tile transposed
+      named_bar_sync(bar_wg, 128);
+#pragma unroll
+      for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+        for (int jp = 0; jp < 8; ++jp)
+          stmatrix_x4_trans(frag_addr_trans(stg, 64 * hm, warp, 2 * jp, lane), dv[hm][jp][0], dv[hm][jp][1],
+                            dv[hm][jp][2], dv[hm][jp][3]);
+      named_bar_sync(bar_wg, 128);
+#pragma unroll 4
+      for (int i = 0; i < 16; ++i) {
+        const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
+        const int row = ni * BN + r, col = mi * BM + 8 * k;  // row: a column of D, col: rows of D
+        if (row >= p.N || col >= p.M) continue;
+        const uint4 v = lds128(stg + stage_off(r, k));
+        __nv_bfloat16* dst = Db + (long long)row * p.ldd + col;
+        if (col + 8 <= p.M) {
+          stg128(dst, v);
+        } else {  // ragged last rows of D (M % 8 != 0)
+          for (int e = 0; e < p.M - col; ++e) {
+            const uint32_t wv = e < 2 ? v.x : e < 4 ? v.y : e < 6 ? v.z : v.w;
+            reinterpret_cast<uint16_t*>(dst)[e] = (uint16_t)(wv >> (16 * (e & 1)));
+          }
+        }
       }
     }
   }
@@ -372,12 +567,13 @@ int launch(Args& a, int n, cudaStream_t stream) {
     work += a.p[i].tiles_per_batch * a.p[i].batch * a.p[i].k_splits;
   }
   a.n_problems = n;
+  a.total_work = work;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     attr_set = true;
   }
-  gemm_wgmma_kernel<<<work, THREADS, SMEM_BYTES, stream>>>(a);
+  gemm_wgmma_kernel<<<work < num_sms() ? work : num_sms(), THREADS, SMEM_BYTES, stream>>>(a);
   B200_CHECK_LAUNCH();
   for (int i = 0; i < n; ++i) {
     const Problem& q = a.p[i];
