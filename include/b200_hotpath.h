@@ -55,6 +55,36 @@ int b200_gemm_bf16(int a_mn, int b_mn, int M, int N, int K, int batch,
                    int out_f32, float alpha, float beta,
                    const float* alpha_vec, const float* beta_vec, int force_bn, void* stream);
 
+/* Grouped launch of the same engine: up to 6 independent batched problems in one persistent grid, work items
+ * ordered heaviest K range first.  bf16 C/D; per problem, besides the b200_gemm_bf16 arguments:
+ *   symmetric=1: D == D^T asserted (M == N): tiles on/above the diagonal computed, the rest mirror-written;
+ *   k_splits>1:  K cut into k_splits ranges, fp32 partials in splitk_ws ([k_splits][batch][M][N], required) and a
+ *                deterministic finalize; ignored (one split) when beta != 0;
+ *   peer_D:      HOST array of n_peers <= 7 extra copies of D (same ldd/strideD) written by the same epilogue;
+ *                not combinable with symmetric or split-K.
+ * N % 8 == 0, ldd >= N, leading dimensions and batch strides multiples of 8, C/D/peer pointers 16-byte aligned. */
+typedef struct b200_gemm_problem {
+  int a_mn, b_mn;
+  int M, N, K, batch;
+  const void* A;
+  long long lda, strideA;
+  const void* B;
+  long long ldb, strideB;
+  const void* C;
+  long long ldc, strideC;
+  void* D;
+  long long ldd, strideD;
+  float alpha, beta;
+  const float* alpha_vec;       /* [batch] or NULL */
+  const float* beta_vec;        /* [batch] or NULL */
+  int symmetric;
+  int k_splits;
+  float* splitk_ws;
+  const void* const* peer_D;
+  int n_peers;
+} b200_gemm_problem;
+int b200_gemm_grouped(const b200_gemm_problem* problems, int n, void* stream);
+
 /* ---- Muon (optimizers/muon.py) ---------------------------------------------------------------
  * b200_newton_schulz: Muon.zeropower_via_newtonschulz5 (muon.py:54-83) on a batch of same-shape
  * matrices.  x_in: bf16 [batch,rows,cols], *un-normalised*; inv_norm[b] = 1/(||x_b||_F+eps) and

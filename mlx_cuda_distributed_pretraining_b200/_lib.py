@@ -77,6 +77,15 @@ class NsGroup(C.Structure):
                 ("inv_norm_sq", _vp), ("peer_out", C.POINTER(_vp)), ("n_peers", _i)]
 
 
+class GemmProblem(C.Structure):
+    """b200_gemm_problem (include/b200_hotpath.h)"""
+    _fields_ = [("a_mn", _i), ("b_mn", _i), ("M", _i), ("N", _i), ("K", _i), ("batch", _i),
+                ("A", _vp), ("lda", _ll), ("strideA", _ll), ("B", _vp), ("ldb", _ll), ("strideB", _ll),
+                ("C", _vp), ("ldc", _ll), ("strideC", _ll), ("D", _vp), ("ldd", _ll), ("strideD", _ll),
+                ("alpha", _f), ("beta", _f), ("alpha_vec", _vp), ("beta_vec", _vp), ("symmetric", _i),
+                ("k_splits", _i), ("splitk_ws", _vp), ("peer_D", C.POINTER(_vp)), ("n_peers", _i)]
+
+
 class DwJob(C.Structure):
     """b200_dw_job (include/b200_hotpath.h)"""
     _fields_ = [("partials", _vp), ("dw", _vp), ("n_partials", _i), ("dw_is_bf16", _i), ("accumulate", _i),
@@ -84,6 +93,7 @@ class DwJob(C.Structure):
 
 
 SIGNATURES["b200_rmsnorm_dw_reduce"] = (_i, [C.POINTER(DwJob), _i, _i, _vp])
+SIGNATURES["b200_gemm_grouped"] = (_i, [C.POINTER(GemmProblem), _i, _vp])
 SIGNATURES["b200_newton_schulz_multi_workspace_bytes"] = (_sz, [C.POINTER(NsGroup), _i, _i])
 SIGNATURES["b200_newton_schulz_multi"] = (_i, [C.POINTER(NsGroup), _i, _i, _f, _f, _f, _vp, _sz, _vp])
 

@@ -102,7 +102,7 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
 
 extern "C" {
 
-int b200_version(void) { return 2; }
+int b200_version(void) { return 3; }
 const char* b200_last_error(void) { return b200::last_error(); }
 
 unsigned long long b200_launch_count(void) { return b200::launch_count(); }
@@ -127,6 +127,36 @@ int b200_gemm_bf16(int a_mn, int b_mn, int M, int N, int K, int batch, const voi
   return b200::gemm_bf16(a_mn != 0, b_mn != 0, M, N, K, batch, A, lda, strideA, B, ldb, strideB, C,
                          ldc, strideC, D, ldd, strideD, out_f32 != 0, alpha, beta, alpha_vec,
                          beta_vec, force_bn, S_(stream));
+}
+
+static_assert(sizeof(b200_gemm_problem) == sizeof(b200::GroupedGemm) &&
+                  offsetof(b200_gemm_problem, A) == offsetof(b200::GroupedGemm, A) &&
+                  offsetof(b200_gemm_problem, alpha) == offsetof(b200::GroupedGemm, alpha) &&
+                  offsetof(b200_gemm_problem, symmetric) == offsetof(b200::GroupedGemm, symmetric) &&
+                  offsetof(b200_gemm_problem, n_peers) == offsetof(b200::GroupedGemm, n_peers),
+              "b200_gemm_problem layout");
+// The internal gemm_grouped trusts its callers (the Newton-Schulz drivers); from outside, check what its
+// epilogues assume: 16-byte rows and pointers, room for N columns in D, a split-K workspace when one is asked for.
+int b200_gemm_grouped(const b200_gemm_problem* problems, int n, void* stream) {
+  B200_CHECK_ARG(problems != nullptr && n >= 1, "gemm_grouped: no problems (n=%d)", n);
+  auto misaligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) != 0; };
+  for (int i = 0; i < n; ++i) {
+    const b200_gemm_problem& h = problems[i];
+    B200_CHECK_ARG(h.D != nullptr && h.A != nullptr && h.B != nullptr, "gemm_grouped: problem %d: null operand", i);
+    B200_CHECK_ARG(!misaligned(h.D) && !misaligned(h.C), "gemm_grouped: problem %d: C/D must be 16-byte aligned", i);
+    B200_CHECK_ARG(h.ldd >= h.N && (h.C == nullptr || h.beta == 0.0f || h.ldc >= h.N),
+                   "gemm_grouped: problem %d: ldd=%lld / ldc=%lld shorter than N=%d", i, h.ldd, h.ldc, h.N);
+    B200_CHECK_ARG(h.strideA % 8 == 0 && h.strideB % 8 == 0 && h.strideC % 8 == 0 && h.strideD % 8 == 0,
+                   "gemm_grouped: problem %d: batch strides must keep 16-byte alignment", i);
+    B200_CHECK_ARG(h.k_splits <= 1 || h.splitk_ws != nullptr, "gemm_grouped: problem %d: k_splits=%d needs splitk_ws",
+                   i, h.k_splits);
+    B200_CHECK_ARG(h.n_peers >= 0 && h.n_peers <= 7 && (h.n_peers == 0 || h.peer_D != nullptr),
+                   "gemm_grouped: problem %d: bad peer list (n_peers=%d, 0..7)", i, h.n_peers);
+    for (int p = 0; p < h.n_peers; ++p)
+      B200_CHECK_ARG(h.peer_D[p] != nullptr && !misaligned(h.peer_D[p]),
+                     "gemm_grouped: problem %d: peer %d must be a 16-byte aligned pointer", i, p);
+  }
+  return b200::gemm_grouped(reinterpret_cast<const b200::GroupedGemm*>(problems), n, S_(stream));
 }
 
 size_t b200_newton_schulz_workspace_bytes(int batch, int rows, int cols, int steps) {

@@ -478,18 +478,11 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
 #pragma unroll 4
       for (int i = 0; i < 16; ++i) {
         const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
-        const int row = ni * BN + r, col = mi * BM + 8 * k;  // row: a column of D, col: rows of D
+        // row: a column of D, col: rows of D.  Both entries reject symmetric output unless M == N is a
+        // multiple of 8, so every 8-row piece of the mirror is whole.
+        const int row = ni * BN + r, col = mi * BM + 8 * k;
         if (row >= p.N || col >= p.M) continue;
-        const uint4 v = lds128(stg + stage_off(r, k));
-        __nv_bfloat16* dst = Db + (long long)row * p.ldd + col;
-        if (col + 8 <= p.M) {
-          stg128(dst, v);
-        } else {  // ragged last rows of D (M % 8 != 0)
-          for (int e = 0; e < p.M - col; ++e) {
-            const uint32_t wv = e < 2 ? v.x : e < 4 ? v.y : e < 6 ? v.z : v.w;
-            reinterpret_cast<uint16_t*>(dst)[e] = (uint16_t)(wv >> (16 * (e & 1)));
-          }
-        }
+        stg128(Db + (long long)row * p.ldd + col, lds128(stg + stage_off(r, k)));
       }
     }
   }

@@ -63,9 +63,10 @@ int make_tensor_map(CUtensorMap* out, const void* base, CUtensorMapDataType dtyp
 int num_sms();
 
 // One problem of a grouped GEMM launch (gemm_wgmma.cu: gemm_grouped): D = alpha*av[b]*op(A)op(B) +
-// beta*bv[b]*C, bf16 in/out, batched; layouts as in b200_gemm_bf16.
+// beta*bv[b]*C, bf16 in/out, batched; layouts as in b200_gemm_bf16.  Mirrors b200_gemm_problem of the public
+// header field for field.
 struct GroupedGemm {
-  bool a_mn, b_mn;
+  int a_mn, b_mn;
   int M, N, K, batch;
   const void* A;
   long long lda, strideA;
