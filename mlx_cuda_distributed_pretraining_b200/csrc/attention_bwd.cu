@@ -2,17 +2,27 @@
 // the reference obtains from MLX autograd of arch/flash_attention.py:123-151 (core/training.py:1580,1650),
 // including the sum of dK/dV over the query heads that share a kv head (adjoint of mx.repeat, :107-120).
 //
-//   delta = rowsum(dO * O)                                  (pre-pass kernel, also zeroes the dQ accumulator)
-//   per (128-key tile, kv head, batch) CTA, 256 threads: thread 0 loads K / V once by TMA and prefetches the Q / dO tiles
-//   (64 queries) of every query head of the GQA group one item ahead through a 2-stage ring; warpgroups 0-1 own 64 keys
-//   each (a separate producer warp would cap the MMA warpgroups at 168 registers and make them spill):
-//     S^T  = K Q^T , dP^T = V dO^T          wgmma, both operands K-major in shared memory
-//     P^T  = exp2(S^T * scale*log2e - LSE*log2e),  dS^T = P^T * (dP^T - delta)      (registers)
-//     dV  += P^T dO , dK += dS^T Q          wgmma with P^T / dS^T as register A operands, dO / Q MN-major in smem
-//     dS^T -> shared memory (the 128B-swizzled MN-major layout wgmma reads), then dQ_tile = dS K as wgmma with
-//     both operands MN-major, added into the fp32 dq_acc with atomics
+//   delta = rowsum(dO * O), LSE * log2e                     (pre-pass kernel, also zeroes the dQ accumulator)
+//   per CTA: one 128-key tile of one (kv head, batch), or a pair of them (below); 384 threads in 3 roles:
+//     warp 0         producer: K / V once per key tile, then the Q / dO tiles (64 queries) of every query head of the
+//                    GQA group through a ring of STAGES stages, with the tile's 64 LSE and delta values (bulk copies
+//                    on the same mbarrier)
+//     warp 1         dQ writer: adds each item's fp32 dQ tile from shared memory into the fp32 dq_acc with TMA
+//                    reductions (cp.reduce.async.bulk.tensor .add), then releases the buffer
+//     warpgroups 1-2 consumers, 64 keys each:
+//       S^T  = K Q^T , dP^T = V dO^T          wgmma, both operands K-major in shared memory
+//       P^T  = exp2(S^T * scale*log2e - LSE*log2e),  dS^T = P^T * (dP^T - delta)      (registers; the causal / bounds
+//                                             mask only on tiles that cross the diagonal or the sequence end)
+//       dV  += P^T dO , dK += dS^T Q          wgmma with P^T / dS^T as register A operands, dO / Q MN-major in smem
+//       dS^T -> shared memory (the 128B-swizzled MN-major layout wgmma reads, double-buffered), then
+//       dQ_tile = dS K over all 128 keys, split between the warpgroups by head-dim columns, -> a double-buffered
+//       fp32 shared tile in the 128B-swizzled layout of the dq_acc tensor map
 //   dq_acc (fp32) * scale -> dq (bf16)                       (post-pass kernel)
 // dK and dQ leave the softmax scale out of dS and apply it once at the end.
+//
+// Causal balance: key tile t has work for the queries from t*128 on, so tile 0 has n_kt times the items of the last
+// one.  With an even tile count a CTA runs tile t and then tile n_kt-1-t (equal work in every CTA); the n_kt/2 CTAs of
+// one (kv head, batch) are adjacent in launch order and share its Q / dO rows in L2.
 #include "common.cuh"
 #include "host.h"
 
@@ -22,36 +32,60 @@ int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, in
 
 namespace {
 
-constexpr int BWD_THREADS = 256;  // two MMA warpgroups; thread 0 also issues the TMA loads
-constexpr int BKV = 128;          // keys per CTA (64 per warpgroup)
-constexpr int BQ = 64;            // queries per inner tile
+constexpr int BWD_THREADS = 384;  // producer / dQ-writer warpgroup + two MMA warpgroups
+constexpr int BKV = 128;          // keys per tile (64 per consumer warpgroup)
+constexpr int BQ = 64;            // queries per item
 constexpr float kLog2e = 1.4426950408889634f;
 
 template <int D>
 struct BwdCfg {
-  static constexpr int NB = D / 64;                // 64-column (128-byte) blocks per row
-  static constexpr int KV_BYTES = BKV * D * 2;     // K or V
-  static constexpr int QS_BYTES = BQ * D * 2;      // one Q or dO stage
+  static constexpr int NB = D / 64;                 // 64-column (128-byte) blocks per bf16 row
+  static constexpr int STAGES = D == 64 ? 3 : 2;    // Q / dO ring depth (D = 128: two fill the shared memory)
+  static constexpr int KV_BYTES = BKV * D * 2;      // K or V
+  static constexpr int QS_BYTES = BQ * D * 2;       // one Q or dO stage
+  static constexpr int DS_BYTES = BKV * BQ * 2;     // dS^T [128 keys][64 queries] bf16
+  static constexpr int DQ_BYTES = BQ * D * 4;       // fp32 dQ tile: D/32 blocks of [64 rows][32 floats], swizzled
+  static constexpr int L_BYTES = 2 * BQ * 4;        // LSE*log2e, delta of one item
   static constexpr int OFF_K = 0;
   static constexpr int OFF_V = OFF_K + KV_BYTES;
-  static constexpr int OFF_Q = OFF_V + KV_BYTES;        // 2 stages
-  static constexpr int OFF_DO = OFF_Q + 2 * QS_BYTES;   // 2 stages
-  static constexpr int OFF_DS = OFF_DO + 2 * QS_BYTES;  // dS^T [128 keys][64 queries] bf16
-  static constexpr int OFF_BAR = OFF_DS + BKV * BQ * 2;
-  static constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;
+  static constexpr int OFF_Q = OFF_V + KV_BYTES;
+  static constexpr int OFF_DO = OFF_Q + STAGES * QS_BYTES;
+  static constexpr int OFF_DS = OFF_DO + STAGES * QS_BYTES;  // 2 buffers
+  static constexpr int OFF_DQ = OFF_DS + 2 * DS_BYTES;        // 2 buffers
+  static constexpr int OFF_L = OFF_DQ + 2 * DQ_BYTES;         // STAGES x L_BYTES
+  static constexpr int OFF_BAR = OFF_L + STAGES * L_BYTES;
+  static constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;
+  static_assert(SMEM_BYTES <= 232448, "attn_bwd shared memory");
 };
 
 struct BwdArgs {
-  const float* lse;    // [B,H,S]
-  const float* delta;  // [B,H,S]
-  float* dq_acc;       // [B,S,H,D] fp32
+  const float* lse2;   // [B,H,S_pad] LSE * log2e
+  const float* delta;  // [B,H,S_pad]
   __nv_bfloat16* dk;   // [B,S,dkv_rh,D]-strided rows
   __nv_bfloat16* dv;
   int B, S, H, Hk;
+  int S_pad;           // S rounded up to BQ
   int dkv_rh;          // heads per dk/dv token row (>= Hk)
   float scale;
   int causal;
+  int paired;          // CTA x runs key tiles x and n_kt-1-x
 };
+
+// The work of one key tile: `group * per_head` items, item j = (query head h0 + j / per_head, query tile
+// qt0 + j % per_head).
+struct Tile {
+  int kt, k0, qt0, per_head, n_items;
+};
+__device__ __forceinline__ Tile tile_of(const BwdArgs& p, int pass) {
+  Tile t;
+  t.kt = pass == 0 ? (int)blockIdx.x : (p.S + BKV - 1) / BKV - 1 - (int)blockIdx.x;
+  t.k0 = t.kt * BKV;
+  const int n_qt = (p.S + BQ - 1) / BQ;
+  t.qt0 = p.causal ? t.k0 / BQ : 0;
+  t.per_head = n_qt - t.qt0;
+  t.n_items = (p.H / p.Hk) * t.per_head;
+  return t;
+}
 
 template <int D>
 __device__ __forceinline__ void rs_mma(float* acc, const uint32_t* a, uint64_t db) {
@@ -62,189 +96,272 @@ __device__ __forceinline__ void rs_mma(float* acc, const uint32_t* a, uint64_t d
 template <int D>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO, const BwdArgs p) {
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
+                const __grid_constant__ CUtensorMap tmDQ, const BwdArgs p) {
   using Cfg = BwdCfg<D>;
+  constexpr int ST = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const uint32_t s0 = smem_u32(smem);
+  const uint32_t s0 = (smem_u32(smem_raw) + 1023) & ~1023u;
   const uint32_t sK = s0 + Cfg::OFF_K, sV = s0 + Cfg::OFF_V, sQ = s0 + Cfg::OFF_Q, sDO = s0 + Cfg::OFF_DO;
-  const uint32_t sDS = s0 + Cfg::OFF_DS;
-  const uint32_t kv_full = s0 + Cfg::OFF_BAR, q_full0 = kv_full + 8, q_empty0 = kv_full + 24;
-  const int kt = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
-  const int k0 = kt * BKV;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t sDS = s0 + Cfg::OFF_DS, sDQ = s0 + Cfg::OFF_DQ, sL = s0 + Cfg::OFF_L;
+  const uint32_t kv_full = s0 + Cfg::OFF_BAR, kv_empty = kv_full + 8;
+  const uint32_t q_full0 = kv_full + 16, q_empty0 = q_full0 + 8 * ST;
+  const uint32_t dq_full0 = q_empty0 + 8 * ST, dq_empty0 = dq_full0 + 16;
+  const int hk = blockIdx.y, b = blockIdx.z;
   const int group = p.H / p.Hk;
-  const int n_qt = (p.S + BQ - 1) / BQ;
-  const int qt_first = p.causal ? k0 / BQ : 0;
-  const int per_head = n_qt - qt_first;
-  const int n_items = group * per_head;
+  const int n_pass = p.paired ? 2 : 1;
+  const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     mbar_init(kv_full, 1);
-    for (int s = 0; s < 2; ++s) {
+    mbar_init(kv_empty, 2);  // one arrival per consumer warpgroup
+    for (int s = 0; s < ST; ++s) {
       mbar_init(q_full0 + 8 * s, 1);
-      mbar_init(q_empty0 + 8 * s, 2);  // one arrival per consumer warpgroup
+      mbar_init(q_empty0 + 8 * s, 2);
+    }
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(dq_full0 + 8 * s, 8);  // one arrival per consumer warp
+      mbar_init(dq_empty0 + 8 * s, 1);
     }
     fence_mbar_init();
   }
   __syncthreads();
 
-  // one elected thread: K / V once, then the Q / dO tiles of item `it` into stage it % 2 once both warpgroups
-  // have released that stage (item it - 2)
-  auto issue_item = [&](int it) {
-    const int s = it & 1;
-    const int h = hk * group + it / per_head;
-    const int q0 = (qt_first + it % per_head) * BQ;
-    mbar_wait(q_empty0 + 8 * s, ((it >> 1) & 1) ^ 1u);
-    const uint32_t full = q_full0 + 8 * s;
-    mbar_arrive_expect_tx(full, 2 * Cfg::QS_BYTES);
-    for (int nb = 0; nb < Cfg::NB; ++nb) {
-      tma_load_4d(sQ + s * Cfg::QS_BYTES + nb * BQ * 128, &tmQ, full, nb * 64, h, q0, b);
-      tma_load_4d(sDO + s * Cfg::QS_BYTES + nb * BQ * 128, &tmDO, full, nb * 64, h, q0, b);
+  if (wg == 0) {
+    setmaxnreg_dec<24>();
+    if (warp == 0 && lane == 0) {  // producer
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmDO);
+      int slot = 0;
+      uint32_t phase = 0;
+      for (int pass = 0; pass < n_pass; ++pass) {
+        const Tile t = tile_of(p, pass);
+        if (pass > 0) mbar_wait(kv_empty, 0);
+        mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
+        for (int nb = 0; nb < Cfg::NB; ++nb) {
+          tma_load_4d(sK + nb * BKV * 128, &tmK, kv_full, nb * 64, hk, t.k0, b);
+          tma_load_4d(sV + nb * BKV * 128, &tmV, kv_full, nb * 64, hk, t.k0, b);
+        }
+        for (int j = 0; j < t.n_items; ++j) {
+          const int h = hk * group + j / t.per_head;
+          const int q0 = (t.qt0 + j % t.per_head) * BQ;
+          mbar_wait(q_empty0 + 8 * slot, phase ^ 1u);
+          const uint32_t full = q_full0 + 8 * slot;
+          mbar_arrive_expect_tx(full, 2 * Cfg::QS_BYTES + Cfg::L_BYTES);
+          for (int nb = 0; nb < Cfg::NB; ++nb) {
+            tma_load_4d(sQ + slot * Cfg::QS_BYTES + nb * BQ * 128, &tmQ, full, nb * 64, h, q0, b);
+            tma_load_4d(sDO + slot * Cfg::QS_BYTES + nb * BQ * 128, &tmDO, full, nb * 64, h, q0, b);
+          }
+          const long long lrow = ((long long)b * p.H + h) * p.S_pad + q0;
+          bulk_load(sL + slot * Cfg::L_BYTES, p.lse2 + lrow, BQ * 4, full);
+          bulk_load(sL + slot * Cfg::L_BYTES + BQ * 4, p.delta + lrow, BQ * 4, full);
+          if (++slot == ST) {
+            slot = 0;
+            phase ^= 1u;
+          }
+        }
+      }
+    } else if (warp == 1 && lane == 0) {  // dQ writer
+      tma_prefetch_desc(&tmDQ);
+      int it = 0;
+      for (int pass = 0; pass < n_pass; ++pass) {
+        const Tile t = tile_of(p, pass);
+        for (int j = 0; j < t.n_items; ++j, ++it) {
+          const int h = hk * group + j / t.per_head;
+          const int q0 = (t.qt0 + j % t.per_head) * BQ;
+          const int buf = it & 1;
+          mbar_wait(dq_full0 + 8 * buf, (it >> 1) & 1);
+#pragma unroll
+          for (int blk = 0; blk < D / 32; ++blk)
+            tma_reduce_add_4d(sDQ + buf * Cfg::DQ_BYTES + blk * 8192, &tmDQ, blk * 32, h, q0, b);
+          bulk_commit();
+          bulk_wait_read<0>();
+          mbar_arrive(dq_empty0 + 8 * buf);
+        }
+      }
+      bulk_wait<0>();
     }
-  };
-  if (threadIdx.x == 0) {
-    mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
-    for (int nb = 0; nb < Cfg::NB; ++nb) {
-      tma_load_4d(sK + nb * BKV * 128, &tmK, kv_full, nb * 64, hk, k0, b);
-      tma_load_4d(sV + nb * BKV * 128, &tmV, kv_full, nb * 64, hk, k0, b);
-    }
-    if (n_items > 0) issue_item(0);
+    return;
   }
 
-  const int wg = warp >> 2, wq = warp & 3;
+  setmaxnreg_inc<240>();
+  const int c = wg - 1;  // consumer warpgroup: keys 64c .. 64c+63 of the tile
+  const int wq = warp & 3;
   const int g = lane >> 2, cq = (lane & 3) * 2;
-  const int key_a = k0 + wg * 64 + wq * 16 + g;  // this thread's keys: key_a, key_a + 8
-  float dk[D / 2], dv[D / 2];
-#pragma unroll
-  for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
   const float sl2 = p.scale * kLog2e;
-  mbar_wait(kv_full, 0);
+  int slot = 0;
+  uint32_t phase = 0;
+  int it = 0;
 
-  for (int it = 0; it < n_items; ++it) {
-    const int s = it & 1;
-    const int h = hk * group + it / per_head;
-    const int q0 = (qt_first + it % per_head) * BQ;
-    if (threadIdx.x == 0 && it + 1 < n_items) issue_item(it + 1);
-    mbar_wait(q_full0 + 8 * s, (it >> 1) & 1);
-    const uint32_t tQ = sQ + s * Cfg::QS_BYTES, tDO = sDO + s * Cfg::QS_BYTES;
+  for (int pass = 0; pass < n_pass; ++pass) {
+    const Tile t = tile_of(p, pass);
+    const int key_a = t.k0 + c * 64 + wq * 16 + g;  // this thread's keys: key_a, key_a + 8
+    const int wkey_hi = t.k0 + c * 64 + 63;          // last key of this warpgroup
+    float dk[D / 2], dv[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
+    mbar_wait_outlined(kv_full, pass & 1);
 
-    // S^T = K Q^T and dP^T = V dO^T: 64 keys x 64 queries per warpgroup
-    float st[32], dpt[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) st[i] = dpt[i] = 0.f;
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t ka = (kk >> 2) * BKV * 128 + wg * 64 * 128 + (kk & 3) * 32;
-      const uint32_t qb = (kk >> 2) * BQ * 128 + (kk & 3) * 32;
-      wgmma_m64n64k16_ss<0, 0>(st, make_wgmma_desc_sw128(sK + ka, 16, 1024), make_wgmma_desc_sw128(tQ + qb, 16, 1024));
-      wgmma_m64n64k16_ss<0, 0>(dpt, make_wgmma_desc_sw128(sV + ka, 16, 1024), make_wgmma_desc_sw128(tDO + qb, 16, 1024));
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
+    for (int j = 0; j < t.n_items; ++j, ++it) {
+      const int q0 = (t.qt0 + j % t.per_head) * BQ;
+      mbar_wait_outlined(q_full0 + 8 * slot, phase);
+      const uint32_t tQ = sQ + slot * Cfg::QS_BYTES, tDO = sDO + slot * Cfg::QS_BYTES;
+      const uint32_t tL = sL + slot * Cfg::L_BYTES, tDlt = tL + BQ * 4;  // LSE*log2e, delta of the 64 queries
 
-    // P^T and dS^T (unscaled); masked entries are exactly 0.  Chunk nc holds queries 8 nc + cq + {0, 1}.
-    const long long lrow = ((long long)b * p.H + h) * p.S;
+      // S^T = K Q^T and dP^T = V dO^T: 64 keys x 64 queries per warpgroup
+      float st[32], dpt[32];
 #pragma unroll
-    for (int nc = 0; nc < 8; ++nc) {
+      for (int i = 0; i < 32; ++i) st[i] = dpt[i] = 0.f;
+      wgmma_fence();
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int qi = q0 + nc * 8 + cq + (e & 1);
-        const int key = key_a + ((e >> 1) << 3);
-        const bool ok = qi < p.S && key < p.S && !(p.causal && key > qi);
-        const float pv = ok ? exp2f(st[4 * nc + e] * sl2 - p.lse[lrow + qi] * kLog2e) : 0.f;
-        st[4 * nc + e] = pv;
-        dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] - p.delta[lrow + qi]) : 0.f;
+      for (int kk = 0; kk < D / 16; ++kk) {
+        const uint32_t ka = (kk >> 2) * BKV * 128 + c * 64 * 128 + (kk & 3) * 32;
+        const uint32_t qb = (kk >> 2) * BQ * 128 + (kk & 3) * 32;
+        wgmma_m64n64k16_ss<0, 0>(st, make_wgmma_desc_sw128(sK + ka, 16, 1024), make_wgmma_desc_sw128(tQ + qb, 16, 1024));
+        wgmma_m64n64k16_ss<0, 0>(dpt, make_wgmma_desc_sw128(sV + ka, 16, 1024), make_wgmma_desc_sw128(tDO + qb, 16, 1024));
       }
-    }
-    uint32_t pa[4][4], da[4][4];
+      wgmma_commit();
+      wgmma_wait<0>();
+
+      // P^T and dS^T (unscaled).  Chunk nc holds queries 8 nc + cq + {0, 1}.  Only tiles that cross the causal
+      // diagonal or the end of the sequence are masked; masked entries are exactly 0.
+      const bool masked = (p.causal && wkey_hi > q0) || q0 + BQ > p.S || wkey_hi >= p.S;
+      if (masked) {
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
+        for (int nc = 0; nc < 8; ++nc) {
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        pa[kk][i] = pack_bf16x2(st[8 * kk + 2 * i], st[8 * kk + 2 * i + 1]);
-        da[kk][i] = pack_bf16x2(dpt[8 * kk + 2 * i], dpt[8 * kk + 2 * i + 1]);
+          for (int e = 0; e < 4; ++e) {
+            const int qc = nc * 8 + cq + (e & 1);
+            const int qi = q0 + qc;
+            const int key = key_a + ((e >> 1) << 3);
+            const bool ok = qi < p.S && key < p.S && !(p.causal && key > qi);
+            const float pv = ok ? exp2f(st[4 * nc + e] * sl2 - lds32f(tL + qc * 4)) : 0.f;
+            st[4 * nc + e] = pv;
+            dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] - lds32f(tDlt + qc * 4)) : 0.f;
+          }
+        }
+      } else {
+#pragma unroll
+        for (int nc = 0; nc < 8; ++nc) {
+          const float2 l = lds64f(tL + (nc * 8 + cq) * 4);
+          const float2 d = lds64f(tDlt + (nc * 8 + cq) * 4);
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float pv = exp2f(st[4 * nc + e] * sl2 - ((e & 1) ? l.y : l.x));
+            st[4 * nc + e] = pv;
+            dpt[4 * nc + e] = pv * (dpt[4 * nc + e] - ((e & 1) ? d.y : d.x));
+          }
+        }
       }
-    }
-    // dS^T rows of this thread -> [key][64 queries] tile, 128 B per row, 16-byte chunks XOR (row % 8)
-    {
-      const int r = wg * 64 + wq * 16 + g;
+      uint32_t pa[4][4], da[4][4];
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
-          const int row = r + ((i & 1) << 3), chunk = 2 * kk + (i >> 1);
-          *reinterpret_cast<uint32_t*>(smem + Cfg::OFF_DS + row * 128 + ((chunk ^ (row & 7)) << 4) + cq * 2) = da[kk][i];
+          pa[kk][i] = pack_bf16x2(st[8 * kk + 2 * i], st[8 * kk + 2 * i + 1]);
+          da[kk][i] = pack_bf16x2(dpt[8 * kk + 2 * i], dpt[8 * kk + 2 * i + 1]);
         }
       }
-    }
-    fence_proxy_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads below
+      // dS^T rows of this thread -> [key][64 queries] tile, 128 B per row, 16-byte chunks XOR (row % 8)
+      const uint32_t tDS = sDS + (it & 1) * Cfg::DS_BYTES;
+      {
+        const int r = c * 64 + wq * 16 + g;
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int row = r + ((i & 1) << 3), chunk = 2 * kk + (i >> 1);
+            sts32(tDS + row * 128 + ((chunk ^ (row & 7)) << 4) + cq * 2, da[kk][i]);
+          }
+        }
+      }
+      fence_proxy_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads below
 
-    // dV += P^T dO, dK += dS^T Q: k = queries (16 rows of 128 B per step), n = head dim (64-column blocks)
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) rs_mma<D>(dv, pa[kk], make_wgmma_desc_sw128(tDO + kk * 2048, BQ * 128, 1024));
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) rs_mma<D>(dk, da[kk], make_wgmma_desc_sw128(tQ + kk * 2048, BQ * 128, 1024));
-    wgmma_commit();
-    named_bar_sync(1, 256);  // both warpgroups' dS^T rows are in shared memory
-
-    // dQ[64 queries, head-dim block] = dS K over all 128 keys; at D = 64 warpgroup 0 does the whole tile
-    float dq[32];
-    const bool do_dq = (D == 128) || wg == 0;
-    const int nblk = (D == 128) ? wg : 0;
-    if (do_dq) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+      // dV += P^T dO, dK += dS^T Q: k = queries (16 rows of 128 B per step), n = head dim (64-column blocks)
       wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < BKV / 16; ++kk)
-        wgmma_m64n64k16_ss<1, 1>(dq, make_wgmma_desc_sw128(sDS + kk * 2048, 8192, 1024),
-                                 make_wgmma_desc_sw128(sK + nblk * BKV * 128 + kk * 2048, BKV * 128, 1024));
+      for (int kk = 0; kk < 4; ++kk) rs_mma<D>(dv, pa[kk], make_wgmma_desc_sw128(tDO + kk * 2048, BQ * 128, 1024));
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) rs_mma<D>(dk, da[kk], make_wgmma_desc_sw128(tQ + kk * 2048, BQ * 128, 1024));
       wgmma_commit();
-    }
-    wgmma_wait<0>();
-    if ((threadIdx.x & 127) == 0) mbar_arrive(q_empty0 + 8 * s);
-    if (do_dq) {
-      float* dqb = p.dq_acc + ((long long)b * p.S * p.H + h) * D + nblk * 64;
+      // both warpgroups' dS^T rows are in shared memory.  dS^T is double-buffered: this barrier of item it+1 also
+      // orders the dQ reads of item it before the rewrite of its buffer by item it+2.
+      named_bar_sync(1, 256);
+      wgmma_wait<0>();  // P^T / dS^T registers are free before the dQ accumulators are live
+
+      // dQ[64 queries, D/2 head-dim columns of this warpgroup] = dS K over all 128 keys
+      constexpr int NQ = D / 4;  // accumulators per thread
+      float dq[NQ];
 #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int qi = q0 + wq * 16 + g + 8 * r;
-        if (qi >= p.S) continue;
-        float* row = dqb + (long long)qi * p.H * D + cq;
+      for (int i = 0; i < NQ; ++i) dq[i] = 0.f;
+      wgmma_fence();
 #pragma unroll
-        for (int nc = 0; nc < 8; ++nc) {
-          atomicAdd(row + nc * 8, dq[4 * nc + 2 * r]);
-          atomicAdd(row + nc * 8 + 1, dq[4 * nc + 2 * r + 1]);
+      for (int kk = 0; kk < BKV / 16; ++kk) {
+        const uint64_t da_ = make_wgmma_desc_sw128(tDS + kk * 2048, 8192, 1024);
+        if constexpr (D == 128)
+          wgmma_m64n64k16_ss<1, 1>(dq, da_, make_wgmma_desc_sw128(sK + c * BKV * 128 + kk * 2048, BKV * 128, 1024));
+        else  // columns 32c .. 32c+31: half c of each 128-byte K row
+          wgmma_m64n32k16_ss<1, 1>(dq, da_, make_wgmma_desc_sw128(sK + kk * 2048 + c * 64, BKV * 128, 1024));
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(q_empty0 + 8 * slot);
+      if (++slot == ST) {
+        slot = 0;
+        phase ^= 1u;
+      }
+
+      // dQ fragment -> fp32 tile in the dq_acc map's layout: block of 32 columns = [64 rows][128 B], 16-byte chunk
+      // index XOR (row % 8).  Row g / g+8 of a warp hit 8 distinct chunk pairs: conflict-free 8-byte stores.
+      const int buf = it & 1;
+      mbar_wait_outlined(dq_empty0 + 8 * buf, ((it >> 1) & 1) ^ 1u);
+      {
+        const uint32_t tDQ = sDQ + buf * Cfg::DQ_BYTES;
+#pragma unroll
+        for (int nc = 0; nc < NQ / 4; ++nc) {
+          // columns c*D/2 + 8 nc + cq + {0, 1}: 32-column block, 16-byte chunk and 8-byte half within it
+          const int blk = c * (D / 64) + (nc >> 2);
+          const int chunk = 2 * (nc & 3) + (cq >> 2);
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int row = wq * 16 + g + 8 * r;  // row % 8 == g
+            sts64f(tDQ + blk * 8192 + row * 128 + ((chunk ^ g) << 4) + (cq & 2) * 4, dq[4 * nc + 2 * r],
+                   dq[4 * nc + 2 * r + 1]);
+          }
         }
       }
+      fence_proxy_async_smem();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(dq_full0 + 8 * buf);
     }
-    named_bar_sync(1, 256);  // the dS^T tile is rewritten by the next item
-  }
+    // every read of this tile's K / V has completed (the last dQ wgmma was waited for)
+    if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty);
 
-  // dK (scale applied here), dV -> bf16 rows of dkv_rh heads
+    // dK (scale applied here), dV -> bf16 rows of dkv_rh heads
 #pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int key = key_a + 8 * r;
-    if (key >= p.S) continue;
-    const long long off = ((long long)b * p.S + key) * p.dkv_rh * D + (long long)hk * D + cq;
+    for (int r = 0; r < 2; ++r) {
+      const int key = key_a + 8 * r;
+      if (key >= p.S) continue;
+      const long long off = ((long long)b * p.S + key) * p.dkv_rh * D + (long long)hk * D + cq;
 #pragma unroll
-    for (int dc = 0; dc < D / 8; ++dc) {
-      *reinterpret_cast<uint32_t*>(p.dk + off + dc * 8) =
-          pack_bf16x2(dk[4 * dc + 2 * r] * p.scale, dk[4 * dc + 2 * r + 1] * p.scale);
-      *reinterpret_cast<uint32_t*>(p.dv + off + dc * 8) = pack_bf16x2(dv[4 * dc + 2 * r], dv[4 * dc + 2 * r + 1]);
+      for (int dc = 0; dc < D / 8; ++dc) {
+        *reinterpret_cast<uint32_t*>(p.dk + off + dc * 8) =
+            pack_bf16x2(dk[4 * dc + 2 * r] * p.scale, dk[4 * dc + 2 * r + 1] * p.scale);
+        *reinterpret_cast<uint32_t*>(p.dv + off + dc * 8) = pack_bf16x2(dv[4 * dc + 2 * r], dv[4 * dc + 2 * r + 1]);
+      }
     }
   }
 }
 
-// delta[b,h,s] = sum_d o[b,s,h,d] * do[b,s,h,d]; LPR = D/8 lanes cooperate on one row.  The same pass zeroes the
-// fp32 dQ accumulator (same [B,S,H,D] index space: each thread clears the 8 floats under the 8 bf16 it reads), so the
-// backward needs no separate memset launch over 4*B*S*H*D bytes.
+// delta[b,h,s] = sum_d o[b,s,h,d] * do[b,s,h,d] and lse2[b,h,s] = lse[b,h,s] * log2e, both in rows of S_pad floats
+// (whole 64-query tiles, 16-byte aligned, for the backward's bulk copies); LPR = D/8 lanes cooperate on one row.  The
+// same pass zeroes the fp32 dQ accumulator (same [B,S,H,D] index space: each thread clears the 8 floats under the 8
+// bf16 it reads), so the backward needs no separate memset launch over 4*B*S*H*D bytes.
 template <int D>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o,
-                  float* __restrict__ delta, float* __restrict__ dq_acc, int B, int S, int H) {
+                  const float* __restrict__ lse, float* __restrict__ delta, float* __restrict__ lse2,
+                  float* __restrict__ dq_acc, int B, int S, int H, int S_pad) {
   constexpr int LPR = D / 8;
   const long long rows = (long long)B * S * H;
   const long long gtid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -272,7 +389,8 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __re
     const long long bs = r / H;
     const int s = (int)(bs % S);
     const long long bb = bs / S;
-    delta[(bb * H + hh) * S + s] = acc;
+    delta[(bb * H + hh) * S_pad + s] = acc;
+    lse2[(bb * H + hh) * S_pad + s] = lse[(bb * H + hh) * S + s] * kLog2e;
   }
 }
 
@@ -293,7 +411,7 @@ f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ ds
 
 template <int D>
 int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmDO,
-               const BwdArgs& a, cudaStream_t stream) {
+               const CUtensorMap& tmDQ, const BwdArgs& a, cudaStream_t stream) {
   using Cfg = BwdCfg<D>;
   auto kern = attn_bwd_kernel<D>;
   static bool attr_set = false;
@@ -301,19 +419,29 @@ int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set = true;
   }
-  dim3 grid((a.S + BKV - 1) / BKV, a.Hk, a.B);
-  kern<<<grid, BWD_THREADS, Cfg::SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmDO, a);
+  const int n_kt = (a.S + BKV - 1) / BKV;
+  dim3 grid(a.paired ? n_kt / 2 : n_kt, a.Hk, a.B);
+  kern<<<grid, BWD_THREADS, Cfg::SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmDO, tmDQ, a);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
 inline size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
+inline int pad_q(int S) { return (S + BQ - 1) / BQ * BQ; }
+
+// fp32 [B, S, H, D] dQ accumulator -> 4-D tensor map {D, H, S, B}, box {32, 1, 64, 1} (one 128-byte swizzle span)
+int make_dq_acc_map(CUtensorMap* tm, const float* base, int B, int S, int H, int D) {
+  const uint64_t dims[4] = {(uint64_t)D, (uint64_t)H, (uint64_t)S, (uint64_t)B};
+  const uint64_t strides[3] = {(uint64_t)D * 4, (uint64_t)H * D * 4, (uint64_t)S * H * D * 4};
+  const uint32_t box[4] = {32, 1, (uint32_t)BQ, 1};
+  return make_tensor_map(tm, base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 4, dims, strides, box, true);
+}
 
 }  // namespace
 
 size_t attn_bwd_workspace_bytes(int B, int S, int H, int Hk, int D) {
   (void)Hk;
-  return al256((size_t)B * S * H * D * 4) + al256((size_t)B * H * S * 4);
+  return al256((size_t)B * S * H * D * 4) + 2 * al256((size_t)B * H * pad_q(S) * 4);
 }
 
 int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
@@ -337,37 +465,44 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
                    reinterpret_cast<uintptr_t>(o) | reinterpret_cast<uintptr_t>(d_o)) & 15u) == 0,
                  "attn_bwd: q/k/v/o/do must be 16-byte aligned");
   float* dq_acc = reinterpret_cast<float*>(ws);
+  const int S_pad = pad_q(S);
   float* delta = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + al256((size_t)B * S * H * D * 4));
+  float* lse2 = reinterpret_cast<float*>(reinterpret_cast<char*>(delta) + al256((size_t)B * H * S_pad * 4));
   const long long n = (long long)B * S * H * D;
   {
     const long long threads = (long long)B * S * H * (D / 8);
     const int blocks = (int)((threads + 255) / 256);
     if (D == 64)
-      attn_delta_kernel<64><<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, delta, dq_acc, B, S, H);
+      attn_delta_kernel<64><<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, lse, delta,
+                                                        lse2, dq_acc, B, S, H, S_pad);
     else
-      attn_delta_kernel<128><<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, delta, dq_acc, B, S, H);
+      attn_delta_kernel<128><<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, lse, delta,
+                                                         lse2, dq_acc, B, S, H, S_pad);
     B200_CHECK_LAUNCH();
   }
-  CUtensorMap tmQ, tmK, tmV, tmDO;
+  CUtensorMap tmQ, tmK, tmV, tmDO, tmDQ;
   int rc;
   if ((rc = make_bshd_map(&tmQ, q, B, S, H, D, BQ))) return rc;
   if ((rc = make_bshd_map(&tmK, k, B, S, Hk, D, BKV))) return rc;
   if ((rc = make_bshd_map(&tmV, v, B, S, Hk, D, BKV))) return rc;
   if ((rc = make_bshd_map(&tmDO, d_o, B, S, H, D, BQ))) return rc;
+  if ((rc = make_dq_acc_map(&tmDQ, dq_acc, B, S, H, D))) return rc;
   BwdArgs a;
-  a.lse = lse;
+  a.lse2 = lse2;
   a.delta = delta;
-  a.dq_acc = dq_acc;
   a.dk = reinterpret_cast<__nv_bfloat16*>(dk);
   a.dv = reinterpret_cast<__nv_bfloat16*>(dv);
   a.B = B;
   a.S = S;
   a.H = H;
   a.Hk = Hk;
+  a.S_pad = S_pad;
   a.dkv_rh = dkv_row_heads;
   a.scale = scale;
   a.causal = causal;
-  rc = D == 64 ? launch_bwd<64>(tmQ, tmK, tmV, tmDO, a, stream) : launch_bwd<128>(tmQ, tmK, tmV, tmDO, a, stream);
+  a.paired = causal && ((S + BKV - 1) / BKV) % 2 == 0;
+  rc = D == 64 ? launch_bwd<64>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+               : launch_bwd<128>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
   if (rc) return rc;
   {
     const long long nvec = n / 8;

@@ -66,6 +66,12 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if ((++spins & 0x3ffu) == 0 && globaltimer_ns() - t0 > 4000000000ull) __trap();
   }
 }
+// The same bounded wait with its slow path out of line, for code after setmaxnreg.inc: a __trap() inlined there makes
+// ptxas allocate the whole region within the launch-bound register count (168 at 384 threads) instead of the raised one.
+static __device__ __noinline__ void mbar_wait_slow(uint32_t bar, uint32_t parity) { mbar_wait(bar, parity); }
+__device__ __forceinline__ void mbar_wait_outlined(uint32_t bar, uint32_t parity) {
+  if (!mbar_try_wait(bar, parity)) mbar_wait_slow(bar, parity);
+}
 
 // ---------------------------------------------------------------------------------------------
 // TMA (cp.async.bulk.tensor), tiled mode
@@ -140,6 +146,19 @@ __device__ __forceinline__ void wgmma_m64n64k16_ss(float* d, uint64_t da, uint64
         "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
 }
+// D[64 x 32] (+)= A[64 x 16] B[16 x 32], both operands in shared memory; TA / TB = 1 when MN-major.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n32k16_ss(float* d, uint64_t da, uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %20, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, %18, %19;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "n"(TA), "n"(TB), "r"(1));
+}
 // D[64 x 128] (+)= A[64 x 16] B[16 x 128] with A in registers (the accumulator fragment layout packed to bf16)
 template <int TB>
 __device__ __forceinline__ void wgmma_m64n128k16_rs(float* d, const uint32_t* a, uint64_t db) {
@@ -210,6 +229,22 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t* r) {
                : "r"(addr)
                : "memory");
 }
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void sts64f(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ float lds32f(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ float2 lds64f(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+  return v;
+}
 __device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
   asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
                : "memory");
@@ -229,6 +264,32 @@ __device__ __forceinline__ void tma_load_4d(uint32_t smem_dst, const CUtensorMap
       " [%0], [%1, {%3, %4, %5, %6}], [%2];"
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
+}
+// 1-D bulk copy global -> shared, completing `bytes` (a multiple of 16, both addresses 16-byte aligned) on `bar`
+__device__ __forceinline__ void bulk_load(uint32_t smem_dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
+               : "memory");
+}
+// global[box at {c0..c3}] += shared tile (fp32 add in L2), tracked by the issuing thread's bulk groups.  Rows of the
+// box outside the tensor are skipped.
+__device__ __forceinline__ void tma_reduce_add_4d(uint32_t smem_src, const CUtensorMap* m, int c0, int c1, int c2,
+                                                  int c3) {
+  asm volatile(
+      "cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+      ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// wait until at most N committed bulk groups still read their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// wait until at most N committed bulk groups are still incomplete
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------
