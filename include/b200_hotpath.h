@@ -195,6 +195,20 @@ int b200_shampoo_stats(const void* g_hi, const void* g_lo, long long ldg, long l
 size_t b200_shampoo_root_workspace_bytes(int batch, int k);
 int b200_shampoo_root(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float p,
                       float eps, int iters, void* workspace, size_t workspace_bytes, void* stream);
+/* b200_shampoo_root_newton -- a true inverse 4th root, offered next to the literal b200_shampoo_root (which
+ * MatrixSqrt.matrix_inverse_pth_root, shampoo.py:88-126, is not: SURVEY D10); selected by ShampooParams.inverse_root:
+ *   P = (M + ridge*I_k)^(-1/4),  ridge = eps * max(lambda_max(M), 1e-6)   (lambda_max by power iteration)
+ *   coupled Newton, r = 4: Mt = M + ridge I ; z = 5 / (2 ||Mt||_F) ; Mc = z Mt ; X = z^(1/4) I ;
+ *   up to max_iters x { T = 1.25 I - Mc/4 ; Mc' = T^4 Mc ; e' = max|Mc' - I| ; accept iff e' <= 1.2 e:
+ *   X = X T, Mc = Mc', e = e' } ; a matrix freezes once e <= tol or a step is rejected ; P = X.
+ *   Products at fp32 accuracy (3-way bf16 split; hh over 64-wide K slices, five more products).
+ *   M, P: f32 [batch,kp,kp] (distinct), padding of P exactly zero; P_hi/P_lo (nullable): bf16 split of P;
+ *   iters_out (int) / residual_out (f32, the final e) [batch], nullable.  Bit-identical run to run and independent of the batch a matrix is launched in.
+ *   Synchronises `stream` every 4 iterations to stop once every matrix is frozen. */
+size_t b200_shampoo_root_newton_workspace_bytes(int batch, int k);
+int b200_shampoo_root_newton(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float eps,
+                             int max_iters, float tol, int* iters_out, float* residual_out, void* workspace,
+                             size_t workspace_bytes, void* stream);
 /* b200_shampoo_precond -- Shampoo._apply_preconditioners (shampoo.py:257-295):
  *   out[:k1,:k2] = alpha * PL @ m[:k1,:k2] @ PR   (elements of `out` outside the block are left alone)
  *   m_hi/m_lo: bf16 split of the (bias-corrected) momentum, [batch][rows][ldm]; out: f32 [batch][rows][ldo];

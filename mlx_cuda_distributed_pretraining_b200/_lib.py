@@ -32,6 +32,8 @@ SIGNATURES = {
     "b200_shampoo_stats": (_i, [_vp, _vp, _ll, _ll, _vp, _vp, _i, _i, _i, _f, _f, _vp]),
     "b200_shampoo_root_workspace_bytes": (_sz, [_i, _i]),
     "b200_shampoo_root": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _f, _i, _vp, _sz, _vp]),
+    "b200_shampoo_root_newton_workspace_bytes": (_sz, [_i, _i]),
+    "b200_shampoo_root_newton": (_i, [_vp, _vp, _vp, _vp, _i, _i, _f, _i, _f, _vp, _vp, _vp, _sz, _vp]),
     "b200_shampoo_precond_workspace_bytes": (_sz, [_i, _i, _i]),
     "b200_shampoo_precond": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _ll, _ll, _vp, _ll, _ll, _i, _i, _i, _f, _vp,
                                   _sz, _vp]),

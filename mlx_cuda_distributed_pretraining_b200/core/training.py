@@ -368,7 +368,8 @@ class OptimizationManager:
                 start_preconditioning_step=cfg.get("start_preconditioning_step", 1000),
                 preconditioner_epsilon=cfg.get("preconditioner_epsilon", 1e-6),
                 exponent_override=cfg.get("exponent_override", 0.75), use_bias_correction=True,
-                grafting_optimizer=cfg.get("grafting_optimizer", "adam"), use_decoupled_weight_decay=True)
+                grafting_optimizer=cfg.get("grafting_optimizer", "adam"), use_decoupled_weight_decay=True,
+                inverse_root=cfg.get("inverse_root", "reference"))
             return Shampoo(learning_rate=schedule, params=params)
         if name == "hybrid":
             m_cfg = {k: v for k, v in cfg.items() if k not in ("optimizer", "non_matrix_optimizer")}

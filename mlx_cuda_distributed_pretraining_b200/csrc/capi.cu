@@ -40,6 +40,10 @@ int shampoo_stats(const void* g_hi, const void* g_lo, long long ldg, long long s
 size_t shampoo_root_workspace_bytes(int batch, int k);
 int shampoo_root(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float p, float eps, int iters,
                  void* ws, size_t ws_bytes, cudaStream_t stream);
+size_t shampoo_root_newton_workspace_bytes(int batch, int k);
+int shampoo_root_newton(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float eps, int max_iters,
+                        float tol, int* iters_out, float* residual_out, void* ws, size_t ws_bytes,
+                        cudaStream_t stream);
 size_t shampoo_precond_workspace_bytes(int batch, int k1, int k2);
 int shampoo_precond(const void* PL_hi, const void* PL_lo, const void* PR_hi, const void* PR_lo, const void* m_hi,
                     const void* m_lo, long long ldm, long long strideM, float* out, long long ldo, long long strideO,
@@ -102,7 +106,7 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
 
 extern "C" {
 
-int b200_version(void) { return 3; }
+int b200_version(void) { return 4; }
 const char* b200_last_error(void) { return b200::last_error(); }
 
 unsigned long long b200_launch_count(void) { return b200::launch_count(); }
@@ -211,6 +215,15 @@ size_t b200_shampoo_root_workspace_bytes(int batch, int k) { return b200::shampo
 int b200_shampoo_root(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float p,
                       float eps, int iters, void* workspace, size_t workspace_bytes, void* stream) {
   return b200::shampoo_root(M, P, P_hi, P_lo, batch, k, p, eps, iters, workspace, workspace_bytes, S_(stream));
+}
+size_t b200_shampoo_root_newton_workspace_bytes(int batch, int k) {
+  return b200::shampoo_root_newton_workspace_bytes(batch, k);
+}
+int b200_shampoo_root_newton(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float eps,
+                             int max_iters, float tol, int* iters_out, float* residual_out, void* workspace,
+                             size_t workspace_bytes, void* stream) {
+  return b200::shampoo_root_newton(M, P, P_hi, P_lo, batch, k, eps, max_iters, tol, iters_out, residual_out,
+                                   workspace, workspace_bytes, S_(stream));
 }
 size_t b200_shampoo_precond_workspace_bytes(int batch, int k1, int k2) {
   return b200::shampoo_precond_workspace_bytes(batch, k1, k2);

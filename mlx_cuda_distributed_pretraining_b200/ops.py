@@ -771,6 +771,27 @@ def shampoo_root(M: torch.Tensor, P: torch.Tensor, P_hi: Optional[torch.Tensor],
     return P
 
 
+def shampoo_root_newton(M: torch.Tensor, P: torch.Tensor, P_hi: Optional[torch.Tensor], P_lo: Optional[torch.Tensor],
+                        k: int, eps: float, max_iters: int = 40, tol: float = 1e-5,
+                        workspace: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """True inverse 4th root P = (M + ridge I)^(-1/4), ridge = eps * max(lambda_max(M), 1e-6), of M [batch, kp, kp]
+    fp32 by the coupled Newton iteration.  Returns the per-matrix accepted iteration counts (int32) and final
+    residuals max|Mc - I| (fp32), both [batch] on the device."""
+    _need(M, torch.float32, "M")
+    _need(P, torch.float32, "P")
+    batch = M.shape[0]
+    need = int(lib().b200_shampoo_root_newton_workspace_bytes(batch, int(k)))
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, device=M.device, dtype=torch.uint8)
+    iters = torch.empty(batch, device=M.device, dtype=torch.int32)
+    residual = torch.empty(batch, device=M.device, dtype=torch.float32)
+    check(lib().b200_shampoo_root_newton(M.data_ptr(), P.data_ptr(), _ptr(P_hi), _ptr(P_lo), batch, int(k),
+                                         float(eps), int(max_iters), float(tol), iters.data_ptr(), residual.data_ptr(),
+                                         workspace.data_ptr(), workspace.numel(), _stream()),
+          "b200_shampoo_root_newton")
+    return iters, residual
+
+
 def shampoo_precond(PLh, PLl, PRh, PRl, m_hi, m_lo, ldm: int, stride_m: int, out: torch.Tensor, ldo: int,
                     stride_o: int, batch: int, k1: int, k2: int, alpha: float,
                     workspace: Optional[torch.Tensor] = None) -> None:

@@ -11,6 +11,7 @@ Per step (shampoo.py:314-378, with the wiring defects D1/D2/D9 of SURVEY 2.3 fix
   every `update_period` steps after `start_preconditioning_step`:                          b200_shampoo_root
         P = matrix_inverse_pth_root(stat)  -- the reference's literal formula (:88-126):
         Z0 = (M+eps I)/tr ; 6x Z <- Z + Z Z / p ; P = Z * tr^(-1/p^2)        (not a true inverse root)
+        or, inverse_root="newton": P = (M + ridge I)^(-1/4) by coupled Newton    b200_shampoo_root_newton
   m = b1 m + (1-b1) g ; mhat = m/(1-b1^t) ; pre = mhat with pre[:1024,:1024] = PL mhat PR   (:257-295)
                                                                                            b200_shampoo_precond
   upd = -lr*pre rescaled to ||d||_F (grafting, :297-312) ; decoupled wd: upd -= lr*wd*p     (:372-373)
@@ -29,13 +30,18 @@ for a group (momentum + grafting only) -- impossible with ParamStore's cols % 8 
 """
 from __future__ import annotations
 
-from dataclasses import dataclass
+from dataclasses import InitVar, dataclass
 from typing import Callable, Dict, List, Optional, Union
 
 import torch
 
 from .. import ops
 from ..flat import MatGroup, ParamStore, get_store
+
+# inverse_root="newton": the iteration reaches max|Mc - I| ~ 5e-7 from ~6e-4 in one step (fp32 floor ~2.4e-7 at
+# k = 1024), so 1e-5 costs no extra iteration; statistics with condition numbers up to the ridge's 1e6 take <= 25.
+NEWTON_MAX_ITERS = 40
+NEWTON_TOL = 1e-5
 
 
 @dataclass
@@ -52,8 +58,15 @@ class ShampooParams:
     use_bias_correction: bool = True
     grafting_optimizer: str = "adam"
     use_decoupled_weight_decay: bool = True
+    # "reference": the reference's literal matrix_inverse_pth_root (shampoo.py:88-126, not an inverse root);
+    # "newton": P = (M + ridge I)^(-1/4), ridge = preconditioner_epsilon * max(lambda_max(M), 1e-6), by the
+    # coupled Newton iteration.  exponent_override only parameterises the literal formula; newton ignores it.
+    # An init-only argument stored as an attribute, so the dataclass fields stay the reference's ShampooParams:
+    # dataclasses.replace() carries it over, but asdict(), repr() and == see the reference's fields only.
+    inverse_root: InitVar[str] = "reference"
 
-    def __post_init__(self):
+    def __post_init__(self, inverse_root: str = "reference"):
+        self.inverse_root = inverse_root
         assert 0.0 <= self.beta1 < 1.0, "beta1 must be in [0, 1)"
         assert 0.0 <= self.beta2 < 1.0, "beta2 must be in [0, 1)"
         assert self.epsilon > 0.0, "epsilon must be positive"
@@ -63,6 +76,8 @@ class ShampooParams:
         assert 0.0 < self.exponent_override <= 1.0, "exponent_override must be in (0, 1]"
         assert self.grafting_optimizer in ["sgd", "adam", "momentum"], \
             "grafting_optimizer must be one of 'sgd', 'adam', 'momentum'"
+        if self.inverse_root not in ("reference", "newton"):
+            raise ValueError(f"inverse_root must be 'reference' or 'newton', got {self.inverse_root!r}")
 
 
 class _GroupState:
@@ -133,8 +148,9 @@ class Shampoo:
         for g, s in zip(store.mat_groups, self._gs):
             ws = max(ws, int(lib.b200_shampoo_graft_workspace_bytes(g.batch)))
             if s.enabled:
-                ws = max(ws, int(lib.b200_shampoo_root_workspace_bytes(g.batch, s.k1)),
-                         int(lib.b200_shampoo_root_workspace_bytes(g.batch, s.k2)),
+                root_ws = (lib.b200_shampoo_root_newton_workspace_bytes if self.params.inverse_root == "newton"
+                           else lib.b200_shampoo_root_workspace_bytes)
+                ws = max(ws, int(root_ws(g.batch, s.k1)), int(root_ws(g.batch, s.k2)),
                          int(lib.b200_shampoo_precond_workspace_bytes(g.batch, s.k1, s.k2)))
         # non-2-D parameters: consecutive equal-length entries are grafted as one batched call
         self._vec_runs = []
@@ -162,9 +178,14 @@ class Shampoo:
 
     def _inverse_pth_root(self, stat: torch.Tensor, P: torch.Tensor, Ph: torch.Tensor, Pl: torch.Tensor,
                           k: int) -> None:
-        """MatrixSqrt.matrix_inverse_pth_root (shampoo.py:88-126), batched over stat [b, kp, kp]."""
+        """Preconditioner of stat [b, kp, kp]: MatrixSqrt.matrix_inverse_pth_root (shampoo.py:88-126) literally, or
+        with inverse_root="newton" the true (stat + ridge I)^(-1/4)."""
         hp = self.params
-        ops.shampoo_root(stat, P, Ph, Pl, k, hp.exponent_override, hp.preconditioner_epsilon, 6, self._ws)
+        if hp.inverse_root == "newton":
+            ops.shampoo_root_newton(stat, P, Ph, Pl, k, hp.preconditioner_epsilon, NEWTON_MAX_ITERS, NEWTON_TOL,
+                                    self._ws)
+        else:
+            ops.shampoo_root(stat, P, Ph, Pl, k, hp.exponent_override, hp.preconditioner_epsilon, 6, self._ws)
 
     @torch.no_grad()
     def after_load(self) -> None:
