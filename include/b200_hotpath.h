@@ -156,6 +156,28 @@ int b200_adam_direction(float* d, const void* g, int g_is_bf16, float* m, float*
                         float lr, float b1, float b2, float eps, float bc1, float bc2,
                         float gscale, void* stream);
 
+/* ---- Lion / SGD (optimizers/enhanced_optimizers.py:200-488; core/training.py:809-818,891-894) ------
+ * Shared by both entries:
+ *   gradient  gj = (g*gscale) * s,  s = min(1, max_norm / (sqrt(*clip_ss)*gscale + 1e-6)) when clip_ss != NULL
+ *             (_clip_gradients :417-432 / :285-300; *clip_ss = sum(g^2) over the same range from b200_sumsq with
+ *             batch = 1, read on the device: no host synchronisation), else s = 1.
+ *   EMA       ema_mode 0: none; 1: ema = p_new; 2: ema = ema_decay*ema + (1-ema_decay)*p_new
+ *             (_compute_ema :396-415 / :248-267, on the post-update parameters).
+ *   p16 = bf16(p32) when p16 != NULL.  g bf16 (g_is_bf16=1) or f32; every buffer 16-byte aligned; any n.
+ * b200_lion (LionEnhanced.update :434-484): c = b_sign*m + (1-b_sign)*gj ; p = p*decay - lr*sign(c) ;
+ *   m = b_mom*m + (1-b_mom)*gj ; sign(0) = 0.  b_sign == b_mom and decay = 1 is the reference as written
+ *   (b2 unused; its weight decay :471-472 never reaches the parameters); otherwise Chen et al. (2023)
+ *   with decay = 1 - lr*wd. */
+int b200_lion(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* ema, long long n,
+              float lr, float b_sign, float b_mom, float decay, float gscale, const float* clip_ss,
+              float max_norm, float ema_decay, int ema_mode, void* stream);
+/* b200_sgd (SGDEnhanced.update :302-351): gj += coupled_wd*p (coupled_wd = lr*wd, :269-283) ;
+ *   buf = mu*buf + (1-dampening)*gj ; p += -lr*(nesterov ? gj + mu*buf : buf).
+ *   buf == NULL: p += -lr*gj (mlx.optimizers.SGD with momentum 0, what the factory builds for `sgd`). */
+int b200_sgd(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, float* ema, long long n,
+             float lr, float mu, float dampening, int nesterov, float coupled_wd, float gscale,
+             const float* clip_ss, float max_norm, float ema_decay, int ema_mode, void* stream);
+
 /* ---- gradient post-processing (core/training.py:1664-1666,1671-1680) --------------------------
  * acc = (init?0:acc) + clamp(g,-clip,clip)*scale ; clip<=0 disables the clamp */
 int b200_clip_accum(const void* g, int g_is_bf16, float* acc, long long n, float clip,

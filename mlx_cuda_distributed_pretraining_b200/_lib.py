@@ -44,6 +44,8 @@ SIGNATURES = {
     "b200_sgd_momentum": (_i, [_vp, _vp, _vp, _i, _vp, _ll, _f, _i, _f, _f, _vp]),
     "b200_adamw": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _ll, _f, _f, _f, _f, _f, _f, _f, _f, _vp]),
     "b200_adam_direction": (_i, [_vp, _vp, _i, _vp, _vp, _ll, _f, _f, _f, _f, _f, _f, _f, _vp]),
+    "b200_lion": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _ll, _f, _f, _f, _f, _f, _vp, _f, _f, _i, _vp]),
+    "b200_sgd": (_i, [_vp, _vp, _vp, _i, _vp, _vp, _ll, _f, _f, _f, _i, _f, _f, _vp, _f, _f, _i, _vp]),
     "b200_clip_accum": (_i, [_vp, _i, _vp, _ll, _f, _f, _i, _vp]),
     "b200_sumsq": (_i, [_vp, _i, _vp, _ll, _i, _i, _vp, _sz, _vp]),
     "b200_split_bf16": (_i, [_vp, _ll, _vp, _vp, _ll, _i, _i, _f, _f, _vp]),

@@ -39,7 +39,7 @@ from .. import ops
 from ..arch.llama import Model, ModelArgs
 from ..distributed import dp
 from ..flat import ParamStore
-from ..optimizers import AdamW, HybridOptimizer, Muon, Shampoo, ShampooParams
+from ..optimizers import SGD, AdamW, HybridOptimizer, Lion, Muon, SGDEnhanced, Shampoo, ShampooParams
 
 
 # ------------------------------------------------------------------------------------------------
@@ -371,6 +371,22 @@ class OptimizationManager:
                 grafting_optimizer=cfg.get("grafting_optimizer", "adam"), use_decoupled_weight_decay=True,
                 inverse_root=cfg.get("inverse_root", "reference"))
             return Shampoo(learning_rate=schedule, params=params)
+        # the enhanced optimizers' extras (core/training.py:800-803): forwarded where the optimizer has them
+        extras = {k: cfg[k] for k in ("grad_clip_norm", "ema_momentum") if k in cfg}
+        if name == "lion":
+            kwargs.pop("eps", None)
+            return Lion(lion_variant=cfg.get("lion_variant", "reference"), **kwargs, **extras)
+        if name == "sgd_enhanced":
+            kwargs.pop("betas", None)
+            kwargs.pop("eps", None)
+            return SGDEnhanced(momentum=cfg.get("momentum", 0.9), nesterov=cfg.get("nesterov", False),
+                               **kwargs, **extras)
+        if name == "sgd":
+            # mlx.optimizers.SGD given the learning rate only (:891-894); the reference would raise TypeError on
+            # the extras, and dropping them silently would train without them
+            if extras:
+                raise ValueError(f"optimizer 'sgd' does not take {sorted(extras)}; use 'sgd_enhanced'")
+            return SGD(learning_rate=schedule)
         if name == "hybrid":
             m_cfg = {k: v for k, v in cfg.items() if k not in ("optimizer", "non_matrix_optimizer")}
             n_cfg = {k: v for k, v in cfg.items() if k not in ("optimizer", "matrix_optimizer")}

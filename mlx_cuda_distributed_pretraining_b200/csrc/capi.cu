@@ -63,6 +63,12 @@ int adamw(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* 
 int adam_direction(float* d, const void* g, int g_is_bf16, float* m, float* v, long long n,
                    float lr, float b1, float b2, float eps, float bc1, float bc2, float gscale,
                    cudaStream_t stream);
+int lion(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* ema, long long n, float lr,
+         float b_sign, float b_mom, float decay, float gscale, const float* clip_ss, float max_norm,
+         float ema_decay, int ema_mode, cudaStream_t stream);
+int sgd(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, float* ema, long long n, float lr,
+        float mu, float dampening, int nesterov, float coupled_wd, float gscale, const float* clip_ss,
+        float max_norm, float ema_decay, int ema_mode, cudaStream_t stream);
 int clip_accum(const void* g, int g_is_bf16, float* acc, long long n, float clip, float scale,
                int init, cudaStream_t stream);
 int sumsq(const void* x, int x_is_bf16, float* out, long long numel, int batch, int zero_first,
@@ -263,6 +269,18 @@ int b200_adam_direction(float* d, const void* g, int g_is_bf16, float* m, float*
                         float gscale, void* stream) {
   return b200::adam_direction(d, g, g_is_bf16, m, v, n, lr, b1, b2, eps, bc1, bc2, gscale,
                               S_(stream));
+}
+int b200_lion(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* ema, long long n,
+              float lr, float b_sign, float b_mom, float decay, float gscale, const float* clip_ss,
+              float max_norm, float ema_decay, int ema_mode, void* stream) {
+  return b200::lion(p32, p16, g, g_is_bf16, m, ema, n, lr, b_sign, b_mom, decay, gscale, clip_ss, max_norm,
+                    ema_decay, ema_mode, S_(stream));
+}
+int b200_sgd(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, float* ema, long long n,
+             float lr, float mu, float dampening, int nesterov, float coupled_wd, float gscale,
+             const float* clip_ss, float max_norm, float ema_decay, int ema_mode, void* stream) {
+  return b200::sgd(p32, p16, g, g_is_bf16, buf, ema, n, lr, mu, dampening, nesterov, coupled_wd, gscale, clip_ss,
+                   max_norm, ema_decay, ema_mode, S_(stream));
 }
 int b200_clip_accum(const void* g, int g_is_bf16, float* acc, long long n, float clip,
                     float scale, int init, void* stream) {

@@ -5,6 +5,8 @@
 //  axpy_update     optimizers/muon.py:111-114  p += s*X ; bf16 shadow copy refreshed in the same pass
 //  sgd_momentum    optimizers/muon.py:123-138  non-2-D fallback
 //  adamw           core/training.py:821 (mlx.optimizers.AdamW; formula also enhanced_optimizers.py:157-184)
+//  lion            optimizers/enhanced_optimizers.py:358-488 LionEnhanced (+ Chen et al.'s variant)
+//  sgd             enhanced_optimizers.py:200-355 SGDEnhanced; mlx.optimizers.SGD (core/training.py:891-894)
 //  clip_accum      core/training.py:1664-1666,1671-1680  clamp to +-clip, scale by 1/k, accumulate
 //  sumsq           Frobenius norms for Shampoo grafting (optimizers/shampoo.py:300-310)
 //
@@ -283,6 +285,123 @@ adam_direction_kernel(float* __restrict__ d, const G* __restrict__ g, float* __r
       m[i] = mm;
       v[i] = vv;
       d[i] = -step * mm / (sqrtf(vv) * rs_bc2 + eps);
+    }
+  }
+}
+
+// ---- Lion / SGD of enhanced_optimizers.py, with global-norm clipping and EMA weights fused in ----
+// The arithmetic is written with explicit round-to-nearest products and sums (no fma contraction), in
+// the reference's order of operations, so the fp32 results follow the reference's own rounding.
+
+// Factor the reference's _clip_gradients (:417-432, :285-300) applies to gradients of norm ||g*gscale||:
+// min(1, max_norm / (||g*gscale|| + 1e-6)).  `clip_ss` is the device sum of squares of the raw range
+// (b200_sumsq, batch 1: a fixed grid and summation order), so every thread forms the same factor with no
+// host read, and data-parallel replicas holding identical gradients form identical factors.
+__device__ __forceinline__ float clip_factor(const float* __restrict__ clip_ss, float max_norm, float gscale) {
+  if (clip_ss == nullptr) return 1.0f;
+  const float coef = max_norm / (sqrtf(*clip_ss) * gscale + 1e-6f);
+  return coef < 1.0f ? coef : 1.0f;
+}
+
+// ema_mode 0: none; 1: ema = p_new (first update); 2: ema = d*ema + (1-d)*p_new   (:396-415, :248-267)
+__device__ __forceinline__ float ema_step(float e, float p, float d, float omd, int ema_mode) {
+  return ema_mode == 1 ? p : __fadd_rn(__fmul_rn(d, e), __fmul_rn(omd, p));
+}
+
+// LionEnhanced.update (:434-484).  c = bs*m + (1-bs)*g ; p = p*decay - lr*sign(c) ; m = bm*m + (1-bm)*g.
+// bs == bm and decay == 1 is the reference as written (c is the stored momentum; its weight decay is
+// discarded); otherwise Chen et al.'s Lion with decoupled decay.  sign(0) = 0.
+__device__ __forceinline__ void lion_elem(float& p, float g, float& m, float& e, float lr, float bs, float obs,
+                                          float bm, float obm, float decay, float d, float omd, int ema_mode) {
+  const float c = __fadd_rn(__fmul_rn(bs, m), __fmul_rn(obs, g));
+  const float s = c > 0.f ? 1.0f : (c < 0.f ? -1.0f : 0.0f);
+  m = __fadd_rn(__fmul_rn(bm, m), __fmul_rn(obm, g));
+  p = __fadd_rn(__fmul_rn(p, decay), -lr * s);
+  if (ema_mode) e = ema_step(e, p, d, omd, ema_mode);
+}
+
+template <typename G>
+__global__ void __launch_bounds__(EW_THREADS)
+lion_kernel(float* __restrict__ p32, __nv_bfloat16* __restrict__ p16, const G* __restrict__ g,
+            float* __restrict__ m, float* __restrict__ ema, long long n, float lr, float bs, float bm,
+            float decay, float gscale, const float* __restrict__ clip_ss, float max_norm, float d,
+            int ema_mode) {
+  const float cf = clip_factor(clip_ss, max_norm, gscale);
+  const float obs = 1.0f - bs, obm = 1.0f - bm, omd = 1.0f - d;
+  const long long nvec = n / 8;
+  for (long long i = (long long)blockIdx.x * EW_THREADS + threadIdx.x; i < nvec;
+       i += (long long)gridDim.x * EW_THREADS) {
+    float pv[8], gv[8], mv[8], ev[8];
+    load8(p32 + i * 8, pv);
+    load8(g + i * 8, gv);
+    load8(m + i * 8, mv);
+    if (ema_mode == 2) load8(ema + i * 8, ev);
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      lion_elem(pv[j], __fmul_rn(__fmul_rn(gv[j], gscale), cf), mv[j], ev[j], lr, bs, obs, bm, obm, decay, d, omd,
+                ema_mode);
+    store8(p32 + i * 8, pv);
+    store8(m + i * 8, mv);
+    if (ema_mode) store8(ema + i * 8, ev);
+    if (p16) store8(p16 + i * 8, pv);
+  }
+  if (blockIdx.x == 0) {
+    for (long long i = nvec * 8 + threadIdx.x; i < n; i += EW_THREADS) {
+      float p = p32[i], mm = m[i], e = ema_mode == 2 ? ema[i] : 0.f;
+      lion_elem(p, __fmul_rn(__fmul_rn(ldf(g + i), gscale), cf), mm, e, lr, bs, obs, bm, obm, decay, d, omd,
+                ema_mode);
+      p32[i] = p;
+      m[i] = mm;
+      if (ema_mode) ema[i] = e;
+      if (p16) p16[i] = __float2bfloat16_rn(p);
+    }
+  }
+}
+
+// SGDEnhanced.update (:302-351) and mlx SGD:  g += wd_c*p (coupled decay, :269-283) ;
+// buf = mu*buf + (1-damp)*g ; p += -lr*(nesterov ? g + mu*buf : buf).  buf == NULL: p += -lr*g.
+template <typename G>
+__global__ void __launch_bounds__(EW_THREADS)
+sgd_kernel(float* __restrict__ p32, __nv_bfloat16* __restrict__ p16, const G* __restrict__ g,
+           float* __restrict__ buf, float* __restrict__ ema, long long n, float lr, float mu, float damp,
+           int nesterov, float wd_c, float gscale, const float* __restrict__ clip_ss, float max_norm, float d,
+           int ema_mode) {
+  const float cf = clip_factor(clip_ss, max_norm, gscale);
+  const float omdamp = 1.0f - damp, omd = 1.0f - d;
+  auto elem = [&](float& p, float gj, float& b, float& e) {
+    gj = __fmul_rn(__fmul_rn(gj, gscale), cf);
+    if (wd_c != 0.f) gj = __fadd_rn(gj, __fmul_rn(wd_c, p));
+    float u = gj;
+    if (buf) {
+      b = __fadd_rn(__fmul_rn(mu, b), __fmul_rn(omdamp, gj));
+      u = nesterov ? __fadd_rn(gj, __fmul_rn(mu, b)) : b;
+    }
+    p = __fadd_rn(p, __fmul_rn(-lr, u));
+    if (ema_mode) e = ema_step(e, p, d, omd, ema_mode);
+  };
+  const long long nvec = n / 8;
+  for (long long i = (long long)blockIdx.x * EW_THREADS + threadIdx.x; i < nvec;
+       i += (long long)gridDim.x * EW_THREADS) {
+    float pv[8], gv[8], bv[8], ev[8];
+    load8(p32 + i * 8, pv);
+    load8(g + i * 8, gv);
+    if (buf) load8(buf + i * 8, bv);
+    if (ema_mode == 2) load8(ema + i * 8, ev);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) elem(pv[j], gv[j], bv[j], ev[j]);
+    store8(p32 + i * 8, pv);
+    if (buf) store8(buf + i * 8, bv);
+    if (ema_mode) store8(ema + i * 8, ev);
+    if (p16) store8(p16 + i * 8, pv);
+  }
+  if (blockIdx.x == 0) {
+    for (long long i = nvec * 8 + threadIdx.x; i < n; i += EW_THREADS) {
+      float p = p32[i], b = buf ? buf[i] : 0.f, e = ema_mode == 2 ? ema[i] : 0.f;
+      elem(p, ldf(g + i), b, e);
+      p32[i] = p;
+      if (buf) buf[i] = b;
+      if (ema_mode) ema[i] = e;
+      if (p16) p16[i] = __float2bfloat16_rn(p);
     }
   }
 }
@@ -574,6 +693,50 @@ int adam_direction(float* d, const void* g, int g_is_bf16, float* m, float* v, l
   else
     adam_direction_kernel<float><<<grid, EW_THREADS, 0, stream>>>(d, (const float*)g, m, v, n, lr,
                                                                  b1, b2, eps, bc1, bc2, gscale);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+int lion(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* ema, long long n, float lr,
+         float b_sign, float b_mom, float decay, float gscale, const float* clip_ss, float max_norm,
+         float ema_decay, int ema_mode, cudaStream_t stream) {
+  B200_CHECK_ARG(n > 0, "lion: empty");
+  B200_CHECK_ARG(p32 && g && m, "lion: p32, g and m are required");
+  B200_CHECK_ARG(ema_mode >= 0 && ema_mode <= 2 && (ema_mode == 0 || ema), "lion: ema_mode %d needs ema (0..2)",
+                 ema_mode);
+  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(g) && aligned16(m) && aligned16(ema),
+                 "lion: buffers must be 16-byte aligned");
+  const int grid = ew_grid(n / 8 + 1);
+  if (g_is_bf16)
+    lion_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+        p32, (__nv_bfloat16*)p16, (const __nv_bfloat16*)g, m, ema, n, lr, b_sign, b_mom, decay, gscale, clip_ss,
+        max_norm, ema_decay, ema_mode);
+  else
+    lion_kernel<float><<<grid, EW_THREADS, 0, stream>>>(p32, (__nv_bfloat16*)p16, (const float*)g, m, ema, n, lr,
+                                                       b_sign, b_mom, decay, gscale, clip_ss, max_norm, ema_decay,
+                                                       ema_mode);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+int sgd(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, float* ema, long long n, float lr,
+        float mu, float dampening, int nesterov, float coupled_wd, float gscale, const float* clip_ss,
+        float max_norm, float ema_decay, int ema_mode, cudaStream_t stream) {
+  B200_CHECK_ARG(n > 0, "sgd: empty");
+  B200_CHECK_ARG(p32 && g, "sgd: p32 and g are required");
+  B200_CHECK_ARG(ema_mode >= 0 && ema_mode <= 2 && (ema_mode == 0 || ema), "sgd: ema_mode %d needs ema (0..2)",
+                 ema_mode);
+  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(g) && aligned16(buf) && aligned16(ema),
+                 "sgd: buffers must be 16-byte aligned");
+  const int grid = ew_grid(n / 8 + 1);
+  if (g_is_bf16)
+    sgd_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+        p32, (__nv_bfloat16*)p16, (const __nv_bfloat16*)g, buf, ema, n, lr, mu, dampening, nesterov, coupled_wd,
+        gscale, clip_ss, max_norm, ema_decay, ema_mode);
+  else
+    sgd_kernel<float><<<grid, EW_THREADS, 0, stream>>>(p32, (__nv_bfloat16*)p16, (const float*)g, buf, ema, n, lr,
+                                                      mu, dampening, nesterov, coupled_wd, gscale, clip_ss,
+                                                      max_norm, ema_decay, ema_mode);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

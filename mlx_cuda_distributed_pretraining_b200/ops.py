@@ -269,6 +269,67 @@ def adamw(p32, p16, g, m, v, lr: float, b1: float, b2: float, eps: float, wd: fl
           "b200_adamw")
 
 
+def _check_update_operands(what: str, p32, p16, g, state: dict) -> int:
+    """Shared checks of the fused optimizer updates: fp32 master, optional bf16 shadow, bf16|fp32 gradient and
+    fp32 state buffers, all contiguous CUDA tensors of p32's length starting on a 16-byte boundary."""
+    _need(p32, torch.float32, f"{what}: p32")
+    if p16 is not None:
+        _need(p16, torch.bfloat16, f"{what}: p16")
+    if not g.is_cuda or not g.is_contiguous():
+        raise ValueError(f"{what}: g must be a contiguous CUDA tensor")
+    g_bf16 = _is_bf16(g, f"{what}: g")
+    n = p32.numel()
+    for name, t in [("p16", p16), ("g", g)] + list(state.items()):
+        if t is None:
+            continue
+        if name not in ("p16", "g"):
+            _need(t, torch.float32, f"{what}: {name}")
+        if t.numel() != n:
+            raise ValueError(f"{what}: {name} has {t.numel()} elements, p32 has {n}")
+    for name, t in [("p32", p32), ("p16", p16), ("g", g)] + list(state.items()):
+        if t is not None and t.data_ptr() % 16:
+            raise ValueError(f"{what}: {name} must start on a 16-byte boundary")
+    return g_bf16
+
+
+def _clip_args(clip_ss: Optional[torch.Tensor], max_norm: Optional[float]):
+    if clip_ss is None:
+        return None, 0.0
+    _need(clip_ss, torch.float32, "clip_ss")
+    if max_norm is None:
+        raise ValueError("clip_ss needs max_norm")
+    return clip_ss.data_ptr(), float(max_norm)
+
+
+def lion(p32, p16, g, m, lr: float, b_sign: float, b_mom: float, decay: float = 1.0, gscale: float = 1.0,
+         clip_ss: Optional[torch.Tensor] = None, max_norm: Optional[float] = None,
+         ema: Optional[torch.Tensor] = None, ema_decay: float = 0.0, ema_mode: int = 0) -> None:
+    """Fused Lion update in place (b200_lion).  clip_ss: device fp32 sum of squares of g's range (sumsq) to clip
+    by global norm against max_norm; ema_mode 0 none, 1 ema := p_new, 2 ema = d*ema + (1-d)*p_new."""
+    if ema_mode and ema is None:
+        raise ValueError("lion: ema_mode needs an ema buffer")
+    g_bf16 = _check_update_operands("lion", p32, p16, g, {"m": m, "ema": ema})
+    ss, mn = _clip_args(clip_ss, max_norm)
+    check(lib().b200_lion(p32.data_ptr(), _ptr(p16), g.data_ptr(), g_bf16, m.data_ptr(), _ptr(ema), p32.numel(),
+                          float(lr), float(b_sign), float(b_mom), float(decay), float(gscale), ss, mn,
+                          float(ema_decay), int(ema_mode), _stream()), "b200_lion")
+
+
+def sgd(p32, p16, g, buf: Optional[torch.Tensor], lr: float, mu: float = 0.0, dampening: float = 0.0,
+        nesterov: bool = False, coupled_wd: float = 0.0, gscale: float = 1.0,
+        clip_ss: Optional[torch.Tensor] = None, max_norm: Optional[float] = None,
+        ema: Optional[torch.Tensor] = None, ema_decay: float = 0.0, ema_mode: int = 0) -> None:
+    """Fused SGD update in place (b200_sgd): buf None is plain mlx SGD (p -= lr*g); otherwise SGDEnhanced's
+    momentum with coupled weight decay coupled_wd = lr*wd.  Clip and EMA arguments as in lion()."""
+    if ema_mode and ema is None:
+        raise ValueError("sgd: ema_mode needs an ema buffer")
+    g_bf16 = _check_update_operands("sgd", p32, p16, g, {"buf": buf, "ema": ema})
+    ss, mn = _clip_args(clip_ss, max_norm)
+    check(lib().b200_sgd(p32.data_ptr(), _ptr(p16), g.data_ptr(), g_bf16, _ptr(buf), _ptr(ema), p32.numel(),
+                         float(lr), float(mu), float(dampening), int(nesterov), float(coupled_wd), float(gscale),
+                         ss, mn, float(ema_decay), int(ema_mode), _stream()), "b200_sgd")
+
+
 def adam_direction(d, g, m, v, lr, b1, b2, eps, bc1=1.0, bc2=1.0, gscale=1.0) -> None:
     check(lib().b200_adam_direction(d.data_ptr(), g.data_ptr(), _is_bf16(g, "g"), m.data_ptr(),
                                     v.data_ptr(), d.numel(), float(lr), float(b1), float(b2),

@@ -1,23 +1,24 @@
 """HybridOptimizer (optimizers/hybrid_optimizer.py:78-114): 2-D parameters -> matrix optimizer
-(Muon), everything else -> non-matrix optimizer (AdamW).  The reference's factory recursion for
+(Muon), everything else -> non-matrix optimizer (AdamW, Lion, SGD or SGDEnhanced: anything with AdamW's
+`init_range` / `update_range` surface).  The reference's factory recursion for
 `optimizer: hybrid` crashes (SURVEY D12); the routing it intended is exactly Muon's
 `alternate_optimizer` hook, so this class is a thin composition.
 
-Checkpointing: `state_dict()` holds both sub-optimizers' tensors plus `alt_count` (the AdamW's own
-step counter drives its schedule and bias correction); `count` is settable so the trainer's resume
-path (`optimizer.count = saved`) restores the matrix optimizer's counter."""
+Checkpointing: `state_dict()` holds both sub-optimizers' tensors plus `alt_count` (the non-matrix
+optimizer's own step counter drives its schedule, bias correction and EMA initialisation); `count` is
+settable so the trainer's resume path (`optimizer.count = saved`) restores the matrix optimizer's counter."""
 from __future__ import annotations
 
 import torch
 
-from .adamw import AdamW
 from .muon import Muon
 
 _FORWARDED = ("grad_scale", "use_accumulated", "shard_ns")
 
 
 class HybridOptimizer:
-    def __init__(self, learning_rate=None, matrix_optimizer: Muon = None, non_matrix_optimizer: AdamW = None):
+    def __init__(self, learning_rate=None, matrix_optimizer: Muon = None, non_matrix_optimizer=None):
+        """non_matrix_optimizer: AdamW-like (AdamW, Lion, SGD, SGDEnhanced)."""
         if matrix_optimizer is None or non_matrix_optimizer is None:
             raise ValueError("HybridOptimizer needs a matrix_optimizer and a non_matrix_optimizer")
         if not isinstance(matrix_optimizer, Muon):
