@@ -280,6 +280,13 @@ __device__ __forceinline__ void tma_reduce_add_4d(uint32_t smem_src, const CUten
       ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// global[box at {c0, c1, c2}] = shared tile, tracked by the issuing thread's bulk groups.  Parts of the box outside
+// the tensor are not written.  Generic-proxy writes of the tile must be made visible first (fence_proxy_async_smem).
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, uint32_t smem_src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // wait until at most N committed bulk groups still read their shared-memory source
 template <int N>

@@ -10,10 +10,14 @@
 //                   named barriers orders their mainloops, so one warpgroup's epilogue runs while the other
 //                   keeps the tensor cores busy.  A stage is handed back once the wgmma batch that read it has
 //                   retired, so one batch is always in flight behind the next TMA wait.
-//   epilogue        bf16 outputs go through a 32 KB shared-memory tile per consumer (stmatrix in, 16-byte
-//                   coalesced rows out): alpha/beta/C (C read as 16-byte rows), the symmetric-output mirror
-//                   (stmatrix.trans), peer stores and the two fused MLP epilogues.  fp32 outputs and split-K
-//                   partials are stored straight from the accumulators.
+//   epilogue        bf16 outputs go through a 32 KB shared-memory tile per consumer, laid out as TMA boxes: the
+//                   accumulators go in with stmatrix and leave as bulk tensor stores issued by one thread, which
+//                   drain while the warpgroup runs its next mainloop.  Epilogue inputs (C for beta != 0, the saved
+//                   GLU activations of the adjoint) are loaded into the tile by the producer right after the
+//                   tile's k-blocks, so they land while the tile's own MMAs run.  This covers alpha/beta/C, the
+//                   symmetric-output mirror (stmatrix.trans), and the two fused MLP epilogues; peer copies are
+//                   written from the tile as 16-byte rows.  fp32 outputs and split-K partials are stored straight
+//                   from the accumulators.
 // Operand layouts (K-major or MN-major for A and for B) are per-problem run-time flags: they select the TMA
 // box shape and the transpose bits of the wgmma instruction.  Grouped launches are how the Newton-Schulz chain
 // runs each stage over all shape groups at once.
@@ -31,6 +35,8 @@ constexpr int A_BYTES = BM * BK * 2;  // 16 KB
 constexpr int B_BYTES = BN * BK * 2;  // 16 KB
 constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr int OUT_BYTES = BM * BN * 2;  // bf16 staging tile of one consumer warpgroup
+constexpr int HALF_BYTES = BM * 128;    // one [128 rows x 64 columns] half of it
+constexpr int BOX_BYTES = 64 * 128;     // one [64 x 64] TMA box of the epilogue tensor maps
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * OUT_BYTES + 1024 + 256;
 static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget of one block");
 constexpr int MAX_PROBLEMS = 6;
@@ -65,8 +71,11 @@ struct Args {
   Problem p[MAX_PROBLEMS];
   CUtensorMap tmA[MAX_PROBLEMS];
   CUtensorMap tmB[MAX_PROBLEMS];
+  CUtensorMap tmD[MAX_PROBLEMS];  // bf16 D (plain), gu (epi 1) or dgu (epi 2); unset for fp32 / split-K outputs
+  CUtensorMap tmE[MAX_PROBLEMS];  // C (plain, beta != 0), y (epi 1) or the saved gu (epi 2)
 };
-static_assert(sizeof(Args) <= 4096, "kernel parameter block");
+// sm_90 with CUDA >= 12.1 takes up to 32764 bytes of kernel parameters (4096 before)
+static_assert(sizeof(Args) <= 32764, "kernel parameter block");
 
 __device__ __forceinline__ void tile_coords(const Problem& p, int r, int& mi, int& ni) {
   if (p.symmetric) {  // upper triangle, row by row
@@ -165,9 +174,13 @@ __device__ __forceinline__ void mainloop(float* acc, uint32_t sbase, uint32_t fu
   if (prev >= 0 && leader) mbar_arrive(empty0 + 8 * prev);
 }
 
-// Staging tile: 128 rows of 256 B (16 chunks of 8 bf16); chunk k of row r sits at chunk k ^ (r & 7), so the
-// eight rows of an 8x8 stmatrix / ldmatrix and the eight chunks of a 128-byte row hit distinct banks.
-__device__ __forceinline__ uint32_t stage_off(int row, int chunk) { return row * 256 + ((chunk ^ (row & 7)) << 4); }
+// Staging tile: two [128 rows x 64 columns] halves of 128-byte rows in the TMA SWIZZLE_128B pattern (16-byte chunk c
+// of row r at c ^ (r & 7)), so the epilogue tensor maps load into it and store from it directly, and the eight rows of
+// an 8x8 stmatrix / ldmatrix hit distinct banks.  `chunk` in [0, 16) counts 8-column groups across both halves; the
+// [64 x 64] box (column half h, row half v) starts at h * HALF_BYTES + v * BOX_BYTES.
+__device__ __forceinline__ uint32_t stage_off(int row, int chunk) {
+  return (chunk >> 3) * HALF_BYTES + row * 128 + (((chunk & 7) ^ (row & 7)) << 4);
+}
 
 // Row addresses of the x4 matrix group (h = 0/1 row halves of 8, column groups j0, j0 + 1) of warp `warp`
 // at tile row offset `row0`; lane 8i + rr addresses row rr of matrix i.
@@ -181,18 +194,64 @@ __device__ __forceinline__ uint32_t frag_addr_trans(uint32_t stg, int row0, int 
   return stg + stage_off(8 * (j0 + (mi >> 1)) + rr, (row0 >> 3) + 2 * warp + (mi & 1));
 }
 
+// Whether a problem's epilogue reads an input into the staging tile (C of a bf16 output, the saved gu of epi 2).
+__device__ __forceinline__ bool epi_input(const Problem& p) { return p.epi == 2 || (p.C != nullptr && !p.out_f32); }
+
+// The whole [128 x 128] tile at column col0, row row0 of batch b as four 64 x 64 boxes (loads complete on `bar`).
+__device__ __forceinline__ void tile_load(const CUtensorMap* m, uint32_t stg, uint32_t bar, int col0, int row0, int b) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int v = 0; v < 2; ++v) tma_load_3d(stg + h * HALF_BYTES + v * BOX_BYTES, m, bar, col0 + 64 * h, row0 + 64 * v, b);
+}
+__device__ __forceinline__ void tile_store(const CUtensorMap* m, uint32_t stg, int col0, int row0, int b) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int v = 0; v < 2; ++v) tma_store_3d(m, stg + h * HALF_BYTES + v * BOX_BYTES, col0 + 64 * h, row0 + 64 * v, b);
+}
+// Epi 2's half tile: 128 columns from col0 of 64 rows from row0, g in staging rows [0, 64) and u in [64, 128); the
+// {I, 2, M} view of gu / dgu clips at column I, so a box never reaches from g into u.
+__device__ __forceinline__ void glu_half_load(const CUtensorMap* m, uint32_t stg, uint32_t bar, int col0, int row0) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int gu = 0; gu < 2; ++gu) tma_load_3d(stg + h * HALF_BYTES + gu * BOX_BYTES, m, bar, col0 + 64 * h, gu, row0);
+}
+__device__ __forceinline__ void glu_half_store(const CUtensorMap* m, uint32_t stg, int col0, int row0) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int gu = 0; gu < 2; ++gu) tma_store_3d(m, stg + h * HALF_BYTES + gu * BOX_BYTES, col0 + 64 * h, gu, row0);
+}
+
+// Closes a bulk group of the leader's stores.  `drain` after the warpgroup's last tile: the CTA's shared memory must
+// outlive the stores reading it.
+__device__ __forceinline__ void commit_stores(bool drain) {
+  bulk_commit();
+  if (drain) bulk_wait<0>();
+}
+
 __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ Args g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sbase = smem_u32(smem);
   const uint32_t full0 = sbase + STAGES * STAGE_BYTES + 2 * OUT_BYTES;
   const uint32_t empty0 = full0 + STAGES * 8;
+  // per consumer c: epi_full0 + 8c = its staging tile holds the epilogue input, epi_empty0 + 8c = the tile may be
+  // refilled (the consumer's earlier stores have read it)
+  const uint32_t epi_full0 = empty0 + STAGES * 8;
+  const uint32_t epi_empty0 = epi_full0 + 16;
   const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1);
       mbar_init(empty0 + 8 * s, 1);  // one arrival by the consumer warpgroup that read the stage
+    }
+    for (int c = 0; c < 2; ++c) {
+      mbar_init(epi_full0 + 8 * c, 1);
+      mbar_init(epi_empty0 + 8 * c, 1);
     }
     fence_mbar_init();
   }
@@ -206,8 +265,8 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
         tma_prefetch_desc(&g.tmB[i]);
       }
       int slot = 0;
-      uint32_t phase = 0;
-      for (int w = blockIdx.x; w < g.total_work; w += gridDim.x) {
+      uint32_t phase = 0, epi_phase = 0;  // epi_phase bit c: parity of consumer c's next epi_empty completion
+      for (int w = blockIdx.x, t = 0; w < g.total_work; w += gridDim.x, ++t) {
         const Item it = decode(g, w);
         const Problem& p = g.p[it.pi];
         const CUtensorMap* tmA = &g.tmA[it.pi];
@@ -239,6 +298,15 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
             phase ^= 1u;
           }
         }
+        if (epi_input(p)) {  // into the owning consumer's staging tile, once its previous stores have read it
+          const int c = t & 1;
+          mbar_wait(epi_empty0 + 8 * c, (epi_phase >> c) & 1u);
+          epi_phase ^= 1u << c;
+          const uint32_t stg = sbase + STAGES * STAGE_BYTES + c * OUT_BYTES, bar = epi_full0 + 8 * c;
+          mbar_arrive_expect_tx(bar, OUT_BYTES);
+          if (p.epi == 2) glu_half_load(&g.tmE[it.pi], stg, bar, ni * BN, mi * BM);  // first 64-row half
+          else tile_load(&g.tmE[it.pi], stg, bar, ni * BN, mi * BM, b);
+        }
       }
     }
     return;
@@ -249,8 +317,11 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
   const int tid = threadIdx.x & 127, lane = threadIdx.x & 31, warp = tid >> 5;
   const uint32_t stg = sbase + STAGES * STAGE_BYTES + c * OUT_BYTES;
   const uint32_t bar_wg = BAR_WG + c;
+  const uint32_t epi_full = epi_full0 + 8 * c;
+  // thread 0 of the warpgroup hands ring stages back and issues (and so owns) the warpgroup's bulk stores
+  const bool leader = tid == 0;
   int slot = 0;
-  uint32_t phase = 0;
+  uint32_t phase = 0, epi_phase = 0;
   for (int w = blockIdx.x, t = 0; w < g.total_work; w += gridDim.x, ++t) {
     if ((t & 1) != c) {  // the other warpgroup's tile: step the ring past its k-blocks
       const int n = slot + item_kbs(g, w);
@@ -261,13 +332,17 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
     const Item it = decode(g, w);
     const Problem& p = g.p[it.pi];
     const int mi = it.mi, ni = it.ni, b = it.b;
+    const bool last = w + 2 * (int)gridDim.x >= g.total_work;  // this warpgroup's last tile
 
     float acc[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     if (t > 0) named_bar_sync(BAR_ORDER + c, 256);  // the other warpgroup's mainloop is done
+    if (epi_input(p) && leader) {  // every thread is past the last tile's epilogue: free the staging tile
+      bulk_wait_read<0>();
+      mbar_arrive(epi_empty0 + 8 * c);
+    }
     const int n_kb = max(it.kb_end - it.kb_begin, 0);
-    const bool leader = tid == 0;
     if (p.a_mn) {
       if (p.b_mn) mainloop<1, 1>(acc, sbase, full0, empty0, n_kb, slot, phase, leader);
       else mainloop<1, 0>(acc, sbase, full0, empty0, n_kb, slot, phase, leader);
@@ -321,10 +396,17 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
             *reinterpret_cast<float2*>(Db + (long long)row * ld + col) = make_float2(v0, v1);
           }
         }
+      if (last) bulk_wait<0>();  // stores of an earlier bf16 tile of a grouped launch
       continue;
     }
 
-    named_bar_sync(bar_wg, 128);  // this warpgroup's previous tile has left the staging buffer
+    const CUtensorMap* tmD = &g.tmD[it.pi];
+    const CUtensorMap* tmE = &g.tmE[it.pi];
+    const bool has_input = epi_input(p);
+    if (!has_input) {  // this warpgroup's previous stores have left the staging tile
+      if (leader) bulk_wait_read<0>();
+      named_bar_sync(bar_wg, 128);
+    }
 
     if (p.epi == 1) {  // acc columns [0, 64) = gate, [64, 128) = up of the same 64 output columns
 #pragma unroll
@@ -335,15 +417,16 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
           stmatrix_x4(frag_addr(stg, 64 * hm, warp, j, lane), pack_bf16x2(a[0], a[1]), pack_bf16x2(a[2], a[3]),
                       pack_bf16x2(a[4], a[5]), pack_bf16x2(a[6], a[7]));
         }
+      fence_proxy_async_smem();
       named_bar_sync(bar_wg, 128);
-      __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.D);
-#pragma unroll 4
-      for (int i = 0; i < 16; ++i) {  // chunk k < 8: gate columns, k >= 8: the up columns I later
-        const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
-        const int row = mi * BM + r;
-        if (row < p.M)
-          stg128(gu + (long long)row * p.ldd + (k >= 8 ? p.glu_I : 0) + ni * 64 + 8 * (k & 7),
-                 lds128(stg + stage_off(r, k)));
+      if (leader) {  // staging half 0 = gate columns, half 1 = the up columns I later
+#pragma unroll
+        for (int gu = 0; gu < 2; ++gu) {
+          tma_store_3d(tmD, stg + gu * HALF_BYTES, ni * 64, gu, mi * BM);
+          tma_store_3d(tmD, stg + gu * HALF_BYTES + BOX_BYTES, ni * 64, gu, mi * BM + 64);
+          commit_stores(last);
+        }
+        bulk_wait_read<1>();  // the gate half has been read: y goes there
       }
       named_bar_sync(bar_wg, 128);
 #pragma unroll
@@ -358,32 +441,26 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
             yv[q] = pack_bf16x2(g[2 * q] * fast_sigmoid(u[2 * q]) * 2.0f, g[2 * q + 1] * fast_sigmoid(u[2 * q + 1]) * 2.0f);
           stmatrix_x4(frag_addr(stg, 64 * hm, warp, j, lane), yv[0], yv[1], yv[2], yv[3]);
         }
+      fence_proxy_async_smem();
       named_bar_sync(bar_wg, 128);
-      __nv_bfloat16* y = reinterpret_cast<__nv_bfloat16*>(p.aux);
-#pragma unroll 4
-      for (int i = 0; i < 8; ++i) {
-        const int idx = i * 128 + tid, r = idx >> 3, k = idx & 7;
-        const int row = mi * BM + r;
-        if (row < p.M) stg128(y + (long long)row * p.ld_aux + ni * 64 + 8 * k, lds128(stg + stage_off(r, k)));
+      if (leader) {
+        tma_store_3d(tmE, stg, ni * 64, mi * BM, 0);
+        tma_store_3d(tmE, stg + BOX_BYTES, ni * 64, mi * BM + 64, 0);
+        commit_stores(last);
       }
       continue;
     }
 
     if (p.epi == 2) {  // acc = d = dy Wd; dg = d s 2, du = d g s (1 - s) 2 with g, u from the saved gu
-      const __nv_bfloat16* gu = reinterpret_cast<const __nv_bfloat16*>(p.aux);
-      __nv_bfloat16* dgu = reinterpret_cast<__nv_bfloat16*>(p.D);
 #pragma unroll
       for (int hm = 0; hm < 2; ++hm) {  // staging rows [0, 64): g, [64, 128): u of tile rows [64 hm, 64 hm + 64)
-        if (hm) named_bar_sync(bar_wg, 128);
-#pragma unroll 2
-        for (int i = 0; i < 16; ++i) {
-          const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
-          const int row = mi * BM + 64 * hm + (r & 63), col = ni * BN + 8 * k;
-          uint4 v = make_uint4(0, 0, 0, 0);
-          if (row < p.M && col < p.glu_I) v = ldg128(gu + (long long)row * p.ld_aux + (r >= 64 ? p.glu_I : 0) + col);
-          sts128(stg + stage_off(r, k), v);
+        if (hm && leader) {  // the producer loaded the first half; load the second once its stores have read the tile
+          bulk_wait_read<0>();
+          mbar_arrive_expect_tx(epi_full, OUT_BYTES);
+          glu_half_load(tmE, stg, epi_full, ni * BN, mi * BM + 64);
         }
-        named_bar_sync(bar_wg, 128);
+        mbar_wait_outlined(epi_full, epi_phase);
+        epi_phase ^= 1u;
 #pragma unroll
         for (int j = 0; j < 16; j += 2) {  // each warp reads and rewrites only its own 16 rows: in place
           const uint32_t ga = frag_addr(stg, 0, warp, j, lane), ua = frag_addr(stg, 64, warp, j, lane);
@@ -403,13 +480,11 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
           stmatrix_x4(ga, dg[0], dg[1], dg[2], dg[3]);
           stmatrix_x4(ua, du[0], du[1], du[2], du[3]);
         }
+        fence_proxy_async_smem();
         named_bar_sync(bar_wg, 128);
-#pragma unroll 1
-        for (int i = 0; i < 16; ++i) {
-          const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
-          const int row = mi * BM + 64 * hm + (r & 63), col = ni * BN + 8 * k;
-          if (row < p.M && col < p.glu_I)
-            stg128(dgu + (long long)row * p.ldd + (r >= 64 ? p.glu_I : 0) + col, lds128(stg + stage_off(r, k)));
+        if (leader) {
+          glu_half_store(tmD, stg, ni * BN, mi * BM + 64 * hm);
+          commit_stores(last);
         }
       }
       continue;
@@ -418,19 +493,9 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
     // ---- plain bf16: D = alpha acc + beta C, optional mirror and peer copies ----
     const float alpha = p.alpha * (p.alpha_vec ? p.alpha_vec[b] : 1.0f);
     const float beta = p.beta * (p.beta_vec ? p.beta_vec[b] : 1.0f);
-    __nv_bfloat16* Db = reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)b * p.strideD;
-    const __nv_bfloat16* Cb =
-        p.C ? reinterpret_cast<const __nv_bfloat16*>(p.C) + (long long)b * p.strideC : nullptr;
-    if (Cb) {
-#pragma unroll 4
-      for (int i = 0; i < 16; ++i) {
-        const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
-        const int row = mi * BM + r, col = ni * BN + 8 * k;
-        uint4 v = make_uint4(0, 0, 0, 0);
-        if (row < p.M && col < p.n_store) v = ldg128(Cb + (long long)row * p.ldc + col);
-        sts128(stg + stage_off(r, k), v);
-      }
-      named_bar_sync(bar_wg, 128);
+    if (has_input) {  // C, loaded by the producer under this tile's MMAs
+      mbar_wait_outlined(epi_full, epi_phase);
+      epi_phase ^= 1u;
     }
     uint32_t dv[2][8][4];  // the tile as packed bf16 pairs, kept for the mirror
 #pragma unroll
@@ -439,12 +504,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
       for (int jp = 0; jp < 8; ++jp) {  // each warp reads and rewrites only its own 16 rows: in place
         const uint32_t fa = frag_addr(stg, 64 * hm, warp, 2 * jp, lane);
         uint32_t cq4[4];
-        if (Cb) ldmatrix_x4(fa, cq4);
+        if (has_input) ldmatrix_x4(fa, cq4);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const float* a = acc + 64 * hm + 4 * (2 * jp + (q >> 1)) + 2 * (q & 1);
           float v0 = alpha * a[0], v1 = alpha * a[1];
-          if (Cb) {
+          if (has_input) {
             const float2 cv = unpack_bf16x2(cq4[q]);
             v0 += beta * cv.x;
             v1 += beta * cv.y;
@@ -454,19 +519,25 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
         __syncwarp();
         stmatrix_x4(fa, dv[hm][jp][0], dv[hm][jp][1], dv[hm][jp][2], dv[hm][jp][3]);
       }
+    fence_proxy_async_smem();
     named_bar_sync(bar_wg, 128);
+    if (leader) {
+      tile_store(tmD, stg, ni * BN, mi * BM, b);
+      commit_stores(last);
+    }
+    if (p.n_peers) {  // peer-mapped copies of D, as 16-byte rows
 #pragma unroll 4
-    for (int i = 0; i < 16; ++i) {
-      const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
-      const int row = mi * BM + r, col = ni * BN + 8 * k;
-      if (row >= p.M || col >= p.n_store) continue;
-      const uint4 v = lds128(stg + stage_off(r, k));
-      const long long od = (long long)row * p.ldd + col;
-      stg128(Db + od, v);
-      for (int pe = 0; pe < p.n_peers; ++pe)
-        stg128(reinterpret_cast<__nv_bfloat16*>(p.peer_D[pe]) + (long long)b * p.strideD + od, v);
+      for (int i = 0; i < 16; ++i) {
+        const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
+        const int row = mi * BM + r, col = ni * BN + 8 * k;
+        if (row >= p.M || col >= p.n_store) continue;
+        const uint4 v = lds128(stg + stage_off(r, k));
+        const long long od = (long long)b * p.strideD + (long long)row * p.ldd + col;
+        for (int pe = 0; pe < p.n_peers; ++pe) stg128(reinterpret_cast<__nv_bfloat16*>(p.peer_D[pe]) + od, v);
+      }
     }
     if (p.symmetric && mi != ni) {  // D == D^T: block (ni, mi) is this tile transposed
+      if (leader) bulk_wait_read<0>();
       named_bar_sync(bar_wg, 128);
 #pragma unroll
       for (int hm = 0; hm < 2; ++hm)
@@ -474,15 +545,13 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
         for (int jp = 0; jp < 8; ++jp)
           stmatrix_x4_trans(frag_addr_trans(stg, 64 * hm, warp, 2 * jp, lane), dv[hm][jp][0], dv[hm][jp][1],
                             dv[hm][jp][2], dv[hm][jp][3]);
+      fence_proxy_async_smem();
       named_bar_sync(bar_wg, 128);
-#pragma unroll 4
-      for (int i = 0; i < 16; ++i) {
-        const int idx = i * 128 + tid, r = idx >> 4, k = idx & 15;
-        // row: a column of D, col: rows of D.  Both entries reject symmetric output unless M == N is a
-        // multiple of 8, so every 8-row piece of the mirror is whole.
-        const int row = ni * BN + r, col = mi * BM + 8 * k;
-        if (row >= p.N || col >= p.M) continue;
-        stg128(Db + (long long)row * p.ldd + col, lds128(stg + stage_off(r, k)));
+      // staging row r = column ni BN + r of D, staging column = row mi BM + col.  Both entries reject symmetric
+      // output unless M == N is a multiple of 8, so the map's bounds clip the mirror exactly.
+      if (leader) {
+        tile_store(tmD, stg, mi * BM, ni * BN, b);
+        commit_stores(last);
       }
     }
   }
@@ -534,6 +603,33 @@ int operand_map(CUtensorMap* m, const void* base, bool mn, int rows, int K, int 
   const uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)(batch > 1 ? stride : (long long)dims[1] * ld) * 2};
   const uint32_t box[3] = {64, (uint32_t)(mn ? 64 : box_rows), 1};
   return make_tensor_map(m, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 3, dims, strides, box, true);
+}
+
+// TMA map of a bf16 epilogue tile (D, C, y): dims {cols, rows, batch}, 128B-swizzled 64 x 64 boxes, so each half
+// of the staging tile is two boxes.  `cols` is the stored width (N rounded up to 8 for D): the padded columns of a
+// ragged output are written, and rows >= `rows` are clipped.
+int tile_map(CUtensorMap* m, const void* base, int cols, int rows, int batch, long long ld, long long stride) {
+  const uint64_t dims[3] = {(uint64_t)cols, (uint64_t)rows, (uint64_t)batch};
+  const uint64_t strides[2] = {(uint64_t)ld * 2, (uint64_t)(batch > 1 ? stride : (long long)rows * ld) * 2};
+  const uint32_t box[3] = {64, 64, 1};
+  return make_tensor_map(m, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 3, dims, strides, box, true);
+}
+// TMA map of the GLU activations gu / dgu [M, 2I] (row pitch ld) viewed as {I, 2 (gate, up), M}, boxes of 64 columns
+// by 64 rows: column I clips a box instead of running into the other half.
+int glu_map(CUtensorMap* m, const void* base, int I, int M, long long ld) {
+  const uint64_t dims[3] = {(uint64_t)I, 2, (uint64_t)M};
+  const uint64_t strides[2] = {(uint64_t)I * 2, (uint64_t)ld * 2};
+  const uint32_t box[3] = {64, 1, 64};
+  return make_tensor_map(m, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 3, dims, strides, box, true);
+}
+
+// The bf16 epilogue's maps of a plain problem: D and, when beta != 0, C.
+int plain_epi_maps(Args& a, int i) {
+  const Problem& q = a.p[i];
+  if (q.out_f32 || q.k_splits > 1) return B200_OK;
+  int rc = tile_map(&a.tmD[i], q.D, q.n_store, q.M, q.batch, q.ldd, q.strideD);
+  if (rc == B200_OK && q.C) rc = tile_map(&a.tmE[i], q.C, q.n_store, q.M, q.batch, q.ldc, q.strideC);
+  return rc;
 }
 
 Problem base_problem(int M, int N, int K, int batch, int tiles_n, int epi) {
@@ -626,6 +722,7 @@ int gemm_bf16_ex(bool a_mn, bool b_mn, int M, int N, int K, int batch, const voi
   q.ws = splitk_ws;
   q.n_peers = n_peers;
   for (int i = 0; i < n_peers; ++i) q.peer_D[i] = const_cast<void*>(peer_D[i]);
+  if ((rc = plain_epi_maps(a, 0))) return rc;
   return launch(a, 1, stream);
 }
 
@@ -679,6 +776,8 @@ int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K,
   q.glu_I = I;
   q.aux = y;
   q.ld_aux = I;
+  if ((rc = glu_map(&a.tmD[0], gu, I, M, q.ldd))) return rc;
+  if ((rc = tile_map(&a.tmE[0], y, I, M, 1, I, 0))) return rc;
   return launch(a, 1, stream);
 }
 
@@ -699,6 +798,8 @@ int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int 
   q.glu_I = I;
   q.aux = const_cast<void*>(gu);
   q.ld_aux = 2LL * I;
+  if ((rc = glu_map(&a.tmD[0], dgu, I, M, q.ldd))) return rc;
+  if ((rc = glu_map(&a.tmE[0], gu, I, M, q.ld_aux))) return rc;
   return launch(a, 1, stream);
 }
 
@@ -757,6 +858,7 @@ int gemm_grouped(const GroupedGemm* probs, int n, cudaStream_t stream) {
     q.ws = h.splitk_ws;
     q.n_peers = h.n_peers;
     for (int i = 0; i < h.n_peers; ++i) q.peer_D[i] = const_cast<void*>(h.peer_D[i]);
+    if ((rc = plain_epi_maps(a, oi))) return rc;
   }
   return launch(a, n, stream);
 }
