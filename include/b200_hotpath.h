@@ -336,6 +336,28 @@ int b200_attn_bwd_strided(const void* q, const void* k, const void* v, const voi
                           int D, float scale, int causal, int dkv_row_heads, void* workspace,
                           size_t workspace_bytes, void* stream);
 
+/* ---- generation: decode attention over a KV cache (arch/flash_attention.py:97-156, last query row) ------------
+ * One new query per sequence against its cached keys, causal by construction (every cached key precedes it):
+ *   q, o: [B,H,D]; k_cache, v_cache: [B,s_max,Hk,D] (the training layout [B,S,Hk,D]); q head h reads kv head
+ *   h/(H/Hk).  All bf16 (is_bf16=1) or all f32 (is_bf16=0); softmax and accumulation in f32 either way.
+ *   lens: device int32 [B], keys valid per row including the new token, 1 <= lens[b] <= s_max; keys at or beyond
+ *   lens[b] are never read.  lse: f32 [B,H] natural-log sum-exp of the scaled scores, or NULL.
+ *   D in {16,32,64,128}, (H/Hk)*D <= 2048, s_max >= 32.
+ * Keys split into fixed 256-key chunks from position 0, each chunk's f32 partial (m, l, acc) goes to the workspace
+ * and a second pass merges them in chunk order: a row's output is bit-identical alone or in any batch.
+ * No host synchronisation; the K/V tensor maps are cached per buffer. */
+size_t b200_attn_decode_workspace_bytes(int B, int H, int s_max, int D);
+int b200_attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
+                     int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* workspace,
+                     size_t workspace_bytes, void* stream);
+/* Appends one token per row at pos = lens[b] - 1: k_cache[b,pos] = rot(k[b]), v_cache[b,pos] = v[b] (k, v:
+ * [B,Hk,D]).  With cos_t/sin_t (f32 [>= max pos + 1, D/2], ops.rope_tables) the interleaved-pair rotation of
+ * b200_rope (arch/llama_standard.py:90-131) is applied to k and, in place, to q [B,H,D], with b200_rope's exact
+ * arithmetic; with both NULL k is copied and q is untouched.  Same dtype rule as above; D % 8 == 0. */
+int b200_kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                   const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif

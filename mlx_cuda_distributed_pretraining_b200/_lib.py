@@ -71,6 +71,9 @@ SIGNATURES = {
     "b200_attn_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i,
                            _vp, _sz, _vp]),
     "b200_attn_bwd_strided": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _vp, _sz, _vp]),
+    "b200_attn_decode_workspace_bytes": (_sz, [_i, _i, _i, _i]),
+    "b200_attn_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
+    "b200_kv_append": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
 

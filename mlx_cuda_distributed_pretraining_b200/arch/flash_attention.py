@@ -82,3 +82,43 @@ class FlashAttention(nn.Module):
         ctx = self._flash_attention(q, k, v, mask)
         ctx = ctx.reshape(B, S, self.num_heads * self.head_dim)
         return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
+
+    # -- generation: the same layer against a KV cache ([B, s_max, Hk, D] K and V buffers) ----------------------
+    def _project(self, x: torch.Tensor):
+        if self.q_proj.bias is None and self.k_proj.bias is None and self.v_proj.bias is None:
+            return ops.multi_linear(x, (self.q_proj.weight, self.k_proj.weight, self.v_proj.weight))
+        return self.q_proj(x), self.k_proj(x), self.v_proj(x)
+
+    def _out(self, ctx: torch.Tensor) -> torch.Tensor:
+        return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
+
+    def forward_prefill(self, x: torch.Tensor, mask, k_cache: torch.Tensor, v_cache: torch.Tensor) -> torch.Tensor:
+        """forward(x, mask) over a right-padded prompt batch x [B, S, hidden] that also stores the (rotated) keys and
+        values in cache positions [0, S).  Attention runs through _flash_attention, so the numerics are the
+        training forward's."""
+        B, S, _ = x.shape
+        q, k, v = self._project(x)
+        q = q.reshape(B, S, self.num_heads, self.head_dim)
+        k = k.reshape(B, S, self.num_kv_heads, self.head_dim)
+        v = v.reshape(B, S, self.num_kv_heads, self.head_dim)
+        if self.rope_tables is not None:
+            cos_t, sin_t = self.rope_tables
+            q = ops.rope(q, cos_t[:S], sin_t[:S])
+            k = ops.rope(k, cos_t[:S], sin_t[:S])
+        k_cache[:, :S].copy_(k)
+        v_cache[:, :S].copy_(v)
+        ctx = self._flash_attention(q, k, v, mask)
+        return self._out(ctx.reshape(B, S, self.num_heads * self.head_dim))
+
+    def forward_decode(self, x: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
+                       workspace: torch.Tensor) -> torch.Tensor:
+        """One new token per row, x [B, hidden]: its k and v go to cache position lens[b] - 1 (rotated there when
+        RoPE is on), then its query attends over the row's first lens[b] cached keys."""
+        B = x.shape[0]
+        q, k, v = self._project(x)
+        q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
+        k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
+        v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
+        ops.kv_append(q, k, v, k_cache, v_cache, lens, self.rope_tables)
+        ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace)
+        return self._out(ctx.reshape(B, self.num_heads * self.head_dim))

@@ -102,6 +102,15 @@ class AttentionModule(nn.Module):
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
         return self.attn(x, mask=mask)
 
+    def cached(self, x: torch.Tensor, cache: "KVCache", layer: int) -> torch.Tensor:
+        """This layer's attention against the KV cache: prefill when x is [B, S, hidden], one decode step when x is
+        [B, hidden]."""
+        if self.apply_rope and self.attn.rope_tables is None:
+            self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
+        if x.dim() == 3:
+            return self.attn.forward_prefill(x, CausalMask(x.shape[1]), cache.k[layer], cache.v[layer])
+        return self.attn.forward_decode(x, cache.k[layer], cache.v[layer], cache.lens, cache.workspace)
+
 
 class TransformerBlock(nn.Module):
     def __init__(self, args: ModelArgs):
@@ -135,6 +144,49 @@ class TransformerBlock(nn.Module):
         a = self.self_attn(y, mask=mask, position_ids=position_ids)
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
         return h, self.mlp(y)
+
+    def forward_cached(self, h: torch.Tensor, pending, cache: "KVCache", layer: int):
+        """forward_fused with the attention run against the KV cache (AttentionModule.cached)."""
+        n1, n2 = self.input_layernorm, self.post_attention_layernorm
+        if pending is None:
+            y = n1(h)
+        else:
+            h, y = ops.add_rmsnorm(h, pending, n1.weight, n1.eps)
+        a = self.self_attn.cached(y, cache, layer)
+        h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
+        return h, self.mlp(y)
+
+
+class KVCache:
+    """Per-layer K and V buffers [B, s_max, Hk, D] in the model's activation dtype, and the number of valid positions
+    per row: `lens` on the device (read by the kernels) and `host_lens` (so sizing a launch never reads the device).
+    s_max is rounded up to a multiple of 256, the decode kernel's chunk."""
+
+    def __init__(self, model: "Model", batch: int, s_max: int):
+        a = model.args
+        attn = model.layers[0].self_attn
+        w = model.embed_tokens.weight
+        self.s_max = max(256, -(-s_max // 256) * 256)
+        shape = (batch, self.s_max, attn.num_kv_heads, attn.head_dim)
+        self.k = [torch.zeros(shape, device=w.device, dtype=w.dtype) for _ in range(a.num_hidden_layers)]
+        self.v = [torch.zeros(shape, device=w.device, dtype=w.dtype) for _ in range(a.num_hidden_layers)]
+        self.lens = torch.zeros(batch, device=w.device, dtype=torch.int32)
+        self.host_lens = [0] * batch
+        nbytes = ops.attention_decode_workspace_bytes(batch, attn.num_heads, self.s_max, attn.head_dim)
+        self.workspace = torch.empty(max(nbytes, 16), device=w.device, dtype=torch.uint8)
+
+    def set_lengths(self, lengths) -> None:
+        if any(n < 1 or n > self.s_max for n in lengths):
+            raise ValueError(f"lengths must lie in [1, {self.s_max}], got {list(lengths)}")
+        self.host_lens = [int(n) for n in lengths]
+        self.lens.copy_(torch.tensor(self.host_lens, dtype=torch.int32))
+
+    def advance(self) -> None:
+        """One more position per row (the token a decode step is about to append)."""
+        if max(self.host_lens) + 1 > self.s_max:
+            raise ValueError(f"KV cache full ({self.s_max} positions)")
+        self.host_lens = [n + 1 for n in self.host_lens]
+        self.lens.add_(1)
 
 
 class Model(nn.Module):
@@ -194,6 +246,42 @@ class Model(nn.Module):
         if self.logit_scale is not None:
             logits = logits * self.logit_scale
         return logits
+
+    # -- generation: prefill and decode steps against a KVCache ---------------------------------------------------
+    def _row_logits(self, h: torch.Tensor, pending: Optional[torch.Tensor]) -> torch.Tensor:
+        """Final norm and fp32 logits [B, V] of one hidden row per sequence (forward's arithmetic)."""
+        y = self.norm(h) if pending is None else ops.add_rmsnorm(h, pending, self.norm.weight, self.norm.eps)[1]
+        logits = torch.nn.functional.linear(y, self._logits_weight())[..., :self.vocab_size]
+        if self.logit_scale is not None:
+            logits = logits * self.logit_scale
+        return logits.float()
+
+    @torch.no_grad()
+    def prefill(self, tokens: torch.Tensor, lengths, cache: KVCache) -> torch.Tensor:
+        """Runs the right-padded prompts tokens [B, S] (row b valid in [0, lengths[b])) through the block stack as
+        training does, fills cache positions [0, S) and sets the cache lengths.  Returns the fp32 logits [B, V] at
+        each row's last prompt position only.  Padding is harmless: under the causal mask no valid position sees it,
+        and the decode steps never read cache positions at or past a row's length."""
+        B, S = tokens.shape
+        cache.set_lengths(lengths)
+        h = ops.embedding(tokens, self.embed_tokens.weight)
+        pending = None
+        for i, layer in enumerate(self.layers):
+            h, pending = layer.forward_cached(h, pending, cache, i)
+        rows = torch.arange(B, device=tokens.device)
+        last = torch.tensor([n - 1 for n in lengths], device=tokens.device)
+        return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])
+
+    @torch.no_grad()
+    def decode_step(self, tokens: torch.Tensor, cache: KVCache) -> torch.Tensor:
+        """Appends one token per row (tokens [B]) at position cache.host_lens[b] and returns the fp32 logits [B, V]
+        that follow it."""
+        cache.advance()
+        h = ops.embedding(tokens, self.embed_tokens.weight)
+        pending = None
+        for i, layer in enumerate(self.layers):
+            h, pending = layer.forward_cached(h, pending, cache, i)
+        return self._row_logits(h, pending)
 
     # mlx nn.Module-style accessors used by the optimizers' update(model, grads) surface
     def parameters_dict(self) -> Dict[str, torch.Tensor]:

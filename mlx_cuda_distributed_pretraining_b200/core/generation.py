@@ -1,0 +1,250 @@
+"""Text generation from a trained run (core/generation.py of the reference) on the KV-cached decode path.
+
+    python -m core.generation --run <name> --prompt "..." [--max-tokens 256 --temperature 1.0 --min-p 0.05
+                              --repetition-penalty 1.1 --repetition-context-size 20]
+                              [--top-p P --seed N --num-samples N --checkpoint step_N --runs-dir runs]
+
+The run's config.yaml (written by the trainer) rebuilds the model through Trainer(cfg, for_training=False), the
+checkpoint's weights are loaded into it, and `generate` prefills [BOS] + tokenize(prompt) once and then decodes one
+token per step against the cache (arch/llama.py: Model.prefill / Model.decode_step).
+
+Sampling follows the reference's mlx_lm_utils.make_sampler / make_logits_processors (DESIGN.md §2 records each
+decision): repetition penalty over the literal window tokens[max(0, idx - R):idx] with idx = len(tokens) - 1, then
+min-p when min_p is truthy, else top-p when top_p is truthy, else plain temperature sampling; temperature 0 is
+argmax.  The filters below are device-agnostic torch over [..., V] fp32 logits.
+"""
+from __future__ import annotations
+
+import argparse
+import random
+import sys
+import time
+from pathlib import Path
+from typing import Callable, List, Optional, Sequence
+
+import torch
+
+
+# ------------------------------------------------------------------------------------------------
+# logits processing and sampling distributions (mlx_lm_utils.py:57-142)
+# ------------------------------------------------------------------------------------------------
+def repetition_window(tokens: Sequence[int], context_size: int) -> List[int]:
+    """tokens[max(0, idx - R):idx] with idx = len(tokens) - 1: the window the reference's processor divides over
+    (it leaves out the token just fed)."""
+    idx = len(tokens) - 1
+    return list(tokens[max(0, idx - context_size):idx])
+
+
+def apply_repetition_penalty(logits: torch.Tensor, windows: Sequence[Sequence[int]], penalty: float) -> torch.Tensor:
+    """logits [B, V]: logits[b, t] / penalty once per occurrence of t in windows[b] (sign ignored, as written)."""
+    if penalty == 1.0 or not any(len(w) for w in windows):
+        return logits
+    B, V = logits.shape
+    width = max(len(w) for w in windows)
+    ids = torch.zeros((B, width), dtype=torch.int64)
+    ones = torch.zeros((B, width), dtype=logits.dtype)
+    for b, w in enumerate(windows):
+        ids[b, :len(w)] = torch.tensor(list(w), dtype=torch.int64)
+        ones[b, :len(w)] = 1.0
+    counts = torch.zeros_like(logits).scatter_add_(1, ids.to(logits.device), ones.to(logits.device))
+    return logits / torch.pow(torch.full_like(logits, float(penalty)), counts)
+
+
+def _sorted_desc(x: torch.Tensor) -> torch.Tensor:
+    """argsort(-x) along the last axis, ties in index order (stable)."""
+    return torch.sort(x, dim=-1, descending=True, stable=True).indices
+
+
+def _unsort(sorted_vals: torch.Tensor, order: torch.Tensor) -> torch.Tensor:
+    return torch.zeros_like(sorted_vals).scatter_(-1, order, sorted_vals)
+
+
+def min_p_distribution(logits: torch.Tensor, temp: float, min_p: float) -> torch.Tensor:
+    """make_sampler's min-p branch (mlx_lm_utils.py:69-84) as a distribution over the vocabulary: softmax(l / temp),
+    keep the sorted probabilities p >= min_p * p_max (always the top one), renormalise."""
+    probs = torch.softmax(logits * (1 / temp), dim=-1)
+    order = _sorted_desc(logits)
+    sp = torch.gather(probs, -1, order)
+    remove = sp < min_p * sp[..., :1]
+    remove[..., 0] = False
+    sel = torch.where(remove, torch.zeros_like(sp), sp)
+    sel = sel / sel.sum(dim=-1, keepdim=True)
+    return _unsort(sel, order)
+
+
+def top_p_distribution(logits: torch.Tensor, temp: float, top_p: float) -> torch.Tensor:
+    """make_sampler's top-p branch (mlx_lm_utils.py:85-103): keep the sorted prefix with cumsum <= top_p (the token
+    crossing the threshold is dropped), or the top token alone when that prefix is empty; renormalise."""
+    probs = torch.softmax(logits * (1 / temp), dim=-1)
+    order = _sorted_desc(probs)
+    sp = torch.gather(probs, -1, order)
+    mask = torch.cumsum(sp, dim=-1) <= top_p
+    mask[..., 0] |= ~mask.any(dim=-1)
+    sel = torch.where(mask, sp, torch.zeros_like(sp))
+    sel = sel / sel.sum(dim=-1, keepdim=True)
+    return _unsort(sel, order)
+
+
+def temperature_distribution(logits: torch.Tensor, temp: float) -> torch.Tensor:
+    """make_sampler's plain branch (mlx_lm_utils.py:104-107): categorical(l / temp)."""
+    return torch.softmax(logits * (1 / temp), dim=-1)
+
+
+def sampling_distribution(logits: torch.Tensor, temp: float, min_p: Optional[float] = None,
+                          top_p: Optional[float] = None) -> torch.Tensor:
+    if min_p:
+        return min_p_distribution(logits, temp, min_p)
+    if top_p:
+        return top_p_distribution(logits, temp, top_p)
+    return temperature_distribution(logits, temp)
+
+
+def sample(logits: torch.Tensor, temp: float, min_p: Optional[float], top_p: Optional[float],
+           generator: Optional[torch.Generator]) -> torch.Tensor:
+    """Next tokens [B] from fp32 logits [B, V], on the logits' device.  Like the reference, the sampler sees
+    log-probabilities (logits - logsumexp); temperature 0 is argmax."""
+    logprobs = logits - torch.logsumexp(logits, dim=-1, keepdim=True)
+    if temp == 0:
+        return torch.argmax(logprobs, dim=-1)
+    probs = sampling_distribution(logprobs, temp, min_p, top_p)
+    return torch.multinomial(probs, 1, generator=generator).squeeze(-1)
+
+
+# ------------------------------------------------------------------------------------------------
+# generation
+# ------------------------------------------------------------------------------------------------
+def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature: float = 1.0,
+             min_p: Optional[float] = 0.05, top_p: Optional[float] = None, repetition_penalty: float = 1.1,
+             repetition_context_size: int = 20, eos_token: Optional[int] = None, seed: Optional[int] = None,
+             on_step: Optional[Callable[[List[int]], None]] = None) -> List[List[int]]:
+    """Generates up to max_tokens tokens for each of the ragged prompts in one batch.  A row stops at EOS, which is
+    included in its output.  Returns the generated tokens per row (prompt excluded).  Per step, the sampled tokens
+    are the one value read back from the device."""
+    from ..arch.llama import KVCache
+
+    if not prompts or any(len(p) == 0 for p in prompts):
+        raise ValueError("every prompt needs at least one token")
+    limit = model.args.max_position_embeddings
+    longest = max(len(p) for p in prompts)
+    if longest + max_tokens > limit:
+        raise ValueError(f"prompt ({longest} tokens) + max_tokens ({max_tokens}) exceeds max_position_embeddings "
+                         f"({limit}): training truncates there and the RoPE tables end there")
+    device = model.embed_tokens.weight.device
+    gen = None
+    if temperature != 0:
+        gen = torch.Generator(device=device)
+        gen.manual_seed(seed if seed is not None else time.time_ns() % (1 << 63))
+    B = len(prompts)
+    tokens = torch.zeros((B, longest), dtype=torch.int64)
+    for b, p in enumerate(prompts):
+        tokens[b, :len(p)] = torch.tensor(p, dtype=torch.int64)
+    cache = KVCache(model, B, longest + max_tokens)
+    logits = model.prefill(tokens.to(device), [len(p) for p in prompts], cache)
+    history = [list(p) for p in prompts]
+    out: List[List[int]] = [[] for _ in prompts]
+    done = [False] * B
+    for step in range(max_tokens):
+        if repetition_penalty != 1.0 and repetition_context_size > 0:
+            logits = apply_repetition_penalty(logits, [repetition_window(h, repetition_context_size) for h in history],
+                                              repetition_penalty)
+        nxt = sample(logits, temperature, min_p, top_p, gen)
+        picked = nxt.tolist()
+        for b, t in enumerate(picked):
+            if done[b]:
+                continue
+            out[b].append(t)
+            history[b].append(t)
+            if eos_token is not None and t == eos_token:
+                done[b] = True
+        if on_step is not None:
+            on_step(picked)
+        if all(done) or step + 1 == max_tokens:
+            break
+        logits = model.decode_step(nxt, cache)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# CLI (core/generation.py:10-78 of the reference)
+# ------------------------------------------------------------------------------------------------
+def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
+    ap = argparse.ArgumentParser(description="Generate text using a trained model")
+    ap.add_argument("--run", type=str, required=True, help="Name of the training run to use")
+    ap.add_argument("--prompt", type=str, required=True, help="Text prompt to start generation")
+    ap.add_argument("--max-tokens", type=int, default=256, help="Maximum number of tokens to generate")
+    ap.add_argument("--temperature", type=float, default=1.0, help="Sampling temperature (0: greedy)")
+    ap.add_argument("--min-p", type=float, default=0.05, help="Minimum probability for min-p sampling")
+    ap.add_argument("--repetition-penalty", type=float, default=1.1, help="Repetition penalty factor")
+    ap.add_argument("--repetition-context-size", type=int, default=20, help="Context size for repetition penalty")
+    ap.add_argument("--top-p", type=float, default=None, help="Nucleus threshold (used when --min-p is 0)")
+    ap.add_argument("--seed", type=int, default=None, help="Sampling seed (default: from the clock)")
+    ap.add_argument("--num-samples", type=int, default=1, help="Rows decoded as one batch")
+    ap.add_argument("--checkpoint", type=str, default=None,
+                    help="Checkpoint to load, e.g. step_1000 (default: the final checkpoint)")
+    ap.add_argument("--runs-dir", type=str, default="runs", help="Directory holding the run directories")
+    a = ap.parse_args(argv)
+    if a.num_samples < 1:
+        ap.error("--num-samples must be >= 1")
+    return a
+
+
+def resolve_checkpoint(run_dir: Path, checkpoint: Optional[str] = None) -> Path:
+    """Model weights of a run: checkpoints/<checkpoint>_model.safetensors (or the exact file name given), else
+    step_final_model.safetensors, then step_final.safetensors, as the reference looks them up."""
+    ck = Path(run_dir) / "checkpoints"
+    if checkpoint is not None:
+        for cand in (ck / f"{checkpoint}_model.safetensors", ck / checkpoint, ck / f"{checkpoint}.safetensors"):
+            if cand.is_file():
+                return cand
+        raise ValueError(f"Checkpoint {checkpoint} not found in {ck}")
+    for name in ("step_final_model.safetensors", "step_final.safetensors"):
+        if (ck / name).is_file():
+            return ck / name
+    raise ValueError(f"Final checkpoint not found for run: {Path(run_dir).name}")
+
+
+def load_run(run: str, runs_dir: str = "runs", checkpoint: Optional[str] = None):
+    """Trainer(cfg, for_training=False) of a run with the checkpoint's weights in its parameter store."""
+    from safetensors.torch import load_file
+    from .training import Config, Trainer
+
+    run_dir = Path(runs_dir) / run
+    cfg_path = run_dir / "config.yaml"
+    if not cfg_path.is_file():
+        raise ValueError(f"Config not found for run: {run} ({cfg_path})")
+    path = resolve_checkpoint(run_dir, checkpoint)
+    cfg = Config.from_yaml(str(cfg_path))
+    trainer = Trainer(cfg, for_training=False, run_root=str(Path(runs_dir)), quiet=True)
+    weights = load_file(str(path))
+    store = trainer.store
+    with torch.no_grad():
+        for name, (_, shape) in store.index.items():
+            if name not in weights:
+                raise ValueError(f"{path.name}: parameter {name} missing")
+            if tuple(weights[name].shape) != tuple(shape):
+                raise ValueError(f"{path.name}: parameter {name} has shape {tuple(weights[name].shape)}, "
+                                 f"the model expects {tuple(shape)}")
+        for name, t in weights.items():
+            if name in store.index:  # non-strict, like Trainer.load_checkpoint
+                store.view(store.master, name).copy_(t.to(trainer.device))
+        store.refresh_shadow()
+    trainer.model.eval()
+    return trainer
+
+
+def main(argv: Optional[List[str]] = None) -> None:
+    a = parse_args(argv)
+    trainer = load_run(a.run, a.runs_dir, a.checkpoint)
+    tok = trainer.tokenizer
+    prompt = [tok.BOS_TOKEN] + tok.tokenize(a.prompt)
+    seed = a.seed if a.seed is not None else random.SystemRandom().randrange(1 << 62)
+    outs = generate(trainer.model, [prompt] * a.num_samples, max_tokens=a.max_tokens, temperature=a.temperature,
+                    min_p=a.min_p, top_p=a.top_p, repetition_penalty=a.repetition_penalty,
+                    repetition_context_size=a.repetition_context_size, eos_token=tok.EOS_TOKEN, seed=seed)
+    for o in outs:
+        print(f"Greedy Output: {tok.detokenize(o)}")
+    sys.stdout.flush()
+
+
+if __name__ == "__main__":
+    main()

@@ -26,7 +26,7 @@ import os
 import random
 import sys
 import time
-from dataclasses import dataclass, field
+from dataclasses import asdict, dataclass, field
 from datetime import datetime
 from pathlib import Path
 from typing import Any, Callable, Dict, List, Optional, Tuple
@@ -712,8 +712,22 @@ class Trainer:
             tot_loss, tot_tok = v[0], v[1]
         return float((tot_loss / tot_tok).item())
 
+    def save_config(self) -> Path:
+        """Writes the effective config (CLI overrides applied) to <run_dir>/config.yaml, where the reference writes it
+        (core/training.py:1173-1176) and where `python -m core.generation --run` finds it.  A run forced onto
+        synthetic tokens records `data.input_file: synthetic` (a `synthetic:<kind>` value is kept), so that
+        Trainer(cfg, for_training=False) rebuilds the same vocabulary."""
+        d = asdict(self.config)
+        if self.synthetic and not str(d["data"]["input_file"]).startswith("synthetic"):
+            d["data"]["input_file"] = "synthetic"
+        path = self.run_dir / "config.yaml"
+        path.write_text(yaml.safe_dump(d, sort_keys=False))
+        return path
+
     # -- main loop (core/training.py:1637-1768) ---------------------------------------------------
     def train(self) -> Dict[str, Any]:
+        if self.rank == 0:
+            self.save_config()
         start_step = 0
         if self.config.resume and self.config.resume.checkpoint:
             start_step = self.load_checkpoint(self.config.resume.checkpoint, self.config.resume.reset_optimizer)

@@ -1,0 +1,457 @@
+// Decode-time attention over a KV cache, and the per-token cache append.
+//
+// attn_decode computes what FlashAttention._flash_attention (arch/flash_attention.py:97-156 of the reference) computes
+// for the LAST query row of a causal sequence: o = softmax(q K^T * scale) V over the row's lens[b] cached keys, with
+// q-head h reading kv-head h / (H/Hk).  One new query per sequence makes this memory-bound, so the kernel is built
+// around reading every K/V byte exactly once:
+//
+//   grid (chunk, kv head, batch row), 128 threads.  A CTA owns keys [256 c, min(256 (c + 1), lens[b])) of one kv head
+//   and ALL G = H/Hk query heads that share it.  Chunk boundaries depend on lens[b] alone (not on B, s_max or the SM
+//   count), and CTAs past the row's last chunk exit at once.
+//   Thread 0 streams the chunk through a 4-stage ring of 32-key K and V tiles (TMA boxes {D, 1, 32, 1} over the
+//   [B, s_max, Hk, D] cache, one mbarrier per stage).  The last tile of a chunk is anchored at its end (rows
+//   [end - 32, end)), so no key at or beyond lens[b] is ever read; the rows it re-reads from the previous chunk (or
+//   the zero rows TMA fills in below position 0) are masked out of the softmax.
+//   Per tile: scores (D/8 lanes per key, fp32 dot products, shuffle-reduced), an online softmax per query head (one
+//   warp per head, lane = key), then acc += p v with each thread owning (head, 8 columns) x (a fixed subset of keys).
+//   A chunk's fp32 partial (m, l, acc) goes to the workspace; attn_decode_combine_kernel merges a row's chunks in
+//   chunk order.  Rows with a single chunk are finished by the first kernel.
+//
+// Every reduction has a fixed order that depends only on the row's own data, so a row's output is bit-identical
+// whether it runs alone or inside any batch, and from launch to launch.
+#include "common.cuh"
+#include "host.h"
+
+namespace b200 {
+
+namespace {
+
+constexpr int DEC_CHUNK = 256;    // keys per split
+constexpr int DEC_TILE = 32;      // keys per TMA box / ring stage (= warp size: one lane per key in the softmax)
+constexpr int DEC_STAGES = 4;
+constexpr int DEC_THREADS = 128;
+constexpr int DEC_MAX_ITEMS = 2;  // (head, 8-column slice) accumulators per thread: G * D <= 2048
+constexpr float kLog2e = 1.4426950408889634f;
+
+__device__ __forceinline__ void ld8(const __nv_bfloat16* p, float* f) {
+  const uint4 a = *reinterpret_cast<const uint4*>(p);
+  const float2 v0 = unpack_bf16x2(a.x), v1 = unpack_bf16x2(a.y), v2 = unpack_bf16x2(a.z), v3 = unpack_bf16x2(a.w);
+  f[0] = v0.x; f[1] = v0.y; f[2] = v1.x; f[3] = v1.y;
+  f[4] = v2.x; f[5] = v2.y; f[6] = v3.x; f[7] = v3.y;
+}
+__device__ __forceinline__ void ld8(const float* p, float* f) {
+  const float4 a = *reinterpret_cast<const float4*>(p);
+  const float4 b = *reinterpret_cast<const float4*>(p + 4);
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w;
+  f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+__device__ __forceinline__ void st8(__nv_bfloat16* p, const float* f) {
+  uint4 o;
+  o.x = pack_bf16x2(f[0], f[1]);
+  o.y = pack_bf16x2(f[2], f[3]);
+  o.z = pack_bf16x2(f[4], f[5]);
+  o.w = pack_bf16x2(f[6], f[7]);
+  *reinterpret_cast<uint4*>(p) = o;
+}
+__device__ __forceinline__ void st8(float* p, const float* f) {
+  *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(f[4], f[5], f[6], f[7]);
+}
+
+// Shared-memory layout (offsets from a 128-byte aligned base): the K/V ring, then q [G][D] f32 (pre-scaled by
+// scale * log2 e), scores / probabilities [G][32] f32, per-head alpha, m, l, and the cross-thread reduction buffer.
+struct DecSmem {
+  int ring, q, s, ml, red, bar, total;
+  __host__ __device__ DecSmem(int D, int elem, int G) {
+    ring = 0;
+    q = ring + DEC_STAGES * 2 * DEC_TILE * D * elem;
+    s = q + G * D * 4;
+    ml = s + G * DEC_TILE * 4;
+    red = ml + ((3 * G + 3) & ~3) * 4;
+    bar = red + DEC_THREADS * 8 * 4;
+    total = bar + DEC_STAGES * 8 + 128;  // + alignment slack of the dynamic base
+  }
+};
+
+struct DecArgs {
+  const void* q;      // [B, H, D]
+  void* o;            // [B, H, D]
+  float* lse;         // [B, H] or null
+  const int* lens;    // [B]
+  float* part_acc;    // [B, H, max_chunks, D]
+  float* part_ml;     // [B, H, max_chunks, 2]
+  int H, G, s_max, max_chunks;
+  float scale_log2;   // scale * log2 e
+};
+
+template <typename T, int D>
+__global__ void __launch_bounds__(DEC_THREADS)
+attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const DecArgs p) {
+  constexpr int L = D / 8;                        // 8-column slices per row
+  constexpr int TILE_ELEMS = DEC_TILE * D;
+  constexpr int TILE_BYTES = TILE_ELEMS * (int)sizeof(T);
+  const int c = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
+  const int len = min(p.lens[b], p.s_max);
+  const int c0 = c * DEC_CHUNK;
+  if (c0 >= len) return;
+  const int end = min(len, c0 + DEC_CHUNK);
+  const int n_tiles = (end - c0 + DEC_TILE - 1) / DEC_TILE;
+  const int n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK;
+  const int G = p.G;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+  const DecSmem lay(D, (int)sizeof(T), G);
+  T* ring = reinterpret_cast<T*>(smem + lay.ring);  // stage st: K at 2 st, V at 2 st + 1 (TILE_ELEMS each)
+  float* sq = reinterpret_cast<float*>(smem + lay.q);
+  float* ss = reinterpret_cast<float*>(smem + lay.s);
+  float* salpha = reinterpret_cast<float*>(smem + lay.ml);
+  float* sm = salpha + G;
+  float* sl = sm + G;
+  float* sred = reinterpret_cast<float*>(smem + lay.red);
+  const uint32_t bar0 = smem_u32(smem + lay.bar);
+
+  auto tile_start = [&](int j) { return min(c0 + j * DEC_TILE, end - DEC_TILE); };
+  auto issue = [&](int j) {
+    const int st = j % DEC_STAGES;
+    const uint32_t bar = bar0 + 8 * st;
+    mbar_arrive_expect_tx(bar, 2 * TILE_BYTES);
+    tma_load_4d(smem_u32(ring + (2 * st) * TILE_ELEMS), &tmK, bar, 0, hk, tile_start(j), b);
+    tma_load_4d(smem_u32(ring + (2 * st + 1) * TILE_ELEMS), &tmV, bar, 0, hk, tile_start(j), b);
+  };
+
+  if (tid == 0) {
+    for (int s = 0; s < DEC_STAGES; ++s) mbar_init(bar0 + 8 * s, 1);
+    fence_mbar_init();
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+  }
+  __syncthreads();
+  if (tid == 0)
+    for (int j = 0; j < min(n_tiles, DEC_STAGES); ++j) issue(j);
+
+  // the G query heads of this kv head are contiguous in [B, H, D]
+  const T* qb = reinterpret_cast<const T*>(p.q) + ((long long)b * p.H + (long long)hk * G) * D;
+  for (int i = tid; i < G * L; i += DEC_THREADS) {
+    float f[8];
+    ld8(qb + i * 8, f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) sq[i * 8 + e] = f[e] * p.scale_log2;
+  }
+  for (int g = tid; g < G; g += DEC_THREADS) {
+    sm[g] = -INFINITY;
+    sl[g] = 0.f;
+  }
+
+  // accumulator ownership: item = (head g, slice) with g = item / L; keys my_ks, my_ks + ks_n, ... of every tile
+  const int items = G * L;
+  const int ks_n = items <= DEC_THREADS ? DEC_THREADS / items : 1;
+  int my_item[DEC_MAX_ITEMS], my_ks;
+  if (items <= DEC_THREADS) {
+    my_ks = tid / items;
+    my_item[0] = my_ks < ks_n ? tid % items : -1;
+    my_item[1] = -1;
+  } else {
+    my_ks = 0;
+    my_item[0] = tid;
+    my_item[1] = tid + DEC_THREADS < items ? tid + DEC_THREADS : -1;
+  }
+  float acc[DEC_MAX_ITEMS][8];
+#pragma unroll
+  for (int r = 0; r < DEC_MAX_ITEMS; ++r)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[r][e] = 0.f;
+  __syncthreads();
+
+  for (int j = 0; j < n_tiles; ++j) {
+    const int st = j % DEC_STAGES;
+    mbar_wait(bar0 + 8 * st, (j / DEC_STAGES) & 1);
+    const T* tK = ring + (2 * st) * TILE_ELEMS;
+    const T* tV = ring + (2 * st + 1) * TILE_ELEMS;
+    const int start = tile_start(j);
+    const int first_valid = c0 + j * DEC_TILE;  // rows of an end-anchored tile below this belong to earlier tiles
+
+    // scores: L consecutive lanes per key, 8 columns each
+    {
+      const int kl = tid % L;
+      for (int key = tid / L; key < DEC_TILE; key += DEC_THREADS / L) {
+        float kf[8];
+        ld8(tK + key * D + kl * 8, kf);
+        const bool valid = start + key >= first_valid;
+        for (int g = 0; g < G; ++g) {
+          const float4 qa = *reinterpret_cast<const float4*>(sq + g * D + kl * 8);
+          const float4 qc = *reinterpret_cast<const float4*>(sq + g * D + kl * 8 + 4);
+          float d = qa.x * kf[0];
+          d = fmaf(qa.y, kf[1], d);
+          d = fmaf(qa.z, kf[2], d);
+          d = fmaf(qa.w, kf[3], d);
+          d = fmaf(qc.x, kf[4], d);
+          d = fmaf(qc.y, kf[5], d);
+          d = fmaf(qc.z, kf[6], d);
+          d = fmaf(qc.w, kf[7], d);
+#pragma unroll
+          for (int off = L / 2; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+          if (kl == 0) ss[g * DEC_TILE + key] = valid ? d : -INFINITY;
+        }
+      }
+    }
+    __syncthreads();
+
+    // online softmax (log2 domain): one warp per head, one lane per key; every tile holds at least one valid key
+    for (int g = warp; g < G; g += DEC_THREADS / 32) {
+      const float x = ss[g * DEC_TILE + lane];
+      const float m_old = sm[g];
+      const float m_new = fmaxf(m_old, warp_max(x));
+      const float pe = exp2f(x - m_new);
+      const float sum = warp_sum(pe);
+      ss[g * DEC_TILE + lane] = pe;
+      __syncwarp();
+      if (lane == 0) {
+        const float alpha = exp2f(m_old - m_new);
+        salpha[g] = alpha;
+        sl[g] = sl[g] * alpha + sum;
+        sm[g] = m_new;
+      }
+    }
+    __syncthreads();
+
+    // acc = acc * alpha + sum over this thread's keys of p v
+#pragma unroll
+    for (int r = 0; r < DEC_MAX_ITEMS; ++r) {
+      if (my_item[r] < 0) continue;
+      const int g = my_item[r] / L, sc = my_item[r] % L;
+      const float a = salpha[g];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[r][e] *= a;
+      for (int key = my_ks; key < DEC_TILE; key += ks_n) {
+        const float pe = ss[g * DEC_TILE + key];
+        float vf[8];
+        ld8(tV + key * D + sc * 8, vf);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[r][e] = fmaf(pe, vf[e], acc[r][e]);
+      }
+    }
+    __syncthreads();  // stage st and the score buffer are free again
+    if (tid == 0 && j + DEC_STAGES < n_tiles) issue(j + DEC_STAGES);
+  }
+
+  // merge the key subsets in subset order
+  if (ks_n > 1) {
+    if (my_item[0] >= 0)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) sred[(my_ks * items + my_item[0]) * 8 + e] = acc[0][e];
+    __syncthreads();
+    if (tid < items) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[0][e] = sred[tid * 8 + e];
+      for (int k = 1; k < ks_n; ++k)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[0][e] += sred[(k * items + tid) * 8 + e];
+      my_item[0] = tid;
+    } else {
+      my_item[0] = -1;
+    }
+  }
+
+#pragma unroll
+  for (int r = 0; r < DEC_MAX_ITEMS; ++r) {
+    if (my_item[r] < 0) continue;
+    const int g = my_item[r] / L, sc = my_item[r] % L;
+    const int h = hk * G + g;
+    const long long bh = (long long)b * p.H + h;
+    const float m = sm[g], l = sl[g];
+    if (n_chunks == 1) {
+      const float inv = 1.0f / l;
+      float f[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) f[e] = acc[r][e] * inv;
+      st8(reinterpret_cast<T*>(p.o) + bh * D + sc * 8, f);
+      if (p.lse != nullptr && sc == 0) p.lse[bh] = (m + log2f(l)) / kLog2e;
+    } else {
+      st8(p.part_acc + (bh * p.max_chunks + c) * D + sc * 8, acc[r]);
+      if (sc == 0) {
+        p.part_ml[(bh * p.max_chunks + c) * 2] = m;
+        p.part_ml[(bh * p.max_chunks + c) * 2 + 1] = l;
+      }
+    }
+  }
+}
+
+// o = sum_c exp2(m_c - M) acc_c / sum_c exp2(m_c - M) l_c over a row's chunks, in chunk order; one thread per column
+template <typename T, int D>
+__global__ void __launch_bounds__(D)
+attn_decode_combine_kernel(const DecArgs p) {
+  const int h = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
+  const int n = (min(p.lens[b], p.s_max) + DEC_CHUNK - 1) / DEC_CHUNK;
+  if (n <= 1) return;  // finished by attn_decode_kernel
+  const long long bh = (long long)b * p.H + h;
+  const float* ml = p.part_ml + bh * p.max_chunks * 2;
+  const float* pa = p.part_acc + bh * p.max_chunks * D + d;
+  float M = -INFINITY;
+  for (int c = 0; c < n; ++c) M = fmaxf(M, ml[2 * c]);
+  float l = 0.f, acc = 0.f;
+  for (int c = 0; c < n; ++c) {
+    const float w = exp2f(ml[2 * c] - M);
+    l = fmaf(ml[2 * c + 1], w, l);
+    acc = fmaf(pa[(long long)c * D], w, acc);
+  }
+  const float out = acc / l;
+  if constexpr (sizeof(T) == 2) reinterpret_cast<__nv_bfloat16*>(p.o)[bh * D + d] = __float2bfloat16(out);
+  else reinterpret_cast<float*>(p.o)[bh * D + d] = out;
+  if (p.lse != nullptr && d == 0) p.lse[bh] = (M + log2f(l)) / kLog2e;
+}
+
+template <typename T, int D>
+int launch_decode(const CUtensorMap& tmK, const CUtensorMap& tmV, const DecArgs& a, int B, int Hk,
+                  cudaStream_t stream) {
+  auto kern = attn_decode_kernel<T, D>;
+  const DecSmem lay(D, (int)sizeof(T), a.G);
+  static int attr_bytes = 0;
+  if (lay.total > 48 * 1024 && lay.total > attr_bytes) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+    attr_bytes = lay.total;
+  }
+  kern<<<dim3(a.max_chunks, Hk, B), DEC_THREADS, lay.total, stream>>>(tmK, tmV, a);
+  B200_CHECK_LAUNCH();
+  if (a.max_chunks > 1) {
+    attn_decode_combine_kernel<T, D><<<dim3(a.H, B), D, 0, stream>>>(a);
+    B200_CHECK_LAUNCH();
+  }
+  return B200_OK;
+}
+
+template <typename T>
+int launch_decode_d(int D, const CUtensorMap& tmK, const CUtensorMap& tmV, const DecArgs& a, int B, int Hk,
+                    cudaStream_t stream) {
+  switch (D) {
+    case 16: return launch_decode<T, 16>(tmK, tmV, a, B, Hk, stream);
+    case 32: return launch_decode<T, 32>(tmK, tmV, a, B, Hk, stream);
+    case 64: return launch_decode<T, 64>(tmK, tmV, a, B, Hk, stream);
+    default: return launch_decode<T, 128>(tmK, tmV, a, B, Hk, stream);
+  }
+}
+
+// One thread per 8-column vector: q heads (rotated in place, RoPE only), then k heads (rotated when RoPE is on) and
+// v heads, both written to cache row pos = lens[b] - 1.  The rotation is b200_rope's arithmetic, statement for
+// statement, so a token rotated here equals the same token rotated by the prefill.
+template <typename T>
+__global__ void __launch_bounds__(256)
+kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v, T* __restrict__ k_cache,
+                 T* __restrict__ v_cache, const int* __restrict__ lens, const float* __restrict__ cos_t,
+                 const float* __restrict__ sin_t, long long nvec, int s_max, int H, int Hk, int D) {
+  const int L = D / 8;
+  const int q_heads = cos_t != nullptr ? H : 0;
+  const int heads = q_heads + 2 * Hk;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
+    const int dv = (int)(i % L);
+    const int hh = (int)(i / L % heads);
+    const int b = (int)(i / L / heads);
+    const int pos = lens[b] - 1;
+    if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
+    const T* src;
+    T* dst;
+    bool rotate = cos_t != nullptr;
+    if (hh < q_heads) {
+      src = dst = q + ((long long)b * H + hh) * D + dv * 8;
+    } else if (hh < q_heads + Hk) {
+      const int h = hh - q_heads;
+      src = k + ((long long)b * Hk + h) * D + dv * 8;
+      dst = k_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+    } else {
+      const int h = hh - q_heads - Hk;
+      src = v + ((long long)b * Hk + h) * D + dv * 8;
+      dst = v_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+      rotate = false;
+    }
+    float xv[8], o[8];
+    ld8(src, xv);
+    if (rotate) {
+      const float4 c = *reinterpret_cast<const float4*>(cos_t + (long long)pos * (D / 2) + dv * 4);
+      const float4 sn = *reinterpret_cast<const float4*>(sin_t + (long long)pos * (D / 2) + dv * 4);
+      o[0] = xv[0] * c.x - xv[1] * sn.x;  o[1] = xv[0] * sn.x + xv[1] * c.x;
+      o[2] = xv[2] * c.y - xv[3] * sn.y;  o[3] = xv[2] * sn.y + xv[3] * c.y;
+      o[4] = xv[4] * c.z - xv[5] * sn.z;  o[5] = xv[4] * sn.z + xv[5] * c.z;
+      o[6] = xv[6] * c.w - xv[7] * sn.w;  o[7] = xv[6] * sn.w + xv[7] * c.w;
+      st8(dst, o);
+    } else {
+      st8(dst, xv);
+    }
+  }
+}
+
+bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+}  // namespace
+
+size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D) {
+  if (B <= 0 || H <= 0 || s_max <= 0 || D <= 0) return 0;
+  const size_t chunks = (size_t)(s_max + DEC_CHUNK - 1) / DEC_CHUNK;
+  return (size_t)B * H * chunks * (size_t)(D + 2) * sizeof(float);
+}
+
+int attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse, int B,
+                int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes,
+                cudaStream_t stream) {
+  B200_CHECK_ARG(B > 0 && H > 0 && Hk > 0 && H % Hk == 0, "attn_decode: bad shape B=%d H=%d Hk=%d", B, H, Hk);
+  B200_CHECK_ARG(D == 16 || D == 32 || D == 64 || D == 128, "attn_decode: head_dim %d unsupported (16/32/64/128)", D);
+  B200_CHECK_ARG(s_max >= DEC_TILE, "attn_decode: s_max=%d must be >= %d", s_max, DEC_TILE);
+  const int G = H / Hk;
+  B200_CHECK_ARG(G * D <= DEC_MAX_ITEMS * DEC_THREADS * 8, "attn_decode: (H/Hk) * D = %d exceeds %d", G * D,
+                 DEC_MAX_ITEMS * DEC_THREADS * 8);
+  B200_CHECK_ARG(al16(q) && al16(o) && lens != nullptr, "attn_decode: q / o must be 16-byte aligned, lens non-null");
+  const size_t need = attn_decode_workspace_bytes(B, H, s_max, D);
+  if (ws_bytes < need || (need > 0 && ws == nullptr)) {
+    set_error("attn_decode: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    return B200_ERR_WORKSPACE;
+  }
+  const int elem = is_bf16 ? 2 : 4;
+  const CUtensorMapDataType dt = is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const uint64_t dims[4] = {(uint64_t)D, (uint64_t)Hk, (uint64_t)s_max, (uint64_t)B};
+  const uint64_t strides[3] = {(uint64_t)D * elem, (uint64_t)Hk * D * elem, (uint64_t)s_max * Hk * D * elem};
+  const uint32_t box[4] = {(uint32_t)D, 1, (uint32_t)DEC_TILE, 1};
+  CUtensorMap tmK, tmV;
+  int rc;
+  if ((rc = make_tensor_map(&tmK, k_cache, dt, elem, 4, dims, strides, box, false))) return rc;
+  if ((rc = make_tensor_map(&tmV, v_cache, dt, elem, 4, dims, strides, box, false))) return rc;
+  DecArgs a;
+  a.q = q;
+  a.o = o;
+  a.lse = lse;
+  a.lens = lens;
+  a.max_chunks = (s_max + DEC_CHUNK - 1) / DEC_CHUNK;
+  a.part_acc = reinterpret_cast<float*>(ws);
+  a.part_ml = a.part_acc + (size_t)B * H * a.max_chunks * D;
+  a.H = H;
+  a.G = G;
+  a.s_max = s_max;
+  a.scale_log2 = scale * kLog2e;
+  return is_bf16 ? launch_decode_d<__nv_bfloat16>(D, tmK, tmV, a, B, Hk, stream)
+                 : launch_decode_d<float>(D, tmK, tmV, a, B, Hk, stream);
+}
+
+int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+              const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+              cudaStream_t stream) {
+  B200_CHECK_ARG(B > 0 && s_max > 0 && H > 0 && Hk > 0 && D > 0 && D % 8 == 0,
+                 "kv_append: bad shape B=%d s_max=%d H=%d Hk=%d D=%d (D %% 8 == 0)", B, s_max, H, Hk, D);
+  B200_CHECK_ARG((cos_t == nullptr) == (sin_t == nullptr), "kv_append: give both RoPE tables or neither");
+  B200_CHECK_ARG(al16(k) && al16(v) && al16(k_cache) && al16(v_cache) && (cos_t == nullptr || (al16(q) && al16(cos_t) && al16(sin_t))),
+                 "kv_append: alignment");
+  const int heads = (cos_t != nullptr ? H : 0) + 2 * Hk;
+  const long long nvec = (long long)B * heads * (D / 8);
+  long long blocks = (nvec + 255) / 256;
+  if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+  if (is_bf16)
+    kv_append_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, stream>>>(
+        (__nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (__nv_bfloat16*)k_cache,
+        (__nv_bfloat16*)v_cache, lens, cos_t, sin_t, nvec, s_max, H, Hk, D);
+  else
+    kv_append_kernel<float><<<(int)blocks, 256, 0, stream>>>((float*)q, (const float*)k, (const float*)v,
+                                                             (float*)k_cache, (float*)v_cache, lens, cos_t, sin_t,
+                                                             nvec, s_max, H, Hk, D);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+}  // namespace b200

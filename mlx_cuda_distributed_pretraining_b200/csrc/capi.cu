@@ -106,6 +106,13 @@ size_t attn_bwd_workspace_bytes(int B, int S, int H, int Hk, int D);
 int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
              const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
              float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
+size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D);
+int attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse, int B,
+                int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes,
+                cudaStream_t stream);
+int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+              const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+              cudaStream_t stream);
 }  // namespace b200
 
 #define S_(x) reinterpret_cast<cudaStream_t>(x)
@@ -370,6 +377,21 @@ int b200_attn_bwd_strided(const void* q, const void* k, const void* v, const voi
                           size_t workspace_bytes, void* stream) {
   return b200::attn_bwd(q, k, v, o, d_o, lse, dq, dk, dv, B, S, H, Hk, D, scale, causal, dkv_row_heads,
                         workspace, workspace_bytes, S_(stream));
+}
+
+size_t b200_attn_decode_workspace_bytes(int B, int H, int s_max, int D) {
+  return b200::attn_decode_workspace_bytes(B, H, s_max, D);
+}
+int b200_attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
+                     int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* workspace,
+                     size_t workspace_bytes, void* stream) {
+  return b200::attn_decode(q, k_cache, v_cache, lens, o, lse, B, s_max, H, Hk, D, scale, is_bf16, workspace,
+                           workspace_bytes, S_(stream));
+}
+int b200_kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                   const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                   void* stream) {
+  return b200::kv_append(q, k, v, k_cache, v_cache, lens, cos_t, sin_t, B, s_max, H, Hk, D, is_bf16, S_(stream));
 }
 
 }  // extern "C"

@@ -763,6 +763,83 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional
 
 
 # ------------------------------------------------------------------------------------------------
+# generation: decode attention over a KV cache and the per-token cache append
+# ------------------------------------------------------------------------------------------------
+def attention_decode_workspace_bytes(B: int, H: int, s_max: int, D: int) -> int:
+    return int(lib().b200_attn_decode_workspace_bytes(B, H, s_max, D))
+
+
+def _check_cache(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor, what: str):
+    _is_bf16(q, "q")
+    for t, nm in ((q, "q"), (k_cache, "k_cache"), (v_cache, "v_cache")):
+        _need(t, q.dtype, f"{what}: {nm}")
+    if q.dim() != 3 or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
+        raise ValueError(f"{what}: expected q [B,H,D] and k_cache == v_cache [B,s_max,Hk,D], got "
+                         f"{tuple(q.shape)}, {tuple(k_cache.shape)}, {tuple(v_cache.shape)}")
+    B, H, D = q.shape
+    Bc, s_max, Hk, Dc = k_cache.shape
+    if Bc != B or Dc != D or H % Hk != 0:
+        raise ValueError(f"{what}: q {tuple(q.shape)} does not match cache {tuple(k_cache.shape)}")
+    if lens.dtype != torch.int32 or lens.device != q.device or lens.shape != (B,) or not lens.is_contiguous():
+        raise ValueError(f"{what}: lens must be a contiguous int32 [B] tensor on {q.device}, got {lens.dtype} "
+                         f"{tuple(lens.shape)} on {lens.device}")
+    return B, H, D, s_max, Hk
+
+
+def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
+                     scale: Optional[float] = None, workspace: Optional[torch.Tensor] = None,
+                     return_lse: bool = False):
+    """softmax(q K^T * scale) V for one new query per row over its first lens[b] cached keys (b200_attn_decode).
+
+    q [B,H,D]; k_cache, v_cache [B,s_max,Hk,D]; all bf16 or all fp32, D in {16, 32, 64, 128}; lens int32 [B] on the
+    device, 1 <= lens[b] <= s_max (not checked here: that would read the device).  `workspace` (uint8, at least
+    attention_decode_workspace_bytes(B, H, s_max, D)) is allocated when not given.  Returns o [B,H,D] in q's dtype,
+    and the natural-log LSE [B,H] fp32 with return_lse."""
+    B, H, D, s_max, Hk = _check_cache(q, k_cache, v_cache, lens, "attention_decode")
+    if D not in (16, 32, 64, 128):
+        raise ValueError(f"attention_decode: head_dim {D} unsupported (16, 32, 64 or 128)")
+    if scale is None:
+        scale = D ** -0.5
+    need = attention_decode_workspace_bytes(B, H, s_max, D)
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
+    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need:
+        raise ValueError(f"attention_decode: workspace must be uint8 on {q.device} with >= {need} bytes")
+    o = torch.empty_like(q)
+    lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
+    tok = _t0("attn_decode")
+    check(lib().b200_attn_decode(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr(), o.data_ptr(),
+                                 _ptr(lse), B, s_max, H, Hk, D, float(scale), _is_bf16(q, "q"), workspace.data_ptr(),
+                                 workspace.numel(), _stream()), "b200_attn_decode")
+    _t1(tok)
+    return (o, lse) if return_lse else o
+
+
+def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
+              lens: torch.Tensor, rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> None:
+    """Writes each row's new k [B,Hk,D] and v into the caches at pos = lens[b] - 1 (b200_kv_append).  With
+    rope_tables = (cos, sin) from rope_tables(), k and, in place, q [B,H,D] get the rotation ops.rope applies at
+    position pos, with the same arithmetic.  The caller keeps pos below the tables' length."""
+    B, H, D, s_max, Hk = _check_cache(q, k_cache, v_cache, lens, "kv_append")
+    for t, nm in ((k, "k"), (v, "v")):
+        _need(t, q.dtype, f"kv_append: {nm}")
+        if t.shape != (B, Hk, D):
+            raise ValueError(f"kv_append: {nm} must be [{B},{Hk},{D}], got {tuple(t.shape)}")
+    if D % 8 != 0:
+        raise ValueError(f"kv_append: head_dim {D} must be a multiple of 8")
+    cos_t = sin_t = None
+    if rope_tables is not None:
+        cos_t, sin_t = rope_tables
+        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
+            _need(t, torch.float32, f"kv_append: {nm}")
+            if t.dim() != 2 or t.shape[1] != D // 2:
+                raise ValueError(f"kv_append: RoPE tables must be [positions, {D // 2}]")
+    check(lib().b200_kv_append(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                               lens.data_ptr(), _ptr(cos_t), _ptr(sin_t), B, s_max, H, Hk, D, _is_bf16(q, "q"),
+                               _stream()), "b200_kv_append")
+
+
+# ------------------------------------------------------------------------------------------------
 # raw strided GEMM + Shampoo elementwise helpers
 # ------------------------------------------------------------------------------------------------
 def gemm_raw(a_mn: bool, b_mn: bool, M: int, N: int, K: int, batch: int,
