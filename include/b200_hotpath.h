@@ -282,6 +282,11 @@ int b200_add_rmsnorm_bwd(const void* dy, const void* dres, const void* x, const 
 /* x,y: [B,S,NH,D]; cos_t,sin_t: f32 [S,D/2]; backward=1 applies the inverse rotation */
 int b200_rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, int S, int NH,
               int D, int backward, int is_bf16, void* stream);
+/* b200_rope for packed sequences: token s of row b is rotated by the angle of pos[b, s] (int32 [B,S], its position
+ * within its document, 4-byte aligned) instead of s, so each document gets the rotation it would get alone
+ * (arch/llama_standard.py:90-131 with position_ids).  The tables must hold max(pos) + 1 rows. */
+int b200_rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S,
+                  int NH, int D, int backward, int is_bf16, void* stream);
 
 /* ---- MLP block on the in-tree GEMM engine with the GLU in the epilogue (SURVEY 8f row f1) ----------------
  * arch/llama.py:142-151: down( gate(x) * sigmoid(up(x)) * 2 ).  gate_proj.weight and up_proj.weight must be
@@ -335,6 +340,19 @@ int b200_attn_bwd_strided(const void* q, const void* k, const void* v, const voi
                           const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk,
                           int D, float scale, int causal, int dkv_row_heads, void* workspace,
                           size_t workspace_bytes, void* stream);
+/* Document-causal attention for packed sequences, replacing b200_attn_fwd / b200_attn_bwd_strided with causal=1
+ * when a row holds several documents.  pos (int32 [B,S], 4-byte aligned) is each token's position within its
+ * document (0 at a document's first token, +1 per token inside it); query s sees keys s - pos[b,s] .. s, the causal
+ * mask of each document run alone (the block-diagonal mask the reference would build as an additive [B,1,S,S] mask,
+ * arch/flash_attention.py:123-134).  Key / query tiles wholly outside a query's document are skipped.  The backward
+ * takes b200_attn_bwd_strided's dk / dv rows and a workspace of b200_attn_bwd_doc_workspace_bytes
+ * (b200_attn_bwd_workspace_bytes plus the per-row document bounds). */
+int b200_attn_fwd_doc(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B,
+                      int S, int H, int Hk, int D, float scale, void* stream);
+size_t b200_attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D);
+int b200_attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                      const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                      int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- generation: decode attention over a KV cache (arch/flash_attention.py:97-156, last query row) ------------
  * One new query per sequence against its cached keys, causal by construction (every cached key precedes it):

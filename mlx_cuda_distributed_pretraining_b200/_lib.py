@@ -58,6 +58,7 @@ SIGNATURES = {
     "b200_add_rmsnorm_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _f, _i, _vp]),
     "b200_add_rmsnorm_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp, _sz, _vp]),
     "b200_rope": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_rope_pos": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_mlp_gateup_glu_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "b200_mlp_down_glu_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "b200_embedding_bwd_workspace_bytes": (_sz, [_i, _i]),
@@ -71,6 +72,10 @@ SIGNATURES = {
     "b200_attn_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i,
                            _vp, _sz, _vp]),
     "b200_attn_bwd_strided": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _vp, _sz, _vp]),
+    "b200_attn_fwd_doc": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_attn_bwd_doc_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "b200_attn_bwd_doc": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz,
+                               _vp]),
     "b200_attn_decode_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "b200_attn_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
     "b200_kv_append": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),

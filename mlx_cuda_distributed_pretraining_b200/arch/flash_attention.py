@@ -26,6 +26,28 @@ class CausalMask:
         return torch.triu(m, diagonal=1)[None, None]
 
 
+class DocumentCausalMask:
+    """Marker for the document-causal mask of packed rows: pos (int32 [B, S]) is each token's position within its
+    document (0 at a document's first token, +1 per token inside it), and query q sees key k iff
+    q - pos[q] <= k <= q -- the causal mask of every document run alone.  The fused document kernels apply it
+    implicitly, and RoPE rotates by pos."""
+
+    def __init__(self, pos: torch.Tensor):
+        if pos.dim() != 2:
+            raise ValueError(f"DocumentCausalMask: pos must be [B, S], got {list(pos.shape)}")
+        self.pos = pos.to(torch.int32).contiguous()
+        self.seq_len = pos.shape[1]
+
+    def dense(self, dtype=torch.float32, device="cpu") -> torch.Tensor:
+        """The additive [B, 1, S, S] mask (0 where visible, -inf elsewhere)."""
+        pos = self.pos.to(device=device, dtype=torch.int64)
+        s = torch.arange(self.seq_len, device=device)
+        q, k = s[:, None], s[None, :]
+        ok = (k <= q) & (k >= (s - pos)[:, :, None])
+        m = torch.zeros(ok.shape, dtype=dtype, device=device).masked_fill(~ok, float("-inf"))
+        return m[:, None]
+
+
 class FlashAttention(nn.Module):
     def __init__(self, hidden_size: int, num_heads: int, num_kv_heads: Optional[int] = None,
                  head_dim: Optional[int] = None, dropout: float = 0.0, use_bias: bool = False,
@@ -48,22 +70,25 @@ class FlashAttention(nn.Module):
 
     def _flash_attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask=None) -> torch.Tensor:
         """q [B,S,H,D], k/v [B,S,Hk,D] -> [B,S,H,D]."""
+        pos = None
         if mask is None:
             causal = False
         elif isinstance(mask, CausalMask):
             causal = True
+        elif isinstance(mask, DocumentCausalMask):
+            causal, pos = True, mask.pos
         else:
             raise NotImplementedError(
-                "the fused kernel supports mask=None or the causal mask (CausalMask); "
-                "arbitrary additive masks are outside the reference's training path")
+                "the fused kernel supports mask=None, the causal mask (CausalMask) or the document-causal mask of "
+                "packed rows (DocumentCausalMask); arbitrary additive masks are outside the reference's training path")
         dt = q.dtype
         if dt == torch.float32 and 3 * self.head_dim <= 128:
             # full-precision configs (mixed_precision: false, e.g. BASELINE C1, head_dim 16): logits through
             # three-term bf16 products (hi/lo split operands), ~fp32-accurate scores on the same kernels
-            return ops.attention_fp32(q, k, v, self.scale, causal)
+            return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos)
         if dt != torch.bfloat16:  # larger head dims: bf16 operands with fp32 accumulation (stated in DESIGN.md)
             q, k, v = q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
-        o = ops.attention(q, k, v, self.scale, causal)
+        o = ops.attention(q, k, v, self.scale, causal, pos=pos)
         return o if dt == torch.bfloat16 else o.to(dt)
 
     def forward(self, x: torch.Tensor, mask=None) -> torch.Tensor:
@@ -77,8 +102,9 @@ class FlashAttention(nn.Module):
         v = v.reshape(B, S, self.num_kv_heads, self.head_dim)
         if self.rope_tables is not None:
             cos_t, sin_t = self.rope_tables
-            q = ops.rope(q, cos_t[:S], sin_t[:S])
-            k = ops.rope(k, cos_t[:S], sin_t[:S])
+            pos = mask.pos if isinstance(mask, DocumentCausalMask) else None  # packed rows: position in document
+            q = ops.rope(q, cos_t[:S], sin_t[:S], pos)
+            k = ops.rope(k, cos_t[:S], sin_t[:S], pos)
         ctx = self._flash_attention(q, k, v, mask)
         ctx = ctx.reshape(B, S, self.num_heads * self.head_dim)
         return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)

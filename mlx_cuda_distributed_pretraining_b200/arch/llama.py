@@ -22,7 +22,7 @@ import torch
 from torch import nn
 
 from .. import ops
-from .flash_attention import CausalMask, FlashAttention
+from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention
 
 
 @dataclass
@@ -202,8 +202,18 @@ class Model(nn.Module):
         self.lm_head = None if args.tie_word_embeddings else nn.Linear(args.hidden_size, args.vocab_size, bias=False)
 
     def hidden_states(self, inputs: torch.Tensor, position_ids=None, attention_mask=None) -> torch.Tensor:
+        """position_ids (int [B, S], optional): packed rows, each token's position within its document (0 at the
+        document's first token).  It selects the document-causal mask and, with RoPE on, the rotation angles, so
+        every document is computed as if it ran alone.  None keeps the causal mask over whole rows."""
         B, S = inputs.shape
-        mask = CausalMask(S) if attention_mask is None else attention_mask
+        if attention_mask is not None:
+            mask = attention_mask
+        elif position_ids is not None:
+            if tuple(position_ids.shape) != (B, S):
+                raise ValueError(f"position_ids must be [B, S] = {[B, S]}, got {list(position_ids.shape)}")
+            mask = DocumentCausalMask(position_ids)
+        else:
+            mask = CausalMask(S)
         h = ops.embedding(inputs, self.embed_tokens.weight)
         pending = None
         for layer in self.layers:
@@ -226,7 +236,7 @@ class Model(nn.Module):
             return self._tied_w
         return self.embed_tokens.weight
 
-    def padded_logits(self, inputs: torch.Tensor):
+    def padded_logits(self, inputs: torch.Tensor, position_ids=None):
         """(logits [B*S, ld], V) with ld >= V, ld % 8 == 0 when the fused cross-entropy can take them
         (bf16 weights, tied + row-padded embedding alias or an aligned vocabulary); else (None, V).
         Eligibility is decided BEFORE the forward pass, so an ineligible config (fp32, logit_scale,
@@ -236,7 +246,7 @@ class Model(nn.Module):
         w = self._logits_weight()
         if w.shape[0] % 8 != 0 or w.dtype != torch.bfloat16:
             return None, self.vocab_size
-        h = self.hidden_states(inputs)
+        h = self.hidden_states(inputs, position_ids)
         logits = torch.nn.functional.linear(h, w)
         return logits.view(-1, logits.shape[-1]), self.vocab_size
 

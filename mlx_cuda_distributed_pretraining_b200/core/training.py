@@ -259,7 +259,56 @@ class SyntheticData:
         return out
 
 
+def pack_first_fit(lengths: List[int], capacity: int) -> List[List[int]]:
+    """First-fit bin packing in the given order: item i goes to the lowest-numbered row with at least lengths[i]
+    free slots, or opens a new row.  Returns each row's item indices in placement order.  A max-tree over the rows'
+    free space finds that row in O(log rows)."""
+    size = 1
+    while size < max(len(lengths), 1):
+        size *= 2
+    free = [0] * (2 * size)  # leaves: free slots of rows (0 until opened); inner nodes: max of the children
+    rows: List[List[int]] = []
+    for i, n in enumerate(lengths):
+        if n > capacity:
+            raise ValueError(f"item {i} of length {n} exceeds the row capacity {capacity}")
+        if free[1] >= n:
+            node = 1
+            while node < size:
+                node = 2 * node if free[2 * node] >= n else 2 * node + 1
+            r = node - size
+        else:
+            r = len(rows)
+            rows.append([])
+            node = size + r
+            free[node] = capacity
+        rows[r].append(i)
+        free[node] -= n
+        node //= 2
+        while node:
+            free[node] = max(free[2 * node], free[2 * node + 1])
+            node //= 2
+    return rows
+
+
+def document_positions(inputs: torch.Tensor, bos_token: int) -> torch.Tensor:
+    """pos (int32, inputs' shape [B, S]) of packed token rows: each token's position within its document, where a
+    document starts at every BOS token.  Tokens before a row's first BOS count from the row start.  Runs on the
+    inputs' device without a host synchronisation."""
+    S = inputs.shape[-1]
+    idx = torch.arange(S, device=inputs.device, dtype=torch.int64).expand_as(inputs)
+    start = torch.where(inputs == bos_token, idx, torch.zeros_like(idx)).cummax(dim=-1).values
+    return (idx - start).to(torch.int32)
+
+
 class DataManager:
+    """Unpacked (default): each training row is one chunk, padded to the longest chunk of its batch.
+
+    `data.preprocessing.pack_sequences: true`: training rows of max_context_size + 1 tokens hold whole tokenised
+    chunks (tokenize_doc: BOS first), placed first-fit in the shuffled order, tails filled with PAD; a chunk longer
+    than a row is cut to the row.  Every chunk appears once per epoch.  The packed batches are walked in a permuted
+    order drawn from the same global RNG after the unpacked state, so the validation batches (never packed) are the
+    unpacked run's."""
+
     def __init__(self, config: DataConfig, tokenizer: TokenizerManager, batch_size: int = 1, rank: int = 0,
                  world: int = 1):
         self.config, self.tokenizer, self.batch_size = config, tokenizer, batch_size
@@ -278,6 +327,30 @@ class DataManager:
             vidx = sorted(range(len(self.val_docs)), key=lambda i: len(self.val_docs[i]))
             self.val_batch_idx = [vidx[i:min(i + batch_size, len(vidx))] for i in range(0, len(vidx), batch_size)]
             self.val_indices = np.random.permutation(len(self.val_batch_idx))
+        self.pack = bool(config.preprocessing.get("pack_sequences", False))
+        if self.pack:
+            self._setup_packing(idx)
+
+    def _setup_packing(self, order: List[int]) -> None:
+        row_len = self.config.preprocessing["max_context_size"] + 1
+        bos = self.tokenizer.BOS_TOKEN
+        self.packed_tokens: List[List[int]] = []
+        for i in order:
+            t = self.tokenizer.tokenize_doc(self.train_docs[i])
+            if bos in t[1:]:
+                raise ValueError(f"document {i} ({self.train_docs[i][:40]!r}...) contains the BOS token id {bos} "
+                                 "after its first position: packed rows find document starts at BOS tokens")
+            self.packed_tokens.append(t[:row_len])
+        self.packed_rows = pack_first_fit([len(t) for t in self.packed_tokens], row_len)
+        bs = self.batch_size
+        self.packed_batch_idx = [list(range(i, min(i + bs, len(self.packed_rows))))
+                                 for i in range(0, len(self.packed_rows), bs)]
+        self.packed_indices = np.random.permutation(len(self.packed_batch_idx))
+
+    @property
+    def num_train_batches(self) -> int:
+        """Training batches per epoch (packed batches when packing is on)."""
+        return len(self.packed_batch_idx) if self.pack else len(self.train_batch_idx)
 
     def _load_file(self, file_path: str, docs: List[str]) -> None:
         chunk = self.config.preprocessing["max_context_size"]
@@ -289,9 +362,22 @@ class DataManager:
                     docs.append(text[i:i + chunk])
 
     def generate_batch(self, step: int) -> torch.Tensor:
+        if self.pack:
+            return self._packed_batch(step)
         # data-parallel ranks walk disjoint batches of the shared shuffled order
         j = (step * self.world + self.rank) % len(self.train_indices)
         return self._create_batch([self.train_docs[i] for i in self.train_batch_idx[self.train_indices[j]]])
+
+    def _packed_batch(self, step: int) -> torch.Tensor:
+        """[batch_size, max_context_size + 1] rows of whole documents; the last batch of an epoch may hold rows
+        of PAD only (no loss, no tokens)."""
+        j = (step * self.world + self.rank) % len(self.packed_indices)
+        row_len = self.config.preprocessing["max_context_size"] + 1
+        out = torch.full((self.batch_size, row_len), self.tokenizer.PAD_TOKEN, dtype=torch.int64)
+        for r, row in enumerate(self.packed_batch_idx[self.packed_indices[j]]):
+            toks = [t for d in self.packed_rows[row] for t in self.packed_tokens[d]]
+            out[r, :len(toks)] = torch.tensor(toks, dtype=torch.int64)
+        return out
 
     def generate_validation_batch(self, batch_idx: int) -> torch.Tensor:
         if not self.val_batch_idx:
@@ -593,7 +679,10 @@ class Trainer:
 
     def setup_training(self) -> None:
         hp = self.config.training.hyperparameters
-        steps_per_epoch = max(len(self.data_manager.train_docs) // hp["batch_size"], 1)
+        if getattr(self.data_manager, "pack", False):
+            steps_per_epoch = max(self.data_manager.num_train_batches, 1)
+        else:
+            steps_per_epoch = max(len(self.data_manager.train_docs) // hp["batch_size"], 1)
         self.steps_per_epoch = steps_per_epoch
         self.total_steps = (steps_per_epoch * self.config.training.epochs if self.config.training.epochs is not None
                             else hp.get("iters", steps_per_epoch))
@@ -616,18 +705,31 @@ class Trainer:
         self._pin = None
 
     # -- loss --------------------------------------------------------------------------------------
-    def compute_loss(self, model, inputs: torch.Tensor, targets: torch.Tensor):
+    def compute_loss(self, model, inputs: torch.Tensor, targets: torch.Tensor, packed: bool = False):
+        """Masked token-mean cross-entropy.  packed: the rows hold several documents (DataManager with
+        pack_sequences); the model then attends within documents (position_ids from the BOS tokens), and the one
+        target per document boundary that an unpacked row never has -- a document's last token predicting the
+        next document's BOS -- becomes PAD, so the loss terms and ntoks are those of the documents run alone."""
         max_ctx = self.config.model.attention.get("max_position_embeddings", 2048)
         if inputs.shape[1] > max_ctx:
             inputs, targets = inputs[:, :max_ctx], targets[:, :max_ctx]
+        position_ids = None
+        if packed:
+            position_ids = document_positions(inputs, self.tokenizer.BOS_TOKEN)
+            targets = targets.masked_fill(targets == self.tokenizer.BOS_TOKEN, self.tokenizer.PAD_TOKEN)
         pad_mask = targets != self.tokenizer.PAD_TOKEN
         ntoks = pad_mask.sum()
-        logits2d, V = model.padded_logits(inputs) if hasattr(model, "padded_logits") else (None, None)
+        if not hasattr(model, "padded_logits"):
+            logits2d, V = None, None
+        elif position_ids is None:
+            logits2d, V = model.padded_logits(inputs)
+        else:
+            logits2d, V = model.padded_logits(inputs, position_ids)
         if logits2d is not None:
             # fused path: fp32 log-sum-exp over bf16 logits, pad mask applied per row, no fp32 [B,S,V] copy
             rows = ops.cross_entropy_rows(logits2d, targets.reshape(-1).contiguous(), V, self.tokenizer.PAD_TOKEN)
             return rows.sum() / ntoks, ntoks
-        logits = model(inputs).float()  # loss always in fp32 (core/training.py:1226)
+        logits = (model(inputs) if position_ids is None else model(inputs, position_ids)).float()  # fp32 loss (:1226)
         ce = torch.nn.functional.cross_entropy(logits.view(-1, logits.shape[-1]), targets.reshape(-1),
                                                reduction="none").view(targets.shape)
         return (ce * pad_mask).sum() / ntoks, ntoks
@@ -674,7 +776,8 @@ class Trainer:
         """Forward + backward of one micro-batch already resident on the device, gradient clamp / 1/k
         accumulation (core/training.py:1664-1696), and -- on the k-th micro-step -- the data-parallel
         exchange and the optimizer update.  Returns (loss, ntoks, did_update)."""
-        loss, ntoks = self.compute_loss(self.model, dev_batch[:, :-1], dev_batch[:, 1:])
+        loss, ntoks = self.compute_loss(self.model, dev_batch[:, :-1], dev_batch[:, 1:],
+                                        packed=getattr(self.data_manager, "pack", False))
         loss.backward()
         k = self.grad_accum_steps
         store = self.store

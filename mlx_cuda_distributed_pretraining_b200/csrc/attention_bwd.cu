@@ -23,6 +23,14 @@
 // Causal balance: key tile t has work for the queries from t*128 on, so tile 0 has n_kt times the items of the last
 // one.  With an even tile count a CTA runs tile t and then tile n_kt-1-t (equal work in every CTA); the n_kt/2 CTAs of
 // one (kv head, batch) are adjacent in launch order and share its Q / dO rows in L2.
+//
+// Document variant (DOC = true, packed sequences; pos[b, s] = position of token s within its document, so query q sees
+// keys q - pos[q] .. q).  The pre-pass also writes each token's document start (rows of S_pad ints) and, per (row,
+// key tile), the end of the query-tile range: the tile holding the last token of the document that contains the key
+// tile's last key.  Query tiles past it see none of the tile's keys and are skipped.  Each item's 64 document starts
+// arrive with its LSE and delta; the mask `key >= q - pos[q]` joins the causal one only on items whose queries'
+// highest document start lies above the warpgroup's first key.  Document launches use the unpaired order.  DOC = false
+// compiles to the causal / non-causal kernels unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -37,7 +45,7 @@ constexpr int BKV = 128;          // keys per tile (64 per consumer warpgroup)
 constexpr int BQ = 64;            // queries per item
 constexpr float kLog2e = 1.4426950408889634f;
 
-template <int D>
+template <int D, bool DOC = false>
 struct BwdCfg {
   static constexpr int NB = D / 64;                 // 64-column (128-byte) blocks per bf16 row
   static constexpr int STAGES = D == 64 ? 3 : 2;    // Q / dO ring depth (D = 128: two fill the shared memory)
@@ -45,7 +53,7 @@ struct BwdCfg {
   static constexpr int QS_BYTES = BQ * D * 2;       // one Q or dO stage
   static constexpr int DS_BYTES = BKV * BQ * 2;     // dS^T [128 keys][64 queries] bf16
   static constexpr int DQ_BYTES = BQ * D * 4;       // fp32 dQ tile: D/32 blocks of [64 rows][32 floats], swizzled
-  static constexpr int L_BYTES = 2 * BQ * 4;        // LSE*log2e, delta of one item
+  static constexpr int L_BYTES = (DOC ? 3 : 2) * BQ * 4;  // LSE*log2e, delta (and DOC: document starts) of one item
   static constexpr int OFF_K = 0;
   static constexpr int OFF_V = OFF_K + KV_BYTES;
   static constexpr int OFF_Q = OFF_V + KV_BYTES;
@@ -69,6 +77,8 @@ struct BwdArgs {
   float scale;
   int causal;
   int paired;          // CTA x runs key tiles x and n_kt-1-x
+  const int* dstart;   // DOC: [B,S_pad] document start of every query
+  const int* qt_end;   // DOC: [B,n_kt] end of each key tile's query-tile range
 };
 
 // The work of one key tile: `group * per_head` items, item j = (query head h0 + j / per_head, query tile
@@ -76,15 +86,23 @@ struct BwdArgs {
 struct Tile {
   int kt, k0, qt0, per_head, n_items;
 };
+template <bool DOC>
 __device__ __forceinline__ Tile tile_of(const BwdArgs& p, int pass) {
   Tile t;
   t.kt = pass == 0 ? (int)blockIdx.x : (p.S + BKV - 1) / BKV - 1 - (int)blockIdx.x;
   t.k0 = t.kt * BKV;
-  const int n_qt = (p.S + BQ - 1) / BQ;
+  int n_qt = (p.S + BQ - 1) / BQ;
+  if constexpr (DOC) n_qt = __ldg(p.qt_end + (long long)blockIdx.z * gridDim.x + t.kt);  // unpaired: x = kt
   t.qt0 = p.causal ? t.k0 / BQ : 0;
   t.per_head = n_qt - t.qt0;
   t.n_items = (p.H / p.Hk) * t.per_head;
   return t;
+}
+
+__device__ __forceinline__ int lds32i(uint32_t addr) {
+  int v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
 }
 
 template <int D>
@@ -93,12 +111,12 @@ __device__ __forceinline__ void rs_mma(float* acc, const uint32_t* a, uint64_t d
   else wgmma_m64n64k16_rs<1>(acc, a, db);
 }
 
-template <int D>
+template <int D, bool DOC>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
                 const __grid_constant__ CUtensorMap tmDQ, const BwdArgs p) {
-  using Cfg = BwdCfg<D>;
+  using Cfg = BwdCfg<D, DOC>;
   constexpr int ST = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t s0 = (smem_u32(smem_raw) + 1023) & ~1023u;
@@ -135,7 +153,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       int slot = 0;
       uint32_t phase = 0;
       for (int pass = 0; pass < n_pass; ++pass) {
-        const Tile t = tile_of(p, pass);
+        const Tile t = tile_of<DOC>(p, pass);
         if (pass > 0) mbar_wait(kv_empty, 0);
         mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
         for (int nb = 0; nb < Cfg::NB; ++nb) {
@@ -155,6 +173,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
           const long long lrow = ((long long)b * p.H + h) * p.S_pad + q0;
           bulk_load(sL + slot * Cfg::L_BYTES, p.lse2 + lrow, BQ * 4, full);
           bulk_load(sL + slot * Cfg::L_BYTES + BQ * 4, p.delta + lrow, BQ * 4, full);
+          if constexpr (DOC) bulk_load(sL + slot * Cfg::L_BYTES + 2 * BQ * 4, p.dstart + (long long)b * p.S_pad + q0,
+                                       BQ * 4, full);
           if (++slot == ST) {
             slot = 0;
             phase ^= 1u;
@@ -165,7 +185,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       tma_prefetch_desc(&tmDQ);
       int it = 0;
       for (int pass = 0; pass < n_pass; ++pass) {
-        const Tile t = tile_of(p, pass);
+        const Tile t = tile_of<DOC>(p, pass);
         for (int j = 0; j < t.n_items; ++j, ++it) {
           const int h = hk * group + j / t.per_head;
           const int q0 = (t.qt0 + j % t.per_head) * BQ;
@@ -194,7 +214,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   int it = 0;
 
   for (int pass = 0; pass < n_pass; ++pass) {
-    const Tile t = tile_of(p, pass);
+    const Tile t = tile_of<DOC>(p, pass);
     const int key_a = t.k0 + c * 64 + wq * 16 + g;  // this thread's keys: key_a, key_a + 8
     const int wkey_hi = t.k0 + c * 64 + 63;          // last key of this warpgroup
     float dk[D / 2], dv[D / 2];
@@ -225,8 +245,27 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
       // P^T and dS^T (unscaled).  Chunk nc holds queries 8 nc + cq + {0, 1}.  Only tiles that cross the causal
       // diagonal or the end of the sequence are masked; masked entries are exactly 0.
-      const bool masked = (p.causal && wkey_hi > q0) || q0 + BQ > p.S || wkey_hi >= p.S;
+      bool masked = (p.causal && wkey_hi > q0) || q0 + BQ > p.S || wkey_hi >= p.S;
+      // DOC: also where the item's highest document start (its last query's; padded rows repeat the last real one)
+      // lies above the warpgroup's first key
+      if constexpr (DOC) masked = masked || lds32i(tL + 2 * BQ * 4 + (BQ - 1) * 4) > wkey_hi - 63;
       if (masked) {
+        // DOC: document starts are monotone over the item's queries, so the queries that may see key k are a prefix
+        // of the item; n_vis[r] = its length for this thread's key key_a + 8 r (binary search over the 64 starts)
+        int n_vis[2] = {BQ, BQ};
+        if constexpr (DOC) {
+          const uint32_t tDs = tL + 2 * BQ * 4;
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int key = key_a + 8 * r;
+            int n = 0;
+#pragma unroll
+            for (int step = BQ / 2; step > 0; step >>= 1)
+              if (lds32i(tDs + (n + step - 1) * 4) <= key) n += step;
+            if (lds32i(tDs + n * 4) <= key) ++n;
+            n_vis[r] = n;
+          }
+        }
 #pragma unroll
         for (int nc = 0; nc < 8; ++nc) {
 #pragma unroll
@@ -234,7 +273,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             const int qc = nc * 8 + cq + (e & 1);
             const int qi = q0 + qc;
             const int key = key_a + ((e >> 1) << 3);
-            const bool ok = qi < p.S && key < p.S && !(p.causal && key > qi);
+            bool ok = qi < p.S && key < p.S && !(p.causal && key > qi);
+            if constexpr (DOC) ok = ok && qc < n_vis[e >> 1];
             const float pv = ok ? exp2f(st[4 * nc + e] * sl2 - lds32f(tL + qc * 4)) : 0.f;
             st[4 * nc + e] = pv;
             dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] - lds32f(tDlt + qc * 4)) : 0.f;
@@ -357,11 +397,16 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 // (whole 64-query tiles, 16-byte aligned, for the backward's bulk copies); LPR = D/8 lanes cooperate on one row.  The
 // same pass zeroes the fp32 dQ accumulator (same [B,S,H,D] index space: each thread clears the 8 floats under the 8
 // bf16 it reads), so the backward needs no separate memset launch over 4*B*S*H*D bytes.
-template <int D>
+//
+// DOC: the threads of head 0 also write dstart[b, s] = s - pos[b, s] (rows of S_pad, the tail repeating the last
+// token's start) and, at each document's last token s, the query-tile end s / BQ + 1 of every key tile whose last key
+// lies in that document: exactly one document holds each key tile's last key, so each entry has one writer.
+template <int D, bool DOC>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o,
                   const float* __restrict__ lse, float* __restrict__ delta, float* __restrict__ lse2,
-                  float* __restrict__ dq_acc, int B, int S, int H, int S_pad) {
+                  float* __restrict__ dq_acc, int B, int S, int H, int S_pad, const int* __restrict__ pos,
+                  int* __restrict__ dstart, int* __restrict__ qt_end) {
   constexpr int LPR = D / 8;
   const long long rows = (long long)B * S * H;
   const long long gtid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -391,6 +436,21 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __re
     const long long bb = bs / S;
     delta[(bb * H + hh) * S_pad + s] = acc;
     lse2[(bb * H + hh) * S_pad + s] = lse[(bb * H + hh) * S + s] * kLog2e;
+    if constexpr (DOC) {
+      if (hh == 0) {
+        const int* prow = pos + bb * S;
+        const int start = max(0, s - prow[s]);
+        int* drow = dstart + bb * S_pad;
+        drow[s] = start;
+        if (s == S - 1)
+          for (int x = S; x < S_pad; ++x) drow[x] = start;
+        if (s == S - 1 || prow[s + 1] == 0) {  // s ends its document
+          const int n_kt = (S + BKV - 1) / BKV;
+          const int kt_hi = s == S - 1 ? n_kt - 1 : (s + 1) / BKV - 1;  // last key tile whose last key is <= s
+          for (int kt = start / BKV; kt <= kt_hi; ++kt) qt_end[bb * n_kt + kt] = s / BQ + 1;
+        }
+      }
+    }
   }
 }
 
@@ -409,11 +469,11 @@ f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ ds
   }
 }
 
-template <int D>
+template <int D, bool DOC>
 int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmDO,
                const CUtensorMap& tmDQ, const BwdArgs& a, cudaStream_t stream) {
-  using Cfg = BwdCfg<D>;
-  auto kern = attn_bwd_kernel<D>;
+  using Cfg = BwdCfg<D, DOC>;
+  auto kern = attn_bwd_kernel<D, DOC>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -444,9 +504,17 @@ size_t attn_bwd_workspace_bytes(int B, int S, int H, int Hk, int D) {
   return al256((size_t)B * S * H * D * 4) + 2 * al256((size_t)B * H * pad_q(S) * 4);
 }
 
-int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
-             const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
-             float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+// the document variant adds the [B, S_pad] document starts and the [B, n_kt] query-tile ends
+size_t attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return attn_bwd_workspace_bytes(B, S, H, Hk, D) + al256((size_t)B * pad_q(S) * 4) +
+         al256((size_t)B * ((S + BKV - 1) / BKV) * 4);
+}
+
+namespace {
+
+int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                  const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                  int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
   // dk / dv rows may be strided: dkv_row_heads heads per token row (0 = Hk, i.e. contiguous [B,S,Hk,D]).
   // With dk = base, dv = base + Hk*D and dkv_row_heads = 2*Hk both land in ONE [B,S,2*Hk*D] buffer, which lets
   // the k/v projections' dgrad and wgrad run as single GEMMs over the concatenated weight.
@@ -455,9 +523,9 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_bwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_bwd: head_dim %d unsupported (64 or 128)", D);
-  if (ws_bytes < attn_bwd_workspace_bytes(B, S, H, Hk, D)) {
-    set_error("attn_bwd: workspace too small (%zu < %zu)", ws_bytes,
-              attn_bwd_workspace_bytes(B, S, H, Hk, D));
+  const size_t need = pos ? attn_bwd_doc_workspace_bytes(B, S, H, Hk, D) : attn_bwd_workspace_bytes(B, S, H, Hk, D);
+  if (ws_bytes < need) {
+    set_error("attn_bwd: workspace too small (%zu < %zu)", ws_bytes, need);
     return B200_ERR_WORKSPACE;
   }
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 255u) == 0, "attn_bwd: workspace must be 256-byte aligned");
@@ -466,18 +534,19 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
                  "attn_bwd: q/k/v/o/do must be 16-byte aligned");
   float* dq_acc = reinterpret_cast<float*>(ws);
   const int S_pad = pad_q(S);
+  const int n_kt = (S + BKV - 1) / BKV;
   float* delta = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + al256((size_t)B * S * H * D * 4));
   float* lse2 = reinterpret_cast<float*>(reinterpret_cast<char*>(delta) + al256((size_t)B * H * S_pad * 4));
+  int* dstart = reinterpret_cast<int*>(reinterpret_cast<char*>(lse2) + al256((size_t)B * H * S_pad * 4));
+  int* qt_end = reinterpret_cast<int*>(reinterpret_cast<char*>(dstart) + al256((size_t)B * S_pad * 4));
   const long long n = (long long)B * S * H * D;
   {
     const long long threads = (long long)B * S * H * (D / 8);
     const int blocks = (int)((threads + 255) / 256);
-    if (D == 64)
-      attn_delta_kernel<64><<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, lse, delta,
-                                                        lse2, dq_acc, B, S, H, S_pad);
-    else
-      attn_delta_kernel<128><<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, lse, delta,
-                                                         lse2, dq_acc, B, S, H, S_pad);
+    auto delta_kern = D == 64 ? (pos ? attn_delta_kernel<64, true> : attn_delta_kernel<64, false>)
+                              : (pos ? attn_delta_kernel<128, true> : attn_delta_kernel<128, false>);
+    delta_kern<<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, lse, delta, lse2,
+                                           dq_acc, B, S, H, S_pad, pos, dstart, qt_end);
     B200_CHECK_LAUNCH();
   }
   CUtensorMap tmQ, tmK, tmV, tmDO, tmDQ;
@@ -500,9 +569,15 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
   a.dkv_rh = dkv_row_heads;
   a.scale = scale;
   a.causal = causal;
-  a.paired = causal && ((S + BKV - 1) / BKV) % 2 == 0;
-  rc = D == 64 ? launch_bwd<64>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
-               : launch_bwd<128>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
+  a.paired = causal && !pos && n_kt % 2 == 0;
+  a.dstart = pos ? dstart : nullptr;
+  a.qt_end = pos ? qt_end : nullptr;
+  if (pos)
+    rc = D == 64 ? launch_bwd<64, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+                 : launch_bwd<128, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
+  else
+    rc = D == 64 ? launch_bwd<64, false>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+                 : launch_bwd<128, false>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
   if (rc) return rc;
   {
     const long long nvec = n / 8;
@@ -513,6 +588,25 @@ int attn_bwd(const void* q, const void* k, const void* v, const void* o, const v
     B200_CHECK_LAUNCH();
   }
   return B200_OK;
+}
+
+}  // namespace
+
+int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
+             const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
+             float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  return attn_bwd_impl(q, k, v, o, d_o, lse, nullptr, dq, dk, dv, B, S, H, Hk, D, scale, causal, dkv_row_heads, ws,
+                       ws_bytes, stream);
+}
+
+// document-causal backward: query s of row b sees keys s - pos[b, s] .. s
+int attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                 const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                 int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
+                 "attn_bwd_doc: pos must be a non-null, 4-byte aligned int32 [B, S] array");
+  return attn_bwd_impl(q, k, v, o, d_o, lse, pos, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads, ws, ws_bytes,
+                       stream);
 }
 
 }  // namespace b200

@@ -11,6 +11,12 @@
 //   warpgroups 0-1  64 query rows each: S = Q K^T as wgmma.m64n128k16 with both operands in shared memory,
 //                   online softmax on the fp32 accumulators in registers, then O += P V as wgmma with P as the
 //                   register A operand (the accumulator fragment packed to bf16) and V read MN-major from smem.
+//
+// Document variant (DOC = true, packed sequences): pos[b, s] is token s's position within its document, so query q
+// sees keys q - pos[q] .. q.  The key loop starts at the tile of the CTA's first query's document start (doc starts
+// are monotone in q, so that is the lowest start of the CTA's rows) and the extra `key < q - pos[q]` mask runs only
+// on tiles below the CTA's highest document start.  Rows with no visible key in a tile pass through the online
+// softmax as the causal rows do (m_use).  DOC = false compiles to the causal / non-causal kernel unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -41,6 +47,7 @@ struct FwdArgs {
   int B, S, H, Hk;
   float scale;
   int causal;
+  const int* pos;  // [B, S] positions within documents (DOC kernels only)
 };
 
 template <int D>
@@ -49,7 +56,7 @@ __device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db)
   else wgmma_m64n64k16_rs<1>(o, a, db);
 }
 
-template <int D>
+template <int D, bool DOC>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdArgs p) {
@@ -65,6 +72,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_kv_all = (p.S + ATT_BKV - 1) / ATT_BKV;
   const int n_kv = p.causal ? min(n_kv_all, (q0 + ATT_BQ - 1) / ATT_BKV + 1) : n_kv_all;
+  // first key tile: the start of the first query's document (0 without documents)
+  int j0 = 0;
+  if constexpr (DOC) j0 = max(0, q0 - __ldg(p.pos + (long long)b * p.S + q0)) / ATT_BKV;
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
@@ -83,9 +93,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       tma_prefetch_desc(&tmV);
       mbar_arrive_expect_tx(q_full, Cfg::Q_BYTES);
       for (int nb = 0; nb < Cfg::NB; ++nb) tma_load_4d(sQ + nb * ATT_BQ * 128, &tmQ, q_full, nb * 64, h, q0, b);
-      for (int j = 0; j < n_kv; ++j) {
-        const int s = j & 1;
-        mbar_wait(kv_empty0 + 8 * s, ((j >> 1) & 1) ^ 1u);
+      for (int j = j0; j < n_kv; ++j) {
+        const int s = (j - j0) & 1;
+        mbar_wait(kv_empty0 + 8 * s, (((j - j0) >> 1) & 1) ^ 1u);
         const uint32_t full = kv_full0 + 8 * s;
         mbar_arrive_expect_tx(full, 2 * Cfg::KV_BYTES);
         for (int nb = 0; nb < Cfg::NB; ++nb) {
@@ -104,11 +114,23 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
   const float sl2 = p.scale * kLog2e;
   const int row_a = q0 + wg * 64 + wq * 16 + (lane >> 2);  // this thread's rows: row_a, row_a + 8
+  // DOC: document start of each of this thread's rows, and the highest start of the CTA's rows (its last row's)
+  int dstart[2] = {0, 0}, dstart_hi = 0;
+  if constexpr (DOC) {
+    const int* prow = p.pos + (long long)b * p.S;
+    const int q_hi = min(q0 + ATT_BQ, p.S) - 1;
+    dstart_hi = q_hi - __ldg(prow + q_hi);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = row_a + 8 * r;
+      dstart[r] = row < p.S ? row - __ldg(prow + row) : 0;
+    }
+  }
   mbar_wait(q_full, 0);
 
-  for (int j = 0; j < n_kv; ++j) {
-    const int s = j & 1;
-    mbar_wait(kv_full0 + 8 * s, (j >> 1) & 1);
+  for (int j = j0; j < n_kv; ++j) {
+    const int s = (j - j0) & 1;
+    mbar_wait(kv_full0 + 8 * s, ((j - j0) >> 1) & 1);
     const uint32_t tK = sK + s * Cfg::KV_BYTES, tV = sV + s * Cfg::KV_BYTES;
     const int k0 = j * ATT_BKV;
 
@@ -125,6 +147,19 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     }
     wgmma_commit();
     wgmma_wait<0>();
+
+    if constexpr (DOC) {
+      if (k0 < dstart_hi) {  // the tile reaches below some row's document start
+#pragma unroll
+        for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
+            if (key < dstart[e >> 1]) sc[4 * nc + e] = -INFINITY;
+          }
+        }
+      }
+    }
 
     // scale (log2 domain), mask, online softmax; accumulator chunk nc holds keys 8 nc + 2 (lane % 4) + {0, 1}
     float mx[2] = {-INFINITY, -INFINITY};
@@ -208,11 +243,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-template <int D>
+template <int D, bool DOC>
 int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
                cudaStream_t stream) {
   using Cfg = FwdCfg<D>;
-  auto kern = attn_fwd_kernel<D>;
+  auto kern = attn_fwd_kernel<D, DOC>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -234,8 +269,10 @@ int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, in
   return make_tensor_map(tm, base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, 4, dims, strides, box, true);
 }
 
-int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int H,
-             int Hk, int D, float scale, int causal, cudaStream_t stream) {
+namespace {
+
+int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B, int S,
+                  int H, int Hk, int D, float scale, int causal, cudaStream_t stream) {
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_fwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd: head_dim %d unsupported (64 or 128; pad smaller dims)", D);
@@ -254,7 +291,24 @@ int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, i
   a.Hk = Hk;
   a.scale = scale;
   a.causal = causal;
-  return D == 64 ? launch_fwd<64>(tmQ, tmK, tmV, a, stream) : launch_fwd<128>(tmQ, tmK, tmV, a, stream);
+  a.pos = pos;
+  if (pos) return D == 64 ? launch_fwd<64, true>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, true>(tmQ, tmK, tmV, a, stream);
+  return D == 64 ? launch_fwd<64, false>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, false>(tmQ, tmK, tmV, a, stream);
+}
+
+}  // namespace
+
+int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int H,
+             int Hk, int D, float scale, int causal, cudaStream_t stream) {
+  return attn_fwd_impl(q, k, v, o, lse, nullptr, B, S, H, Hk, D, scale, causal, stream);
+}
+
+// document-causal: query s of row b sees keys s - pos[b, s] .. s
+int attn_fwd_doc(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B, int S,
+                 int H, int Hk, int D, float scale, cudaStream_t stream) {
+  B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
+                 "attn_fwd_doc: pos must be a non-null, 4-byte aligned int32 [B, S] array");
+  return attn_fwd_impl(q, k, v, o, lse, pos, B, S, H, Hk, D, scale, 1, stream);
 }
 
 }  // namespace b200

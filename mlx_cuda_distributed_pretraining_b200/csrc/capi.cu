@@ -94,6 +94,8 @@ int add_rmsnorm_bwd(const void* dy, const void* dres, const void* x, const void*
                     cudaStream_t stream);
 int rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, int S, int NH,
          int D, int backward, int is_bf16, cudaStream_t stream);
+int rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
+             int D, int backward, int is_bf16, cudaStream_t stream);
 int glu_fwd(const void* g, const void* u, void* y, long long n, cudaStream_t stream);
 int glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, cudaStream_t stream);
 int ce_fwd(const void* logits, long long ld, const long long* targets, int rows, int V, long long pad_token,
@@ -106,6 +108,12 @@ size_t attn_bwd_workspace_bytes(int B, int S, int H, int Hk, int D);
 int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
              const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
              float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
+int attn_fwd_doc(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B, int S,
+                 int H, int Hk, int D, float scale, cudaStream_t stream);
+size_t attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D);
+int attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                 const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                 int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D);
 int attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse, int B,
                 int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes,
@@ -343,6 +351,10 @@ int b200_rope(const void* x, void* y, const float* cos_t, const float* sin_t, in
               int D, int backward, int is_bf16, void* stream) {
   return b200::rope(x, y, cos_t, sin_t, B, S, NH, D, backward, is_bf16, S_(stream));
 }
+int b200_rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S,
+                  int NH, int D, int backward, int is_bf16, void* stream) {
+  return b200::rope_pos(x, y, cos_t, sin_t, pos, B, S, NH, D, backward, is_bf16, S_(stream));
+}
 int b200_glu_fwd(const void* g, const void* u, void* y, long long n, void* stream) {
   return b200::glu_fwd(g, u, y, n, S_(stream));
 }
@@ -377,6 +389,19 @@ int b200_attn_bwd_strided(const void* q, const void* k, const void* v, const voi
                           size_t workspace_bytes, void* stream) {
   return b200::attn_bwd(q, k, v, o, d_o, lse, dq, dk, dv, B, S, H, Hk, D, scale, causal, dkv_row_heads,
                         workspace, workspace_bytes, S_(stream));
+}
+int b200_attn_fwd_doc(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B,
+                      int S, int H, int Hk, int D, float scale, void* stream) {
+  return b200::attn_fwd_doc(q, k, v, o, lse, pos, B, S, H, Hk, D, scale, S_(stream));
+}
+size_t b200_attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return b200::attn_bwd_doc_workspace_bytes(B, S, H, Hk, D);
+}
+int b200_attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                      const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                      int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream) {
+  return b200::attn_bwd_doc(q, k, v, o, d_o, lse, pos, dq, dk, dv, B, S, H, Hk, D, scale, dkv_row_heads, workspace,
+                            workspace_bytes, S_(stream));
 }
 
 size_t b200_attn_decode_workspace_bytes(int B, int H, int s_max, int D) {

@@ -432,17 +432,21 @@ __global__ void __launch_bounds__(1024) rmsnorm_dw_reduce_batched_kernel(const _
 }
 
 // x: [B, S, NH, D]; cos/sin: [S, D/2] fp32. out[2i] = x[2i]*c - x[2i+1]*s ; out[2i+1] = x[2i]*s +
-// x[2i+1]*c. The backward pass is the same rotation with sign = -1.
-template <typename T>
+// x[2i+1]*c. The backward pass is the same rotation with sign = -1.  POS: token s of row b is rotated by the angle of
+// pos[b, s] (its position within its document) instead of s.
+template <typename T, bool POS>
 __global__ void __launch_bounds__(256)
 rope_kernel(const T* __restrict__ x, T* __restrict__ y, const float* __restrict__ cos_t,
-            const float* __restrict__ sin_t, long long nvec, int S, int NH, int D, float sign) {
+            const float* __restrict__ sin_t, long long nvec, int S, int NH, int D, float sign,
+            const int* __restrict__ pos) {
   const int vec_per_head = D / 8;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec;
        i += (long long)gridDim.x * blockDim.x) {
     const int dv = (int)(i % vec_per_head);
     const long long t = i / vec_per_head / NH;  // token index b*S + s
-    const int s = (int)(t % S);
+    int s;
+    if constexpr (POS) s = __ldg(pos + t);
+    else s = (int)(t % S);
     float xv[8], o[8];
     ld8(x + i * 8, xv);
     const float4 c = *reinterpret_cast<const float4*>(cos_t + (long long)s * (D / 2) + dv * 4);
@@ -606,8 +610,10 @@ int rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd,
   return add_rmsnorm_bwd(dy, nullptr, x, w, rstd, dx, dw, rows, H, is_bf16, ws, ws_bytes, stream);
 }
 
-int rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, int S, int NH,
-         int D, int backward, int is_bf16, cudaStream_t stream) {
+namespace {
+
+int rope_impl(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
+              int D, int backward, int is_bf16, cudaStream_t stream) {
   B200_CHECK_ARG(B > 0 && S > 0 && NH > 0 && D > 0 && D % 8 == 0, "rope: D=%d must be a multiple of 8",
                  D);
   B200_CHECK_ARG(al16(x) && al16(y) && al16(cos_t) && al16(sin_t), "rope: alignment");
@@ -615,14 +621,34 @@ int rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, 
   long long blocks = (nvec + 255) / 256;
   if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
   const float sign = backward ? -1.0f : 1.0f;
-  if (is_bf16)
-    rope_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, stream>>>(
-        (const __nv_bfloat16*)x, (__nv_bfloat16*)y, cos_t, sin_t, nvec, S, NH, D, sign);
-  else
-    rope_kernel<float><<<(int)blocks, 256, 0, stream>>>((const float*)x, (float*)y, cos_t, sin_t,
-                                                        nvec, S, NH, D, sign);
+  auto launch = [&](auto kern, auto* xx, auto* yy) {
+    kern<<<(int)blocks, 256, 0, stream>>>(xx, yy, cos_t, sin_t, nvec, S, NH, D, sign, pos);
+  };
+  using bf = __nv_bfloat16;
+  if (is_bf16) {
+    if (pos) launch(rope_kernel<bf, true>, (const bf*)x, (bf*)y);
+    else launch(rope_kernel<bf, false>, (const bf*)x, (bf*)y);
+  } else {
+    if (pos) launch(rope_kernel<float, true>, (const float*)x, (float*)y);
+    else launch(rope_kernel<float, false>, (const float*)x, (float*)y);
+  }
   B200_CHECK_LAUNCH();
   return B200_OK;
+}
+
+}  // namespace
+
+int rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, int S, int NH,
+         int D, int backward, int is_bf16, cudaStream_t stream) {
+  return rope_impl(x, y, cos_t, sin_t, nullptr, B, S, NH, D, backward, is_bf16, stream);
+}
+
+// pos: int32 [B, S]; the tables must cover max(pos) + 1 rows
+int rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
+             int D, int backward, int is_bf16, cudaStream_t stream) {
+  B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
+                 "rope_pos: pos must be a non-null, 4-byte aligned int32 [B, S] array");
+  return rope_impl(x, y, cos_t, sin_t, pos, B, S, NH, D, backward, is_bf16, stream);
 }
 
 }  // namespace b200

@@ -601,31 +601,49 @@ def rope_tables(seq_len: int, head_dim: int, theta: float, device) -> Tuple[torc
     return torch.cos(ang).to(device).contiguous(), torch.sin(ang).to(device).contiguous()
 
 
+def _rope_call(x, y, cos_t, sin_t, pos, backward: int, what: str) -> None:
+    B, S, NH, D = x.shape
+    if pos is None:
+        check(lib().b200_rope(x.data_ptr(), y.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), B, S,
+                              NH, D, backward, _is_bf16(x, "x"), _stream()), what)
+    else:
+        check(lib().b200_rope_pos(x.data_ptr(), y.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), pos.data_ptr(), B,
+                                  S, NH, D, backward, _is_bf16(x, "x"), _stream()), what)
+
+
 class _RopeFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, cos_t, sin_t):
+    def forward(ctx, x, cos_t, sin_t, pos):
         xs = x.contiguous()
-        B, S, NH, D = xs.shape
         y = torch.empty_like(xs)
-        check(lib().b200_rope(xs.data_ptr(), y.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), B, S,
-                              NH, D, 0, _is_bf16(xs, "x"), _stream()), "b200_rope")
-        ctx.save_for_backward(cos_t, sin_t)
+        _rope_call(xs, y, cos_t, sin_t, pos, 0, "b200_rope")
+        ctx.save_for_backward(cos_t, sin_t, pos)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        cos_t, sin_t = ctx.saved_tensors
+        cos_t, sin_t, pos = ctx.saved_tensors
         dy = dy.contiguous()
-        B, S, NH, D = dy.shape
         dx = torch.empty_like(dy)
-        check(lib().b200_rope(dy.data_ptr(), dx.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), B, S,
-                              NH, D, 1, _is_bf16(dy, "dy"), _stream()), "b200_rope(bwd)")
-        return dx, None, None
+        _rope_call(dy, dx, cos_t, sin_t, pos, 1, "b200_rope(bwd)")
+        return dx, None, None, None
 
 
-def rope(x: torch.Tensor, cos_t: torch.Tensor, sin_t: torch.Tensor) -> torch.Tensor:
-    """x: [B, S, heads, D]; interleaved-pair rotation."""
-    return _RopeFn.apply(x, cos_t, sin_t)
+def _check_pos(pos: torch.Tensor, x: torch.Tensor, what: str) -> torch.Tensor:
+    """pos: int32 [B, S] positions within documents on x's device (x: [B, S, ...])."""
+    if pos.dtype != torch.int32 or pos.dim() != 2 or tuple(pos.shape) != tuple(x.shape[:2]):
+        raise ValueError(f"{what}: pos must be int32 [B, S] = {list(x.shape[:2])}, got {pos.dtype} {list(pos.shape)}")
+    if pos.device != x.device:
+        raise ValueError(f"{what}: pos is on {pos.device}, the operands on {x.device}")
+    return pos.contiguous()
+
+
+def rope(x: torch.Tensor, cos_t: torch.Tensor, sin_t: torch.Tensor, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x: [B, S, heads, D]; interleaved-pair rotation of token s by the angle of position s, or of pos[b, s] (int32
+    [B, S], the position within its document; the tables must then hold max(pos) + 1 rows) when pos is given."""
+    if pos is not None:
+        pos = _check_pos(pos, x, "rope")
+    return _RopeFn.apply(x, cos_t, sin_t, pos)
 
 
 def _pad_head_dim(D: int) -> int:
@@ -636,8 +654,9 @@ def _pad_head_dim(D: int) -> int:
     raise ValueError(f"attention: head_dim {D} > 128 is not supported")
 
 
-def attention_fwd_raw(q, k, v, scale: float, causal: bool):
-    """q [B,S,H,D], k/v [B,S,Hk,D] bf16 contiguous, D in {64,128}. Returns (o, lse[B,H,S])."""
+def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.Tensor] = None):
+    """q [B,S,H,D], k/v [B,S,Hk,D] bf16 contiguous, D in {64,128}. Returns (o, lse[B,H,S]).  With pos (int32 [B,S]
+    contiguous, positions within documents) the mask is document-causal and `causal` is ignored."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         _need(t, torch.bfloat16, nm)
     B, S, H, D = q.shape
@@ -645,13 +664,17 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool):
     o = torch.empty_like(q)
     lse = torch.empty((B, H, S), device=q.device, dtype=torch.float32)
     tok = _t0("attn_fwd")
-    check(lib().b200_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
-                              B, S, H, Hk, D, float(scale), int(causal), _stream()), "b200_attn_fwd")
+    if pos is None:
+        check(lib().b200_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+                                  B, S, H, Hk, D, float(scale), int(causal), _stream()), "b200_attn_fwd")
+    else:
+        check(lib().b200_attn_fwd_doc(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+                                      pos.data_ptr(), B, S, H, Hk, D, float(scale), _stream()), "b200_attn_fwd_doc")
     _t1(tok)
     return o, lse
 
 
-def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool):
+def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Optional[torch.Tensor] = None):
     B, S, H, D = q.shape
     Hk = k.shape[2]
     dq = torch.empty_like(q)
@@ -659,41 +682,49 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool):
     # k/v projections' backward can then treat [dk | dv] as ONE matrix against the concatenated weight
     dkv = torch.empty((B, S, 2 * Hk, D), device=k.device, dtype=k.dtype)
     dk, dv = dkv[:, :, :Hk], dkv[:, :, Hk:]
-    nbytes = int(lib().b200_attn_bwd_workspace_bytes(B, S, H, Hk, D))
-    ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
     tok = _t0("attn_bwd")
-    check(lib().b200_attn_bwd_strided(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
-                                      lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H,
-                                      Hk, D, float(scale), int(causal), 2 * Hk, ws.data_ptr(), ws.numel(),
-                                      _stream()), "b200_attn_bwd_strided")
+    if pos is None:
+        nbytes = int(lib().b200_attn_bwd_workspace_bytes(B, S, H, Hk, D))
+        ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
+        check(lib().b200_attn_bwd_strided(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                          lse.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H,
+                                          Hk, D, float(scale), int(causal), 2 * Hk, ws.data_ptr(), ws.numel(),
+                                          _stream()), "b200_attn_bwd_strided")
+    else:
+        nbytes = int(lib().b200_attn_bwd_doc_workspace_bytes(B, S, H, Hk, D))
+        ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
+        check(lib().b200_attn_bwd_doc(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                      lse.data_ptr(), pos.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B,
+                                      S, H, Hk, D, float(scale), 2 * Hk, ws.data_ptr(), ws.numel(), _stream()),
+              "b200_attn_bwd_doc")
     _t1(tok)
     return dq, dk, dv
 
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal):
+    def forward(ctx, q, k, v, scale, causal, pos):
         D = q.shape[-1]
         Dp = _pad_head_dim(D)
         if Dp != D:  # zero-padding the head dim leaves QK^T and the first D columns of PV unchanged
             q, k, v = (torch.nn.functional.pad(t, (0, Dp - D)) for t in (q, k, v))
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        o, lse = attention_fwd_raw(q, k, v, scale, causal)
-        ctx.save_for_backward(q, k, v, o, lse)
+        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos)
+        ctx.save_for_backward(q, k, v, o, lse, pos)
         ctx.scale, ctx.causal, ctx.D = scale, causal, D
         return o[..., :D] if Dp != D else o
 
     @staticmethod
     def backward(ctx, do):
-        q, k, v, o, lse = ctx.saved_tensors
+        q, k, v, o, lse, pos = ctx.saved_tensors
         Dp = q.shape[-1]
         if Dp != ctx.D:
             do = torch.nn.functional.pad(do, (0, Dp - ctx.D))
         do = do.contiguous()
-        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal)
+        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos)
         if Dp != ctx.D:
             dq, dk, dv = dq[..., :ctx.D], dk[..., :ctx.D], dv[..., :ctx.D]
-        return dq, dk, dv, None, None
+        return dq, dk, dv, None, None, None
 
 
 def _hi_lo(x: torch.Tensor):
@@ -715,7 +746,7 @@ class _AttentionX3Fn(torch.autograd.Function):
     to fp32-like accuracy; P and the kernel outputs still pass through one bf16 rounding each."""
 
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal):
+    def forward(ctx, q, k, v, scale, causal, pos):
         D = q.shape[-1]
         Dp = _pad_head_dim(3 * D)
         (qh, ql), (kh, kl), (vh, vl) = _hi_lo(q), _hi_lo(k), _hi_lo(v)
@@ -724,42 +755,50 @@ class _AttentionX3Fn(torch.autograd.Function):
             t = torch.cat([a, b, c], dim=-1)
             return (torch.nn.functional.pad(t, (0, Dp - 3 * D)) if Dp != 3 * D else t).contiguous()
         q3, k3, v3 = cat3(qh, ql, qh), cat3(kh, kh, kl), cat3(vh, vh, vl)
-        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal)
-        ctx.save_for_backward(q3, k3, v3, o3, lse)
+        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos)
+        ctx.save_for_backward(q3, k3, v3, o3, lse, pos)
         ctx.scale, ctx.causal, ctx.D, ctx.Dp = scale, causal, D, Dp
         return o3[..., :D].float() + o3[..., 2 * D:3 * D].float()
 
     @staticmethod
     def backward(ctx, do):
-        q3, k3, v3, o3, lse = ctx.saved_tensors
+        q3, k3, v3, o3, lse, pos = ctx.saved_tensors
         D, Dp = ctx.D, ctx.Dp
         gh, gl = _hi_lo(do.float())
         g3 = torch.cat([gh, gl, gh], dim=-1)
         if Dp != 3 * D:
             g3 = torch.nn.functional.pad(g3, (0, Dp - 3 * D))
-        dq3, dk3, dv3 = attention_bwd_raw(q3, k3, v3, o3, g3.contiguous(), lse, ctx.scale, ctx.causal)
+        dq3, dk3, dv3 = attention_bwd_raw(q3, k3, v3, o3, g3.contiguous(), lse, ctx.scale, ctx.causal, pos)
         dq = dq3[..., :D].float() + dq3[..., 2 * D:3 * D].float()
         dk = dk3[..., :D].float() + dk3[..., D:2 * D].float()
         dv = dv3[..., :D].float() + dv3[..., D:2 * D].float()
-        return dq, dk, dv, None, None
+        return dq, dk, dv, None, None, None
 
 
 def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
-                   causal: bool = True) -> torch.Tensor:
-    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42."""
+                   causal: bool = True, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos: as attention."""
     if 3 * q.shape[-1] > 128:
         raise ValueError("attention_fp32: head_dim must be <= 42 (three bf16 copies must fit a 128-wide tile)")
     if scale is None:
         scale = q.shape[-1] ** -0.5
-    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal))
+    if pos is not None:
+        pos, causal = _check_pos(pos, q, "attention_fp32"), True
+    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos)
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
-              causal: bool = True) -> torch.Tensor:
-    """softmax(q k^T * scale + causal_mask) v with GQA head sharing; [B,S,H,D] layout, bf16."""
+              causal: bool = True, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """softmax(q k^T * scale + causal_mask) v with GQA head sharing; [B,S,H,D] layout, bf16.
+
+    pos (int32 [B, S]) packs several documents per row: pos[b, s] is token s's position within its document (0 at a
+    document's first token, +1 per token inside it), and query s sees only keys s - pos[b, s] .. s -- the causal
+    attention of each document run alone.  It implies causal."""
     if scale is None:
         scale = q.shape[-1] ** -0.5
-    return _AttentionFn.apply(q, k, v, float(scale), bool(causal))
+    if pos is not None:
+        pos, causal = _check_pos(pos, q, "attention"), True
+    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos)
 
 
 # ------------------------------------------------------------------------------------------------
