@@ -353,6 +353,19 @@ size_t b200_attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D);
 int b200_attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                       const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
                       int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
+/* Sliding-window causal attention, with or without packed documents: query s sees key k iff
+ * 0 <= s - k <= min(pos[b,s], window), i.e. at most window + 1 keys, itself included (the sliding causal window of
+ * the reference's FlexAttention example, README-FlexAttention.md:47-59, with its block mask skipping whole tiles,
+ * arch/flex_attention.py:90-139).  pos is as for b200_attn_fwd_doc, or NULL for one document per row
+ * (pos[b,s] = s); window >= 0, and window >= S - 1 gives the causal / document-causal mask.  Key and query tiles
+ * outside every row's window are skipped, so the cost grows linearly in S.  The backward's workspace is
+ * b200_attn_bwd_window_workspace_bytes (equal to the document variant's). */
+int b200_attn_fwd_window(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                         int B, int S, int H, int Hk, int D, float scale, void* stream);
+size_t b200_attn_bwd_window_workspace_bytes(int B, int S, int H, int Hk, int D);
+int b200_attn_bwd_window(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                         const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
+                         float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- generation: decode attention over a KV cache (arch/flash_attention.py:97-156, last query row) ------------
  * One new query per sequence against its cached keys, causal by construction (every cached key precedes it):
@@ -368,6 +381,13 @@ size_t b200_attn_decode_workspace_bytes(int B, int H, int s_max, int D);
 int b200_attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                      int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* workspace,
                      size_t workspace_bytes, void* stream);
+/* b200_attn_decode under a sliding window (README-FlexAttention.md:47-59): the query at position p = lens[b] - 1
+ * sees cached keys max(0, p - window) .. p only, window >= 0.  Chunks wholly below the window are skipped and
+ * never read; chunk boundaries and the merge order depend on lens[b] and window alone, so a row's output is still
+ * bit-identical alone or in any batch.  Same workspace as b200_attn_decode. */
+int b200_attn_decode_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o,
+                            float* lse, int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
+                            void* workspace, size_t workspace_bytes, void* stream);
 /* Appends one token per row at pos = lens[b] - 1: k_cache[b,pos] = rot(k[b]), v_cache[b,pos] = v[b] (k, v:
  * [B,Hk,D]).  With cos_t/sin_t (f32 [>= max pos + 1, D/2], ops.rope_tables) the interleaved-pair rotation of
  * b200_rope (arch/llama_standard.py:90-131) is applied to k and, in place, to q [B,H,D], with b200_rope's exact

@@ -14,29 +14,46 @@ from torch import nn
 from .. import ops
 
 
+def _window(window: Optional[int]) -> Optional[int]:
+    if window is not None and (isinstance(window, bool) or not isinstance(window, int) or window < 0):
+        raise ValueError(f"sliding window must be None or a non-negative int, got {window!r}")
+    return window
+
+
 class CausalMask:
     """Marker for the additive causal mask the reference builds in arch/llama.py:384-387
-    (-inf strictly above the diagonal).  The fused kernel applies it implicitly."""
+    (-inf strictly above the diagonal).  The fused kernel applies it implicitly.
 
-    def __init__(self, seq_len: int):
+    window (optional int >= 0): the sliding causal window of the reference's FlexAttention example
+    (README-FlexAttention.md:47-59): query q sees key k iff 0 <= q - k <= window."""
+
+    def __init__(self, seq_len: int, window: Optional[int] = None):
         self.seq_len = seq_len
+        self.window = _window(window)
 
     def dense(self, dtype=torch.float32, device="cpu") -> torch.Tensor:
         m = torch.full((self.seq_len, self.seq_len), float("-inf"), dtype=dtype, device=device)
-        return torch.triu(m, diagonal=1)[None, None]
+        m = torch.triu(m, diagonal=1)
+        if self.window is not None:
+            m = m + torch.tril(torch.full_like(m, float("-inf")), diagonal=-self.window - 1)
+        return m[None, None]
 
 
 class DocumentCausalMask:
     """Marker for the document-causal mask of packed rows: pos (int32 [B, S]) is each token's position within its
     document (0 at a document's first token, +1 per token inside it), and query q sees key k iff
     q - pos[q] <= k <= q -- the causal mask of every document run alone.  The fused document kernels apply it
-    implicitly, and RoPE rotates by pos."""
+    implicitly, and RoPE rotates by pos.
 
-    def __init__(self, pos: torch.Tensor):
+    window (optional int >= 0) intersects it with the sliding window 0 <= q - k <= window, which is the same mask
+    with pos clamped at window.  RoPE still rotates by the unclamped pos."""
+
+    def __init__(self, pos: torch.Tensor, window: Optional[int] = None):
         if pos.dim() != 2:
             raise ValueError(f"DocumentCausalMask: pos must be [B, S], got {list(pos.shape)}")
         self.pos = pos.to(torch.int32).contiguous()
         self.seq_len = pos.shape[1]
+        self.window = _window(window)
 
     def dense(self, dtype=torch.float32, device="cpu") -> torch.Tensor:
         """The additive [B, 1, S, S] mask (0 where visible, -inf elsewhere)."""
@@ -44,6 +61,8 @@ class DocumentCausalMask:
         s = torch.arange(self.seq_len, device=device)
         q, k = s[:, None], s[None, :]
         ok = (k <= q) & (k >= (s - pos)[:, :, None])
+        if self.window is not None:
+            ok = ok & (q - k <= self.window)
         m = torch.zeros(ok.shape, dtype=dtype, device=device).masked_fill(~ok, float("-inf"))
         return m[:, None]
 
@@ -70,13 +89,13 @@ class FlashAttention(nn.Module):
 
     def _flash_attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask=None) -> torch.Tensor:
         """q [B,S,H,D], k/v [B,S,Hk,D] -> [B,S,H,D]."""
-        pos = None
+        pos = window = None
         if mask is None:
             causal = False
         elif isinstance(mask, CausalMask):
-            causal = True
+            causal, window = True, mask.window
         elif isinstance(mask, DocumentCausalMask):
-            causal, pos = True, mask.pos
+            causal, pos, window = True, mask.pos, mask.window
         else:
             raise NotImplementedError(
                 "the fused kernel supports mask=None, the causal mask (CausalMask) or the document-causal mask of "
@@ -85,10 +104,10 @@ class FlashAttention(nn.Module):
         if dt == torch.float32 and 3 * self.head_dim <= 128:
             # full-precision configs (mixed_precision: false, e.g. BASELINE C1, head_dim 16): logits through
             # three-term bf16 products (hi/lo split operands), ~fp32-accurate scores on the same kernels
-            return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos)
+            return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos, window=window)
         if dt != torch.bfloat16:  # larger head dims: bf16 operands with fp32 accumulation (stated in DESIGN.md)
             q, k, v = q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
-        o = ops.attention(q, k, v, self.scale, causal, pos=pos)
+        o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window)
         return o if dt == torch.bfloat16 else o.to(dt)
 
     def forward(self, x: torch.Tensor, mask=None) -> torch.Tensor:
@@ -137,14 +156,15 @@ class FlashAttention(nn.Module):
         return self._out(ctx.reshape(B, S, self.num_heads * self.head_dim))
 
     def forward_decode(self, x: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
-                       workspace: torch.Tensor) -> torch.Tensor:
+                       workspace: torch.Tensor, window: Optional[int] = None) -> torch.Tensor:
         """One new token per row, x [B, hidden]: its k and v go to cache position lens[b] - 1 (rotated there when
-        RoPE is on), then its query attends over the row's first lens[b] cached keys."""
+        RoPE is on), then its query attends over the row's first lens[b] cached keys (the last window + 1 of them
+        with a sliding window)."""
         B = x.shape[0]
         q, k, v = self._project(x)
         q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
         k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         ops.kv_append(q, k, v, k_cache, v_cache, lens, self.rope_tables)
-        ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace)
+        ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace, window=window)
         return self._out(ctx.reshape(B, self.num_heads * self.head_dim))

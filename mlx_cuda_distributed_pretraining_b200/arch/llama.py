@@ -51,6 +51,7 @@ class ModelArgs:
     num_local_experts: int = 0
     num_experts_per_tok: int = 0
     apply_rope: bool = False  # extension; see module docstring
+    sliding_window: Optional[int] = None  # extension: query q sees keys q - W .. q in every layer (None: causal)
 
 
 class RMSNorm(nn.Module):
@@ -102,14 +103,14 @@ class AttentionModule(nn.Module):
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
         return self.attn(x, mask=mask)
 
-    def cached(self, x: torch.Tensor, cache: "KVCache", layer: int) -> torch.Tensor:
+    def cached(self, x: torch.Tensor, cache: "KVCache", layer: int, window: Optional[int] = None) -> torch.Tensor:
         """This layer's attention against the KV cache: prefill when x is [B, S, hidden], one decode step when x is
-        [B, hidden]."""
+        [B, hidden].  window: the model's sliding window (None: causal)."""
         if self.apply_rope and self.attn.rope_tables is None:
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
         if x.dim() == 3:
-            return self.attn.forward_prefill(x, CausalMask(x.shape[1]), cache.k[layer], cache.v[layer])
-        return self.attn.forward_decode(x, cache.k[layer], cache.v[layer], cache.lens, cache.workspace)
+            return self.attn.forward_prefill(x, CausalMask(x.shape[1], window), cache.k[layer], cache.v[layer])
+        return self.attn.forward_decode(x, cache.k[layer], cache.v[layer], cache.lens, cache.workspace, window)
 
 
 class TransformerBlock(nn.Module):
@@ -145,14 +146,14 @@ class TransformerBlock(nn.Module):
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
         return h, self.mlp(y)
 
-    def forward_cached(self, h: torch.Tensor, pending, cache: "KVCache", layer: int):
+    def forward_cached(self, h: torch.Tensor, pending, cache: "KVCache", layer: int, window: Optional[int] = None):
         """forward_fused with the attention run against the KV cache (AttentionModule.cached)."""
         n1, n2 = self.input_layernorm, self.post_attention_layernorm
         if pending is None:
             y = n1(h)
         else:
             h, y = ops.add_rmsnorm(h, pending, n1.weight, n1.eps)
-        a = self.self_attn.cached(y, cache, layer)
+        a = self.self_attn.cached(y, cache, layer, window)
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
         return h, self.mlp(y)
 
@@ -204,16 +205,17 @@ class Model(nn.Module):
     def hidden_states(self, inputs: torch.Tensor, position_ids=None, attention_mask=None) -> torch.Tensor:
         """position_ids (int [B, S], optional): packed rows, each token's position within its document (0 at the
         document's first token).  It selects the document-causal mask and, with RoPE on, the rotation angles, so
-        every document is computed as if it ran alone.  None keeps the causal mask over whole rows."""
+        every document is computed as if it ran alone.  None keeps the causal mask over whole rows.  Both masks carry
+        args.sliding_window."""
         B, S = inputs.shape
         if attention_mask is not None:
             mask = attention_mask
         elif position_ids is not None:
             if tuple(position_ids.shape) != (B, S):
                 raise ValueError(f"position_ids must be [B, S] = {[B, S]}, got {list(position_ids.shape)}")
-            mask = DocumentCausalMask(position_ids)
+            mask = DocumentCausalMask(position_ids, self.args.sliding_window)
         else:
-            mask = CausalMask(S)
+            mask = CausalMask(S, self.args.sliding_window)
         h = ops.embedding(inputs, self.embed_tokens.weight)
         pending = None
         for layer in self.layers:
@@ -277,7 +279,7 @@ class Model(nn.Module):
         h = ops.embedding(tokens, self.embed_tokens.weight)
         pending = None
         for i, layer in enumerate(self.layers):
-            h, pending = layer.forward_cached(h, pending, cache, i)
+            h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window)
         rows = torch.arange(B, device=tokens.device)
         last = torch.tensor([n - 1 for n in lengths], device=tokens.device)
         return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])
@@ -290,7 +292,7 @@ class Model(nn.Module):
         h = ops.embedding(tokens, self.embed_tokens.weight)
         pending = None
         for i, layer in enumerate(self.layers):
-            h, pending = layer.forward_cached(h, pending, cache, i)
+            h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window)
         return self._row_logits(h, pending)
 
     # mlx nn.Module-style accessors used by the optimizers' update(model, grads) surface

@@ -64,6 +64,12 @@ class ModelConfig:
     rope: Dict[str, Any]
     misc: Dict[str, bool]
 
+    def __post_init__(self):
+        # extension: attention.sliding_window W (absent / null: full causal); query q sees keys q - W .. q
+        w = self.attention.get("sliding_window")
+        if w is not None and (isinstance(w, bool) or not isinstance(w, int) or w < 0):
+            raise ValueError(f"model.attention.sliding_window must be null or a non-negative integer, got {w!r}")
+
 
 @dataclass
 class TrainingConfig:
@@ -651,7 +657,8 @@ class Trainer:
             use_flash_attention=m.attention.get("use_flash_attention", True),
             use_flex_attention=m.attention.get("use_flex_attention", False),
             flash_block_size=m.attention.get("flash_block_size", 128),
-            apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")))
+            apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")),
+            sliding_window=m.attention.get("sliding_window"))
         self.model_args = args
         model = Model(args)
         init_model_(model, args, self.config.system.seed)

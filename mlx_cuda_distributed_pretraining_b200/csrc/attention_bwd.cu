@@ -31,6 +31,11 @@
 // arrive with its LSE and delta; the mask `key >= q - pos[q]` joins the causal one only on items whose queries'
 // highest document start lies above the warpgroup's first key.  Document launches use the unpaired order.  DOC = false
 // compiles to the causal / non-causal kernels unchanged.
+//
+// Sliding window (same DOC kernels): query q sees keys q - min(pos[q], W) .. q, the document mask with pos clamped at W
+// (pos == nullptr reads as pos[q] = q).  Only the pre-pass knows about W: it writes the clamped starts, and bounds each
+// key tile's query range by k0 + BKV - 1 + W as well, since no later query reaches back to the tile.  The starts stay
+// monotone, so the kernel's skipping, masked-item test and binary search are unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -398,15 +403,16 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 // same pass zeroes the fp32 dQ accumulator (same [B,S,H,D] index space: each thread clears the 8 floats under the 8
 // bf16 it reads), so the backward needs no separate memset launch over 4*B*S*H*D bytes.
 //
-// DOC: the threads of head 0 also write dstart[b, s] = s - pos[b, s] (rows of S_pad, the tail repeating the last
-// token's start) and, at each document's last token s, the query-tile end s / BQ + 1 of every key tile whose last key
-// lies in that document: exactly one document holds each key tile's last key, so each entry has one writer.
+// DOC: the threads of head 0 also write dstart[b, s] = s - min(pos[b, s], window) (rows of S_pad, the tail repeating
+// the last token's start) and, at each document's last token s, the query-tile end min(s, k0 + BKV - 1 + window) / BQ
+// + 1 of every key tile (first key k0) whose last key lies in that document: exactly one document holds each key
+// tile's last key, so each entry has one writer.  pos == nullptr reads as pos[b, s] = s: one document per row.
 template <int D, bool DOC>
 __global__ void __launch_bounds__(256)
 attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __restrict__ d_o,
                   const float* __restrict__ lse, float* __restrict__ delta, float* __restrict__ lse2,
                   float* __restrict__ dq_acc, int B, int S, int H, int S_pad, const int* __restrict__ pos,
-                  int* __restrict__ dstart, int* __restrict__ qt_end) {
+                  int* __restrict__ dstart, int* __restrict__ qt_end, int window) {
   constexpr int LPR = D / 8;
   const long long rows = (long long)B * S * H;
   const long long gtid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -438,16 +444,19 @@ attn_delta_kernel(const __nv_bfloat16* __restrict__ o, const __nv_bfloat16* __re
     lse2[(bb * H + hh) * S_pad + s] = lse[(bb * H + hh) * S + s] * kLog2e;
     if constexpr (DOC) {
       if (hh == 0) {
-        const int* prow = pos + bb * S;
-        const int start = max(0, s - prow[s]);
+        const int* prow = pos ? pos + bb * S : nullptr;
+        const int ps = prow ? prow[s] : s;
+        const int doc0 = max(0, s - ps);               // document start
+        const int start = max(0, s - min(ps, window));  // first visible key
         int* drow = dstart + bb * S_pad;
         drow[s] = start;
         if (s == S - 1)
           for (int x = S; x < S_pad; ++x) drow[x] = start;
-        if (s == S - 1 || prow[s + 1] == 0) {  // s ends its document
+        if (s == S - 1 || (prow && prow[s + 1] == 0)) {  // s ends its document
           const int n_kt = (S + BKV - 1) / BKV;
           const int kt_hi = s == S - 1 ? n_kt - 1 : (s + 1) / BKV - 1;  // last key tile whose last key is <= s
-          for (int kt = start / BKV; kt <= kt_hi; ++kt) qt_end[bb * n_kt + kt] = s / BQ + 1;
+          for (int kt = doc0 / BKV; kt <= kt_hi; ++kt)
+            qt_end[bb * n_kt + kt] = min(s, kt * BKV + BKV - 1 + window) / BQ + 1;
         }
       }
     }
@@ -512,9 +521,10 @@ size_t attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
 
 namespace {
 
+// doc selects the document / window kernels; window < 0 means none
 int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                  const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
-                  int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+                  bool doc, const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk,
+                  int D, float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
   // dk / dv rows may be strided: dkv_row_heads heads per token row (0 = Hk, i.e. contiguous [B,S,Hk,D]).
   // With dk = base, dv = base + Hk*D and dkv_row_heads = 2*Hk both land in ONE [B,S,2*Hk*D] buffer, which lets
   // the k/v projections' dgrad and wgrad run as single GEMMs over the concatenated weight.
@@ -523,7 +533,7 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_bwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_bwd: head_dim %d unsupported (64 or 128)", D);
-  const size_t need = pos ? attn_bwd_doc_workspace_bytes(B, S, H, Hk, D) : attn_bwd_workspace_bytes(B, S, H, Hk, D);
+  const size_t need = doc ? attn_bwd_doc_workspace_bytes(B, S, H, Hk, D) : attn_bwd_workspace_bytes(B, S, H, Hk, D);
   if (ws_bytes < need) {
     set_error("attn_bwd: workspace too small (%zu < %zu)", ws_bytes, need);
     return B200_ERR_WORKSPACE;
@@ -543,10 +553,11 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
   {
     const long long threads = (long long)B * S * H * (D / 8);
     const int blocks = (int)((threads + 255) / 256);
-    auto delta_kern = D == 64 ? (pos ? attn_delta_kernel<64, true> : attn_delta_kernel<64, false>)
-                              : (pos ? attn_delta_kernel<128, true> : attn_delta_kernel<128, false>);
+    auto delta_kern = D == 64 ? (doc ? attn_delta_kernel<64, true> : attn_delta_kernel<64, false>)
+                              : (doc ? attn_delta_kernel<128, true> : attn_delta_kernel<128, false>);
     delta_kern<<<blocks, 256, 0, stream>>>((const __nv_bfloat16*)o, (const __nv_bfloat16*)d_o, lse, delta, lse2,
-                                           dq_acc, B, S, H, S_pad, pos, dstart, qt_end);
+                                           dq_acc, B, S, H, S_pad, pos, dstart, qt_end,
+                                           window < 0 || window > S ? S : window);
     B200_CHECK_LAUNCH();
   }
   CUtensorMap tmQ, tmK, tmV, tmDO, tmDQ;
@@ -569,10 +580,10 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
   a.dkv_rh = dkv_row_heads;
   a.scale = scale;
   a.causal = causal;
-  a.paired = causal && !pos && n_kt % 2 == 0;
-  a.dstart = pos ? dstart : nullptr;
-  a.qt_end = pos ? qt_end : nullptr;
-  if (pos)
+  a.paired = causal && !doc && n_kt % 2 == 0;
+  a.dstart = doc ? dstart : nullptr;
+  a.qt_end = doc ? qt_end : nullptr;
+  if (doc)
     rc = D == 64 ? launch_bwd<64, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
                  : launch_bwd<128, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
   else
@@ -595,8 +606,8 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
 int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
              const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
              float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
-  return attn_bwd_impl(q, k, v, o, d_o, lse, nullptr, dq, dk, dv, B, S, H, Hk, D, scale, causal, dkv_row_heads, ws,
-                       ws_bytes, stream);
+  return attn_bwd_impl(q, k, v, o, d_o, lse, false, nullptr, -1, dq, dk, dv, B, S, H, Hk, D, scale, causal,
+                       dkv_row_heads, ws, ws_bytes, stream);
 }
 
 // document-causal backward: query s of row b sees keys s - pos[b, s] .. s
@@ -605,8 +616,19 @@ int attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, con
                  int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
   B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
                  "attn_bwd_doc: pos must be a non-null, 4-byte aligned int32 [B, S] array");
-  return attn_bwd_impl(q, k, v, o, d_o, lse, pos, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads, ws, ws_bytes,
-                       stream);
+  return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, -1, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads, ws,
+                       ws_bytes, stream);
+}
+
+// sliding-window backward: query s sees keys s - min(pos[b, s], window) .. s; pos == nullptr means pos[b, s] = s.
+// Same workspace as the document variant.
+int attn_bwd_window(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                    const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
+                    float scale, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_bwd_window: pos must be 4-byte aligned int32");
+  B200_CHECK_ARG(window >= 0, "attn_bwd_window: window=%d must be >= 0", window);
+  return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
+                       ws, ws_bytes, stream);
 }
 
 }  // namespace b200

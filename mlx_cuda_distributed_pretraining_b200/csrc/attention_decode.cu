@@ -19,6 +19,12 @@
 //
 // Every reduction has a fixed order that depends only on the row's own data, so a row's output is bit-identical
 // whether it runs alone or inside any batch, and from launch to launch.
+//
+// Sliding window (attn_decode_window): the query at position len - 1 sees keys kv0 = max(0, len - 1 - W) .. len - 1.
+// Chunk boundaries stay at multiples of 256 from position 0; chunks that end at or below kv0 exit at once, the first
+// live chunk starts at the 32-key tile holding kv0 and masks the keys below it, and the combine merges the live chunks
+// only.  A row's result still depends on lens[b] and W alone.  Without a window W = s_max, so kv0 = 0 and the
+// arithmetic is the unwindowed kernel's.
 #include "common.cuh"
 #include "host.h"
 
@@ -82,7 +88,11 @@ struct DecArgs {
   float* part_ml;     // [B, H, max_chunks, 2]
   int H, G, s_max, max_chunks;
   float scale_log2;   // scale * log2 e
+  int window;         // keys len - 1 - window .. len - 1 are visible; s_max without a window
 };
+
+// kv0: the first cached key the row's query sees
+__device__ __forceinline__ int first_visible_key(const DecArgs& p, int len) { return max(0, len - 1 - p.window); }
 
 template <typename T, int D>
 __global__ void __launch_bounds__(DEC_THREADS)
@@ -93,10 +103,12 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   const int c = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
   const int len = min(p.lens[b], p.s_max);
   const int c0 = c * DEC_CHUNK;
-  if (c0 >= len) return;
+  const int kv0 = first_visible_key(p, len);
+  if (c0 >= len || c0 + DEC_CHUNK <= kv0) return;
+  const int lo = max(c0, kv0 & ~(DEC_TILE - 1));  // the first live chunk starts at the tile holding kv0
   const int end = min(len, c0 + DEC_CHUNK);
-  const int n_tiles = (end - c0 + DEC_TILE - 1) / DEC_TILE;
-  const int n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK;
+  const int n_tiles = (end - lo + DEC_TILE - 1) / DEC_TILE;
+  const int n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK - kv0 / DEC_CHUNK;  // live chunks of the row
   const int G = p.G;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
@@ -112,7 +124,7 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   float* sred = reinterpret_cast<float*>(smem + lay.red);
   const uint32_t bar0 = smem_u32(smem + lay.bar);
 
-  auto tile_start = [&](int j) { return min(c0 + j * DEC_TILE, end - DEC_TILE); };
+  auto tile_start = [&](int j) { return min(lo + j * DEC_TILE, end - DEC_TILE); };
   auto issue = [&](int j) {
     const int st = j % DEC_STAGES;
     const uint32_t bar = bar0 + 8 * st;
@@ -170,7 +182,8 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     const T* tK = ring + (2 * st) * TILE_ELEMS;
     const T* tV = ring + (2 * st + 1) * TILE_ELEMS;
     const int start = tile_start(j);
-    const int first_valid = c0 + j * DEC_TILE;  // rows of an end-anchored tile below this belong to earlier tiles
+    // rows of an end-anchored tile below lo + 32 j belong to earlier tiles; keys below kv0 are outside the window
+    const int first_valid = max(lo + j * DEC_TILE, kv0);
 
     // scores: L consecutive lanes per key, 8 columns each
     {
@@ -199,6 +212,7 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     __syncthreads();
 
     // online softmax (log2 domain): one warp per head, one lane per key; every tile holds at least one valid key
+    // (kv0 < end, and kv0 lies in the first tile)
     for (int g = warp; g < G; g += DEC_THREADS / 32) {
       const float x = ss[g * DEC_TILE + lane];
       const float m_old = sm[g];
@@ -278,20 +292,23 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   }
 }
 
-// o = sum_c exp2(m_c - M) acc_c / sum_c exp2(m_c - M) l_c over a row's chunks, in chunk order; one thread per column
+// o = sum_c exp2(m_c - M) acc_c / sum_c exp2(m_c - M) l_c over a row's live chunks, in chunk order; one thread per
+// column
 template <typename T, int D>
 __global__ void __launch_bounds__(D)
 attn_decode_combine_kernel(const DecArgs p) {
   const int h = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
-  const int n = (min(p.lens[b], p.s_max) + DEC_CHUNK - 1) / DEC_CHUNK;
-  if (n <= 1) return;  // finished by attn_decode_kernel
+  const int len = min(p.lens[b], p.s_max);
+  const int c_lo = first_visible_key(p, len) / DEC_CHUNK;
+  const int n = (len + DEC_CHUNK - 1) / DEC_CHUNK;
+  if (n - c_lo <= 1) return;  // finished by attn_decode_kernel
   const long long bh = (long long)b * p.H + h;
   const float* ml = p.part_ml + bh * p.max_chunks * 2;
   const float* pa = p.part_acc + bh * p.max_chunks * D + d;
   float M = -INFINITY;
-  for (int c = 0; c < n; ++c) M = fmaxf(M, ml[2 * c]);
+  for (int c = c_lo; c < n; ++c) M = fmaxf(M, ml[2 * c]);
   float l = 0.f, acc = 0.f;
-  for (int c = 0; c < n; ++c) {
+  for (int c = c_lo; c < n; ++c) {
     const float w = exp2f(ml[2 * c] - M);
     l = fmaf(ml[2 * c + 1], w, l);
     acc = fmaf(pa[(long long)c * D], w, acc);
@@ -390,9 +407,11 @@ size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D) {
   return (size_t)B * H * chunks * (size_t)(D + 2) * sizeof(float);
 }
 
-int attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse, int B,
-                int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes,
-                cudaStream_t stream) {
+namespace {
+
+int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
+                     int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
+                     size_t ws_bytes, cudaStream_t stream) {
   B200_CHECK_ARG(B > 0 && H > 0 && Hk > 0 && H % Hk == 0, "attn_decode: bad shape B=%d H=%d Hk=%d", B, H, Hk);
   B200_CHECK_ARG(D == 16 || D == 32 || D == 64 || D == 128, "attn_decode: head_dim %d unsupported (16/32/64/128)", D);
   B200_CHECK_ARG(s_max >= DEC_TILE, "attn_decode: s_max=%d must be >= %d", s_max, DEC_TILE);
@@ -426,8 +445,27 @@ int attn_decode(const void* q, const void* k_cache, const void* v_cache, const i
   a.G = G;
   a.s_max = s_max;
   a.scale_log2 = scale * kLog2e;
+  a.window = window < 0 || window > s_max ? s_max : window;
   return is_bf16 ? launch_decode_d<__nv_bfloat16>(D, tmK, tmV, a, B, Hk, stream)
                  : launch_decode_d<float>(D, tmK, tmV, a, B, Hk, stream);
+}
+
+}  // namespace
+
+int attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse, int B,
+                int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes,
+                cudaStream_t stream) {
+  return attn_decode_impl(q, k_cache, v_cache, lens, o, lse, -1, B, s_max, H, Hk, D, scale, is_bf16, ws, ws_bytes,
+                          stream);
+}
+
+// sliding window: the query at position lens[b] - 1 sees cached keys max(0, lens[b] - 1 - window) .. lens[b] - 1
+int attn_decode_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
+                       int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
+                       size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG(window >= 0, "attn_decode_window: window=%d must be >= 0", window);
+  return attn_decode_impl(q, k_cache, v_cache, lens, o, lse, window, B, s_max, H, Hk, D, scale, is_bf16, ws,
+                          ws_bytes, stream);
 }
 
 int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,

@@ -17,6 +17,10 @@
 // are monotone in q, so that is the lowest start of the CTA's rows) and the extra `key < q - pos[q]` mask runs only
 // on tiles below the CTA's highest document start.  Rows with no visible key in a tile pass through the online
 // softmax as the causal rows do (m_use).  DOC = false compiles to the causal / non-causal kernel unchanged.
+//
+// Sliding window (same DOC instantiation): query q sees keys q - min(pos[q], W) .. q, i.e. the document mask with pos
+// clamped at W, which keeps the starts monotone in q.  pos == nullptr reads as pos[q] = q (one document per row), so
+// an unpacked windowed launch needs no [B, S] buffer.  Without a window W = S, and min(pos[q], S) = pos[q].
 #include "common.cuh"
 #include "host.h"
 
@@ -47,8 +51,16 @@ struct FwdArgs {
   int B, S, H, Hk;
   float scale;
   int causal;
-  const int* pos;  // [B, S] positions within documents (DOC kernels only)
+  const int* pos;  // [B, S] positions within documents (DOC kernels only; null: pos[q] = q)
+  int window;      // DOC: query q sees keys from q - min(pos[q], window); S when there is no window
 };
+
+// first key query `row` of batch row b may see: its document start, or its window start when that is later
+__device__ __forceinline__ int key_start(const FwdArgs& p, int b, int row) {
+  // (the null-pos form max(0, row - window) is row - min(row, window); written so, it keeps D = 128 within 168
+  // registers without spills)
+  return p.pos ? row - min(__ldg(p.pos + (long long)b * p.S + row), p.window) : max(0, row - p.window);
+}
 
 template <int D>
 __device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db) {
@@ -72,9 +84,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_kv_all = (p.S + ATT_BKV - 1) / ATT_BKV;
   const int n_kv = p.causal ? min(n_kv_all, (q0 + ATT_BQ - 1) / ATT_BKV + 1) : n_kv_all;
-  // first key tile: the start of the first query's document (0 without documents)
+  // first key tile: the first query's document / window start (0 without documents)
   int j0 = 0;
-  if constexpr (DOC) j0 = max(0, q0 - __ldg(p.pos + (long long)b * p.S + q0)) / ATT_BKV;
+  if constexpr (DOC) j0 = max(0, key_start(p, b, q0)) / ATT_BKV;
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
@@ -114,16 +126,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
   const float sl2 = p.scale * kLog2e;
   const int row_a = q0 + wg * 64 + wq * 16 + (lane >> 2);  // this thread's rows: row_a, row_a + 8
-  // DOC: document start of each of this thread's rows, and the highest start of the CTA's rows (its last row's)
+  // DOC: document / window start of each of this thread's rows, and the highest start of the CTA's rows (its last
+  // row's)
   int dstart[2] = {0, 0}, dstart_hi = 0;
   if constexpr (DOC) {
-    const int* prow = p.pos + (long long)b * p.S;
-    const int q_hi = min(q0 + ATT_BQ, p.S) - 1;
-    dstart_hi = q_hi - __ldg(prow + q_hi);
+    dstart_hi = key_start(p, b, min(q0 + ATT_BQ, p.S) - 1);
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int row = row_a + 8 * r;
-      dstart[r] = row < p.S ? row - __ldg(prow + row) : 0;
+      dstart[r] = row < p.S ? key_start(p, b, row) : 0;
     }
   }
   mbar_wait(q_full, 0);
@@ -271,8 +282,9 @@ int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, in
 
 namespace {
 
-int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B, int S,
-                  int H, int Hk, int D, float scale, int causal, cudaStream_t stream) {
+// doc selects the document / window instantiation; window < 0 means none
+int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, bool doc, const int* pos,
+                  int window, int B, int S, int H, int Hk, int D, float scale, int causal, cudaStream_t stream) {
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_fwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd: head_dim %d unsupported (64 or 128; pad smaller dims)", D);
@@ -292,7 +304,8 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   a.scale = scale;
   a.causal = causal;
   a.pos = pos;
-  if (pos) return D == 64 ? launch_fwd<64, true>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, true>(tmQ, tmK, tmV, a, stream);
+  a.window = window < 0 || window > S ? S : window;
+  if (doc) return D == 64 ? launch_fwd<64, true>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, true>(tmQ, tmK, tmV, a, stream);
   return D == 64 ? launch_fwd<64, false>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, false>(tmQ, tmK, tmV, a, stream);
 }
 
@@ -300,7 +313,7 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
 
 int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int H,
              int Hk, int D, float scale, int causal, cudaStream_t stream) {
-  return attn_fwd_impl(q, k, v, o, lse, nullptr, B, S, H, Hk, D, scale, causal, stream);
+  return attn_fwd_impl(q, k, v, o, lse, false, nullptr, -1, B, S, H, Hk, D, scale, causal, stream);
 }
 
 // document-causal: query s of row b sees keys s - pos[b, s] .. s
@@ -308,7 +321,15 @@ int attn_fwd_doc(const void* q, const void* k, const void* v, void* o, float* ls
                  int H, int Hk, int D, float scale, cudaStream_t stream) {
   B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
                  "attn_fwd_doc: pos must be a non-null, 4-byte aligned int32 [B, S] array");
-  return attn_fwd_impl(q, k, v, o, lse, pos, B, S, H, Hk, D, scale, 1, stream);
+  return attn_fwd_impl(q, k, v, o, lse, true, pos, -1, B, S, H, Hk, D, scale, 1, stream);
+}
+
+// sliding window: query s sees keys s - min(pos[b, s], window) .. s; pos == nullptr means pos[b, s] = s
+int attn_fwd_window(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                    int B, int S, int H, int Hk, int D, float scale, cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_fwd_window: pos must be 4-byte aligned int32");
+  B200_CHECK_ARG(window >= 0, "attn_fwd_window: window=%d must be >= 0", window);
+  return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, stream);
 }
 
 }  // namespace b200

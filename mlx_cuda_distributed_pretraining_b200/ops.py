@@ -654,9 +654,18 @@ def _pad_head_dim(D: int) -> int:
     raise ValueError(f"attention: head_dim {D} > 128 is not supported")
 
 
-def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.Tensor] = None):
+def _check_window(window, what: str) -> int:
+    """A sliding-window size: a non-negative int (query q sees keys q - window .. q)."""
+    if isinstance(window, bool) or not isinstance(window, int) or window < 0:
+        raise ValueError(f"{what}: window must be a non-negative int, got {window!r}")
+    return window
+
+
+def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
+                      window: Optional[int] = None):
     """q [B,S,H,D], k/v [B,S,Hk,D] bf16 contiguous, D in {64,128}. Returns (o, lse[B,H,S]).  With pos (int32 [B,S]
-    contiguous, positions within documents) the mask is document-causal and `causal` is ignored."""
+    contiguous, positions within documents) the mask is document-causal and `causal` is ignored.  With window (an
+    int >= 0) query s sees keys s - min(pos[s], window) .. s (pos[s] = s without pos), and `causal` is ignored."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         _need(t, torch.bfloat16, nm)
     B, S, H, D = q.shape
@@ -664,7 +673,11 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
     o = torch.empty_like(q)
     lse = torch.empty((B, H, S), device=q.device, dtype=torch.float32)
     tok = _t0("attn_fwd")
-    if pos is None:
+    if window is not None:
+        check(lib().b200_attn_fwd_window(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+                                         _ptr(pos), min(int(window), S), B, S, H, Hk, D, float(scale), _stream()),
+              "b200_attn_fwd_window")
+    elif pos is None:
         check(lib().b200_attn_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
                                   B, S, H, Hk, D, float(scale), int(causal), _stream()), "b200_attn_fwd")
     else:
@@ -674,7 +687,8 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
     return o, lse
 
 
-def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Optional[torch.Tensor] = None):
+def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
+                      window: Optional[int] = None):
     B, S, H, D = q.shape
     Hk = k.shape[2]
     dq = torch.empty_like(q)
@@ -683,7 +697,14 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
     dkv = torch.empty((B, S, 2 * Hk, D), device=k.device, dtype=k.dtype)
     dk, dv = dkv[:, :, :Hk], dkv[:, :, Hk:]
     tok = _t0("attn_bwd")
-    if pos is None:
+    if window is not None:
+        nbytes = int(lib().b200_attn_bwd_window_workspace_bytes(B, S, H, Hk, D))
+        ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
+        check(lib().b200_attn_bwd_window(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                         lse.data_ptr(), _ptr(pos), min(int(window), S), dq.data_ptr(), dk.data_ptr(),
+                                         dv.data_ptr(), B, S, H, Hk, D, float(scale), 2 * Hk, ws.data_ptr(),
+                                         ws.numel(), _stream()), "b200_attn_bwd_window")
+    elif pos is None:
         nbytes = int(lib().b200_attn_bwd_workspace_bytes(B, S, H, Hk, D))
         ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
         check(lib().b200_attn_bwd_strided(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
@@ -703,15 +724,15 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos):
+    def forward(ctx, q, k, v, scale, causal, pos, window):
         D = q.shape[-1]
         Dp = _pad_head_dim(D)
         if Dp != D:  # zero-padding the head dim leaves QK^T and the first D columns of PV unchanged
             q, k, v = (torch.nn.functional.pad(t, (0, Dp - D)) for t in (q, k, v))
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos)
+        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos, window)
         ctx.save_for_backward(q, k, v, o, lse, pos)
-        ctx.scale, ctx.causal, ctx.D = scale, causal, D
+        ctx.scale, ctx.causal, ctx.D, ctx.window = scale, causal, D, window
         return o[..., :D] if Dp != D else o
 
     @staticmethod
@@ -721,10 +742,10 @@ class _AttentionFn(torch.autograd.Function):
         if Dp != ctx.D:
             do = torch.nn.functional.pad(do, (0, Dp - ctx.D))
         do = do.contiguous()
-        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos)
+        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos, ctx.window)
         if Dp != ctx.D:
             dq, dk, dv = dq[..., :ctx.D], dk[..., :ctx.D], dv[..., :ctx.D]
-        return dq, dk, dv, None, None, None
+        return dq, dk, dv, None, None, None, None
 
 
 def _hi_lo(x: torch.Tensor):
@@ -746,7 +767,7 @@ class _AttentionX3Fn(torch.autograd.Function):
     to fp32-like accuracy; P and the kernel outputs still pass through one bf16 rounding each."""
 
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos):
+    def forward(ctx, q, k, v, scale, causal, pos, window):
         D = q.shape[-1]
         Dp = _pad_head_dim(3 * D)
         (qh, ql), (kh, kl), (vh, vl) = _hi_lo(q), _hi_lo(k), _hi_lo(v)
@@ -755,9 +776,9 @@ class _AttentionX3Fn(torch.autograd.Function):
             t = torch.cat([a, b, c], dim=-1)
             return (torch.nn.functional.pad(t, (0, Dp - 3 * D)) if Dp != 3 * D else t).contiguous()
         q3, k3, v3 = cat3(qh, ql, qh), cat3(kh, kh, kl), cat3(vh, vh, vl)
-        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos)
+        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos, window)
         ctx.save_for_backward(q3, k3, v3, o3, lse, pos)
-        ctx.scale, ctx.causal, ctx.D, ctx.Dp = scale, causal, D, Dp
+        ctx.scale, ctx.causal, ctx.D, ctx.Dp, ctx.window = scale, causal, D, Dp, window
         return o3[..., :D].float() + o3[..., 2 * D:3 * D].float()
 
     @staticmethod
@@ -768,37 +789,47 @@ class _AttentionX3Fn(torch.autograd.Function):
         g3 = torch.cat([gh, gl, gh], dim=-1)
         if Dp != 3 * D:
             g3 = torch.nn.functional.pad(g3, (0, Dp - 3 * D))
-        dq3, dk3, dv3 = attention_bwd_raw(q3, k3, v3, o3, g3.contiguous(), lse, ctx.scale, ctx.causal, pos)
+        dq3, dk3, dv3 = attention_bwd_raw(q3, k3, v3, o3, g3.contiguous(), lse, ctx.scale, ctx.causal, pos,
+                                          ctx.window)
         dq = dq3[..., :D].float() + dq3[..., 2 * D:3 * D].float()
         dk = dk3[..., :D].float() + dk3[..., D:2 * D].float()
         dv = dv3[..., :D].float() + dv3[..., D:2 * D].float()
-        return dq, dk, dv, None, None, None
+        return dq, dk, dv, None, None, None, None
 
 
 def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
-                   causal: bool = True, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos: as attention."""
+                   causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None) -> torch.Tensor:
+    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos, window: as
+    attention."""
     if 3 * q.shape[-1] > 128:
         raise ValueError("attention_fp32: head_dim must be <= 42 (three bf16 copies must fit a 128-wide tile)")
     if scale is None:
         scale = q.shape[-1] ** -0.5
     if pos is not None:
         pos, causal = _check_pos(pos, q, "attention_fp32"), True
-    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos)
+    if window is not None:
+        window, causal = _check_window(window, "attention_fp32"), True
+    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos, window)
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
-              causal: bool = True, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+              causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None) -> torch.Tensor:
     """softmax(q k^T * scale + causal_mask) v with GQA head sharing; [B,S,H,D] layout, bf16.
 
     pos (int32 [B, S]) packs several documents per row: pos[b, s] is token s's position within its document (0 at a
     document's first token, +1 per token inside it), and query s sees only keys s - pos[b, s] .. s -- the causal
-    attention of each document run alone.  It implies causal."""
+    attention of each document run alone.  It implies causal.
+
+    window (int >= 0) is a sliding causal window: query s sees key k iff 0 <= s - k <= window, at most window + 1
+    keys, intersected with the document when pos is given (keys s - min(pos[b, s], window) .. s).  Tiles outside
+    every row's window are skipped, so the cost is linear in S.  It implies causal."""
     if scale is None:
         scale = q.shape[-1] ** -0.5
     if pos is not None:
         pos, causal = _check_pos(pos, q, "attention"), True
-    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos)
+    if window is not None:
+        window, causal = _check_window(window, "attention"), True
+    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos, window)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -827,16 +858,19 @@ def _check_cache(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, 
 
 def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
                      scale: Optional[float] = None, workspace: Optional[torch.Tensor] = None,
-                     return_lse: bool = False):
+                     return_lse: bool = False, window: Optional[int] = None):
     """softmax(q K^T * scale) V for one new query per row over its first lens[b] cached keys (b200_attn_decode).
 
     q [B,H,D]; k_cache, v_cache [B,s_max,Hk,D]; all bf16 or all fp32, D in {16, 32, 64, 128}; lens int32 [B] on the
     device, 1 <= lens[b] <= s_max (not checked here: that would read the device).  `workspace` (uint8, at least
     attention_decode_workspace_bytes(B, H, s_max, D)) is allocated when not given.  Returns o [B,H,D] in q's dtype,
-    and the natural-log LSE [B,H] fp32 with return_lse."""
+    and the natural-log LSE [B,H] fp32 with return_lse.  window (int >= 0): the query at position p = lens[b] - 1
+    sees only keys max(0, p - window) .. p (b200_attn_decode_window), and only those are read."""
     B, H, D, s_max, Hk = _check_cache(q, k_cache, v_cache, lens, "attention_decode")
     if D not in (16, 32, 64, 128):
         raise ValueError(f"attention_decode: head_dim {D} unsupported (16, 32, 64 or 128)")
+    if window is not None:
+        window = _check_window(window, "attention_decode")
     if scale is None:
         scale = D ** -0.5
     need = attention_decode_workspace_bytes(B, H, s_max, D)
@@ -847,9 +881,16 @@ def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     o = torch.empty_like(q)
     lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_decode")
-    check(lib().b200_attn_decode(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr(), o.data_ptr(),
-                                 _ptr(lse), B, s_max, H, Hk, D, float(scale), _is_bf16(q, "q"), workspace.data_ptr(),
-                                 workspace.numel(), _stream()), "b200_attn_decode")
+    if window is None:
+        check(lib().b200_attn_decode(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr(),
+                                     o.data_ptr(), _ptr(lse), B, s_max, H, Hk, D, float(scale), _is_bf16(q, "q"),
+                                     workspace.data_ptr(), workspace.numel(), _stream()), "b200_attn_decode")
+    else:
+        check(lib().b200_attn_decode_window(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr(),
+                                            o.data_ptr(), _ptr(lse), min(int(window), s_max), B, s_max, H, Hk, D,
+                                            float(scale), _is_bf16(q, "q"), workspace.data_ptr(), workspace.numel(),
+                                            _stream()),
+              "b200_attn_decode_window")
     _t1(tok)
     return (o, lse) if return_lse else o
 
