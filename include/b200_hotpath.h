@@ -287,6 +287,11 @@ int b200_rope(const void* x, void* y, const float* cos_t, const float* sin_t, in
  * (arch/llama_standard.py:90-131 with position_ids).  The tables must hold max(pos) + 1 rows. */
 int b200_rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S,
                   int NH, int D, int backward, int is_bf16, void* stream);
+/* Half-split RoPE, mlx_lm's nn.RoPE(traditional=False) (and Hugging Face Llama's rotate_half): for i < D/2 the pair
+ * (x[i], x[i + D/2]) is rotated by pos * theta^(-2i/D), with the same cos_t / sin_t tables as b200_rope.  pos is as
+ * for b200_rope_pos, or NULL for position s.  D % 16 == 0; backward=1 applies the inverse rotation. */
+int b200_rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S,
+                   int NH, int D, int backward, int is_bf16, void* stream);
 
 /* ---- MLP block on the in-tree GEMM engine with the GLU in the epilogue (SURVEY 8f row f1) ----------------
  * arch/llama.py:142-151: down( gate(x) * sigmoid(up(x)) * 2 ).  gate_proj.weight and up_proj.weight must be
@@ -301,12 +306,24 @@ int b200_rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t
 int b200_mlp_gateup_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, void* stream);
 int b200_mlp_down_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
                           void* stream);
+/* The same pair for mlx_lm's Llama MLP (mlx_lm/models/llama.py: down(silu(gate(x)) * up(x)), model.misc.variant:
+ * mlx_lm), with the same arguments, shapes and alignment rules:
+ * b200_mlp_gateup_silu_fwd: y = silu(g) * u = g * sigmoid(g) * u from the fp32 accumulators.
+ * b200_mlp_down_silu_bwd:   dgu = [ d * u * sigmoid(g) * (1 + g * (1 - sigmoid(g))) | d * silu(g) ].
+ * Their sigmoid is accurate relative to its value (not just to 1), so silu stays accurate in the negative tail. */
+int b200_mlp_gateup_silu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, void* stream);
+int b200_mlp_down_silu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
+                           void* stream);
 
 /* ---- block-adjacent fused elementwise steps (SURVEY 8f row f1) ------------------------------------
  * arch/llama.py:151: y = gate * sigmoid(up) * 2 and its adjoint; bf16, n % 8 == 0 */
 int b200_glu_fwd(const void* gate, const void* up, void* y, long long n, void* stream);
 int b200_glu_bwd(const void* dy, const void* gate, const void* up, void* dgate, void* dup, long long n,
                  void* stream);
+/* mlx_lm's Llama MLP activation: y = silu(gate) * up and its adjoint; bf16, n % 8 == 0 */
+int b200_silu_glu_fwd(const void* gate, const void* up, void* y, long long n, void* stream);
+int b200_silu_glu_bwd(const void* dy, const void* gate, const void* up, void* dgate, void* dup, long long n,
+                      void* stream);
 /* Adjoint of the embedding gather (arch/llama.py:389): grad[tokens[r], :] += dh[r, :] for r in [0, rows);
  * dh bf16 [rows, H]; grad bf16 or f32 [V, H] (accumulated into: it may already hold the tied-logits wgrad);
  * fp32 accumulation per vocabulary row in the workspace (V*H floats), tokens outside [0, V) are ignored. */
@@ -395,6 +412,11 @@ int b200_attn_decode_window(const void* q, const void* k_cache, const void* v_ca
 int b200_kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
                    const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
                    void* stream);
+/* b200_kv_append with b200_rope_half's half-split rotation, statement for statement, so a token rotated here is
+ * bit-equal to the same token rotated by the prefill.  cos_t / sin_t are required; D % 16 == 0. */
+int b200_kv_append_half(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                        const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                        void* stream);
 
 #ifdef __cplusplus
 }

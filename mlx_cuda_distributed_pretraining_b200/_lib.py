@@ -84,6 +84,12 @@ SIGNATURES = {
     "b200_attn_decode_workspace_bytes": (_sz, [_i, _i, _i, _i]),
     "b200_attn_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
     "b200_kv_append": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_rope_half": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_mlp_gateup_silu_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "b200_mlp_down_silu_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "b200_silu_glu_fwd": (_i, [_vp, _vp, _vp, _ll, _vp]),
+    "b200_silu_glu_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _vp]),
+    "b200_kv_append_half": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
 

@@ -110,7 +110,8 @@ class FlashAttention(nn.Module):
         o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window)
         return o if dt == torch.bfloat16 else o.to(dt)
 
-    def forward(self, x: torch.Tensor, mask=None) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, mask=None, rope_layout: str = "interleaved") -> torch.Tensor:
+        """rope_layout: ops.rope's pair layout when RoPE is on ("interleaved" or mlx_lm's "half")."""
         B, S, _ = x.shape
         if self.q_proj.bias is None and self.k_proj.bias is None and self.v_proj.bias is None:
             q, k, v = ops.multi_linear(x, (self.q_proj.weight, self.k_proj.weight, self.v_proj.weight))
@@ -122,8 +123,8 @@ class FlashAttention(nn.Module):
         if self.rope_tables is not None:
             cos_t, sin_t = self.rope_tables
             pos = mask.pos if isinstance(mask, DocumentCausalMask) else None  # packed rows: position in document
-            q = ops.rope(q, cos_t[:S], sin_t[:S], pos)
-            k = ops.rope(k, cos_t[:S], sin_t[:S], pos)
+            q = ops.rope(q, cos_t[:S], sin_t[:S], pos, rope_layout)
+            k = ops.rope(k, cos_t[:S], sin_t[:S], pos, rope_layout)
         ctx = self._flash_attention(q, k, v, mask)
         ctx = ctx.reshape(B, S, self.num_heads * self.head_dim)
         return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
@@ -137,7 +138,8 @@ class FlashAttention(nn.Module):
     def _out(self, ctx: torch.Tensor) -> torch.Tensor:
         return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
 
-    def forward_prefill(self, x: torch.Tensor, mask, k_cache: torch.Tensor, v_cache: torch.Tensor) -> torch.Tensor:
+    def forward_prefill(self, x: torch.Tensor, mask, k_cache: torch.Tensor, v_cache: torch.Tensor,
+                        rope_layout: str = "interleaved") -> torch.Tensor:
         """forward(x, mask) over a right-padded prompt batch x [B, S, hidden] that also stores the (rotated) keys and
         values in cache positions [0, S).  Attention runs through _flash_attention, so the numerics are the
         training forward's."""
@@ -148,15 +150,16 @@ class FlashAttention(nn.Module):
         v = v.reshape(B, S, self.num_kv_heads, self.head_dim)
         if self.rope_tables is not None:
             cos_t, sin_t = self.rope_tables
-            q = ops.rope(q, cos_t[:S], sin_t[:S])
-            k = ops.rope(k, cos_t[:S], sin_t[:S])
+            q = ops.rope(q, cos_t[:S], sin_t[:S], layout=rope_layout)
+            k = ops.rope(k, cos_t[:S], sin_t[:S], layout=rope_layout)
         k_cache[:, :S].copy_(k)
         v_cache[:, :S].copy_(v)
         ctx = self._flash_attention(q, k, v, mask)
         return self._out(ctx.reshape(B, S, self.num_heads * self.head_dim))
 
     def forward_decode(self, x: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
-                       workspace: torch.Tensor, window: Optional[int] = None) -> torch.Tensor:
+                       workspace: torch.Tensor, window: Optional[int] = None,
+                       rope_layout: str = "interleaved") -> torch.Tensor:
         """One new token per row, x [B, hidden]: its k and v go to cache position lens[b] - 1 (rotated there when
         RoPE is on), then its query attends over the row's first lens[b] cached keys (the last window + 1 of them
         with a sliding window)."""
@@ -165,6 +168,6 @@ class FlashAttention(nn.Module):
         q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
         k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
-        ops.kv_append(q, k, v, k_cache, v_cache, lens, self.rope_tables)
+        ops.kv_append(q, k, v, k_cache, v_cache, lens, self.rope_tables, layout=rope_layout)
         ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace, window=window)
         return self._out(ctx.reshape(B, self.num_heads * self.head_dim))

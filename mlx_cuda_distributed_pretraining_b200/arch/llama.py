@@ -12,6 +12,10 @@ Flattened parameter names equal mlx's tree_flatten(model.parameters()) names, e.
 RoPE: arch/llama.py constructs a RotaryPositionEncoding and never applies it (SURVEY D6); the
 faithful default is therefore no positional rotation.  `ModelArgs.apply_rope=True` enables the
 interleaved-pair rotation of arch/llama_standard.py:213-215 through ops.rope.
+
+`ModelArgs.variant = "mlx_lm"` builds the block the reference's trainer actually runs (mlx_lm.models.llama, DESIGN
+D4): MLP down(silu(gate(x)) * up(x)), and RoPE always on q and k, half-split pairs (x[i], x[i + D/2]) unless
+rope_traditional.  Parameter names are unchanged.
 """
 from __future__ import annotations
 
@@ -23,6 +27,8 @@ from torch import nn
 
 from .. import ops
 from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention
+
+VARIANTS = (None, "reference", "mlx_lm")
 
 
 @dataclass
@@ -52,6 +58,7 @@ class ModelArgs:
     num_experts_per_tok: int = 0
     apply_rope: bool = False  # extension; see module docstring
     sliding_window: Optional[int] = None  # extension: query q sees keys q - W .. q in every layer (None: causal)
+    variant: Optional[str] = None  # extension: None / "reference" (this block) or "mlx_lm" (module docstring)
 
 
 class RMSNorm(nn.Module):
@@ -65,16 +72,18 @@ class RMSNorm(nn.Module):
 
 
 class MLP(nn.Module):
-    def __init__(self, hidden_size: int, intermediate_size: int, use_bias: bool = False):
+    def __init__(self, hidden_size: int, intermediate_size: int, use_bias: bool = False, act: str = "sigmoid2"):
+        """act: "sigmoid2" (the reference's gate * sigmoid(up) * 2) or "silu" (mlx_lm's silu(gate) * up)."""
         super().__init__()
+        self.act = act
         self.gate_proj = nn.Linear(hidden_size, intermediate_size, bias=use_bias)
         self.up_proj = nn.Linear(hidden_size, intermediate_size, bias=use_bias)
         self.down_proj = nn.Linear(intermediate_size, hidden_size, bias=use_bias)
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
         if self.gate_proj.bias is not None:
-            return self.down_proj(ops.glu(self.gate_proj(x), self.up_proj(x)))
-        return ops.mlp(x, self.gate_proj.weight, self.up_proj.weight, self.down_proj.weight)
+            return self.down_proj(ops.glu(self.gate_proj(x), self.up_proj(x), self.act))
+        return ops.mlp(x, self.gate_proj.weight, self.up_proj.weight, self.down_proj.weight, self.act)
 
 
 class AttentionModule(nn.Module):
@@ -82,8 +91,9 @@ class AttentionModule(nn.Module):
                  head_dim: Optional[int] = None, max_positions: int = 4096, rope_theta: float = 10000.0,
                  rope_traditional: bool = False, rope_scaling: Optional[Dict[str, Any]] = None,
                  use_bias: bool = False, use_flash_attention: bool = True, use_flex_attention: bool = False,
-                 flash_block_size: int = 128, apply_rope: bool = False):
+                 flash_block_size: int = 128, apply_rope: bool = False, rope_layout: str = "interleaved"):
         super().__init__()
+        self.rope_layout = rope_layout
         if use_flex_attention:
             raise NotImplementedError("FlexAttention (arch/flex_attention.py) is out of scope of the hot path")
         self.hidden_size = hidden_size
@@ -101,7 +111,7 @@ class AttentionModule(nn.Module):
     def forward(self, x: torch.Tensor, mask=None, position_ids=None) -> torch.Tensor:
         if self.apply_rope and self.attn.rope_tables is None:
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
-        return self.attn(x, mask=mask)
+        return self.attn(x, mask=mask, rope_layout=self.rope_layout)
 
     def cached(self, x: torch.Tensor, cache: "KVCache", layer: int, window: Optional[int] = None) -> torch.Tensor:
         """This layer's attention against the KV cache: prefill when x is [B, S, hidden], one decode step when x is
@@ -109,14 +119,19 @@ class AttentionModule(nn.Module):
         if self.apply_rope and self.attn.rope_tables is None:
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
         if x.dim() == 3:
-            return self.attn.forward_prefill(x, CausalMask(x.shape[1], window), cache.k[layer], cache.v[layer])
-        return self.attn.forward_decode(x, cache.k[layer], cache.v[layer], cache.lens, cache.workspace, window)
+            return self.attn.forward_prefill(x, CausalMask(x.shape[1], window), cache.k[layer], cache.v[layer],
+                                             self.rope_layout)
+        return self.attn.forward_decode(x, cache.k[layer], cache.v[layer], cache.lens, cache.workspace, window,
+                                        self.rope_layout)
 
 
 class TransformerBlock(nn.Module):
     def __init__(self, args: ModelArgs):
         super().__init__()
         inter = args.intermediate_size or 4 * args.hidden_size
+        if args.variant not in VARIANTS:
+            raise ValueError(f"ModelArgs.variant must be one of {VARIANTS}, got {args.variant!r}")
+        mlx_lm = args.variant == "mlx_lm"
         self.input_layernorm = RMSNorm(args.hidden_size, eps=args.rms_norm_eps)
         self.self_attn = AttentionModule(
             hidden_size=args.hidden_size, num_heads=args.num_attention_heads,
@@ -125,9 +140,10 @@ class TransformerBlock(nn.Module):
             rope_traditional=args.rope_traditional, rope_scaling=args.rope_scaling,
             use_bias=args.attention_bias, use_flash_attention=args.use_flash_attention,
             use_flex_attention=args.use_flex_attention, flash_block_size=args.flash_block_size,
-            apply_rope=args.apply_rope)
+            apply_rope=args.apply_rope or mlx_lm,
+            rope_layout="half" if mlx_lm and not args.rope_traditional else "interleaved")
         self.post_attention_layernorm = RMSNorm(args.hidden_size, eps=args.rms_norm_eps)
-        self.mlp = MLP(args.hidden_size, inter, use_bias=args.mlp_bias)
+        self.mlp = MLP(args.hidden_size, inter, use_bias=args.mlp_bias, act="silu" if mlx_lm else "sigmoid2")
 
     def forward(self, x: torch.Tensor, mask=None, position_ids=None) -> torch.Tensor:
         x = x + self.self_attn(self.input_layernorm(x), mask=mask, position_ids=position_ids)

@@ -69,6 +69,17 @@ class ModelConfig:
         w = self.attention.get("sliding_window")
         if w is not None and (isinstance(w, bool) or not isinstance(w, int) or w < 0):
             raise ValueError(f"model.attention.sliding_window must be null or a non-negative integer, got {w!r}")
+        # extension: misc.variant selects the block (absent / null / "reference": arch/llama.py's; "mlx_lm": the
+        # mlx_lm.models.llama block the reference's trainer actually imports, DESIGN D4)
+        v = (self.misc or {}).get("variant")
+        if v is not None and (not isinstance(v, str) or v not in ("reference", "mlx_lm")):
+            raise ValueError(f"model.misc.variant must be null, 'reference' or 'mlx_lm', got {v!r}")
+        if v == "mlx_lm":
+            if self.rope.get("enabled", True) is False:
+                raise ValueError("model.misc.variant: mlx_lm always applies RoPE; rope.enabled: false contradicts it")
+            if self.rope.get("scaling") is not None:
+                raise ValueError(f"model.misc.variant: mlx_lm does not support rope.scaling "
+                                 f"(got {self.rope.get('scaling')!r}); set it to null")
 
 
 @dataclass
@@ -657,8 +668,8 @@ class Trainer:
             use_flash_attention=m.attention.get("use_flash_attention", True),
             use_flex_attention=m.attention.get("use_flex_attention", False),
             flash_block_size=m.attention.get("flash_block_size", 128),
-            apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")),
-            sliding_window=m.attention.get("sliding_window"))
+            apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")) or m.misc.get("variant") == "mlx_lm",
+            sliding_window=m.attention.get("sliding_window"), variant=m.misc.get("variant"))
         self.model_args = args
         model = Model(args)
         init_model_(model, args, self.config.system.seed)

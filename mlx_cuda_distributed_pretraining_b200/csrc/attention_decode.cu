@@ -397,6 +397,53 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
   }
 }
 
+// kv_append_kernel for the half-split layout: one thread per 8-column slice pair (columns [8 dv, 8 dv + 8) and the
+// same D/2 later) of a q, k or v head.  q and k are rotated by rope_half8, b200_rope_half's own rotation.
+template <typename T>
+__global__ void __launch_bounds__(256)
+kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v, T* __restrict__ k_cache,
+                      T* __restrict__ v_cache, const int* __restrict__ lens, const float* __restrict__ cos_t,
+                      const float* __restrict__ sin_t, long long nslice, int s_max, int H, int Hk, int D) {
+  const int L = D / 16;
+  const int heads = H + 2 * Hk;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nslice; i += (long long)gridDim.x * blockDim.x) {
+    const int dv = (int)(i % L);
+    const int hh = (int)(i / L % heads);
+    const int b = (int)(i / L / heads);
+    const int pos = lens[b] - 1;
+    if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
+    const T* src;
+    T* dst;
+    bool rotate = true;
+    if (hh < H) {
+      src = dst = q + ((long long)b * H + hh) * D + dv * 8;
+    } else if (hh < H + Hk) {
+      const int h = hh - H;
+      src = k + ((long long)b * Hk + h) * D + dv * 8;
+      dst = k_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+    } else {
+      const int h = hh - H - Hk;
+      src = v + ((long long)b * Hk + h) * D + dv * 8;
+      dst = v_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+      rotate = false;
+    }
+    float xl[8], xh[8];
+    ld8(src, xl);
+    ld8(src + D / 2, xh);
+    if (rotate) {
+      float c[8], sn[8], ol[8], oh[8];
+      ld8(cos_t + (long long)pos * (D / 2) + dv * 8, c);
+      ld8(sin_t + (long long)pos * (D / 2) + dv * 8, sn);
+      rope_half8(xl, xh, c, sn, ol, oh);
+      st8(dst, ol);
+      st8(dst + D / 2, oh);
+    } else {
+      st8(dst, xl);
+      st8(dst + D / 2, xh);
+    }
+  }
+}
+
 bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 }  // namespace
@@ -488,6 +535,30 @@ int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cach
     kv_append_kernel<float><<<(int)blocks, 256, 0, stream>>>((float*)q, (const float*)k, (const float*)v,
                                                              (float*)k_cache, (float*)v_cache, lens, cos_t, sin_t,
                                                              nvec, s_max, H, Hk, D);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// kv_append with the half-split rotation of b200_rope_half; the tables are required and D % 16 == 0
+int kv_append_half(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                   const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                   cudaStream_t stream) {
+  B200_CHECK_ARG(B > 0 && s_max > 0 && H > 0 && Hk > 0 && D > 0 && D % 16 == 0,
+                 "kv_append_half: bad shape B=%d s_max=%d H=%d Hk=%d D=%d (D %% 16 == 0)", B, s_max, H, Hk, D);
+  B200_CHECK_ARG(cos_t != nullptr && sin_t != nullptr && lens != nullptr, "kv_append_half: RoPE tables and lens required");
+  B200_CHECK_ARG(al16(q) && al16(k) && al16(v) && al16(k_cache) && al16(v_cache) && al16(cos_t) && al16(sin_t),
+                 "kv_append_half: alignment");
+  const long long nslice = (long long)B * (H + 2 * Hk) * (D / 16);
+  long long blocks = (nslice + 255) / 256;
+  if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+  if (is_bf16)
+    kv_append_half_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, stream>>>(
+        (__nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (__nv_bfloat16*)k_cache,
+        (__nv_bfloat16*)v_cache, lens, cos_t, sin_t, nslice, s_max, H, Hk, D);
+  else
+    kv_append_half_kernel<float><<<(int)blocks, 256, 0, stream>>>((float*)q, (const float*)k, (const float*)v,
+                                                                  (float*)k_cache, (float*)v_cache, lens, cos_t,
+                                                                  sin_t, nslice, s_max, H, Hk, D);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

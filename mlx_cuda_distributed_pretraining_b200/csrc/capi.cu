@@ -25,9 +25,9 @@ struct NsGroup {
 size_t newton_schulz_multi_workspace_bytes(const NsGroup* g, int n, int steps);
 int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, float c, void* ws, size_t ws_bytes,
                         cudaStream_t stream);
-int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, cudaStream_t stream);
-int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
-                      cudaStream_t stream);
+int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, int silu, cudaStream_t stream);
+int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I, int silu,
+                 cudaStream_t stream);
 size_t embedding_bwd_workspace_bytes(int V, int H);
 int embedding_bwd(const void* dh, const long long* tokens, void* grad, int grad_is_bf16, long long rows, int V, int H,
                   void* ws, size_t ws_bytes, cudaStream_t stream);
@@ -96,6 +96,10 @@ int rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, 
          int D, int backward, int is_bf16, cudaStream_t stream);
 int rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
              int D, int backward, int is_bf16, cudaStream_t stream);
+int rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
+              int D, int backward, int is_bf16, cudaStream_t stream);
+int silu_glu_fwd(const void* g, const void* u, void* y, long long n, cudaStream_t stream);
+int silu_glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, cudaStream_t stream);
 int glu_fwd(const void* g, const void* u, void* y, long long n, cudaStream_t stream);
 int glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, cudaStream_t stream);
 int ce_fwd(const void* logits, long long ld, const long long* targets, int rows, int V, long long pad_token,
@@ -129,6 +133,9 @@ int attn_decode(const void* q, const void* k_cache, const void* v_cache, const i
 int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
               const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
               cudaStream_t stream);
+int kv_append_half(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                   const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                   cudaStream_t stream);
 }  // namespace b200
 
 #define S_(x) reinterpret_cast<cudaStream_t>(x)
@@ -218,11 +225,18 @@ int b200_newton_schulz_multi(const b200_ns_group* groups, int n_groups, int step
                                    workspace_bytes, S_(stream));
 }
 int b200_mlp_gateup_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, void* stream) {
-  return b200::gemm_glu_fwd(x, W2, gu, y, M, K, I, S_(stream));
+  return b200::gemm_glu_fwd(x, W2, gu, y, M, K, I, 0, S_(stream));
 }
 int b200_mlp_down_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
                           void* stream) {
-  return b200::gemm_glu_bwd(dy, Wd, gu, dgu, M, H, I, S_(stream));
+  return b200::gemm_glu_bwd(dy, Wd, gu, dgu, M, H, I, 0, S_(stream));
+}
+int b200_mlp_gateup_silu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, void* stream) {
+  return b200::gemm_glu_fwd(x, W2, gu, y, M, K, I, 1, S_(stream));
+}
+int b200_mlp_down_silu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
+                           void* stream) {
+  return b200::gemm_glu_bwd(dy, Wd, gu, dgu, M, H, I, 1, S_(stream));
 }
 size_t b200_embedding_bwd_workspace_bytes(int V, int H) { return b200::embedding_bwd_workspace_bytes(V, H); }
 int b200_embedding_bwd(const void* dh, const long long* tokens, void* grad, int grad_is_bf16, long long rows,
@@ -363,6 +377,16 @@ int b200_rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t
                   int NH, int D, int backward, int is_bf16, void* stream) {
   return b200::rope_pos(x, y, cos_t, sin_t, pos, B, S, NH, D, backward, is_bf16, S_(stream));
 }
+int b200_rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S,
+                   int NH, int D, int backward, int is_bf16, void* stream) {
+  return b200::rope_half(x, y, cos_t, sin_t, pos, B, S, NH, D, backward, is_bf16, S_(stream));
+}
+int b200_silu_glu_fwd(const void* g, const void* u, void* y, long long n, void* stream) {
+  return b200::silu_glu_fwd(g, u, y, n, S_(stream));
+}
+int b200_silu_glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, void* stream) {
+  return b200::silu_glu_bwd(dy, g, u, dg, du, n, S_(stream));
+}
 int b200_glu_fwd(const void* g, const void* u, void* y, long long n, void* stream) {
   return b200::glu_fwd(g, u, y, n, S_(stream));
 }
@@ -445,6 +469,12 @@ int b200_kv_append(void* q, const void* k, const void* v, void* k_cache, void* v
                    const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
                    void* stream) {
   return b200::kv_append(q, k, v, k_cache, v_cache, lens, cos_t, sin_t, B, s_max, H, Hk, D, is_bf16, S_(stream));
+}
+int b200_kv_append_half(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                        const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                        void* stream) {
+  return b200::kv_append_half(q, k, v, k_cache, v_cache, lens, cos_t, sin_t, B, s_max, H, Hk, D, is_bf16,
+                              S_(stream));
 }
 
 }  // extern "C"

@@ -325,4 +325,16 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// Half-split RoPE (mlx_lm's nn.RoPE(traditional=False), HF Llama's rotate_half) on one 8-column slice: lo = x[c..c+8),
+// hi = x[c+D/2..c+D/2+8), c / s the cos / sin of the pairs' angles.  b200_rope_half and b200_kv_append_half both rotate
+// through this one function, so a token rotated at decode is bit-equal to the same token rotated by the prefill.
+__device__ __forceinline__ void rope_half8(const float* lo, const float* hi, const float* c, const float* s, float* olo,
+                                           float* ohi) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    olo[k] = lo[k] * c[k] - hi[k] * s[k];
+    ohi[k] = lo[k] * s[k] + hi[k] * c[k];
+  }
+}
+
 }  // namespace b200

@@ -143,6 +143,49 @@ __device__ __forceinline__ float fast_sigmoid(float x) {
   return fmaf(0.5f, t, 0.5f);
 }
 
+// sigmoid with a small RELATIVE error over the whole range, for the SiLU epilogues: silu(g) = g sigmoid(g) is used
+// deep in the negative tail (sigmoid(-8) = 3.4e-4), where fast_sigmoid's 2^-12 absolute error would be tens of
+// percent.  ex2.approx and rcp.approx are each within about 2^-22 relative; rounding -x log2(e) adds |x| 2^-24 ln 2.
+// Large negative x: 2^(-x log2 e) overflows to inf and the result is 0, below bf16's smallest normal anyway.
+__device__ __forceinline__ float rel_sigmoid(float x) {
+  float e, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+  return r;
+}
+
+// Epi 1's activation y(g, u) from the fp32 accumulators.  SiLU: rel_sigmoid inlined, with g entering only through
+// t = -g log2(e) and y = t (-u ln 2) / (1 + 2^t): the pass then keeps one value per g and one per u live, as the
+// reference activation does (g reused after the exponent pushed the pass past the register budget).
+template <bool SILU>
+__device__ __forceinline__ float glu_y(float g, float u) {
+  if constexpr (SILU) {
+    const float t = g * -1.4426950408889634f;
+    float e, r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(t));
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+    return t * (u * -0.6931471805599453f) * r;
+  } else {
+    return g * fast_sigmoid(u) * 2.0f;
+  }
+}
+
+// Epi 2's adjoint of y(g, u) at d = dL/dy:
+//   reference: dg = d s(u) 2,                       du = d g s(u) (1 - s(u)) 2
+//   SiLU:      dg = d u s(g) (1 + g (1 - s(g))),    du = d g s(g)
+template <bool SILU>
+__device__ __forceinline__ void glu_adjoint(float d, float g, float u, float& dg, float& du) {
+  if constexpr (SILU) {
+    const float s = rel_sigmoid(g);
+    dg = d * u * s * fmaf(g, 1.0f - s, 1.0f);
+    du = d * (g * s);
+  } else {
+    const float s = fast_sigmoid(u);
+    dg = d * s * 2.0f;
+    du = d * g * s * (1.0f - s) * 2.0f;
+  }
+}
+
 // One tile's k-blocks [kb_begin, kb_end) from the ring: acc[0, 64) = rows [0, 64), acc[64, 128) = rows [64, 128).
 template <int TA, int TB>
 __device__ __forceinline__ void mainloop(float* acc, uint32_t sbase, uint32_t full0, uint32_t empty0, int n_kb,
@@ -225,6 +268,48 @@ __device__ __forceinline__ void glu_half_store(const CUtensorMap* m, uint32_t st
     for (int gu = 0; gu < 2; ++gu) tma_store_3d(m, stg + h * HALF_BYTES + gu * BOX_BYTES, col0 + 64 * h, gu, row0);
 }
 
+// Epi 1's second pass: y of the 64 output columns (gate accumulators [0, 64), up [64, 128)) into staging half 0.
+template <bool SILU>
+__device__ __forceinline__ void glu_y_tile(const float* acc, uint32_t stg, int warp, int lane) {
+#pragma unroll
+  for (int hm = 0; hm < 2; ++hm)
+#pragma unroll
+    for (int j = 0; j < 8; j += 2) {
+      const float* g = acc + 64 * hm + 4 * j;
+      const float* u = g + 32;
+      uint32_t yv[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) yv[q] = pack_bf16x2(glu_y<SILU>(g[2 * q], u[2 * q]), glu_y<SILU>(g[2 * q + 1], u[2 * q + 1]));
+      stmatrix_x4(frag_addr(stg, 64 * hm, warp, j, lane), yv[0], yv[1], yv[2], yv[3]);
+    }
+}
+
+// Epi 2 on one 64-row half: staging rows [0, 64) hold g, [64, 128) u; acc = d of those rows.  Each warp reads and
+// rewrites only its own 16 rows, so dg and du replace g and u in place.
+template <bool SILU>
+__device__ __forceinline__ void glu_adjoint_half(const float* acc, uint32_t stg, int warp, int lane) {
+#pragma unroll
+  for (int j = 0; j < 16; j += 2) {
+    const uint32_t ga = frag_addr(stg, 0, warp, j, lane), ua = frag_addr(stg, 64, warp, j, lane);
+    uint32_t gq[4], uq[4], dg[4], du[4];
+    ldmatrix_x4(ga, gq);
+    ldmatrix_x4(ua, uq);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {  // q = (column group j + q / 2, row half q % 2)
+      const float* a = acc + 4 * (j + (q >> 1)) + 2 * (q & 1);
+      const float2 gg = unpack_bf16x2(gq[q]), uu = unpack_bf16x2(uq[q]);
+      float dg0, du0, dg1, du1;
+      glu_adjoint<SILU>(a[0], gg.x, uu.x, dg0, du0);
+      glu_adjoint<SILU>(a[1], gg.y, uu.y, dg1, du1);
+      dg[q] = pack_bf16x2(dg0, dg1);
+      du[q] = pack_bf16x2(du0, du1);
+    }
+    __syncwarp();
+    stmatrix_x4(ga, dg[0], dg[1], dg[2], dg[3]);
+    stmatrix_x4(ua, du[0], du[1], du[2], du[3]);
+  }
+}
+
 // Closes a bulk group of the leader's stores.  `drain` after the warpgroup's last tile: the CTA's shared memory must
 // outlive the stores reading it.
 __device__ __forceinline__ void commit_stores(bool drain) {
@@ -232,6 +317,10 @@ __device__ __forceinline__ void commit_stores(bool drain) {
   if (drain) bulk_wait<0>();
 }
 
+// SILU selects epi 1/2's activation at compile time: g sigmoid(u) 2 (the reference block) or silu(g) u (SiLU-GLU).
+// A run-time flag cost the kernel spills at its 168-register budget; the SILU = false instantiation is the engine
+// every other launch uses.
+template <bool SILU>
 __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ Args g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -429,18 +518,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
         bulk_wait_read<1>();  // the gate half has been read: y goes there
       }
       named_bar_sync(bar_wg, 128);
-#pragma unroll
-      for (int hm = 0; hm < 2; ++hm)
-#pragma unroll
-        for (int j = 0; j < 8; j += 2) {  // y = g sigmoid(u) 2 from the fp32 accumulators
-          const float* g = acc + 64 * hm + 4 * j;
-          const float* u = g + 32;
-          uint32_t yv[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q)
-            yv[q] = pack_bf16x2(g[2 * q] * fast_sigmoid(u[2 * q]) * 2.0f, g[2 * q + 1] * fast_sigmoid(u[2 * q + 1]) * 2.0f);
-          stmatrix_x4(frag_addr(stg, 64 * hm, warp, j, lane), yv[0], yv[1], yv[2], yv[3]);
-        }
+      glu_y_tile<SILU>(acc, stg, warp, lane);  // y from the fp32 accumulators
       fence_proxy_async_smem();
       named_bar_sync(bar_wg, 128);
       if (leader) {
@@ -451,7 +529,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
       continue;
     }
 
-    if (p.epi == 2) {  // acc = d = dy Wd; dg = d s 2, du = d g s (1 - s) 2 with g, u from the saved gu
+    if (p.epi == 2) {  // acc = d = dy Wd; dg, du = glu_adjoint(d, g, u) with g, u from the saved gu
 #pragma unroll
       for (int hm = 0; hm < 2; ++hm) {  // staging rows [0, 64): g, [64, 128): u of tile rows [64 hm, 64 hm + 64)
         if (hm && leader) {  // the producer loaded the first half; load the second once its stores have read the tile
@@ -461,25 +539,7 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
         }
         mbar_wait_outlined(epi_full, epi_phase);
         epi_phase ^= 1u;
-#pragma unroll
-        for (int j = 0; j < 16; j += 2) {  // each warp reads and rewrites only its own 16 rows: in place
-          const uint32_t ga = frag_addr(stg, 0, warp, j, lane), ua = frag_addr(stg, 64, warp, j, lane);
-          uint32_t gq[4], uq[4], dg[4], du[4];
-          ldmatrix_x4(ga, gq);
-          ldmatrix_x4(ua, uq);
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {  // q = (column group j + q / 2, row half q % 2)
-            const float* a = acc + 64 * hm + 4 * (j + (q >> 1)) + 2 * (q & 1);
-            const float2 gg = unpack_bf16x2(gq[q]), uu = unpack_bf16x2(uq[q]);
-            const float d0 = a[0], d1 = a[1];
-            const float s0 = fast_sigmoid(uu.x), s1 = fast_sigmoid(uu.y);
-            dg[q] = pack_bf16x2(d0 * s0 * 2.0f, d1 * s1 * 2.0f);
-            du[q] = pack_bf16x2(d0 * gg.x * s0 * (1.0f - s0) * 2.0f, d1 * gg.y * s1 * (1.0f - s1) * 2.0f);
-          }
-          __syncwarp();
-          stmatrix_x4(ga, dg[0], dg[1], dg[2], dg[3]);
-          stmatrix_x4(ua, du[0], du[1], du[2], du[3]);
-        }
+        glu_adjoint_half<SILU>(acc + 64 * hm, stg, warp, lane);
         fence_proxy_async_smem();
         named_bar_sync(bar_wg, 128);
         if (leader) {
@@ -649,7 +709,7 @@ Problem base_problem(int M, int N, int K, int batch, int tiles_n, int epi) {
   return q;
 }
 
-int launch(Args& a, int n, cudaStream_t stream) {
+int launch(Args& a, int n, cudaStream_t stream, bool silu = false) {
   int work = 0;
   for (int i = 0; i < n; ++i) {
     a.p[i].work_begin = work;
@@ -657,12 +717,15 @@ int launch(Args& a, int n, cudaStream_t stream) {
   }
   a.n_problems = n;
   a.total_work = work;
-  static bool attr_set = false;
-  if (!attr_set) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(gemm_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    attr_set = true;
+  static bool attr_set[2] = {false, false};
+  if (!attr_set[silu]) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(silu ? gemm_wgmma_kernel<true> : gemm_wgmma_kernel<false>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    attr_set[silu] = true;
   }
-  gemm_wgmma_kernel<<<work < num_sms() ? work : num_sms(), THREADS, SMEM_BYTES, stream>>>(a);
+  const int grid = work < num_sms() ? work : num_sms();
+  if (silu) gemm_wgmma_kernel<true><<<grid, THREADS, SMEM_BYTES, stream>>>(a);
+  else gemm_wgmma_kernel<false><<<grid, THREADS, SMEM_BYTES, stream>>>(a);
   B200_CHECK_LAUNCH();
   for (int i = 0; i < n; ++i) {
     const Problem& q = a.p[i];
@@ -760,9 +823,11 @@ int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* 
                       stream);
 }
 
-// ---- fused MLP GEMMs (arch/llama.py:142-151: down(gate(x) * sigmoid(up(x)) * 2)) --------------------------
-// gu[M, 2I] = x[M, K] [Wg ; Wu]^T (W2: [2I, K] row-major, gate rows first), y[M, I] = g * sigmoid(u) * 2
-int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, cudaStream_t stream) {
+// ---- fused MLP GEMMs (arch/llama.py:142-151: down(gate(x) * sigmoid(up(x)) * 2); silu: mlx_lm's
+// down(silu(gate(x)) * up(x))) ----------------------------------------------------------------------------------
+// gu[M, 2I] = x[M, K] [Wg ; Wu]^T (W2: [2I, K] row-major, gate rows first), y[M, I] = g * sigmoid(u) * 2, or
+// silu(g) * u with `silu`
+int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, int silu, cudaStream_t stream) {
   B200_CHECK_ARG(M > 0 && K > 0 && I > 0 && K % 8 == 0 && I % 128 == 0,
                  "mlp_glu_fwd: need K %% 8 == 0 and intermediate size %% 128 == 0 (M=%d K=%d I=%d)", M, K, I);
   Args a;
@@ -778,12 +843,14 @@ int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K,
   q.ld_aux = I;
   if ((rc = glu_map(&a.tmD[0], gu, I, M, q.ldd))) return rc;
   if ((rc = tile_map(&a.tmE[0], y, I, M, 1, I, 0))) return rc;
-  return launch(a, 1, stream);
+  return launch(a, 1, stream, silu != 0);
 }
 
 // dgu[M, 2I] = GLU adjoint of d = dy[M, H] Wd (Wd: [H, I] row-major = down_proj.weight), gu[M, 2I] the saved
-// forward activations: dg = d * sigmoid(u) * 2 ; du = d * g * sigmoid(u) * (1 - sigmoid(u)) * 2
-int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I, cudaStream_t stream) {
+// forward activations: dg = d * sigmoid(u) * 2 ; du = d * g * sigmoid(u) * (1 - sigmoid(u)) * 2, or with `silu`
+// dg = d * u * sigmoid(g) * (1 + g * (1 - sigmoid(g))) ; du = d * silu(g)
+int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I, int silu,
+                 cudaStream_t stream) {
   B200_CHECK_ARG(M > 0 && H > 0 && I > 0 && H % 8 == 0 && I % 8 == 0, "mlp_glu_bwd: bad shape M=%d H=%d I=%d", M, H, I);
   Args a;
   int rc;
@@ -800,7 +867,7 @@ int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int 
   q.ld_aux = 2LL * I;
   if ((rc = glu_map(&a.tmD[0], dgu, I, M, q.ldd))) return rc;
   if ((rc = glu_map(&a.tmE[0], gu, I, M, q.ld_aux))) return rc;
-  return launch(a, 1, stream);
+  return launch(a, 1, stream, silu != 0);
 }
 
 // ---- grouped launch: up to MAX_PROBLEMS independent batched problems in one grid ----------------------------

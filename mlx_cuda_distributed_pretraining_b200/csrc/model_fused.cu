@@ -2,6 +2,7 @@
 // single HBM passes.
 //
 //  glu_fwd / glu_bwd   arch/llama.py:151   y = gate * sigmoid(up) * 2            (sic: not SiLU-GLU)
+//  silu_glu_fwd / _bwd mlx_lm's Llama MLP  y = silu(gate) * up                   (model.misc.variant: mlx_lm)
 //  ce_fwd  / ce_bwd    core/training.py:1226-1234  per-token cross entropy on fp32-upcast logits with
 //                      the pad mask; never materialises the fp32 [B,S,V] copy of the logits.  The
 //                      backward overwrites the logits buffer with d(loss)/d(logits) in place.
@@ -57,6 +58,41 @@ glu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __rest
       const float s = sigmoidf_(uv[j]);
       og[j] = dv[j] * s * 2.0f;
       ou[j] = dv[j] * gv[j] * s * (1.0f - s) * 2.0f;
+    }
+    st8f(dg + i * 8, og);
+    st8f(du + i * 8, ou);
+  }
+}
+
+// silu(g) u and its adjoint dg = d u s (1 + g (1 - s)), du = d g s with s = sigmoid(g).  sigmoidf_ is relatively
+// accurate in the negative tail, where silu(g) is small.
+__global__ void __launch_bounds__(256)
+silu_glu_fwd_kernel(const __nv_bfloat16* __restrict__ g, const __nv_bfloat16* __restrict__ u,
+                    __nv_bfloat16* __restrict__ y, long long nvec) {
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nvec; i += (long long)gridDim.x * 256) {
+    float gv[8], uv[8], o[8];
+    ld8f(g + i * 8, gv);
+    ld8f(u + i * 8, uv);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j] = gv[j] * sigmoidf_(gv[j]) * uv[j];
+    st8f(y + i * 8, o);
+  }
+}
+
+__global__ void __launch_bounds__(256)
+silu_glu_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ g,
+                    const __nv_bfloat16* __restrict__ u, __nv_bfloat16* __restrict__ dg,
+                    __nv_bfloat16* __restrict__ du, long long nvec) {
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < nvec; i += (long long)gridDim.x * 256) {
+    float dv[8], gv[8], uv[8], og[8], ou[8];
+    ld8f(dy + i * 8, dv);
+    ld8f(g + i * 8, gv);
+    ld8f(u + i * 8, uv);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float s = sigmoidf_(gv[j]);
+      og[j] = dv[j] * uv[j] * s * fmaf(gv[j], 1.0f - s, 1.0f);
+      ou[j] = dv[j] * (gv[j] * s);
     }
     st8f(dg + i * 8, og);
     st8f(du + i * 8, ou);
@@ -225,6 +261,25 @@ int glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, lo
   glu_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)g,
                                                      (const __nv_bfloat16*)u, (__nv_bfloat16*)dg,
                                                      (__nv_bfloat16*)du, n / 8);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+int silu_glu_fwd(const void* g, const void* u, void* y, long long n, cudaStream_t stream) {
+  B200_CHECK_ARG(n > 0 && n % 8 == 0, "silu_glu_fwd: n=%lld must be a positive multiple of 8", n);
+  B200_CHECK_ARG(al16(g) && al16(u) && al16(y), "silu_glu_fwd: 16-byte alignment required");
+  silu_glu_fwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>((const __nv_bfloat16*)g, (const __nv_bfloat16*)u,
+                                                          (__nv_bfloat16*)y, n / 8);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+int silu_glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, cudaStream_t stream) {
+  B200_CHECK_ARG(n > 0 && n % 8 == 0, "silu_glu_bwd: n=%lld must be a positive multiple of 8", n);
+  B200_CHECK_ARG(al16(dy) && al16(g) && al16(u) && al16(dg) && al16(du), "silu_glu_bwd: alignment");
+  silu_glu_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)g,
+                                                          (const __nv_bfloat16*)u, (__nv_bfloat16*)dg,
+                                                          (__nv_bfloat16*)du, n / 8);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

@@ -1,5 +1,5 @@
-// RMSNorm (arch/llama.py:50-56 of the reference) and interleaved-pair RoPE
-// (arch/llama_standard.py:74-75,117-127) as single-pass vectorised HBM kernels, forward + backward.
+// RMSNorm (arch/llama.py:50-56 of the reference), interleaved-pair RoPE (arch/llama_standard.py:74-75,117-127) and
+// half-split RoPE (mlx_lm's nn.RoPE(traditional=False)) as single-pass vectorised HBM kernels, forward + backward.
 #include "common.cuh"
 #include "host.h"
 
@@ -460,6 +460,37 @@ rope_kernel(const T* __restrict__ x, T* __restrict__ y, const float* __restrict_
   }
 }
 
+// Half-split RoPE: pairs (x[i], x[i + D/2]) for i < D/2, angle of pair i as in rope_kernel.  One thread per 8-column
+// slice i in [8 dv, 8 dv + 8): it loads the 16-byte vectors at column 8 dv and at 8 dv + D/2, both coalesced across
+// the warp, which needs D % 16 == 0.  Backward: sign = -1.
+template <typename T, bool POS>
+__global__ void __launch_bounds__(256)
+rope_half_kernel(const T* __restrict__ x, T* __restrict__ y, const float* __restrict__ cos_t,
+                 const float* __restrict__ sin_t, long long nslice, int S, int NH, int D, float sign,
+                 const int* __restrict__ pos) {
+  const int per_head = D / 16;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nslice;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int dv = (int)(i % per_head);
+    const long long head = i / per_head;  // (b*S + s)*NH + h
+    const long long t = head / NH;        // token index b*S + s
+    int s;
+    if constexpr (POS) s = __ldg(pos + t);
+    else s = (int)(t % S);
+    const long long lo = head * D + dv * 8, hi = lo + D / 2;
+    float xl[8], xh[8], c[8], sn[8], ol[8], oh[8];
+    ld8(x + lo, xl);
+    ld8(x + hi, xh);
+    ld8(cos_t + (long long)s * (D / 2) + dv * 8, c);
+    ld8(sin_t + (long long)s * (D / 2) + dv * 8, sn);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) sn[k] *= sign;
+    rope_half8(xl, xh, c, sn, ol, oh);
+    st8(y + lo, ol);
+    st8(y + hi, oh);
+  }
+}
+
 constexpr int RW_MAX_H = 1024;  // NVW <= 4: beyond that the packed row no longer fits 128 registers
 
 template <typename T>
@@ -637,6 +668,31 @@ int rope_impl(const void* x, void* y, const float* cos_t, const float* sin_t, co
 }
 
 }  // namespace
+
+// pos: nullable int32 [B, S]; D % 16 == 0 (both halves of a slice are 16-byte vectors)
+int rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
+              int D, int backward, int is_bf16, cudaStream_t stream) {
+  B200_CHECK_ARG(B > 0 && S > 0 && NH > 0 && D > 0 && D % 16 == 0, "rope_half: D=%d must be a multiple of 16", D);
+  B200_CHECK_ARG(al16(x) && al16(y) && al16(cos_t) && al16(sin_t) && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
+                 "rope_half: alignment");
+  const long long nslice = (long long)B * S * NH * D / 16;
+  long long blocks = (nslice + 255) / 256;
+  if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+  const float sign = backward ? -1.0f : 1.0f;
+  auto launch = [&](auto kern, auto* xx, auto* yy) {
+    kern<<<(int)blocks, 256, 0, stream>>>(xx, yy, cos_t, sin_t, nslice, S, NH, D, sign, pos);
+  };
+  using bf = __nv_bfloat16;
+  if (is_bf16) {
+    if (pos) launch(rope_half_kernel<bf, true>, (const bf*)x, (bf*)y);
+    else launch(rope_half_kernel<bf, false>, (const bf*)x, (bf*)y);
+  } else {
+    if (pos) launch(rope_half_kernel<float, true>, (const float*)x, (float*)y);
+    else launch(rope_half_kernel<float, false>, (const float*)x, (float*)y);
+  }
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
 
 int rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, int S, int NH,
          int D, int backward, int is_bf16, cudaStream_t stream) {

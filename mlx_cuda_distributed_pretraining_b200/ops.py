@@ -601,9 +601,22 @@ def rope_tables(seq_len: int, head_dim: int, theta: float, device) -> Tuple[torc
     return torch.cos(ang).to(device).contiguous(), torch.sin(ang).to(device).contiguous()
 
 
-def _rope_call(x, y, cos_t, sin_t, pos, backward: int, what: str) -> None:
+ROPE_LAYOUTS = ("interleaved", "half")
+GLU_ACTS = ("sigmoid2", "silu")
+
+
+def _check_choice(value, allowed, what: str) -> str:
+    if not isinstance(value, str) or value not in allowed:
+        raise ValueError(f"{what} must be one of {allowed}, got {value!r}")
+    return value
+
+
+def _rope_call(x, y, cos_t, sin_t, pos, backward: int, what: str, layout: str = "interleaved") -> None:
     B, S, NH, D = x.shape
-    if pos is None:
+    if layout == "half":
+        check(lib().b200_rope_half(x.data_ptr(), y.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), _ptr(pos), B, S,
+                                   NH, D, backward, _is_bf16(x, "x"), _stream()), what)
+    elif pos is None:
         check(lib().b200_rope(x.data_ptr(), y.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), B, S,
                               NH, D, backward, _is_bf16(x, "x"), _stream()), what)
     else:
@@ -613,11 +626,12 @@ def _rope_call(x, y, cos_t, sin_t, pos, backward: int, what: str) -> None:
 
 class _RopeFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, cos_t, sin_t, pos):
+    def forward(ctx, x, cos_t, sin_t, pos, layout):
         xs = x.contiguous()
         y = torch.empty_like(xs)
-        _rope_call(xs, y, cos_t, sin_t, pos, 0, "b200_rope")
+        _rope_call(xs, y, cos_t, sin_t, pos, 0, "b200_rope", layout)
         ctx.save_for_backward(cos_t, sin_t, pos)
+        ctx.layout = layout
         return y
 
     @staticmethod
@@ -625,8 +639,8 @@ class _RopeFn(torch.autograd.Function):
         cos_t, sin_t, pos = ctx.saved_tensors
         dy = dy.contiguous()
         dx = torch.empty_like(dy)
-        _rope_call(dy, dx, cos_t, sin_t, pos, 1, "b200_rope(bwd)")
-        return dx, None, None, None
+        _rope_call(dy, dx, cos_t, sin_t, pos, 1, "b200_rope(bwd)", ctx.layout)
+        return dx, None, None, None, None
 
 
 def _check_pos(pos: torch.Tensor, x: torch.Tensor, what: str) -> torch.Tensor:
@@ -638,12 +652,18 @@ def _check_pos(pos: torch.Tensor, x: torch.Tensor, what: str) -> torch.Tensor:
     return pos.contiguous()
 
 
-def rope(x: torch.Tensor, cos_t: torch.Tensor, sin_t: torch.Tensor, pos: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """x: [B, S, heads, D]; interleaved-pair rotation of token s by the angle of position s, or of pos[b, s] (int32
-    [B, S], the position within its document; the tables must then hold max(pos) + 1 rows) when pos is given."""
+def rope(x: torch.Tensor, cos_t: torch.Tensor, sin_t: torch.Tensor, pos: Optional[torch.Tensor] = None,
+         layout: str = "interleaved") -> torch.Tensor:
+    """x: [B, S, heads, D]; rotation of token s by the angle of position s, or of pos[b, s] (int32 [B, S], the
+    position within its document; the tables must then hold max(pos) + 1 rows) when pos is given.
+    layout "interleaved" rotates pairs (x[2i], x[2i+1]) (b200_rope); "half" rotates (x[i], x[i + D/2]), mlx_lm's
+    nn.RoPE(traditional=False) (b200_rope_half, D % 16 == 0).  Pair i's angle is pos * theta^(-2i/D) in both."""
+    _check_choice(layout, ROPE_LAYOUTS, "rope: layout")
+    if layout == "half" and x.shape[-1] % 16 != 0:
+        raise ValueError(f"rope: the half layout needs head_dim % 16 == 0, got {x.shape[-1]}")
     if pos is not None:
         pos = _check_pos(pos, x, "rope")
-    return _RopeFn.apply(x, cos_t, sin_t, pos)
+    return _RopeFn.apply(x, cos_t, sin_t, pos, layout)
 
 
 def _pad_head_dim(D: int) -> int:
@@ -896,10 +916,13 @@ def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
 
 
 def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
-              lens: torch.Tensor, rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]] = None) -> None:
+              lens: torch.Tensor, rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+              layout: str = "interleaved") -> None:
     """Writes each row's new k [B,Hk,D] and v into the caches at pos = lens[b] - 1 (b200_kv_append).  With
-    rope_tables = (cos, sin) from rope_tables(), k and, in place, q [B,H,D] get the rotation ops.rope applies at
-    position pos, with the same arithmetic.  The caller keeps pos below the tables' length."""
+    rope_tables = (cos, sin) from rope_tables(), k and, in place, q [B,H,D] get the rotation ops.rope(layout=layout)
+    applies at position pos, with the same arithmetic (b200_kv_append_half for the half layout).  The caller keeps
+    pos below the tables' length."""
+    _check_choice(layout, ROPE_LAYOUTS, "kv_append: layout")
     B, H, D, s_max, Hk = _check_cache(q, k_cache, v_cache, lens, "kv_append")
     for t, nm in ((k, "k"), (v, "v")):
         _need(t, q.dtype, f"kv_append: {nm}")
@@ -914,6 +937,13 @@ def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.
             _need(t, torch.float32, f"kv_append: {nm}")
             if t.dim() != 2 or t.shape[1] != D // 2:
                 raise ValueError(f"kv_append: RoPE tables must be [positions, {D // 2}]")
+    if layout == "half" and cos_t is not None:
+        if D % 16 != 0:
+            raise ValueError(f"kv_append: the half layout needs head_dim % 16 == 0, got {D}")
+        check(lib().b200_kv_append_half(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(),
+                                        v_cache.data_ptr(), lens.data_ptr(), cos_t.data_ptr(), sin_t.data_ptr(), B,
+                                        s_max, H, Hk, D, _is_bf16(q, "q"), _stream()), "b200_kv_append_half")
+        return
     check(lib().b200_kv_append(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                lens.data_ptr(), _ptr(cos_t), _ptr(sin_t), B, s_max, H, Hk, D, _is_bf16(q, "q"),
                                _stream()), "b200_kv_append")
@@ -1037,11 +1067,13 @@ def shampoo_graft(p32: torch.Tensor, p16: Optional[torch.Tensor], upd: torch.Ten
 # ------------------------------------------------------------------------------------------------
 class _GluFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, gate, up):
+    def forward(ctx, gate, up, act):
         g, u = gate.contiguous(), up.contiguous()
         y = torch.empty_like(g)
-        check(lib().b200_glu_fwd(g.data_ptr(), u.data_ptr(), y.data_ptr(), g.numel(), _stream()), "b200_glu_fwd")
+        fwd = "b200_silu_glu_fwd" if act == "silu" else "b200_glu_fwd"
+        check(getattr(lib(), fwd)(g.data_ptr(), u.data_ptr(), y.data_ptr(), g.numel(), _stream()), fwd)
         ctx.save_for_backward(g, u)
+        ctx.act = act
         return y
 
     @staticmethod
@@ -1049,9 +1081,10 @@ class _GluFn(torch.autograd.Function):
         g, u = ctx.saved_tensors
         dy = dy.contiguous()
         dg, du = torch.empty_like(g), torch.empty_like(u)
-        check(lib().b200_glu_bwd(dy.data_ptr(), g.data_ptr(), u.data_ptr(), dg.data_ptr(), du.data_ptr(),
-                                 g.numel(), _stream()), "b200_glu_bwd")
-        return dg, du
+        bwd = "b200_silu_glu_bwd" if ctx.act == "silu" else "b200_glu_bwd"
+        check(getattr(lib(), bwd)(dy.data_ptr(), g.data_ptr(), u.data_ptr(), dg.data_ptr(), du.data_ptr(),
+                                  g.numel(), _stream()), bwd)
+        return dg, du, None
 
 
 _EMB_WS = {}
@@ -1112,22 +1145,24 @@ class _MlpFn(torch.autograd.Function):
                 d[Wg ; Wu] += [dg | du]^T x                              ONE library GEMM into the flat gradient
 
     Needs gate_proj.weight and up_proj.weight adjacent in memory (flat.ParamStore) with flat-buffer gradients,
-    bf16, intermediate size % 128 == 0; `mlp()` falls back to the unfused path otherwise."""
+    bf16, intermediate size % 128 == 0; `mlp()` falls back to the unfused path otherwise.  act "silu" runs mlx_lm's
+    down(silu(gate(x)) * up(x)) through b200_mlp_gateup_silu_fwd / b200_mlp_down_silu_bwd instead."""
 
     @staticmethod
-    def forward(ctx, x, wg, wu, wd):
+    def forward(ctx, x, wg, wu, wd, act):
         I, K = wg.shape
         x2 = x.reshape(-1, K).contiguous()
         M = x2.shape[0]
         gu = torch.empty((M, 2 * I), device=x.device, dtype=torch.bfloat16)
         y = torch.empty((M, I), device=x.device, dtype=torch.bfloat16)
+        fwd = "b200_mlp_gateup_silu_fwd" if act == "silu" else "b200_mlp_gateup_glu_fwd"
         tok = _t0("mlp_glu_fwd")
-        check(lib().b200_mlp_gateup_glu_fwd(x2.data_ptr(), wg.data_ptr(), gu.data_ptr(), y.data_ptr(), M, K, I,
-                                            _stream()), "b200_mlp_gateup_glu_fwd")
+        check(getattr(lib(), fwd)(x2.data_ptr(), wg.data_ptr(), gu.data_ptr(), y.data_ptr(), M, K, I, _stream()), fwd)
         _t1(tok)
         out = y @ wd.t()
         ctx.save_for_backward(x2, gu, y, wg, wu, wd)
         ctx.x_shape = x.shape
+        ctx.act = act
         return out.view(*x.shape[:-1], wd.shape[0])
 
     @staticmethod
@@ -1139,15 +1174,15 @@ class _MlpFn(torch.autograd.Function):
         d2 = dout.reshape(-1, H).contiguous()
         wd.grad.addmm_(d2.t(), y)                                   # dWd
         dgu = torch.empty((M, 2 * I), device=d2.device, dtype=torch.bfloat16)
+        bwd = "b200_mlp_down_silu_bwd" if ctx.act == "silu" else "b200_mlp_down_glu_bwd"
         tok = _t0("mlp_glu_bwd")
-        check(lib().b200_mlp_down_glu_bwd(d2.data_ptr(), wd.data_ptr(), gu.data_ptr(), dgu.data_ptr(), M, H, I,
-                                          _stream()), "b200_mlp_down_glu_bwd")
+        check(getattr(lib(), bwd)(d2.data_ptr(), wd.data_ptr(), gu.data_ptr(), dgu.data_ptr(), M, H, I, _stream()), bwd)
         _t1(tok)
         w2 = torch.as_strided(wg, (2 * I, K), (K, 1))               # [Wg ; Wu], adjacent in the flat store
         g2 = torch.as_strided(wg.grad, (2 * I, K), (K, 1))
         dx = dgu @ w2 if ctx.needs_input_grad[0] else None
         g2.addmm_(dgu.t(), x2)
-        return (dx.view(ctx.x_shape) if dx is not None else None), None, None, None
+        return (dx.view(ctx.x_shape) if dx is not None else None), None, None, None, None
 
 
 def mlp_fusable(x: torch.Tensor, wg: torch.Tensor, wu: torch.Tensor, wd: torch.Tensor) -> bool:
@@ -1160,12 +1195,14 @@ def mlp_fusable(x: torch.Tensor, wg: torch.Tensor, wu: torch.Tensor, wd: torch.T
     return flat and _adjacent_rows(wg, wu) and _adjacent_rows(wg.grad, wu.grad)
 
 
-def mlp(x: torch.Tensor, wg: torch.Tensor, wu: torch.Tensor, wd: torch.Tensor) -> torch.Tensor:
-    """The reference MLP (arch/llama.py:149-151) on three bias-free projections."""
+def mlp(x: torch.Tensor, wg: torch.Tensor, wu: torch.Tensor, wd: torch.Tensor, act: str = "sigmoid2") -> torch.Tensor:
+    """The reference MLP (arch/llama.py:149-151) on three bias-free projections; act "silu" gives mlx_lm's
+    down(silu(gate(x)) * up(x))."""
+    _check_choice(act, GLU_ACTS, "mlp: act")
     if mlp_fusable(x, wg, wu, wd) and _MLP_FUSED:
-        return _MlpFn.apply(x, wg, wu, wd)
+        return _MlpFn.apply(x, wg, wu, wd, act)
     g, u = multi_linear(x, (wg, wu))
-    return linear(glu(g, u), wd)
+    return linear(glu(g, u, act), wd)
 
 
 # B200_MLP_FUSED=0 restores the library GEMMs + elementwise GLU kernels (A/B switch for measurements; the first
@@ -1173,11 +1210,15 @@ def mlp(x: torch.Tensor, wg: torch.Tensor, wu: torch.Tensor, wd: torch.Tensor) -
 _MLP_FUSED = os.environ.get("B200_MLP_FUSED", "1") != "0"
 
 
-def glu(gate: torch.Tensor, up: torch.Tensor) -> torch.Tensor:
-    """gate * sigmoid(up) * 2 (arch/llama.py:151).  bf16 tensors with numel % 8 == 0 take the fused
-    kernel; other dtypes (fp32 configs) use the same formula through torch ops."""
+def glu(gate: torch.Tensor, up: torch.Tensor, act: str = "sigmoid2") -> torch.Tensor:
+    """gate * sigmoid(up) * 2 (arch/llama.py:151), or silu(gate) * up with act "silu" (mlx_lm's Llama MLP).  bf16
+    tensors with numel % 8 == 0 take the fused kernel; other dtypes (fp32 configs) use the same formula through
+    torch ops."""
+    _check_choice(act, GLU_ACTS, "glu: act")
     if gate.dtype == torch.bfloat16 and gate.is_cuda and gate.numel() % 8 == 0:
-        return _GluFn.apply(gate, up)
+        return _GluFn.apply(gate, up, act)
+    if act == "silu":
+        return torch.nn.functional.silu(gate) * up
     return gate * torch.sigmoid(up) * 2
 
 

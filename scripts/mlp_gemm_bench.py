@@ -33,6 +33,8 @@ def load(path):
     from mlx_cuda_distributed_pretraining_b200._lib import SIGNATURES
     handle = ctypes.CDLL(str(path))
     for name, (res, args) in SIGNATURES.items():
+        if not hasattr(handle, name):  # an older build: entries added since are not compared
+            continue
         fn = getattr(handle, name)
         fn.restype, fn.argtypes = res, args
     return handle
