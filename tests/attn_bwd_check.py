@@ -8,6 +8,10 @@ uses that same O for delta = rowsum(dO * O).  The per-element bound has the form
                                                                    W uses |P| * (|dP| + |delta|) for dS, which covers
                                                                    the cancellation in dP - delta, and the logit
                                                                    magnitude s * (|q| @ |k|) that exp2 amplifies
+  C32 * 2^-24 * D * |P| * (|dO| @ |V|^T + rowsum(|dO| * |O|))       the fp32 sums over D inside dP and delta: their
+                                                                   error does not shrink when dP or delta cancels
+                                                                   (a query that sees one key has dS = 0 exactly,
+                                                                   the kernel the fp32 rounding of dP - delta)
   2^-8 * |R|                                                        bf16 output
 """
 from __future__ import annotations
@@ -18,8 +22,9 @@ C32 = 4.0
 U8, U24 = 2.0 ** -8, 2.0 ** -24
 
 
-def forward64(q, k, v, scale, causal):
-    """fp64 attention forward of bf16 [B,S,H,D] / [B,S,Hk,D] inputs -> (o bf16, lse fp32 [B,H,S])."""
+def forward64(q, k, v, scale, causal, mask=None):
+    """fp64 attention forward of bf16 [B,S,H,D] / [B,S,Hk,D] inputs -> (o bf16, lse fp32 [B,H,S]).  mask: an optional
+    boolean visibility mask [S, S] or [B, S, S] (tests/attn_fwd_check.visible), intersected with `causal`."""
     B, S, H, D = q.shape
     g = H // k.shape[2]
     qd, kd, vd = (t.double().transpose(1, 2) for t in (q, k, v))
@@ -27,15 +32,18 @@ def forward64(q, k, v, scale, causal):
     s = scale * qd @ kd.transpose(-1, -2)
     if causal:
         s = s.masked_fill(torch.ones(S, S, dtype=torch.bool, device=q.device).triu(1), float("-inf"))
+    if mask is not None:
+        s = s.masked_fill(~(mask[:, None] if mask.dim() == 3 else mask), float("-inf"))
     lse = torch.logsumexp(s, -1)
     o = torch.softmax(s, -1) @ vd
     return o.transpose(1, 2).to(torch.bfloat16).contiguous(), lse.float().contiguous()
 
 
-def reference(q, k, v, o, do, lse, scale, causal, rows=None, mask_shift=0, drop_keys=None):
+def reference(q, k, v, o, do, lse, scale, causal, rows=None, mask_shift=0, drop_keys=None, mask=None):
     """fp64 dq, dk, dv (one batch row at a time) and their element-wise bounds for the batch rows `rows`.
-    Returns dict name -> (ref [len(rows),S,heads,D], bound).  Fault tests: `mask_shift` moves the causal diagonal,
-    `drop_keys` (a slice) leaves those keys out of P."""
+    Returns dict name -> (ref [len(rows),S,heads,D], bound).  mask: an optional boolean visibility mask [S, S] or
+    [B, S, S] (documents, windows: tests/attn_fwd_check.visible), intersected with `causal`.  Fault tests:
+    `mask_shift` moves the causal diagonal, `drop_keys` (a slice) leaves those keys out of P."""
     B, S, H, D = q.shape
     Hk = k.shape[2]
     g = H // Hk
@@ -51,6 +59,8 @@ def reference(q, k, v, o, do, lse, scale, causal, rows=None, mask_shift=0, drop_
         p = torch.exp(s - lse[b].double()[..., None])
         if keep is not None:
             p = p * keep
+        if mask is not None:
+            p = p * (mask[b] if mask.dim() == 3 else mask)
         if drop_keys is not None:
             p[..., drop_keys] = 0
         dp = dod @ vd.transpose(-1, -2)
@@ -62,11 +72,12 @@ def reference(q, k, v, o, do, lse, scale, causal, rows=None, mask_shift=0, drop_
         # weights of the fp32 terms
         amp = 1.0 + scale * qd.abs() @ kd.abs().transpose(-1, -2)  # exp2 turns a logit error into a relative one
         pw = p.abs() * amp
-        dsw = p.abs() * amp * (dp.abs() + delta.abs())
         n = S
-        b_dq = U8 * scale * ds.abs() @ kd.abs() + C32 * U24 * (D + n) * scale * dsw @ kd.abs() + U8 * dq.abs()
+        dsw = (D + n) * p.abs() * amp * (dp.abs() + delta.abs()) \
+            + D * p.abs() * (dod.abs() @ vd.abs().transpose(-1, -2) + (dod.abs() * od.abs()).sum(-1, keepdim=True))
+        b_dq = U8 * scale * ds.abs() @ kd.abs() + C32 * U24 * scale * dsw @ kd.abs() + U8 * dq.abs()
         b_dk = U8 * scale * ds.abs().transpose(-1, -2) @ qd.abs() \
-            + C32 * U24 * (D + n) * scale * dsw.transpose(-1, -2) @ qd.abs()
+            + C32 * U24 * scale * dsw.transpose(-1, -2) @ qd.abs()
         b_dv = U8 * p.abs().transpose(-1, -2) @ dod.abs() + C32 * U24 * (D + n) * pw.transpose(-1, -2) @ dod.abs()
         dk, dv = dk.reshape(Hk, g, S, D).sum(1), dv.reshape(Hk, g, S, D).sum(1)
         b_dk, b_dv = b_dk.reshape(Hk, g, S, D).sum(1), b_dv.reshape(Hk, g, S, D).sum(1)

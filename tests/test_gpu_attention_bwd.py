@@ -3,7 +3,10 @@ element by element with the fp64 reference of tests/attn_bwd_check.py.
 
 O and LSE come from an fp64 forward (rounded to bf16 / fp32), so the backward is tested alone.  The small-shape
 matrix covers single, ragged and exact query / key tiles, every GQA ratio up to 8, both masks, D = 64 and 128, and
-odd and even key-tile counts (causal launches with an even count pair key tiles t and n-1-t in one CTA).
+odd and even key-tile counts (causal launches with an even count pair key tiles t and n-1-t in one CTA).  The
+document and window kernels (b200_attn_bwd_doc / _window) run on the layouts of test_gpu_packed_attention and the
+windows of test_gpu_sliding_window, checked with the same reference under the visibility mask of
+tests/attn_fwd_check.py.
 """
 import ctypes
 import itertools
@@ -12,6 +15,9 @@ import pytest
 import torch
 
 from tests import attn_bwd_check as ac
+from tests import attn_fwd_check as fc
+from tests.test_gpu_packed_attention import layouts, positions
+from tests.test_gpu_sliding_window import windows
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
 
@@ -57,8 +63,8 @@ def _run(L, q, k, v, o, do, lse, causal, dk=None, dv=None, row_heads=0):
     return dq, dk, dv
 
 
-def _compare(tag, got, q, k, v, o, do, lse, causal, rows):
-    ref = ac.reference(q, k, v, o, do, lse, q.shape[-1] ** -0.5, causal, rows=rows)
+def _compare(tag, got, q, k, v, o, do, lse, causal, rows, mask=None):
+    ref = ac.reference(q, k, v, o, do, lse, q.shape[-1] ** -0.5, causal, rows=rows, mask=mask)
     for name, g in zip(("dq", "dk", "dv"), got):
         r, bd = ref[name]
         RATIOS[f"{tag} {name}"] = max(RATIOS.get(f"{tag} {name}", 0.0), ac.check(name, g[list(rows)], r, bd))
@@ -104,3 +110,70 @@ def test_attn_bwd_dk_dv_deterministic(L, D):
     for _ in range(2):
         _, dk2, dv2 = _run(L, *t, True)
         assert torch.equal(dk, dk2) and torch.equal(dv, dv2)
+
+
+# ---- documents and windows: b200_attn_bwd_doc / b200_attn_bwd_window ------------------------------------------------
+def _masked_inputs(B, S, H, Hk, D, mask, seed):
+    """bf16 q, k, v, dO and the fp64 forward's O / LSE under `mask`, rounded to bf16 / fp32."""
+    torch.manual_seed(seed)
+    q = torch.randn(B, S, H, D, device="cuda").to(torch.bfloat16)
+    k = torch.randn(B, S, Hk, D, device="cuda").to(torch.bfloat16)
+    v = torch.randn(B, S, Hk, D, device="cuda").to(torch.bfloat16)
+    do = torch.randn(B, S, H, D, device="cuda").to(torch.bfloat16)
+    o, lse = fc.forward64(q, k, v, D ** -0.5, mask)
+    return q, k, v, o.to(torch.bfloat16).contiguous(), do, lse.float().contiguous()
+
+
+def _run_masked(L, q, k, v, o, do, lse, pos, window):
+    """b200_attn_bwd_doc (window None) or b200_attn_bwd_window."""
+    B, S, H, D = q.shape
+    Hk = k.shape[2]
+    dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    ws = torch.empty(max(int(L.b200_attn_bwd_doc_workspace_bytes(B, S, H, Hk, D)), 16), device="cuda",
+                     dtype=torch.uint8)
+    st = torch.cuda.current_stream().cuda_stream
+    ins = (q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(), lse.data_ptr())
+    outs = (dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H, Hk, D, ctypes.c_float(D ** -0.5), 0,
+            ws.data_ptr(), ws.numel(), st)
+    pp = None if pos is None else pos.data_ptr()
+    if window is None:
+        rc = L.b200_attn_bwd_doc(*ins, pp, *outs)
+    else:
+        rc = L.b200_attn_bwd_window(*ins, pp, window, *outs)
+    assert rc == 0, L.b200_last_error()
+    torch.cuda.synchronize()
+    return dq, dk, dv
+
+
+@pytest.mark.parametrize("S,D,group", list(itertools.product((257, 1000), (64, 128), (1, 2, 8))))
+def test_attn_bwd_documents(L, S, D, group):
+    pos = torch.stack([positions(lay, S) for lay in layouts(S, seed=D)]).int().cuda()
+    B, Hk = pos.shape[0], 2
+    mask = fc.visible(S, pos=pos, device="cuda")
+    t = _masked_inputs(B, S, Hk * group, Hk, D, mask, seed=S + D + group)
+    got = _run_masked(L, *t, pos, None)
+    _compare(f"document D{D}", got, *t, True, rows=range(B), mask=mask)
+
+
+@pytest.mark.parametrize("packed", [False, True], ids=["rows", "packed"])
+@pytest.mark.parametrize("D,group", list(itertools.product((64, 128), (1, 2, 8))))
+def test_attn_bwd_windows(L, D, group, packed):
+    S, Hk = 1000, 2
+    pos = torch.stack([positions(lay, S) for lay in layouts(S, seed=D)]).int().cuda() if packed else None
+    B = 5 if packed else 2
+    for W in windows(S):
+        mask = fc.visible(S, pos=pos, window=W, device="cuda")
+        t = _masked_inputs(B, S, Hk * group, Hk, D, mask, seed=W + D + group)
+        got = _run_masked(L, *t, pos, W)
+        _compare(f"window D{D}", got, *t, True, rows=range(B), mask=mask)
+
+
+def test_attn_bwd_documents_c3_shape(L):
+    """A C3 layer micro-batch (B16 S2048 H16/8 D64) of packed rows, the five layouts repeated; rows 0 and 15."""
+    B, S, H, Hk, D = 16, 2048, 16, 8, 64
+    lay = layouts(S, seed=2)
+    pos = torch.stack([positions(lay[b % len(lay)], S) for b in range(B)]).int().cuda()
+    mask = fc.visible(S, pos=pos, device="cuda")
+    t = _masked_inputs(B, S, H, Hk, D, mask, seed=11)
+    got = _run_masked(L, *t, pos, None)
+    _compare("document C3", got, *t, True, rows=(0, B - 1), mask=mask)
