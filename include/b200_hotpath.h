@@ -418,6 +418,61 @@ int b200_kv_append_half(void* q, const void* k, const void* v, void* k_cache, vo
                         const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
                         void* stream);
 
+/* ---- mixture-of-experts MLP (Mixtral's sparse MoE block, model.misc.num_local_experts) -------------------------
+ * T tokens, E experts (2..64), k experts per token (1..min(E, 8)), hidden H, per-expert intermediate I (H, I % 8 == 0).
+ * Everything stays on the device and nothing uses atomics: the same inputs give the same bits on every run.
+ *
+ * b200_moe_route: logits f32 [T, E] -> probs = softmax f32 [T, E]; ids int32 [T, k] = the top-k of probs (larger
+ *   first; on an exact tie the lower expert index); weights f32 [T, k] = probs of the ids renormalised to sum 1;
+ *   counts int32 [E] rows per expert; seg_off int32 [E + 1]: expert e owns rows [seg_off[e], seg_off[e + 1]) of the
+ *   permuted buffer, its count padded up to a multiple of 128; tile_expert int32 [b200_moe_max_tiles]: the expert of
+ *   each 128-row tile, n_tiles int32 [1]: seg_off[E] / 128; dest int32 [T, k]: each assignment's row, a stable
+ *   counting sort (tokens keep their order inside an expert).  With aux_counts / aux_psum (f32 [E], or both NULL to
+ *   skip) it also writes the load-balancing loss partials over the tokens whose mask byte is non-zero (mask NULL: all):
+ *   assignments per expert and the sum of probs per expert. */
+size_t b200_moe_route_workspace_bytes(int T, int E, int k);
+int b200_moe_max_tiles(int T, int E, int k);
+int b200_moe_route(const float* logits, const unsigned char* mask, int T, int E, int k, int* ids, float* weights,
+                   float* probs, int* counts, int* seg_off, int* tile_expert, int* n_tiles, int* dest,
+                   float* aux_counts, float* aux_psum, void* workspace, size_t workspace_bytes, void* stream);
+/* xp[dest[t, j]] = x[t] (bf16 rows of H); every pad row of every segment is zero-filled. */
+int b200_moe_permute(const void* x, const int* dest, const int* counts, const int* seg_off, int T, int H, int k,
+                     int E, void* xp, void* stream);
+/* Expert-segmented GEMMs over the permuted buffer, on the wgmma engine's expert-segmented instantiation (TMA +
+ * wgmma, persistent).  128-row tile x uses expert tile_expert[x] and tiles at or past *n_tiles are skipped, so the
+ * work list is sized by max_tiles (b200_moe_max_tiles) without a host round trip.  Weights are expert-stacked:
+ * Wg, Wu [E, I, H] with Wu a whole number (>= E) of [I, H] matrices after Wg in memory (one tensor map addresses
+ * both; flat.ParamStore lays a layer's experts out that way), Wd [E, H, I]; H % 8 == 0, I % 64 == 0.
+ * act 0: gate * sigmoid(up) * 2, 1: silu(gate) * up.
+ *   mode 0 (gate/up forward):  A = xp [rows, H], W0 = Wg, W1 = Wu -> C = gu [rows, 2I] (g | u), Y = act(g, u) [rows, I]
+ *                               from the fp32 accumulators
+ *   mode 1 (down forward):     A = y [rows, I], W0 = Wd -> C [rows, H]
+ *   mode 2 (down dgrad + act adjoint): A = dy [rows, H], W0 = Wd, gu -> C = dgu [rows, 2I] (dg | du)
+ *   mode 3 (gate/up dgrad):    A = dgu [rows, 2I], W0 = Wg, W1 = Wu -> C = dg Wg_e + du Wu_e [rows, H] */
+int b200_moe_gemm(int mode, int act, const void* A, const void* W0, const void* W1, const void* gu, void* C, void* Y,
+                  const int* tile_expert, const int* n_tiles, int max_tiles, int H, int I, int E, void* stream);
+/* Weight gradient per expert on the same instantiation: G[e] [R, C] += P[rows_e]^T Q[rows_e] over expert e's counts[e]
+ * rows from seg_off[e] (P, Q bf16 buffers of `rows` rows with leading dimensions ldp, ldq; K runs in 64-row blocks
+ * inside the 128-padded segment, so the pad rows of P or of Q must be zero, as b200_moe_permute and
+ * b200_moe_combine_bwd leave them); fp32 accumulation added to the bf16 G (beta = 1); an expert with no rows is
+ * skipped and G[e] left untouched. */
+int b200_moe_wgrad(const void* P, long long ldp, const void* Q, long long ldq, void* G, int R, int Cc, int E, int rows,
+                   const int* counts, const int* seg_off, void* stream);
+/* out[t] = sum_j weights[t, j] * yp[dest[t, j]] in f32, j ascending, bf16 out. */
+int b200_moe_combine_fwd(const void* yp, const int* dest, const float* weights, int T, int H, int k, void* out,
+                         void* stream);
+/* Backward of the combine and the router: dyp[dest[t, j]] = weights[t, j] * dout[t] and zeros in every pad row of
+ * every segment (counts / seg_off of b200_moe_route); dw[t, j] = <dout[t],
+ * yp[dest[t, j]]> (f32, or NULL); dlogits f32 [T, E] (or NULL) through the renormalisation and the softmax, plus
+ * aux_grad[e] (d loss / d aux_psum[e], or NULL) on every token whose mask byte is non-zero. */
+int b200_moe_combine_bwd(const void* dout, const void* yp, const int* dest, const int* ids, const float* weights,
+                         const float* probs, const float* aux_grad, const unsigned char* mask, const int* counts,
+                         const int* seg_off, int T, int H, int E, int k, void* dyp, float* dw, float* dlogits,
+                         void* stream);
+/* dx[t] = sum_j dxp[dest[t, j]] (+ addend[t], f32 [T, H], or NULL) in f32, bf16 out. */
+int b200_moe_unpermute(const void* dxp, const int* dest, const float* addend, int T, int H, int k, void* dx,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -90,6 +90,16 @@ SIGNATURES = {
     "b200_silu_glu_fwd": (_i, [_vp, _vp, _vp, _ll, _vp]),
     "b200_silu_glu_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "b200_kv_append_half": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_moe_route_workspace_bytes": (_sz, [_i, _i, _i]),
+    "b200_moe_max_tiles": (_i, [_i, _i, _i]),
+    "b200_moe_route": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "b200_moe_permute": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
+    "b200_moe_gemm": (_i, [_i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "b200_moe_wgrad": (_i, [_vp, _ll, _vp, _ll, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "b200_moe_combine_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
+    "b200_moe_combine_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp,
+                                  _vp]),
+    "b200_moe_unpermute": (_i, [_vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
 }
 
 

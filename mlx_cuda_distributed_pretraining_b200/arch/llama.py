@@ -59,6 +59,7 @@ class ModelArgs:
     apply_rope: bool = False  # extension; see module docstring
     sliding_window: Optional[int] = None  # extension: query q sees keys q - W .. q in every layer (None: causal)
     variant: Optional[str] = None  # extension: None / "reference" (this block) or "mlx_lm" (module docstring)
+    router_aux_loss_coef: float = 0.001  # with num_local_experts > 0: weight of the load-balancing loss
 
 
 class RMSNorm(nn.Module):
@@ -84,6 +85,52 @@ class MLP(nn.Module):
         if self.gate_proj.bias is not None:
             return self.down_proj(ops.glu(self.gate_proj(x), self.up_proj(x), self.act))
         return ops.mlp(x, self.gate_proj.weight, self.up_proj.weight, self.down_proj.weight, self.act)
+
+
+class _ExpertLinear(nn.Module):
+    """E bias-free projections stacked as one [E, out, in] weight (mlx-lm's SwitchLinear)."""
+
+    def __init__(self, num_experts: int, in_features: int, out_features: int):
+        super().__init__()
+        self.weight = nn.Parameter(torch.empty(num_experts, out_features, in_features))
+        bound = in_features ** -0.5
+        nn.init.uniform_(self.weight, -bound, bound)
+
+
+class SwitchGLU(nn.Module):
+    def __init__(self, hidden_size: int, intermediate_size: int, num_experts: int):
+        super().__init__()
+        self.gate_proj = _ExpertLinear(num_experts, hidden_size, intermediate_size)
+        self.up_proj = _ExpertLinear(num_experts, hidden_size, intermediate_size)
+        self.down_proj = _ExpertLinear(num_experts, intermediate_size, hidden_size)
+
+
+class SparseMoeBlock(nn.Module):
+    """Mixtral's sparse MoE block without jitter (model.misc.num_local_experts): the router `gate` [E, hidden] picks
+    each token's top-k experts by softmax probability, their weights renormalised to sum 1, and the token's output is
+    the weighted sum of those experts' MLPs (the block's activation, per-expert width intermediate_size).  Dropless.
+    Parameter names follow mlx-lm's Mixtral (block_sparse_moe.gate / block_sparse_moe.switch_mlp.*).
+
+    `last_aux` holds the (assignment counts, probability sums) [E] over the unmasked tokens of the last forward that
+    asked for them (Model.moe_aux_loss), else None."""
+
+    def __init__(self, hidden_size: int, intermediate_size: int, num_experts: int, top_k: int, act: str):
+        super().__init__()
+        self.num_experts, self.top_k, self.act = num_experts, top_k, act
+        self.gate = nn.Linear(hidden_size, num_experts, bias=False)
+        if num_experts % 8:
+            # a router with E % 8 != 0 rows cannot go through Newton-Schulz (its GEMMs need N % 8 == 0): the flat
+            # store keeps it with the elementwise parameters, so Muon / hybrid update it with their non-matrix rule
+            self.gate.weight._b200_elementwise = True
+        self.switch_mlp = SwitchGLU(hidden_size, intermediate_size, num_experts)
+        self.last_aux = None
+
+    def forward(self, x: torch.Tensor, token_mask: Optional[torch.Tensor] = None, aux: bool = False) -> torch.Tensor:
+        s = self.switch_mlp
+        out, counts, psum = ops.moe(x, self.gate.weight, s.gate_proj.weight, s.up_proj.weight, s.down_proj.weight,
+                                    self.top_k, self.act, pad_mask=token_mask, aux=aux)
+        self.last_aux = (counts, psum) if aux else None
+        return out
 
 
 class AttentionModule(nn.Module):
@@ -143,13 +190,27 @@ class TransformerBlock(nn.Module):
             apply_rope=args.apply_rope or mlx_lm,
             rope_layout="half" if mlx_lm and not args.rope_traditional else "interleaved")
         self.post_attention_layernorm = RMSNorm(args.hidden_size, eps=args.rms_norm_eps)
-        self.mlp = MLP(args.hidden_size, inter, use_bias=args.mlp_bias, act="silu" if mlx_lm else "sigmoid2")
+        act = "silu" if mlx_lm else "sigmoid2"
+        self.moe = bool(args.num_local_experts)
+        if self.moe:
+            if args.mlp_bias:
+                raise ValueError("ModelArgs.mlp_bias is not supported with num_local_experts > 0")
+            self.block_sparse_moe = SparseMoeBlock(args.hidden_size, inter, args.num_local_experts,
+                                                   args.num_experts_per_tok, act)
+        else:
+            self.mlp = MLP(args.hidden_size, inter, use_bias=args.mlp_bias, act=act)
+
+    def _ffn(self, y: torch.Tensor, token_mask=None, aux: bool = False) -> torch.Tensor:
+        if self.moe:
+            return self.block_sparse_moe(y, token_mask, aux)
+        return self.mlp(y)
 
     def forward(self, x: torch.Tensor, mask=None, position_ids=None) -> torch.Tensor:
         x = x + self.self_attn(self.input_layernorm(x), mask=mask, position_ids=position_ids)
-        return x + self.mlp(self.post_attention_layernorm(x))
+        return x + self._ffn(self.post_attention_layernorm(x))
 
-    def forward_fused(self, h: torch.Tensor, pending, mask=None, position_ids=None):
+    def forward_fused(self, h: torch.Tensor, pending, mask=None, position_ids=None, token_mask=None,
+                      aux: bool = False):
         """Same block with every residual add fused into the norm that consumes it.  `pending` is the
         previous block's MLP output not yet added to the stream h (None for the first block); returns
         (h after the attention residual, this block's MLP output still to be added)."""
@@ -160,7 +221,7 @@ class TransformerBlock(nn.Module):
             h, y = ops.add_rmsnorm(h, pending, n1.weight, n1.eps)
         a = self.self_attn(y, mask=mask, position_ids=position_ids)
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
-        return h, self.mlp(y)
+        return h, self._ffn(y, token_mask, aux)
 
     def forward_cached(self, h: torch.Tensor, pending, cache: "KVCache", layer: int, window: Optional[int] = None):
         """forward_fused with the attention run against the KV cache (AttentionModule.cached)."""
@@ -171,7 +232,7 @@ class TransformerBlock(nn.Module):
             h, y = ops.add_rmsnorm(h, pending, n1.weight, n1.eps)
         a = self.self_attn.cached(y, cache, layer, window)
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
-        return h, self.mlp(y)
+        return h, self._ffn(y)
 
 
 class KVCache:
@@ -218,11 +279,13 @@ class Model(nn.Module):
         self._tied_w = None  # padded alias of the embedding for the logits GEMM (set lazily)
         self.lm_head = None if args.tie_word_embeddings else nn.Linear(args.hidden_size, args.vocab_size, bias=False)
 
-    def hidden_states(self, inputs: torch.Tensor, position_ids=None, attention_mask=None) -> torch.Tensor:
+    def hidden_states(self, inputs: torch.Tensor, position_ids=None, attention_mask=None,
+                      token_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
         """position_ids (int [B, S], optional): packed rows, each token's position within its document (0 at the
         document's first token).  It selects the document-causal mask and, with RoPE on, the rotation angles, so
         every document is computed as if it ran alone.  None keeps the causal mask over whole rows.  Both masks carry
-        args.sliding_window."""
+        args.sliding_window.  token_mask (bool [B, S], optional; MoE models): the tokens the load-balancing loss
+        counts; given, every MoE layer keeps its partials for moe_aux_loss()."""
         B, S = inputs.shape
         if attention_mask is not None:
             mask = attention_mask
@@ -234,11 +297,30 @@ class Model(nn.Module):
             mask = CausalMask(S, self.args.sliding_window)
         h = ops.embedding(inputs, self.embed_tokens.weight)
         pending = None
-        for layer in self.layers:
-            h, pending = layer.forward_fused(h, pending, mask=mask, position_ids=position_ids)
+        if self.args.num_local_experts:
+            aux = token_mask is not None
+            self._moe_tokens = token_mask.sum() if aux else None
+            for layer in self.layers:
+                h, pending = layer.forward_fused(h, pending, mask=mask, position_ids=position_ids,
+                                                 token_mask=token_mask, aux=aux)
+        else:
+            for layer in self.layers:
+                h, pending = layer.forward_fused(h, pending, mask=mask, position_ids=position_ids)
         if pending is None:
             return self.norm(h)
         return ops.add_rmsnorm(h, pending, self.norm.weight, self.norm.eps)[1]
+
+    def moe_aux_loss(self) -> Optional[torch.Tensor]:
+        """transformers' load_balancing_loss_func over all layers' router logits of the last hidden_states call that
+        had a token_mask, with attention_mask = token_mask: E * sum_e f_e P_e, f_e = assignments to expert e and P_e =
+        the sum of its router probabilities, both over (layers x unmasked tokens) and divided by their number.  The
+        gradient flows through P only.  None for a dense model or when no partials were kept."""
+        if not self.args.num_local_experts or any(l.block_sparse_moe.last_aux is None for l in self.layers):
+            return None
+        counts = torch.stack([l.block_sparse_moe.last_aux[0] for l in self.layers]).sum(0)
+        psum = torch.stack([l.block_sparse_moe.last_aux[1] for l in self.layers]).sum(0)
+        n = self._moe_tokens.float() * len(self.layers)
+        return self.args.num_local_experts * (counts * psum).sum() / (n * n)
 
     def _logits_weight(self) -> torch.Tensor:
         """[V or V_pad, hidden] weight of the logits GEMM: lm_head, or the embedding (tied,
@@ -254,7 +336,7 @@ class Model(nn.Module):
             return self._tied_w
         return self.embed_tokens.weight
 
-    def padded_logits(self, inputs: torch.Tensor, position_ids=None):
+    def padded_logits(self, inputs: torch.Tensor, position_ids=None, token_mask=None):
         """(logits [B*S, ld], V) with ld >= V, ld % 8 == 0 when the fused cross-entropy can take them
         (bf16 weights, tied + row-padded embedding alias or an aligned vocabulary); else (None, V).
         Eligibility is decided BEFORE the forward pass, so an ineligible config (fp32, logit_scale,
@@ -264,12 +346,12 @@ class Model(nn.Module):
         w = self._logits_weight()
         if w.shape[0] % 8 != 0 or w.dtype != torch.bfloat16:
             return None, self.vocab_size
-        h = self.hidden_states(inputs, position_ids)
+        h = self.hidden_states(inputs, position_ids, token_mask=token_mask)
         logits = torch.nn.functional.linear(h, w)
         return logits.view(-1, logits.shape[-1]), self.vocab_size
 
-    def forward(self, inputs: torch.Tensor, position_ids=None, attention_mask=None) -> torch.Tensor:
-        h = self.hidden_states(inputs, position_ids, attention_mask)
+    def forward(self, inputs: torch.Tensor, position_ids=None, attention_mask=None, token_mask=None) -> torch.Tensor:
+        h = self.hidden_states(inputs, position_ids, attention_mask, token_mask)
         logits = torch.nn.functional.linear(h, self._logits_weight())[..., :self.vocab_size]
         if self.logit_scale is not None:
             logits = logits * self.logit_scale

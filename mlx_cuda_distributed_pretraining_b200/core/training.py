@@ -80,6 +80,35 @@ class ModelConfig:
             if self.rope.get("scaling") is not None:
                 raise ValueError(f"model.misc.variant: mlx_lm does not support rope.scaling "
                                  f"(got {self.rope.get('scaling')!r}); set it to null")
+        validate_moe_keys(self.misc or {})
+
+
+def _int_or_none(misc: Dict[str, Any], key: str) -> int:
+    v = misc.get(key)
+    if v is None:
+        return 0
+    if isinstance(v, bool) or not isinstance(v, int):
+        raise ValueError(f"model.misc.{key} must be null or an integer, got {v!r}")
+    return v
+
+
+def validate_moe_keys(misc: Dict[str, Any]) -> None:
+    """model.misc.num_local_experts E (absent / null / 0: dense MLP; 2..64: every layer's MLP becomes a sparse MLP of E
+    experts), num_experts_per_tok k (1..min(E, 8); absent / null / 0 when dense) and router_aux_loss_coef c (finite,
+    >= 0; default 0.001 as in MixtralConfig)."""
+    E = _int_or_none(misc, "num_local_experts")
+    k = _int_or_none(misc, "num_experts_per_tok")
+    if E != 0 and not 2 <= E <= 64:
+        raise ValueError(f"model.misc.num_local_experts must be null, 0 or 2..64, got {E!r}")
+    if E == 0 and k != 0:
+        raise ValueError(f"model.misc.num_experts_per_tok={k} needs num_local_experts > 0")
+    if E > 0 and not 1 <= k <= min(E, 8):
+        raise ValueError(f"model.misc.num_experts_per_tok must lie in 1..{min(E, 8)} with {E} experts, got {k!r}")
+    c = misc.get("router_aux_loss_coef", 0.001)
+    if isinstance(c, bool) or not isinstance(c, (int, float)) or not math.isfinite(c) or c < 0:
+        raise ValueError(f"model.misc.router_aux_loss_coef must be a finite number >= 0, got {c!r}")
+    if E > 0 and misc.get("mlp_bias"):
+        raise ValueError("model.misc.mlp_bias: true is not supported with num_local_experts > 0 (experts have no bias)")
 
 
 @dataclass
@@ -145,6 +174,23 @@ class Config:
     system: SystemConfig
     resume: Optional[ResumeConfig] = None
     overwrite: bool = False
+
+    def __post_init__(self):
+        E = _int_or_none(self.model.misc or {}, "num_local_experts")
+        if E > 0:
+            opt = self.training.optimization or {}
+            names = {opt.get("optimizer"),
+                     opt.get("matrix_optimizer", "muon") if opt.get("optimizer") == "hybrid" else None}
+            inter = (self.model.dimensions or {}).get("intermediate_size")
+            if not isinstance(inter, int) or inter % 64 != 0:
+                raise ValueError(f"model.dimensions.intermediate_size must be a multiple of 64 with num_local_experts "
+                                 f"> 0 (the expert GEMMs' k-blocks), got {inter!r}")
+            if "shampoo" in names:
+                raise ValueError("optimization.optimizer: shampoo is not supported with num_local_experts > 0 "
+                                 "(Shampoo on stacked expert weights is out of scope); use muon, adamw, lion or sgd")
+            if not self.system.mixed_precision:
+                raise ValueError("model.misc.num_local_experts > 0 needs system.mixed_precision: true "
+                                 "(the expert kernels take bf16 operands)")
 
     @classmethod
     def from_dict(cls, d: Dict[str, Any]) -> "Config":
@@ -669,7 +715,10 @@ class Trainer:
             use_flex_attention=m.attention.get("use_flex_attention", False),
             flash_block_size=m.attention.get("flash_block_size", 128),
             apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")) or m.misc.get("variant") == "mlx_lm",
-            sliding_window=m.attention.get("sliding_window"), variant=m.misc.get("variant"))
+            sliding_window=m.attention.get("sliding_window"), variant=m.misc.get("variant"),
+            num_local_experts=m.misc.get("num_local_experts") or 0,
+            num_experts_per_tok=m.misc.get("num_experts_per_tok") or 0,
+            router_aux_loss_coef=float(m.misc.get("router_aux_loss_coef", 0.001)))
         self.model_args = args
         model = Model(args)
         init_model_(model, args, self.config.system.seed)
@@ -723,7 +772,8 @@ class Trainer:
         self._pin = None
 
     # -- loss --------------------------------------------------------------------------------------
-    def compute_loss(self, model, inputs: torch.Tensor, targets: torch.Tensor, packed: bool = False):
+    def compute_loss(self, model, inputs: torch.Tensor, targets: torch.Tensor, packed: bool = False,
+                     aux: bool = True):
         """Masked token-mean cross-entropy.  packed: the rows hold several documents (DataManager with
         pack_sequences); the model then attends within documents (position_ids from the BOS tokens), and the one
         target per document boundary that an unpacked row never has -- a document's last token predicting the
@@ -737,17 +787,28 @@ class Trainer:
             targets = targets.masked_fill(targets == self.tokenizer.BOS_TOKEN, self.tokenizer.PAD_TOKEN)
         pad_mask = targets != self.tokenizer.PAD_TOKEN
         ntoks = pad_mask.sum()
+        # MoE models: the load-balancing loss counts the non-PAD inputs; it is kept in self.last_aux_loss for
+        # micro_step, and skipped entirely when its coefficient is 0 or aux is off (validation reports CE only)
+        args = getattr(self, "model_args", None)
+        self.last_aux_loss = None
+        moe_kw = {}
+        if aux and args is not None and args.num_local_experts and args.router_aux_loss_coef > 0:
+            moe_kw = {"token_mask": inputs != self.tokenizer.PAD_TOKEN}
         if not hasattr(model, "padded_logits"):
             logits2d, V = None, None
         elif position_ids is None:
-            logits2d, V = model.padded_logits(inputs)
+            logits2d, V = model.padded_logits(inputs, **moe_kw)
         else:
-            logits2d, V = model.padded_logits(inputs, position_ids)
+            logits2d, V = model.padded_logits(inputs, position_ids, **moe_kw)
+        if moe_kw and logits2d is not None:
+            self.last_aux_loss = model.moe_aux_loss()
         if logits2d is not None:
             # fused path: fp32 log-sum-exp over bf16 logits, pad mask applied per row, no fp32 [B,S,V] copy
             rows = ops.cross_entropy_rows(logits2d, targets.reshape(-1).contiguous(), V, self.tokenizer.PAD_TOKEN)
             return rows.sum() / ntoks, ntoks
-        logits = (model(inputs) if position_ids is None else model(inputs, position_ids)).float()  # fp32 loss (:1226)
+        logits = (model(inputs, **moe_kw) if position_ids is None else model(inputs, position_ids, **moe_kw)).float()
+        if moe_kw:
+            self.last_aux_loss = model.moe_aux_loss()
         ce = torch.nn.functional.cross_entropy(logits.view(-1, logits.shape[-1]), targets.reshape(-1),
                                                reduction="none").view(targets.shape)
         return (ce * pad_mask).sum() / ntoks, ntoks
@@ -796,7 +857,12 @@ class Trainer:
         exchange and the optimizer update.  Returns (loss, ntoks, did_update)."""
         loss, ntoks = self.compute_loss(self.model, dev_batch[:, :-1], dev_batch[:, 1:],
                                         packed=getattr(self.data_manager, "pack", False))
-        loss.backward()
+        aux = getattr(self, "last_aux_loss", None)
+        if aux is None:
+            loss.backward()
+        else:   # MoE: the training loss is CE + c * aux; `loss` stays the CE that is logged
+            (loss + self.model_args.router_aux_loss_coef * aux).backward()
+            self.step_aux_loss = aux.detach()
         k = self.grad_accum_steps
         store = self.store
         if self.use_acc:
@@ -824,7 +890,7 @@ class Trainer:
         with torch.no_grad():
             for i in range(min(self.data_manager.num_validation_batches, 50)):
                 b = self._to_device(self.data_manager.generate_validation_batch(i))
-                loss, ntoks = self.compute_loss(self.model, b[:, :-1], b[:, 1:])
+                loss, ntoks = self.compute_loss(self.model, b[:, :-1], b[:, 1:], aux=False)
                 tot_loss += loss * ntoks
                 tot_tok += ntoks
         if self.distributed:
@@ -905,6 +971,8 @@ class Trainer:
                 metrics = {**pending, "loss": loss_val, "ppl": float(np.exp(min(loss_val, 80.0))),
                            "lr": float(self.lr_schedule(step)), "tokens": ntok_val, "total_tokens": tt,
                            "tokens_per_sec": float(tt / max(time.time() - start_time, 1e-9))}
+                if getattr(self, "step_aux_loss", None) is not None:
+                    metrics["aux_loss"] = float(self.step_aux_loss.item())
                 pending = {}
                 last = metrics
                 if logf:
@@ -987,7 +1055,7 @@ def init_model_(model: Model, args: ModelArgs, seed: int) -> None:
             elif name == "embed_tokens.weight":
                 p.copy_(torch.randn(p.shape, generator=g, dtype=torch.float32) * args.hidden_size ** -0.5)
             else:
-                bound = 1.0 / math.sqrt(p.shape[1])
+                bound = 1.0 / math.sqrt(p.shape[-1])   # [E, out, in] experts: each slice as its nn.Linear
                 p.copy_((torch.rand(p.shape, generator=g, dtype=torch.float32) * 2 - 1) * bound)
 
 

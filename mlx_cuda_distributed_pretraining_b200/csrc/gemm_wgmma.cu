@@ -64,6 +64,18 @@ struct Problem {
   int glu_I;
   void* aux;  // epi 1: y [M, I] (written); epi 2: gu [M, 2I] (read)
   long long ld_aux;
+  // expert-segmented problems (the SEG instantiation only; a MoE layer's expert GEMMs, csrc/moe.cu):
+  //   seg 1: M-segmented.  Row tile mi of A / D belongs to expert seg_tile[mi]; tiles at or past *seg_ntiles are
+  //          skipped.  B is the expert-stacked weight [E', rows, cols] and is read at batch e (A, D at batch 0).
+  //   seg 2: K-segmented weight gradient.  Batch b = expert b: K runs over that expert's seg_counts[b] rows from
+  //          seg_off[b] of A and B (batch 0); an expert without rows is skipped and its D untouched.
+  int seg;
+  int up_off;   // seg 1: batch offset of the up-projection experts behind the gate experts in B's map
+  int k_split;  // seg 1, MN-major B: k rows >= k_split are rows k - k_split of batch e + up_off ([Wg_e ; Wu_e])
+  const int* seg_tile;
+  const int* seg_ntiles;
+  const int* seg_counts;
+  const int* seg_off;
 };
 
 struct Args {
@@ -99,6 +111,8 @@ __device__ __forceinline__ void tile_coords(const Problem& p, int r, int& mi, in
 
 struct Item {
   int pi, split, b, mi, ni, kb_begin, kb_end;
+  int e, koff;  // SEG: the expert of B (seg 1) and the first A / B row of the K range (seg 2)
+  bool live;    // SEG: false for a skipped item (no loads, no epilogue)
 };
 
 __device__ __forceinline__ int problem_of(const Args& g, int w) {
@@ -116,6 +130,7 @@ __device__ __forceinline__ void kb_range(const Problem& p, int split, int& kb_be
   kb_end = min(p.num_kb, kb_begin + kb_per);
 }
 
+template <bool SEG>
 __device__ __forceinline__ Item decode(const Args& g, int w) {
   Item it;
   it.pi = problem_of(g, w);
@@ -126,10 +141,34 @@ __device__ __forceinline__ Item decode(const Args& g, int w) {
   it.b = r / p.tiles_per_batch;
   tile_coords(p, r - it.b * p.tiles_per_batch, it.mi, it.ni);
   kb_range(p, it.split, it.kb_begin, it.kb_end);
+  if constexpr (SEG) {  // expert of the tile / K range of the expert, read from the device (no host round trip)
+    it.e = 0;
+    it.koff = 0;
+    it.live = true;
+    if (p.seg == 1) {
+      if (it.mi >= *p.seg_ntiles) {
+        it.live = false;
+        it.kb_end = it.kb_begin;
+      } else {
+        it.e = p.seg_tile[it.mi];
+      }
+    } else if (p.seg == 2) {
+      const int cnt = p.seg_counts[it.b];
+      it.kb_begin = 0;
+      it.kb_end = (cnt + BK - 1) / BK;
+      it.koff = p.seg_off[it.b];
+      it.live = cnt > 0;
+    }
+  }
   return it;
 }
 
+template <bool SEG>
 __device__ __forceinline__ int item_kbs(const Args& g, int w) {
+  if constexpr (SEG) {
+    const Item it = decode<true>(g, w);
+    return max(it.kb_end - it.kb_begin, 0);
+  }
   const Problem& p = g.p[problem_of(g, w)];
   int kb_begin, kb_end;
   kb_range(p, (w - p.work_begin) % p.k_splits, kb_begin, kb_end);
@@ -317,10 +356,37 @@ __device__ __forceinline__ void commit_stores(bool drain) {
   if (drain) bulk_wait<0>();
 }
 
+// One k-block of a SEG problem (see Problem::seg): A and B boxes as for the dense layouts, at the expert's batch.
+__device__ __forceinline__ void seg_loads(const Problem& p, const Item& it, const CUtensorMap* tmA,
+                                          const CUtensorMap* tmB, uint32_t sA, uint32_t sB, uint32_t full, int k0) {
+  const int mi = it.mi, ni = it.ni, kA = k0 + it.koff;
+  if (p.a_mn) {
+    tma_load_3d(sA, tmA, full, mi * BM, kA, 0);
+    tma_load_3d(sA + 8192, tmA, full, mi * BM + 64, kA, 0);
+  } else {
+    tma_load_3d(sA, tmA, full, kA, mi * BM, 0);
+  }
+  if (p.epi == 1) {  // 64 gate rows of expert e, then the same 64 up rows of expert e (batch e + up_off)
+    tma_load_3d(sB, tmB, full, k0, ni * 64, it.e);
+    tma_load_3d(sB + 8192, tmB, full, k0, ni * 64, it.e + p.up_off);
+  } else if (p.b_mn) {
+    int kr = kA, bb = p.seg == 2 ? 0 : it.e;
+    if (p.k_split && kr >= p.k_split) {
+      kr -= p.k_split;
+      bb += p.up_off;
+    }
+    tma_load_3d(sB, tmB, full, ni * BN, kr, bb);
+    tma_load_3d(sB + 8192, tmB, full, ni * BN + 64, kr, bb);
+  } else {
+    tma_load_3d(sB, tmB, full, k0, ni * BN, it.e);
+  }
+}
+
 // SILU selects epi 1/2's activation at compile time: g sigmoid(u) 2 (the reference block) or silu(g) u (SiLU-GLU).
 // A run-time flag cost the kernel spills at its 168-register budget; the SILU = false instantiation is the engine
 // every other launch uses.
-template <bool SILU>
+// SEG adds the expert-segmented problems (Problem::seg); SEG = false compiles exactly the dense engine.
+template <bool SILU, bool SEG>
 __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ Args g) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -356,7 +422,10 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
       int slot = 0;
       uint32_t phase = 0, epi_phase = 0;  // epi_phase bit c: parity of consumer c's next epi_empty completion
       for (int w = blockIdx.x, t = 0; w < g.total_work; w += gridDim.x, ++t) {
-        const Item it = decode(g, w);
+        const Item it = decode<SEG>(g, w);
+        if constexpr (SEG) {
+          if (!it.live) continue;
+        }
         const Problem& p = g.p[it.pi];
         const CUtensorMap* tmA = &g.tmA[it.pi];
         const CUtensorMap* tmB = &g.tmB[it.pi];
@@ -367,6 +436,14 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
           mbar_arrive_expect_tx(full, STAGE_BYTES);
           const uint32_t sA = sbase + slot * STAGE_BYTES, sB = sA + A_BYTES;
           const int k0 = kb * BK;
+          if constexpr (SEG) {
+            seg_loads(p, it, tmA, tmB, sA, sB, full, k0);
+            if (++slot == STAGES) {
+              slot = 0;
+              phase ^= 1u;
+            }
+            continue;
+          }
           if (p.a_mn) {  // two [64 k-rows x 64 m] boxes
             tma_load_3d(sA, tmA, full, mi * BM, k0, b);
             tma_load_3d(sA + 8192, tmA, full, mi * BM + 64, k0, b);
@@ -413,21 +490,23 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
   uint32_t phase = 0, epi_phase = 0;
   for (int w = blockIdx.x, t = 0; w < g.total_work; w += gridDim.x, ++t) {
     if ((t & 1) != c) {  // the other warpgroup's tile: step the ring past its k-blocks
-      const int n = slot + item_kbs(g, w);
+      const int n = slot + item_kbs<SEG>(g, w);
       phase ^= (uint32_t)(n / STAGES) & 1u;
       slot = n % STAGES;
       continue;
     }
-    const Item it = decode(g, w);
+    const Item it = decode<SEG>(g, w);
     const Problem& p = g.p[it.pi];
     const int mi = it.mi, ni = it.ni, b = it.b;
+    bool live = true;
+    if constexpr (SEG) live = it.live;
     const bool last = w + 2 * (int)gridDim.x >= g.total_work;  // this warpgroup's last tile
 
     float acc[128];
 #pragma unroll
     for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     if (t > 0) named_bar_sync(BAR_ORDER + c, 256);  // the other warpgroup's mainloop is done
-    if (epi_input(p) && leader) {  // every thread is past the last tile's epilogue: free the staging tile
+    if (epi_input(p) && leader && live) {  // every thread is past the last tile's epilogue: free the staging tile
       bulk_wait_read<0>();
       mbar_arrive(epi_empty0 + 8 * c);
     }
@@ -440,6 +519,12 @@ __global__ void __launch_bounds__(THREADS, 1) gemm_wgmma_kernel(const __grid_con
       else mainloop<0, 0>(acc, sbase, full0, empty0, n_kb, slot, phase, leader);
     }
     if (w + (int)gridDim.x < g.total_work) named_bar_arrive(BAR_ORDER + (c ^ 1), 256);
+    if constexpr (SEG) {
+      if (!live) {  // skipped item: no epilogue; the warpgroup's last item drains its earlier stores
+        if (last && leader) bulk_wait<0>();
+        continue;
+      }
+    }
 
     // accumulator fragment: acc[64 hm + 4 j + 2 h + e] = tile (64 hm + 16 warp + 8 h + lane / 4, 8 j + cq + e)
     const int cq = (lane & 3) * 2;
@@ -709,7 +794,7 @@ Problem base_problem(int M, int N, int K, int batch, int tiles_n, int epi) {
   return q;
 }
 
-int launch(Args& a, int n, cudaStream_t stream, bool silu = false) {
+int launch(Args& a, int n, cudaStream_t stream, bool silu = false, bool seg = false) {
   int work = 0;
   for (int i = 0; i < n; ++i) {
     a.p[i].work_begin = work;
@@ -717,15 +802,16 @@ int launch(Args& a, int n, cudaStream_t stream, bool silu = false) {
   }
   a.n_problems = n;
   a.total_work = work;
-  static bool attr_set[2] = {false, false};
-  if (!attr_set[silu]) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(silu ? gemm_wgmma_kernel<true> : gemm_wgmma_kernel<false>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
-    attr_set[silu] = true;
+  static bool attr_set[2][2] = {{false, false}, {false, false}};
+  auto kernel = seg ? (silu ? gemm_wgmma_kernel<true, true> : gemm_wgmma_kernel<false, true>)
+                    : (silu ? gemm_wgmma_kernel<true, false> : gemm_wgmma_kernel<false, false>);
+  if (!attr_set[silu][seg]) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+    attr_set[silu][seg] = true;
   }
+  if (work == 0) return B200_OK;
   const int grid = work < num_sms() ? work : num_sms();
-  if (silu) gemm_wgmma_kernel<true><<<grid, THREADS, SMEM_BYTES, stream>>>(a);
-  else gemm_wgmma_kernel<false><<<grid, THREADS, SMEM_BYTES, stream>>>(a);
+  kernel<<<grid, THREADS, SMEM_BYTES, stream>>>(a);
   B200_CHECK_LAUNCH();
   for (int i = 0; i < n; ++i) {
     const Problem& q = a.p[i];
@@ -928,6 +1014,107 @@ int gemm_grouped(const GroupedGemm* probs, int n, cudaStream_t stream) {
     if ((rc = plain_epi_maps(a, oi))) return rc;
   }
   return launch(a, n, stream);
+}
+
+// ---- expert-segmented GEMMs of a MoE layer (csrc/moe.cu) on the SEG instantiation ----------------------------
+// rows = max_tiles * 128 rows of the permuted buffers; tile x of them belongs to expert tile_expert[x], tiles at or
+// past *n_tiles are skipped.  Wg / Wu [E, I, H] must lie in one strided group of [I, H] matrices with Wu = Wg +
+// up_off matrices (flat.ParamStore lays a layer's gate experts and then its up experts out that way), so one tensor
+// map addresses both.  Wd [E, H, I].  mode 0: gu [rows, 2I], y [rows, I] = act(x Wg_e^T, x Wu_e^T); 1: C [rows, H] =
+// y Wd_e^T; 2: dgu [rows, 2I] = act adjoint of dy Wd_e at the saved gu; 3: C [rows, H] = dg Wg_e + du Wu_e.
+int moe_gemm(int mode, int silu, const void* A, const void* Wg, int up_off, const void* Wd, const void* gu, void* C,
+             void* Y, const int* tile_expert, const int* n_tiles, int max_tiles, int H, int I, int E,
+             cudaStream_t stream) {
+  B200_CHECK_ARG(H > 0 && I > 0 && E > 0 && H % 8 == 0 && I % 64 == 0,
+                 "moe_gemm: need hidden %% 8 == 0 and intermediate %% 64 == 0 (H=%d I=%d E=%d)", H, I, E);
+  B200_CHECK_ARG((mode != 0 && mode != 3) || up_off >= E, "moe_gemm: up_off=%d must be >= E=%d", up_off, E);
+  if (max_tiles == 0) return B200_OK;
+  const int rows = max_tiles * BM;
+  Args a;
+  int rc;
+  Problem& q = a.p[0];
+  switch (mode) {
+    case 0:
+      if ((rc = operand_map(&a.tmA[0], A, false, rows, H, 1, H, 0, BM))) return rc;
+      if ((rc = operand_map(&a.tmB[0], Wg, false, I, H, up_off + E, H, (long long)I * H, 64))) return rc;
+      q = base_problem(rows, I, H, 1, I / 64, 1);
+      q.D = C;
+      q.ldd = 2LL * I;
+      q.glu_I = I;
+      q.aux = Y;
+      q.ld_aux = I;
+      if ((rc = glu_map(&a.tmD[0], C, I, rows, q.ldd))) return rc;
+      if ((rc = tile_map(&a.tmE[0], Y, I, rows, 1, I, 0))) return rc;
+      break;
+    case 1:
+      if ((rc = operand_map(&a.tmA[0], A, false, rows, I, 1, I, 0, BM))) return rc;
+      if ((rc = operand_map(&a.tmB[0], Wd, false, H, I, E, I, (long long)H * I, BN))) return rc;
+      q = base_problem(rows, H, I, 1, (H + BN - 1) / BN, 0);
+      q.D = C;
+      q.ldd = H;
+      if ((rc = plain_epi_maps(a, 0))) return rc;
+      break;
+    case 2:
+      if ((rc = operand_map(&a.tmA[0], A, false, rows, H, 1, H, 0, BM))) return rc;
+      if ((rc = operand_map(&a.tmB[0], Wd, true, I, H, E, I, (long long)H * I, BN))) return rc;
+      q = base_problem(rows, I, H, 1, (I + BN - 1) / BN, 2);
+      q.b_mn = 1;
+      q.D = C;
+      q.ldd = 2LL * I;
+      q.glu_I = I;
+      q.aux = const_cast<void*>(gu);
+      q.ld_aux = 2LL * I;
+      if ((rc = glu_map(&a.tmD[0], C, I, rows, q.ldd))) return rc;
+      if ((rc = glu_map(&a.tmE[0], gu, I, rows, q.ld_aux))) return rc;
+      break;
+    case 3:
+      if ((rc = operand_map(&a.tmA[0], A, false, rows, 2 * I, 1, 2LL * I, 0, BM))) return rc;
+      if ((rc = operand_map(&a.tmB[0], Wg, true, H, I, up_off + E, H, (long long)I * H, BN))) return rc;
+      q = base_problem(rows, H, 2 * I, 1, (H + BN - 1) / BN, 0);
+      q.b_mn = 1;
+      q.k_split = I;
+      q.D = C;
+      q.ldd = H;
+      if ((rc = plain_epi_maps(a, 0))) return rc;
+      break;
+    default:
+      B200_CHECK_ARG(false, "moe_gemm: unknown mode %d", mode);
+  }
+  q.seg = 1;
+  q.up_off = up_off;
+  q.seg_tile = tile_expert;
+  q.seg_ntiles = n_tiles;
+  return launch(a, 1, stream, silu != 0, true);
+}
+
+// G[e] [R, Cc] += P[rows_e]^T Q[rows_e] over expert e's counts[e] rows from seg_off[e] (P, Q: `rows` rows of leading
+// dimension ldp / ldq); the pad rows of every segment must be zero in P or in Q, since K runs in blocks of 64 rows
+// inside the 128-padded segment.  beta = 1 through the epilogue's C input; an expert without rows is skipped.
+int moe_wgrad(const void* P, long long ldp, const void* Q, long long ldq, void* G, int R, int Cc, int E, int rows,
+              const int* counts, const int* seg_off, cudaStream_t stream) {
+  B200_CHECK_ARG(R > 0 && Cc > 0 && E > 0 && rows >= 0 && R % 8 == 0 && Cc % 8 == 0 && ldp % 8 == 0 && ldq % 8 == 0,
+                 "moe_wgrad: R=%d, C=%d, ldp=%lld, ldq=%lld must be multiples of 8", R, Cc, ldp, ldq);
+  if (rows == 0) return B200_OK;
+  Args a;
+  int rc;
+  if ((rc = operand_map(&a.tmA[0], P, true, R, rows, 1, ldp, 0, BM))) return rc;
+  if ((rc = operand_map(&a.tmB[0], Q, true, Cc, rows, 1, ldq, 0, BN))) return rc;
+  Problem& q = a.p[0];
+  q = base_problem(R, Cc, rows, E, (Cc + BN - 1) / BN, 0);
+  q.a_mn = 1;
+  q.b_mn = 1;
+  q.beta = 1.0f;
+  q.C = G;
+  q.ldc = Cc;
+  q.strideC = (long long)R * Cc;
+  q.D = G;
+  q.ldd = Cc;
+  q.strideD = (long long)R * Cc;
+  if ((rc = plain_epi_maps(a, 0))) return rc;
+  q.seg = 2;
+  q.seg_counts = counts;
+  q.seg_off = seg_off;
+  return launch(a, 1, stream, false, true);
 }
 
 }  // namespace b200

@@ -9,7 +9,9 @@ HBM layout (one allocation each, sized for one 80 GB H100 -- nothing is sharded 
 
 Every 2-D parameter of a given shape sits in one contiguous [batch, rows, cols] block, so the
 optimizer runs ONE batched kernel sequence per shape (Newton-Schulz over 24 q_proj/o_proj matrices
-is a single batched GEMM chain) and the data-parallel all-reduce is a single NCCL call on `grad`.
+is a single batched GEMM chain) and the data-parallel all-reduce is a single NCCL call on `grad`.  A 3-D parameter
+[E, r, c] (a MoE layer's stacked expert weights) enters the (r, c) group as E consecutive matrices, so each expert
+is orthogonalised on its own; the parameter and its .grad stay single [E, r, c] views.
 The reference keeps a Python dict of separate arrays and loops over it (optimizers/muon.py:91).
 """
 from __future__ import annotations
@@ -66,13 +68,21 @@ class ParamStore:
         groups: "OrderedDict[Tuple[int, int], MatGroup]" = OrderedDict()
         vec_named = []
         for name, p in named:
-            if p.dim() == 2:
+            if p.dim() == 2 and not getattr(p, "_b200_elementwise", False):
                 r, c = p.shape
                 if c % 8 != 0:
                     raise ValueError(
                         f"2-D parameter {name} has {c} columns; the tensor-core path needs a multiple of 8 "
                         "(16-byte TMA rows)")
                 groups.setdefault((r, c), MatGroup(r, c)).names.append(name)
+            elif p.dim() == 3:
+                # stacked expert weights [E, r, c]: E consecutive matrices of the (r, c) group, one entry per matrix
+                # (the name repeated), so Newton-Schulz treats every expert as its own matrix
+                nb, r, c = p.shape
+                if c % 8 != 0:
+                    raise ValueError(
+                        f"3-D parameter {name} has {c} columns; the tensor-core path needs a multiple of 8")
+                groups.setdefault((r, c), MatGroup(r, c)).names.extend([name] * nb)
             else:
                 vec_named.append((name, p))
         off = 0
@@ -100,9 +110,13 @@ class ParamStore:
         self.acc: Optional[torch.Tensor] = None
 
         self.index: Dict[str, Tuple[int, Tuple[int, ...]]] = {}
+        params_by_name = dict(named)
         for g in self.mat_groups:
             for i, n in enumerate(g.names):
-                self.index[n] = (g.offset + i * g.rows * g.cols, (g.rows, g.cols))
+                if n in self.index:
+                    continue
+                shape = tuple(params_by_name[n].shape)
+                self.index[n] = (g.offset + i * g.rows * g.cols, shape)
         for e in self.vec_entries:
             self.index[e.name] = (e.offset, e.shape)
 

@@ -1222,6 +1222,240 @@ def glu(gate: torch.Tensor, up: torch.Tensor, act: str = "sigmoid2") -> torch.Te
     return gate * torch.sigmoid(up) * 2
 
 
+MOE_MODES = {"gateup": 0, "down": 1, "down_bwd": 2, "gateup_dgrad": 3}
+_MOE_ACT = {"sigmoid2": 0, "silu": 1}
+
+
+class MoeRouting:
+    """Device-side result of b200_moe_route for T tokens: ids / weights [T, k], probs [T, E], counts [E],
+    seg_off [E + 1], tile_expert [max_tiles], n_tiles [1], dest [T, k], and with aux the load-balancing partials
+    aux_counts / aux_psum [E] over the unmasked tokens.  rows = max_tiles * 128 bounds the permuted buffer."""
+
+    def __init__(self, logits: torch.Tensor, k: int, mask: Optional[torch.Tensor], aux: bool):
+        _need(logits, torch.float32, "logits")
+        T, E = logits.shape
+        dev = logits.device
+        L = lib()
+        self.T, self.E, self.k = T, E, k
+        self.max_tiles = int(L.b200_moe_max_tiles(T, E, k))
+        self.rows = self.max_tiles * 128
+        i32 = dict(device=dev, dtype=torch.int32)
+        self.ids = torch.empty((T, k), **i32)
+        self.dest = torch.empty((T, k), **i32)
+        self.weights = torch.empty((T, k), device=dev, dtype=torch.float32)
+        self.probs = torch.empty((T, E), device=dev, dtype=torch.float32)
+        self.counts = torch.empty(E, **i32)
+        self.seg_off = torch.empty(E + 1, **i32)
+        self.tile_expert = torch.empty(max(self.max_tiles, 1), **i32)
+        self.n_tiles = torch.empty(1, **i32)
+        self.mask = mask
+        self.aux_counts = torch.empty(E, device=dev, dtype=torch.float32) if aux else None
+        self.aux_psum = torch.empty(E, device=dev, dtype=torch.float32) if aux else None
+        ws = torch.empty(int(L.b200_moe_route_workspace_bytes(T, E, k)), device=dev, dtype=torch.uint8)
+        tok = _t0("moe_route")
+        check(L.b200_moe_route(logits.data_ptr(), _ptr(mask), T, E, k, self.ids.data_ptr(), self.weights.data_ptr(),
+                               self.probs.data_ptr(), self.counts.data_ptr(), self.seg_off.data_ptr(),
+                               self.tile_expert.data_ptr(), self.n_tiles.data_ptr(), self.dest.data_ptr(),
+                               _ptr(self.aux_counts), _ptr(self.aux_psum), ws.data_ptr(), ws.numel(), _stream()),
+              "b200_moe_route")
+        _t1(tok)
+
+
+def moe_route(logits: torch.Tensor, k: int, mask: Optional[torch.Tensor] = None, aux: bool = False) -> MoeRouting:
+    return MoeRouting(logits, k, mask, aux)
+
+
+def moe_permute(x2: torch.Tensor, r: MoeRouting) -> torch.Tensor:
+    """[r.rows, H] bf16: token rows at their destinations, pad rows of every segment zero (rows past the last
+    segment are not written and never read)."""
+    T, H = x2.shape
+    xp = torch.empty((r.rows, H), device=x2.device, dtype=torch.bfloat16)
+    tok = _t0("moe_permute")
+    check(lib().b200_moe_permute(x2.data_ptr(), r.dest.data_ptr(), r.counts.data_ptr(), r.seg_off.data_ptr(), T, H,
+                                 r.k, r.E, xp.data_ptr(), _stream()), "b200_moe_permute")
+    _t1(tok)
+    return xp
+
+
+def moe_gemm(mode: str, act: str, a: torch.Tensor, w0: torch.Tensor, w1: Optional[torch.Tensor], r: MoeRouting,
+             gu: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """One expert-segmented GEMM (include/b200_hotpath.h b200_moe_gemm).  Returns (C, Y); Y only for "gateup"."""
+    m = MOE_MODES[mode]
+    if mode in ("gateup", "gateup_dgrad"):
+        E, I, H = w0.shape
+    else:
+        E, H, I = w0.shape
+    rows = r.rows
+    ncol = {"gateup": 2 * I, "down": H, "down_bwd": 2 * I, "gateup_dgrad": H}[mode]
+    c = torch.empty((rows, ncol), device=a.device, dtype=torch.bfloat16)
+    y = torch.empty((rows, I), device=a.device, dtype=torch.bfloat16) if mode == "gateup" else None
+    tok = _t0(f"moe_{mode}")
+    check(lib().b200_moe_gemm(m, _MOE_ACT[act], a.data_ptr(), w0.data_ptr(), _ptr(w1), _ptr(gu), c.data_ptr(),
+                              _ptr(y), r.tile_expert.data_ptr(), r.n_tiles.data_ptr(), r.max_tiles, H, I, E,
+                              _stream()),
+          "b200_moe_gemm")
+    _t1(tok)
+    return c, y
+
+
+def moe_wgrad(p: torch.Tensor, ldp: int, q: torch.Tensor, ldq: int, g: torch.Tensor, r: MoeRouting) -> None:
+    """g[e] ([E, R, C] bf16, contiguous) += p[rows_e]^T q[rows_e] for every expert (the pad rows of p or q are zero)."""
+    E, R, Cc = g.shape
+    tok = _t0("moe_wgrad")
+    check(lib().b200_moe_wgrad(p.data_ptr(), ldp, q.data_ptr(), ldq, g.data_ptr(), R, Cc, E, r.rows,
+                               r.counts.data_ptr(), r.seg_off.data_ptr(), _stream()), "b200_moe_wgrad")
+    _t1(tok)
+
+
+def moe_combine(yp: torch.Tensor, r: MoeRouting) -> torch.Tensor:
+    H = yp.shape[1]
+    out = torch.empty((r.T, H), device=yp.device, dtype=torch.bfloat16)
+    tok = _t0("moe_combine")
+    check(lib().b200_moe_combine_fwd(yp.data_ptr(), r.dest.data_ptr(), r.weights.data_ptr(), r.T, H, r.k,
+                                     out.data_ptr(), _stream()), "b200_moe_combine_fwd")
+    _t1(tok)
+    return out
+
+
+def moe_combine_bwd(dout: torch.Tensor, yp: torch.Tensor, r: MoeRouting, aux_grad: Optional[torch.Tensor]):
+    """(dyp [rows, H] bf16 (pad rows zero), dw [T, k] fp32, dlogits [T, E] fp32)."""
+    T, H = dout.shape
+    dyp = torch.empty_like(yp)
+    dw = torch.empty((T, r.k), device=dout.device, dtype=torch.float32)
+    dlogits = torch.empty((T, r.E), device=dout.device, dtype=torch.float32)
+    tok = _t0("moe_combine_bwd")
+    check(lib().b200_moe_combine_bwd(dout.data_ptr(), yp.data_ptr(), r.dest.data_ptr(), r.ids.data_ptr(),
+                                     r.weights.data_ptr(), r.probs.data_ptr(), _ptr(aux_grad), _ptr(r.mask),
+                                     r.counts.data_ptr(), r.seg_off.data_ptr(), T, H, r.E, r.k, dyp.data_ptr(),
+                                     dw.data_ptr(), dlogits.data_ptr(), _stream()),
+          "b200_moe_combine_bwd")
+    _t1(tok)
+    return dyp, dw, dlogits
+
+
+def moe_unpermute(dxp: torch.Tensor, r: MoeRouting, addend: Optional[torch.Tensor] = None) -> torch.Tensor:
+    H = dxp.shape[1]
+    dx = torch.empty((r.T, H), device=dxp.device, dtype=torch.bfloat16)
+    tok = _t0("moe_unpermute")
+    check(lib().b200_moe_unpermute(dxp.data_ptr(), r.dest.data_ptr(), _ptr(addend), r.T, H, r.k, dx.data_ptr(),
+                                   _stream()), "b200_moe_unpermute")
+    _t1(tok)
+    return dx
+
+
+def _grad_sink(w: torch.Tensor) -> Tuple[torch.Tensor, bool]:
+    """(buffer the expert wgrad accumulates into, whether it is the flat-store .grad itself)."""
+    if getattr(w, "_b200_flat_grad", False) and w.grad is not None and w.grad.dtype == torch.bfloat16:
+        return w.grad, True
+    return torch.zeros_like(w, dtype=torch.bfloat16), False
+
+
+class _MoeFn(torch.autograd.Function):
+    """Mixtral's sparse MoE block on the expert-segmented kernels:
+
+      forward   logits   = x Wr^T                      fp32 library GEMM (bf16 operands, fp32 accumulation and output)
+                routing  = b200_moe_route(logits)      softmax, top-k, renormalised weights, stable counting sort
+                xp       = b200_moe_permute(x)         rows grouped by expert, segments padded to 128 rows
+                gu, y    = b200_moe_gemm(gateup)       x Wg_e^T | x Wu_e^T and the activation, per 128-row tile
+                yo       = b200_moe_gemm(down)         y Wd_e^T
+                out      = b200_moe_combine_fwd        sum_j w_j yo[dest[t, j]]
+      backward  b200_moe_combine_bwd (dyo, router adjoint), b200_moe_wgrad into the experts' flat gradients,
+                b200_moe_gemm(down_bwd), b200_moe_gemm(gateup_dgrad), b200_moe_unpermute (+ the router's dgrad).
+
+    Returns (out, aux_counts, aux_psum); the last two are the load-balancing partials over the unmasked tokens (zeros
+    when aux is off), and aux_psum carries a gradient."""
+
+    @staticmethod
+    def forward(ctx, x, wr, wg, wu, wd, k, act, mask, aux):
+        H = x.shape[-1]
+        x2 = x.reshape(-1, H).contiguous()
+        logits = torch.matmul(x2.float(), wr.float().t())
+        r = MoeRouting(logits, k, mask, aux)
+        xp = moe_permute(x2, r)
+        gu, y = moe_gemm("gateup", act, xp, wg, wu, r)
+        yo, _ = moe_gemm("down", act, y, wd, None, r)
+        out = moe_combine(yo, r)
+        ctx.save_for_backward(x2, xp, gu, y, yo, wr, wg, wu, wd)
+        ctx.routing, ctx.act, ctx.x_shape = r, act, x.shape
+        E = wr.shape[0]
+        counts = r.aux_counts if aux else torch.zeros(E, device=x.device, dtype=torch.float32)
+        psum = r.aux_psum if aux else torch.zeros(E, device=x.device, dtype=torch.float32)
+        ctx.mark_non_differentiable(counts)
+        ctx.aux = aux
+        return out.view(*x.shape[:-1], H), counts, psum
+
+    @staticmethod
+    def backward(ctx, dout, _dcounts, dpsum):
+        x2, xp, gu, y, yo, wr, wg, wu, wd = ctx.saved_tensors
+        r, act = ctx.routing, ctx.act
+        H = x2.shape[1]
+        I = wg.shape[1]
+        d2 = dout.reshape(-1, H).contiguous().to(torch.bfloat16)
+        aux_grad = dpsum.float().contiguous() if (ctx.aux and dpsum is not None) else None
+        dyo, _dw, dlogits = moe_combine_bwd(d2, yo, r, aux_grad)
+        gwd, flat_d = _grad_sink(wd)
+        moe_wgrad(dyo, H, y, I, gwd, r)                                   # dWd_e += dyo^T y
+        dgu, _ = moe_gemm("down_bwd", act, dyo, wd, None, r, gu=gu)
+        gwg, flat_g = _grad_sink(wg)
+        gwu, flat_u = _grad_sink(wu)
+        moe_wgrad(dgu, 2 * I, xp, H, gwg, r)                              # dWg_e += dg^T x
+        moe_wgrad(dgu[:, I:], 2 * I, xp, H, gwu, r)                       # dWu_e += du^T x
+        dxp, _ = moe_gemm("gateup_dgrad", act, dgu, wg, wu, r)
+        dx = None
+        if ctx.needs_input_grad[0]:
+            dx = moe_unpermute(dxp, r, torch.matmul(dlogits, wr.float())).view(ctx.x_shape)
+        dwr = torch.matmul(dlogits.t(), x2.float())
+        if getattr(wr, "_b200_flat_grad", False) and wr.grad is not None:
+            wr.grad.copy_(wr.grad.float() + dwr)
+            dwr = None
+        else:
+            dwr = dwr.to(wr.dtype)
+        return (dx, dwr, None if flat_g else gwg, None if flat_u else gwu, None if flat_d else gwd,
+                None, None, None, None)
+
+
+def moe(x: torch.Tensor, w_router: torch.Tensor, wg: torch.Tensor, wu: torch.Tensor, wd: torch.Tensor, k: int,
+        act: str = "sigmoid2", pad_mask: Optional[torch.Tensor] = None, aux: bool = False):
+    """Mixtral's sparse MoE block (no jitter): x [..., H] bf16, w_router [E, H], wg / wu [E, I, H], wd [E, H, I], all
+    bf16 and contiguous.  Each token goes to the top-k experts of softmax(x Wr^T) with the renormalised weights;
+    expert e computes down_e(act(gate_e x, up_e x)).  pad_mask (bool [...], optional) selects the tokens of the
+    load-balancing partials; aux=False skips them and their gradient.  Returns (out [..., H], aux_counts [E],
+    aux_psum [E])."""
+    _check_choice(act, GLU_ACTS, "moe: act")
+    for t, nm in ((x, "x"), (w_router, "w_router"), (wg, "wg"), (wu, "wu"), (wd, "wd")):
+        _need(t, torch.bfloat16, nm)
+    H = x.shape[-1]
+    if w_router.dim() != 2 or w_router.shape[1] != H:
+        raise ValueError(f"w_router must be [E, {H}], got {list(w_router.shape)}")
+    E = w_router.shape[0]
+    if not 2 <= E <= 64:
+        raise ValueError(f"w_router: number of experts must lie in 2..64, got {E}")
+    if wg.dim() != 3 or wg.shape[0] != E or wg.shape[2] != H:
+        raise ValueError(f"wg must be [{E}, I, {H}], got {list(wg.shape)}")
+    I = wg.shape[1]
+    if wu.shape != wg.shape:
+        raise ValueError(f"wu must be {list(wg.shape)}, got {list(wu.shape)}")
+    if tuple(wd.shape) != (E, H, I):
+        raise ValueError(f"wd must be {[E, H, I]}, got {list(wd.shape)}")
+    if H % 8 != 0 or I % 64 != 0:
+        raise ValueError(f"x: hidden {H} must be a multiple of 8 and the intermediate size {I} of 64")
+    step = I * H * wg.element_size()
+    d = wu.data_ptr() - wg.data_ptr()
+    if d <= 0 or d % step or d // step < E:
+        raise ValueError("wu must lie E or more whole [I, hidden] matrices after wg in memory (one tensor map "
+                         "addresses both; flat.ParamStore lays a layer's gate and up experts out that way)")
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(E, 8):
+        raise ValueError(f"k must be an integer in 1..{min(E, 8)}, got {k!r}")
+    mask = None
+    if pad_mask is not None:
+        if tuple(pad_mask.shape) != tuple(x.shape[:-1]):
+            raise ValueError(f"pad_mask must be {list(x.shape[:-1])}, got {list(pad_mask.shape)}")
+        mask = pad_mask.reshape(-1).to(device=x.device, dtype=torch.uint8).contiguous()
+    if x.numel() == 0:
+        raise ValueError("x: no tokens")
+    return _MoeFn.apply(x, w_router, wg, wu, wd, k, act, mask, bool(aux))
+
+
 class _CrossEntropyFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits2d, targets, V, pad_token):

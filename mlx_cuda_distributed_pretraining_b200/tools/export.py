@@ -1,5 +1,6 @@
 """Export a run trained with `model.misc.variant: mlx_lm` as an mlx-lm / Hugging Face `LlamaForCausalLM` directory
-(the reference's tools/convert-to-mlx-lm.py, with its CLI and config fields).
+(the reference's tools/convert-to-mlx-lm.py, with its CLI and config fields), or as `MixtralForCausalLM` when the run
+has `model.misc.num_local_experts > 0`.
 
 The run's checkpoint holds the fp32 master weights under the trainer's flat names; they are renamed to the mlx-lm /
 HF names and written as fp32 `model.safetensors` next to `config.json`.  q / k weights are not permuted: the
@@ -26,6 +27,26 @@ _LAYER_NAMES = {
 }
 
 
+_MOE = re.compile(r"block_sparse_moe\.switch_mlp\.(gate_proj|up_proj|down_proj)\.weight")
+_MOE_HF = {"gate_proj": "w1", "down_proj": "w2", "up_proj": "w3"}
+
+
+def hf_tensors(name: str, t: torch.Tensor) -> Dict[str, torch.Tensor]:
+    """One trainer parameter -> its mlx-lm / HF tensors.  Stacked experts [E, out, in] are split into Mixtral's
+    per-expert checkpoint names `block_sparse_moe.experts.J.w1|w2|w3.weight` (gate, down, up), the layout both
+    transformers' MixtralForCausalLM.from_pretrained and mlx-lm's Mixtral loader convert from."""
+    m = _LAYER.fullmatch(name)
+    if m:
+        e = _MOE.fullmatch(m.group(2))
+        if e:
+            w = _MOE_HF[e.group(1)]
+            return {f"model.layers.{m.group(1)}.block_sparse_moe.experts.{j}.{w}.weight": t[j].contiguous()
+                    for j in range(t.shape[0])}
+        if m.group(2) == "block_sparse_moe.gate.weight":
+            return {f"model.layers.{m.group(1)}.block_sparse_moe.gate.weight": t}
+    return {hf_name(name): t}
+
+
 def hf_name(name: str) -> str:
     """The trainer's flat parameter name -> the mlx-lm / HF Llama name."""
     if name in ("embed_tokens.weight", "norm.weight"):
@@ -45,7 +66,8 @@ def check_exportable(model_cfg) -> None:
     misc, rope, attn = model_cfg.misc, model_cfg.rope, model_cfg.attention
     if misc.get("variant") != "mlx_lm":
         raise ValueError("only runs trained with model.misc.variant: mlx_lm can be exported: the reference block "
-                         "(gate * sigmoid(up) * 2, no or interleaved RoPE) is not LlamaForCausalLM")
+                         "(gate * sigmoid(up) * 2, no or interleaved RoPE) is not LlamaForCausalLM"
+                         + (" or MixtralForCausalLM" if misc.get("num_local_experts") else ""))
     if rope.get("traditional"):
         raise ValueError("rope.traditional: true (interleaved RoPE) has no LlamaForCausalLM config")
     if attn.get("sliding_window") is not None:
@@ -55,7 +77,21 @@ def check_exportable(model_cfg) -> None:
 
 
 def hf_config(cfg, vocab_size: int, bos: int, eos: int) -> dict:
-    """config.json: the reference exporter's fields, plus num_key_value_heads, head_dim and model_type "llama"."""
+    """config.json: the reference exporter's fields, plus num_key_value_heads, head_dim and model_type "llama"; a
+    MoE run (model.misc.num_local_experts > 0) is a MixtralForCausalLM config with its expert fields."""
+    m = cfg.model
+    d = _llama_config(cfg, vocab_size, bos, eos)
+    E = m.misc.get("num_local_experts") or 0
+    if E:
+        d.pop("mlp_bias")
+        d.update(architectures=["MixtralForCausalLM"], model_type="mixtral", num_local_experts=E,
+                 num_experts_per_tok=m.misc["num_experts_per_tok"],
+                 router_aux_loss_coef=float(m.misc.get("router_aux_loss_coef", 0.001)), router_jitter_noise=0.0,
+                 output_router_logits=False, sliding_window=None)
+    return d
+
+
+def _llama_config(cfg, vocab_size: int, bos: int, eos: int) -> dict:
     m = cfg.model
     heads = m.attention["num_heads"]
     return {
@@ -116,7 +152,7 @@ def export_run(run: str, out_path: str, runs_dir: str = "runs", checkpoint: Opti
     weights = load_file(str(ck))
     out: Dict[str, torch.Tensor] = {}
     for name, t in weights.items():
-        out[hf_name(name)] = t.float().contiguous()
+        out.update(hf_tensors(name, t.float().contiguous()))
     tied = bool(cfg.model.misc["tie_word_embeddings"])
     if tied:
         out.pop("lm_head.weight", None)
