@@ -51,6 +51,23 @@ __device__ __forceinline__ float ldf(const __nv_bfloat16* p) { return __bfloat16
 __device__ __forceinline__ void stf(float* p, float v) { *p = v; }
 __device__ __forceinline__ void stf(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
+// The last, partial vector of a range whose length is not a multiple of 8: `cnt` valid elements, the other lanes 0.
+// A kernel that sends it through the same arithmetic as the full vectors gives every element the same bits wherever
+// it falls in a flat buffer (the compiler contracts a separate scalar loop's multiply-adds differently).
+template <typename T>
+__device__ __forceinline__ void load8n(const T* p, float* f, int cnt) {
+  if (cnt == 8) return load8(p, f);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) f[j] = j < cnt ? ldf(p + j) : 0.f;
+}
+template <typename T>
+__device__ __forceinline__ void store8n(T* p, const float* f, int cnt) {
+  if (cnt == 8) return store8(p, f);
+#pragma unroll
+  for (int j = 0; j < 8; ++j)
+    if (j < cnt) stf(p + j, f[j]);
+}
+
 __device__ __forceinline__ float block_sum(float v) {
   __shared__ float red[EW_THREADS / 32];
   v = warp_sum(v);
@@ -259,13 +276,14 @@ adam_direction_kernel(float* __restrict__ d, const G* __restrict__ g, float* __r
                       float bc1, float bc2, float gscale) {
   const float step = lr / bc1;
   const float rs_bc2 = rsqrtf(bc2);
-  const long long nvec = n / 8;
-  for (long long i = (long long)blockIdx.x * EW_THREADS + threadIdx.x; i < nvec;
+  const long long nvec = n / 8, nvec_all = (n + 7) / 8;   // the tail (n % 8) is one more, partial vector
+  for (long long i = (long long)blockIdx.x * EW_THREADS + threadIdx.x; i < nvec_all;
        i += (long long)gridDim.x * EW_THREADS) {
+    const int cnt = i < nvec ? 8 : (int)(n - nvec * 8);
     float gv[8], mv[8], vv[8], dv[8];
-    load8(g + i * 8, gv);
-    load8(m + i * 8, mv);
-    load8(v + i * 8, vv);
+    load8n(g + i * 8, gv, cnt);
+    load8n(m + i * 8, mv, cnt);
+    load8n(v + i * 8, vv, cnt);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const float gj = gv[j] * gscale;
@@ -273,19 +291,9 @@ adam_direction_kernel(float* __restrict__ d, const G* __restrict__ g, float* __r
       vv[j] = b2 * vv[j] + (1.0f - b2) * gj * gj;
       dv[j] = -step * mv[j] / (sqrtf(vv[j]) * rs_bc2 + eps);
     }
-    store8(m + i * 8, mv);
-    store8(v + i * 8, vv);
-    store8(d + i * 8, dv);
-  }
-  if (blockIdx.x == 0) {
-    for (long long i = nvec * 8 + threadIdx.x; i < n; i += EW_THREADS) {
-      const float gj = ldf(g + i) * gscale;
-      const float mm = b1 * m[i] + (1.0f - b1) * gj;
-      const float vv = b2 * v[i] + (1.0f - b2) * gj * gj;
-      m[i] = mm;
-      v[i] = vv;
-      d[i] = -step * mm / (sqrtf(vv) * rs_bc2 + eps);
-    }
+    store8n(m + i * 8, mv, cnt);
+    store8n(v + i * 8, vv, cnt);
+    store8n(d + i * 8, dv, cnt);
   }
 }
 
@@ -531,13 +539,14 @@ graft_update_kernel(float* __restrict__ p32, __nv_bfloat16* __restrict__ p16,
   const long long base = (long long)blockIdx.y * numel;
   const float c = coef[blockIdx.y], cd = coef_d[blockIdx.y];
   // batched use has numel % 8 == 0 (checked by the host wrapper), so `base` keeps 16-byte alignment
-  const long long nvec = numel / 8;
-  for (long long i = (long long)blockIdx.x * EW_THREADS + threadIdx.x; i < nvec;
+  const long long nvec = numel / 8, nvec_all = (numel + 7) / 8;   // the tail (numel % 8) is one more, partial vector
+  for (long long i = (long long)blockIdx.x * EW_THREADS + threadIdx.x; i < nvec_all;
        i += (long long)gridDim.x * EW_THREADS) {
+    const int cnt = i < nvec ? 8 : (int)(numel - nvec * 8);
     float pv[8], rv[8], dv[8];
-    load8(p32 + base + i * 8, pv);
-    load8(pre + base + i * 8, rv);
-    load8(d + base + i * 8, dv);
+    load8n(p32 + base + i * 8, pv, cnt);
+    load8n(pre + base + i * 8, rv, cnt);
+    load8n(d + base + i * 8, dv, cnt);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       // a zero coefficient must drop its term even when the term is inf/nan (overflowed Shampoo step, D10)
@@ -546,17 +555,8 @@ graft_update_kernel(float* __restrict__ p32, __nv_bfloat16* __restrict__ p16,
       if (cd != 0.f) v += cd * dv[j];
       pv[j] = v;
     }
-    store8(p32 + base + i * 8, pv);
-    if (p16) store8(p16 + base + i * 8, pv);
-  }
-  if (blockIdx.x == 0) {
-    for (long long i = nvec * 8 + threadIdx.x; i < numel; i += EW_THREADS) {
-      float v = p32[base + i] * decay;
-      if (c != 0.f) v += c * pre[base + i];
-      if (cd != 0.f) v += cd * d[base + i];
-      p32[base + i] = v;
-      if (p16) p16[base + i] = __float2bfloat16_rn(v);
-    }
+    store8n(p32 + base + i * 8, pv, cnt);
+    if (p16) store8n(p16 + base + i * 8, pv, cnt);
   }
 }
 
