@@ -383,6 +383,20 @@ size_t b200_attn_bwd_window_workspace_bytes(int B, int S, int H, int Hk, int D);
 int b200_attn_bwd_window(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                          const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
                          float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
+/* ALiBi (Press et al., "Train Short, Test Long"): b200_attn_fwd_window / b200_attn_bwd_window with the bias
+ * slopes[h] * (k - s) <= 0 added to the scaled score of query s, key k, query head h before the mask and the softmax
+ * (the order of the reference's FlexAttention score_mod, arch/flex_attention.py:193-235).  slopes: device fp32 [H],
+ * one per QUERY head (the heads of a GQA group keep their own slopes), 4-byte aligned and non-null; its values are not
+ * checked, since that would read the device.  pos and window as for the window entries (pos NULL: one document per
+ * row; window < 0: no window).  k - s is also the distance inside a document, so packed rows need no more input.
+ * Causal only.  The backward's workspace is b200_attn_bwd_window_workspace_bytes.  Zero slopes give the window
+ * entries' results bit for bit. */
+int b200_attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                        const float* slopes, int B, int S, int H, int Hk, int D, float scale, void* stream);
+int b200_attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                        const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                        int H, int Hk, int D, float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes,
+                        void* stream);
 
 /* ---- generation: decode attention over a KV cache (arch/flash_attention.py:97-156, last query row) ------------
  * One new query per sequence against its cached keys, causal by construction (every cached key precedes it):
@@ -405,6 +419,12 @@ int b200_attn_decode(const void* q, const void* k_cache, const void* v_cache, co
 int b200_attn_decode_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o,
                             float* lse, int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
                             void* workspace, size_t workspace_bytes, void* stream);
+/* b200_attn_decode_window (window < 0: no window) with ALiBi: the query at position p = lens[b] - 1 adds
+ * slopes[h] * (k - p) to the scaled score of cached key k, slopes as for b200_attn_fwd_alibi (device fp32 [H], not
+ * checked).  Same workspace as b200_attn_decode; a row's output is still bit-identical alone or in any batch. */
+int b200_attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o,
+                           float* lse, int window, const float* slopes, int B, int s_max, int H, int Hk, int D,
+                           float scale, int is_bf16, void* workspace, size_t workspace_bytes, void* stream);
 /* Appends one token per row at pos = lens[b] - 1: k_cache[b,pos] = rot(k[b]), v_cache[b,pos] = v[b] (k, v:
  * [B,Hk,D]).  With cos_t/sin_t (f32 [>= max pos + 1, D/2], ops.rope_tables) the interleaved-pair rotation of
  * b200_rope (arch/llama_standard.py:90-131) is applied to k and, in place, to q [B,H,D], with b200_rope's exact

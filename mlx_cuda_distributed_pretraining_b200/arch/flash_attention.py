@@ -14,6 +14,21 @@ from torch import nn
 from .. import ops
 
 
+def alibi_slopes(num_heads: int) -> torch.Tensor:
+    """ALiBi's per-head slopes (Press et al., "Train Short, Test Long"), fp32 [num_heads] on the CPU.  For H a power
+    of two, m_i = 2^(-8 i / H), i = 1 .. H.  Otherwise, with n = 2^floor(log2 H): the n slopes of the rule for n,
+    then the odd-indexed slopes (i = 1, 3, 5, ...) of the rule for 2n, the first H - n of them."""
+    if isinstance(num_heads, bool) or not isinstance(num_heads, int) or num_heads < 1:
+        raise ValueError(f"alibi_slopes: num_heads must be a positive int, got {num_heads!r}")
+
+    def pow2(n: int):
+        return [2.0 ** (-8.0 * i / n) for i in range(1, n + 1)]
+
+    n = 1 << (num_heads.bit_length() - 1)
+    slopes = pow2(n) + pow2(2 * n)[0::2][:num_heads - n]
+    return torch.tensor(slopes, dtype=torch.float32)
+
+
 def _window(window: Optional[int]) -> Optional[int]:
     if window is not None and (isinstance(window, bool) or not isinstance(window, int) or window < 0):
         raise ValueError(f"sliding window must be None or a non-negative int, got {window!r}")
@@ -68,9 +83,12 @@ class DocumentCausalMask:
 
 
 class FlashAttention(nn.Module):
+    """alibi: add ALiBi's bias alibi_slopes(num_heads)[h] * (k - q) to every causal score (the slopes are not
+    parameters: a device tensor made on first use, like rope_tables)."""
+
     def __init__(self, hidden_size: int, num_heads: int, num_kv_heads: Optional[int] = None,
                  head_dim: Optional[int] = None, dropout: float = 0.0, use_bias: bool = False,
-                 flash_block_size: int = 128):
+                 flash_block_size: int = 128, alibi: bool = False):
         super().__init__()
         self.hidden_size = hidden_size
         self.num_heads = num_heads
@@ -86,6 +104,16 @@ class FlashAttention(nn.Module):
         self.o_proj = nn.Linear(self.num_heads * self.head_dim, hidden_size, bias=use_bias)
         self.scale = self.head_dim ** -0.5
         self.rope_tables = None  # (cos, sin) set by the parent when RoPE is enabled
+        self.alibi = bool(alibi)
+        self._alibi_slopes = None  # fp32 [num_heads] on the device, made on first use
+
+    def alibi_slopes(self, device) -> Optional[torch.Tensor]:
+        """The ALiBi slopes on `device` (None without ALiBi)."""
+        if not self.alibi:
+            return None
+        if self._alibi_slopes is None or self._alibi_slopes.device != torch.device(device):
+            self._alibi_slopes = alibi_slopes(self.num_heads).to(device)
+        return self._alibi_slopes
 
     def _flash_attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask=None) -> torch.Tensor:
         """q [B,S,H,D], k/v [B,S,Hk,D] -> [B,S,H,D]."""
@@ -100,14 +128,15 @@ class FlashAttention(nn.Module):
             raise NotImplementedError(
                 "the fused kernel supports mask=None, the causal mask (CausalMask) or the document-causal mask of "
                 "packed rows (DocumentCausalMask); arbitrary additive masks are outside the reference's training path")
+        alibi = self.alibi_slopes(q.device)
         dt = q.dtype
         if dt == torch.float32 and 3 * self.head_dim <= 128:
             # full-precision configs (mixed_precision: false, e.g. BASELINE C1, head_dim 16): logits through
             # three-term bf16 products (hi/lo split operands), ~fp32-accurate scores on the same kernels
-            return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos, window=window)
+            return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi)
         if dt != torch.bfloat16:  # larger head dims: bf16 operands with fp32 accumulation (stated in DESIGN.md)
             q, k, v = q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
-        o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window)
+        o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi)
         return o if dt == torch.bfloat16 else o.to(dt)
 
     def forward(self, x: torch.Tensor, mask=None, rope_layout: str = "interleaved") -> torch.Tensor:
@@ -162,12 +191,13 @@ class FlashAttention(nn.Module):
                        rope_layout: str = "interleaved") -> torch.Tensor:
         """One new token per row, x [B, hidden]: its k and v go to cache position lens[b] - 1 (rotated there when
         RoPE is on), then its query attends over the row's first lens[b] cached keys (the last window + 1 of them
-        with a sliding window)."""
+        with a sliding window), with the ALiBi bias when the module has it."""
         B = x.shape[0]
         q, k, v = self._project(x)
         q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
         k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         ops.kv_append(q, k, v, k_cache, v_cache, lens, self.rope_tables, layout=rope_layout)
-        ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace, window=window)
+        ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace, window=window,
+                                   alibi=self.alibi_slopes(q.device))
         return self._out(ctx.reshape(B, self.num_heads * self.head_dim))

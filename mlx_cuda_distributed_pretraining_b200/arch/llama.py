@@ -58,6 +58,7 @@ class ModelArgs:
     num_experts_per_tok: int = 0
     apply_rope: bool = False  # extension; see module docstring
     sliding_window: Optional[int] = None  # extension: query q sees keys q - W .. q in every layer (None: causal)
+    alibi: bool = False  # extension: ALiBi's bias slope_h * (k - q) on every layer's attention scores
     variant: Optional[str] = None  # extension: None / "reference" (this block) or "mlx_lm" (module docstring)
     router_aux_loss_coef: float = 0.001  # with num_local_experts > 0: weight of the load-balancing loss
 
@@ -138,7 +139,8 @@ class AttentionModule(nn.Module):
                  head_dim: Optional[int] = None, max_positions: int = 4096, rope_theta: float = 10000.0,
                  rope_traditional: bool = False, rope_scaling: Optional[Dict[str, Any]] = None,
                  use_bias: bool = False, use_flash_attention: bool = True, use_flex_attention: bool = False,
-                 flash_block_size: int = 128, apply_rope: bool = False, rope_layout: str = "interleaved"):
+                 flash_block_size: int = 128, apply_rope: bool = False, rope_layout: str = "interleaved",
+                 alibi: bool = False):
         super().__init__()
         self.rope_layout = rope_layout
         if use_flex_attention:
@@ -149,7 +151,7 @@ class AttentionModule(nn.Module):
         self.head_dim = head_dim or (hidden_size // num_heads)
         # SimpleAttention (use_flash_attention=False) computes the same function; one kernel serves both
         self.attn = FlashAttention(hidden_size, num_heads, self.num_kv_heads, self.head_dim,
-                                   use_bias=use_bias, flash_block_size=flash_block_size)
+                                   use_bias=use_bias, flash_block_size=flash_block_size, alibi=alibi)
         self.scale = self.head_dim ** -0.5
         self.apply_rope = apply_rope
         self.max_positions = max_positions
@@ -188,7 +190,7 @@ class TransformerBlock(nn.Module):
             use_bias=args.attention_bias, use_flash_attention=args.use_flash_attention,
             use_flex_attention=args.use_flex_attention, flash_block_size=args.flash_block_size,
             apply_rope=args.apply_rope or mlx_lm,
-            rope_layout="half" if mlx_lm and not args.rope_traditional else "interleaved")
+            rope_layout="half" if mlx_lm and not args.rope_traditional else "interleaved", alibi=args.alibi)
         self.post_attention_layernorm = RMSNorm(args.hidden_size, eps=args.rms_norm_eps)
         act = "silu" if mlx_lm else "sigmoid2"
         self.moe = bool(args.num_local_experts)

@@ -113,6 +113,16 @@ def sample(logits: torch.Tensor, temp: float, min_p: Optional[float], top_p: Opt
 # ------------------------------------------------------------------------------------------------
 # generation
 # ------------------------------------------------------------------------------------------------
+def position_limit(args) -> Optional[int]:
+    """The longest sequence a model may generate: max_position_embeddings, or None (no limit) for an ALiBi model
+    without RoPE, whose attention depends on key distances alone and so runs past its training length (the KV cache
+    is sized to prompt + max_tokens)."""
+    rope = getattr(args, "apply_rope", False) or getattr(args, "variant", None) == "mlx_lm"
+    if getattr(args, "alibi", False) and not rope:
+        return None
+    return args.max_position_embeddings
+
+
 def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature: float = 1.0,
              min_p: Optional[float] = 0.05, top_p: Optional[float] = None, repetition_penalty: float = 1.1,
              repetition_context_size: int = 20, eos_token: Optional[int] = None, seed: Optional[int] = None,
@@ -124,9 +134,9 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
 
     if not prompts or any(len(p) == 0 for p in prompts):
         raise ValueError("every prompt needs at least one token")
-    limit = model.args.max_position_embeddings
+    limit = position_limit(model.args)
     longest = max(len(p) for p in prompts)
-    if longest + max_tokens > limit:
+    if limit is not None and longest + max_tokens > limit:
         raise ValueError(f"prompt ({longest} tokens) + max_tokens ({max_tokens}) exceeds max_position_embeddings "
                          f"({limit}): training truncates there and the RoPE tables end there")
     device = model.embed_tokens.weight.device

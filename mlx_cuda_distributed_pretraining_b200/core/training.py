@@ -69,6 +69,10 @@ class ModelConfig:
         w = self.attention.get("sliding_window")
         if w is not None and (isinstance(w, bool) or not isinstance(w, int) or w < 0):
             raise ValueError(f"model.attention.sliding_window must be null or a non-negative integer, got {w!r}")
+        # extension: attention.alibi (absent / null / false: off); ALiBi's bias slope_h * (k - q) on every score
+        a = self.attention.get("alibi")
+        if a is not None and not isinstance(a, bool):
+            raise ValueError(f"model.attention.alibi must be null, true or false, got {a!r}")
         # extension: misc.variant selects the block (absent / null / "reference": arch/llama.py's; "mlx_lm": the
         # mlx_lm.models.llama block the reference's trainer actually imports, DESIGN D4)
         v = (self.misc or {}).get("variant")
@@ -715,7 +719,8 @@ class Trainer:
             use_flex_attention=m.attention.get("use_flex_attention", False),
             flash_block_size=m.attention.get("flash_block_size", 128),
             apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")) or m.misc.get("variant") == "mlx_lm",
-            sliding_window=m.attention.get("sliding_window"), variant=m.misc.get("variant"),
+            sliding_window=m.attention.get("sliding_window"), alibi=bool(m.attention.get("alibi")),
+            variant=m.misc.get("variant"),
             num_local_experts=m.misc.get("num_local_experts") or 0,
             num_experts_per_tok=m.misc.get("num_experts_per_tok") or 0,
             router_aux_loss_coef=float(m.misc.get("router_aux_loss_coef", 0.001)))

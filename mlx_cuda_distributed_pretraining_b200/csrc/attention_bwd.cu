@@ -36,6 +36,13 @@
 // (pos == nullptr reads as pos[q] = q).  Only the pre-pass knows about W: it writes the clamped starts, and bounds each
 // key tile's query range by k0 + BKV - 1 + W as well, since no later query reaches back to the tile.  The starts stay
 // monotone, so the kernel's skipping, masked-item test and binary search are unchanged.
+//
+// ALiBi (ALIBI = true, DOC kernels only): P^T = exp2(S^T * scale*log2e + b - LSE*log2e) with the forward's bias
+// b = m_h log2e (k - q) of the item's query head h (slopes[h], read once per item: items run over the GQA group's
+// heads), on the masked and the unmasked path alike.  The bias is constant in Q and K, so dS^T = P^T (dP^T - delta) and
+// the pre-pass are unchanged.  A thread's queries are q0 + 8 nc + cq + {0, 1}: per item one integer per key is
+// converted, base = m log2e (key - q0 - cq), and each element's bias is fmaf(m log2e, -c, base) for the compile-time
+// column c.  With m = 0 the bias is exactly 0 and P^T is the DOC kernel's.  ALIBI = false compiles unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -84,6 +91,7 @@ struct BwdArgs {
   int paired;          // CTA x runs key tiles x and n_kt-1-x
   const int* dstart;   // DOC: [B,S_pad] document start of every query
   const int* qt_end;   // DOC: [B,n_kt] end of each key tile's query-tile range
+  const float* slopes; // ALIBI: [H] fp32 per-query-head slopes
 };
 
 // The work of one key tile: `group * per_head` items, item j = (query head h0 + j / per_head, query tile
@@ -116,7 +124,7 @@ __device__ __forceinline__ void rs_mma(float* acc, const uint32_t* a, uint64_t d
   else wgmma_m64n64k16_rs<1>(acc, a, db);
 }
 
-template <int D, bool DOC>
+template <int D, bool DOC, bool ALIBI = false>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
@@ -248,6 +256,15 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       wgmma_commit();
       wgmma_wait<0>();
 
+      // ALIBI: the item's head slope in log2 units, and the bias of each of this thread's keys against query
+      // q0 + cq
+      float ml2 = 0.f, abase[2] = {0.f, 0.f};
+      if constexpr (ALIBI) {
+        ml2 = __ldg(p.slopes + hk * group + j / t.per_head) * kLog2e;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) abase[r] = ml2 * (float)(key_a + 8 * r - q0 - cq);
+      }
+
       // P^T and dS^T (unscaled).  Chunk nc holds queries 8 nc + cq + {0, 1}.  Only tiles that cross the causal
       // diagonal or the end of the sequence are masked; masked entries are exactly 0.
       bool masked = (p.causal && wkey_hi > q0) || q0 + BQ > p.S || wkey_hi >= p.S;
@@ -280,7 +297,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             const int key = key_a + ((e >> 1) << 3);
             bool ok = qi < p.S && key < p.S && !(p.causal && key > qi);
             if constexpr (DOC) ok = ok && qc < n_vis[e >> 1];
-            const float pv = ok ? exp2f(st[4 * nc + e] * sl2 - lds32f(tL + qc * 4)) : 0.f;
+            float pv;
+            if constexpr (ALIBI)
+              pv = ok ? exp2f(st[4 * nc + e] * sl2 +
+                              (fmaf(ml2, -(float)(nc * 8 + (e & 1)), abase[e >> 1]) - lds32f(tL + qc * 4)))
+                      : 0.f;
+            else
+              pv = ok ? exp2f(st[4 * nc + e] * sl2 - lds32f(tL + qc * 4)) : 0.f;
             st[4 * nc + e] = pv;
             dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] - lds32f(tDlt + qc * 4)) : 0.f;
           }
@@ -292,7 +315,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
           const float2 d = lds64f(tDlt + (nc * 8 + cq) * 4);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            const float pv = exp2f(st[4 * nc + e] * sl2 - ((e & 1) ? l.y : l.x));
+            float pv;
+            if constexpr (ALIBI)
+              pv = exp2f(st[4 * nc + e] * sl2 +
+                         (fmaf(ml2, -(float)(nc * 8 + (e & 1)), abase[e >> 1]) - ((e & 1) ? l.y : l.x)));
+            else
+              pv = exp2f(st[4 * nc + e] * sl2 - ((e & 1) ? l.y : l.x));
             st[4 * nc + e] = pv;
             dpt[4 * nc + e] = pv * (dpt[4 * nc + e] - ((e & 1) ? d.y : d.x));
           }
@@ -478,11 +506,11 @@ f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ ds
   }
 }
 
-template <int D, bool DOC>
+template <int D, bool DOC, bool ALIBI = false>
 int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmDO,
                const CUtensorMap& tmDQ, const BwdArgs& a, cudaStream_t stream) {
   using Cfg = BwdCfg<D, DOC>;
-  auto kern = attn_bwd_kernel<D, DOC>;
+  auto kern = attn_bwd_kernel<D, DOC, ALIBI>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -521,10 +549,11 @@ size_t attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
 
 namespace {
 
-// doc selects the document / window kernels; window < 0 means none
+// doc selects the document / window kernels; window < 0 means none; slopes (doc only) selects ALiBi
 int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                   bool doc, const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk,
-                  int D, float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+                  int D, float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream,
+                  const float* slopes = nullptr) {
   // dk / dv rows may be strided: dkv_row_heads heads per token row (0 = Hk, i.e. contiguous [B,S,Hk,D]).
   // With dk = base, dv = base + Hk*D and dkv_row_heads = 2*Hk both land in ONE [B,S,2*Hk*D] buffer, which lets
   // the k/v projections' dgrad and wgrad run as single GEMMs over the concatenated weight.
@@ -583,7 +612,11 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
   a.paired = causal && !doc && n_kt % 2 == 0;
   a.dstart = doc ? dstart : nullptr;
   a.qt_end = doc ? qt_end : nullptr;
-  if (doc)
+  a.slopes = slopes;
+  if (slopes)
+    rc = D == 64 ? launch_bwd<64, true, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+                 : launch_bwd<128, true, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
+  else if (doc)
     rc = D == 64 ? launch_bwd<64, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
                  : launch_bwd<128, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
   else
@@ -629,6 +662,17 @@ int attn_bwd_window(const void* q, const void* k, const void* v, const void* o, 
   B200_CHECK_ARG(window >= 0, "attn_bwd_window: window=%d must be >= 0", window);
   return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
                        ws, ws_bytes, stream);
+}
+
+// ALiBi backward: attn_bwd_window (window < 0: none) with the forward's bias slopes[h] * (k - s).  Same workspace.
+int attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                   const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S, int H,
+                   int Hk, int D, float scale, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_bwd_alibi: pos must be 4-byte aligned int32");
+  B200_CHECK_ARG(slopes != nullptr && (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
+                 "attn_bwd_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
+  return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
+                       ws, ws_bytes, stream, slopes);
 }
 
 }  // namespace b200

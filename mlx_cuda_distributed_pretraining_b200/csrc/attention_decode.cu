@@ -25,6 +25,12 @@
 // live chunk starts at the 32-key tile holding kv0 and masks the keys below it, and the combine merges the live chunks
 // only.  A row's result still depends on lens[b] and W alone.  Without a window W = s_max, so kv0 = 0 and the
 // arithmetic is the unwindowed kernel's.
+//
+// ALiBi (attn_decode_alibi, ALIBI = true): the query at position len - 1 adds m_h log2e (k - (len - 1)) to the score
+// of key k, with query head h's slope m_h = slopes[h].  The slopes (times log2e) of the CTA's G heads are read once
+// into the reduction buffer, which is free until the key subsets merge.  Per tile each lane converts its key's distance
+// start + lane - (len - 1) once for all G heads, and the online-softmax step adds slope * distance to the score; keys
+// below the tile start or the window stay -inf.  With zero slopes the scores are the window kernel's.
 #include "common.cuh"
 #include "host.h"
 
@@ -89,13 +95,16 @@ struct DecArgs {
   int H, G, s_max, max_chunks;
   float scale_log2;   // scale * log2 e
   int window;         // keys len - 1 - window .. len - 1 are visible; s_max without a window
+  const float* slopes;  // ALIBI: [H] fp32 per-query-head slopes
 };
 
 // kv0: the first cached key the row's query sees
 __device__ __forceinline__ int first_visible_key(const DecArgs& p, int len) { return max(0, len - 1 - p.window); }
 
-template <typename T, int D>
-__global__ void __launch_bounds__(DEC_THREADS)
+// ALIBI: at least 4 CTAs per SM (<= 128 registers); left to itself ptxas keeps the ALiBi kernels at 64 registers and
+// spills the bf16 D = 32 / 128 ones.  ALIBI = false keeps the plain bound (0 = none).
+template <typename T, int D, bool ALIBI = false>
+__global__ void __launch_bounds__(DEC_THREADS, ALIBI ? 4 : 0)
 attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const DecArgs p) {
   constexpr int L = D / 8;                        // 8-column slices per row
   constexpr int TILE_ELEMS = DEC_TILE * D;
@@ -154,6 +163,7 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   for (int g = tid; g < G; g += DEC_THREADS) {
     sm[g] = -INFINITY;
     sl[g] = 0.f;
+    if constexpr (ALIBI) sred[g] = __ldg(p.slopes + hk * G + g) * kLog2e;  // G <= DEC_THREADS * 8
   }
 
   // accumulator ownership: item = (head g, slice) with g = item / L; keys my_ks, my_ks + ks_n, ... of every tile
@@ -212,9 +222,12 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     __syncthreads();
 
     // online softmax (log2 domain): one warp per head, one lane per key; every tile holds at least one valid key
-    // (kv0 < end, and kv0 lies in the first tile)
+    // (kv0 < end, and kv0 lies in the first tile).  ALIBI: kd = this lane's key distance, converted once per tile
+    float kd = 0.f;
+    if constexpr (ALIBI) kd = (float)(start + lane - (len - 1));
     for (int g = warp; g < G; g += DEC_THREADS / 32) {
-      const float x = ss[g * DEC_TILE + lane];
+      float x = ss[g * DEC_TILE + lane];
+      if constexpr (ALIBI) x = x + sred[g] * kd;
       const float m_old = sm[g];
       const float m_new = fmaxf(m_old, warp_max(x));
       const float pe = exp2f(x - m_new);
@@ -319,10 +332,10 @@ attn_decode_combine_kernel(const DecArgs p) {
   if (p.lse != nullptr && d == 0) p.lse[bh] = (M + log2f(l)) / kLog2e;
 }
 
-template <typename T, int D>
+template <typename T, int D, bool ALIBI = false>
 int launch_decode(const CUtensorMap& tmK, const CUtensorMap& tmV, const DecArgs& a, int B, int Hk,
                   cudaStream_t stream) {
-  auto kern = attn_decode_kernel<T, D>;
+  auto kern = attn_decode_kernel<T, D, ALIBI>;
   const DecSmem lay(D, (int)sizeof(T), a.G);
   static int attr_bytes = 0;
   if (lay.total > 48 * 1024 && lay.total > attr_bytes) {
@@ -338,14 +351,14 @@ int launch_decode(const CUtensorMap& tmK, const CUtensorMap& tmV, const DecArgs&
   return B200_OK;
 }
 
-template <typename T>
+template <typename T, bool ALIBI = false>
 int launch_decode_d(int D, const CUtensorMap& tmK, const CUtensorMap& tmV, const DecArgs& a, int B, int Hk,
                     cudaStream_t stream) {
   switch (D) {
-    case 16: return launch_decode<T, 16>(tmK, tmV, a, B, Hk, stream);
-    case 32: return launch_decode<T, 32>(tmK, tmV, a, B, Hk, stream);
-    case 64: return launch_decode<T, 64>(tmK, tmV, a, B, Hk, stream);
-    default: return launch_decode<T, 128>(tmK, tmV, a, B, Hk, stream);
+    case 16: return launch_decode<T, 16, ALIBI>(tmK, tmV, a, B, Hk, stream);
+    case 32: return launch_decode<T, 32, ALIBI>(tmK, tmV, a, B, Hk, stream);
+    case 64: return launch_decode<T, 64, ALIBI>(tmK, tmV, a, B, Hk, stream);
+    default: return launch_decode<T, 128, ALIBI>(tmK, tmV, a, B, Hk, stream);
   }
 }
 
@@ -456,9 +469,10 @@ size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D) {
 
 namespace {
 
+// window < 0 means none; slopes selects ALiBi
 int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                      int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
-                     size_t ws_bytes, cudaStream_t stream) {
+                     size_t ws_bytes, cudaStream_t stream, const float* slopes = nullptr) {
   B200_CHECK_ARG(B > 0 && H > 0 && Hk > 0 && H % Hk == 0, "attn_decode: bad shape B=%d H=%d Hk=%d", B, H, Hk);
   B200_CHECK_ARG(D == 16 || D == 32 || D == 64 || D == 128, "attn_decode: head_dim %d unsupported (16/32/64/128)", D);
   B200_CHECK_ARG(s_max >= DEC_TILE, "attn_decode: s_max=%d must be >= %d", s_max, DEC_TILE);
@@ -493,6 +507,10 @@ int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, co
   a.s_max = s_max;
   a.scale_log2 = scale * kLog2e;
   a.window = window < 0 || window > s_max ? s_max : window;
+  a.slopes = slopes;
+  if (slopes)
+    return is_bf16 ? launch_decode_d<__nv_bfloat16, true>(D, tmK, tmV, a, B, Hk, stream)
+                   : launch_decode_d<float, true>(D, tmK, tmV, a, B, Hk, stream);
   return is_bf16 ? launch_decode_d<__nv_bfloat16>(D, tmK, tmV, a, B, Hk, stream)
                  : launch_decode_d<float>(D, tmK, tmV, a, B, Hk, stream);
 }
@@ -513,6 +531,16 @@ int attn_decode_window(const void* q, const void* k_cache, const void* v_cache, 
   B200_CHECK_ARG(window >= 0, "attn_decode_window: window=%d must be >= 0", window);
   return attn_decode_impl(q, k_cache, v_cache, lens, o, lse, window, B, s_max, H, Hk, D, scale, is_bf16, ws,
                           ws_bytes, stream);
+}
+
+// ALiBi: attn_decode_window (window < 0: none) with the bias slopes[h] * (k - (lens[b] - 1)) on every cached key k
+int attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
+                      int window, const float* slopes, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
+                      void* ws, size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG(slopes != nullptr && (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
+                 "attn_decode_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
+  return attn_decode_impl(q, k_cache, v_cache, lens, o, lse, window, B, s_max, H, Hk, D, scale, is_bf16, ws,
+                          ws_bytes, stream, slopes);
 }
 
 int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,

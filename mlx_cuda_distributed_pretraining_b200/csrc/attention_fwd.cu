@@ -21,6 +21,14 @@
 // Sliding window (same DOC instantiation): query q sees keys q - min(pos[q], W) .. q, i.e. the document mask with pos
 // clamped at W, which keeps the starts monotone in q.  pos == nullptr reads as pos[q] = q (one document per row), so
 // an unpacked windowed launch needs no [B, S] buffer.  Without a window W = S, and min(pos[q], S) = pos[q].
+//
+// ALiBi (ALIBI = true, DOC kernels only): every score gets the bias m_h (k - q) <= 0 of the query head's slope
+// m_h = slopes[h], added to the scaled score before the mask and the softmax, on every tile.  In log2 units the bias is
+// b = m_h log2e (k - q).  A thread's keys in a tile are k0 + 2 (lane % 4) + c with the compile-time column c = 8 nc +
+// {0, 1}, so each tile converts one integer per row, base = m log2e (k0 + 2 (lane % 4) - row), and the element's bias
+// is fmaf(m log2e, c, base): no int -> float conversion per element (that pipe is the one exp2 already fills).  With
+// m = 0 the bias is exactly 0 and the scores are the DOC kernel's.  k - q is also the distance within a document, so
+// packed rows need nothing more.  ALIBI = false compiles to the kernels above unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -53,6 +61,7 @@ struct FwdArgs {
   int causal;
   const int* pos;  // [B, S] positions within documents (DOC kernels only; null: pos[q] = q)
   int window;      // DOC: query q sees keys from q - min(pos[q], window); S when there is no window
+  const float* slopes;  // ALIBI: [H] fp32 per-query-head slopes
 };
 
 // first key query `row` of batch row b may see: its document start, or its window start when that is later
@@ -68,7 +77,7 @@ __device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db)
   else wgmma_m64n64k16_rs<1>(o, a, db);
 }
 
-template <int D, bool DOC>
+template <int D, bool DOC, bool ALIBI = false>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdArgs p) {
@@ -137,6 +146,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       dstart[r] = row < p.S ? key_start(p, b, row) : 0;
     }
   }
+  float ml2 = 0.f;  // ALIBI: this head's slope in log2 units
+  if constexpr (ALIBI) ml2 = __ldg(p.slopes + h) * kLog2e;
   mbar_wait(q_full, 0);
 
   for (int j = j0; j < n_kv; ++j) {
@@ -174,16 +185,41 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
     // scale (log2 domain), mask, online softmax; accumulator chunk nc holds keys 8 nc + 2 (lane % 4) + {0, 1}
     float mx[2] = {-INFINITY, -INFINITY};
+    if constexpr (ALIBI) {
+      // keys k0 + 2 (lane % 4) + c with the compile-time column c = 8 nc + (e & 1): row r sees c <= c_hi[r] (causal,
+      // in bounds), and its bias is fmaf(m log2e, c, abase[r]) with abase[r] = m log2e (k0 + 2 (lane % 4) - row)
+      const int k_lane = k0 + (lane & 3) * 2;
+      int c_hi[2];
+      float abase[2];
 #pragma unroll
-    for (int nc = 0; nc < 16; ++nc) {
+      for (int r = 0; r < 2; ++r) {
+        const int row = row_a + 8 * r;
+        c_hi[r] = min(row, p.S - 1) - k_lane;
+        abase[r] = ml2 * (float)(k_lane - row);
+      }
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
-        const int row = row_a + ((e >> 1) << 3);
-        float x = sc[4 * nc + e] * sl2;
-        if (key >= p.S || (p.causal && key > row)) x = -INFINITY;
-        sc[4 * nc + e] = x;
-        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int c = nc * 8 + (e & 1);
+          float x = sc[4 * nc + e] * sl2 + fmaf(ml2, (float)c, abase[e >> 1]);
+          if (c > c_hi[e >> 1]) x = -INFINITY;
+          sc[4 * nc + e] = x;
+          mx[e >> 1] = fmaxf(mx[e >> 1], x);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
+          const int row = row_a + ((e >> 1) << 3);
+          float x = sc[4 * nc + e] * sl2;
+          if (key >= p.S || (p.causal && key > row)) x = -INFINITY;
+          sc[4 * nc + e] = x;
+          mx[e >> 1] = fmaxf(mx[e >> 1], x);
+        }
       }
     }
     float alpha[2], m_use[2];
@@ -254,11 +290,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-template <int D, bool DOC>
+template <int D, bool DOC, bool ALIBI = false>
 int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
                cudaStream_t stream) {
   using Cfg = FwdCfg<D>;
-  auto kern = attn_fwd_kernel<D, DOC>;
+  auto kern = attn_fwd_kernel<D, DOC, ALIBI>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -282,9 +318,10 @@ int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, in
 
 namespace {
 
-// doc selects the document / window instantiation; window < 0 means none
+// doc selects the document / window instantiation; window < 0 means none; slopes (doc only) selects ALiBi
 int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, bool doc, const int* pos,
-                  int window, int B, int S, int H, int Hk, int D, float scale, int causal, cudaStream_t stream) {
+                  int window, int B, int S, int H, int Hk, int D, float scale, int causal, cudaStream_t stream,
+                  const float* slopes = nullptr) {
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_fwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd: head_dim %d unsupported (64 or 128; pad smaller dims)", D);
@@ -305,6 +342,10 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   a.causal = causal;
   a.pos = pos;
   a.window = window < 0 || window > S ? S : window;
+  a.slopes = slopes;
+  if (slopes)
+    return D == 64 ? launch_fwd<64, true, true>(tmQ, tmK, tmV, a, stream)
+                   : launch_fwd<128, true, true>(tmQ, tmK, tmV, a, stream);
   if (doc) return D == 64 ? launch_fwd<64, true>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, true>(tmQ, tmK, tmV, a, stream);
   return D == 64 ? launch_fwd<64, false>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, false>(tmQ, tmK, tmV, a, stream);
 }
@@ -330,6 +371,15 @@ int attn_fwd_window(const void* q, const void* k, const void* v, void* o, float*
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_fwd_window: pos must be 4-byte aligned int32");
   B200_CHECK_ARG(window >= 0, "attn_fwd_window: window=%d must be >= 0", window);
   return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, stream);
+}
+
+// ALiBi: attn_fwd_window (window < 0: none) with the bias slopes[h] * (k - s) added to every visible score
+int attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                   const float* slopes, int B, int S, int H, int Hk, int D, float scale, cudaStream_t stream) {
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_fwd_alibi: pos must be 4-byte aligned int32");
+  B200_CHECK_ARG(slopes != nullptr && (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
+                 "attn_fwd_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
+  return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, stream, slopes);
 }
 
 }  // namespace b200

@@ -123,7 +123,15 @@ int attn_fwd_window(const void* q, const void* k, const void* v, void* o, float*
 int attn_bwd_window(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                     const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
                     float scale, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
+int attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                   const float* slopes, int B, int S, int H, int Hk, int D, float scale, cudaStream_t stream);
+int attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                   const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S, int H,
+                   int Hk, int D, float scale, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D);
+int attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
+                      int window, const float* slopes, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
+                      void* ws, size_t ws_bytes, cudaStream_t stream);
 int attn_decode_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                        int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
                        size_t ws_bytes, cudaStream_t stream);
@@ -450,6 +458,18 @@ int b200_attn_bwd_window(const void* q, const void* k, const void* v, const void
                                workspace, workspace_bytes, S_(stream));
 }
 
+int b200_attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                        const float* slopes, int B, int S, int H, int Hk, int D, float scale, void* stream) {
+  return b200::attn_fwd_alibi(q, k, v, o, lse, pos, window, slopes, B, S, H, Hk, D, scale, S_(stream));
+}
+int b200_attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                        const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                        int H, int Hk, int D, float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes,
+                        void* stream) {
+  return b200::attn_bwd_alibi(q, k, v, o, d_o, lse, pos, window, slopes, dq, dk, dv, B, S, H, Hk, D, scale,
+                              dkv_row_heads, workspace, workspace_bytes, S_(stream));
+}
+
 size_t b200_attn_decode_workspace_bytes(int B, int H, int s_max, int D) {
   return b200::attn_decode_workspace_bytes(B, H, s_max, D);
 }
@@ -464,6 +484,12 @@ int b200_attn_decode_window(const void* q, const void* k_cache, const void* v_ca
                             void* workspace, size_t workspace_bytes, void* stream) {
   return b200::attn_decode_window(q, k_cache, v_cache, lens, o, lse, window, B, s_max, H, Hk, D, scale, is_bf16,
                                   workspace, workspace_bytes, S_(stream));
+}
+int b200_attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o,
+                           float* lse, int window, const float* slopes, int B, int s_max, int H, int Hk, int D,
+                           float scale, int is_bf16, void* workspace, size_t workspace_bytes, void* stream) {
+  return b200::attn_decode_alibi(q, k_cache, v_cache, lens, o, lse, window, slopes, B, s_max, H, Hk, D, scale,
+                                 is_bf16, workspace, workspace_bytes, S_(stream));
 }
 int b200_kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
                    const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,

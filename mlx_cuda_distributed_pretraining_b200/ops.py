@@ -681,11 +681,26 @@ def _check_window(window, what: str) -> int:
     return window
 
 
+def _check_alibi(alibi: torch.Tensor, q: torch.Tensor, causal: bool, what: str) -> torch.Tensor:
+    """ALiBi slopes: a contiguous fp32 [H] tensor on q's device (q: [B, S, H, D] or [B, H, D]), causal attention only.
+    The values are not checked: that would read the device."""
+    if not causal:
+        raise ValueError(f"{what}: ALiBi is defined for causal attention only (causal=False given)")
+    H = q.shape[-2]
+    if not isinstance(alibi, torch.Tensor) or alibi.dtype != torch.float32 or tuple(alibi.shape) != (H,):
+        raise ValueError(f"{what}: alibi must be an fp32 [H] = [{H}] tensor of slopes, got "
+                         f"{getattr(alibi, 'dtype', type(alibi))} {list(getattr(alibi, 'shape', []))}")
+    if alibi.device != q.device or not alibi.is_contiguous():
+        raise ValueError(f"{what}: alibi must be contiguous and on {q.device}, got {alibi.device}")
+    return alibi
+
+
 def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
-                      window: Optional[int] = None):
+                      window: Optional[int] = None, alibi: Optional[torch.Tensor] = None):
     """q [B,S,H,D], k/v [B,S,Hk,D] bf16 contiguous, D in {64,128}. Returns (o, lse[B,H,S]).  With pos (int32 [B,S]
     contiguous, positions within documents) the mask is document-causal and `causal` is ignored.  With window (an
-    int >= 0) query s sees keys s - min(pos[s], window) .. s (pos[s] = s without pos), and `causal` is ignored."""
+    int >= 0) query s sees keys s - min(pos[s], window) .. s (pos[s] = s without pos), and `causal` is ignored.
+    With alibi (fp32 [H] slopes, checked by the caller) the causal / document / window mask gets the ALiBi bias."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         _need(t, torch.bfloat16, nm)
     B, S, H, D = q.shape
@@ -693,7 +708,11 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
     o = torch.empty_like(q)
     lse = torch.empty((B, H, S), device=q.device, dtype=torch.float32)
     tok = _t0("attn_fwd")
-    if window is not None:
+    if alibi is not None:
+        check(lib().b200_attn_fwd_alibi(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+                                        _ptr(pos), -1 if window is None else min(int(window), S), alibi.data_ptr(),
+                                        B, S, H, Hk, D, float(scale), _stream()), "b200_attn_fwd_alibi")
+    elif window is not None:
         check(lib().b200_attn_fwd_window(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
                                          _ptr(pos), min(int(window), S), B, S, H, Hk, D, float(scale), _stream()),
               "b200_attn_fwd_window")
@@ -708,7 +727,7 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
 
 
 def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
-                      window: Optional[int] = None):
+                      window: Optional[int] = None, alibi: Optional[torch.Tensor] = None):
     B, S, H, D = q.shape
     Hk = k.shape[2]
     dq = torch.empty_like(q)
@@ -717,7 +736,15 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
     dkv = torch.empty((B, S, 2 * Hk, D), device=k.device, dtype=k.dtype)
     dk, dv = dkv[:, :, :Hk], dkv[:, :, Hk:]
     tok = _t0("attn_bwd")
-    if window is not None:
+    if alibi is not None:
+        nbytes = int(lib().b200_attn_bwd_window_workspace_bytes(B, S, H, Hk, D))
+        ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
+        check(lib().b200_attn_bwd_alibi(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                        lse.data_ptr(), _ptr(pos), -1 if window is None else min(int(window), S),
+                                        alibi.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H, Hk, D,
+                                        float(scale), 2 * Hk, ws.data_ptr(), ws.numel(), _stream()),
+              "b200_attn_bwd_alibi")
+    elif window is not None:
         nbytes = int(lib().b200_attn_bwd_window_workspace_bytes(B, S, H, Hk, D))
         ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
         check(lib().b200_attn_bwd_window(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
@@ -744,28 +771,28 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos, window):
+    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None):
         D = q.shape[-1]
         Dp = _pad_head_dim(D)
         if Dp != D:  # zero-padding the head dim leaves QK^T and the first D columns of PV unchanged
             q, k, v = (torch.nn.functional.pad(t, (0, Dp - D)) for t in (q, k, v))
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos, window)
-        ctx.save_for_backward(q, k, v, o, lse, pos)
+        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos, window, alibi)
+        ctx.save_for_backward(q, k, v, o, lse, pos, alibi)
         ctx.scale, ctx.causal, ctx.D, ctx.window = scale, causal, D, window
         return o[..., :D] if Dp != D else o
 
     @staticmethod
     def backward(ctx, do):
-        q, k, v, o, lse, pos = ctx.saved_tensors
+        q, k, v, o, lse, pos, alibi = ctx.saved_tensors
         Dp = q.shape[-1]
         if Dp != ctx.D:
             do = torch.nn.functional.pad(do, (0, Dp - ctx.D))
         do = do.contiguous()
-        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos, ctx.window)
+        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos, ctx.window, alibi)
         if Dp != ctx.D:
             dq, dk, dv = dq[..., :ctx.D], dk[..., :ctx.D], dv[..., :ctx.D]
-        return dq, dk, dv, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None
 
 
 def _hi_lo(x: torch.Tensor):
@@ -787,7 +814,7 @@ class _AttentionX3Fn(torch.autograd.Function):
     to fp32-like accuracy; P and the kernel outputs still pass through one bf16 rounding each."""
 
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos, window):
+    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None):
         D = q.shape[-1]
         Dp = _pad_head_dim(3 * D)
         (qh, ql), (kh, kl), (vh, vl) = _hi_lo(q), _hi_lo(k), _hi_lo(v)
@@ -796,30 +823,31 @@ class _AttentionX3Fn(torch.autograd.Function):
             t = torch.cat([a, b, c], dim=-1)
             return (torch.nn.functional.pad(t, (0, Dp - 3 * D)) if Dp != 3 * D else t).contiguous()
         q3, k3, v3 = cat3(qh, ql, qh), cat3(kh, kh, kl), cat3(vh, vh, vl)
-        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos, window)
-        ctx.save_for_backward(q3, k3, v3, o3, lse, pos)
+        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos, window, alibi)
+        ctx.save_for_backward(q3, k3, v3, o3, lse, pos, alibi)
         ctx.scale, ctx.causal, ctx.D, ctx.Dp, ctx.window = scale, causal, D, Dp, window
         return o3[..., :D].float() + o3[..., 2 * D:3 * D].float()
 
     @staticmethod
     def backward(ctx, do):
-        q3, k3, v3, o3, lse, pos = ctx.saved_tensors
+        q3, k3, v3, o3, lse, pos, alibi = ctx.saved_tensors
         D, Dp = ctx.D, ctx.Dp
         gh, gl = _hi_lo(do.float())
         g3 = torch.cat([gh, gl, gh], dim=-1)
         if Dp != 3 * D:
             g3 = torch.nn.functional.pad(g3, (0, Dp - 3 * D))
         dq3, dk3, dv3 = attention_bwd_raw(q3, k3, v3, o3, g3.contiguous(), lse, ctx.scale, ctx.causal, pos,
-                                          ctx.window)
+                                          ctx.window, alibi)
         dq = dq3[..., :D].float() + dq3[..., 2 * D:3 * D].float()
         dk = dk3[..., :D].float() + dk3[..., D:2 * D].float()
         dv = dv3[..., :D].float() + dv3[..., D:2 * D].float()
-        return dq, dk, dv, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None
 
 
 def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
-                   causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None) -> torch.Tensor:
-    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos, window: as
+                   causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None,
+                   alibi: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos, window, alibi: as
     attention."""
     if 3 * q.shape[-1] > 128:
         raise ValueError("attention_fp32: head_dim must be <= 42 (three bf16 copies must fit a 128-wide tile)")
@@ -829,11 +857,14 @@ def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Opt
         pos, causal = _check_pos(pos, q, "attention_fp32"), True
     if window is not None:
         window, causal = _check_window(window, "attention_fp32"), True
-    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos, window)
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, causal, "attention_fp32")
+    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos, window, alibi)
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
-              causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None) -> torch.Tensor:
+              causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None,
+              alibi: Optional[torch.Tensor] = None) -> torch.Tensor:
     """softmax(q k^T * scale + causal_mask) v with GQA head sharing; [B,S,H,D] layout, bf16.
 
     pos (int32 [B, S]) packs several documents per row: pos[b, s] is token s's position within its document (0 at a
@@ -842,14 +873,20 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional
 
     window (int >= 0) is a sliding causal window: query s sees key k iff 0 <= s - k <= window, at most window + 1
     keys, intersected with the document when pos is given (keys s - min(pos[b, s], window) .. s).  Tiles outside
-    every row's window are skipped, so the cost is linear in S.  It implies causal."""
+    every row's window are skipped, so the cost is linear in S.  It implies causal.
+
+    alibi (fp32 [H] slopes on q's device, one per query head; see arch.flash_attention.alibi_slopes) adds ALiBi's
+    bias alibi[h] * (k - s) to the scaled score of query s and key k before the mask and the softmax.  k - s is also
+    the distance inside a document, so it composes with pos and window.  Causal only: causal=False raises."""
     if scale is None:
         scale = q.shape[-1] ** -0.5
     if pos is not None:
         pos, causal = _check_pos(pos, q, "attention"), True
     if window is not None:
         window, causal = _check_window(window, "attention"), True
-    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos, window)
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, causal, "attention")
+    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos, window, alibi)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -878,19 +915,22 @@ def _check_cache(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, 
 
 def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
                      scale: Optional[float] = None, workspace: Optional[torch.Tensor] = None,
-                     return_lse: bool = False, window: Optional[int] = None):
+                     return_lse: bool = False, window: Optional[int] = None, alibi: Optional[torch.Tensor] = None):
     """softmax(q K^T * scale) V for one new query per row over its first lens[b] cached keys (b200_attn_decode).
 
     q [B,H,D]; k_cache, v_cache [B,s_max,Hk,D]; all bf16 or all fp32, D in {16, 32, 64, 128}; lens int32 [B] on the
     device, 1 <= lens[b] <= s_max (not checked here: that would read the device).  `workspace` (uint8, at least
     attention_decode_workspace_bytes(B, H, s_max, D)) is allocated when not given.  Returns o [B,H,D] in q's dtype,
     and the natural-log LSE [B,H] fp32 with return_lse.  window (int >= 0): the query at position p = lens[b] - 1
-    sees only keys max(0, p - window) .. p (b200_attn_decode_window), and only those are read."""
+    sees only keys max(0, p - window) .. p (b200_attn_decode_window), and only those are read.  alibi (fp32 [H]
+    slopes on the device): ALiBi's bias alibi[h] * (k - p) on every cached key k (b200_attn_decode_alibi)."""
     B, H, D, s_max, Hk = _check_cache(q, k_cache, v_cache, lens, "attention_decode")
     if D not in (16, 32, 64, 128):
         raise ValueError(f"attention_decode: head_dim {D} unsupported (16, 32, 64 or 128)")
     if window is not None:
         window = _check_window(window, "attention_decode")
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, True, "attention_decode")
     if scale is None:
         scale = D ** -0.5
     need = attention_decode_workspace_bytes(B, H, s_max, D)
@@ -901,7 +941,13 @@ def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     o = torch.empty_like(q)
     lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_decode")
-    if window is None:
+    if alibi is not None:
+        check(lib().b200_attn_decode_alibi(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr(),
+                                           o.data_ptr(), _ptr(lse), -1 if window is None else min(int(window), s_max),
+                                           alibi.data_ptr(), B, s_max, H, Hk, D, float(scale), _is_bf16(q, "q"),
+                                           workspace.data_ptr(), workspace.numel(), _stream()),
+              "b200_attn_decode_alibi")
+    elif window is None:
         check(lib().b200_attn_decode(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), lens.data_ptr(),
                                      o.data_ptr(), _ptr(lse), B, s_max, H, Hk, D, float(scale), _is_bf16(q, "q"),
                                      workspace.data_ptr(), workspace.numel(), _stream()), "b200_attn_decode")
