@@ -159,3 +159,193 @@ def test_accepts_fp32_rounding_of_a_cancelling_dp():
     eps = 2.0 ** -24 * (do.double().abs() * vq.abs()).sum(-1, keepdim=True)      # [B, S, H, 1]
     dq = ref["dq"][0] + SCALE * eps * k.double().repeat_interleave(H // Hk, 2)
     assert ac.check("dq", dq, *ref["dq"]) < 0.1
+
+
+# ---- ALiBi (b200_attn_bwd_alibi): O and LSE from the biased fp64 forward --------------------------------------------
+SLOPES = {"steep": 0.5, "gentle": 1 / 256}
+HA, HkA = 8, 2
+
+
+def _alibi(kind):
+    if kind == "mixed":
+        return torch.tensor([(0.0, 1 / 256, 0.5)[h % 3] for h in range(HA)], dtype=torch.float32)
+    return torch.full((HA,), SLOPES[kind], dtype=torch.float32)
+
+
+@pytest.fixture(scope="module")
+def alibi_inputs():
+    torch.manual_seed(31)
+    q = torch.randn(B, S, HA, D).to(torch.bfloat16)
+    k = torch.randn(B, S, HkA, D).to(torch.bfloat16)
+    v = torch.randn(B, S, HkA, D).to(torch.bfloat16)
+    do = torch.randn(B, S, HA, D).to(torch.bfloat16)
+    return q, k, v, do
+
+
+def _alibi_case(t, kind):
+    q, k, v, do = t
+    sl = _alibi(kind)
+    o, lse = ac.forward64(q, k, v, SCALE, True, slopes=sl)
+    return (q, k, v, o, do, lse), sl
+
+
+@pytest.mark.parametrize("kind", ["steep", "gentle", "mixed"])
+def test_alibi_accepts_rounded_reference_and_chunks_agree(alibi_inputs, kind):
+    t, sl = _alibi_case(alibi_inputs, kind)
+    ref = ac.reference(*t, SCALE, True, slopes=sl)
+    chunked = ac.reference(*t, SCALE, True, slopes=sl, head_chunk=4)
+    for name in ("dq", "dk", "dv"):
+        r, bd = ref[name]
+        assert ac.check(name, _bf16(r), r, bd) <= 1.0
+        assert torch.allclose(chunked[name][0], r, rtol=1e-12, atol=1e-14)
+        assert torch.allclose(chunked[name][1], bd, rtol=1e-12, atol=1e-20)
+
+
+def _p_bias(sl, fault):
+    """The bias the faulty kernel would put into P: unmasked: missing on the items that skip the mask (the 64-key
+    warpgroup's last key at or before the item's first query); key_base: keys 8..15 of every 16 with the base of the
+    key 8 before (b - 8 m)."""
+    pos = torch.arange(S)
+
+    def f(h0, h1):
+        from tests.attn_fwd_check import alibi_bias
+        b = alibi_bias(sl, S, h0, h1)
+        if fault == "unmasked":
+            unmasked = (pos // 64 * 64 + 63)[None, :] <= (pos // 64 * 64)[:, None]   # [query, key]
+            b = b.masked_fill(unmasked[None], 0.0)
+        elif fault == "key_base":
+            b = b - 8 * sl[h0:h1].double()[:, None, None] * ((pos % 16) >= 8)[None, None, :]
+        return b
+    return f
+
+
+@pytest.mark.parametrize("fault", ["unmasked", "key_base"])
+def test_alibi_rejects_bias_fault(alibi_inputs, fault):
+    """Gentle slope (1/256).  Records that the relative Frobenius check of tests/test_gpu_alibi.py (< 1e-2) also
+    notices both at this shape (errors 0.23-0.28 and 0.017-0.019): here the element check adds the named element."""
+    t, sl = _alibi_case(alibi_inputs, "gentle")
+    ref = ac.reference(*t, SCALE, True, slopes=sl)
+    bad = ac.reference(*t, SCALE, True, slopes=sl, bias=_p_bias(sl, fault))
+    frob = {}
+    for name in ("dq", "dk", "dv"):
+        _rejects(name, _bf16(bad[name][0]), ref)
+        r = ref[name][0]
+        frob[name] = float((bad[name][0] - r).norm() / r.norm())
+    passes = {n for n, e in frob.items() if e < 1e-2}
+    assert passes == set(), frob
+
+
+def test_alibi_rejects_group_first_slope(alibi_inputs):
+    """Every query head of a GQA group given the group's first head's slope (slopes[hk * group]), alibi_slopes(8)."""
+    from mlx_cuda_distributed_pretraining_b200.arch.flash_attention import alibi_slopes
+    from tests.attn_fwd_check import alibi_bias
+    q, k, v, do = alibi_inputs
+    sl = alibi_slopes(HA)
+    o, lse = ac.forward64(q, k, v, SCALE, True, slopes=sl)
+    ref = ac.reference(q, k, v, o, do, lse, SCALE, True, slopes=sl)
+    g = HA // HkA
+    wrong = sl[torch.arange(HA) // g * g]
+    bad = ac.reference(q, k, v, o, do, lse, SCALE, True, slopes=sl, bias=lambda h0, h1: alibi_bias(wrong, S, h0, h1))
+    for name in ("dq", "dk", "dv"):
+        _rejects(name, _bf16(bad[name][0]), ref)
+
+
+# ---- the bf16x3 backward (ops.attention_fp32) -----------------------------------------------------------------------
+D3 = 16
+
+
+def _x3_case(mul, seed, mask=None, slopes=None):
+    """fp32 inputs; the kernel's forward emulated in fp64 on the three-term operands: O' rounded to bf16 part by part,
+    LSE of Q'K'^T.  Returns fp32 (q, k, v, do), the x3 operands with O', LSE, and the fp32 o."""
+    torch.manual_seed(seed)
+    q = torch.randn(B, S, HA, D3) * mul
+    k = torch.randn(B, S, HkA, D3) * mul
+    v = torch.randn(B, S, HkA, D3)
+    do = torch.randn(B, S, HA, D3)
+    q3, k3, v3, g3 = ac.x3_operands(q, k, v, do)
+    o3, lse = ac.forward64(q3, k3, v3, D3 ** -0.5, True, mask=mask, slopes=slopes)
+    o = o3[..., :D3].float() + o3[..., 2 * D3:3 * D3].float()
+    return (q, k, v, do), (q3, k3, v3, o3, g3, lse), o
+
+
+def _x3_emulated(parts, mask=None, slopes=None):
+    """The kernel's three-term gradients: the bf16 reference on the x3 operands, each part rounded to bf16, summed in
+    fp32 as _AttentionX3Fn sums them."""
+    r = ac.reference(*parts, D3 ** -0.5, True, mask=mask, slopes=slopes)
+    dq3, dk3, dv3 = (_bf16(r[n][0]).float() for n in ("dq", "dk", "dv"))
+    return {"dq": dq3[..., :D3] + dq3[..., 2 * D3:3 * D3], "dk": dk3[..., :D3] + dk3[..., D3:2 * D3],
+            "dv": dv3[..., :D3] + dv3[..., D3:2 * D3]}, r
+
+
+@pytest.mark.parametrize("kind", ["plain", "alibi", "window0"])
+def test_x3_accepts_emulated_backward(kind):
+    from tests.attn_fwd_check import visible
+    mask = visible(S, window=0) if kind == "window0" else None
+    sl = _alibi("mixed") if kind == "alibi" else None
+    (q, k, v, do), parts, o = _x3_case(1.0, 41, mask, sl)
+    got, _ = _x3_emulated(parts, mask, sl)
+    ref = ac.reference(q, k, v, o, do, parts[5], D3 ** -0.5, True, mask=mask, slopes=sl, x3=True, kernel_d=64)
+    for name in ("dq", "dk", "dv"):
+        assert ac.check(name, got[name], *ref[name]) < 0.5
+
+
+def test_x3_bound_rejects_hi_only_logits_at_large_logits():
+    """|s| ~ 40: the plain bf16 backward (logits of the hi halves, bf16 inputs) misses by 2^-9 |s| in the exponent,
+    outside the x3 bound; the x3 emulation stays inside it."""
+    (q, k, v, do), parts, o = _x3_case(4.0, 42)
+    ref = ac.reference(q, k, v, o, do, parts[5], D3 ** -0.5, True, x3=True, kernel_d=64)
+    got, _ = _x3_emulated(parts)
+    for name in ("dq", "dk", "dv"):
+        assert ac.check(name, got[name], *ref[name]) <= 1.0
+    qh, kh, vh, gh = (t.to(torch.bfloat16) for t in (q, k, v, do))
+    oh, lh = ac.forward64(qh, kh, vh, D3 ** -0.5, True)
+    plain = ac.reference(qh, kh, vh, oh, gh, lh, D3 ** -0.5, True)
+    rejected = 0
+    for name in ("dq", "dk", "dv"):
+        try:
+            ac.check(name, _bf16(plain[name][0]), *ref[name])
+        except AssertionError:
+            rejected += 1
+    assert rejected >= 2
+
+
+@pytest.mark.parametrize("fault", ["dq_without_dS_kl", "dv_without_PT_gl", "delta_without_P_vl"])
+def test_x3_layout_faults_are_rejected_part_by_part(fault):
+    """Each fault drops one lo part.  Against the summed gradient it is at most 2^-9 of the bound's P / dS rounding
+    term (module docstring), so it is checked where it lives: the part's own bf16 reference on the x3 operands.
+    delta_without_P_vl (O' saved with its P vl third zeroed) shows where dP - delta cancels: window 0, dS = 0."""
+    from tests.attn_fwd_check import visible
+    mask = visible(S, window=0) if fault == "delta_without_P_vl" else None
+    _, parts, _ = _x3_case(1.0, 43, mask)
+    ref = ac.reference(*parts, D3 ** -0.5, True, mask=mask)
+    dq3, dk3, dv3 = (_bf16(ref[n][0]) for n in ("dq", "dk", "dv"))
+    if fault == "dq_without_dS_kl":
+        dq3[..., 2 * D3:3 * D3] = 0
+        _rejects("dq", dq3, ref)
+    elif fault == "dv_without_PT_gl":
+        dv3[..., D3:2 * D3] = 0
+        _rejects("dv", dv3, ref)
+    else:
+        q3, k3, v3, o3, g3, lse = parts
+        o3b = o3.clone()
+        o3b[..., 2 * D3:3 * D3] = 0
+        bad = ac.reference(q3, k3, v3, o3b, g3, lse, D3 ** -0.5, True, mask=mask)
+        _rejects("dq", _bf16(bad["dq"][0]), ref)
+        _rejects("dk", _bf16(bad["dk"][0]), ref)
+
+
+def test_alibi_reference_stays_finite_where_the_future_bias_overflows():
+    """m (k - q) on a masked future key reaches 0.5 * 1499 > 709, where exp overflows fp64: the reference masks
+    before exp, and check() fails a NaN reference instead of passing it."""
+    S_ = 1500
+    torch.manual_seed(44)
+    q, k, v, do = (torch.randn(1, S_, 1, D).to(torch.bfloat16) for _ in range(4))
+    sl = torch.full((1,), 0.5)
+    o, lse = ac.forward64(q, k, v, SCALE, True, slopes=sl)
+    ref = ac.reference(q, k, v, o, do, lse, SCALE, True, slopes=sl)
+    for name in ("dq", "dk", "dv"):
+        r, bd = ref[name]
+        assert torch.isfinite(r).all() and torch.isfinite(bd).all()
+        assert ac.check(name, _bf16(r), r, bd) <= 1.0
+        with pytest.raises(AssertionError):
+            ac.check(name, _bf16(r), r * float("nan"), bd)

@@ -216,3 +216,168 @@ def test_visible_matches_product_masks(S_):
         assert torch.equal(fc.visible(S_, pos=pos, window=W),
                            DocumentCausalMask(pos, W).dense(torch.float64)[:, 0] == 0), W
     assert fc.visible(S_, causal=False).all()
+
+
+# ---- ALiBi (b200_attn_fwd_alibi) ------------------------------------------------------------------------------------
+# one row, GQA group 4; faults go into the CTA (128-query tile QA, head HA).  Every fault below changes the bias only.
+SA, HA_, HkA, QA, HA = 1024, 8, 2, 6, 1
+QA0, QA1 = QA * 128, QA * 128 + 128
+SLOPES = {"steep": [0.5] * HA_, "gentle": [1 / 256] * HA_, "mixed": [(0.0, 1 / 256, 0.5)[h % 3] for h in range(HA_)],
+          "zero": [0.0] * HA_}
+
+
+def _slopes(kind):
+    return torch.tensor(SLOPES[kind], dtype=torch.float32)
+
+
+@pytest.fixture(scope="module")
+def alibi_case():
+    torch.manual_seed(21)
+    q = torch.randn(1, SA, HA_, D).to(torch.bfloat16)
+    k = torch.randn(1, SA, HkA, D).to(torch.bfloat16)
+    v = torch.randn(1, SA, HkA, D).to(torch.bfloat16)
+    return q, k, v
+
+
+def _alibi_ref(t, kind, mask=None):
+    return fc.reference(*t, SCALE, fc.visible(SA) if mask is None else mask, slopes=_slopes(kind))
+
+
+def _cta(ref, o_bad, lse_bad):
+    o, lse = ref["o"][0].clone(), ref["lse"][0].clone()
+    o[:, QA0:QA1, HA] = o_bad[:, QA0:QA1, HA]
+    lse[:, HA, QA0:QA1] = lse_bad[:, HA, QA0:QA1]
+    return o, lse
+
+
+def _verdict(ref, o, lse):
+    """(O rejected, LSE rejected, O's Frobenius error over the row < 1e-2, LSE's max abs error < 1e-3): the last two
+    are the kernel checks of tests/test_gpu_alibi.py."""
+    out = []
+    for name, got in (("o", o.to(torch.bfloat16)), ("lse", lse.float())):
+        try:
+            fc.check(name, got, *ref[name])
+            out.append(False)
+        except AssertionError:
+            out.append(True)
+    return (out[0], out[1], _frob(o, ref["o"][0]) < 1e-2,
+            float((lse.double() - ref["lse"][0]).abs().max()) < 1e-3)
+
+
+@pytest.mark.parametrize("kind", list(SLOPES))
+@pytest.mark.parametrize("layout", ["rows", "packed", "window"])
+def test_alibi_accepts_rounded_reference_and_kernel_emulation(alibi_case, kind, layout):
+    """The emulation forms the bias as the kernel does (fp32 m log2e, a per-row base, fmaf per column): it must sit
+    inside the bound with margin for steep, gentle, mixed and zero slopes, on plain, packed and windowed rows."""
+    mask = None
+    if layout == "packed":
+        mask = fc.visible(SA, pos=positions([100, 200, 129, 300, 295], SA)[None])[0]
+    elif layout == "window":
+        mask = fc.visible(SA, window=129)
+    ref = _alibi_ref(alibi_case, kind, mask)
+    r, bd = ref["o"]
+    assert fc.check("o", r.to(torch.bfloat16), r, bd) < 0.5
+    o, lse = fc.emulate_kernel(*alibi_case, SCALE, fc.visible(SA) if mask is None else mask, slopes=_slopes(kind))
+    assert fc.check("o", o, *ref["o"]) < 0.75
+    assert fc.check("lse", lse, *ref["lse"]) < 0.25
+
+
+def test_alibi_zero_slopes_are_the_causal_reference(alibi_case):
+    a, c = _alibi_ref(alibi_case, "zero"), fc.reference(*alibi_case, SCALE, fc.visible(SA))
+    for name in ("o", "lse"):
+        assert torch.equal(a[name][0], c[name][0]) and torch.equal(a[name][1], c[name][1])
+
+
+def _bias_fn(kind, fault):
+    sl = _slopes(kind)
+    pos = torch.arange(SA, dtype=torch.float64)
+
+    def f(h0, h1):
+        b = fc.alibi_bias(sl, SA, h0, h1)
+        m = sl[h0:h1].double()[:, None, None]
+        if fault == "interior":        # key tiles wholly below the CTA's first query get no bias
+            b[:, QA0:QA1, :QA0] = 0
+        elif fault == "odd_columns":   # c = 8 nc: the odd keys' bias one key short
+            b = b - m * (pos % 2)[None, None, :]
+        elif fault == "bf16":          # the log2-unit bias rounded through bf16 before the add
+            b = (b * fc.LOG2E).to(torch.bfloat16).double() / fc.LOG2E
+        elif fault == "scaled":        # the bias multiplied by the softmax scale
+            b = b * SCALE
+        elif fault == "row_half":      # rows + 8 of each 16 use the first half's base: b + 8 m
+            b = b + 8 * m * ((pos % 16) >= 8)[None, :, None]
+        elif fault == "uniform_shift":  # every distance off by one: b + m on every element
+            b = b + m
+        return b
+    return f
+
+
+# (fault, slopes, O rejected, LSE rejected, O's Frobenius check passes it, LSE's max-abs check passes it).  At this
+# shape the max-abs LSE check of tests/test_gpu_alibi.py notices every one of them (|dLSE| >= 2.3e-3); the Frobenius
+# check on O passes four, which only the element check of O or LSE sees.
+FAULTS = [("interior", "gentle", True, True, False, False),
+          ("odd_columns", "gentle", False, True, True, False),
+          ("odd_columns", "steep", True, True, False, False),
+          ("bf16", "steep", False, True, True, False),
+          ("scaled", "gentle", True, True, False, False),
+          ("row_half", "gentle", False, True, True, False),
+          ("row_half", "steep", False, True, True, False)]
+
+
+@pytest.mark.parametrize("fault,kind,o_rej,lse_rej,frob_passes,lse_abs_passes", FAULTS)
+def test_alibi_rejects_bias_fault_in_one_cta(alibi_case, fault, kind, o_rej, lse_rej, frob_passes, lse_abs_passes):
+    """One CTA's bias wrong; at least one of O and LSE rejects it.  interior: the key tiles wholly below the CTA's
+    first query without bias (a fast path that skips it); odd_columns: c = 8 nc, the e & 1 term dropped; bf16: the
+    log2-unit bias rounded through bf16; scaled: the bias times the softmax scale; row_half: rows 8..15 of every 16
+    with the first half's base, a row-uniform shift, so O cannot change and LSE moves by 8 m."""
+    ref = _alibi_ref(alibi_case, kind)
+    o, lse = _cta(ref, *fc.forward64(*alibi_case, SCALE, fc.visible(SA), bias=_bias_fn(kind, fault)))
+    assert _verdict(ref, o, lse) == (o_rej, lse_rej, frob_passes, lse_abs_passes)
+
+
+@pytest.mark.parametrize("first", [True, False], ids=["group_first", "next_head"])
+def test_alibi_rejects_neighbouring_head_slope(alibi_case, first):
+    """alibi_slopes(8) and every head of a GQA group given the group's first head's slope, or query head h + 1's."""
+    from mlx_cuda_distributed_pretraining_b200.arch.flash_attention import alibi_slopes
+    sl = alibi_slopes(HA_)
+    g = HA_ // HkA
+    idx = torch.arange(HA_) // g * g if first else torch.clamp(torch.arange(HA_) + 1, max=HA_ - 1)
+    ref = fc.reference(*alibi_case, SCALE, fc.visible(SA), slopes=sl)
+    o, lse = fc.forward64(*alibi_case, SCALE, fc.visible(SA), slopes=sl[idx])
+    h = 2 if first else 5    # a head whose slope the fault changes: 1/16 -> 1/4, 1/32 -> 1/64
+    o_h, lse_h = ref["o"][0].clone(), ref["lse"][0].clone()
+    o_h[..., h, :], lse_h[:, h] = o[0, :, h], lse[0, h]
+    assert _verdict(ref, o_h, lse_h)[:2] == (True, True)
+
+
+def test_alibi_uniform_shift_is_invisible_to_o_by_construction(alibi_case):
+    """A bias off by the same amount on every key of a row (distance off by one everywhere) leaves the softmax and O
+    unchanged: no checker of O can see it, and this is no gap in the bound.  LSE moves by exactly m, which its check
+    catches."""
+    for kind in ("steep", "gentle"):
+        ref = _alibi_ref(alibi_case, kind)
+        o, lse = fc.forward64(*alibi_case, SCALE, fc.visible(SA), bias=_bias_fn(kind, "uniform_shift"))
+        assert float((o[0] - ref["o"][0]).abs().max()) < 1e-12
+        assert _verdict(ref, o[0], lse[0])[:2] == (False, True), kind
+
+
+def test_alibi_bf16_bias_at_gentle_slopes_is_below_the_noise():
+    """Stated limit.  The bf16-rounded bias errs by up to 2^-9 |b| per key with pseudo-random sign; at slope 1/256
+    |b| stays near 1 where P has weight, so O and LSE move by less than P's own bf16 rounding.  Steep slopes (0.5) and
+    far-back heavy keys (the underflow regime) are where the fault shows, and the GPU suite runs both."""
+    torch.manual_seed(22)
+    q = torch.randn(1, SA, HA_, D).to(torch.bfloat16)
+    k = torch.randn(1, SA, HkA, D).to(torch.bfloat16)
+    v = torch.randn(1, SA, HkA, D).to(torch.bfloat16)
+    ref = _alibi_ref((q, k, v), "gentle")
+    o, lse = fc.forward64(q, k, v, SCALE, fc.visible(SA), bias=_bias_fn("gentle", "bf16"))
+    assert _verdict(ref, o[0], lse[0])[:2] == (False, False)
+    # far-back heavy keys: keys 0..127 dominate every later row, 700-900 positions back (test_fwd_logit_regimes)
+    q = torch.randn(1, SA, HA_, D) * 0.1
+    k = torch.randn(1, SA, HkA, D) * 0.1
+    q[..., 0] = 4.0
+    k[..., 0] = -60.0
+    k[:, :128, :, 0] = 30.0
+    t = (q.to(torch.bfloat16), k.to(torch.bfloat16), v)
+    ref = fc.reference(*t, 1.0, fc.visible(SA), slopes=_slopes("steep"))
+    o, lse = fc.forward64(*t, 1.0, fc.visible(SA), bias=_bias_fn("steep", "bf16"))
+    assert _verdict(ref, o[0], lse[0])[:2] == (True, True)

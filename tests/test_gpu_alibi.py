@@ -3,7 +3,9 @@ gets the bias m_h (k - q) of query head h's slope before the mask and the softma
 
 The fp64 reference and the tolerances are those of tests/test_gpu_sliding_window.py: o / dq / dk / dv relative
 Frobenius error < 1e-2, lse max abs error < 1e-3; model level bf16 loss 5e-3 / gradients 3e-2, fp32 (bf16x3
-attention) 1e-3 / 8e-3; decode the bound of tests/test_gpu_generation.py."""
+attention) 1e-3 / 8e-3; decode the bound of tests/test_gpu_generation.py.  The element-by-element checks of the
+kernels are in tests/test_gpu_attention_alibi_check.py; the Frobenius checks here stay as a cross-check through the
+autograd path (ops.attention / ops.attention_fp32 with padding and the saved tensors), which those tests bypass."""
 import tempfile
 from pathlib import Path
 
