@@ -397,6 +397,19 @@ int b200_attn_bwd_alibi(const void* q, const void* k, const void* v, const void*
                         const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
                         int H, int Hk, int D, float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes,
                         void* stream);
+/* Prefix-LM: causal attention in which each row's prefix attends bidirectionally within itself.  prefix: device
+ * int32 [B], 4-byte aligned and non-null; query s of row b sees key k iff k <= s or k < P_b, with P_b = prefix[b]
+ * clamped to [0, S] by the kernels (its values are not checked on the host, since that would read the device, and
+ * the clamp keeps any value from reaching past the row).  P_b <= 1 gives b200_attn_fwd / b200_attn_bwd_strided with
+ * causal=1 bit for bit (O, LSE, dK, dV); P_b = S is full non-causal attention.  The backward takes
+ * b200_attn_bwd_strided's dk / dv rows and a workspace of b200_attn_bwd_prefix_workspace_bytes (equal to
+ * b200_attn_bwd_workspace_bytes). */
+int b200_attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float* lse, const int* prefix, int B,
+                         int S, int H, int Hk, int D, float scale, void* stream);
+size_t b200_attn_bwd_prefix_workspace_bytes(int B, int S, int H, int Hk, int D);
+int b200_attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                         const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
+                         float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- generation: decode attention over a KV cache (arch/flash_attention.py:97-156, last query row) ------------
  * One new query per sequence against its cached keys, causal by construction (every cached key precedes it):

@@ -82,6 +82,28 @@ class DocumentCausalMask:
         return m[:, None]
 
 
+class PrefixCausalMask:
+    """Marker for the prefix-LM mask: prefix (int32 [B]) holds each row's prefix length P_b, and query q sees key k
+    iff k <= q or k < P_b -- the prefix attends bidirectionally within itself and every later token is causal over
+    everything before it.  P_b <= 1 is the causal mask and P_b = S full attention; the fused kernels clamp P_b to
+    [0, S], and dense() does the same."""
+
+    def __init__(self, prefix: torch.Tensor, seq_len: int):
+        if prefix.dim() != 1:
+            raise ValueError(f"PrefixCausalMask: prefix must be [B], got {list(prefix.shape)}")
+        self.prefix = prefix.to(torch.int32).contiguous()
+        self.seq_len = seq_len
+
+    def dense(self, dtype=torch.float32, device="cpu") -> torch.Tensor:
+        """The additive [B, 1, S, S] mask (0 where visible, -inf elsewhere)."""
+        P = self.prefix.to(device=device, dtype=torch.int64).clamp(0, self.seq_len)
+        s = torch.arange(self.seq_len, device=device)
+        q, k = s[:, None], s[None, :]
+        ok = (k <= q)[None] | (k[None] < P[:, None, None])
+        m = torch.zeros(ok.shape, dtype=dtype, device=device).masked_fill(~ok, float("-inf"))
+        return m[:, None]
+
+
 class FlashAttention(nn.Module):
     """alibi: add ALiBi's bias alibi_slopes(num_heads)[h] * (k - q) to every causal score (the slopes are not
     parameters: a device tensor made on first use, like rope_tables)."""
@@ -117,26 +139,30 @@ class FlashAttention(nn.Module):
 
     def _flash_attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask=None) -> torch.Tensor:
         """q [B,S,H,D], k/v [B,S,Hk,D] -> [B,S,H,D]."""
-        pos = window = None
+        pos = window = prefix = None
         if mask is None:
             causal = False
         elif isinstance(mask, CausalMask):
             causal, window = True, mask.window
         elif isinstance(mask, DocumentCausalMask):
             causal, pos, window = True, mask.pos, mask.window
+        elif isinstance(mask, PrefixCausalMask):
+            causal, prefix = True, mask.prefix
         else:
             raise NotImplementedError(
-                "the fused kernel supports mask=None, the causal mask (CausalMask) or the document-causal mask of "
-                "packed rows (DocumentCausalMask); arbitrary additive masks are outside the reference's training path")
+                "the fused kernel supports mask=None, the causal mask (CausalMask), the document-causal mask of "
+                "packed rows (DocumentCausalMask) or the prefix-LM mask (PrefixCausalMask); arbitrary additive masks "
+                "are outside the reference's training path")
         alibi = self.alibi_slopes(q.device)
         dt = q.dtype
         if dt == torch.float32 and 3 * self.head_dim <= 128:
             # full-precision configs (mixed_precision: false, e.g. BASELINE C1, head_dim 16): logits through
             # three-term bf16 products (hi/lo split operands), ~fp32-accurate scores on the same kernels
-            return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi)
+            return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi,
+                                      prefix=prefix)
         if dt != torch.bfloat16:  # larger head dims: bf16 operands with fp32 accumulation (stated in DESIGN.md)
             q, k, v = q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
-        o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi)
+        o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi, prefix=prefix)
         return o if dt == torch.bfloat16 else o.to(dt)
 
     def forward(self, x: torch.Tensor, mask=None, rope_layout: str = "interleaved") -> torch.Tensor:

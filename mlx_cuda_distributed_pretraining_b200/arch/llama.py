@@ -26,7 +26,7 @@ import torch
 from torch import nn
 
 from .. import ops
-from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention
+from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask
 
 VARIANTS = (None, "reference", "mlx_lm")
 
@@ -59,6 +59,7 @@ class ModelArgs:
     apply_rope: bool = False  # extension; see module docstring
     sliding_window: Optional[int] = None  # extension: query q sees keys q - W .. q in every layer (None: causal)
     alibi: bool = False  # extension: ALiBi's bias slope_h * (k - q) on every layer's attention scores
+    prefix_lm: bool = False  # extension: prefix-LM models (the prompt is the bidirectional prefix in prefill)
     variant: Optional[str] = None  # extension: None / "reference" (this block) or "mlx_lm" (module docstring)
     router_aux_loss_coef: float = 0.001  # with num_local_experts > 0: weight of the load-balancing loss
 
@@ -162,14 +163,16 @@ class AttentionModule(nn.Module):
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
         return self.attn(x, mask=mask, rope_layout=self.rope_layout)
 
-    def cached(self, x: torch.Tensor, cache: "KVCache", layer: int, window: Optional[int] = None) -> torch.Tensor:
+    def cached(self, x: torch.Tensor, cache: "KVCache", layer: int, window: Optional[int] = None,
+               prefix: Optional[torch.Tensor] = None) -> torch.Tensor:
         """This layer's attention against the KV cache: prefill when x is [B, S, hidden], one decode step when x is
-        [B, hidden].  window: the model's sliding window (None: causal)."""
+        [B, hidden].  window: the model's sliding window (None: causal).  prefix (int32 [B], prefill only): the
+        prefix-LM mask's prefix lengths."""
         if self.apply_rope and self.attn.rope_tables is None:
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
         if x.dim() == 3:
-            return self.attn.forward_prefill(x, CausalMask(x.shape[1], window), cache.k[layer], cache.v[layer],
-                                             self.rope_layout)
+            mask = CausalMask(x.shape[1], window) if prefix is None else PrefixCausalMask(prefix, x.shape[1])
+            return self.attn.forward_prefill(x, mask, cache.k[layer], cache.v[layer], self.rope_layout)
         return self.attn.forward_decode(x, cache.k[layer], cache.v[layer], cache.lens, cache.workspace, window,
                                         self.rope_layout)
 
@@ -225,14 +228,15 @@ class TransformerBlock(nn.Module):
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
         return h, self._ffn(y, token_mask, aux)
 
-    def forward_cached(self, h: torch.Tensor, pending, cache: "KVCache", layer: int, window: Optional[int] = None):
+    def forward_cached(self, h: torch.Tensor, pending, cache: "KVCache", layer: int, window: Optional[int] = None,
+                       prefix: Optional[torch.Tensor] = None):
         """forward_fused with the attention run against the KV cache (AttentionModule.cached)."""
         n1, n2 = self.input_layernorm, self.post_attention_layernorm
         if pending is None:
             y = n1(h)
         else:
             h, y = ops.add_rmsnorm(h, pending, n1.weight, n1.eps)
-        a = self.self_attn.cached(y, cache, layer, window)
+        a = self.self_attn.cached(y, cache, layer, window, prefix)
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
         return h, self._ffn(y)
 
@@ -282,14 +286,25 @@ class Model(nn.Module):
         self.lm_head = None if args.tie_word_embeddings else nn.Linear(args.hidden_size, args.vocab_size, bias=False)
 
     def hidden_states(self, inputs: torch.Tensor, position_ids=None, attention_mask=None,
-                      token_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+                      token_mask: Optional[torch.Tensor] = None,
+                      prefix_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
         """position_ids (int [B, S], optional): packed rows, each token's position within its document (0 at the
         document's first token).  It selects the document-causal mask and, with RoPE on, the rotation angles, so
         every document is computed as if it ran alone.  None keeps the causal mask over whole rows.  Both masks carry
         args.sliding_window.  token_mask (bool [B, S], optional; MoE models): the tokens the load-balancing loss
-        counts; given, every MoE layer keeps its partials for moe_aux_loss()."""
+        counts; given, every MoE layer keeps its partials for moe_aux_loss().  prefix_lens (int32 [B] on the device,
+        optional): prefix-LM rows, query q of row b sees key k iff k <= q or k < prefix_lens[b] (PrefixCausalMask);
+        it does not combine with position_ids or a sliding window."""
         B, S = inputs.shape
-        if attention_mask is not None:
+        if prefix_lens is not None:
+            if position_ids is not None or attention_mask is not None:
+                raise ValueError("prefix_lens does not combine with position_ids or attention_mask")
+            if self.args.sliding_window is not None or self.args.alibi:
+                raise ValueError("prefix_lens does not combine with a sliding window or ALiBi")
+            if tuple(prefix_lens.shape) != (B,):
+                raise ValueError(f"prefix_lens must be [B] = [{B}], got {list(prefix_lens.shape)}")
+            mask = PrefixCausalMask(prefix_lens, S)
+        elif attention_mask is not None:
             mask = attention_mask
         elif position_ids is not None:
             if tuple(position_ids.shape) != (B, S):
@@ -338,7 +353,7 @@ class Model(nn.Module):
             return self._tied_w
         return self.embed_tokens.weight
 
-    def padded_logits(self, inputs: torch.Tensor, position_ids=None, token_mask=None):
+    def padded_logits(self, inputs: torch.Tensor, position_ids=None, token_mask=None, prefix_lens=None):
         """(logits [B*S, ld], V) with ld >= V, ld % 8 == 0 when the fused cross-entropy can take them
         (bf16 weights, tied + row-padded embedding alias or an aligned vocabulary); else (None, V).
         Eligibility is decided BEFORE the forward pass, so an ineligible config (fp32, logit_scale,
@@ -348,12 +363,13 @@ class Model(nn.Module):
         w = self._logits_weight()
         if w.shape[0] % 8 != 0 or w.dtype != torch.bfloat16:
             return None, self.vocab_size
-        h = self.hidden_states(inputs, position_ids, token_mask=token_mask)
+        h = self.hidden_states(inputs, position_ids, token_mask=token_mask, prefix_lens=prefix_lens)
         logits = torch.nn.functional.linear(h, w)
         return logits.view(-1, logits.shape[-1]), self.vocab_size
 
-    def forward(self, inputs: torch.Tensor, position_ids=None, attention_mask=None, token_mask=None) -> torch.Tensor:
-        h = self.hidden_states(inputs, position_ids, attention_mask, token_mask)
+    def forward(self, inputs: torch.Tensor, position_ids=None, attention_mask=None, token_mask=None,
+                prefix_lens=None) -> torch.Tensor:
+        h = self.hidden_states(inputs, position_ids, attention_mask, token_mask, prefix_lens)
         logits = torch.nn.functional.linear(h, self._logits_weight())[..., :self.vocab_size]
         if self.logit_scale is not None:
             logits = logits * self.logit_scale
@@ -373,13 +389,18 @@ class Model(nn.Module):
         """Runs the right-padded prompts tokens [B, S] (row b valid in [0, lengths[b])) through the block stack as
         training does, fills cache positions [0, S) and sets the cache lengths.  Returns the fp32 logits [B, V] at
         each row's last prompt position only.  Padding is harmless: under the causal mask no valid position sees it,
-        and the decode steps never read cache positions at or past a row's length."""
+        and the decode steps never read cache positions at or past a row's length.  A prefix-LM model (args.prefix_lm)
+        runs the prompt as its prefix, P_b = lengths[b]: valid positions see the whole prompt and no padding, and
+        every later (decoded) query sees all cached keys, which is the prefix mask's rule for it."""
         B, S = tokens.shape
         cache.set_lengths(lengths)
+        prefix = None
+        if self.args.prefix_lm:
+            prefix = torch.tensor([int(n) for n in lengths], dtype=torch.int32).to(tokens.device)
         h = ops.embedding(tokens, self.embed_tokens.weight)
         pending = None
         for i, layer in enumerate(self.layers):
-            h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window)
+            h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window, prefix)
         rows = torch.arange(B, device=tokens.device)
         last = torch.tensor([n - 1 for n in lengths], device=tokens.device)
         return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])

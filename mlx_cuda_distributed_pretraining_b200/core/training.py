@@ -73,6 +73,15 @@ class ModelConfig:
         a = self.attention.get("alibi")
         if a is not None and not isinstance(a, bool):
             raise ValueError(f"model.attention.alibi must be null, true or false, got {a!r}")
+        # extension: attention.prefix_lm (absent / null / false: off); each row's prefix attends bidirectionally
+        pl = self.attention.get("prefix_lm")
+        if pl is not None and not isinstance(pl, bool):
+            raise ValueError(f"model.attention.prefix_lm must be null, true or false, got {pl!r}")
+        if pl:
+            if w is not None:
+                raise ValueError("model.attention.prefix_lm does not combine with model.attention.sliding_window")
+            if a:
+                raise ValueError("model.attention.prefix_lm does not combine with model.attention.alibi")
         # extension: misc.variant selects the block (absent / null / "reference": arch/llama.py's; "mlx_lm": the
         # mlx_lm.models.llama block the reference's trainer actually imports, DESIGN D4)
         v = (self.misc or {}).get("variant")
@@ -180,6 +189,9 @@ class Config:
     overwrite: bool = False
 
     def __post_init__(self):
+        if self.model.attention.get("prefix_lm") and (self.data.preprocessing or {}).get("pack_sequences"):
+            raise ValueError("model.attention.prefix_lm does not combine with data.preprocessing.pack_sequences "
+                             "(a prefix per packed document is not supported)")
         E = _int_or_none(self.model.misc or {}, "num_local_experts")
         if E > 0:
             opt = self.training.optimization or {}
@@ -299,8 +311,9 @@ class SyntheticData:
                                          oracle's twin is reference_math.synthetic_batch_markov (same draws)."""
 
     def __init__(self, vocab: int, batch_size: int, seq_len: int, rank: int = 0, num_batches: int = 1 << 30,
-                 kind: str = "uniform"):
+                 kind: str = "uniform", prefix_lm: bool = False):
         self.vocab, self.batch_size, self.seq_len, self.rank = vocab, batch_size, seq_len, rank
+        self.prefix_lm = prefix_lm
         self.train_docs = range(num_batches * batch_size)
         self.has_validation_data = False
         self.num_validation_batches = 0
@@ -312,6 +325,15 @@ class SyntheticData:
                       if kind == "markov" else None)
 
     def generate_batch(self, step: int) -> torch.Tensor:
+        """[B, S + 1] tokens; with prefix_lm, [B, 1 + S + 1] with each row's split point in column 0, drawn uniformly
+        from [0, S] by split_points (the tokens are the same draws as without prefix_lm)."""
+        toks = self._tokens(step)
+        if not self.prefix_lm:
+            return toks
+        P = split_points([self.seq_len] * self.batch_size, train_split_seed(step, self.rank))
+        return torch.cat([P[:, None], toks], dim=1)
+
+    def _tokens(self, step: int) -> torch.Tensor:
         g = torch.Generator().manual_seed(42 + 1000 * step + self.rank)
         B, S = self.batch_size, self.seq_len
         if self.kind == "uniform":
@@ -324,6 +346,33 @@ class SyntheticData:
         for t in range(S):
             out[:, t + 1] = torch.where(noisy[:, t], rnd[:, t], self._succ[out[:, t], choice[:, t]])
         return out
+
+
+def train_split_seed(step: int, rank: int) -> int:
+    """Seed of the prefix-LM split points of training step `step` on data-parallel rank `rank`."""
+    return 0x5EED_0000 + 4096 * step + rank
+
+
+def val_split_seed(batch_idx: int) -> int:
+    """Seed of the prefix-LM split points of validation batch `batch_idx`."""
+    return 0x7A1_0000 + batch_idx
+
+
+def split_points(lengths: List[int], seed: int) -> torch.Tensor:
+    """Prefix-LM split points (int64 [len(lengths)]): row b's P is uniform in [0, lengths[b]], drawn from a generator
+    of its own seeded with `seed`, so the shuffling and the token stream are untouched by the draws."""
+    g = torch.Generator().manual_seed(seed)
+    u = torch.rand(len(lengths), generator=g, dtype=torch.float64)
+    n = torch.tensor(lengths, dtype=torch.float64)
+    return torch.minimum((u * (n + 1)).floor(), n).to(torch.int64)
+
+
+def prefix_targets(targets: torch.Tensor, prefix: torch.Tensor, pad_token: int) -> torch.Tensor:
+    """Targets [B, S] of prefix-LM rows with prefix lengths prefix [B]: a prefix position q <= P_b - 2 sees its own
+    target x[q + 1], so those targets become PAD (no loss, no token count); the target at q = P_b - 1, the first token
+    after the prefix, is kept.  Runs on the targets' device without a host synchronisation."""
+    q = torch.arange(targets.shape[1], device=targets.device)
+    return targets.masked_fill(q[None, :] < (prefix.to(targets.device)[:, None] - 1), pad_token)
 
 
 def pack_first_fit(lengths: List[int], capacity: int) -> List[List[int]]:
@@ -367,6 +416,11 @@ def document_positions(inputs: torch.Tensor, bos_token: int) -> torch.Tensor:
     return (idx - start).to(torch.int32)
 
 
+def _doc_len(doc) -> int:
+    """Characters of a text chunk or of a prompt / completion pair (the order the batches are formed in)."""
+    return len(doc) if isinstance(doc, str) else len(doc[0]) + len(doc[1])
+
+
 class DataManager:
     """Unpacked (default): each training row is one chunk, padded to the longest chunk of its batch.
 
@@ -374,24 +428,30 @@ class DataManager:
     chunks (tokenize_doc: BOS first), placed first-fit in the shuffled order, tails filled with PAD; a chunk longer
     than a row is cut to the row.  Every chunk appears once per epoch.  The packed batches are walked in a permuted
     order drawn from the same global RNG after the unpacked state, so the validation batches (never packed) are the
-    unpacked run's."""
+    unpacked run's.
+
+    prefix_lm: a `{"prompt": ..., "completion": ...}` line is one document, never chunked, whose row is
+    [BOS] + tokenize(prompt) + tokenize(completion) + [EOS] with the prefix P = 1 + len(tokenize(prompt)); a `{"text":
+    ...}` chunk's P is drawn uniformly from [0, n_b] (n_b: the row's non-PAD inputs) by split_points.  Rows are
+    truncated as without prefix_lm and P is clipped to the row.  Batches are then [B, 1 + S + 1] with P in column 0."""
 
     def __init__(self, config: DataConfig, tokenizer: TokenizerManager, batch_size: int = 1, rank: int = 0,
-                 world: int = 1):
+                 world: int = 1, prefix_lm: bool = False):
         self.config, self.tokenizer, self.batch_size = config, tokenizer, batch_size
         self.rank, self.world = rank, world
-        self.train_docs: List[str] = []
-        self.val_docs: List[str] = []
+        self.prefix_lm = prefix_lm
+        self.train_docs: List[Any] = []
+        self.val_docs: List[Any] = []
         self.val_ptr = 0
         self._load_file(config.input_file, self.train_docs)
-        idx = sorted(range(len(self.train_docs)), key=lambda i: len(self.train_docs[i]))
+        idx = sorted(range(len(self.train_docs)), key=lambda i: _doc_len(self.train_docs[i]))
         random.shuffle(idx)
         self.train_batch_idx = [idx[i:i + batch_size] for i in range(0, len(idx) - batch_size + 1, batch_size)]
         self.train_indices = np.random.permutation(len(self.train_batch_idx))
         self.val_batch_idx: List[List[int]] = []
         if config.validation_file:
             self._load_file(config.validation_file, self.val_docs)
-            vidx = sorted(range(len(self.val_docs)), key=lambda i: len(self.val_docs[i]))
+            vidx = sorted(range(len(self.val_docs)), key=lambda i: _doc_len(self.val_docs[i]))
             self.val_batch_idx = [vidx[i:min(i + batch_size, len(vidx))] for i in range(0, len(vidx), batch_size)]
             self.val_indices = np.random.permutation(len(self.val_batch_idx))
         self.pack = bool(config.preprocessing.get("pack_sequences", False))
@@ -419,12 +479,19 @@ class DataManager:
         """Training batches per epoch (packed batches when packing is on)."""
         return len(self.packed_batch_idx) if self.pack else len(self.train_batch_idx)
 
-    def _load_file(self, file_path: str, docs: List[str]) -> None:
+    def _load_file(self, file_path: str, docs: List[Any]) -> None:
         chunk = self.config.preprocessing["max_context_size"]
         stride = chunk - self.config.preprocessing.get("chunk_overlap", 0)
         with open(file_path, "r") as f:
             for line in f:
-                text = json.loads(line)["text"]
+                rec = json.loads(line)
+                if self.prefix_lm and "text" not in rec and "prompt" in rec and "completion" in rec:
+                    docs.append((str(rec["prompt"]), str(rec["completion"])))  # a pair is never chunked
+                    continue
+                if "text" not in rec:
+                    keys = '"text", or "prompt" and "completion"' if self.prefix_lm else '"text"'
+                    raise ValueError(f"{file_path}: a line has keys {sorted(rec)}; expected {keys}")
+                text = rec["text"]
                 for i in range(0, len(text), stride):
                     docs.append(text[i:i + chunk])
 
@@ -433,7 +500,8 @@ class DataManager:
             return self._packed_batch(step)
         # data-parallel ranks walk disjoint batches of the shared shuffled order
         j = (step * self.world + self.rank) % len(self.train_indices)
-        return self._create_batch([self.train_docs[i] for i in self.train_batch_idx[self.train_indices[j]]])
+        return self._create_batch([self.train_docs[i] for i in self.train_batch_idx[self.train_indices[j]]],
+                                  train_split_seed(step, self.rank))
 
     def _packed_batch(self, step: int) -> torch.Tensor:
         """[batch_size, max_context_size + 1] rows of whole documents; the last batch of an epoch may hold rows
@@ -451,13 +519,29 @@ class DataManager:
             raise ValueError("No validation data available")
         ids = self.val_batch_idx[self.val_indices[self.val_ptr % len(self.val_indices)]]
         self.val_ptr += 1
-        return self._create_batch([self.val_docs[i] for i in ids])
+        return self._create_batch([self.val_docs[i] for i in ids], val_split_seed(batch_idx))
 
-    def _create_batch(self, docs: List[str]) -> torch.Tensor:
-        batch = [self.tokenizer.tokenize_doc(d) for d in docs]
+    def _tokenize_pair(self, doc) -> Tuple[List[int], int]:
+        """A prompt / completion pair -> ([BOS] + prompt + completion + [EOS], its prefix 1 + len(prompt))."""
+        t = self.tokenizer
+        p = t.tokenize(doc[0])
+        return [t.BOS_TOKEN] + p + t.tokenize(doc[1]) + [t.EOS_TOKEN], 1 + len(p)
+
+    def _create_batch(self, docs: List[Any], split_seed: int = 0) -> torch.Tensor:
+        pairs = [self._tokenize_pair(d) if isinstance(d, tuple) else (self.tokenizer.tokenize_doc(d), None)
+                 for d in docs]
+        batch = [x for x, _ in pairs]
         max_len = min(max(len(x) for x in batch), self.config.preprocessing.get("max_context_size", 2048))
         rows = [x[:max_len] + [self.tokenizer.PAD_TOKEN] * (max_len - len(x[:max_len])) for x in batch]
-        return torch.tensor(rows, dtype=torch.int64)
+        out = torch.tensor(rows, dtype=torch.int64)
+        if not self.prefix_lm:
+            return out
+        # inputs are row[:-1]: row b has min(len, max_len - 1) non-PAD inputs
+        n_in = [min(len(x), max_len - 1) for x in batch]
+        drawn = split_points(n_in, split_seed)
+        P = torch.tensor([min(p, max_len) if p is not None else int(drawn[b]) for b, (_, p) in enumerate(pairs)],
+                         dtype=torch.int64)
+        return torch.cat([P[:, None], out], dim=1)
 
     @property
     def has_validation_data(self) -> bool:
@@ -720,7 +804,7 @@ class Trainer:
             flash_block_size=m.attention.get("flash_block_size", 128),
             apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")) or m.misc.get("variant") == "mlx_lm",
             sliding_window=m.attention.get("sliding_window"), alibi=bool(m.attention.get("alibi")),
-            variant=m.misc.get("variant"),
+            prefix_lm=bool(m.attention.get("prefix_lm")), variant=m.misc.get("variant"),
             num_local_experts=m.misc.get("num_local_experts") or 0,
             num_experts_per_tok=m.misc.get("num_experts_per_tok") or 0,
             router_aux_loss_coef=float(m.misc.get("router_aux_loss_coef", 0.001)))
@@ -745,9 +829,11 @@ class Trainer:
         if self.synthetic:
             kind = self.config.data.input_file.split(":", 1)[1] if ":" in self.config.data.input_file else "uniform"
             self.data_manager = SyntheticData(self.config.data.tokenizer["normal_vocab_size"], bs, seq, self.rank,
-                                              num_batches=hp.get("iters", 1000), kind=kind)
+                                              num_batches=hp.get("iters", 1000), kind=kind,
+                                              prefix_lm=self.model_args.prefix_lm)
         else:
-            self.data_manager = DataManager(self.config.data, self.tokenizer, bs, self.rank, self.world)
+            self.data_manager = DataManager(self.config.data, self.tokenizer, bs, self.rank, self.world,
+                                            prefix_lm=self.model_args.prefix_lm)
 
     def setup_training(self) -> None:
         hp = self.config.training.hyperparameters
@@ -778,20 +864,29 @@ class Trainer:
 
     # -- loss --------------------------------------------------------------------------------------
     def compute_loss(self, model, inputs: torch.Tensor, targets: torch.Tensor, packed: bool = False,
-                     aux: bool = True):
+                     aux: bool = True, prefix: Optional[torch.Tensor] = None):
         """Masked token-mean cross-entropy.  packed: the rows hold several documents (DataManager with
         pack_sequences); the model then attends within documents (position_ids from the BOS tokens), and the one
         target per document boundary that an unpacked row never has -- a document's last token predicting the
-        next document's BOS -- becomes PAD, so the loss terms and ntoks are those of the documents run alone."""
+        next document's BOS -- becomes PAD, so the loss terms and ntoks are those of the documents run alone.
+        prefix (int [B] on the device): prefix-LM rows; the model attends with PrefixCausalMask and the targets a
+        prefix position can see become PAD (prefix_targets)."""
         max_ctx = self.config.model.attention.get("max_position_embeddings", 2048)
         if inputs.shape[1] > max_ctx:
             inputs, targets = inputs[:, :max_ctx], targets[:, :max_ctx]
         position_ids = None
+        kw = {}
+        if prefix is not None:
+            targets = prefix_targets(targets, prefix, self.tokenizer.PAD_TOKEN)
+            kw = {"prefix_lens": prefix.to(torch.int32)}
         if packed:
             position_ids = document_positions(inputs, self.tokenizer.BOS_TOKEN)
             targets = targets.masked_fill(targets == self.tokenizer.BOS_TOKEN, self.tokenizer.PAD_TOKEN)
         pad_mask = targets != self.tokenizer.PAD_TOKEN
         ntoks = pad_mask.sum()
+        # prefix-LM rows can keep no target (a prompt that fills the row, or a split point at the row's end), so a
+        # micro-batch may have none: its loss is then 0 with no gradient, and ntoks reports the true count 0
+        denom = ntoks if prefix is None else ntoks.clamp_min(1)
         # MoE models: the load-balancing loss counts the non-PAD inputs; it is kept in self.last_aux_loss for
         # micro_step, and skipped entirely when its coefficient is 0 or aux is off (validation reports CE only)
         args = getattr(self, "model_args", None)
@@ -802,21 +897,22 @@ class Trainer:
         if not hasattr(model, "padded_logits"):
             logits2d, V = None, None
         elif position_ids is None:
-            logits2d, V = model.padded_logits(inputs, **moe_kw)
+            logits2d, V = model.padded_logits(inputs, **moe_kw, **kw)
         else:
-            logits2d, V = model.padded_logits(inputs, position_ids, **moe_kw)
+            logits2d, V = model.padded_logits(inputs, position_ids, **moe_kw, **kw)
         if moe_kw and logits2d is not None:
             self.last_aux_loss = model.moe_aux_loss()
         if logits2d is not None:
             # fused path: fp32 log-sum-exp over bf16 logits, pad mask applied per row, no fp32 [B,S,V] copy
             rows = ops.cross_entropy_rows(logits2d, targets.reshape(-1).contiguous(), V, self.tokenizer.PAD_TOKEN)
-            return rows.sum() / ntoks, ntoks
-        logits = (model(inputs, **moe_kw) if position_ids is None else model(inputs, position_ids, **moe_kw)).float()
+            return rows.sum() / denom, ntoks
+        logits = (model(inputs, **moe_kw, **kw) if position_ids is None
+                  else model(inputs, position_ids, **moe_kw, **kw)).float()
         if moe_kw:
             self.last_aux_loss = model.moe_aux_loss()
         ce = torch.nn.functional.cross_entropy(logits.view(-1, logits.shape[-1]), targets.reshape(-1),
                                                reduction="none").view(targets.shape)
-        return (ce * pad_mask).sum() / ntoks, ntoks
+        return (ce * pad_mask).sum() / denom, ntoks
 
     def _to_device(self, batch: torch.Tensor) -> torch.Tensor:
         """Per-step host->device copy of the token batch from pinned memory.  The CPU can run a whole step
@@ -860,8 +956,11 @@ class Trainer:
         """Forward + backward of one micro-batch already resident on the device, gradient clamp / 1/k
         accumulation (core/training.py:1664-1696), and -- on the k-th micro-step -- the data-parallel
         exchange and the optimizer update.  Returns (loss, ntoks, did_update)."""
+        prefix = None
+        if self.model_args.prefix_lm:  # column 0 holds each row's prefix length
+            prefix, dev_batch = dev_batch[:, 0], dev_batch[:, 1:]
         loss, ntoks = self.compute_loss(self.model, dev_batch[:, :-1], dev_batch[:, 1:],
-                                        packed=getattr(self.data_manager, "pack", False))
+                                        packed=getattr(self.data_manager, "pack", False), prefix=prefix)
         aux = getattr(self, "last_aux_loss", None)
         if aux is None:
             loss.backward()
@@ -895,13 +994,19 @@ class Trainer:
         with torch.no_grad():
             for i in range(min(self.data_manager.num_validation_batches, 50)):
                 b = self._to_device(self.data_manager.generate_validation_batch(i))
-                loss, ntoks = self.compute_loss(self.model, b[:, :-1], b[:, 1:], aux=False)
+                prefix = None
+                if self.model_args.prefix_lm:
+                    prefix, b = b[:, 0], b[:, 1:]
+                loss, ntoks = self.compute_loss(self.model, b[:, :-1], b[:, 1:], aux=False, prefix=prefix)
                 tot_loss += loss * ntoks
                 tot_tok += ntoks
         if self.distributed:
             v = torch.stack([tot_loss, tot_tok])
             dp.all_reduce_sum_(v)
             tot_loss, tot_tok = v[0], v[1]
+        if self.model_args.prefix_lm and float(tot_tok.item()) == 0:
+            raise ValueError("prefix_lm: no validation target is left after the prefix masking (every prompt fills "
+                             "its row); shorten the prompts or raise data.preprocessing.max_context_size")
         return float((tot_loss / tot_tok).item())
 
     def save_config(self) -> Path:

@@ -43,6 +43,13 @@
 // the pre-pass are unchanged.  A thread's queries are q0 + 8 nc + cq + {0, 1}: per item one integer per key is
 // converted, base = m log2e (key - q0 - cq), and each element's bias is fmaf(m log2e, -c, base) for the compile-time
 // column c.  With m = 0 the bias is exactly 0 and P^T is the DOC kernel's.  ALIBI = false compiles unchanged.
+//
+// Prefix-LM (PREFIX = true, causal DOC = false kernels only): query q sees key k iff k <= q or k < P_b, with
+// P_b = prefix[b] clamped to [0, S].  A key tile below P_b is seen by every query, so its query range starts at query
+// tile 0; other key tiles start at the causal k0 / BQ.  An item is masked when the warpgroup's last key exceeds
+// max(q0, P_b - 1) or it crosses S, and the element mask is `key > q && key >= P_b` plus the bounds.  The pre-pass is
+// unchanged.  Prefix launches use the unpaired order: the causal pairing no longer balances the work.  P_b <= 1 gives
+// the causal kernel's items and values.  PREFIX = false compiles unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -92,14 +99,18 @@ struct BwdArgs {
   const int* dstart;   // DOC: [B,S_pad] document start of every query
   const int* qt_end;   // DOC: [B,n_kt] end of each key tile's query-tile range
   const float* slopes; // ALIBI: [H] fp32 per-query-head slopes
+  const int* prefix;   // PREFIX: [B] int32 prefix lengths (clamped to [0, S])
 };
+
+// PREFIX: batch row b's prefix length
+__device__ __forceinline__ int prefix_len(const BwdArgs& p, int b) { return min(max(__ldg(p.prefix + b), 0), p.S); }
 
 // The work of one key tile: `group * per_head` items, item j = (query head h0 + j / per_head, query tile
 // qt0 + j % per_head).
 struct Tile {
   int kt, k0, qt0, per_head, n_items;
 };
-template <bool DOC>
+template <bool DOC, bool PREFIX = false>
 __device__ __forceinline__ Tile tile_of(const BwdArgs& p, int pass) {
   Tile t;
   t.kt = pass == 0 ? (int)blockIdx.x : (p.S + BKV - 1) / BKV - 1 - (int)blockIdx.x;
@@ -107,6 +118,9 @@ __device__ __forceinline__ Tile tile_of(const BwdArgs& p, int pass) {
   int n_qt = (p.S + BQ - 1) / BQ;
   if constexpr (DOC) n_qt = __ldg(p.qt_end + (long long)blockIdx.z * gridDim.x + t.kt);  // unpaired: x = kt
   t.qt0 = p.causal ? t.k0 / BQ : 0;
+  if constexpr (PREFIX) {
+    if (t.k0 < prefix_len(p, blockIdx.z)) t.qt0 = 0;  // every query sees the tile's prefix keys
+  }
   t.per_head = n_qt - t.qt0;
   t.n_items = (p.H / p.Hk) * t.per_head;
   return t;
@@ -124,11 +138,12 @@ __device__ __forceinline__ void rs_mma(float* acc, const uint32_t* a, uint64_t d
   else wgmma_m64n64k16_rs<1>(acc, a, db);
 }
 
-template <int D, bool DOC, bool ALIBI = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
                 const __grid_constant__ CUtensorMap tmDQ, const BwdArgs p) {
+  static_assert(!PREFIX || (!DOC && !ALIBI), "the prefix mask is built on the causal kernel");
   using Cfg = BwdCfg<D, DOC>;
   constexpr int ST = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -166,7 +181,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       int slot = 0;
       uint32_t phase = 0;
       for (int pass = 0; pass < n_pass; ++pass) {
-        const Tile t = tile_of<DOC>(p, pass);
+        const Tile t = tile_of<DOC, PREFIX>(p, pass);
         if (pass > 0) mbar_wait(kv_empty, 0);
         mbar_arrive_expect_tx(kv_full, 2 * Cfg::KV_BYTES);
         for (int nb = 0; nb < Cfg::NB; ++nb) {
@@ -198,7 +213,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       tma_prefetch_desc(&tmDQ);
       int it = 0;
       for (int pass = 0; pass < n_pass; ++pass) {
-        const Tile t = tile_of<DOC>(p, pass);
+        const Tile t = tile_of<DOC, PREFIX>(p, pass);
         for (int j = 0; j < t.n_items; ++j, ++it) {
           const int h = hk * group + j / t.per_head;
           const int q0 = (t.qt0 + j % t.per_head) * BQ;
@@ -227,7 +242,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   int it = 0;
 
   for (int pass = 0; pass < n_pass; ++pass) {
-    const Tile t = tile_of<DOC>(p, pass);
+    const Tile t = tile_of<DOC, PREFIX>(p, pass);
     const int key_a = t.k0 + c * 64 + wq * 16 + g;  // this thread's keys: key_a, key_a + 8
     const int wkey_hi = t.k0 + c * 64 + 63;          // last key of this warpgroup
     float dk[D / 2], dv[D / 2];
@@ -267,7 +282,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
       // P^T and dS^T (unscaled).  Chunk nc holds queries 8 nc + cq + {0, 1}.  Only tiles that cross the causal
       // diagonal or the end of the sequence are masked; masked entries are exactly 0.
-      bool masked = (p.causal && wkey_hi > q0) || q0 + BQ > p.S || wkey_hi >= p.S;
+      const int pfx = PREFIX ? prefix_len(p, b) : 0;  // PREFIX: this row's prefix length
+      bool masked;
+      // PREFIX: keys below the prefix are visible to every query, so only keys past max(q0, P_b - 1) need the mask
+      if constexpr (PREFIX) masked = wkey_hi > max(q0, pfx - 1) || q0 + BQ > p.S || wkey_hi >= p.S;
+      else masked = (p.causal && wkey_hi > q0) || q0 + BQ > p.S || wkey_hi >= p.S;
       // DOC: also where the item's highest document start (its last query's; padded rows repeat the last real one)
       // lies above the warpgroup's first key
       if constexpr (DOC) masked = masked || lds32i(tL + 2 * BQ * 4 + (BQ - 1) * 4) > wkey_hi - 63;
@@ -295,7 +314,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             const int qc = nc * 8 + cq + (e & 1);
             const int qi = q0 + qc;
             const int key = key_a + ((e >> 1) << 3);
-            bool ok = qi < p.S && key < p.S && !(p.causal && key > qi);
+            bool ok;
+            if constexpr (PREFIX) ok = qi < p.S && key < p.S && (key <= qi || key < pfx);
+            else ok = qi < p.S && key < p.S && !(p.causal && key > qi);
             if constexpr (DOC) ok = ok && qc < n_vis[e >> 1];
             float pv;
             if constexpr (ALIBI)
@@ -506,11 +527,11 @@ f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ ds
   }
 }
 
-template <int D, bool DOC, bool ALIBI = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
 int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmDO,
                const CUtensorMap& tmDQ, const BwdArgs& a, cudaStream_t stream) {
   using Cfg = BwdCfg<D, DOC>;
-  auto kern = attn_bwd_kernel<D, DOC, ALIBI>;
+  auto kern = attn_bwd_kernel<D, DOC, ALIBI, PREFIX>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -549,11 +570,12 @@ size_t attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
 
 namespace {
 
-// doc selects the document / window kernels; window < 0 means none; slopes (doc only) selects ALiBi
+// doc selects the document / window kernels; window < 0 means none; slopes (doc only) selects ALiBi; prefix (causal,
+// not doc) selects the prefix-LM kernels
 int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                   bool doc, const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk,
                   int D, float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream,
-                  const float* slopes = nullptr) {
+                  const float* slopes = nullptr, const int* prefix = nullptr) {
   // dk / dv rows may be strided: dkv_row_heads heads per token row (0 = Hk, i.e. contiguous [B,S,Hk,D]).
   // With dk = base, dv = base + Hk*D and dkv_row_heads = 2*Hk both land in ONE [B,S,2*Hk*D] buffer, which lets
   // the k/v projections' dgrad and wgrad run as single GEMMs over the concatenated weight.
@@ -609,11 +631,15 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
   a.dkv_rh = dkv_row_heads;
   a.scale = scale;
   a.causal = causal;
-  a.paired = causal && !doc && n_kt % 2 == 0;
+  a.paired = causal && !doc && !prefix && n_kt % 2 == 0;
   a.dstart = doc ? dstart : nullptr;
   a.qt_end = doc ? qt_end : nullptr;
   a.slopes = slopes;
-  if (slopes)
+  a.prefix = prefix;
+  if (prefix)
+    rc = D == 64 ? launch_bwd<64, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+                 : launch_bwd<128, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
+  else if (slopes)
     rc = D == 64 ? launch_bwd<64, true, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
                  : launch_bwd<128, true, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
   else if (doc)
@@ -673,6 +699,17 @@ int attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, c
                  "attn_bwd_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
   return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
                        ws, ws_bytes, stream, slopes);
+}
+
+// prefix-LM backward: query s of row b sees key k iff k <= s or k < prefix[b] (clamped to [0, S] in the kernel).
+// Same workspace as the causal backward.
+int attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                    const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                    int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG(prefix != nullptr && (reinterpret_cast<uintptr_t>(prefix) & 3u) == 0,
+                 "attn_bwd_prefix: prefix must be a non-null, 4-byte aligned int32 [B] array");
+  return attn_bwd_impl(q, k, v, o, d_o, lse, false, nullptr, -1, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
+                       ws, ws_bytes, stream, nullptr, prefix);
 }
 
 }  // namespace b200

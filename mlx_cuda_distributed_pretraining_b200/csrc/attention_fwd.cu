@@ -29,6 +29,14 @@
 // is fmaf(m log2e, c, base): no int -> float conversion per element (that pipe is the one exp2 already fills).  With
 // m = 0 the bias is exactly 0 and the scores are the DOC kernel's.  k - q is also the distance within a document, so
 // packed rows need nothing more.  ALIBI = false compiles to the kernels above unchanged.
+//
+// Prefix-LM (PREFIX = true, causal DOC = false kernels only): row b has a prefix length P_b = prefix[b], clamped to
+// [0, S] in the kernel so that no value can send the key loop past the sequence.  Query q sees key k iff k <= q or
+// k < P_b: the prefix attends bidirectionally within itself and later queries are causal over everything before them.
+// The visible keys of a query are still 0 .. max(q, P_b - 1), monotone in q, so the key loop ends at
+// max(causal end, ceil(P_b / 128)) and the element mask `key >= S || (key > row && key >= P_b)` runs only on tiles
+// whose last key exceeds max(q0, P_b - 1) or that cross S.  P_b <= 1 is the causal mask (the same tiles, the same
+// values); P_b = S is the non-causal one.  PREFIX = false compiles to the kernels above unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -62,6 +70,7 @@ struct FwdArgs {
   const int* pos;  // [B, S] positions within documents (DOC kernels only; null: pos[q] = q)
   int window;      // DOC: query q sees keys from q - min(pos[q], window); S when there is no window
   const float* slopes;  // ALIBI: [H] fp32 per-query-head slopes
+  const int* prefix;    // PREFIX: [B] int32 prefix lengths (clamped to [0, S])
 };
 
 // first key query `row` of batch row b may see: its document start, or its window start when that is later
@@ -77,10 +86,11 @@ __device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db)
   else wgmma_m64n64k16_rs<1>(o, a, db);
 }
 
-template <int D, bool DOC, bool ALIBI = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdArgs p) {
+  static_assert(!PREFIX || (!DOC && !ALIBI), "the prefix mask is built on the causal kernel");
   using Cfg = FwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -92,7 +102,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int q0 = qt * ATT_BQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_kv_all = (p.S + ATT_BKV - 1) / ATT_BKV;
-  const int n_kv = p.causal ? min(n_kv_all, (q0 + ATT_BQ - 1) / ATT_BKV + 1) : n_kv_all;
+  int n_kv = p.causal ? min(n_kv_all, (q0 + ATT_BQ - 1) / ATT_BKV + 1) : n_kv_all;
+  // PREFIX: this row's prefix length, and the key loop extended to the last tile holding a prefix key
+  int pfx = 0;
+  if constexpr (PREFIX) {
+    pfx = min(max(__ldg(p.prefix + b), 0), p.S);
+    n_kv = max(n_kv, (pfx + ATT_BKV - 1) / ATT_BKV);
+  }
   // first key tile: the first query's document / window start (0 without documents)
   int j0 = 0;
   if constexpr (DOC) j0 = max(0, key_start(p, b, q0)) / ATT_BKV;
@@ -208,6 +224,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
           mx[e >> 1] = fmaxf(mx[e >> 1], x);
         }
       }
+    } else if constexpr (PREFIX) {
+      // tiles wholly inside the prefix or at or below every row's diagonal, and inside S, are visible throughout
+      const bool edge = k0 + ATT_BKV - 1 > max(q0, pfx - 1) || k0 + ATT_BKV > p.S;
+#pragma unroll
+      for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
+          const int row = row_a + ((e >> 1) << 3);
+          float x = sc[4 * nc + e] * sl2;
+          if (edge && (key >= p.S || (key > row && key >= pfx))) x = -INFINITY;
+          sc[4 * nc + e] = x;
+          mx[e >> 1] = fmaxf(mx[e >> 1], x);
+        }
+      }
     } else {
 #pragma unroll
       for (int nc = 0; nc < 16; ++nc) {
@@ -290,11 +321,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-template <int D, bool DOC, bool ALIBI = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
 int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
                cudaStream_t stream) {
   using Cfg = FwdCfg<D>;
-  auto kern = attn_fwd_kernel<D, DOC, ALIBI>;
+  auto kern = attn_fwd_kernel<D, DOC, ALIBI, PREFIX>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -318,10 +349,11 @@ int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, in
 
 namespace {
 
-// doc selects the document / window instantiation; window < 0 means none; slopes (doc only) selects ALiBi
+// doc selects the document / window instantiation; window < 0 means none; slopes (doc only) selects ALiBi; prefix
+// (causal, not doc) selects the prefix-LM kernels
 int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, bool doc, const int* pos,
                   int window, int B, int S, int H, int Hk, int D, float scale, int causal, cudaStream_t stream,
-                  const float* slopes = nullptr) {
+                  const float* slopes = nullptr, const int* prefix = nullptr) {
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_fwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd: head_dim %d unsupported (64 or 128; pad smaller dims)", D);
@@ -343,6 +375,10 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   a.pos = pos;
   a.window = window < 0 || window > S ? S : window;
   a.slopes = slopes;
+  a.prefix = prefix;
+  if (prefix)
+    return D == 64 ? launch_fwd<64, false, false, true>(tmQ, tmK, tmV, a, stream)
+                   : launch_fwd<128, false, false, true>(tmQ, tmK, tmV, a, stream);
   if (slopes)
     return D == 64 ? launch_fwd<64, true, true>(tmQ, tmK, tmV, a, stream)
                    : launch_fwd<128, true, true>(tmQ, tmK, tmV, a, stream);
@@ -380,6 +416,14 @@ int attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* 
   B200_CHECK_ARG(slopes != nullptr && (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
                  "attn_fwd_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
   return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, stream, slopes);
+}
+
+// prefix-LM: query s of row b sees key k iff k <= s or k < prefix[b] (clamped to [0, S] in the kernel)
+int attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float* lse, const int* prefix, int B, int S,
+                    int H, int Hk, int D, float scale, cudaStream_t stream) {
+  B200_CHECK_ARG(prefix != nullptr && (reinterpret_cast<uintptr_t>(prefix) & 3u) == 0,
+                 "attn_fwd_prefix: prefix must be a non-null, 4-byte aligned int32 [B] array");
+  return attn_fwd_impl(q, k, v, o, lse, false, nullptr, -1, B, S, H, Hk, D, scale, 1, stream, nullptr, prefix);
 }
 
 }  // namespace b200

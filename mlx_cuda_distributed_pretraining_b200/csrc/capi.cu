@@ -128,6 +128,11 @@ int attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* 
 int attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                    const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S, int H,
                    int Hk, int D, float scale, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
+int attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float* lse, const int* prefix, int B, int S,
+                    int H, int Hk, int D, float scale, cudaStream_t stream);
+int attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                    const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                    int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D);
 int attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                       int window, const float* slopes, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
@@ -455,6 +460,20 @@ int b200_attn_bwd_window(const void* q, const void* k, const void* v, const void
                          const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
                          float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream) {
   return b200::attn_bwd_window(q, k, v, o, d_o, lse, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, dkv_row_heads,
+                               workspace, workspace_bytes, S_(stream));
+}
+
+int b200_attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float* lse, const int* prefix, int B,
+                         int S, int H, int Hk, int D, float scale, void* stream) {
+  return b200::attn_fwd_prefix(q, k, v, o, lse, prefix, B, S, H, Hk, D, scale, S_(stream));
+}
+size_t b200_attn_bwd_prefix_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return b200::attn_bwd_workspace_bytes(B, S, H, Hk, D);
+}
+int b200_attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                         const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
+                         float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream) {
+  return b200::attn_bwd_prefix(q, k, v, o, d_o, lse, prefix, dq, dk, dv, B, S, H, Hk, D, scale, dkv_row_heads,
                                workspace, workspace_bytes, S_(stream));
 }
 

@@ -695,12 +695,31 @@ def _check_alibi(alibi: torch.Tensor, q: torch.Tensor, causal: bool, what: str) 
     return alibi
 
 
+def _check_prefix(prefix: torch.Tensor, q: torch.Tensor, causal: bool, pos, window, alibi, what: str) -> torch.Tensor:
+    """Prefix lengths: an int32 [B] tensor on q's device.  The prefix mask is its own causal mask, so it does not
+    combine with pos, window, alibi or causal=False.  The values are not checked (that would read the device): the
+    kernels clamp them to [0, S]."""
+    for name, given in (("pos", pos is not None), ("window", window is not None), ("alibi", alibi is not None),
+                        ("causal=False", not causal)):
+        if given:
+            raise ValueError(f"{what}: prefix does not combine with {name}")
+    B = q.shape[0]
+    if not isinstance(prefix, torch.Tensor) or prefix.dtype != torch.int32 or tuple(prefix.shape) != (B,):
+        raise ValueError(f"{what}: prefix must be an int32 [B] = [{B}] tensor of prefix lengths, got "
+                         f"{getattr(prefix, 'dtype', type(prefix))} {list(getattr(prefix, 'shape', []))}")
+    if prefix.device != q.device:
+        raise ValueError(f"{what}: prefix is on {prefix.device}, the operands on {q.device}")
+    return prefix.contiguous()
+
+
 def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
-                      window: Optional[int] = None, alibi: Optional[torch.Tensor] = None):
+                      window: Optional[int] = None, alibi: Optional[torch.Tensor] = None,
+                      prefix: Optional[torch.Tensor] = None):
     """q [B,S,H,D], k/v [B,S,Hk,D] bf16 contiguous, D in {64,128}. Returns (o, lse[B,H,S]).  With pos (int32 [B,S]
     contiguous, positions within documents) the mask is document-causal and `causal` is ignored.  With window (an
     int >= 0) query s sees keys s - min(pos[s], window) .. s (pos[s] = s without pos), and `causal` is ignored.
-    With alibi (fp32 [H] slopes, checked by the caller) the causal / document / window mask gets the ALiBi bias."""
+    With alibi (fp32 [H] slopes, checked by the caller) the causal / document / window mask gets the ALiBi bias.
+    With prefix (int32 [B], checked by the caller) query s of row b sees key k iff k <= s or k < prefix[b]."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         _need(t, torch.bfloat16, nm)
     B, S, H, D = q.shape
@@ -708,7 +727,11 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
     o = torch.empty_like(q)
     lse = torch.empty((B, H, S), device=q.device, dtype=torch.float32)
     tok = _t0("attn_fwd")
-    if alibi is not None:
+    if prefix is not None:
+        check(lib().b200_attn_fwd_prefix(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+                                         prefix.data_ptr(), B, S, H, Hk, D, float(scale), _stream()),
+              "b200_attn_fwd_prefix")
+    elif alibi is not None:
         check(lib().b200_attn_fwd_alibi(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
                                         _ptr(pos), -1 if window is None else min(int(window), S), alibi.data_ptr(),
                                         B, S, H, Hk, D, float(scale), _stream()), "b200_attn_fwd_alibi")
@@ -727,7 +750,8 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
 
 
 def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
-                      window: Optional[int] = None, alibi: Optional[torch.Tensor] = None):
+                      window: Optional[int] = None, alibi: Optional[torch.Tensor] = None,
+                      prefix: Optional[torch.Tensor] = None):
     B, S, H, D = q.shape
     Hk = k.shape[2]
     dq = torch.empty_like(q)
@@ -736,7 +760,14 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
     dkv = torch.empty((B, S, 2 * Hk, D), device=k.device, dtype=k.dtype)
     dk, dv = dkv[:, :, :Hk], dkv[:, :, Hk:]
     tok = _t0("attn_bwd")
-    if alibi is not None:
+    if prefix is not None:
+        nbytes = int(lib().b200_attn_bwd_prefix_workspace_bytes(B, S, H, Hk, D))
+        ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
+        check(lib().b200_attn_bwd_prefix(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                         lse.data_ptr(), prefix.data_ptr(), dq.data_ptr(), dk.data_ptr(),
+                                         dv.data_ptr(), B, S, H, Hk, D, float(scale), 2 * Hk, ws.data_ptr(),
+                                         ws.numel(), _stream()), "b200_attn_bwd_prefix")
+    elif alibi is not None:
         nbytes = int(lib().b200_attn_bwd_window_workspace_bytes(B, S, H, Hk, D))
         ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
         check(lib().b200_attn_bwd_alibi(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
@@ -771,28 +802,28 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None):
+    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None, prefix=None):
         D = q.shape[-1]
         Dp = _pad_head_dim(D)
         if Dp != D:  # zero-padding the head dim leaves QK^T and the first D columns of PV unchanged
             q, k, v = (torch.nn.functional.pad(t, (0, Dp - D)) for t in (q, k, v))
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos, window, alibi)
-        ctx.save_for_backward(q, k, v, o, lse, pos, alibi)
+        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos, window, alibi, prefix)
+        ctx.save_for_backward(q, k, v, o, lse, pos, alibi, prefix)
         ctx.scale, ctx.causal, ctx.D, ctx.window = scale, causal, D, window
         return o[..., :D] if Dp != D else o
 
     @staticmethod
     def backward(ctx, do):
-        q, k, v, o, lse, pos, alibi = ctx.saved_tensors
+        q, k, v, o, lse, pos, alibi, prefix = ctx.saved_tensors
         Dp = q.shape[-1]
         if Dp != ctx.D:
             do = torch.nn.functional.pad(do, (0, Dp - ctx.D))
         do = do.contiguous()
-        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos, ctx.window, alibi)
+        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos, ctx.window, alibi, prefix)
         if Dp != ctx.D:
             dq, dk, dv = dq[..., :ctx.D], dk[..., :ctx.D], dv[..., :ctx.D]
-        return dq, dk, dv, None, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None, None
 
 
 def _hi_lo(x: torch.Tensor):
@@ -814,7 +845,7 @@ class _AttentionX3Fn(torch.autograd.Function):
     to fp32-like accuracy; P and the kernel outputs still pass through one bf16 rounding each."""
 
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None):
+    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None, prefix=None):
         D = q.shape[-1]
         Dp = _pad_head_dim(3 * D)
         (qh, ql), (kh, kl), (vh, vl) = _hi_lo(q), _hi_lo(k), _hi_lo(v)
@@ -823,32 +854,32 @@ class _AttentionX3Fn(torch.autograd.Function):
             t = torch.cat([a, b, c], dim=-1)
             return (torch.nn.functional.pad(t, (0, Dp - 3 * D)) if Dp != 3 * D else t).contiguous()
         q3, k3, v3 = cat3(qh, ql, qh), cat3(kh, kh, kl), cat3(vh, vh, vl)
-        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos, window, alibi)
-        ctx.save_for_backward(q3, k3, v3, o3, lse, pos, alibi)
+        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos, window, alibi, prefix)
+        ctx.save_for_backward(q3, k3, v3, o3, lse, pos, alibi, prefix)
         ctx.scale, ctx.causal, ctx.D, ctx.Dp, ctx.window = scale, causal, D, Dp, window
         return o3[..., :D].float() + o3[..., 2 * D:3 * D].float()
 
     @staticmethod
     def backward(ctx, do):
-        q3, k3, v3, o3, lse, pos, alibi = ctx.saved_tensors
+        q3, k3, v3, o3, lse, pos, alibi, prefix = ctx.saved_tensors
         D, Dp = ctx.D, ctx.Dp
         gh, gl = _hi_lo(do.float())
         g3 = torch.cat([gh, gl, gh], dim=-1)
         if Dp != 3 * D:
             g3 = torch.nn.functional.pad(g3, (0, Dp - 3 * D))
         dq3, dk3, dv3 = attention_bwd_raw(q3, k3, v3, o3, g3.contiguous(), lse, ctx.scale, ctx.causal, pos,
-                                          ctx.window, alibi)
+                                          ctx.window, alibi, prefix)
         dq = dq3[..., :D].float() + dq3[..., 2 * D:3 * D].float()
         dk = dk3[..., :D].float() + dk3[..., D:2 * D].float()
         dv = dv3[..., :D].float() + dv3[..., D:2 * D].float()
-        return dq, dk, dv, None, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None, None
 
 
 def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
                    causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None,
-                   alibi: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos, window, alibi: as
-    attention."""
+                   alibi: Optional[torch.Tensor] = None, prefix: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos, window, alibi,
+    prefix: as attention."""
     if 3 * q.shape[-1] > 128:
         raise ValueError("attention_fp32: head_dim must be <= 42 (three bf16 copies must fit a 128-wide tile)")
     if scale is None:
@@ -857,14 +888,17 @@ def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Opt
         pos, causal = _check_pos(pos, q, "attention_fp32"), True
     if window is not None:
         window, causal = _check_window(window, "attention_fp32"), True
+    if prefix is not None:
+        prefix = _check_prefix(prefix, q, causal, pos, window, alibi, "attention_fp32")
     if alibi is not None:
         alibi = _check_alibi(alibi, q, causal, "attention_fp32")
-    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos, window, alibi)
+    return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos, window, alibi,
+                                prefix)
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
               causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None,
-              alibi: Optional[torch.Tensor] = None) -> torch.Tensor:
+              alibi: Optional[torch.Tensor] = None, prefix: Optional[torch.Tensor] = None) -> torch.Tensor:
     """softmax(q k^T * scale + causal_mask) v with GQA head sharing; [B,S,H,D] layout, bf16.
 
     pos (int32 [B, S]) packs several documents per row: pos[b, s] is token s's position within its document (0 at a
@@ -877,16 +911,23 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional
 
     alibi (fp32 [H] slopes on q's device, one per query head; see arch.flash_attention.alibi_slopes) adds ALiBi's
     bias alibi[h] * (k - s) to the scaled score of query s and key k before the mask and the softmax.  k - s is also
-    the distance inside a document, so it composes with pos and window.  Causal only: causal=False raises."""
+    the distance inside a document, so it composes with pos and window.  Causal only: causal=False raises.
+
+    prefix (int32 [B] on q's device) is the prefix-LM mask: query s of row b sees key k iff k <= s or k < prefix[b],
+    so each row's prefix attends bidirectionally within itself and the rest of the row is causal.  prefix[b] <= 1 is
+    the causal mask and prefix[b] = S full attention; values outside [0, S] act as their clamps.  It implies causal
+    for the rest of the row and raises together with pos, window, alibi or causal=False."""
     if scale is None:
         scale = q.shape[-1] ** -0.5
+    if prefix is not None:
+        prefix = _check_prefix(prefix, q, causal, pos, window, alibi, "attention")
     if pos is not None:
         pos, causal = _check_pos(pos, q, "attention"), True
     if window is not None:
         window, causal = _check_window(window, "attention"), True
     if alibi is not None:
         alibi = _check_alibi(alibi, q, causal, "attention")
-    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos, window, alibi)
+    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos, window, alibi, prefix)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -5,7 +5,8 @@ has `model.misc.num_local_experts > 0`.
 The run's checkpoint holds the fp32 master weights under the trainer's flat names; they are renamed to the mlx-lm /
 HF names and written as fp32 `model.safetensors` next to `config.json`.  q / k weights are not permuted: the
 variant trains in the half-split RoPE layout HF Llama uses.  Runs whose exported config would describe a different
-function (the reference block, interleaved RoPE, a sliding window, ALiBi, logit_scale) are refused.  Runs on the CPU.
+function (the reference block, interleaved RoPE, a sliding window, ALiBi, prefix-LM, logit_scale) are refused.  Runs
+on the CPU.
 """
 from __future__ import annotations
 
@@ -72,6 +73,9 @@ def check_exportable(model_cfg) -> None:
         raise ValueError("rope.traditional: true (interleaved RoPE) has no LlamaForCausalLM config")
     if attn.get("sliding_window") is not None:
         raise ValueError("runs with model.attention.sliding_window cannot be exported as LlamaForCausalLM")
+    if attn.get("prefix_lm"):
+        raise ValueError("runs with model.attention.prefix_lm cannot be exported: LlamaForCausalLM and "
+                         "MixtralForCausalLM attend causally over the prompt")
     if attn.get("alibi"):
         raise ValueError("runs with model.attention.alibi cannot be exported: LlamaForCausalLM and "
                          "MixtralForCausalLM have no ALiBi")
