@@ -410,6 +410,25 @@ size_t b200_attn_bwd_prefix_workspace_bytes(int B, int S, int H, int Hk, int D);
 int b200_attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                          const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
                          float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
+/* Attention dropout (arch/flash_attention.py:146-148, arch/flex_attention.py:283-285 and 552-554,
+ * arch/simple_attention.py:152-154 of the reference: mx.dropout on the softmax weights before @ V):
+ * O = (P o Z / (1 - p_eff)) V with P the ordinary softmax (the LSE is the dropout-free one).  t = min(rint(p 65536),
+ * 65535), p_eff = t / 65536; element (b, h, q, k) is kept iff r >= t with r = (w[(k & 7) >> 1] >> 16 (k & 1)) &
+ * 0xffff of w = Philox4x32-10(counter (k >> 3, q, h, b), key (seed & 0xffffffff, seed >> 32)), b the row of the
+ * launch, h the query head, q and k absolute positions.  pos, window and slopes select the mask as in
+ * b200_attn_fwd_window / b200_attn_fwd_alibi (pos and slopes may be NULL, window < 0 means none; any of them needs
+ * causal = 1); with none of them, causal selects the causal or full mask.  p outside [0, 1) is rejected; t is
+ * rounded from the fp32 p received (ops.attention passes p_eff, so t is that of its double p).  The
+ * backward takes the same p and seed, b200_attn_bwd_strided's dk / dv rows and a workspace of
+ * b200_attn_bwd_dropout_workspace_bytes.  Decode never drops. */
+int b200_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                          const float* slopes, int B, int S, int H, int Hk, int D, float scale, int causal, float p,
+                          unsigned long long seed, void* stream);
+size_t b200_attn_bwd_dropout_workspace_bytes(int B, int S, int H, int Hk, int D);
+int b200_attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                          const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                          int H, int Hk, int D, float scale, int causal, float p, unsigned long long seed,
+                          int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- generation: decode attention over a KV cache (arch/flash_attention.py:97-156, last query row) ------------
  * One new query per sequence against its cached keys, causal by construction (every cached key precedes it):

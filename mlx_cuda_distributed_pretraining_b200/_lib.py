@@ -84,6 +84,11 @@ SIGNATURES = {
     "b200_attn_bwd_prefix_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "b200_attn_bwd_prefix": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp,
                                   _sz, _vp]),
+    "b200_attn_fwd_dropout": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _f, _i, _f, C.c_uint64,
+                                   _vp]),
+    "b200_attn_bwd_dropout_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
+    "b200_attn_bwd_dropout": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f,
+                                   _i, _f, C.c_uint64, _i, _vp, _sz, _vp]),
     "b200_attn_fwd_alibi": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_attn_bwd_alibi": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f,
                                  _i, _vp, _sz, _vp]),

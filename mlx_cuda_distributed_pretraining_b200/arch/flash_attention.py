@@ -106,19 +106,23 @@ class PrefixCausalMask:
 
 class FlashAttention(nn.Module):
     """alibi: add ALiBi's bias alibi_slopes(num_heads)[h] * (k - q) to every causal score (the slopes are not
-    parameters: a device tensor made on first use, like rope_tables)."""
+    parameters: a device tensor made on first use, like rope_tables).  dropout: the probability p of dropping an
+    attention weight after the softmax (arch/flash_attention.py:146-148 of the reference), applied only in training
+    mode with grad enabled; layer_idx (the layer's index in the model) derives the layer's mask seed from the
+    forward's dropout_seed."""
 
     def __init__(self, hidden_size: int, num_heads: int, num_kv_heads: Optional[int] = None,
                  head_dim: Optional[int] = None, dropout: float = 0.0, use_bias: bool = False,
-                 flash_block_size: int = 128, alibi: bool = False):
+                 flash_block_size: int = 128, alibi: bool = False, layer_idx: int = 0):
         super().__init__()
         self.hidden_size = hidden_size
         self.num_heads = num_heads
         self.num_kv_heads = num_kv_heads or num_heads
         self.head_dim = head_dim or (hidden_size // num_heads)
-        if dropout != 0.0:
-            raise ValueError("attention dropout is not supported by the fused kernel (reference default 0.0)")
-        self.dropout = dropout
+        if isinstance(dropout, bool) or not isinstance(dropout, (int, float)) or not 0.0 <= float(dropout) < 1.0:
+            raise ValueError(f"attention dropout must be a float in [0, 1), got {dropout!r}")
+        self.dropout = float(dropout)
+        self.layer_idx = int(layer_idx)
         self.flash_block_size = flash_block_size  # accepted for config compatibility (kernel tiles are 128)
         self.q_proj = nn.Linear(hidden_size, self.num_heads * self.head_dim, bias=use_bias)
         self.k_proj = nn.Linear(hidden_size, self.num_kv_heads * self.head_dim, bias=use_bias)
@@ -137,8 +141,15 @@ class FlashAttention(nn.Module):
             self._alibi_slopes = alibi_slopes(self.num_heads).to(device)
         return self._alibi_slopes
 
-    def _flash_attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask=None) -> torch.Tensor:
-        """q [B,S,H,D], k/v [B,S,Hk,D] -> [B,S,H,D]."""
+    def drops(self) -> bool:
+        """Whether a forward drops: p > 0, training mode and grad enabled (validation, prefill, decode and export
+        never drop)."""
+        return self.dropout > 0.0 and self.training and torch.is_grad_enabled()
+
+    def _flash_attention(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, mask=None,
+                         dropout_seed: Optional[int] = None, drop: bool = False) -> torch.Tensor:
+        """q [B,S,H,D], k/v [B,S,Hk,D] -> [B,S,H,D].  drop: apply self.dropout, with the layer's seed
+        ops.dropout_seed(dropout_seed, layer_idx) (dropout_seed None: a seed drawn by ops.attention)."""
         pos = window = prefix = None
         if mask is None:
             causal = False
@@ -154,19 +165,24 @@ class FlashAttention(nn.Module):
                 "packed rows (DocumentCausalMask) or the prefix-LM mask (PrefixCausalMask); arbitrary additive masks "
                 "are outside the reference's training path")
         alibi = self.alibi_slopes(q.device)
+        p = self.dropout if drop else 0.0
+        seed = None if not drop or dropout_seed is None else ops.dropout_seed(dropout_seed, self.layer_idx)
         dt = q.dtype
         if dt == torch.float32 and 3 * self.head_dim <= 128:
             # full-precision configs (mixed_precision: false, e.g. BASELINE C1, head_dim 16): logits through
             # three-term bf16 products (hi/lo split operands), ~fp32-accurate scores on the same kernels
             return ops.attention_fp32(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi,
-                                      prefix=prefix)
+                                      prefix=prefix, dropout=p, seed=seed)
         if dt != torch.bfloat16:  # larger head dims: bf16 operands with fp32 accumulation (stated in DESIGN.md)
             q, k, v = q.to(torch.bfloat16), k.to(torch.bfloat16), v.to(torch.bfloat16)
-        o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi, prefix=prefix)
+        o = ops.attention(q, k, v, self.scale, causal, pos=pos, window=window, alibi=alibi, prefix=prefix,
+                          dropout=p, seed=seed)
         return o if dt == torch.bfloat16 else o.to(dt)
 
-    def forward(self, x: torch.Tensor, mask=None, rope_layout: str = "interleaved") -> torch.Tensor:
-        """rope_layout: ops.rope's pair layout when RoPE is on ("interleaved" or mlx_lm's "half")."""
+    def forward(self, x: torch.Tensor, mask=None, rope_layout: str = "interleaved",
+                dropout_seed: Optional[int] = None) -> torch.Tensor:
+        """rope_layout: ops.rope's pair layout when RoPE is on ("interleaved" or mlx_lm's "half").  dropout_seed: the
+        model's per-step dropout base (see drops() for when it applies)."""
         B, S, _ = x.shape
         if self.q_proj.bias is None and self.k_proj.bias is None and self.v_proj.bias is None:
             q, k, v = ops.multi_linear(x, (self.q_proj.weight, self.k_proj.weight, self.v_proj.weight))
@@ -180,7 +196,9 @@ class FlashAttention(nn.Module):
             pos = mask.pos if isinstance(mask, DocumentCausalMask) else None  # packed rows: position in document
             q = ops.rope(q, cos_t[:S], sin_t[:S], pos, rope_layout)
             k = ops.rope(k, cos_t[:S], sin_t[:S], pos, rope_layout)
-        ctx = self._flash_attention(q, k, v, mask)
+        # the dropout arguments go only to dropping calls: without them the call is exactly the dropout-free one
+        ctx = (self._flash_attention(q, k, v, mask, dropout_seed, True) if self.drops()
+               else self._flash_attention(q, k, v, mask))
         ctx = ctx.reshape(B, S, self.num_heads * self.head_dim)
         return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
 

@@ -141,7 +141,7 @@ class AttentionModule(nn.Module):
                  rope_traditional: bool = False, rope_scaling: Optional[Dict[str, Any]] = None,
                  use_bias: bool = False, use_flash_attention: bool = True, use_flex_attention: bool = False,
                  flash_block_size: int = 128, apply_rope: bool = False, rope_layout: str = "interleaved",
-                 alibi: bool = False):
+                 alibi: bool = False, dropout: float = 0.0, layer_idx: int = 0):
         super().__init__()
         self.rope_layout = rope_layout
         if use_flex_attention:
@@ -152,16 +152,18 @@ class AttentionModule(nn.Module):
         self.head_dim = head_dim or (hidden_size // num_heads)
         # SimpleAttention (use_flash_attention=False) computes the same function; one kernel serves both
         self.attn = FlashAttention(hidden_size, num_heads, self.num_kv_heads, self.head_dim,
-                                   use_bias=use_bias, flash_block_size=flash_block_size, alibi=alibi)
+                                   dropout=dropout, use_bias=use_bias, flash_block_size=flash_block_size, alibi=alibi,
+                                   layer_idx=layer_idx)
         self.scale = self.head_dim ** -0.5
         self.apply_rope = apply_rope
         self.max_positions = max_positions
         self.rope_theta = rope_theta
 
-    def forward(self, x: torch.Tensor, mask=None, position_ids=None) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, mask=None, position_ids=None,
+                dropout_seed: Optional[int] = None) -> torch.Tensor:
         if self.apply_rope and self.attn.rope_tables is None:
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
-        return self.attn(x, mask=mask, rope_layout=self.rope_layout)
+        return self.attn(x, mask=mask, rope_layout=self.rope_layout, dropout_seed=dropout_seed)
 
     def cached(self, x: torch.Tensor, cache: "KVCache", layer: int, window: Optional[int] = None,
                prefix: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -178,7 +180,7 @@ class AttentionModule(nn.Module):
 
 
 class TransformerBlock(nn.Module):
-    def __init__(self, args: ModelArgs):
+    def __init__(self, args: ModelArgs, layer_idx: int = 0):
         super().__init__()
         inter = args.intermediate_size or 4 * args.hidden_size
         if args.variant not in VARIANTS:
@@ -193,7 +195,8 @@ class TransformerBlock(nn.Module):
             use_bias=args.attention_bias, use_flash_attention=args.use_flash_attention,
             use_flex_attention=args.use_flex_attention, flash_block_size=args.flash_block_size,
             apply_rope=args.apply_rope or mlx_lm,
-            rope_layout="half" if mlx_lm and not args.rope_traditional else "interleaved", alibi=args.alibi)
+            rope_layout="half" if mlx_lm and not args.rope_traditional else "interleaved", alibi=args.alibi,
+            dropout=args.attention_dropout, layer_idx=layer_idx)
         self.post_attention_layernorm = RMSNorm(args.hidden_size, eps=args.rms_norm_eps)
         act = "silu" if mlx_lm else "sigmoid2"
         self.moe = bool(args.num_local_experts)
@@ -215,7 +218,7 @@ class TransformerBlock(nn.Module):
         return x + self._ffn(self.post_attention_layernorm(x))
 
     def forward_fused(self, h: torch.Tensor, pending, mask=None, position_ids=None, token_mask=None,
-                      aux: bool = False):
+                      aux: bool = False, dropout_seed: Optional[int] = None):
         """Same block with every residual add fused into the norm that consumes it.  `pending` is the
         previous block's MLP output not yet added to the stream h (None for the first block); returns
         (h after the attention residual, this block's MLP output still to be added)."""
@@ -224,7 +227,7 @@ class TransformerBlock(nn.Module):
             y = n1(h)
         else:
             h, y = ops.add_rmsnorm(h, pending, n1.weight, n1.eps)
-        a = self.self_attn(y, mask=mask, position_ids=position_ids)
+        a = self.self_attn(y, mask=mask, position_ids=position_ids, dropout_seed=dropout_seed)
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
         return h, self._ffn(y, token_mask, aux)
 
@@ -279,7 +282,7 @@ class Model(nn.Module):
         self.args = args
         self.vocab_size = args.vocab_size
         self.embed_tokens = nn.Embedding(args.vocab_size, args.hidden_size)
-        self.layers = nn.ModuleList([TransformerBlock(args) for _ in range(args.num_hidden_layers)])
+        self.layers = nn.ModuleList([TransformerBlock(args, i) for i in range(args.num_hidden_layers)])
         self.norm = RMSNorm(args.hidden_size, eps=args.rms_norm_eps)
         self.logit_scale = args.logit_scale
         self._tied_w = None  # padded alias of the embedding for the logits GEMM (set lazily)
@@ -287,14 +290,17 @@ class Model(nn.Module):
 
     def hidden_states(self, inputs: torch.Tensor, position_ids=None, attention_mask=None,
                       token_mask: Optional[torch.Tensor] = None,
-                      prefix_lens: Optional[torch.Tensor] = None) -> torch.Tensor:
+                      prefix_lens: Optional[torch.Tensor] = None,
+                      dropout_seed: Optional[int] = None) -> torch.Tensor:
         """position_ids (int [B, S], optional): packed rows, each token's position within its document (0 at the
         document's first token).  It selects the document-causal mask and, with RoPE on, the rotation angles, so
         every document is computed as if it ran alone.  None keeps the causal mask over whole rows.  Both masks carry
         args.sliding_window.  token_mask (bool [B, S], optional; MoE models): the tokens the load-balancing loss
         counts; given, every MoE layer keeps its partials for moe_aux_loss().  prefix_lens (int32 [B] on the device,
         optional): prefix-LM rows, query q of row b sees key k iff k <= q or k < prefix_lens[b] (PrefixCausalMask);
-        it does not combine with position_ids or a sliding window."""
+        it does not combine with position_ids or a sliding window.  dropout_seed (an int in [0, 2^64), optional): the
+        base of the attention-dropout masks when args.attention_dropout > 0 and the model trains with grad enabled;
+        layer i draws with ops.dropout_seed(dropout_seed, i).  None draws fresh seeds from torch's CPU generator."""
         B, S = inputs.shape
         if prefix_lens is not None:
             if position_ids is not None or attention_mask is not None:
@@ -319,10 +325,11 @@ class Model(nn.Module):
             self._moe_tokens = token_mask.sum() if aux else None
             for layer in self.layers:
                 h, pending = layer.forward_fused(h, pending, mask=mask, position_ids=position_ids,
-                                                 token_mask=token_mask, aux=aux)
+                                                 token_mask=token_mask, aux=aux, dropout_seed=dropout_seed)
         else:
             for layer in self.layers:
-                h, pending = layer.forward_fused(h, pending, mask=mask, position_ids=position_ids)
+                h, pending = layer.forward_fused(h, pending, mask=mask, position_ids=position_ids,
+                                                 dropout_seed=dropout_seed)
         if pending is None:
             return self.norm(h)
         return ops.add_rmsnorm(h, pending, self.norm.weight, self.norm.eps)[1]
@@ -353,7 +360,8 @@ class Model(nn.Module):
             return self._tied_w
         return self.embed_tokens.weight
 
-    def padded_logits(self, inputs: torch.Tensor, position_ids=None, token_mask=None, prefix_lens=None):
+    def padded_logits(self, inputs: torch.Tensor, position_ids=None, token_mask=None, prefix_lens=None,
+                      dropout_seed=None):
         """(logits [B*S, ld], V) with ld >= V, ld % 8 == 0 when the fused cross-entropy can take them
         (bf16 weights, tied + row-padded embedding alias or an aligned vocabulary); else (None, V).
         Eligibility is decided BEFORE the forward pass, so an ineligible config (fp32, logit_scale,
@@ -363,13 +371,14 @@ class Model(nn.Module):
         w = self._logits_weight()
         if w.shape[0] % 8 != 0 or w.dtype != torch.bfloat16:
             return None, self.vocab_size
-        h = self.hidden_states(inputs, position_ids, token_mask=token_mask, prefix_lens=prefix_lens)
+        h = self.hidden_states(inputs, position_ids, token_mask=token_mask, prefix_lens=prefix_lens,
+                               dropout_seed=dropout_seed)
         logits = torch.nn.functional.linear(h, w)
         return logits.view(-1, logits.shape[-1]), self.vocab_size
 
     def forward(self, inputs: torch.Tensor, position_ids=None, attention_mask=None, token_mask=None,
-                prefix_lens=None) -> torch.Tensor:
-        h = self.hidden_states(inputs, position_ids, attention_mask, token_mask, prefix_lens)
+                prefix_lens=None, dropout_seed=None) -> torch.Tensor:
+        h = self.hidden_states(inputs, position_ids, attention_mask, token_mask, prefix_lens, dropout_seed)
         logits = torch.nn.functional.linear(h, self._logits_weight())[..., :self.vocab_size]
         if self.logit_scale is not None:
             logits = logits * self.logit_scale

@@ -82,6 +82,13 @@ class ModelConfig:
                 raise ValueError("model.attention.prefix_lm does not combine with model.attention.sliding_window")
             if a:
                 raise ValueError("model.attention.prefix_lm does not combine with model.attention.alibi")
+        # extension: attention.dropout p (absent / null / 0: off); drops attention weights after the softmax in
+        # training (arch/flash_attention.py:146-148 of the reference)
+        d = self.attention.get("dropout")
+        if d is not None and (isinstance(d, bool) or not isinstance(d, (int, float)) or not 0.0 <= d < 1.0):
+            raise ValueError(f"model.attention.dropout must be null or a number in [0, 1), got {d!r}")
+        if d and pl:
+            raise ValueError("model.attention.dropout does not combine with model.attention.prefix_lm")
         # extension: misc.variant selects the block (absent / null / "reference": arch/llama.py's; "mlx_lm": the
         # mlx_lm.models.llama block the reference's trainer actually imports, DESIGN D4)
         v = (self.misc or {}).get("variant")
@@ -805,6 +812,7 @@ class Trainer:
             apply_rope=bool(m.rope.get("enabled", m.architecture == "llama_standard")) or m.misc.get("variant") == "mlx_lm",
             sliding_window=m.attention.get("sliding_window"), alibi=bool(m.attention.get("alibi")),
             prefix_lm=bool(m.attention.get("prefix_lm")), variant=m.misc.get("variant"),
+            attention_dropout=float(m.attention.get("dropout") or 0.0),
             num_local_experts=m.misc.get("num_local_experts") or 0,
             num_experts_per_tok=m.misc.get("num_experts_per_tok") or 0,
             router_aux_loss_coef=float(m.misc.get("router_aux_loss_coef", 0.001)))
@@ -864,21 +872,22 @@ class Trainer:
 
     # -- loss --------------------------------------------------------------------------------------
     def compute_loss(self, model, inputs: torch.Tensor, targets: torch.Tensor, packed: bool = False,
-                     aux: bool = True, prefix: Optional[torch.Tensor] = None):
+                     aux: bool = True, prefix: Optional[torch.Tensor] = None, dropout_seed: Optional[int] = None):
         """Masked token-mean cross-entropy.  packed: the rows hold several documents (DataManager with
         pack_sequences); the model then attends within documents (position_ids from the BOS tokens), and the one
         target per document boundary that an unpacked row never has -- a document's last token predicting the
         next document's BOS -- becomes PAD, so the loss terms and ntoks are those of the documents run alone.
         prefix (int [B] on the device): prefix-LM rows; the model attends with PrefixCausalMask and the targets a
-        prefix position can see become PAD (prefix_targets)."""
+        prefix position can see become PAD (prefix_targets).  dropout_seed: the attention-dropout base of this
+        micro-step (used only when the model drops: attention dropout on, training mode, grad enabled)."""
         max_ctx = self.config.model.attention.get("max_position_embeddings", 2048)
         if inputs.shape[1] > max_ctx:
             inputs, targets = inputs[:, :max_ctx], targets[:, :max_ctx]
         position_ids = None
-        kw = {}
+        kw = {} if dropout_seed is None else {"dropout_seed": dropout_seed}
         if prefix is not None:
             targets = prefix_targets(targets, prefix, self.tokenizer.PAD_TOKEN)
-            kw = {"prefix_lens": prefix.to(torch.int32)}
+            kw["prefix_lens"] = prefix.to(torch.int32)
         if packed:
             position_ids = document_positions(inputs, self.tokenizer.BOS_TOKEN)
             targets = targets.masked_fill(targets == self.tokenizer.BOS_TOKEN, self.tokenizer.PAD_TOKEN)
@@ -959,8 +968,14 @@ class Trainer:
         prefix = None
         if self.model_args.prefix_lm:  # column 0 holds each row's prefix length
             prefix, dev_batch = dev_batch[:, 0], dev_batch[:, 1:]
+        # attention dropout's per-micro-step base: a function of (system.seed, rank, step) only, so a resumed run
+        # draws the masks of the uninterrupted one and the ranks draw different masks
+        seed = None
+        if self.model_args.attention_dropout > 0:
+            seed = ops.dropout_seed(self.config.system.seed, self.rank, step)
         loss, ntoks = self.compute_loss(self.model, dev_batch[:, :-1], dev_batch[:, 1:],
-                                        packed=getattr(self.data_manager, "pack", False), prefix=prefix)
+                                        packed=getattr(self.data_manager, "pack", False), prefix=prefix,
+                                        dropout_seed=seed)
         aux = getattr(self, "last_aux_loss", None)
         if aux is None:
             loss.backward()

@@ -50,6 +50,17 @@
 // max(q0, P_b - 1) or it crosses S, and the element mask is `key > q && key >= P_b` plus the bounds.  The pre-pass is
 // unchanged.  Prefix launches use the unpaired order: the causal pairing no longer balances the work.  P_b <= 1 gives
 // the causal kernel's items and values.  PREFIX = false compiles unchanged.
+//
+// Dropout (DROP = true, on the causal / non-causal and the DOC / ALiBi kernels): the adjoint of the forward's
+// O = (P o Z / (1 - p_eff)) V, with Z regenerated from (seed, b, h, q, k) by the forward's Philox rule (nothing of size
+// S^2 is stored): dV = (P o Z)^T dO / (1 - p_eff) and dS = P o (Z o dP / (1 - p_eff) - delta), where delta =
+// rowsum(dO o O) of the dropped O, so the pre-pass is unchanged.  P^T stays the dropout-free softmax for dS; the bf16
+// P^T fed to the dV MMA has the dropped entries zeroed, dV gets the scale in fp32 at the store, and dS gets it on dP in
+// registers (dS = P (dP zs - delta) with zs the scale or 0; the packed P^T halves are masked after packing, which
+// keeps the D = 128 document kernel's masked-item path free of spills).  A thread's element (nc, e) is query
+// q0 + 8 nc + cq + (e & 1) against key key_a + 8 (e >> 1): the 8 lanes g = 0..7 of one cq share one Philox call per (query, 8-key chunk) and take bit g of it.  Lane g computes the
+// 4 calls of its group's elements (nc = g, e = 0..3) and the group exchanges them with 8 shuffles, so bit 4 nc + e of
+// zk is element (nc, e)'s keep bit.  DROP = false compiles unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -100,6 +111,9 @@ struct BwdArgs {
   const int* qt_end;   // DOC: [B,n_kt] end of each key tile's query-tile range
   const float* slopes; // ALIBI: [H] fp32 per-query-head slopes
   const int* prefix;   // PREFIX: [B] int32 prefix lengths (clamped to [0, S])
+  uint32_t drop_t;     // DROP: keep threshold t = round(p 65536) on the 16-bit Philox values
+  float drop_inv;      // DROP: 1 / (1 - t / 65536)
+  unsigned long long drop_seed;  // DROP: Philox key
 };
 
 // PREFIX: batch row b's prefix length
@@ -138,12 +152,32 @@ __device__ __forceinline__ void rs_mma(float* acc, const uint32_t* a, uint64_t d
   else wgmma_m64n64k16_rs<1>(acc, a, db);
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
+// DROP: keep bits of a consumer thread's 32 elements of the item (query head h, queries from q0, keys from kbase =
+// the warp's first key): bit 4 nc + e for query q0 + 8 nc + cq + (e & 1) and key kbase + g + 8 (e >> 1)
+__device__ __forceinline__ uint32_t drop_keep_bits(const BwdArgs& p, int kbase, int q0, int h, int b, int lane) {
+  const int g = lane >> 2, cq = (lane & 3) * 2;
+  const uint32_t sk0 = (uint32_t)p.drop_seed, sk1 = (uint32_t)(p.drop_seed >> 32);
+  uint32_t own = 0u;  // byte j: the call of element (nc = g, e = j), bit i for key 8 (kbase / 8 + (j >> 1)) + i
+#pragma unroll 1
+  for (int j = 0; j < 4; ++j)
+    own |= philox_keep8((uint32_t)(kbase >> 3) + (j >> 1), q0 + 8 * g + cq + (j & 1), h, b, sk0, sk1, p.drop_t)
+           << (8 * j);
+  uint32_t zk = 0u;
+#pragma unroll
+  for (int m = 0; m < 8; ++m) {  // from lane g ^ m of the group (xor shuffles need no lane-index registers)
+    const uint32_t x = (__shfl_xor_sync(0xffffffffu, own, 4 * m) >> g) & 0x01010101u;
+    zk |= ((x | (x >> 7) | (x >> 14) | (x >> 21)) & 0xfu) << (4 * (g ^ m));
+  }
+  return zk;
+}
+
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmDO,
                 const __grid_constant__ CUtensorMap tmDQ, const BwdArgs p) {
   static_assert(!PREFIX || (!DOC && !ALIBI), "the prefix mask is built on the causal kernel");
+  static_assert(!PREFIX || !DROP, "dropout is not built on the prefix kernels");
   using Cfg = BwdCfg<D, DOC>;
   constexpr int ST = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -252,6 +286,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
     for (int j = 0; j < t.n_items; ++j, ++it) {
       const int q0 = (t.qt0 + j % t.per_head) * BQ;
+      // DROP: the item's keep bits, made before the wait for its Q / dO, where only dK and dV are live (with the S^T
+      // and dP^T fragments live D = 128 spills, and between the MMAs' commit and wait ptxas injects a
+      // warpgroup.arrive)
+      uint32_t zk = 0u;
+      if constexpr (DROP) zk = drop_keep_bits(p, t.k0 + c * 64 + wq * 16, q0, hk * group + j / t.per_head, b, lane);
       mbar_wait_outlined(q_full0 + 8 * slot, phase);
       const uint32_t tQ = sQ + slot * Cfg::QS_BYTES, tDO = sDO + slot * Cfg::QS_BYTES;
       const uint32_t tL = sL + slot * Cfg::L_BYTES, tDlt = tL + BQ * 4;  // LSE*log2e, delta of the 64 queries
@@ -326,7 +365,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             else
               pv = ok ? exp2f(st[4 * nc + e] * sl2 - lds32f(tL + qc * 4)) : 0.f;
             st[4 * nc + e] = pv;
-            dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] - lds32f(tDlt + qc * 4)) : 0.f;
+            if constexpr (DROP) {
+              const float zs = (zk >> (4 * nc + e)) & 1u ? p.drop_inv : 0.f;
+              dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] * zs - lds32f(tDlt + qc * 4)) : 0.f;
+            } else {
+              dpt[4 * nc + e] = ok ? pv * (dpt[4 * nc + e] - lds32f(tDlt + qc * 4)) : 0.f;
+            }
           }
         }
       } else {
@@ -343,7 +387,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
             else
               pv = exp2f(st[4 * nc + e] * sl2 - ((e & 1) ? l.y : l.x));
             st[4 * nc + e] = pv;
-            dpt[4 * nc + e] = pv * (dpt[4 * nc + e] - ((e & 1) ? d.y : d.x));
+            if constexpr (DROP) {
+              const float zs = (zk >> (4 * nc + e)) & 1u ? p.drop_inv : 0.f;
+              dpt[4 * nc + e] = pv * (dpt[4 * nc + e] * zs - ((e & 1) ? d.y : d.x));
+            } else {
+              dpt[4 * nc + e] = pv * (dpt[4 * nc + e] - ((e & 1) ? d.y : d.x));
+            }
           }
         }
       }
@@ -354,6 +403,17 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         for (int i = 0; i < 4; ++i) {
           pa[kk][i] = pack_bf16x2(st[8 * kk + 2 * i], st[8 * kk + 2 * i + 1]);
           da[kk][i] = pack_bf16x2(dpt[8 * kk + 2 * i], dpt[8 * kk + 2 * i + 1]);
+        }
+      }
+      // DROP: P^T for dV with the dropped bf16 halves zeroed (elements 8 kk + 2 i + {0, 1} of pa[kk][i])
+      if constexpr (DROP) {
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const uint32_t x = zk >> (8 * kk + 2 * i);
+            pa[kk][i] &= (x & 1u) * 0xffffu | ((x >> 1) & 1u) * 0xffff0000u;
+          }
         }
       }
       // dS^T rows of this thread -> [key][64 queries] tile, 128 B per row, 16-byte chunks XOR (row % 8)
@@ -431,7 +491,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     // every read of this tile's K / V has completed (the last dQ wgmma was waited for)
     if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty);
 
-    // dK (scale applied here), dV -> bf16 rows of dkv_rh heads
+    // dK (scale applied here), dV (DROP: with the dropout scale) -> bf16 rows of dkv_rh heads
+    const float dv_mul = DROP ? p.drop_inv : 1.f;
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       const int key = key_a + 8 * r;
@@ -441,7 +502,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int dc = 0; dc < D / 8; ++dc) {
         *reinterpret_cast<uint32_t*>(p.dk + off + dc * 8) =
             pack_bf16x2(dk[4 * dc + 2 * r] * p.scale, dk[4 * dc + 2 * r + 1] * p.scale);
-        *reinterpret_cast<uint32_t*>(p.dv + off + dc * 8) = pack_bf16x2(dv[4 * dc + 2 * r], dv[4 * dc + 2 * r + 1]);
+        if constexpr (DROP)
+          *reinterpret_cast<uint32_t*>(p.dv + off + dc * 8) =
+              pack_bf16x2(dv[4 * dc + 2 * r] * dv_mul, dv[4 * dc + 2 * r + 1] * dv_mul);
+        else
+          *reinterpret_cast<uint32_t*>(p.dv + off + dc * 8) = pack_bf16x2(dv[4 * dc + 2 * r], dv[4 * dc + 2 * r + 1]);
       }
     }
   }
@@ -527,11 +592,11 @@ f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ ds
   }
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false>
 int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmDO,
                const CUtensorMap& tmDQ, const BwdArgs& a, cudaStream_t stream) {
   using Cfg = BwdCfg<D, DOC>;
-  auto kern = attn_bwd_kernel<D, DOC, ALIBI, PREFIX>;
+  auto kern = attn_bwd_kernel<D, DOC, ALIBI, PREFIX, DROP>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -571,11 +636,12 @@ size_t attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
 namespace {
 
 // doc selects the document / window kernels; window < 0 means none; slopes (doc only) selects ALiBi; prefix (causal,
-// not doc) selects the prefix-LM kernels
+// not doc) selects the prefix-LM kernels; drop selects the dropout kernels (not with prefix)
 int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                   bool doc, const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk,
                   int D, float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream,
-                  const float* slopes = nullptr, const int* prefix = nullptr) {
+                  const float* slopes = nullptr, const int* prefix = nullptr, bool drop = false,
+                  uint32_t drop_t = 0, float drop_inv = 1.f, unsigned long long drop_seed = 0) {
   // dk / dv rows may be strided: dkv_row_heads heads per token row (0 = Hk, i.e. contiguous [B,S,Hk,D]).
   // With dk = base, dv = base + Hk*D and dkv_row_heads = 2*Hk both land in ONE [B,S,2*Hk*D] buffer, which lets
   // the k/v projections' dgrad and wgrad run as single GEMMs over the concatenated weight.
@@ -636,7 +702,19 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
   a.qt_end = doc ? qt_end : nullptr;
   a.slopes = slopes;
   a.prefix = prefix;
-  if (prefix)
+  a.drop_t = drop_t;
+  a.drop_inv = drop_inv;
+  a.drop_seed = drop_seed;
+  if (drop && slopes)
+    rc = D == 64 ? launch_bwd<64, true, true, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+                 : launch_bwd<128, true, true, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
+  else if (drop && doc)
+    rc = D == 64 ? launch_bwd<64, true, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+                 : launch_bwd<128, true, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
+  else if (drop)
+    rc = D == 64 ? launch_bwd<64, false, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
+                 : launch_bwd<128, false, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
+  else if (prefix)
     rc = D == 64 ? launch_bwd<64, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream)
                  : launch_bwd<128, false, false, true>(tmQ, tmK, tmV, tmDO, tmDQ, a, stream);
   else if (slopes)
@@ -710,6 +788,27 @@ int attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, 
                  "attn_bwd_prefix: prefix must be a non-null, 4-byte aligned int32 [B] array");
   return attn_bwd_impl(q, k, v, o, d_o, lse, false, nullptr, -1, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
                        ws, ws_bytes, stream, nullptr, prefix);
+}
+
+// dropout backward: the causal / non-causal (pos == nullptr, window < 0, slopes == nullptr), document / window or
+// ALiBi backward of attn_fwd_dropout's O = (P o Z / (1 - p_eff)) V, the same p and seed.  Workspace: the document
+// variant's when pos, window or slopes select the DOC kernels, else the causal one's.
+size_t attn_bwd_dropout_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return attn_bwd_doc_workspace_bytes(B, S, H, Hk, D);
+}
+
+int attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                     const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                     int H, int Hk, int D, float scale, int causal, float p, unsigned long long seed,
+                     int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+  B200_CHECK_ARG(p >= 0.f && p < 1.f, "attn_bwd_dropout: p=%g must lie in [0, 1)", (double)p);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_bwd_dropout: pos must be 4-byte aligned int32");
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0, "attn_bwd_dropout: slopes must be 4-byte aligned");
+  const bool doc = pos != nullptr || window >= 0 || slopes != nullptr;
+  B200_CHECK_ARG(!doc || causal, "attn_bwd_dropout: pos, window and slopes need causal=1");
+  const uint32_t t = dropout_threshold(p);
+  return attn_bwd_impl(q, k, v, o, d_o, lse, doc, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, doc ? 1 : causal,
+                       dkv_row_heads, ws, ws_bytes, stream, slopes, nullptr, true, t, dropout_scale(t), seed);
 }
 
 }  // namespace b200

@@ -37,6 +37,17 @@
 // max(causal end, ceil(P_b / 128)) and the element mask `key >= S || (key > row && key >= P_b)` runs only on tiles
 // whose last key exceeds max(q0, P_b - 1) or that cross S.  P_b <= 1 is the causal mask (the same tiles, the same
 // values); P_b = S is the non-causal one.  PREFIX = false compiles to the kernels above unchanged.
+//
+// Dropout (DROP = true, on the causal / non-causal and the DOC / ALiBi kernels): O = (P o Z / (1 - p_eff)) V as
+// arch/flash_attention.py:146-148 of the reference applies mx.dropout after the softmax.  The softmax P, its row sums
+// and the LSE are the dropout-free ones; only the bf16 P fed to the P V MMA has dropped entries zeroed, and O is
+// multiplied by 1 / (1 - p_eff) in fp32 after the normalisation.  Z(b, h, q, k) = [r >= t] with r the 16-bit value
+// of key k in Philox4x32-10(counter (k >> 3, q, h, b), key (seed lo, seed hi)) (philox_keep8), h the query head: the
+// mask depends on positions only, never on the tiling.  A quad's rows are one (row, 8-key chunk) Philox call per
+// chunk nc, whose word w[l] holds exactly lane l's keys 8 nc + 2 l + {0, 1}; so each lane computes 8 of the tile's
+// 32 calls (both rows, chunks nc = 4 m + l) and the quad exchanges the 8-bit results with 4 shuffles per row.  Bit
+// 2 nc + c of keep[r] is this thread's key 8 nc + 2 l + c of row r.  DROP = false compiles to the kernels above
+// unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -71,6 +82,9 @@ struct FwdArgs {
   int window;      // DOC: query q sees keys from q - min(pos[q], window); S when there is no window
   const float* slopes;  // ALIBI: [H] fp32 per-query-head slopes
   const int* prefix;    // PREFIX: [B] int32 prefix lengths (clamped to [0, S])
+  uint32_t drop_t;      // DROP: keep threshold t = round(p 65536) on the 16-bit Philox values
+  float drop_inv;       // DROP: 1 / (1 - t / 65536)
+  unsigned long long drop_seed;  // DROP: Philox key
 };
 
 // first key query `row` of batch row b may see: its document start, or its window start when that is later
@@ -80,17 +94,38 @@ __device__ __forceinline__ int key_start(const FwdArgs& p, int b, int row) {
   return p.pos ? row - min(__ldg(p.pos + (long long)b * p.S + row), p.window) : max(0, row - p.window);
 }
 
+// DROP: keep bits of a thread's 2 x 32 scores in the key tile from k0 (rows row_a, row_a + 8).  Byte m of lane L's
+// `own` is chunk 4 m + L of row r; this lane takes bits 2 (lane % 4) + {0, 1} of every byte.
+__device__ __forceinline__ void drop_keep_bits(const FwdArgs& p, int k0, int row_a, int h, int b, int lane,
+                                               uint32_t* keep) {
+  const uint32_t kc = (uint32_t)(k0 >> 3) + (lane & 3);
+  const uint32_t sk0 = (uint32_t)p.drop_seed, sk1 = (uint32_t)(p.drop_seed >> 32);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    uint32_t own = 0u;
+#pragma unroll 1
+    for (int m = 0; m < 4; ++m) own |= philox_keep8(kc + 4 * m, row_a + 8 * r, h, b, sk0, sk1, p.drop_t) << (8 * m);
+    keep[r] = 0u;
+#pragma unroll
+    for (int L = 0; L < 4; ++L) {
+      const uint32_t w = __shfl_sync(0xffffffffu, own, L, 4);
+      keep[r] |= ((w >> (2 * (lane & 3))) & 0x03030303u) << (2 * L);
+    }
+  }
+}
+
 template <int D>
 __device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db) {
   if constexpr (D == 128) wgmma_m64n128k16_rs<1>(o, a, db);
   else wgmma_m64n64k16_rs<1>(o, a, db);
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdArgs p) {
   static_assert(!PREFIX || (!DOC && !ALIBI), "the prefix mask is built on the causal kernel");
+  static_assert(!PREFIX || !DROP, "dropout is not built on the prefix kernels");
   using Cfg = FwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -282,6 +317,21 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       pa[kk][2] = pack_bf16x2(sc[8 * kk + 4], sc[8 * kk + 5]);
       pa[kk][3] = pack_bf16x2(sc[8 * kk + 6], sc[8 * kk + 7]);
     }
+    // DROP: zero the dropped bf16 halves of P (the row sums above keep every visible key).  The keep bits are made
+    // here, where the S fragment is dead: live across the S MMAs or the softmax they push D = 128 into spills.
+    // pa[kk][i] holds chunk 2 kk + (i >> 1) of row i & 1.
+    if constexpr (DROP) {
+      uint32_t keep[2];
+      drop_keep_bits(p, k0, row_a, h, b, lane, keep);
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const uint32_t x = keep[i & 1] >> (4 * kk + 2 * (i >> 1));
+          pa[kk][i] &= (x & 1u) * 0xffffu | ((x >> 1) & 1u) * 0xffff0000u;
+        }
+      }
+    }
 #pragma unroll
     for (int dc = 0; dc < D / 8; ++dc) {
       o[4 * dc + 0] *= alpha[0];
@@ -305,7 +355,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 1);
     l_r[r] += __shfl_xor_sync(0xffffffffu, l_r[r], 2);
   }
-  const float inv[2] = {1.0f / l_r[0], 1.0f / l_r[1]};
+  // DROP: the normaliser carries the fp32 dropout scale 1 / (1 - p_eff)
+  const float inv[2] = {(DROP ? p.drop_inv : 1.0f) / l_r[0], (DROP ? p.drop_inv : 1.0f) / l_r[1]};
   const long long q_stride = (long long)p.H * D;
   __nv_bfloat16* ob = p.o + (long long)b * p.S * q_stride + (long long)h * D;
 #pragma unroll
@@ -321,11 +372,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false>
 int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
                cudaStream_t stream) {
   using Cfg = FwdCfg<D>;
-  auto kern = attn_fwd_kernel<D, DOC, ALIBI, PREFIX>;
+  auto kern = attn_fwd_kernel<D, DOC, ALIBI, PREFIX, DROP>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -350,10 +401,11 @@ int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, in
 namespace {
 
 // doc selects the document / window instantiation; window < 0 means none; slopes (doc only) selects ALiBi; prefix
-// (causal, not doc) selects the prefix-LM kernels
+// (causal, not doc) selects the prefix-LM kernels; drop selects the dropout kernels (not with prefix)
 int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, bool doc, const int* pos,
                   int window, int B, int S, int H, int Hk, int D, float scale, int causal, cudaStream_t stream,
-                  const float* slopes = nullptr, const int* prefix = nullptr) {
+                  const float* slopes = nullptr, const int* prefix = nullptr, bool drop = false,
+                  uint32_t drop_t = 0, float drop_inv = 1.f, unsigned long long drop_seed = 0) {
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_fwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd: head_dim %d unsupported (64 or 128; pad smaller dims)", D);
@@ -376,6 +428,19 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   a.window = window < 0 || window > S ? S : window;
   a.slopes = slopes;
   a.prefix = prefix;
+  a.drop_t = drop_t;
+  a.drop_inv = drop_inv;
+  a.drop_seed = drop_seed;
+  if (drop) {
+    if (slopes)
+      return D == 64 ? launch_fwd<64, true, true, false, true>(tmQ, tmK, tmV, a, stream)
+                     : launch_fwd<128, true, true, false, true>(tmQ, tmK, tmV, a, stream);
+    if (doc)
+      return D == 64 ? launch_fwd<64, true, false, false, true>(tmQ, tmK, tmV, a, stream)
+                     : launch_fwd<128, true, false, false, true>(tmQ, tmK, tmV, a, stream);
+    return D == 64 ? launch_fwd<64, false, false, false, true>(tmQ, tmK, tmV, a, stream)
+                   : launch_fwd<128, false, false, false, true>(tmQ, tmK, tmV, a, stream);
+  }
   if (prefix)
     return D == 64 ? launch_fwd<64, false, false, true>(tmQ, tmK, tmV, a, stream)
                    : launch_fwd<128, false, false, true>(tmQ, tmK, tmV, a, stream);
@@ -424,6 +489,21 @@ int attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float*
   B200_CHECK_ARG(prefix != nullptr && (reinterpret_cast<uintptr_t>(prefix) & 3u) == 0,
                  "attn_fwd_prefix: prefix must be a non-null, 4-byte aligned int32 [B] array");
   return attn_fwd_impl(q, k, v, o, lse, false, nullptr, -1, B, S, H, Hk, D, scale, 1, stream, nullptr, prefix);
+}
+
+// dropout: the causal / non-causal (pos == nullptr, window < 0, slopes == nullptr), document / window or ALiBi
+// forward with O = (P o Z / (1 - p_eff)) V; t = min(rint(p 65536), 65535), p_eff = t / 65536
+int attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                     const float* slopes, int B, int S, int H, int Hk, int D, float scale, int causal, float p,
+                     unsigned long long seed, cudaStream_t stream) {
+  B200_CHECK_ARG(p >= 0.f && p < 1.f, "attn_fwd_dropout: p=%g must lie in [0, 1)", (double)p);
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_fwd_dropout: pos must be 4-byte aligned int32");
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0, "attn_fwd_dropout: slopes must be 4-byte aligned");
+  const bool doc = pos != nullptr || window >= 0 || slopes != nullptr;
+  B200_CHECK_ARG(!doc || causal, "attn_fwd_dropout: pos, window and slopes need causal=1");
+  const uint32_t t = dropout_threshold(p);
+  return attn_fwd_impl(q, k, v, o, lse, doc, pos, window, B, S, H, Hk, D, scale, doc ? 1 : causal, stream, slopes,
+                       nullptr, true, t, dropout_scale(t), seed);
 }
 
 }  // namespace b200

@@ -133,6 +133,14 @@ int attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float*
 int attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
                     const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
                     int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
+int attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                     const float* slopes, int B, int S, int H, int Hk, int D, float scale, int causal, float p,
+                     unsigned long long seed, cudaStream_t stream);
+size_t attn_bwd_dropout_workspace_bytes(int B, int S, int H, int Hk, int D);
+int attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                     const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                     int H, int Hk, int D, float scale, int causal, float p, unsigned long long seed,
+                     int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream);
 size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D);
 int attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                       int window, const float* slopes, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
@@ -475,6 +483,23 @@ int b200_attn_bwd_prefix(const void* q, const void* k, const void* v, const void
                          float scale, int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream) {
   return b200::attn_bwd_prefix(q, k, v, o, d_o, lse, prefix, dq, dk, dv, B, S, H, Hk, D, scale, dkv_row_heads,
                                workspace, workspace_bytes, S_(stream));
+}
+
+int b200_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                          const float* slopes, int B, int S, int H, int Hk, int D, float scale, int causal, float p,
+                          unsigned long long seed, void* stream) {
+  return b200::attn_fwd_dropout(q, k, v, o, lse, pos, window, slopes, B, S, H, Hk, D, scale, causal, p, seed,
+                                S_(stream));
+}
+size_t b200_attn_bwd_dropout_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return b200::attn_bwd_dropout_workspace_bytes(B, S, H, Hk, D);
+}
+int b200_attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                          const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                          int H, int Hk, int D, float scale, int causal, float p, unsigned long long seed,
+                          int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream) {
+  return b200::attn_bwd_dropout(q, k, v, o, d_o, lse, pos, window, slopes, dq, dk, dv, B, S, H, Hk, D, scale, causal,
+                                p, seed, dkv_row_heads, workspace, workspace_bytes, S_(stream));
 }
 
 int b200_attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,

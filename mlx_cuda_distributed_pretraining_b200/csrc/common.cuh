@@ -29,6 +29,32 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 
+// Attention dropout's keep bits: Philox4x32-10 (Salmon et al., SC'11) of counter (k >> 3, q, h, b) and key
+// (seed lo, seed hi) gives 8 uniform 16-bit values r, one per key 8 (k >> 3) + i, r_i = (w[i >> 1] >> 16 (i & 1)) &
+// 0xffff.  Key i is kept iff r_i >= t; bit i of the result.
+__device__ __forceinline__ uint32_t philox_keep8(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
+                                                 uint32_t k1, uint32_t t) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t lo0 = 0xD2511F53u * c0, hi0 = __umulhi(0xD2511F53u, c0);
+    const uint32_t lo1 = 0xCD9E8D57u * c2, hi1 = __umulhi(0xCD9E8D57u, c2);
+    c0 = hi1 ^ c1 ^ k0;
+    c1 = lo1;
+    c2 = hi0 ^ c3 ^ k1;
+    c3 = lo0;
+    // the key schedule in volatile asm: folded to constants, the 20 round keys would be hoisted out of the
+    // attention kernels' key loops and held in registers
+    asm volatile("add.u32 %0, %0, 0x9E3779B9;" : "+r"(k0));
+    asm volatile("add.u32 %0, %0, 0xBB67AE85;" : "+r"(k1));
+  }
+  const uint32_t w[4] = {c0, c1, c2, c3};
+  uint32_t bits = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    bits |= (uint32_t)((w[i] & 0xffffu) >= t) << (2 * i) | (uint32_t)((w[i] >> 16) >= t) << (2 * i + 1);
+  return bits;
+}
+
 // ---------------------------------------------------------------------------------------------
 // mbarrier
 // ---------------------------------------------------------------------------------------------

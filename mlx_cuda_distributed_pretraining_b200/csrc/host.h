@@ -62,6 +62,14 @@ int make_tensor_map(CUtensorMap* out, const void* base, CUtensorMapDataType dtyp
 
 int num_sms();
 
+// attention dropout: keep threshold t = min(rint(p 65536), 65535) on 16-bit uniforms (p in [0, 1)), and the fp32
+// scale 1 / (1 - p_eff) of p_eff = t / 65536
+inline uint32_t dropout_threshold(float p) {
+  const double t = __builtin_rint((double)p * 65536.0);
+  return t > 65535.0 ? 65535u : (uint32_t)t;
+}
+inline float dropout_scale(uint32_t t) { return (float)(65536.0 / (65536.0 - (double)t)); }
+
 // One problem of a grouped GEMM launch (gemm_wgmma.cu: gemm_grouped): D = alpha*av[b]*op(A)op(B) +
 // beta*bv[b]*C, bf16 in/out, batched; layouts as in b200_gemm_bf16.  Mirrors b200_gemm_problem of the public
 // header field for field.

@@ -712,14 +712,55 @@ def _check_prefix(prefix: torch.Tensor, q: torch.Tensor, causal: bool, pos, wind
     return prefix.contiguous()
 
 
+_MASK64 = (1 << 64) - 1
+
+
+def splitmix64(x: int) -> int:
+    """One step of Steele, Lea and Flood's splitmix64 (OOPSLA 2014): x + golden gamma, then the finaliser."""
+    z = (x + 0x9E3779B97F4A7C15) & _MASK64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _MASK64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _MASK64
+    return z ^ (z >> 31)
+
+
+def dropout_seed(*parts: int) -> int:
+    """The attention-dropout seed chain: x = 0, then x = splitmix64(x ^ part) for each part.  The trainer's per-step
+    base is dropout_seed(system.seed, rank, step) and layer i's launch seed dropout_seed(base, i), so seeds are
+    deterministic in (seed, rank, step, layer) and nothing of them enters a checkpoint."""
+    x = 0
+    for part in parts:
+        x = splitmix64(x ^ (int(part) & _MASK64))
+    return x
+
+
+def _check_dropout(p, seed, prefix, what: str):
+    """(p, seed) of attention dropout, or None when p == 0.  p: a float in [0, 1); seed: an int in [0, 2^64), or None
+    for one drawn from torch's CPU generator (a host draw, no device read)."""
+    if isinstance(p, bool) or not isinstance(p, (float, int)) or not (0.0 <= float(p) < 1.0):
+        raise ValueError(f"{what}: dropout must be a float in [0, 1), got {p!r}")
+    if seed is not None and (isinstance(seed, bool) or not isinstance(seed, int) or not 0 <= seed < 1 << 64):
+        raise ValueError(f"{what}: seed must be an int in [0, 2^64), got {seed!r}")
+    if float(p) == 0.0:
+        return None
+    if prefix is not None:
+        raise ValueError(f"{what}: dropout does not combine with prefix")
+    if seed is None:
+        seed = int(torch.randint(-(1 << 63), (1 << 63) - 1, (1,), dtype=torch.int64).item()) & _MASK64
+    # the C entries quantise their fp32 p; passing p_eff = t / 65536 (exact in fp32) makes t that of the double p
+    t = min(round(float(p) * 65536.0), 65535)
+    return t / 65536.0, int(seed)
+
+
 def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
                       window: Optional[int] = None, alibi: Optional[torch.Tensor] = None,
-                      prefix: Optional[torch.Tensor] = None):
+                      prefix: Optional[torch.Tensor] = None, drop=None):
     """q [B,S,H,D], k/v [B,S,Hk,D] bf16 contiguous, D in {64,128}. Returns (o, lse[B,H,S]).  With pos (int32 [B,S]
     contiguous, positions within documents) the mask is document-causal and `causal` is ignored.  With window (an
     int >= 0) query s sees keys s - min(pos[s], window) .. s (pos[s] = s without pos), and `causal` is ignored.
     With alibi (fp32 [H] slopes, checked by the caller) the causal / document / window mask gets the ALiBi bias.
-    With prefix (int32 [B], checked by the caller) query s of row b sees key k iff k <= s or k < prefix[b]."""
+    With prefix (int32 [B], checked by the caller) query s of row b sees key k iff k <= s or k < prefix[b].
+    With drop = (p, seed) (checked by the caller; not with prefix) the dropout entry computes
+    O = (P o Z / (1 - p_eff)) V under the same mask; the LSE is the dropout-free one."""
     for t, nm in ((q, "q"), (k, "k"), (v, "v")):
         _need(t, torch.bfloat16, nm)
     B, S, H, D = q.shape
@@ -727,7 +768,12 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
     o = torch.empty_like(q)
     lse = torch.empty((B, H, S), device=q.device, dtype=torch.float32)
     tok = _t0("attn_fwd")
-    if prefix is not None:
+    if drop is not None:
+        check(lib().b200_attn_fwd_dropout(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
+                                          _ptr(pos), -1 if window is None else min(int(window), S), _ptr(alibi),
+                                          B, S, H, Hk, D, float(scale), int(causal), drop[0], drop[1], _stream()),
+              "b200_attn_fwd_dropout")
+    elif prefix is not None:
         check(lib().b200_attn_fwd_prefix(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(),
                                          prefix.data_ptr(), B, S, H, Hk, D, float(scale), _stream()),
               "b200_attn_fwd_prefix")
@@ -751,7 +797,7 @@ def attention_fwd_raw(q, k, v, scale: float, causal: bool, pos: Optional[torch.T
 
 def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Optional[torch.Tensor] = None,
                       window: Optional[int] = None, alibi: Optional[torch.Tensor] = None,
-                      prefix: Optional[torch.Tensor] = None):
+                      prefix: Optional[torch.Tensor] = None, drop=None):
     B, S, H, D = q.shape
     Hk = k.shape[2]
     dq = torch.empty_like(q)
@@ -760,7 +806,15 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
     dkv = torch.empty((B, S, 2 * Hk, D), device=k.device, dtype=k.dtype)
     dk, dv = dkv[:, :, :Hk], dkv[:, :, Hk:]
     tok = _t0("attn_bwd")
-    if prefix is not None:
+    if drop is not None:
+        nbytes = int(lib().b200_attn_bwd_dropout_workspace_bytes(B, S, H, Hk, D))
+        ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
+        check(lib().b200_attn_bwd_dropout(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
+                                          lse.data_ptr(), _ptr(pos), -1 if window is None else min(int(window), S),
+                                          _ptr(alibi), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, S, H, Hk, D,
+                                          float(scale), int(causal), drop[0], drop[1], 2 * Hk, ws.data_ptr(),
+                                          ws.numel(), _stream()), "b200_attn_bwd_dropout")
+    elif prefix is not None:
         nbytes = int(lib().b200_attn_bwd_prefix_workspace_bytes(B, S, H, Hk, D))
         ws = torch.empty(max(nbytes, 16), device=q.device, dtype=torch.uint8)
         check(lib().b200_attn_bwd_prefix(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), do.data_ptr(),
@@ -802,15 +856,15 @@ def attention_bwd_raw(q, k, v, o, do, lse, scale: float, causal: bool, pos: Opti
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None, prefix=None):
+    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None, prefix=None, drop=None):
         D = q.shape[-1]
         Dp = _pad_head_dim(D)
         if Dp != D:  # zero-padding the head dim leaves QK^T and the first D columns of PV unchanged
             q, k, v = (torch.nn.functional.pad(t, (0, Dp - D)) for t in (q, k, v))
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos, window, alibi, prefix)
+        o, lse = attention_fwd_raw(q, k, v, scale, causal, pos, window, alibi, prefix, drop)
         ctx.save_for_backward(q, k, v, o, lse, pos, alibi, prefix)
-        ctx.scale, ctx.causal, ctx.D, ctx.window = scale, causal, D, window
+        ctx.scale, ctx.causal, ctx.D, ctx.window, ctx.drop = scale, causal, D, window, drop
         return o[..., :D] if Dp != D else o
 
     @staticmethod
@@ -820,10 +874,11 @@ class _AttentionFn(torch.autograd.Function):
         if Dp != ctx.D:
             do = torch.nn.functional.pad(do, (0, Dp - ctx.D))
         do = do.contiguous()
-        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos, ctx.window, alibi, prefix)
+        dq, dk, dv = attention_bwd_raw(q, k, v, o, do, lse, ctx.scale, ctx.causal, pos, ctx.window, alibi, prefix,
+                                       ctx.drop)
         if Dp != ctx.D:
             dq, dk, dv = dq[..., :ctx.D], dk[..., :ctx.D], dv[..., :ctx.D]
-        return dq, dk, dv, None, None, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None, None, None
 
 
 def _hi_lo(x: torch.Tensor):
@@ -842,10 +897,14 @@ class _AttentionX3Fn(torch.autograd.Function):
                                   dk = dK'[0:D] + dK'[D:2D],    dv = dV'[0:D] + dV'[D:2D]
 
     The logits (where bf16 operand rounding hurts most: an error of |s| * 2^-9 in the exponent) are thus computed
-    to fp32-like accuracy; P and the kernel outputs still pass through one bf16 rounding each."""
+    to fp32-like accuracy; P and the kernel outputs still pass through one bf16 rounding each.
+
+    Dropout needs no kernel of its own here: the keep mask acts on P, which the three concatenated segments share
+    (one softmax per (query, key) pair, whatever the head dim), so O' = [P~ vh | P~ vh | P~ vl] with P~ = P o Z /
+    (1 - p_eff), and the backward's dV' and dS are those of the same P~."""
 
     @staticmethod
-    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None, prefix=None):
+    def forward(ctx, q, k, v, scale, causal, pos, window, alibi=None, prefix=None, drop=None):
         D = q.shape[-1]
         Dp = _pad_head_dim(3 * D)
         (qh, ql), (kh, kl), (vh, vl) = _hi_lo(q), _hi_lo(k), _hi_lo(v)
@@ -854,9 +913,9 @@ class _AttentionX3Fn(torch.autograd.Function):
             t = torch.cat([a, b, c], dim=-1)
             return (torch.nn.functional.pad(t, (0, Dp - 3 * D)) if Dp != 3 * D else t).contiguous()
         q3, k3, v3 = cat3(qh, ql, qh), cat3(kh, kh, kl), cat3(vh, vh, vl)
-        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos, window, alibi, prefix)
+        o3, lse = attention_fwd_raw(q3, k3, v3, scale, causal, pos, window, alibi, prefix, drop)
         ctx.save_for_backward(q3, k3, v3, o3, lse, pos, alibi, prefix)
-        ctx.scale, ctx.causal, ctx.D, ctx.Dp, ctx.window = scale, causal, D, Dp, window
+        ctx.scale, ctx.causal, ctx.D, ctx.Dp, ctx.window, ctx.drop = scale, causal, D, Dp, window, drop
         return o3[..., :D].float() + o3[..., 2 * D:3 * D].float()
 
     @staticmethod
@@ -868,18 +927,19 @@ class _AttentionX3Fn(torch.autograd.Function):
         if Dp != 3 * D:
             g3 = torch.nn.functional.pad(g3, (0, Dp - 3 * D))
         dq3, dk3, dv3 = attention_bwd_raw(q3, k3, v3, o3, g3.contiguous(), lse, ctx.scale, ctx.causal, pos,
-                                          ctx.window, alibi, prefix)
+                                          ctx.window, alibi, prefix, ctx.drop)
         dq = dq3[..., :D].float() + dq3[..., 2 * D:3 * D].float()
         dk = dk3[..., :D].float() + dk3[..., D:2 * D].float()
         dv = dv3[..., :D].float() + dv3[..., D:2 * D].float()
-        return dq, dk, dv, None, None, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None, None, None
 
 
 def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
                    causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None,
-                   alibi: Optional[torch.Tensor] = None, prefix: Optional[torch.Tensor] = None) -> torch.Tensor:
+                   alibi: Optional[torch.Tensor] = None, prefix: Optional[torch.Tensor] = None,
+                   dropout: float = 0.0, seed: Optional[int] = None) -> torch.Tensor:
     """fp32 in / fp32 out attention with bf16x3 logits (see _AttentionX3Fn); head_dim <= 42.  pos, window, alibi,
-    prefix: as attention."""
+    prefix, dropout, seed: as attention."""
     if 3 * q.shape[-1] > 128:
         raise ValueError("attention_fp32: head_dim must be <= 42 (three bf16 copies must fit a 128-wide tile)")
     if scale is None:
@@ -892,13 +952,15 @@ def attention_fp32(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Opt
         prefix = _check_prefix(prefix, q, causal, pos, window, alibi, "attention_fp32")
     if alibi is not None:
         alibi = _check_alibi(alibi, q, causal, "attention_fp32")
+    drop = _check_dropout(dropout, seed, prefix, "attention_fp32")
     return _AttentionX3Fn.apply(q.float(), k.float(), v.float(), float(scale), bool(causal), pos, window, alibi,
-                                prefix)
+                                prefix, drop)
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional[float] = None,
               causal: bool = True, pos: Optional[torch.Tensor] = None, window: Optional[int] = None,
-              alibi: Optional[torch.Tensor] = None, prefix: Optional[torch.Tensor] = None) -> torch.Tensor:
+              alibi: Optional[torch.Tensor] = None, prefix: Optional[torch.Tensor] = None,
+              dropout: float = 0.0, seed: Optional[int] = None) -> torch.Tensor:
     """softmax(q k^T * scale + causal_mask) v with GQA head sharing; [B,S,H,D] layout, bf16.
 
     pos (int32 [B, S]) packs several documents per row: pos[b, s] is token s's position within its document (0 at a
@@ -916,7 +978,14 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional
     prefix (int32 [B] on q's device) is the prefix-LM mask: query s of row b sees key k iff k <= s or k < prefix[b],
     so each row's prefix attends bidirectionally within itself and the rest of the row is causal.  prefix[b] <= 1 is
     the causal mask and prefix[b] = S full attention; values outside [0, S] act as their clamps.  It implies causal
-    for the rest of the row and raises together with pos, window, alibi or causal=False."""
+    for the rest of the row and raises together with pos, window, alibi or causal=False.
+
+    dropout (a float p in [0, 1)) drops attention probabilities as the reference's mx.dropout after the softmax:
+    O = (P o Z / (1 - p_eff)) V, with p_eff = min(rint(p 65536), 65535) / 65536 and Z the Philox keep mask of
+    (seed, b, h, q, k) stated in include/b200_hotpath.h (b200_attn_fwd_dropout); the backward regenerates it.  seed
+    (an int in [0, 2^64)) fixes the mask; None draws one from torch's CPU generator.  It composes with every mask
+    except prefix.  dropout = 0 calls the dropout-free kernels exactly as without it.  The caller decides when to
+    drop: the model does only in training mode with grad enabled."""
     if scale is None:
         scale = q.shape[-1] ** -0.5
     if prefix is not None:
@@ -927,7 +996,8 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, scale: Optional
         window, causal = _check_window(window, "attention"), True
     if alibi is not None:
         alibi = _check_alibi(alibi, q, causal, "attention")
-    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos, window, alibi, prefix)
+    drop = _check_dropout(dropout, seed, prefix, "attention")
+    return _AttentionFn.apply(q, k, v, float(scale), bool(causal), pos, window, alibi, prefix, drop)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -104,7 +104,7 @@ def _llama_config(cfg, vocab_size: int, bos: int, eos: int) -> dict:
     return {
         "architectures": ["LlamaForCausalLM"],
         "attention_bias": m.misc["attention_bias"],
-        "attention_dropout": 0.0,
+        "attention_dropout": float(m.attention.get("dropout") or 0.0),
         "bos_token_id": bos,
         "eos_token_id": [eos],
         "hidden_act": "silu",
