@@ -12,7 +12,11 @@ Tolerances (relative Frobenius error unless noted; see DESIGN.md section 5 "Orac
                                                 element against fp64 in tests/test_gpu_attention_fwd.py
                                                 (tests/attn_fwd_check.py) and tests/test_gpu_attention_bwd.py
                                                 (tests/attn_bwd_check.py), C32 = 4
-  Newton-Schulz 5 steps, bf16 operands 3e-2     (SURVEY 8c; measured ~1e-2)
+  Newton-Schulz 5 steps, bf16 operands 3e-2     (SURVEY 8c; measured ~1e-2).  Pins the reference's semantics; every
+                                                iteration's three stages, the grouped chain, the Muon step and
+                                                Shampoo's bf16x3 statistics / preconditioning are checked element
+                                                by element against fp64 in tests/test_gpu_matrix_optimizers_check.py
+                                                (tests/ns_check.py)
   RMSNorm, RoPE, GLU, cross entropy, embedding scatter and the flat optimizer updates are checked element by element
   against fp64 in tests/test_gpu_rowwise_kernels.py (tests/rowwise_check.py); only their golden-vector tests stay here
 """
