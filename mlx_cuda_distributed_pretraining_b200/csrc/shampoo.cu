@@ -319,7 +319,7 @@ newton_init_kernel(const float* __restrict__ M, int k, int kp, const float* __re
 __global__ void __launch_bounds__(NR_THREADS)
 newton_step_kernel(const float* __restrict__ F, int k, int kp, float tol, Split3 Mc, Split3 Tn, NewtonState st) {
   __shared__ float red[NR_THREADS / 32];
-  __shared__ int mode;  // 1: continue, 2: freeze
+  __shared__ int mode;  // 1: continue, 2: freeze after a rejected step, 3: freeze after an accepted (converged) step
   const int b = blockIdx.x;
   if (st.frozen[b]) {  // uniform over the block; X = X T stops from the iteration after the freeze
     if (threadIdx.x == 0) {
@@ -350,10 +350,17 @@ newton_step_kernel(const float* __restrict__ F, int k, int kp, float tol, Split3
     st.frozen[b] = freeze ? 1 : 0;
     st.av[b] = accept ? 1.f : 0.f;
     st.bv[b] = accept ? 0.f : 1.f;
-    mode = freeze ? 2 : 1;
+    mode = freeze ? (accept ? 3 : 2) : 1;
   }
   __syncthreads();
-  if (mode == 2) {
+  if (mode >= 2) {
+    // a converged step is still accepted: Mc holds the iterate whose residual err records
+    if (mode == 3)
+      for (long long i = threadIdx.x; i < kk4; i += NR_THREADS) {
+        const float4 v = *reinterpret_cast<const float4*>(F + base + i * 4);
+        const float f[4] = {v.x, v.y, v.z, v.w};
+        store_split3(f, Mc.h, Mc.m, Mc.l, base + i * 4);
+      }
     store_identity(Tn, base, k, kp);
     return;
   }
