@@ -65,9 +65,6 @@
 #include "host.h"
 
 namespace b200 {
-
-int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, int D, int box_rows);
-
 namespace {
 
 constexpr int BWD_THREADS = 384;  // producer / dQ-writer warpgroup + two MMA warpgroups
@@ -609,7 +606,6 @@ int launch_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap
   return B200_OK;
 }
 
-inline size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
 inline int pad_q(int S) { return (S + BQ - 1) / BQ * BQ; }
 
 // fp32 [B, S, H, D] dQ accumulator -> 4-D tensor map {D, H, S, B}, box {32, 1, 64, 1} (one 128-byte swizzle span)
@@ -619,21 +615,6 @@ int make_dq_acc_map(CUtensorMap* tm, const float* base, int B, int S, int H, int
   const uint32_t box[4] = {32, 1, (uint32_t)BQ, 1};
   return make_tensor_map(tm, base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 4, dims, strides, box, true);
 }
-
-}  // namespace
-
-size_t attn_bwd_workspace_bytes(int B, int S, int H, int Hk, int D) {
-  (void)Hk;
-  return al256((size_t)B * S * H * D * 4) + 2 * al256((size_t)B * H * pad_q(S) * 4);
-}
-
-// the document variant adds the [B, S_pad] document starts and the [B, n_kt] query-tile ends
-size_t attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
-  return attn_bwd_workspace_bytes(B, S, H, Hk, D) + al256((size_t)B * pad_q(S) * 4) +
-         al256((size_t)B * ((S + BKV - 1) / BKV) * 4);
-}
-
-namespace {
 
 // doc selects the document / window kernels; window < 0 means none; slopes (doc only) selects ALiBi; prefix (causal,
 // not doc) selects the prefix-LM kernels; drop selects the dropout kernels (not with prefix)
@@ -650,7 +631,8 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_bwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_bwd: head_dim %d unsupported (64 or 128)", D);
-  const size_t need = doc ? attn_bwd_doc_workspace_bytes(B, S, H, Hk, D) : attn_bwd_workspace_bytes(B, S, H, Hk, D);
+  const size_t need =
+      doc ? b200_attn_bwd_doc_workspace_bytes(B, S, H, Hk, D) : b200_attn_bwd_workspace_bytes(B, S, H, Hk, D);
   if (ws_bytes < need) {
     set_error("attn_bwd: workspace too small (%zu < %zu)", ws_bytes, need);
     return B200_ERR_WORKSPACE;
@@ -739,68 +721,100 @@ int attn_bwd_impl(const void* q, const void* k, const void* v, const void* o, co
 }
 
 }  // namespace
+}  // namespace b200
 
-int attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
-             const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
-             float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+using namespace b200;
+
+extern "C" {
+
+size_t b200_attn_bwd_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  (void)Hk;
+  return al256((size_t)B * S * H * D * 4) + 2 * al256((size_t)B * H * pad_q(S) * 4);
+}
+
+// the document variant adds the [B, S_pad] document starts and the [B, n_kt] query-tile ends
+size_t b200_attn_bwd_doc_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return b200_attn_bwd_workspace_bytes(B, S, H, Hk, D) + al256((size_t)B * pad_q(S) * 4) +
+         al256((size_t)B * ((S + BKV - 1) / BKV) * 4);
+}
+
+int b200_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* d_o,
+                  const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk,
+                  int D, float scale, int causal, void* ws, size_t ws_bytes, void* stream) {
+  return attn_bwd_impl(q, k, v, o, d_o, lse, false, nullptr, -1, dq, dk, dv, B, S, H, Hk, D, scale, causal, 0, ws,
+                       ws_bytes, static_cast<cudaStream_t>(stream));
+}
+
+int b200_attn_bwd_strided(const void* q, const void* k, const void* v, const void* o, const void* d_o,
+                          const float* lse, void* dq, void* dk, void* dv, int B, int S, int H, int Hk,
+                          int D, float scale, int causal, int dkv_row_heads, void* ws, size_t ws_bytes, void* stream) {
   return attn_bwd_impl(q, k, v, o, d_o, lse, false, nullptr, -1, dq, dk, dv, B, S, H, Hk, D, scale, causal,
-                       dkv_row_heads, ws, ws_bytes, stream);
+                       dkv_row_heads, ws, ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // document-causal backward: query s of row b sees keys s - pos[b, s] .. s
-int attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                 const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
-                 int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_attn_bwd_doc(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                      const int* pos, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
+                      int dkv_row_heads, void* ws, size_t ws_bytes, void* stream) {
   B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
                  "attn_bwd_doc: pos must be a non-null, 4-byte aligned int32 [B, S] array");
   return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, -1, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads, ws,
-                       ws_bytes, stream);
+                       ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // sliding-window backward: query s sees keys s - min(pos[b, s], window) .. s; pos == nullptr means pos[b, s] = s.
 // Same workspace as the document variant.
-int attn_bwd_window(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                    const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
-                    float scale, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+size_t b200_attn_bwd_window_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return b200_attn_bwd_doc_workspace_bytes(B, S, H, Hk, D);
+}
+
+int b200_attn_bwd_window(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                         const int* pos, int window, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
+                         float scale, int dkv_row_heads, void* ws, size_t ws_bytes, void* stream) {
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_bwd_window: pos must be 4-byte aligned int32");
   B200_CHECK_ARG(window >= 0, "attn_bwd_window: window=%d must be >= 0", window);
   return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
-                       ws, ws_bytes, stream);
+                       ws, ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // ALiBi backward: attn_bwd_window (window < 0: none) with the forward's bias slopes[h] * (k - s).  Same workspace.
-int attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                   const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S, int H,
-                   int Hk, int D, float scale, int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_attn_bwd_alibi(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                        const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                        int H, int Hk, int D, float scale, int dkv_row_heads, void* ws, size_t ws_bytes, void* stream) {
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_bwd_alibi: pos must be 4-byte aligned int32");
   B200_CHECK_ARG(slopes != nullptr && (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
                  "attn_bwd_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
   return attn_bwd_impl(q, k, v, o, d_o, lse, true, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
-                       ws, ws_bytes, stream, slopes);
+                       ws, ws_bytes, static_cast<cudaStream_t>(stream), slopes);
 }
 
 // prefix-LM backward: query s of row b sees key k iff k <= s or k < prefix[b] (clamped to [0, S] in the kernel).
 // Same workspace as the causal backward.
-int attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                    const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D, float scale,
-                    int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+size_t b200_attn_bwd_prefix_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return b200_attn_bwd_workspace_bytes(B, S, H, Hk, D);
+}
+
+int b200_attn_bwd_prefix(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                         const int* prefix, void* dq, void* dk, void* dv, int B, int S, int H, int Hk, int D,
+                         float scale, int dkv_row_heads, void* ws, size_t ws_bytes, void* stream) {
   B200_CHECK_ARG(prefix != nullptr && (reinterpret_cast<uintptr_t>(prefix) & 3u) == 0,
                  "attn_bwd_prefix: prefix must be a non-null, 4-byte aligned int32 [B] array");
   return attn_bwd_impl(q, k, v, o, d_o, lse, false, nullptr, -1, dq, dk, dv, B, S, H, Hk, D, scale, 1, dkv_row_heads,
-                       ws, ws_bytes, stream, nullptr, prefix);
+                       ws, ws_bytes, static_cast<cudaStream_t>(stream), nullptr, prefix);
 }
 
 // dropout backward: the causal / non-causal (pos == nullptr, window < 0, slopes == nullptr), document / window or
 // ALiBi backward of attn_fwd_dropout's O = (P o Z / (1 - p_eff)) V, the same p and seed.  Workspace: the document
 // variant's when pos, window or slopes select the DOC kernels, else the causal one's.
-size_t attn_bwd_dropout_workspace_bytes(int B, int S, int H, int Hk, int D) {
-  return attn_bwd_doc_workspace_bytes(B, S, H, Hk, D);
+size_t b200_attn_bwd_dropout_workspace_bytes(int B, int S, int H, int Hk, int D) {
+  return b200_attn_bwd_doc_workspace_bytes(B, S, H, Hk, D);
 }
 
-int attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
-                     const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
-                     int H, int Hk, int D, float scale, int causal, float p, unsigned long long seed,
-                     int dkv_row_heads, void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o, const void* d_o, const float* lse,
+                          const int* pos, int window, const float* slopes, void* dq, void* dk, void* dv, int B, int S,
+                          int H, int Hk, int D, float scale, int causal, float p, unsigned long long seed,
+                          int dkv_row_heads, void* ws, size_t ws_bytes, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(p >= 0.f && p < 1.f, "attn_bwd_dropout: p=%g must lie in [0, 1)", (double)p);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_bwd_dropout: pos must be 4-byte aligned int32");
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0, "attn_bwd_dropout: slopes must be 4-byte aligned");
@@ -808,7 +822,7 @@ int attn_bwd_dropout(const void* q, const void* k, const void* v, const void* o,
   B200_CHECK_ARG(!doc || causal, "attn_bwd_dropout: pos, window and slopes need causal=1");
   const uint32_t t = dropout_threshold(p);
   return attn_bwd_impl(q, k, v, o, d_o, lse, doc, pos, window, dq, dk, dv, B, S, H, Hk, D, scale, doc ? 1 : causal,
-                       dkv_row_heads, ws, ws_bytes, stream, slopes, nullptr, true, t, dropout_scale(t), seed);
+                       dkv_row_heads, ws, ws_bytes, s, slopes, nullptr, true, t, dropout_scale(t), seed);
 }
 
-}  // namespace b200
+}  // extern "C"

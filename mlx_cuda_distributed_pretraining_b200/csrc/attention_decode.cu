@@ -457,18 +457,6 @@ kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __res
   }
 }
 
-bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-}  // namespace
-
-size_t attn_decode_workspace_bytes(int B, int H, int s_max, int D) {
-  if (B <= 0 || H <= 0 || s_max <= 0 || D <= 0) return 0;
-  const size_t chunks = (size_t)(s_max + DEC_CHUNK - 1) / DEC_CHUNK;
-  return (size_t)B * H * chunks * (size_t)(D + 2) * sizeof(float);
-}
-
-namespace {
-
 // window < 0 means none; slopes selects ALiBi
 int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                      int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
@@ -480,7 +468,7 @@ int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, co
   B200_CHECK_ARG(G * D <= DEC_MAX_ITEMS * DEC_THREADS * 8, "attn_decode: (H/Hk) * D = %d exceeds %d", G * D,
                  DEC_MAX_ITEMS * DEC_THREADS * 8);
   B200_CHECK_ARG(al16(q) && al16(o) && lens != nullptr, "attn_decode: q / o must be 16-byte aligned, lens non-null");
-  const size_t need = attn_decode_workspace_bytes(B, H, s_max, D);
+  const size_t need = b200_attn_decode_workspace_bytes(B, H, s_max, D);
   if (ws_bytes < need || (need > 0 && ws == nullptr)) {
     set_error("attn_decode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     return B200_ERR_WORKSPACE;
@@ -516,36 +504,48 @@ int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, co
 }
 
 }  // namespace
+}  // namespace b200
 
-int attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse, int B,
-                int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes,
-                cudaStream_t stream) {
+using namespace b200;
+
+extern "C" {
+
+size_t b200_attn_decode_workspace_bytes(int B, int H, int s_max, int D) {
+  if (B <= 0 || H <= 0 || s_max <= 0 || D <= 0) return 0;
+  const size_t chunks = (size_t)(s_max + DEC_CHUNK - 1) / DEC_CHUNK;
+  return (size_t)B * H * chunks * (size_t)(D + 2) * sizeof(float);
+}
+
+int b200_attn_decode(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
+                     int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes,
+                     void* stream) {
   return attn_decode_impl(q, k_cache, v_cache, lens, o, lse, -1, B, s_max, H, Hk, D, scale, is_bf16, ws, ws_bytes,
-                          stream);
+                          static_cast<cudaStream_t>(stream));
 }
 
 // sliding window: the query at position lens[b] - 1 sees cached keys max(0, lens[b] - 1 - window) .. lens[b] - 1
-int attn_decode_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
-                       int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
-                       size_t ws_bytes, cudaStream_t stream) {
+int b200_attn_decode_window(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o,
+                            float* lse, int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
+                            void* ws, size_t ws_bytes, void* stream) {
   B200_CHECK_ARG(window >= 0, "attn_decode_window: window=%d must be >= 0", window);
   return attn_decode_impl(q, k_cache, v_cache, lens, o, lse, window, B, s_max, H, Hk, D, scale, is_bf16, ws,
-                          ws_bytes, stream);
+                          ws_bytes, static_cast<cudaStream_t>(stream));
 }
 
 // ALiBi: attn_decode_window (window < 0: none) with the bias slopes[h] * (k - (lens[b] - 1)) on every cached key k
-int attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
-                      int window, const float* slopes, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16,
-                      void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o,
+                           float* lse, int window, const float* slopes, int B, int s_max, int H, int Hk, int D,
+                           float scale, int is_bf16, void* ws, size_t ws_bytes, void* stream) {
   B200_CHECK_ARG(slopes != nullptr && (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
                  "attn_decode_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
   return attn_decode_impl(q, k_cache, v_cache, lens, o, lse, window, B, s_max, H, Hk, D, scale, is_bf16, ws,
-                          ws_bytes, stream, slopes);
+                          ws_bytes, static_cast<cudaStream_t>(stream), slopes);
 }
 
-int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
-              const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
-              cudaStream_t stream) {
+int b200_kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                   const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                   void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(B > 0 && s_max > 0 && H > 0 && Hk > 0 && D > 0 && D % 8 == 0,
                  "kv_append: bad shape B=%d s_max=%d H=%d Hk=%d D=%d (D %% 8 == 0)", B, s_max, H, Hk, D);
   B200_CHECK_ARG((cos_t == nullptr) == (sin_t == nullptr), "kv_append: give both RoPE tables or neither");
@@ -556,21 +556,22 @@ int kv_append(void* q, const void* k, const void* v, void* k_cache, void* v_cach
   long long blocks = (nvec + 255) / 256;
   if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
   if (is_bf16)
-    kv_append_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, stream>>>(
+    kv_append_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, s>>>(
         (__nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (__nv_bfloat16*)k_cache,
         (__nv_bfloat16*)v_cache, lens, cos_t, sin_t, nvec, s_max, H, Hk, D);
   else
-    kv_append_kernel<float><<<(int)blocks, 256, 0, stream>>>((float*)q, (const float*)k, (const float*)v,
-                                                             (float*)k_cache, (float*)v_cache, lens, cos_t, sin_t,
-                                                             nvec, s_max, H, Hk, D);
+    kv_append_kernel<float><<<(int)blocks, 256, 0, s>>>((float*)q, (const float*)k, (const float*)v,
+                                                        (float*)k_cache, (float*)v_cache, lens, cos_t, sin_t,
+                                                        nvec, s_max, H, Hk, D);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
 // kv_append with the half-split rotation of b200_rope_half; the tables are required and D % 16 == 0
-int kv_append_half(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
-                   const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
-                   cudaStream_t stream) {
+int b200_kv_append_half(void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int* lens,
+                        const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
+                        void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(B > 0 && s_max > 0 && H > 0 && Hk > 0 && D > 0 && D % 16 == 0,
                  "kv_append_half: bad shape B=%d s_max=%d H=%d Hk=%d D=%d (D %% 16 == 0)", B, s_max, H, Hk, D);
   B200_CHECK_ARG(cos_t != nullptr && sin_t != nullptr && lens != nullptr, "kv_append_half: RoPE tables and lens required");
@@ -580,15 +581,15 @@ int kv_append_half(void* q, const void* k, const void* v, void* k_cache, void* v
   long long blocks = (nslice + 255) / 256;
   if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
   if (is_bf16)
-    kv_append_half_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, stream>>>(
+    kv_append_half_kernel<__nv_bfloat16><<<(int)blocks, 256, 0, s>>>(
         (__nv_bfloat16*)q, (const __nv_bfloat16*)k, (const __nv_bfloat16*)v, (__nv_bfloat16*)k_cache,
         (__nv_bfloat16*)v_cache, lens, cos_t, sin_t, nslice, s_max, H, Hk, D);
   else
-    kv_append_half_kernel<float><<<(int)blocks, 256, 0, stream>>>((float*)q, (const float*)k, (const float*)v,
-                                                                  (float*)k_cache, (float*)v_cache, lens, cos_t,
-                                                                  sin_t, nslice, s_max, H, Hk, D);
+    kv_append_half_kernel<float><<<(int)blocks, 256, 0, s>>>((float*)q, (const float*)k, (const float*)v,
+                                                             (float*)k_cache, (float*)v_cache, lens, cos_t,
+                                                             sin_t, nslice, s_max, H, Hk, D);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -452,58 +452,67 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
 }
 
 }  // namespace
+}  // namespace b200
 
-int attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int H,
-             int Hk, int D, float scale, int causal, cudaStream_t stream) {
-  return attn_fwd_impl(q, k, v, o, lse, false, nullptr, -1, B, S, H, Hk, D, scale, causal, stream);
+using namespace b200;
+
+extern "C" {
+
+int b200_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, int B, int S, int H,
+                  int Hk, int D, float scale, int causal, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  return attn_fwd_impl(q, k, v, o, lse, false, nullptr, -1, B, S, H, Hk, D, scale, causal, s);
 }
 
 // document-causal: query s of row b sees keys s - pos[b, s] .. s
-int attn_fwd_doc(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B, int S,
-                 int H, int Hk, int D, float scale, cudaStream_t stream) {
+int b200_attn_fwd_doc(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int B, int S,
+                      int H, int Hk, int D, float scale, void* stream) {
   B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
                  "attn_fwd_doc: pos must be a non-null, 4-byte aligned int32 [B, S] array");
-  return attn_fwd_impl(q, k, v, o, lse, true, pos, -1, B, S, H, Hk, D, scale, 1, stream);
+  return attn_fwd_impl(q, k, v, o, lse, true, pos, -1, B, S, H, Hk, D, scale, 1, static_cast<cudaStream_t>(stream));
 }
 
 // sliding window: query s sees keys s - min(pos[b, s], window) .. s; pos == nullptr means pos[b, s] = s
-int attn_fwd_window(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
-                    int B, int S, int H, int Hk, int D, float scale, cudaStream_t stream) {
+int b200_attn_fwd_window(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                         int B, int S, int H, int Hk, int D, float scale, void* stream) {
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_fwd_window: pos must be 4-byte aligned int32");
   B200_CHECK_ARG(window >= 0, "attn_fwd_window: window=%d must be >= 0", window);
-  return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, stream);
+  return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, static_cast<cudaStream_t>(stream));
 }
 
 // ALiBi: attn_fwd_window (window < 0: none) with the bias slopes[h] * (k - s) added to every visible score
-int attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
-                   const float* slopes, int B, int S, int H, int Hk, int D, float scale, cudaStream_t stream) {
+int b200_attn_fwd_alibi(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                        const float* slopes, int B, int S, int H, int Hk, int D, float scale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_fwd_alibi: pos must be 4-byte aligned int32");
   B200_CHECK_ARG(slopes != nullptr && (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
                  "attn_fwd_alibi: slopes must be a non-null, 4-byte aligned fp32 [H] array");
-  return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, stream, slopes);
+  return attn_fwd_impl(q, k, v, o, lse, true, pos, window, B, S, H, Hk, D, scale, 1, s, slopes);
 }
 
 // prefix-LM: query s of row b sees key k iff k <= s or k < prefix[b] (clamped to [0, S] in the kernel)
-int attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float* lse, const int* prefix, int B, int S,
-                    int H, int Hk, int D, float scale, cudaStream_t stream) {
+int b200_attn_fwd_prefix(const void* q, const void* k, const void* v, void* o, float* lse, const int* prefix, int B,
+                         int S, int H, int Hk, int D, float scale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(prefix != nullptr && (reinterpret_cast<uintptr_t>(prefix) & 3u) == 0,
                  "attn_fwd_prefix: prefix must be a non-null, 4-byte aligned int32 [B] array");
-  return attn_fwd_impl(q, k, v, o, lse, false, nullptr, -1, B, S, H, Hk, D, scale, 1, stream, nullptr, prefix);
+  return attn_fwd_impl(q, k, v, o, lse, false, nullptr, -1, B, S, H, Hk, D, scale, 1, s, nullptr, prefix);
 }
 
 // dropout: the causal / non-causal (pos == nullptr, window < 0, slopes == nullptr), document / window or ALiBi
 // forward with O = (P o Z / (1 - p_eff)) V; t = min(rint(p 65536), 65535), p_eff = t / 65536
-int attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
-                     const float* slopes, int B, int S, int H, int Hk, int D, float scale, int causal, float p,
-                     unsigned long long seed, cudaStream_t stream) {
+int b200_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, float* lse, const int* pos, int window,
+                          const float* slopes, int B, int S, int H, int Hk, int D, float scale, int causal, float p,
+                          unsigned long long seed, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(p >= 0.f && p < 1.f, "attn_fwd_dropout: p=%g must lie in [0, 1)", (double)p);
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(pos) & 3u) == 0, "attn_fwd_dropout: pos must be 4-byte aligned int32");
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0, "attn_fwd_dropout: slopes must be 4-byte aligned");
   const bool doc = pos != nullptr || window >= 0 || slopes != nullptr;
   B200_CHECK_ARG(!doc || causal, "attn_fwd_dropout: pos, window and slopes need causal=1");
   const uint32_t t = dropout_threshold(p);
-  return attn_fwd_impl(q, k, v, o, lse, doc, pos, window, B, S, H, Hk, D, scale, doc ? 1 : causal, stream, slopes,
+  return attn_fwd_impl(q, k, v, o, lse, doc, pos, window, B, S, H, Hk, D, scale, doc ? 1 : causal, s, slopes,
                        nullptr, true, t, dropout_scale(t), seed);
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -568,24 +568,13 @@ inline int ew_grid(long long n_per_thread_items) {
   return (int)blocks;
 }
 
-inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-}  // namespace
-
-// Scratch of the deterministic grid reductions: one partial per block (at most 8 blocks per SM over the
-// whole batch, plus one per matrix) and one arrival counter per matrix.
-size_t reduce_workspace_bytes(int batch) {
-  if (batch < 1) batch = 1;
-  return (((size_t)num_sms() * 8 + 2 * (size_t)batch) * 4 + 255) & ~size_t(255);
-}
-
 // splits a caller workspace into (partials, counters) and zeroes the counters on `stream`
-static int reduce_ws(void* ws, size_t ws_bytes, int batch, int gx, float** partials, unsigned** counters,
-                     cudaStream_t stream) {
-  if (ws == nullptr || ws_bytes < reduce_workspace_bytes(batch) ||
-      (size_t)gx * batch + batch > reduce_workspace_bytes(batch) / 4) {
+int reduce_ws(void* ws, size_t ws_bytes, int batch, int gx, float** partials, unsigned** counters,
+              cudaStream_t stream) {
+  if (ws == nullptr || ws_bytes < b200_reduce_workspace_bytes(batch) ||
+      (size_t)gx * batch + batch > b200_reduce_workspace_bytes(batch) / 4) {
     set_error("reduction workspace too small (%zu < %zu bytes for batch %d)", ws_bytes,
-              reduce_workspace_bytes(batch), batch);
+              b200_reduce_workspace_bytes(batch), batch);
     return B200_ERR_WORKSPACE;
   }
   *counters = reinterpret_cast<unsigned*>(ws);
@@ -594,11 +583,26 @@ static int reduce_ws(void* ws, size_t ws_bytes, int batch, int gx, float** parti
   return B200_OK;
 }
 
-int muon_momentum(const void* g, int g_is_bf16, float* buf, void* u_bf16, float* sumsq,
-                  long long numel, int batch, float mu, int nesterov, float gscale, void* ws,
-                  size_t ws_bytes, cudaStream_t stream) {
+}  // namespace
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+// Scratch of the deterministic grid reductions: one partial per block (at most 8 blocks per SM over the
+// whole batch, plus one per matrix) and one arrival counter per matrix.
+size_t b200_reduce_workspace_bytes(int batch) {
+  if (batch < 1) batch = 1;
+  return al256(((size_t)num_sms() * 8 + 2 * (size_t)batch) * 4);
+}
+
+int b200_muon_momentum(const void* g, int g_is_bf16, float* buf, void* u_bf16, float* sumsq,
+                       long long numel, int batch, float mu, int nesterov, float gscale, void* ws,
+                       size_t ws_bytes, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(numel > 0 && batch > 0, "muon_momentum: empty");
-  B200_CHECK_ARG(aligned16(g) && aligned16(buf) && aligned16(u_bf16),
+  B200_CHECK_ARG(al16(g) && al16(buf) && al16(u_bf16),
                  "muon_momentum: buffers must be 16-byte aligned");
   B200_CHECK_ARG(batch == 1 || numel % 8 == 0,
                  "muon_momentum: batched use needs numel %% 8 == 0 (got %lld)", numel);
@@ -609,215 +613,224 @@ int muon_momentum(const void* g, int g_is_bf16, float* buf, void* u_bf16, float*
   dim3 grid(gx, batch);
   float* partials;
   unsigned* counters;
-  if (int rc = reduce_ws(ws, ws_bytes, batch, gx, &partials, &counters, stream)) return rc;
+  if (int rc = reduce_ws(ws, ws_bytes, batch, gx, &partials, &counters, s)) return rc;
   if (g_is_bf16)
-    muon_momentum_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    muon_momentum_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>(
         (const __nv_bfloat16*)g, buf, (__nv_bfloat16*)u_bf16, sumsq, numel, mu, nesterov, gscale, partials,
         counters);
   else
-    muon_momentum_kernel<float><<<grid, EW_THREADS, 0, stream>>>(
+    muon_momentum_kernel<float><<<grid, EW_THREADS, 0, s>>>(
         (const float*)g, buf, (__nv_bfloat16*)u_bf16, sumsq, numel, mu, nesterov, gscale, partials, counters);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int ns_scales(const float* sumsq, float* inv_norm, float* inv_norm_sq, int batch, float eps,
-              cudaStream_t stream) {
-  ns_scales_kernel<<<(batch + 127) / 128, 128, 0, stream>>>(sumsq, inv_norm, inv_norm_sq, batch,
-                                                           eps);
+int b200_ns_scales(const float* sumsq, float* inv_norm, float* inv_norm_sq, int batch, float eps,
+                   void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  ns_scales_kernel<<<(batch + 127) / 128, 128, 0, s>>>(sumsq, inv_norm, inv_norm_sq, batch, eps);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int axpy_update(float* p32, void* p16, const void* x, int x_is_bf16, long long n, float s,
-                cudaStream_t stream) {
+int b200_axpy_update(float* p32, void* p16, const void* x, int x_is_bf16, long long n, float s,
+                     void* stream) {
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "axpy_update: empty");
-  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(x),
+  B200_CHECK_ARG(al16(p32) && al16(p16) && al16(x),
                  "axpy_update: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (x_is_bf16)
-    axpy_update_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    axpy_update_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, st>>>(
         p32, (__nv_bfloat16*)p16, (const __nv_bfloat16*)x, n, s);
   else
-    axpy_update_kernel<float><<<grid, EW_THREADS, 0, stream>>>(p32, (__nv_bfloat16*)p16,
-                                                              (const float*)x, n, s);
+    axpy_update_kernel<float><<<grid, EW_THREADS, 0, st>>>(p32, (__nv_bfloat16*)p16,
+                                                          (const float*)x, n, s);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int sgd_momentum(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, long long n,
-                 float mu, int nesterov, float lr, float gscale, cudaStream_t stream) {
+int b200_sgd_momentum(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, long long n,
+                      float mu, int nesterov, float lr, float gscale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "sgd_momentum: empty");
-  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(g) && aligned16(buf),
+  B200_CHECK_ARG(al16(p32) && al16(p16) && al16(g) && al16(buf),
                  "sgd_momentum: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (g_is_bf16)
-    sgd_momentum_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    sgd_momentum_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>(
         p32, (__nv_bfloat16*)p16, (const __nv_bfloat16*)g, buf, n, mu, nesterov, lr, gscale);
   else
-    sgd_momentum_kernel<float><<<grid, EW_THREADS, 0, stream>>>(
+    sgd_momentum_kernel<float><<<grid, EW_THREADS, 0, s>>>(
         p32, (__nv_bfloat16*)p16, (const float*)g, buf, n, mu, nesterov, lr, gscale);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int adamw(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* v, long long n,
-          float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, float gscale,
-          cudaStream_t stream) {
+int b200_adamw(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* v, long long n,
+               float lr, float b1, float b2, float eps, float wd, float bc1, float bc2, float gscale,
+               void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "adamw: empty");
-  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(g) && aligned16(m) && aligned16(v),
+  B200_CHECK_ARG(al16(p32) && al16(p16) && al16(g) && al16(m) && al16(v),
                  "adamw: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (g_is_bf16)
-    adamw_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    adamw_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>(
         p32, (__nv_bfloat16*)p16, (const __nv_bfloat16*)g, m, v, n, lr, b1, b2, eps, wd, bc1, bc2,
         gscale);
   else
-    adamw_kernel<float><<<grid, EW_THREADS, 0, stream>>>(p32, (__nv_bfloat16*)p16, (const float*)g,
-                                                        m, v, n, lr, b1, b2, eps, wd, bc1, bc2,
-                                                        gscale);
+    adamw_kernel<float><<<grid, EW_THREADS, 0, s>>>(p32, (__nv_bfloat16*)p16, (const float*)g,
+                                                   m, v, n, lr, b1, b2, eps, wd, bc1, bc2,
+                                                   gscale);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int adam_direction(float* d, const void* g, int g_is_bf16, float* m, float* v, long long n,
-                   float lr, float b1, float b2, float eps, float bc1, float bc2, float gscale,
-                   cudaStream_t stream) {
+int b200_adam_direction(float* d, const void* g, int g_is_bf16, float* m, float* v, long long n,
+                        float lr, float b1, float b2, float eps, float bc1, float bc2, float gscale,
+                        void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "adam_direction: empty");
-  B200_CHECK_ARG(aligned16(d) && aligned16(g) && aligned16(m) && aligned16(v),
+  B200_CHECK_ARG(al16(d) && al16(g) && al16(m) && al16(v),
                  "adam_direction: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (g_is_bf16)
-    adam_direction_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    adam_direction_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>(
         d, (const __nv_bfloat16*)g, m, v, n, lr, b1, b2, eps, bc1, bc2, gscale);
   else
-    adam_direction_kernel<float><<<grid, EW_THREADS, 0, stream>>>(d, (const float*)g, m, v, n, lr,
-                                                                 b1, b2, eps, bc1, bc2, gscale);
+    adam_direction_kernel<float><<<grid, EW_THREADS, 0, s>>>(d, (const float*)g, m, v, n, lr,
+                                                            b1, b2, eps, bc1, bc2, gscale);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int lion(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* ema, long long n, float lr,
-         float b_sign, float b_mom, float decay, float gscale, const float* clip_ss, float max_norm,
-         float ema_decay, int ema_mode, cudaStream_t stream) {
+int b200_lion(float* p32, void* p16, const void* g, int g_is_bf16, float* m, float* ema, long long n, float lr,
+              float b_sign, float b_mom, float decay, float gscale, const float* clip_ss, float max_norm,
+              float ema_decay, int ema_mode, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "lion: empty");
   B200_CHECK_ARG(p32 && g && m, "lion: p32, g and m are required");
   B200_CHECK_ARG(ema_mode >= 0 && ema_mode <= 2 && (ema_mode == 0 || ema), "lion: ema_mode %d needs ema (0..2)",
                  ema_mode);
-  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(g) && aligned16(m) && aligned16(ema),
+  B200_CHECK_ARG(al16(p32) && al16(p16) && al16(g) && al16(m) && al16(ema),
                  "lion: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (g_is_bf16)
-    lion_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    lion_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>(
         p32, (__nv_bfloat16*)p16, (const __nv_bfloat16*)g, m, ema, n, lr, b_sign, b_mom, decay, gscale, clip_ss,
         max_norm, ema_decay, ema_mode);
   else
-    lion_kernel<float><<<grid, EW_THREADS, 0, stream>>>(p32, (__nv_bfloat16*)p16, (const float*)g, m, ema, n, lr,
-                                                       b_sign, b_mom, decay, gscale, clip_ss, max_norm, ema_decay,
-                                                       ema_mode);
+    lion_kernel<float><<<grid, EW_THREADS, 0, s>>>(p32, (__nv_bfloat16*)p16, (const float*)g, m, ema, n, lr,
+                                                  b_sign, b_mom, decay, gscale, clip_ss, max_norm, ema_decay,
+                                                  ema_mode);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int sgd(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, float* ema, long long n, float lr,
-        float mu, float dampening, int nesterov, float coupled_wd, float gscale, const float* clip_ss,
-        float max_norm, float ema_decay, int ema_mode, cudaStream_t stream) {
+int b200_sgd(float* p32, void* p16, const void* g, int g_is_bf16, float* buf, float* ema, long long n, float lr,
+             float mu, float dampening, int nesterov, float coupled_wd, float gscale, const float* clip_ss,
+             float max_norm, float ema_decay, int ema_mode, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "sgd: empty");
   B200_CHECK_ARG(p32 && g, "sgd: p32 and g are required");
   B200_CHECK_ARG(ema_mode >= 0 && ema_mode <= 2 && (ema_mode == 0 || ema), "sgd: ema_mode %d needs ema (0..2)",
                  ema_mode);
-  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(g) && aligned16(buf) && aligned16(ema),
+  B200_CHECK_ARG(al16(p32) && al16(p16) && al16(g) && al16(buf) && al16(ema),
                  "sgd: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (g_is_bf16)
-    sgd_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    sgd_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>(
         p32, (__nv_bfloat16*)p16, (const __nv_bfloat16*)g, buf, ema, n, lr, mu, dampening, nesterov, coupled_wd,
         gscale, clip_ss, max_norm, ema_decay, ema_mode);
   else
-    sgd_kernel<float><<<grid, EW_THREADS, 0, stream>>>(p32, (__nv_bfloat16*)p16, (const float*)g, buf, ema, n, lr,
-                                                      mu, dampening, nesterov, coupled_wd, gscale, clip_ss,
-                                                      max_norm, ema_decay, ema_mode);
+    sgd_kernel<float><<<grid, EW_THREADS, 0, s>>>(p32, (__nv_bfloat16*)p16, (const float*)g, buf, ema, n, lr,
+                                                 mu, dampening, nesterov, coupled_wd, gscale, clip_ss,
+                                                 max_norm, ema_decay, ema_mode);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int clip_accum(const void* g, int g_is_bf16, float* acc, long long n, float clip, float scale,
-               int init, cudaStream_t stream) {
+int b200_clip_accum(const void* g, int g_is_bf16, float* acc, long long n, float clip, float scale,
+                    int init, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "clip_accum: empty");
-  B200_CHECK_ARG(aligned16(g) && aligned16(acc), "clip_accum: buffers must be 16-byte aligned");
+  B200_CHECK_ARG(al16(g) && al16(acc), "clip_accum: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (g_is_bf16)
-    clip_accum_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>((const __nv_bfloat16*)g, acc,
-                                                                     n, clip, scale, init);
+    clip_accum_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>((const __nv_bfloat16*)g, acc,
+                                                                n, clip, scale, init);
   else
-    clip_accum_kernel<float><<<grid, EW_THREADS, 0, stream>>>((const float*)g, acc, n, clip, scale,
-                                                             init);
+    clip_accum_kernel<float><<<grid, EW_THREADS, 0, s>>>((const float*)g, acc, n, clip, scale,
+                                                        init);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int sumsq(const void* x, int x_is_bf16, float* out, long long numel, int batch, int zero_first,
-          void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_sumsq(const void* x, int x_is_bf16, float* out, long long numel, int batch, int zero_first,
+               void* ws, size_t ws_bytes, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(numel > 0 && batch > 0, "sumsq: empty");
-  B200_CHECK_ARG(aligned16(x) && (batch == 1 || numel % 8 == 0), "sumsq: alignment");
+  B200_CHECK_ARG(al16(x) && (batch == 1 || numel % 8 == 0), "sumsq: alignment");
   int gx = ew_grid(numel / 8 + 1);
   const int cap = (num_sms() * 8 + batch - 1) / batch;
   if (gx > cap) gx = cap < 1 ? 1 : cap;
   dim3 grid(gx, batch);
   float* partials;
   unsigned* counters;
-  if (int rc = reduce_ws(ws, ws_bytes, batch, gx, &partials, &counters, stream)) return rc;
+  if (int rc = reduce_ws(ws, ws_bytes, batch, gx, &partials, &counters, s)) return rc;
   if (x_is_bf16)
-    sumsq_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>((const __nv_bfloat16*)x, out, numel,
-                                                                zero_first ? 0 : 1, partials, counters);
+    sumsq_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>((const __nv_bfloat16*)x, out, numel,
+                                                           zero_first ? 0 : 1, partials, counters);
   else
-    sumsq_kernel<float><<<grid, EW_THREADS, 0, stream>>>((const float*)x, out, numel, zero_first ? 0 : 1,
-                                                        partials, counters);
+    sumsq_kernel<float><<<grid, EW_THREADS, 0, s>>>((const float*)x, out, numel, zero_first ? 0 : 1,
+                                                   partials, counters);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int split_bf16(const float* src, long long ld_src, void* hi, void* lo, long long ld_dst, int rows,
-               int cols, float scale, float diag_add, cudaStream_t stream) {
+int b200_split_bf16(const float* src, long long ld_src, void* hi, void* lo, long long ld_dst, int rows,
+                    int cols, float scale, float diag_add, void* stream) {
   B200_CHECK_ARG(rows > 0 && cols > 0, "split_bf16: empty");
   const int grid = ew_grid((long long)rows * cols);
-  split_bf16_kernel<<<grid, EW_THREADS, 0, stream>>>(src, ld_src, (__nv_bfloat16*)hi,
-                                                     (__nv_bfloat16*)lo, ld_dst, rows, cols, scale,
-                                                     diag_add);
+  split_bf16_kernel<<<grid, EW_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+      src, ld_src, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, ld_dst, rows, cols, scale, diag_add);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int ema_split(const void* g, int g_is_bf16, float* m, float* out32, void* hi, void* lo, long long n,
-              float beta, float gscale, float inv_bc, float out_scale, cudaStream_t stream) {
+int b200_ema_split(const void* g, int g_is_bf16, float* m, float* out32, void* hi, void* lo, long long n,
+                   float beta, float gscale, float inv_bc, float out_scale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0, "ema_split: empty");
-  B200_CHECK_ARG(aligned16(g) && aligned16(m) && aligned16(out32) && aligned16(hi) && aligned16(lo),
+  B200_CHECK_ARG(al16(g) && al16(m) && al16(out32) && al16(hi) && al16(lo),
                  "ema_split: buffers must be 16-byte aligned");
   const int grid = ew_grid(n / 8 + 1);
   if (g_is_bf16)
-    ema_split_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, stream>>>(
+    ema_split_kernel<__nv_bfloat16><<<grid, EW_THREADS, 0, s>>>(
         (const __nv_bfloat16*)g, m, out32, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, n, beta, gscale, inv_bc, out_scale);
   else
-    ema_split_kernel<float><<<grid, EW_THREADS, 0, stream>>>(
+    ema_split_kernel<float><<<grid, EW_THREADS, 0, s>>>(
         (const float*)g, m, out32, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, n, beta, gscale, inv_bc, out_scale);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int graft_update(float* p32, void* p16, const float* pre, const float* d, long long numel, int batch,
-                 const float* coef, const float* coef_d, float decay, cudaStream_t stream) {
+int b200_graft_update(float* p32, void* p16, const float* pre, const float* d, long long numel, int batch,
+                      const float* coef, const float* coef_d, float decay, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(numel > 0 && batch > 0, "graft_update: empty");
-  B200_CHECK_ARG(aligned16(p32) && aligned16(p16) && aligned16(pre) && aligned16(d) &&
+  B200_CHECK_ARG(al16(p32) && al16(p16) && al16(pre) && al16(d) &&
                      (batch == 1 || numel % 8 == 0),
                  "graft_update: buffers must be 16-byte aligned (batched: numel %% 8 == 0)");
   int gx = ew_grid(numel / 8 + 1);
   const int cap = (num_sms() * 8 + batch - 1) / batch;
   if (gx > cap) gx = cap < 1 ? 1 : cap;
   dim3 grid(gx, batch);
-  graft_update_kernel<<<grid, EW_THREADS, 0, stream>>>(p32, (__nv_bfloat16*)p16, pre, d, numel, coef,
-                                                       coef_d, decay);
+  graft_update_kernel<<<grid, EW_THREADS, 0, s>>>(p32, (__nv_bfloat16*)p16, pre, d, numel, coef,
+                                                  coef_d, decay);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -875,7 +875,7 @@ int gemm_bf16_ex(bool a_mn, bool b_mn, int M, int N, int K, int batch, const voi
   return launch(a, 1, stream);
 }
 
-// Internal C++ entry (also used by the Newton-Schulz / Shampoo drivers).
+// b200_gemm_bf16 with bool layout flags (also used by the Newton-Schulz / Shampoo drivers).
 int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
               long long strideA, const void* B, long long ldb, long long strideB, const void* C,
               long long ldc, long long strideC, void* D, long long ldd, long long strideD,
@@ -913,7 +913,8 @@ int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* 
 // down(silu(gate(x)) * up(x))) ----------------------------------------------------------------------------------
 // gu[M, 2I] = x[M, K] [Wg ; Wu]^T (W2: [2I, K] row-major, gate rows first), y[M, I] = g * sigmoid(u) * 2, or
 // silu(g) * u with `silu`
-int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, int silu, cudaStream_t stream) {
+static int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, int silu,
+                        cudaStream_t stream) {
   B200_CHECK_ARG(M > 0 && K > 0 && I > 0 && K % 8 == 0 && I % 128 == 0,
                  "mlp_glu_fwd: need K %% 8 == 0 and intermediate size %% 128 == 0 (M=%d K=%d I=%d)", M, K, I);
   Args a;
@@ -935,8 +936,8 @@ int gemm_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K,
 // dgu[M, 2I] = GLU adjoint of d = dy[M, H] Wd (Wd: [H, I] row-major = down_proj.weight), gu[M, 2I] the saved
 // forward activations: dg = d * sigmoid(u) * 2 ; du = d * g * sigmoid(u) * (1 - sigmoid(u)) * 2, or with `silu`
 // dg = d * u * sigmoid(g) * (1 + g * (1 - sigmoid(g))) ; du = d * silu(g)
-int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I, int silu,
-                 cudaStream_t stream) {
+static int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I, int silu,
+                        cudaStream_t stream) {
   B200_CHECK_ARG(M > 0 && H > 0 && I > 0 && H % 8 == 0 && I % 8 == 0, "mlp_glu_bwd: bad shape M=%d H=%d I=%d", M, H, I);
   Args a;
   int rc;
@@ -959,7 +960,7 @@ int gemm_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int 
 // ---- grouped launch: up to MAX_PROBLEMS independent batched problems in one grid ----------------------------
 // Problems are bf16-out; `k_splits` > 1 requests split-K into fp32 slabs (splitk_ws) + a finalize pass.  Work
 // items are ordered heaviest K range first, so the tail of the launch is made of the cheapest tiles.
-int gemm_grouped(const GroupedGemm* probs, int n, cudaStream_t stream) {
+int gemm_grouped(const b200_gemm_problem* probs, int n, cudaStream_t stream) {
   B200_CHECK_ARG(n >= 1 && n <= MAX_PROBLEMS, "grouped gemm: %d problems (1..%d supported)", n, MAX_PROBLEMS);
   int order[MAX_PROBLEMS];
   for (int i = 0; i < n; ++i) order[i] = i;
@@ -976,7 +977,7 @@ int gemm_grouped(const GroupedGemm* probs, int n, cudaStream_t stream) {
     }
   Args a;
   for (int oi = 0; oi < n; ++oi) {
-    const GroupedGemm& h = probs[order[oi]];
+    const b200_gemm_problem& h = probs[order[oi]];
     B200_CHECK_ARG(h.M > 0 && h.N > 0 && h.K > 0 && h.batch > 0 && h.N % 8 == 0,
                    "grouped gemm: problem %d has an unsupported shape M=%d N=%d K=%d batch=%d", order[oi], h.M, h.N,
                    h.K, h.batch);
@@ -1118,3 +1119,58 @@ int moe_wgrad(const void* P, long long ldp, const void* Q, long long ldq, void* 
 }
 
 }  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_gemm_bf16(int a_mn, int b_mn, int M, int N, int K, int batch, const void* A,
+                   long long lda, long long strideA, const void* B, long long ldb,
+                   long long strideB, const void* C, long long ldc, long long strideC, void* D,
+                   long long ldd, long long strideD, int out_f32, float alpha, float beta,
+                   const float* alpha_vec, const float* beta_vec, int force_bn, void* stream) {
+  return gemm_bf16(a_mn != 0, b_mn != 0, M, N, K, batch, A, lda, strideA, B, ldb, strideB, C, ldc, strideC, D, ldd,
+                   strideD, out_f32 != 0, alpha, beta, alpha_vec, beta_vec, force_bn,
+                   static_cast<cudaStream_t>(stream));
+}
+
+// gemm_grouped trusts its callers (the Newton-Schulz drivers); from outside, check what its epilogues assume:
+// 16-byte rows and pointers, room for N columns in D, a split-K workspace when one is asked for.
+int b200_gemm_grouped(const b200_gemm_problem* problems, int n, void* stream) {
+  B200_CHECK_ARG(problems != nullptr && n >= 1, "gemm_grouped: no problems (n=%d)", n);
+  auto misaligned = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) != 0; };
+  for (int i = 0; i < n; ++i) {
+    const b200_gemm_problem& h = problems[i];
+    B200_CHECK_ARG(h.D != nullptr && h.A != nullptr && h.B != nullptr, "gemm_grouped: problem %d: null operand", i);
+    B200_CHECK_ARG(!misaligned(h.D) && !misaligned(h.C), "gemm_grouped: problem %d: C/D must be 16-byte aligned", i);
+    B200_CHECK_ARG(h.ldd >= h.N && (h.C == nullptr || h.beta == 0.0f || h.ldc >= h.N),
+                   "gemm_grouped: problem %d: ldd=%lld / ldc=%lld shorter than N=%d", i, h.ldd, h.ldc, h.N);
+    B200_CHECK_ARG(h.strideA % 8 == 0 && h.strideB % 8 == 0 && h.strideC % 8 == 0 && h.strideD % 8 == 0,
+                   "gemm_grouped: problem %d: batch strides must keep 16-byte alignment", i);
+    B200_CHECK_ARG(h.k_splits <= 1 || h.splitk_ws != nullptr, "gemm_grouped: problem %d: k_splits=%d needs splitk_ws",
+                   i, h.k_splits);
+    B200_CHECK_ARG(h.n_peers >= 0 && h.n_peers <= 7 && (h.n_peers == 0 || h.peer_D != nullptr),
+                   "gemm_grouped: problem %d: bad peer list (n_peers=%d, 0..7)", i, h.n_peers);
+    for (int p = 0; p < h.n_peers; ++p)
+      B200_CHECK_ARG(h.peer_D[p] != nullptr && !misaligned(h.peer_D[p]),
+                     "gemm_grouped: problem %d: peer %d must be a 16-byte aligned pointer", i, p);
+  }
+  return gemm_grouped(problems, n, static_cast<cudaStream_t>(stream));
+}
+
+int b200_mlp_gateup_glu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, void* stream) {
+  return gemm_glu_fwd(x, W2, gu, y, M, K, I, 0, static_cast<cudaStream_t>(stream));
+}
+int b200_mlp_down_glu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
+                          void* stream) {
+  return gemm_glu_bwd(dy, Wd, gu, dgu, M, H, I, 0, static_cast<cudaStream_t>(stream));
+}
+int b200_mlp_gateup_silu_fwd(const void* x, const void* W2, void* gu, void* y, int M, int K, int I, void* stream) {
+  return gemm_glu_fwd(x, W2, gu, y, M, K, I, 1, static_cast<cudaStream_t>(stream));
+}
+int b200_mlp_down_silu_bwd(const void* dy, const void* Wd, const void* gu, void* dgu, int M, int H, int I,
+                           void* stream) {
+  return gemm_glu_bwd(dy, Wd, gu, dgu, M, H, I, 1, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"

@@ -20,7 +20,6 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-const char* last_error() { return g_err; }
 
 // cuTensorMapEncodeTiled is a driver entry point; resolve it through the runtime so the
 // library has no link-time dependency on libcuda (the CPU build box has no driver).
@@ -60,8 +59,6 @@ std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_maps;
 std::atomic<unsigned long long> g_map_hits{0}, g_map_misses{0};
 constexpr size_t kMapCacheCap = 8192;
 }  // namespace
-unsigned long long tensor_map_cache_hits() { return g_map_hits.load(std::memory_order_relaxed); }
-unsigned long long tensor_map_cache_misses() { return g_map_misses.load(std::memory_order_relaxed); }
 
 int make_tensor_map(CUtensorMap* out, const void* base, CUtensorMapDataType dtype, int elem_bytes,
                     int rank, const uint64_t* dims, const uint64_t* strides_bytes,
@@ -135,7 +132,6 @@ int make_tensor_map(CUtensorMap* out, const void* base, CUtensorMapDataType dtyp
 
 static std::atomic<unsigned long long> g_launches{0};
 void count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
-unsigned long long launch_count() { return g_launches.load(std::memory_order_relaxed); }
 
 int num_sms() {
   static int n = 0;
@@ -149,3 +145,26 @@ int num_sms() {
 }
 
 }  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_version(void) { return 4; }
+const char* b200_last_error(void) { return g_err; }
+
+unsigned long long b200_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
+void b200_tensor_map_cache_stats(unsigned long long* hits, unsigned long long* misses) {
+  if (hits) *hits = g_map_hits.load(std::memory_order_relaxed);
+  if (misses) *misses = g_map_misses.load(std::memory_order_relaxed);
+}
+
+int b200_device_ok(void) {
+  int dev = 0, major = 0, minor = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 0;
+  if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return 0;
+  if (cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev) != cudaSuccess) return 0;
+  return (major == 9 && minor == 0) ? 1 : 0;  // the library holds sm_90a code only
+}
+
+}  // extern "C"

@@ -1,4 +1,5 @@
-// Host-side helpers shared by the C-ABI entry points: error reporting and TMA tensor maps.
+// Host-side helpers shared by the C-ABI entry points: error reporting, TMA tensor maps, and the one declaration
+// of every internal function that a source file other than its own calls.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -10,7 +11,6 @@ namespace b200 {
 
 // thread-local last error message (returned by b200_last_error())
 void set_error(const char* fmt, ...);
-const char* last_error();
 
 // error codes: B200_OK / B200_ERR_* macros from the public header
 
@@ -34,18 +34,6 @@ const char* last_error();
 
 // every kernel launch of the library is counted (bench.py reports it as gpu_launches)
 void count_launch();
-// one deferred RMSNorm weight-gradient reduction (mirrors b200_dw_job of include/b200_hotpath.h)
-struct DwJob {
-  const float* partials;  // [n_partials][H] fp32, left in the workspace by (add_)rmsnorm_bwd with dw == nullptr
-  void* dw;               // [H] bf16 or fp32
-  int n_partials;
-  int dw_is_bf16;
-  int accumulate;         // 1: dw += sum, 0: dw = sum
-  int reserved;
-};
-unsigned long long launch_count();
-unsigned long long tensor_map_cache_hits();     // make_tensor_map calls answered from the descriptor cache
-unsigned long long tensor_map_cache_misses();   // ... that went to cuTensorMapEncodeTiled
 
 #define B200_CHECK_LAUNCH()                  \
   do {                                       \
@@ -62,6 +50,11 @@ int make_tensor_map(CUtensorMap* out, const void* base, CUtensorMapDataType dtyp
 
 int num_sms();
 
+// 16-byte alignment test, 256-byte round-up of workspace slices, round-up to a multiple of 8
+inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+inline size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
+inline int rup8(int k) { return (k + 7) & ~7; }
+
 // attention dropout: keep threshold t = min(rint(p 65536), 65535) on 16-bit uniforms (p in [0, 1)), and the fp32
 // scale 1 / (1 - p_eff) of p_eff = t / 65536
 inline uint32_t dropout_threshold(float p) {
@@ -70,29 +63,30 @@ inline uint32_t dropout_threshold(float p) {
 }
 inline float dropout_scale(uint32_t t) { return (float)(65536.0 / (65536.0 - (double)t)); }
 
-// One problem of a grouped GEMM launch (gemm_wgmma.cu: gemm_grouped): D = alpha*av[b]*op(A)op(B) +
-// beta*bv[b]*C, bf16 in/out, batched; layouts as in b200_gemm_bf16.  Mirrors b200_gemm_problem of the public
-// header field for field.
-struct GroupedGemm {
-  int a_mn, b_mn;
-  int M, N, K, batch;
-  const void* A;
-  long long lda, strideA;
-  const void* B;
-  long long ldb, strideB;
-  const void* C;
-  long long ldc, strideC;
-  void* D;
-  long long ldd, strideD;
-  float alpha, beta;
-  const float* alpha_vec;
-  const float* beta_vec;
-  int symmetric;     // D == D^T asserted by the caller: compute the upper triangle of tiles, mirror the rest
-  int k_splits;      // > 1: split-K into fp32 slabs `splitk_ws` ([k_splits][batch][M][N]) + finalize
-  float* splitk_ws;
-  const void* const* peer_D;  // GEMM -> all-gather: peer-mapped copies of D (n_peers <= 7)
-  int n_peers;
-};
-int gemm_grouped(const GroupedGemm* probs, int n, cudaStream_t stream);
+// ---- the wgmma GEMM engine (gemm_wgmma.cu), shared by the Newton-Schulz, Shampoo and MoE drivers ----
+// b200_gemm_bf16 with bool layout flags
+int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
+              long long strideA, const void* B, long long ldb, long long strideB, const void* C,
+              long long ldc, long long strideC, void* D, long long ldd, long long strideD,
+              bool out_f32, float alpha, float beta, const float* alpha_vec, const float* beta_vec,
+              int force_bn, cudaStream_t stream);
+// gemm_bf16 plus symmetric tiles, split-K and peer stores, without argument checks
+int gemm_bf16_ex(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
+                 long long strideA, const void* B, long long ldb, long long strideB, const void* C,
+                 long long ldc, long long strideC, void* D, long long ldd, long long strideD, bool out_f32,
+                 float alpha, float beta, const float* alpha_vec, const float* beta_vec, int symmetric,
+                 int k_splits, float* splitk_ws, const void* const* peer_D, int n_peers, cudaStream_t stream);
+// b200_gemm_grouped without the entry's pointer, stride and peer-list validation
+int gemm_grouped(const b200_gemm_problem* probs, int n, cudaStream_t stream);
+// b200_moe_gemm with Wu at up_off [I, H] matrices after Wg (modes 0 and 3), and b200_moe_wgrad
+int moe_gemm(int mode, int silu, const void* A, const void* Wg, int up_off, const void* Wd, const void* gu, void* C,
+             void* Y, const int* tile_expert, const int* n_tiles, int max_tiles, int H, int I, int E,
+             cudaStream_t stream);
+int moe_wgrad(const void* P, long long ldp, const void* Q, long long ldq, void* G, int R, int Cc, int E, int rows,
+              const int* counts, const int* seg_off, cudaStream_t stream);
+
+// ---- attention (attention_fwd.cu, also used by attention_bwd.cu) ----
+// [B, S, heads, D] bf16 tensor -> 4-D tensor map {D, heads, S, B}, box {64, 1, rows, 1}, 128B swizzle
+int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, int D, int box_rows);
 
 }  // namespace b200

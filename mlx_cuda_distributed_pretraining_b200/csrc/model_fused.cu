@@ -242,96 +242,107 @@ inline int grid_for(long long nvec) {
   const long long cap = (long long)num_sms() * 8;
   return (int)(b > cap ? cap : (b < 1 ? 1 : b));
 }
-inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 }  // namespace
+}  // namespace b200
 
-int glu_fwd(const void* g, const void* u, void* y, long long n, cudaStream_t stream) {
+using namespace b200;
+
+extern "C" {
+
+int b200_glu_fwd(const void* g, const void* u, void* y, long long n, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n > 0 && n % 8 == 0, "glu_fwd: n=%lld must be a positive multiple of 8", n);
   B200_CHECK_ARG(al16(g) && al16(u) && al16(y), "glu_fwd: 16-byte alignment required");
-  glu_fwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>((const __nv_bfloat16*)g, (const __nv_bfloat16*)u,
+  glu_fwd_kernel<<<grid_for(n / 8), 256, 0, s>>>((const __nv_bfloat16*)g, (const __nv_bfloat16*)u,
+                                                (__nv_bfloat16*)y, n / 8);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+int b200_glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  B200_CHECK_ARG(n > 0 && n % 8 == 0, "glu_bwd: n=%lld must be a positive multiple of 8", n);
+  B200_CHECK_ARG(al16(dy) && al16(g) && al16(u) && al16(dg) && al16(du), "glu_bwd: alignment");
+  glu_bwd_kernel<<<grid_for(n / 8), 256, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)g,
+                                                (const __nv_bfloat16*)u, (__nv_bfloat16*)dg,
+                                                (__nv_bfloat16*)du, n / 8);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+int b200_silu_glu_fwd(const void* g, const void* u, void* y, long long n, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  B200_CHECK_ARG(n > 0 && n % 8 == 0, "silu_glu_fwd: n=%lld must be a positive multiple of 8", n);
+  B200_CHECK_ARG(al16(g) && al16(u) && al16(y), "silu_glu_fwd: 16-byte alignment required");
+  silu_glu_fwd_kernel<<<grid_for(n / 8), 256, 0, s>>>((const __nv_bfloat16*)g, (const __nv_bfloat16*)u,
                                                      (__nv_bfloat16*)y, n / 8);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, cudaStream_t stream) {
-  B200_CHECK_ARG(n > 0 && n % 8 == 0, "glu_bwd: n=%lld must be a positive multiple of 8", n);
-  B200_CHECK_ARG(al16(dy) && al16(g) && al16(u) && al16(dg) && al16(du), "glu_bwd: alignment");
-  glu_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)g,
+int b200_silu_glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  B200_CHECK_ARG(n > 0 && n % 8 == 0, "silu_glu_bwd: n=%lld must be a positive multiple of 8", n);
+  B200_CHECK_ARG(al16(dy) && al16(g) && al16(u) && al16(dg) && al16(du), "silu_glu_bwd: alignment");
+  silu_glu_bwd_kernel<<<grid_for(n / 8), 256, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)g,
                                                      (const __nv_bfloat16*)u, (__nv_bfloat16*)dg,
                                                      (__nv_bfloat16*)du, n / 8);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int silu_glu_fwd(const void* g, const void* u, void* y, long long n, cudaStream_t stream) {
-  B200_CHECK_ARG(n > 0 && n % 8 == 0, "silu_glu_fwd: n=%lld must be a positive multiple of 8", n);
-  B200_CHECK_ARG(al16(g) && al16(u) && al16(y), "silu_glu_fwd: 16-byte alignment required");
-  silu_glu_fwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>((const __nv_bfloat16*)g, (const __nv_bfloat16*)u,
-                                                          (__nv_bfloat16*)y, n / 8);
-  B200_CHECK_LAUNCH();
-  return B200_OK;
-}
+size_t b200_embedding_bwd_workspace_bytes(int V, int H) { return (size_t)V * H * sizeof(float); }
 
-int silu_glu_bwd(const void* dy, const void* g, const void* u, void* dg, void* du, long long n, cudaStream_t stream) {
-  B200_CHECK_ARG(n > 0 && n % 8 == 0, "silu_glu_bwd: n=%lld must be a positive multiple of 8", n);
-  B200_CHECK_ARG(al16(dy) && al16(g) && al16(u) && al16(dg) && al16(du), "silu_glu_bwd: alignment");
-  silu_glu_bwd_kernel<<<grid_for(n / 8), 256, 0, stream>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)g,
-                                                          (const __nv_bfloat16*)u, (__nv_bfloat16*)dg,
-                                                          (__nv_bfloat16*)du, n / 8);
-  B200_CHECK_LAUNCH();
-  return B200_OK;
-}
-
-size_t embedding_bwd_workspace_bytes(int V, int H) { return (size_t)V * H * sizeof(float); }
-
-int embedding_bwd(const void* dh, const long long* tokens, void* grad, int grad_is_bf16, long long rows, int V, int H,
-                  void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_embedding_bwd(const void* dh, const long long* tokens, void* grad, int grad_is_bf16, long long rows, int V,
+                       int H, void* ws, size_t ws_bytes, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(rows > 0 && V > 0 && H > 0 && H % 8 == 0, "embedding_bwd: bad shape rows=%lld V=%d H=%d", rows, V, H);
-  if (ws == nullptr || ws_bytes < embedding_bwd_workspace_bytes(V, H)) {
-    set_error("embedding_bwd: workspace too small (%zu < %zu)", ws_bytes, embedding_bwd_workspace_bytes(V, H));
+  if (ws == nullptr || ws_bytes < b200_embedding_bwd_workspace_bytes(V, H)) {
+    set_error("embedding_bwd: workspace too small (%zu < %zu)", ws_bytes, b200_embedding_bwd_workspace_bytes(V, H));
     return B200_ERR_WORKSPACE;
   }
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 15u) == 0 && (reinterpret_cast<uintptr_t>(grad) & 15u) == 0 &&
                      (reinterpret_cast<uintptr_t>(dh) & 15u) == 0,
                  "embedding_bwd: buffers must be 16-byte aligned");
   float* scratch = reinterpret_cast<float*>(ws);
-  B200_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (size_t)V * H * sizeof(float), stream));
+  B200_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (size_t)V * H * sizeof(float), s));
   long long blocks = (rows + 7) / 8;
   const long long cap = (long long)num_sms() * 8;
   if (blocks > cap) blocks = cap;
-  embedding_scatter_kernel<<<(int)blocks, 256, 0, stream>>>((const __nv_bfloat16*)dh, tokens, scratch, rows, H, V);
+  embedding_scatter_kernel<<<(int)blocks, 256, 0, s>>>((const __nv_bfloat16*)dh, tokens, scratch, rows, H, V);
   B200_CHECK_LAUNCH();
   const long long nvec = (long long)V * H / 8;
   long long b2 = (nvec + 255) / 256;
   if (b2 > cap) b2 = cap;
   if (grad_is_bf16)
-    embedding_accumulate_kernel<__nv_bfloat16><<<(int)b2, 256, 0, stream>>>(scratch, (__nv_bfloat16*)grad, nvec);
+    embedding_accumulate_kernel<__nv_bfloat16><<<(int)b2, 256, 0, s>>>(scratch, (__nv_bfloat16*)grad, nvec);
   else
-    embedding_accumulate_kernel<float><<<(int)b2, 256, 0, stream>>>(scratch, (float*)grad, nvec);
+    embedding_accumulate_kernel<float><<<(int)b2, 256, 0, s>>>(scratch, (float*)grad, nvec);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int ce_fwd(const void* logits, long long ld, const long long* targets, int rows, int V, long long pad_token,
-           float* row_loss, float* row_lse, cudaStream_t stream) {
+int b200_ce_fwd(const void* logits, long long ld, const long long* targets, int rows, int V, long long pad_token,
+                float* row_loss, float* row_lse, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(rows > 0 && V > 0 && ld >= V && ld % 8 == 0, "ce_fwd: bad shape rows=%d V=%d ld=%lld", rows, V, ld);
   B200_CHECK_ARG(al16(logits), "ce_fwd: logits must be 16-byte aligned");
-  ce_fwd_kernel<<<rows, CE_THREADS, 0, stream>>>((const __nv_bfloat16*)logits, ld, targets, V, pad_token, row_loss,
-                                                 row_lse);
+  ce_fwd_kernel<<<rows, CE_THREADS, 0, s>>>((const __nv_bfloat16*)logits, ld, targets, V, pad_token, row_loss,
+                                            row_lse);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-int ce_bwd(void* logits, long long ld, const long long* targets, int rows, int V, long long pad_token,
-           const float* row_lse, const float* row_scale, cudaStream_t stream) {
+int b200_ce_bwd(void* logits, long long ld, const long long* targets, int rows, int V, long long pad_token,
+                const float* row_lse, const float* row_scale, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(rows > 0 && V > 0 && ld >= V && ld % 8 == 0, "ce_bwd: bad shape rows=%d V=%d ld=%lld", rows, V, ld);
   B200_CHECK_ARG(al16(logits), "ce_bwd: logits must be 16-byte aligned");
-  ce_bwd_kernel<<<rows, CE_THREADS, 0, stream>>>((__nv_bfloat16*)logits, ld, targets, V, pad_token, row_lse,
-                                                 row_scale);
+  ce_bwd_kernel<<<rows, CE_THREADS, 0, s>>>((__nv_bfloat16*)logits, ld, targets, V, pad_token, row_lse,
+                                            row_scale);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -290,28 +290,19 @@ __global__ void combine_bwd_kernel(const __nv_bfloat16* __restrict__ dout, const
 
 size_t route_ws_layout(int T, int E, int k, size_t* o_rank, size_t* o_hist, size_t* o_mhist, size_t* o_psum) {
   const size_t nch = (size_t)(T + CHUNK - 1) / CHUNK;
-  auto al = [](size_t x) { return (x + 255) / 256 * 256; };
   size_t o = 0;
   *o_rank = o;
-  o += al((size_t)T * k * 4);
+  o += al256((size_t)T * k * 4);
   *o_hist = o;
-  o += al(nch * E * 4);
+  o += al256(nch * E * 4);
   *o_mhist = o;
-  o += al(nch * E * 4);
+  o += al256(nch * E * 4);
   *o_psum = o;
-  o += al(nch * E * 4);
+  o += al256(nch * E * 4);
   return o;
 }
 
 }  // namespace
-}  // namespace b200
-
-namespace b200 {
-int moe_gemm(int mode, int silu, const void* A, const void* Wg, int up_off, const void* Wd, const void* gu, void* C,
-             void* Y, const int* tile_expert, const int* n_tiles, int max_tiles, int H, int I, int E,
-             cudaStream_t stream);
-int moe_wgrad(const void* P, long long ldp, const void* Q, long long ldq, void* G, int R, int Cc, int E, int rows,
-              const int* counts, const int* seg_off, cudaStream_t stream);
 }  // namespace b200
 
 using namespace b200;

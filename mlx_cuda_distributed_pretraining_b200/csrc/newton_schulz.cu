@@ -14,31 +14,6 @@
 
 namespace b200 {
 
-int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
-              long long strideA, const void* B, long long ldb, long long strideB, const void* C,
-              long long ldc, long long strideC, void* D, long long ldd, long long strideD,
-              bool out_f32, float alpha, float beta, const float* alpha_vec, const float* beta_vec,
-              int force_bn, cudaStream_t stream);
-
-int gemm_bf16_ex(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
-                   long long strideA, const void* B, long long ldb, long long strideB, const void* C,
-                   long long ldc, long long strideC, void* D, long long ldd, long long strideD, bool out_f32,
-                   float alpha, float beta, const float* alpha_vec, const float* beta_vec, int symmetric, int k_splits, float* splitk_ws, const void* const* peer_D, int n_peers,
-                   cudaStream_t stream);
-
-static inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
-// One shape group of the whole-model chain (mirrors b200_ns_group of the public header)
-struct NsGroup {
-  const void* x_in;
-  void* x_out;
-  int batch, rows, cols;
-  const float* inv_norm;
-  const float* inv_norm_sq;
-  const void* const* peer_out;
-  int n_peers;
-};
-
 // G1 of a lone big matrix (the 32003 x 1024 embedding: 36 symmetric 128-tiles, K = 32003) would occupy a
 // fraction of the SMs for hundreds of microseconds.  Cut K so that every SM gets a work item.
 static int g1_k_splits(int batch, int m, int k) {
@@ -60,21 +35,12 @@ static const int kSym = [] {
   return (e != nullptr && e[0] == '1') ? 0 : 1256;
 }();
 
-size_t newton_schulz_workspace_bytes(int batch, int rows, int cols, int steps) {
-  const size_t m = rows < cols ? rows : cols;
-  size_t bytes = 2 * align256((size_t)batch * m * m * 2);
-  if (steps >= 2) bytes += align256((size_t)batch * rows * cols * 2);
-  const int splits = g1_k_splits(batch, (int)m, rows < cols ? cols : rows);
-  if (splits > 1) bytes += align256((size_t)splits * batch * m * m * 4);
-  return bytes;
-}
-
 // peer_out / n_peers: peer-mapped copies of x_out on other GPUs (owner-computes Newton-Schulz under data
 // parallelism).  The LAST iteration's X' = aX + BX GEMM then stores its tiles to x_out and to every peer
 // from its epilogue (GEMM -> all-gather in one kernel); with n_peers == 0 this is the plain chain.
-int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, int steps, float a,
-                  float b, float c, const float* inv_norm, const float* inv_norm_sq, void* ws,
-                  size_t ws_bytes, const void* const* peer_out, int n_peers, cudaStream_t stream) {
+static int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, int steps, float a,
+                         float b, float c, const float* inv_norm, const float* inv_norm_sq, void* ws,
+                         size_t ws_bytes, const void* const* peer_out, int n_peers, cudaStream_t stream) {
   B200_CHECK_ARG(n_peers >= 0 && n_peers <= 7 && (n_peers == 0 || peer_out != nullptr),
                  "newton_schulz: bad peer list (n_peers=%d)", n_peers);
   B200_CHECK_ARG(batch > 0 && rows > 0 && cols > 0 && steps > 0,
@@ -83,9 +49,9 @@ int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, 
   B200_CHECK_ARG(cols % 8 == 0, "newton_schulz: cols=%d must be a multiple of 8 (16-byte rows)",
                  cols);
   B200_CHECK_ARG(x_in != x_out, "newton_schulz: x_in and x_out must be distinct buffers");
-  if (ws_bytes < newton_schulz_workspace_bytes(batch, rows, cols, steps)) {
+  if (ws_bytes < b200_newton_schulz_workspace_bytes(batch, rows, cols, steps)) {
     set_error("newton_schulz: workspace too small (%zu < %zu)", ws_bytes,
-              newton_schulz_workspace_bytes(batch, rows, cols, steps));
+              b200_newton_schulz_workspace_bytes(batch, rows, cols, steps));
     return B200_ERR_WORKSPACE;
   }
   const bool tall = rows > cols;
@@ -94,11 +60,11 @@ int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, 
   const long long rc = (long long)rows * cols;
   char* w = reinterpret_cast<char*>(ws);
   void* Abuf = w;
-  void* Bbuf = w + align256((size_t)batch * mm * 2);
-  void* Xtmp = w + 2 * align256((size_t)batch * mm * 2);
+  void* Bbuf = w + al256((size_t)batch * mm * 2);
+  void* Xtmp = w + 2 * al256((size_t)batch * mm * 2);
   const int splits = g1_k_splits(batch, m, tall ? rows : cols);
   float* splitk_ws = reinterpret_cast<float*>(
-      w + 2 * align256((size_t)batch * mm * 2) + (steps >= 2 ? align256((size_t)batch * rc * 2) : 0));
+      w + 2 * al256((size_t)batch * mm * 2) + (steps >= 2 ? al256((size_t)batch * rc * 2) : 0));
 
   const void* cur = x_in;
   for (int it = 0; it < steps; ++it) {
@@ -146,7 +112,7 @@ int newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, 
 // 3 x groups, and the per-launch wave tail is amortised over all groups' tiles.  Falls back to the per-group
 // chain for small groups (min(rows, cols) <= 128) or when there are more groups than one launch takes.
 // ---------------------------------------------------------------------------------------------------------
-static bool multi_grouped_ok(const NsGroup* g, int n) {
+static bool multi_grouped_ok(const b200_ns_group* g, int n) {
   static const bool off = [] {
     const char* e = getenv("B200_NS_GROUPED");
     return e != nullptr && e[0] == '0';
@@ -163,30 +129,61 @@ struct NsLayout {  // workspace slices of one group
   size_t a, b, xtmp, splitk, end;
   int splits;
 };
-static NsLayout ns_layout(const NsGroup& g, int steps, size_t base) {
+static NsLayout ns_layout(const b200_ns_group& g, int steps, size_t base) {
   const size_t m = g.rows < g.cols ? g.rows : g.cols;
   NsLayout l;
   l.a = base;
-  l.b = l.a + align256((size_t)g.batch * m * m * 2);
-  l.xtmp = l.b + align256((size_t)g.batch * m * m * 2);
-  l.splitk = l.xtmp + (steps >= 2 ? align256((size_t)g.batch * g.rows * g.cols * 2) : 0);
+  l.b = l.a + al256((size_t)g.batch * m * m * 2);
+  l.xtmp = l.b + al256((size_t)g.batch * m * m * 2);
+  l.splitk = l.xtmp + (steps >= 2 ? al256((size_t)g.batch * g.rows * g.cols * 2) : 0);
   l.splits = g1_k_splits(g.batch, (int)m, g.rows < g.cols ? g.cols : g.rows);
-  l.end = l.splitk + (l.splits > 1 ? align256((size_t)l.splits * g.batch * m * m * 4) : 0);
+  l.end = l.splitk + (l.splits > 1 ? al256((size_t)l.splits * g.batch * m * m * 4) : 0);
   return l;
 }
 
-size_t newton_schulz_multi_workspace_bytes(const NsGroup* g, int n, int steps) {
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+size_t b200_newton_schulz_workspace_bytes(int batch, int rows, int cols, int steps) {
+  const size_t m = rows < cols ? rows : cols;
+  size_t bytes = 2 * al256((size_t)batch * m * m * 2);
+  if (steps >= 2) bytes += al256((size_t)batch * rows * cols * 2);
+  const int splits = g1_k_splits(batch, (int)m, rows < cols ? cols : rows);
+  if (splits > 1) bytes += al256((size_t)splits * batch * m * m * 4);
+  return bytes;
+}
+
+int b200_newton_schulz(const void* x_in, void* x_out, int batch, int rows, int cols, int steps,
+                       float a, float b, float c, const float* inv_norm, const float* inv_norm_sq,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+  return newton_schulz(x_in, x_out, batch, rows, cols, steps, a, b, c, inv_norm, inv_norm_sq, workspace,
+                       workspace_bytes, nullptr, 0, static_cast<cudaStream_t>(stream));
+}
+
+int b200_newton_schulz_allgather(const void* x_in, void* x_out, int batch, int rows, int cols, int steps,
+                                 float a, float b, float c, const float* inv_norm, const float* inv_norm_sq,
+                                 void* workspace, size_t workspace_bytes, const void* const* peer_out,
+                                 int n_peers, void* stream) {
+  return newton_schulz(x_in, x_out, batch, rows, cols, steps, a, b, c, inv_norm, inv_norm_sq, workspace,
+                       workspace_bytes, peer_out, n_peers, static_cast<cudaStream_t>(stream));
+}
+
+size_t b200_newton_schulz_multi_workspace_bytes(const b200_ns_group* g, int n, int steps) {
   size_t off = 0;
   for (int i = 0; i < n; ++i) {
     const size_t grouped_end = ns_layout(g[i], steps, off).end;
-    const size_t single_end = off + newton_schulz_workspace_bytes(g[i].batch, g[i].rows, g[i].cols, steps);
+    const size_t single_end = off + b200_newton_schulz_workspace_bytes(g[i].batch, g[i].rows, g[i].cols, steps);
     off = grouped_end > single_end ? grouped_end : single_end;
   }
   return off;
 }
 
-int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, float c, void* ws, size_t ws_bytes,
-                        cudaStream_t stream) {
+int b200_newton_schulz_multi(const b200_ns_group* g, int n, int steps, float a, float b, float c, void* ws,
+                             size_t ws_bytes, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(n >= 1 && g != nullptr && steps > 0, "newton_schulz_multi: bad arguments (n=%d steps=%d)", n, steps);
   for (int i = 0; i < n; ++i) {
     B200_CHECK_ARG(g[i].batch > 0 && g[i].rows > 0 && g[i].cols > 0 && g[i].cols % 8 == 0,
@@ -196,9 +193,9 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
     B200_CHECK_ARG(g[i].n_peers >= 0 && g[i].n_peers <= 7 && (g[i].n_peers == 0 || g[i].peer_out != nullptr),
                    "newton_schulz_multi: group %d: bad peer list", i);
   }
-  if (ws_bytes < newton_schulz_multi_workspace_bytes(g, n, steps)) {
+  if (ws_bytes < b200_newton_schulz_multi_workspace_bytes(g, n, steps)) {
     set_error("newton_schulz_multi: workspace too small (%zu < %zu)", ws_bytes,
-              newton_schulz_multi_workspace_bytes(g, n, steps));
+              b200_newton_schulz_multi_workspace_bytes(g, n, steps));
     return B200_ERR_WORKSPACE;
   }
   char* w = reinterpret_cast<char*>(ws);
@@ -206,9 +203,9 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
     size_t off = 0;
     for (int i = 0; i < n; ++i) {
       const size_t grouped_end = ns_layout(g[i], steps, off).end;
-      const size_t need = newton_schulz_workspace_bytes(g[i].batch, g[i].rows, g[i].cols, steps);
+      const size_t need = b200_newton_schulz_workspace_bytes(g[i].batch, g[i].rows, g[i].cols, steps);
       int rc = newton_schulz(g[i].x_in, g[i].x_out, g[i].batch, g[i].rows, g[i].cols, steps, a, b, c, g[i].inv_norm,
-                             g[i].inv_norm_sq, w + off, need, g[i].peer_out, g[i].n_peers, stream);
+                             g[i].inv_norm_sq, w + off, need, g[i].peer_out, g[i].n_peers, s);
       if (rc) return rc;
       off = grouped_end > off + need ? grouped_end : off + need;
     }
@@ -220,12 +217,12 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
     size_t off = 0;
     for (int i = 0; i < n; ++i) {
       lay[i] = ns_layout(g[i], steps, off);
-      const size_t single_end = off + newton_schulz_workspace_bytes(g[i].batch, g[i].rows, g[i].cols, steps);
+      const size_t single_end = off + b200_newton_schulz_workspace_bytes(g[i].batch, g[i].rows, g[i].cols, steps);
       off = lay[i].end > single_end ? lay[i].end : single_end;
       cur[i] = g[i].x_in;
     }
   }
-  GroupedGemm pr[6];
+  b200_gemm_problem pr[6];
   for (int it = 0; it < steps; ++it) {
     const bool first = it == 0, last = it == steps - 1;
     // ---- G1: A = X X^T (wide) / X^T X (tall), symmetric; iteration 1 carries 1/(||G||+eps)^2 ----
@@ -233,8 +230,8 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       const bool tall = g[i].rows > g[i].cols;
       const int m = tall ? g[i].cols : g[i].rows;
       const long long rc_ = (long long)g[i].rows * g[i].cols, mm = (long long)m * m;
-      GroupedGemm& q = pr[i];
-      q = GroupedGemm{};
+      b200_gemm_problem& q = pr[i];
+      q = b200_gemm_problem{};
       q.a_mn = tall;
       q.b_mn = tall;
       q.M = m;
@@ -257,14 +254,14 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       q.k_splits = lay[i].splits;
       q.splitk_ws = reinterpret_cast<float*>(w + lay[i].splitk);
     }
-    int rc = gemm_grouped(pr, n, stream);
+    int rc = gemm_grouped(pr, n, s);
     if (rc) return rc;
     // ---- G2: B = b A + c A A (A symmetric: A A^T with both operands K-major) ----
     for (int i = 0; i < n; ++i) {
       const int m = g[i].rows > g[i].cols ? g[i].cols : g[i].rows;
       const long long mm = (long long)m * m;
-      GroupedGemm& q = pr[i];
-      q = GroupedGemm{};
+      b200_gemm_problem& q = pr[i];
+      q = b200_gemm_problem{};
       q.M = q.N = q.K = m;
       q.batch = g[i].batch;
       q.A = q.B = q.C = w + lay[i].a;
@@ -276,7 +273,7 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       q.symmetric = kSym ? 1 : 0;
       q.k_splits = 1;
     }
-    rc = gemm_grouped(pr, n, stream);
+    rc = gemm_grouped(pr, n, s);
     if (rc) return rc;
     // ---- G3: X' = a X + B X (wide) / a X + X B (tall); the last one carries the peer stores ----
     for (int i = 0; i < n; ++i) {
@@ -284,8 +281,8 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       const int m = tall ? g[i].cols : g[i].rows;
       const long long rc_ = (long long)g[i].rows * g[i].cols, mm = (long long)m * m;
       void* nxt = ((steps - 1 - it) % 2 == 0) ? g[i].x_out : static_cast<void*>(w + lay[i].xtmp);
-      GroupedGemm& q = pr[i];
-      q = GroupedGemm{};
+      b200_gemm_problem& q = pr[i];
+      q = b200_gemm_problem{};
       if (!tall) {  // [m, cols] = B[m, m] (K-major) x X[m(K), cols] (MN-major)
         q.a_mn = false;
         q.b_mn = true;
@@ -329,10 +326,10 @@ int newton_schulz_multi(const NsGroup* g, int n, int steps, float a, float b, fl
       }
       cur[i] = nxt;
     }
-    rc = gemm_grouped(pr, n, stream);
+    rc = gemm_grouped(pr, n, s);
     if (rc) return rc;
   }
   return B200_OK;
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -393,11 +393,11 @@ rmsnorm_dw_reduce_kernel(const float* __restrict__ dw_part, float* __restrict__ 
 // gradient in its storage type: a Llama backward has 2 norms per layer, and each used to cost four launches (partials,
 // this reduction, a dtype copy and autograd's accumulate) -- ~100 sub-10-us kernels per C2 step, mostly launch latency.
 struct DwJobs {
-  b200::DwJob j[32];
+  b200_dw_job j[32];
 };
 __global__ void __launch_bounds__(1024) rmsnorm_dw_reduce_batched_kernel(const __grid_constant__ DwJobs jobs, int H) {
   __shared__ float part[32][33];
-  const b200::DwJob& job = jobs.j[blockIdx.y];
+  const b200_dw_job& job = jobs.j[blockIdx.y];
   const float* __restrict__ dw_part = job.partials;
   const int nblocks = job.n_partials;
   const int cx = threadIdx.x & 31, ry = threadIdx.x >> 5;
@@ -569,80 +569,6 @@ int rmsnorm_bwd_t(const T* dy, const T* dres, const T* x, const T* w, const floa
   return B200_OK;
 }
 
-inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-}  // namespace
-
-int add_rmsnorm_fwd(const void* x, const void* delta, const void* w, void* sum_out, void* y, float* rstd,
-                    int rows, int H, float eps, int is_bf16, cudaStream_t stream) {
-  B200_CHECK_ARG(rows > 0 && H > 0 && H % 8 == 0 && H <= RN_THREADS * 8 * RN_MAX_VEC,
-                 "rmsnorm_fwd: unsupported shape rows=%d H=%d (H %% 8 == 0, H <= %d)", rows, H,
-                 RN_THREADS * 8 * RN_MAX_VEC);
-  B200_CHECK_ARG(al16(x) && al16(w) && al16(y) && al16(delta) && al16(sum_out),
-                 "rmsnorm_fwd: 16-byte alignment required");
-  B200_CHECK_ARG((delta == nullptr) == (sum_out == nullptr),
-                 "add_rmsnorm_fwd: delta and sum_out must be given together");
-  if (is_bf16)
-    return rmsnorm_fwd_t<__nv_bfloat16>((const __nv_bfloat16*)x, (const __nv_bfloat16*)delta,
-                                        (const __nv_bfloat16*)w, (__nv_bfloat16*)sum_out, (__nv_bfloat16*)y,
-                                        rstd, rows, H, eps, stream);
-  return rmsnorm_fwd_t<float>((const float*)x, (const float*)delta, (const float*)w, (float*)sum_out,
-                              (float*)y, rstd, rows, H, eps, stream);
-}
-
-int rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int rows, int H, float eps,
-                int is_bf16, cudaStream_t stream) {
-  return add_rmsnorm_fwd(x, nullptr, w, nullptr, y, rstd, rows, H, eps, is_bf16, stream);
-}
-
-size_t rmsnorm_bwd_workspace_bytes(int rows, int H) {
-  return (size_t)rmsnorm_bwd_grid(rows, H) * H * sizeof(float);
-}
-
-int rmsnorm_bwd_partial_rows(int rows, int H) { return rmsnorm_bwd_grid(rows, H); }
-
-int rmsnorm_dw_reduce(const DwJob* jobs, int n_jobs, int H, cudaStream_t stream) {
-  B200_CHECK_ARG(n_jobs >= 0 && H > 0 && (jobs != nullptr || n_jobs == 0), "rmsnorm_dw_reduce: bad arguments");
-  for (int i = 0; i < n_jobs; ++i)
-    B200_CHECK_ARG(jobs[i].partials != nullptr && jobs[i].dw != nullptr && jobs[i].n_partials > 0,
-                   "rmsnorm_dw_reduce: job %d has a null pointer or no partial rows", i);
-  for (int i = 0; i < n_jobs; i += 32) {
-    DwJobs a;
-    const int n = n_jobs - i < 32 ? n_jobs - i : 32;
-    for (int k = 0; k < n; ++k) a.j[k] = jobs[i + k];
-    rmsnorm_dw_reduce_batched_kernel<<<dim3((H + 31) / 32, n), 1024, 0, stream>>>(a, H);
-    B200_CHECK_LAUNCH();
-  }
-  return B200_OK;
-}
-
-int add_rmsnorm_bwd(const void* dy, const void* dres, const void* x, const void* w, const float* rstd,
-                    void* dx, float* dw, int rows, int H, int is_bf16, void* ws, size_t ws_bytes,
-                    cudaStream_t stream) {
-  B200_CHECK_ARG(rows > 0 && H > 0 && H % 8 == 0 && H <= RN_THREADS * 8 * RN_MAX_VEC,
-                 "rmsnorm_bwd: unsupported shape rows=%d H=%d", rows, H);
-  B200_CHECK_ARG(al16(dy) && al16(x) && al16(w) && al16(dx) && al16(dres), "rmsnorm_bwd: alignment");
-  if (ws == nullptr || ws_bytes < rmsnorm_bwd_workspace_bytes(rows, H)) {
-    set_error("rmsnorm_bwd: workspace too small (%zu < %zu)", ws_bytes, rmsnorm_bwd_workspace_bytes(rows, H));
-    return B200_ERR_WORKSPACE;
-  }
-  float* part = reinterpret_cast<float*>(ws);
-  if (is_bf16)
-    return rmsnorm_bwd_t<__nv_bfloat16>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)dres,
-                                        (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, rstd,
-                                        (__nv_bfloat16*)dx, dw, part, rows, H, stream);
-  return rmsnorm_bwd_t<float>((const float*)dy, (const float*)dres, (const float*)x, (const float*)w, rstd,
-                              (float*)dx, dw, part, rows, H, stream);
-}
-
-int rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, void* dx,
-                float* dw, int rows, int H, int is_bf16, void* ws, size_t ws_bytes,
-                cudaStream_t stream) {
-  return add_rmsnorm_bwd(dy, nullptr, x, w, rstd, dx, dw, rows, H, is_bf16, ws, ws_bytes, stream);
-}
-
-namespace {
-
 int rope_impl(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
               int D, int backward, int is_bf16, cudaStream_t stream) {
   B200_CHECK_ARG(B > 0 && S > 0 && NH > 0 && D > 0 && D % 8 == 0, "rope: D=%d must be a multiple of 8",
@@ -668,10 +594,86 @@ int rope_impl(const void* x, void* y, const float* cos_t, const float* sin_t, co
 }
 
 }  // namespace
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
+
+int b200_add_rmsnorm_fwd(const void* x, const void* delta, const void* w, void* sum_out, void* y, float* rstd,
+                         int rows, int H, float eps, int is_bf16, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  B200_CHECK_ARG(rows > 0 && H > 0 && H % 8 == 0 && H <= RN_THREADS * 8 * RN_MAX_VEC,
+                 "rmsnorm_fwd: unsupported shape rows=%d H=%d (H %% 8 == 0, H <= %d)", rows, H,
+                 RN_THREADS * 8 * RN_MAX_VEC);
+  B200_CHECK_ARG(al16(x) && al16(w) && al16(y) && al16(delta) && al16(sum_out),
+                 "rmsnorm_fwd: 16-byte alignment required");
+  B200_CHECK_ARG((delta == nullptr) == (sum_out == nullptr),
+                 "add_rmsnorm_fwd: delta and sum_out must be given together");
+  if (is_bf16)
+    return rmsnorm_fwd_t<__nv_bfloat16>((const __nv_bfloat16*)x, (const __nv_bfloat16*)delta,
+                                        (const __nv_bfloat16*)w, (__nv_bfloat16*)sum_out, (__nv_bfloat16*)y,
+                                        rstd, rows, H, eps, s);
+  return rmsnorm_fwd_t<float>((const float*)x, (const float*)delta, (const float*)w, (float*)sum_out,
+                              (float*)y, rstd, rows, H, eps, s);
+}
+
+int b200_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int rows, int H, float eps,
+                     int is_bf16, void* stream) {
+  return b200_add_rmsnorm_fwd(x, nullptr, w, nullptr, y, rstd, rows, H, eps, is_bf16, stream);
+}
+
+size_t b200_rmsnorm_bwd_workspace_bytes(int rows, int H) {
+  return (size_t)rmsnorm_bwd_grid(rows, H) * H * sizeof(float);
+}
+
+int b200_rmsnorm_bwd_partial_rows(int rows, int H) { return rmsnorm_bwd_grid(rows, H); }
+
+int b200_rmsnorm_dw_reduce(const b200_dw_job* jobs, int n_jobs, int H, void* stream) {
+  B200_CHECK_ARG(n_jobs >= 0 && H > 0 && (jobs != nullptr || n_jobs == 0), "rmsnorm_dw_reduce: bad arguments");
+  for (int i = 0; i < n_jobs; ++i)
+    B200_CHECK_ARG(jobs[i].partials != nullptr && jobs[i].dw != nullptr && jobs[i].n_partials > 0,
+                   "rmsnorm_dw_reduce: job %d has a null pointer or no partial rows", i);
+  for (int i = 0; i < n_jobs; i += 32) {
+    DwJobs a;
+    const int n = n_jobs - i < 32 ? n_jobs - i : 32;
+    for (int k = 0; k < n; ++k) a.j[k] = jobs[i + k];
+    rmsnorm_dw_reduce_batched_kernel<<<dim3((H + 31) / 32, n), 1024, 0, static_cast<cudaStream_t>(stream)>>>(a, H);
+    B200_CHECK_LAUNCH();
+  }
+  return B200_OK;
+}
+
+int b200_add_rmsnorm_bwd(const void* dy, const void* dres, const void* x, const void* w, const float* rstd,
+                         void* dx, float* dw, int rows, int H, int is_bf16, void* ws, size_t ws_bytes,
+                         void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  B200_CHECK_ARG(rows > 0 && H > 0 && H % 8 == 0 && H <= RN_THREADS * 8 * RN_MAX_VEC,
+                 "rmsnorm_bwd: unsupported shape rows=%d H=%d", rows, H);
+  B200_CHECK_ARG(al16(dy) && al16(x) && al16(w) && al16(dx) && al16(dres), "rmsnorm_bwd: alignment");
+  if (ws == nullptr || ws_bytes < b200_rmsnorm_bwd_workspace_bytes(rows, H)) {
+    set_error("rmsnorm_bwd: workspace too small (%zu < %zu)", ws_bytes, b200_rmsnorm_bwd_workspace_bytes(rows, H));
+    return B200_ERR_WORKSPACE;
+  }
+  float* part = reinterpret_cast<float*>(ws);
+  if (is_bf16)
+    return rmsnorm_bwd_t<__nv_bfloat16>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)dres,
+                                        (const __nv_bfloat16*)x, (const __nv_bfloat16*)w, rstd,
+                                        (__nv_bfloat16*)dx, dw, part, rows, H, s);
+  return rmsnorm_bwd_t<float>((const float*)dy, (const float*)dres, (const float*)x, (const float*)w, rstd,
+                              (float*)dx, dw, part, rows, H, s);
+}
+
+int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, void* dx,
+                     float* dw, int rows, int H, int is_bf16, void* ws, size_t ws_bytes,
+                     void* stream) {
+  return b200_add_rmsnorm_bwd(dy, nullptr, x, w, rstd, dx, dw, rows, H, is_bf16, ws, ws_bytes, stream);
+}
+
 
 // pos: nullable int32 [B, S]; D % 16 == 0 (both halves of a slice are 16-byte vectors)
-int rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
-              int D, int backward, int is_bf16, cudaStream_t stream) {
+int b200_rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
+                   int D, int backward, int is_bf16, void* stream) {
   B200_CHECK_ARG(B > 0 && S > 0 && NH > 0 && D > 0 && D % 16 == 0, "rope_half: D=%d must be a multiple of 16", D);
   B200_CHECK_ARG(al16(x) && al16(y) && al16(cos_t) && al16(sin_t) && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
                  "rope_half: alignment");
@@ -680,7 +682,7 @@ int rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, co
   if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
   const float sign = backward ? -1.0f : 1.0f;
   auto launch = [&](auto kern, auto* xx, auto* yy) {
-    kern<<<(int)blocks, 256, 0, stream>>>(xx, yy, cos_t, sin_t, nslice, S, NH, D, sign, pos);
+    kern<<<(int)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(xx, yy, cos_t, sin_t, nslice, S, NH, D, sign, pos);
   };
   using bf = __nv_bfloat16;
   if (is_bf16) {
@@ -694,17 +696,17 @@ int rope_half(const void* x, void* y, const float* cos_t, const float* sin_t, co
   return B200_OK;
 }
 
-int rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, int S, int NH,
-         int D, int backward, int is_bf16, cudaStream_t stream) {
-  return rope_impl(x, y, cos_t, sin_t, nullptr, B, S, NH, D, backward, is_bf16, stream);
+int b200_rope(const void* x, void* y, const float* cos_t, const float* sin_t, int B, int S, int NH,
+              int D, int backward, int is_bf16, void* stream) {
+  return rope_impl(x, y, cos_t, sin_t, nullptr, B, S, NH, D, backward, is_bf16, static_cast<cudaStream_t>(stream));
 }
 
 // pos: int32 [B, S]; the tables must cover max(pos) + 1 rows
-int rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
-             int D, int backward, int is_bf16, cudaStream_t stream) {
+int b200_rope_pos(const void* x, void* y, const float* cos_t, const float* sin_t, const int* pos, int B, int S, int NH,
+                  int D, int backward, int is_bf16, void* stream) {
   B200_CHECK_ARG(pos != nullptr && (reinterpret_cast<uintptr_t>(pos) & 3u) == 0,
                  "rope_pos: pos must be a non-null, 4-byte aligned int32 [B, S] array");
-  return rope_impl(x, y, cos_t, sin_t, pos, B, S, NH, D, backward, is_bf16, stream);
+  return rope_impl(x, y, cos_t, sin_t, pos, B, S, NH, D, backward, is_bf16, static_cast<cudaStream_t>(stream));
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -24,23 +24,9 @@
 #include "host.h"
 
 namespace b200 {
-
-int gemm_bf16(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* A, long long lda,
-              long long strideA, const void* B, long long ldb, long long strideB, const void* C,
-              long long ldc, long long strideC, void* D, long long ldd, long long strideD,
-              bool out_f32, float alpha, float beta, const float* alpha_vec, const float* beta_vec,
-              int force_bn, cudaStream_t stream);
-size_t reduce_workspace_bytes(int batch);
-int graft_update(float* p32, void* p16, const float* pre, const float* d, long long numel, int batch,
-                 const float* coef, const float* coef_d, float decay, cudaStream_t stream);
-int sumsq(const void* x, int x_is_bf16, float* out, long long numel, int batch, int zero_first, void* ws,
-          size_t ws_bytes, cudaStream_t stream);
-
 namespace {
 
 constexpr int SH_THREADS = 256;
-inline int rup8(int k) { return (k + 7) & ~7; }
-inline size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
 
 // one block per matrix: tr = sum_i M[i,i] + k*eps (trace of M + eps I, shampoo.py:103,110) in a fixed order,
 // inv_tr = 1/tr, fin = tr^(-1/p^2) (= (tr^(1/p))^(-1/p), shampoo.py:113,124)
@@ -455,34 +441,41 @@ int gemm3(bool a_mn, bool b_mn, int M, int N, int K, int batch, const void* Ah, 
 }
 
 }  // namespace
+}  // namespace b200
+
+using namespace b200;
+
+extern "C" {
 
 // ---- statistics ---------------------------------------------------------------------------------
-int shampoo_stats(const void* g_hi, const void* g_lo, long long ldg, long long strideG, float* L, float* R,
-                  int batch, int k1, int k2, float beta2, float weight, cudaStream_t stream) {
+int b200_shampoo_stats(const void* g_hi, const void* g_lo, long long ldg, long long strideG, float* L, float* R,
+                       int batch, int k1, int k2, float beta2, float weight, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(batch > 0 && k1 > 0 && k2 > 0, "shampoo_stats: empty (batch=%d k1=%d k2=%d)", batch, k1, k2);
   B200_CHECK_ARG(ldg % 8 == 0 && ldg >= k2, "shampoo_stats: ldg=%lld must be a multiple of 8 and >= k2", ldg);
   const int k1p = rup8(k1), k2p = rup8(k2);
   // L (+)= G G^T : K-major x K-major over the k2 columns;  R (+)= G^T G : both operands MN-major (G as stored)
   int rc = gemm3(false, false, k1, k1, k2, batch, g_hi, g_lo, ldg, strideG, g_hi, g_lo, ldg, strideG, L, k1p,
-                 (long long)k1p * k1p, L, k1p, (long long)k1p * k1p, weight, beta2, nullptr, nullptr, stream);
+                 (long long)k1p * k1p, L, k1p, (long long)k1p * k1p, weight, beta2, nullptr, nullptr, s);
   if (rc) return rc;
   return gemm3(true, true, k2, k2, k1, batch, g_hi, g_lo, ldg, strideG, g_hi, g_lo, ldg, strideG, R, k2p,
-               (long long)k2p * k2p, R, k2p, (long long)k2p * k2p, weight, beta2, nullptr, nullptr, stream);
+               (long long)k2p * k2p, R, k2p, (long long)k2p * k2p, weight, beta2, nullptr, nullptr, s);
 }
 
 // ---- matrix_inverse_pth_root ----------------------------------------------------------------------
-size_t shampoo_root_workspace_bytes(int batch, int k) {
+size_t b200_shampoo_root_workspace_bytes(int batch, int k) {
   const size_t kk = (size_t)rup8(k) * rup8(k) * (size_t)(batch > 0 ? batch : 1);
   return al256(kk * 4) + 2 * al256(kk * 2) + al256((size_t)(batch > 0 ? batch : 1) * 8);
 }
 
-int shampoo_root(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float p, float eps, int iters,
-                 void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_shampoo_root(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float p, float eps, int iters,
+                      void* ws, size_t ws_bytes, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(batch > 0 && k > 0 && iters > 0 && p > 0.f, "shampoo_root: bad arguments (batch=%d k=%d iters=%d p=%g)",
                  batch, k, iters, (double)p);
   B200_CHECK_ARG(M != P, "shampoo_root: M and P must be distinct buffers");
-  if (ws == nullptr || ws_bytes < shampoo_root_workspace_bytes(batch, k)) {
-    set_error("shampoo_root: workspace too small (%zu < %zu)", ws_bytes, shampoo_root_workspace_bytes(batch, k));
+  if (ws == nullptr || ws_bytes < b200_shampoo_root_workspace_bytes(batch, k)) {
+    set_error("shampoo_root: workspace too small (%zu < %zu)", ws_bytes, b200_shampoo_root_workspace_bytes(batch, k));
     return B200_ERR_WORKSPACE;
   }
   const int kp = rup8(k);
@@ -497,9 +490,9 @@ int shampoo_root(const float* M, float* P, void* P_hi, void* P_lo, int batch, in
   // ping-pong between P and the workspace so that the LAST iterate lands in P
   float* cur = (iters % 2 == 0) ? P : Zb;
   float* nxt = (iters % 2 == 0) ? Zb : P;
-  root_scalars_kernel<<<batch, SH_THREADS, 0, stream>>>(M, k, kp, eps, p, inv_tr, fin);
+  root_scalars_kernel<<<batch, SH_THREADS, 0, s>>>(M, k, kp, eps, p, inv_tr, fin);
   B200_CHECK_LAUNCH();
-  root_init_kernel<<<sh_grid((long long)n / 4), SH_THREADS, 0, stream>>>(
+  root_init_kernel<<<sh_grid((long long)n / 4), SH_THREADS, 0, s>>>(
       M, cur, (__nv_bfloat16*)Zh, (__nv_bfloat16*)Zl, k, kp, eps, inv_tr, (long long)n / 4);
   B200_CHECK_LAUNCH();
   for (int it = 0; it < iters; ++it) {
@@ -507,40 +500,41 @@ int shampoo_root(const float* M, float* P, void* P_hi, void* P_lo, int batch, in
     // Z' = Z + (1/p) Z Z   (Z @ (I - alpha Z), alpha = -1/p); the final tr^(-1/p^2) rides on the last epilogue
     const float* sv = last ? fin : nullptr;
     int rc = gemm3(false, false, kp, kp, kp, batch, Zh, Zl, kp, kk, Zh, Zl, kp, kk, cur, kp, kk, nxt, kp, kk, 1.0f / p,
-                   1.0f, sv, sv, stream);
+                   1.0f, sv, sv, s);
     if (rc) return rc;
     float* t = cur;
     cur = nxt;
     nxt = t;
     if (!last) {
-      rc = split4(cur, Zh, Zl, (long long)n, stream);
+      rc = split4(cur, Zh, Zl, (long long)n, s);
       if (rc) return rc;
     }
   }
   // cur == P here
-  if (P_hi != nullptr) return split4(P, P_hi, P_lo, (long long)n, stream);
+  if (P_hi != nullptr) return split4(P, P_hi, P_lo, (long long)n, s);
   return B200_OK;
 }
 
 // ---- true inverse 4th root by the coupled Newton iteration ------------------------------------------------
 // Workspace: F (fp32 product), the 3-way splits of T, S (T^2, T^4, then the next T), Mc and X, and per-matrix
 // scalars.
-size_t shampoo_root_newton_workspace_bytes(int batch, int k) {
+size_t b200_shampoo_root_newton_workspace_bytes(int batch, int k) {
   const size_t b = (size_t)(batch > 0 ? batch : 1);
   const size_t kk = (size_t)rup8(k > 0 ? k : 1) * rup8(k > 0 ? k : 1) * b;
   return al256(kk * 4) + 12 * al256(kk * 2) + 7 * al256(b * 4);
 }
 
-int shampoo_root_newton(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float eps, int max_iters,
-                        float tol, int* iters_out, float* residual_out, void* ws, size_t ws_bytes,
-                        cudaStream_t stream) {
+int b200_shampoo_root_newton(const float* M, float* P, void* P_hi, void* P_lo, int batch, int k, float eps,
+                             int max_iters, float tol, int* iters_out, float* residual_out, void* ws, size_t ws_bytes,
+                             void* stream) {
+  const cudaStream_t strm = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(batch > 0 && k > 0 && max_iters > 0 && eps > 0.f && tol >= 0.f,
                  "shampoo_root_newton: bad arguments (batch=%d k=%d max_iters=%d eps=%g tol=%g)", batch, k, max_iters,
                  (double)eps, (double)tol);
   B200_CHECK_ARG(M != P, "shampoo_root_newton: M and P must be distinct buffers");
-  if (ws == nullptr || ws_bytes < shampoo_root_newton_workspace_bytes(batch, k)) {
+  if (ws == nullptr || ws_bytes < b200_shampoo_root_newton_workspace_bytes(batch, k)) {
     set_error("shampoo_root_newton: workspace too small (%zu < %zu)", ws_bytes,
-              shampoo_root_newton_workspace_bytes(batch, k));
+              b200_shampoo_root_newton_workspace_bytes(batch, k));
     return B200_ERR_WORKSPACE;
   }
   const int kp = rup8(k);
@@ -575,64 +569,66 @@ int shampoo_root_newton(const float* M, float* P, void* P_hi, void* P_lo, int ba
   if (vec_smem > 48 * 1024)
     B200_CHECK_CUDA(
         cudaFuncSetAttribute(newton_scalars_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)vec_smem));
-  newton_scalars_kernel<<<batch, NR_THREADS, vec_smem, stream>>>(M, k, kp, eps, ridge, z);
+  newton_scalars_kernel<<<batch, NR_THREADS, vec_smem, strm>>>(M, k, kp, eps, ridge, z);
   B200_CHECK_LAUNCH();
-  newton_init_kernel<<<batch, NR_THREADS, 0, stream>>>(M, k, kp, ridge, z, tol, Mc, T, P, Xs, st);
+  newton_init_kernel<<<batch, NR_THREADS, 0, strm>>>(M, k, kp, ridge, z, tol, Mc, T, P, Xs, st);
   B200_CHECK_LAUNCH();
   const long long n4 = (long long)n / 4;
   std::vector<int> frozen_host(batch);
   for (int it = 0; it < max_iters; ++it) {
     // Mc' = T^4 Mc, with T^2 and T^4 staged through F and S
-    int rc = gemm6(kp, batch, T, T, nullptr, 0.f, F, nullptr, nullptr, stream);
+    int rc = gemm6(kp, batch, T, T, nullptr, 0.f, F, nullptr, nullptr, strm);
     if (rc) return rc;
-    split3_kernel<<<sh_grid(n4), SH_THREADS, 0, stream>>>(F, S.h, S.m, S.l, n4);
+    split3_kernel<<<sh_grid(n4), SH_THREADS, 0, strm>>>(F, S.h, S.m, S.l, n4);
     B200_CHECK_LAUNCH();
-    if ((rc = gemm6(kp, batch, S, S, nullptr, 0.f, F, nullptr, nullptr, stream))) return rc;
-    split3_kernel<<<sh_grid(n4), SH_THREADS, 0, stream>>>(F, S.h, S.m, S.l, n4);
+    if ((rc = gemm6(kp, batch, S, S, nullptr, 0.f, F, nullptr, nullptr, strm))) return rc;
+    split3_kernel<<<sh_grid(n4), SH_THREADS, 0, strm>>>(F, S.h, S.m, S.l, n4);
     B200_CHECK_LAUNCH();
-    if ((rc = gemm6(kp, batch, S, Mc, nullptr, 0.f, F, nullptr, nullptr, stream))) return rc;
+    if ((rc = gemm6(kp, batch, S, Mc, nullptr, 0.f, F, nullptr, nullptr, strm))) return rc;
     // accept / freeze; the next T goes to S because X = X T below still reads this iteration's T
-    newton_step_kernel<<<batch, NR_THREADS, 0, stream>>>(F, k, kp, tol, Mc, S, st);
+    newton_step_kernel<<<batch, NR_THREADS, 0, strm>>>(F, k, kp, tol, Mc, S, st);
     B200_CHECK_LAUNCH();
     // X = av X T + bv X in place: a frozen or rejected matrix keeps its X bit for bit
-    if ((rc = gemm6(kp, batch, Xs, T, P, 1.0f, P, st.av, st.bv, stream))) return rc;
-    split3_kernel<<<sh_grid(n4), SH_THREADS, 0, stream>>>(P, Xs.h, Xs.m, Xs.l, n4);
+    if ((rc = gemm6(kp, batch, Xs, T, P, 1.0f, P, st.av, st.bv, strm))) return rc;
+    split3_kernel<<<sh_grid(n4), SH_THREADS, 0, strm>>>(P, Xs.h, Xs.m, Xs.l, n4);
     B200_CHECK_LAUNCH();
     std::swap(T, S);
     // every 4 iterations the host stops the loop once every matrix is frozen (frozen matrices no longer change,
     // so the result does not depend on where the loop ends)
     if ((it & 3) == 3 && it + 1 < max_iters) {
       B200_CHECK_CUDA(cudaMemcpyAsync(frozen_host.data(), st.frozen, sizeof(int) * batch, cudaMemcpyDeviceToHost,
-                                      stream));
-      B200_CHECK_CUDA(cudaStreamSynchronize(stream));
+                                      strm));
+      B200_CHECK_CUDA(cudaStreamSynchronize(strm));
       bool all = true;
       for (int f : frozen_host) all = all && f != 0;
       if (all) break;
     }
   }
   if (iters_out)
-    B200_CHECK_CUDA(cudaMemcpyAsync(iters_out, st.iters, sizeof(int) * batch, cudaMemcpyDeviceToDevice, stream));
+    B200_CHECK_CUDA(cudaMemcpyAsync(iters_out, st.iters, sizeof(int) * batch, cudaMemcpyDeviceToDevice, strm));
   if (residual_out)
     B200_CHECK_CUDA(
-        cudaMemcpyAsync(residual_out, st.err, sizeof(float) * batch, cudaMemcpyDeviceToDevice, stream));
-  if (P_hi != nullptr) return split4(P, P_hi, P_lo, (long long)n, stream);
+        cudaMemcpyAsync(residual_out, st.err, sizeof(float) * batch, cudaMemcpyDeviceToDevice, strm));
+  if (P_hi != nullptr) return split4(P, P_hi, P_lo, (long long)n, strm);
   return B200_OK;
 }
 
 // ---- PL m PR ------------------------------------------------------------------------------------------
-size_t shampoo_precond_workspace_bytes(int batch, int k1, int k2) {
+size_t b200_shampoo_precond_workspace_bytes(int batch, int k1, int k2) {
   const size_t n = (size_t)(batch > 0 ? batch : 1) * k1 * rup8(k2);
   return al256(n * 4) + 2 * al256(n * 2);
 }
 
-int shampoo_precond(const void* PL_hi, const void* PL_lo, const void* PR_hi, const void* PR_lo, const void* m_hi,
-                    const void* m_lo, long long ldm, long long strideM, float* out, long long ldo, long long strideO,
-                    int batch, int k1, int k2, float alpha, void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_shampoo_precond(const void* PL_hi, const void* PL_lo, const void* PR_hi, const void* PR_lo, const void* m_hi,
+                         const void* m_lo, long long ldm, long long strideM, float* out, long long ldo,
+                         long long strideO, int batch, int k1, int k2, float alpha, void* ws, size_t ws_bytes,
+                         void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(batch > 0 && k1 > 0 && k2 > 0, "shampoo_precond: empty");
   B200_CHECK_ARG(k2 % 8 == 0, "shampoo_precond: k2=%d must be a multiple of 8 (rows k1 may be arbitrary)", k2);
-  if (ws == nullptr || ws_bytes < shampoo_precond_workspace_bytes(batch, k1, k2)) {
+  if (ws == nullptr || ws_bytes < b200_shampoo_precond_workspace_bytes(batch, k1, k2)) {
     set_error("shampoo_precond: workspace too small (%zu < %zu)", ws_bytes,
-              shampoo_precond_workspace_bytes(batch, k1, k2));
+              b200_shampoo_precond_workspace_bytes(batch, k1, k2));
     return B200_ERR_WORKSPACE;
   }
   const int k1p = rup8(k1), k2p = rup8(k2);
@@ -643,40 +639,41 @@ int shampoo_precond(const void* PL_hi, const void* PL_lo, const void* PR_hi, con
   void* Tl = w + al256(n * 4) + al256(n * 2);
   // T = PL @ m[:k1,:k2]: the momentum block is read in place as an MN-major B operand ([K = k1 rows][N = k2])
   int rc = gemm3(false, true, k1, k2, k1, batch, PL_hi, PL_lo, k1p, (long long)k1p * k1p, m_hi, m_lo, ldm, strideM,
-                 nullptr, k2p, (long long)k1 * k2p, T, k2p, (long long)k1 * k2p, 1.0f, 0.0f, nullptr, nullptr, stream);
+                 nullptr, k2p, (long long)k1 * k2p, T, k2p, (long long)k1 * k2p, 1.0f, 0.0f, nullptr, nullptr, s);
   if (rc) return rc;
-  rc = split4(T, Th, Tl, (long long)n, stream);
+  rc = split4(T, Th, Tl, (long long)n, s);
   if (rc) return rc;
   // out[:k1,:k2] = alpha * T @ PR, written straight into the update buffer (ldo = cols of the parameter)
   return gemm3(false, true, k1, k2, k2, batch, Th, Tl, k2p, (long long)k1 * k2p, PR_hi, PR_lo, k2p,
-               (long long)k2p * k2p, nullptr, ldo, strideO, out, ldo, strideO, alpha, 0.0f, nullptr, nullptr, stream);
+               (long long)k2p * k2p, nullptr, ldo, strideO, out, ldo, strideO, alpha, 0.0f, nullptr, nullptr, s);
 }
 
 // ---- grafting + apply ---------------------------------------------------------------------------------
-size_t shampoo_graft_workspace_bytes(int batch) {
-  return reduce_workspace_bytes(batch) + al256((size_t)(batch > 0 ? batch : 1) * 16);
+size_t b200_shampoo_graft_workspace_bytes(int batch) {
+  return b200_reduce_workspace_bytes(batch) + al256((size_t)(batch > 0 ? batch : 1) * 16);
 }
 
-int shampoo_graft(float* p32, void* p16, const float* upd, const float* graft, long long numel, int batch,
-                  float decay, void* ws, size_t ws_bytes, cudaStream_t stream) {
+int b200_shampoo_graft(float* p32, void* p16, const float* upd, const float* graft, long long numel, int batch,
+                       float decay, void* ws, size_t ws_bytes, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
   B200_CHECK_ARG(numel > 0 && batch > 0, "shampoo_graft: empty");
-  if (ws == nullptr || ws_bytes < shampoo_graft_workspace_bytes(batch)) {
-    set_error("shampoo_graft: workspace too small (%zu < %zu)", ws_bytes, shampoo_graft_workspace_bytes(batch));
+  if (ws == nullptr || ws_bytes < b200_shampoo_graft_workspace_bytes(batch)) {
+    set_error("shampoo_graft: workspace too small (%zu < %zu)", ws_bytes, b200_shampoo_graft_workspace_bytes(batch));
     return B200_ERR_WORKSPACE;
   }
   char* w = reinterpret_cast<char*>(ws);
-  const size_t rws = reduce_workspace_bytes(batch);
+  const size_t rws = b200_reduce_workspace_bytes(batch);
   float* n1 = reinterpret_cast<float*>(w + rws);
   float* n2 = n1 + batch;
   float* coef = n2 + batch;
   float* coef_d = coef + batch;
-  int rc = sumsq(upd, 0, n1, numel, batch, 1, w, rws, stream);
+  int rc = b200_sumsq(upd, 0, n1, numel, batch, 1, w, rws, s);
   if (rc) return rc;
-  rc = sumsq(graft, 0, n2, numel, batch, 1, w, rws, stream);
+  rc = b200_sumsq(graft, 0, n2, numel, batch, 1, w, rws, s);
   if (rc) return rc;
-  graft_coef_kernel<<<(batch + 127) / 128, 128, 0, stream>>>(n1, n2, coef, coef_d, batch);
+  graft_coef_kernel<<<(batch + 127) / 128, 128, 0, s>>>(n1, n2, coef, coef_d, batch);
   B200_CHECK_LAUNCH();
-  return graft_update(p32, p16, upd, graft, numel, batch, coef, coef_d, decay, stream);
+  return b200_graft_update(p32, p16, upd, graft, numel, batch, coef, coef_d, decay, s);
 }
 
-}  // namespace b200
+}  // extern "C"

@@ -21,6 +21,39 @@ def test_capi_exports_every_declared_symbol(lib_built):
     assert not missing, f"declared in include/b200_hotpath.h but not exported: {missing}"
     from mlx_cuda_distributed_pretraining_b200._lib import SIGNATURES
     assert set(SIGNATURES) == declared, set(SIGNATURES) ^ declared
+    # the ctypes rows must agree with the header prototypes kind by kind (the compiler checks the header against the
+    # definitions, nothing else checks _lib.py): pointer, int, long long, size_t / unsigned long long (one ctypes type
+    # on LP64), float, void
+    def c_kind(decl):
+        decl = decl.strip()
+        if "*" in decl:
+            return "pointer"
+        words = [w for w in decl.split()[:-1] if w != "const"]  # drop the name
+        return {"void": "void", "int": "int", "long long": "long long", "size_t": "u64",
+                "unsigned long long": "u64", "float": "float"}[" ".join(words)]
+
+    def ctypes_kind(t):
+        if t is None:
+            return "void"
+        if t in (ctypes.c_void_p, ctypes.c_char_p) or issubclass(t, ctypes._Pointer):
+            return "pointer"
+        for ct, kind in ((ctypes.c_int, "int"), (ctypes.c_longlong, "long long"), (ctypes.c_size_t, "u64"),
+                         (ctypes.c_ulonglong, "u64"), (ctypes.c_float, "float")):
+            if t is ct:
+                return kind
+        raise AssertionError(f"unexpected ctypes type {t}")
+
+    code = re.sub(r"/\*.*?\*/", " ", header, flags=re.S)
+    protos = re.findall(r"([A-Za-z_][\w \t*]*?)\b(b200_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", code)
+    assert {name for _, name, _ in protos} == declared
+    mismatched = []
+    for ret, name, params in protos:
+        params = [] if params.strip() in ("", "void") else params.split(",")
+        want = (c_kind(ret.strip() + " r"), [c_kind(p) for p in params])
+        res, args = SIGNATURES[name]
+        if want != (ctypes_kind(res), [ctypes_kind(a) for a in args]):
+            mismatched.append(name)
+    assert not mismatched, f"_lib.SIGNATURES disagrees with include/b200_hotpath.h: {mismatched}"
     handle.b200_version.restype = ctypes.c_int
     assert handle.b200_version() >= 1
     handle.b200_newton_schulz_workspace_bytes.restype = ctypes.c_size_t
