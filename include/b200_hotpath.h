@@ -470,6 +470,32 @@ int b200_kv_append_half(void* q, const void* k, const void* v, void* k_cache, vo
                         const float* cos_t, const float* sin_t, int B, int s_max, int H, int Hk, int D, int is_bf16,
                         void* stream);
 
+/* ---- quantized KV cache (the reference's kv_bits / kv_group_size, core/generation_lite.py:75-90) --------------
+ * Each group of g = group_size consecutive elements of a head vector is stored as x ~ s q + b: n = 2^bits - 1,
+ * s = max((max - min) / n, 1e-7), b = min (-0 stored as +0), q = min(n, rint((x - b) / s)), IEEE fp32 throughout.
+ * Codes uint8 [B, s_max, Hk, D * bits / 8] (4 bits: element 2j in the low nibble of byte j, 2j + 1 in the high one);
+ * parameters f32 [B, Hk, s_max, D / g, 2] holding (s, b).  bits in {4, 8}, g in {32, 64, 128}, D in {32, 64, 128},
+ * g divides D, s_max even; every pointer 16-byte aligned.
+ *
+ * b200_kv_quantize: positions [0, n) of the bf16 / f32 (is_bf16) sources k, v [B, S, Hk, D] into the codes and
+ *   parameters; nothing else is written. */
+int b200_kv_quantize(const void* k, const void* v, int n, int S, void* k_codes, void* v_codes, float* k_params,
+                     float* v_params, int B, int s_max, int Hk, int D, int bits, int group_size, int is_bf16,
+                     void* stream);
+/* b200_kv_append (half == 0) or b200_kv_append_half (half != 0, tables required) into a quantized cache: q is
+ *   rotated in place exactly as there, and k (rotated) and v, rounded to the activation dtype, are quantized into
+ *   position lens[b] - 1.  Nothing else is written. */
+int b200_kv_append_quant(void* q, const void* k, const void* v, void* k_codes, void* v_codes, float* k_params,
+                         float* v_params, const int* lens, const float* cos_t, const float* sin_t, int half, int B,
+                         int s_max, int H, int Hk, int D, int bits, int group_size, int is_bf16, void* stream);
+/* b200_attn_decode_alibi over a quantized cache: window < 0 is no window, slopes NULL is no ALiBi.  q and o bf16 or
+ *   f32 [B, H, D]; same chunking, workspace (b200_attn_decode_workspace_bytes) and merge order, so a row's output is
+ *   bit-identical alone or in any batch. */
+int b200_attn_decode_quant(const void* q, const void* k_codes, const void* v_codes, const float* k_params,
+                           const float* v_params, const int* lens, void* o, float* lse, int window,
+                           const float* slopes, int B, int s_max, int H, int Hk, int D, int bits, int group_size,
+                           float scale, int is_bf16, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- mixture-of-experts MLP (Mixtral's sparse MoE block, model.misc.num_local_experts) -------------------------
  * T tokens, E experts (2..64), k experts per token (1..min(E, 8)), hidden H, per-expert intermediate I (H, I % 8 == 0).
  * Everything stays on the device and nothing uses atomics: the same inputs give the same bits on every run.

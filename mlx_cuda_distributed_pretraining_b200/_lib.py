@@ -104,6 +104,11 @@ SIGNATURES = {
     "b200_silu_glu_fwd": (_i, [_vp, _vp, _vp, _ll, _vp]),
     "b200_silu_glu_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _ll, _vp]),
     "b200_kv_append_half": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_kv_quantize": (_i, [_vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_kv_append_quant": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i,
+                                  _i, _vp]),
+    "b200_attn_decode_quant": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _f,
+                                    _i, _vp, _sz, _vp]),
     "b200_moe_route_workspace_bytes": (_sz, [_i, _i, _i]),
     "b200_moe_max_tiles": (_i, [_i, _i, _i]),
     "b200_moe_route": (_i, [_vp, _vp, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),

@@ -104,6 +104,27 @@ class PrefixCausalMask:
         return m[:, None]
 
 
+class QuantizedKV:
+    """One layer's quantized KV cache (the reference's QuantizedKVCache; DESIGN §4.2.1): for K and for V, codes uint8
+    [B, s_max, Hk, D * bits / 8] and fp32 (scale, bias) parameters [B, Hk, s_max, D / group_size, 2]."""
+
+    def __init__(self, batch: int, s_max: int, num_kv_heads: int, head_dim: int, bits: int, group_size: int,
+                 device):
+        self.bits, self.group_size = bits, group_size
+        cshape, pshape = ops.kv_quant_shapes(batch, s_max, num_kv_heads, head_dim, bits, group_size)
+        self.k_codes = torch.zeros(cshape, device=device, dtype=torch.uint8)
+        self.v_codes = torch.zeros(cshape, device=device, dtype=torch.uint8)
+        self.k_params = torch.zeros(pshape, device=device, dtype=torch.float32)
+        self.v_params = torch.zeros(pshape, device=device, dtype=torch.float32)
+
+    def buffers(self):
+        """(k_codes, v_codes, k_params, v_params), the argument order of the ops.*_quant wrappers."""
+        return self.k_codes, self.v_codes, self.k_params, self.v_params
+
+    def nbytes(self) -> int:
+        return sum(t.numel() * t.element_size() for t in self.buffers())
+
+
 class FlashAttention(nn.Module):
     """alibi: add ALiBi's bias alibi_slopes(num_heads)[h] * (k - q) to every causal score (the slopes are not
     parameters: a device tensor made on first use, like rope_tables).  dropout: the probability p of dropping an
@@ -211,11 +232,12 @@ class FlashAttention(nn.Module):
     def _out(self, ctx: torch.Tensor) -> torch.Tensor:
         return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
 
-    def forward_prefill(self, x: torch.Tensor, mask, k_cache: torch.Tensor, v_cache: torch.Tensor,
+    def forward_prefill(self, x: torch.Tensor, mask, k_cache, v_cache: Optional[torch.Tensor],
                         rope_layout: str = "interleaved") -> torch.Tensor:
         """forward(x, mask) over a right-padded prompt batch x [B, S, hidden] that also stores the (rotated) keys and
-        values in cache positions [0, S).  Attention runs through _flash_attention, so the numerics are the
-        training forward's."""
+        values in cache positions [0, S): in the k_cache and v_cache tensors, or quantized into k_cache when it is a
+        QuantizedKV (v_cache None).  Attention runs through _flash_attention on the unquantized k and v, so the
+        numerics are the training forward's."""
         B, S, _ = x.shape
         q, k, v = self._project(x)
         q = q.reshape(B, S, self.num_heads, self.head_dim)
@@ -225,22 +247,32 @@ class FlashAttention(nn.Module):
             cos_t, sin_t = self.rope_tables
             q = ops.rope(q, cos_t[:S], sin_t[:S], layout=rope_layout)
             k = ops.rope(k, cos_t[:S], sin_t[:S], layout=rope_layout)
-        k_cache[:, :S].copy_(k)
-        v_cache[:, :S].copy_(v)
+        if isinstance(k_cache, QuantizedKV):
+            ops.kv_quantize(k.contiguous(), v.contiguous(), *k_cache.buffers(), k_cache.bits, k_cache.group_size)
+        else:
+            k_cache[:, :S].copy_(k)
+            v_cache[:, :S].copy_(v)
         ctx = self._flash_attention(q, k, v, mask)
         return self._out(ctx.reshape(B, S, self.num_heads * self.head_dim))
 
-    def forward_decode(self, x: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
+    def forward_decode(self, x: torch.Tensor, k_cache, v_cache: Optional[torch.Tensor], lens: torch.Tensor,
                        workspace: torch.Tensor, window: Optional[int] = None,
                        rope_layout: str = "interleaved") -> torch.Tensor:
         """One new token per row, x [B, hidden]: its k and v go to cache position lens[b] - 1 (rotated there when
         RoPE is on), then its query attends over the row's first lens[b] cached keys (the last window + 1 of them
-        with a sliding window), with the ALiBi bias when the module has it."""
+        with a sliding window), with the ALiBi bias when the module has it.  k_cache is a QuantizedKV (v_cache None)
+        for a quantized cache."""
         B = x.shape[0]
         q, k, v = self._project(x)
         q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
         k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
+        if isinstance(k_cache, QuantizedKV):
+            bits, g = k_cache.bits, k_cache.group_size
+            ops.kv_append_quant(q, k, v, *k_cache.buffers(), lens, bits, g, self.rope_tables, layout=rope_layout)
+            ctx = ops.attention_decode_quant(q, *k_cache.buffers(), lens, bits, g, self.scale, workspace,
+                                             window=window, alibi=self.alibi_slopes(q.device))
+            return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
         ops.kv_append(q, k, v, k_cache, v_cache, lens, self.rope_tables, layout=rope_layout)
         ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace, window=window,
                                    alibi=self.alibi_slopes(q.device))

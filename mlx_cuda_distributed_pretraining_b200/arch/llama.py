@@ -26,7 +26,7 @@ import torch
 from torch import nn
 
 from .. import ops
-from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask
+from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask, QuantizedKV
 
 VARIANTS = (None, "reference", "mlx_lm")
 
@@ -174,8 +174,8 @@ class AttentionModule(nn.Module):
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
         if x.dim() == 3:
             mask = CausalMask(x.shape[1], window) if prefix is None else PrefixCausalMask(prefix, x.shape[1])
-            return self.attn.forward_prefill(x, mask, cache.k[layer], cache.v[layer], self.rope_layout)
-        return self.attn.forward_decode(x, cache.k[layer], cache.v[layer], cache.lens, cache.workspace, window,
+            return self.attn.forward_prefill(x, mask, *cache.layer(layer), self.rope_layout)
+        return self.attn.forward_decode(x, *cache.layer(layer), cache.lens, cache.workspace, window,
                                         self.rope_layout)
 
 
@@ -247,26 +247,65 @@ class TransformerBlock(nn.Module):
 class KVCache:
     """Per-layer K and V buffers [B, s_max, Hk, D] in the model's activation dtype, and the number of valid positions
     per row: `lens` on the device (read by the kernels) and `host_lens` (so sizing a launch never reads the device).
-    s_max is rounded up to a multiple of 256, the decode kernel's chunk."""
+    s_max is rounded up to a multiple of 256, the decode kernel's chunk.
 
-    def __init__(self, model: "Model", batch: int, s_max: int):
+    kv_bits (4 or 8), kv_group_size (32, 64 or 128) and quantized_kv_start are the reference's quantized cache
+    (core/generation_lite.py:75-90, :100-108): once the longest row holds more than quantized_kv_start positions,
+    after prefill or after a decode step, every layer converts to a QuantizedKV and the unquantized buffers are
+    released.  When the prompt already passes the start, prefill writes the quantized cache directly and no
+    unquantized buffer is ever allocated; otherwise those buffers hold quantized_kv_start + 1 positions (rounded up to
+    256), all they can hold before conversion.  The buffers are allocated by the first set_lengths (prefill)."""
+
+    def __init__(self, model: "Model", batch: int, s_max: int, kv_bits: Optional[int] = None,
+                 kv_group_size: int = 64, quantized_kv_start: int = 0):
         a = model.args
         attn = model.layers[0].self_attn
+        if kv_bits is not None:
+            ops.check_kv_quant(kv_bits, kv_group_size, attn.head_dim, "KVCache")
+            if isinstance(quantized_kv_start, bool) or not isinstance(quantized_kv_start, int) \
+                    or quantized_kv_start < 0:
+                raise ValueError(f"quantized_kv_start must be a non-negative int, got {quantized_kv_start!r}")
+        self.kv_bits, self.kv_group_size, self.quantized_kv_start = kv_bits, kv_group_size, quantized_kv_start
         w = model.embed_tokens.weight
+        self._layers, self._device, self._dtype = a.num_hidden_layers, w.device, w.dtype
+        self._batch, self._heads = batch, (attn.num_kv_heads, attn.head_dim)
         self.s_max = max(256, -(-s_max // 256) * 256)
-        shape = (batch, self.s_max, attn.num_kv_heads, attn.head_dim)
-        self.k = [torch.zeros(shape, device=w.device, dtype=w.dtype) for _ in range(a.num_hidden_layers)]
-        self.v = [torch.zeros(shape, device=w.device, dtype=w.dtype) for _ in range(a.num_hidden_layers)]
+        self.k = self.v = None  # unquantized buffers, one per layer
+        self.quant = None       # QuantizedKV per layer once quantized
+        if kv_bits is None:
+            self._allocate(self.s_max)
         self.lens = torch.zeros(batch, device=w.device, dtype=torch.int32)
         self.host_lens = [0] * batch
         nbytes = ops.attention_decode_workspace_bytes(batch, attn.num_heads, self.s_max, attn.head_dim)
         self.workspace = torch.empty(max(nbytes, 16), device=w.device, dtype=torch.uint8)
+
+    def _allocate(self, positions: int) -> None:
+        shape = (self._batch, positions) + self._heads
+        self.k = [torch.zeros(shape, device=self._device, dtype=self._dtype) for _ in range(self._layers)]
+        self.v = [torch.zeros(shape, device=self._device, dtype=self._dtype) for _ in range(self._layers)]
+
+    def _allocate_quantized(self) -> None:
+        self.quant = [QuantizedKV(self._batch, self.s_max, *self._heads, self.kv_bits, self.kv_group_size,
+                                  self._device) for _ in range(self._layers)]
+
+    @property
+    def quantized(self) -> bool:
+        return self.quant is not None
+
+    def layer(self, i: int):
+        """(k, v) buffers of layer i, or (QuantizedKV, None) once the cache is quantized."""
+        return (self.quant[i], None) if self.quant is not None else (self.k[i], self.v[i])
 
     def set_lengths(self, lengths) -> None:
         if any(n < 1 or n > self.s_max for n in lengths):
             raise ValueError(f"lengths must lie in [1, {self.s_max}], got {list(lengths)}")
         self.host_lens = [int(n) for n in lengths]
         self.lens.copy_(torch.tensor(self.host_lens, dtype=torch.int32))
+        if self.k is None and self.quant is None:  # kv_bits: the prefill decides the first format
+            if max(self.host_lens) > self.quantized_kv_start:
+                self._allocate_quantized()
+            else:
+                self._allocate(min(self.s_max, -(-(self.quantized_kv_start + 1) // 256) * 256))
 
     def advance(self) -> None:
         """One more position per row (the token a decode step is about to append)."""
@@ -274,6 +313,23 @@ class KVCache:
             raise ValueError(f"KV cache full ({self.s_max} positions)")
         self.host_lens = [n + 1 for n in self.host_lens]
         self.lens.add_(1)
+
+    def maybe_quantize(self) -> None:
+        """maybe_quantize_kv_cache (core/generation_lite.py:75-90): with kv_bits, the first time the longest row
+        holds more than quantized_kv_start positions, convert every layer and release the unquantized buffers."""
+        if self.kv_bits is None or self.quant is not None or max(self.host_lens) <= self.quantized_kv_start:
+            return
+        n = max(self.host_lens)
+        self._allocate_quantized()
+        for k, v, qkv in zip(self.k, self.v, self.quant):
+            ops.kv_quantize(k, v, *qkv.buffers(), self.kv_bits, self.kv_group_size, n=n)
+        self.k = self.v = None
+
+    def nbytes(self) -> int:
+        """Bytes held by the K/V buffers."""
+        if self.quant is not None:
+            return sum(q.nbytes() for q in self.quant)
+        return 0 if self.k is None else sum(t.numel() * t.element_size() for t in self.k + self.v)
 
 
 class Model(nn.Module):
@@ -410,6 +466,7 @@ class Model(nn.Module):
         pending = None
         for i, layer in enumerate(self.layers):
             h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window, prefix)
+        cache.maybe_quantize()
         rows = torch.arange(B, device=tokens.device)
         last = torch.tensor([n - 1 for n in lengths], device=tokens.device)
         return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])
@@ -423,6 +480,7 @@ class Model(nn.Module):
         pending = None
         for i, layer in enumerate(self.layers):
             h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window)
+        cache.maybe_quantize()
         return self._row_logits(h, pending)
 
     # mlx nn.Module-style accessors used by the optimizers' update(model, grads) surface

@@ -3,6 +3,7 @@
     python -m core.generation --run <name> --prompt "..." [--max-tokens 256 --temperature 1.0 --min-p 0.05
                               --repetition-penalty 1.1 --repetition-context-size 20]
                               [--top-p P --seed N --num-samples N --checkpoint step_N --runs-dir runs]
+                              [--kv-bits {4,8} --kv-group-size {32,64,128} --quantized-kv-start N]
 
 The run's config.yaml (written by the trainer) rebuilds the model through Trainer(cfg, for_training=False), the
 checkpoint's weights are loaded into it, and `generate` prefills [BOS] + tokenize(prompt) once and then decodes one
@@ -126,14 +127,21 @@ def position_limit(args) -> Optional[int]:
 def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature: float = 1.0,
              min_p: Optional[float] = 0.05, top_p: Optional[float] = None, repetition_penalty: float = 1.1,
              repetition_context_size: int = 20, eos_token: Optional[int] = None, seed: Optional[int] = None,
-             on_step: Optional[Callable[[List[int]], None]] = None) -> List[List[int]]:
+             on_step: Optional[Callable[[List[int]], None]] = None, kv_bits: Optional[int] = None,
+             kv_group_size: int = 64, quantized_kv_start: int = 0) -> List[List[int]]:
     """Generates up to max_tokens tokens for each of the ragged prompts in one batch.  A row stops at EOS, which is
     included in its output.  Returns the generated tokens per row (prompt excluded).  Per step, the sampled tokens
-    are the one value read back from the device."""
+    are the one value read back from the device.  kv_bits (4 or 8; None: no quantization), kv_group_size and
+    quantized_kv_start select the reference's quantized KV cache (arch.llama.KVCache)."""
+    from .. import ops
     from ..arch.llama import KVCache
 
     if not prompts or any(len(p) == 0 for p in prompts):
         raise ValueError("every prompt needs at least one token")
+    if kv_bits is not None:
+        ops.check_kv_quant(kv_bits, kv_group_size, what="generate")
+        if isinstance(quantized_kv_start, bool) or not isinstance(quantized_kv_start, int) or quantized_kv_start < 0:
+            raise ValueError(f"generate: quantized_kv_start must be a non-negative int, got {quantized_kv_start!r}")
     limit = position_limit(model.args)
     longest = max(len(p) for p in prompts)
     if limit is not None and longest + max_tokens > limit:
@@ -148,7 +156,7 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     tokens = torch.zeros((B, longest), dtype=torch.int64)
     for b, p in enumerate(prompts):
         tokens[b, :len(p)] = torch.tensor(p, dtype=torch.int64)
-    cache = KVCache(model, B, longest + max_tokens)
+    cache = KVCache(model, B, longest + max_tokens, kv_bits, kv_group_size, quantized_kv_start)
     logits = model.prefill(tokens.to(device), [len(p) for p in prompts], cache)
     history = [list(p) for p in prompts]
     out: List[List[int]] = [[] for _ in prompts]
@@ -192,9 +200,17 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
     ap.add_argument("--checkpoint", type=str, default=None,
                     help="Checkpoint to load, e.g. step_1000 (default: the final checkpoint)")
     ap.add_argument("--runs-dir", type=str, default="runs", help="Directory holding the run directories")
+    ap.add_argument("--kv-bits", type=int, choices=(4, 8), default=None,
+                    help="Quantize the KV cache to this many bits (default: no quantization)")
+    ap.add_argument("--kv-group-size", type=int, choices=(32, 64, 128), default=64,
+                    help="Group size of the KV cache quantization")
+    ap.add_argument("--quantized-kv-start", type=int, default=0,
+                    help="Quantize the KV cache once it holds more than this many tokens")
     a = ap.parse_args(argv)
     if a.num_samples < 1:
         ap.error("--num-samples must be >= 1")
+    if a.quantized_kv_start < 0:
+        ap.error("--quantized-kv-start must be >= 0")
     return a
 
 
@@ -250,7 +266,8 @@ def main(argv: Optional[List[str]] = None) -> None:
     seed = a.seed if a.seed is not None else random.SystemRandom().randrange(1 << 62)
     outs = generate(trainer.model, [prompt] * a.num_samples, max_tokens=a.max_tokens, temperature=a.temperature,
                     min_p=a.min_p, top_p=a.top_p, repetition_penalty=a.repetition_penalty,
-                    repetition_context_size=a.repetition_context_size, eos_token=tok.EOS_TOKEN, seed=seed)
+                    repetition_context_size=a.repetition_context_size, eos_token=tok.EOS_TOKEN, seed=seed,
+                    kv_bits=a.kv_bits, kv_group_size=a.kv_group_size, quantized_kv_start=a.quantized_kv_start)
     for o in outs:
         print(f"Greedy Output: {tok.detokenize(o)}")
     sys.stdout.flush()

@@ -362,6 +362,16 @@ int launch_decode_d(int D, const CUtensorMap& tmK, const CUtensorMap& tmV, const
   }
 }
 
+// b200_rope's interleaved-pair rotation of one 8-column vector, c / sn = the vector's 4 table entries
+__device__ __forceinline__ void rope_pairs8(const float* xv, const float* cos4, const float* sin4, float* o) {
+  const float4 c = *reinterpret_cast<const float4*>(cos4);
+  const float4 sn = *reinterpret_cast<const float4*>(sin4);
+  o[0] = xv[0] * c.x - xv[1] * sn.x;  o[1] = xv[0] * sn.x + xv[1] * c.x;
+  o[2] = xv[2] * c.y - xv[3] * sn.y;  o[3] = xv[2] * sn.y + xv[3] * c.y;
+  o[4] = xv[4] * c.z - xv[5] * sn.z;  o[5] = xv[4] * sn.z + xv[5] * c.z;
+  o[6] = xv[6] * c.w - xv[7] * sn.w;  o[7] = xv[6] * sn.w + xv[7] * c.w;
+}
+
 // One thread per 8-column vector: q heads (rotated in place, RoPE only), then k heads (rotated when RoPE is on) and
 // v heads, both written to cache row pos = lens[b] - 1.  The rotation is b200_rope's arithmetic, statement for
 // statement, so a token rotated here equals the same token rotated by the prefill.
@@ -397,12 +407,7 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
     float xv[8], o[8];
     ld8(src, xv);
     if (rotate) {
-      const float4 c = *reinterpret_cast<const float4*>(cos_t + (long long)pos * (D / 2) + dv * 4);
-      const float4 sn = *reinterpret_cast<const float4*>(sin_t + (long long)pos * (D / 2) + dv * 4);
-      o[0] = xv[0] * c.x - xv[1] * sn.x;  o[1] = xv[0] * sn.x + xv[1] * c.x;
-      o[2] = xv[2] * c.y - xv[3] * sn.y;  o[3] = xv[2] * sn.y + xv[3] * c.y;
-      o[4] = xv[4] * c.z - xv[5] * sn.z;  o[5] = xv[4] * sn.z + xv[5] * c.z;
-      o[6] = xv[6] * c.w - xv[7] * sn.w;  o[7] = xv[6] * sn.w + xv[7] * c.w;
+      rope_pairs8(xv, cos_t + (long long)pos * (D / 2) + dv * 4, sin_t + (long long)pos * (D / 2) + dv * 4, o);
       st8(dst, o);
     } else {
       st8(dst, xv);
@@ -455,6 +460,451 @@ kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __res
       st8(dst + D / 2, xh);
     }
   }
+}
+
+// ---- quantized KV cache (DESIGN §4.2.1) --------------------------------------------------------------------------
+// Group-affine codes, mlx's scheme without its scale nudge: each group of g consecutive elements of a head vector is
+// x ~ s q + b with n = 2^BITS - 1, mn / mx the group's extremes, s = max((mx - mn) / n, 1e-7), b = mn (a -0 minimum
+// is stored as +0) and q = min(n, rint((x - b) / s)), all IEEE fp32, so |x - (s q + b)| <= s / 2.
+// Codes uint8 [B, s_max, Hk, D * BITS / 8] (4 bits: element 2j in the low nibble of byte j); parameters f32
+// [B, Hk, s_max, D / g, 2] holding (s, b), so a 32-key tile's parameters are one contiguous block.
+
+// Quantizes one 8-element slice per lane.  The g / 8 slices of a group sit on w = g / 8 consecutive, w-aligned lanes,
+// and every lane of the warp calls this (the min / max reductions shuffle over the full warp).  The group's lead lane
+// writes the parameters when `par` is non-null.
+template <int BITS>
+__device__ __forceinline__ void quantize_slice(const float* x, int w, uint8_t* codes, float* par) {
+  constexpr float n = (float)((1 << BITS) - 1);
+  float mx = x[0], mn = x[0];
+#pragma unroll
+  for (int e = 1; e < 8; ++e) {
+    mx = fmaxf(mx, x[e]);
+    mn = fminf(mn, x[e]);
+  }
+  for (int off = w >> 1; off > 0; off >>= 1) {
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, off));
+  }
+  const float s = fmaxf(__fdiv_rn(mx - mn, n), 1e-7f);
+  const float b = mn + 0.f;
+  uint32_t q[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) q[e] = (uint32_t)fminf(n, rintf(__fdiv_rn(x[e] - b, s)));
+  if (codes != nullptr) {
+    if constexpr (BITS == 8) {
+      *reinterpret_cast<uint2*>(codes) = make_uint2(q[0] | q[1] << 8 | q[2] << 16 | q[3] << 24,
+                                                    q[4] | q[5] << 8 | q[6] << 16 | q[7] << 24);
+    } else {
+      uint32_t u = 0;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) u |= q[e] << (4 * e);
+      *reinterpret_cast<uint32_t*>(codes) = u;
+    }
+    if (par != nullptr && (threadIdx.x & (w - 1)) == 0) *reinterpret_cast<float2*>(par) = make_float2(s, b);
+  }
+}
+
+// the 8 codes of one slice as exact floats 0 .. n (2^23 + c built in the mantissa, then 2^23 subtracted)
+template <int BITS>
+__device__ __forceinline__ void codes8(const uint8_t* p, float* f) {
+  if constexpr (BITS == 8) {
+    const uint2 u = *reinterpret_cast<const uint2*>(p);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      f[e] = __uint_as_float(__byte_perm(u.x, 0x4B000000u, 0x7540 + e)) - 8388608.f;
+      f[4 + e] = __uint_as_float(__byte_perm(u.y, 0x4B000000u, 0x7540 + e)) - 8388608.f;
+    }
+  } else {
+    const uint32_t u = *reinterpret_cast<const uint32_t*>(p);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(((u >> (4 * e)) & 0xFu) | 0x4B000000u) - 8388608.f;
+  }
+}
+
+// Positions [0, n) of a [B, S, Hk, D] K and V source into codes and parameters: one thread per 8-element slice, the
+// threads of a warp advancing together so that every group's lanes meet in quantize_slice.
+template <typename T, int BITS>
+__global__ void __launch_bounds__(256)
+kv_quantize_kernel(const T* __restrict__ k, const T* __restrict__ v, uint8_t* __restrict__ kc, uint8_t* __restrict__ vc,
+                   float* __restrict__ kp, float* __restrict__ vp, int n, int S, int B, int s_max, int Hk, int D,
+                   int g) {
+  const int L = D / 8, ng = D / g, Dc = D * BITS / 8;
+  const long long per = (long long)B * n * Hk * L;  // slices of K (then as many of V)
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) & ~31LL; i0 < 2 * per; i0 += stride) {
+    const long long i = i0 + (threadIdx.x & 31);
+    const bool valid = i < 2 * per;
+    const int which = valid && i >= per;
+    const long long r = valid ? i - which * per : 0;
+    const int sl = (int)(r % L);
+    const int h = (int)(r / L % Hk);
+    const int pos = (int)(r / L / Hk % n);
+    const int b = (int)(r / L / Hk / n);
+    float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (valid) ld8((which ? v : k) + (((long long)b * S + pos) * Hk + h) * D + sl * 8, x);
+    uint8_t* codes = valid ? (which ? vc : kc) + (((long long)b * s_max + pos) * Hk + h) * Dc + sl * BITS : nullptr;
+    float* par = (which ? vp : kp) + ((((long long)b * Hk + h) * s_max + pos) * ng + sl / (g / 8)) * 2;
+    quantize_slice<BITS>(x, g / 8, codes, par);
+  }
+}
+
+// kv_append for the quantized cache: one CTA per (kv head, row).  Its G query heads are rotated in place and its k
+// and v heads rotated / copied exactly as kv_append_kernel (interleaved) or kv_append_half_kernel (half) do, the k and
+// v results rounded to T through shared memory; then warp 0 quantizes both into position lens[b] - 1.
+template <typename T, int BITS>
+__global__ void __launch_bounds__(128)
+kv_append_quant_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v, uint8_t* __restrict__ kc,
+                       uint8_t* __restrict__ vc, float* __restrict__ kp, float* __restrict__ vp,
+                       const int* __restrict__ lens, const float* __restrict__ cos_t, const float* __restrict__ sin_t,
+                       int half, int s_max, int H, int Hk, int D, int g) {
+  __shared__ __align__(16) T kv[2 * 128];  // [k | v] of this head, rounded to T
+  const int hk = blockIdx.x, b = blockIdx.y, G = H / Hk;
+  const int pos = lens[b] - 1;
+  if (pos < 0 || pos >= s_max) return;  // outside the documented 1 <= lens[b] <= s_max: write nothing
+  const bool rope = cos_t != nullptr;
+  const int per_head = half ? D / 16 : D / 8;  // threads per head: slice pairs (half) or 8-column vectors
+  for (int i = threadIdx.x; i < (G + 2) * per_head; i += blockDim.x) {
+    const int dv = i % per_head, hh = i / per_head;  // hh < G: query head hk * G + hh; G: k; G + 1: v
+    if (hh < G && !rope) continue;
+    const T* src;
+    T* dst;
+    if (hh < G) {
+      src = dst = q + ((long long)b * H + hk * G + hh) * D + dv * 8;
+    } else {
+      src = (hh == G ? k : v) + ((long long)b * Hk + hk) * D + dv * 8;
+      dst = kv + (hh - G) * D + dv * 8;
+    }
+    const bool rotate = rope && hh <= G;
+    if (half) {
+      float xl[8], xh[8];
+      ld8(src, xl);
+      ld8(src + D / 2, xh);
+      if (rotate) {
+        float c[8], sn[8], ol[8], oh[8];
+        ld8(cos_t + (long long)pos * (D / 2) + dv * 8, c);
+        ld8(sin_t + (long long)pos * (D / 2) + dv * 8, sn);
+        rope_half8(xl, xh, c, sn, ol, oh);
+        st8(dst, ol);
+        st8(dst + D / 2, oh);
+      } else {
+        st8(dst, xl);
+        st8(dst + D / 2, xh);
+      }
+    } else {
+      float xv[8], o[8];
+      ld8(src, xv);
+      if (rotate) {
+        rope_pairs8(xv, cos_t + (long long)pos * (D / 2) + dv * 4, sin_t + (long long)pos * (D / 2) + dv * 4, o);
+        st8(dst, o);
+      } else {
+        st8(dst, xv);
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x >= 32) return;
+  const int L = D / 8, lane = threadIdx.x, which = lane / L, sl = lane % L;  // 2 L <= 32 lanes hold k and v
+  const bool valid = which < 2;
+  float x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (valid) ld8(kv + which * D + sl * 8, x);
+  const int Dc = D * BITS / 8, ng = D / g;
+  uint8_t* codes = valid ? (which ? vc : kc) + (((long long)b * s_max + pos) * Hk + hk) * Dc + sl * BITS : nullptr;
+  float* par = (which ? vp : kp) + ((((long long)b * Hk + hk) * s_max + pos) * ng + sl / (g / 8)) * 2;
+  quantize_slice<BITS>(x, g / 8, codes, par);
+}
+
+// Parameter positions per TMA box.  A box's first coordinate is innermost ([B, Hk, s_max * ng * 2] floats) and must
+// sit on a 16-byte boundary: with ng even every position does, with ng = 1 the box starts at the even position at or
+// below the tile's start and spans 34 positions (the one or two past the tile are fetched, never used).
+__host__ __device__ __forceinline__ int qdec_param_positions(int ng) { return ng == 1 ? DEC_TILE + 2 : DEC_TILE; }
+
+// Shared memory of attn_decode_quant_kernel: per ring stage the K codes, V codes, K parameters and V parameters of a
+// 32-key tile (each region a multiple of 128 bytes), then attn_decode_kernel's buffers plus the per-slice query sums.
+struct QDecSmem {
+  int kc, vc, kp, vp, stage, q, qs, s, ml, red, bar, total;
+  __host__ __device__ QDecSmem(int Dc, int ng, int D, int G) {
+    const int pr = (qdec_param_positions(ng) * ng * 8 + 127) & ~127;
+    kc = 0;
+    vc = DEC_TILE * Dc;
+    kp = 2 * DEC_TILE * Dc;
+    vp = kp + pr;
+    stage = vp + pr;
+    q = DEC_STAGES * stage;
+    qs = q + G * D * 4;
+    s = qs + G * (D / 8) * 4;
+    ml = s + G * DEC_TILE * 4;
+    red = ml + ((3 * G + 3) & ~3) * 4;
+    bar = red + DEC_THREADS * 8 * 4;
+    total = bar + DEC_STAGES * 8 + 128;
+  }
+};
+
+// attn_decode_kernel over the quantized cache, chunking, ring, softmax, merge and output unchanged.  Per key and
+// 8-column slice (inside one group with scale s, bias b) the score part is s (q . codes) + b (sum q), the slice's
+// query sum computed once per CTA; the value update is acc += (p s) codes, with the p b terms summed apart and added
+// to acc before the key subsets merge.  ALiBi is on when p.slopes is non-null.
+template <typename T, int D, int BITS>
+__global__ void __launch_bounds__(DEC_THREADS, 4)
+attn_decode_quant_kernel(const __grid_constant__ CUtensorMap tmKc, const __grid_constant__ CUtensorMap tmVc,
+                         const __grid_constant__ CUtensorMap tmKp, const __grid_constant__ CUtensorMap tmVp,
+                         const DecArgs p, const int g) {
+  constexpr int L = D / 8;
+  constexpr int Dc = D * BITS / 8;
+  constexpr int SB = BITS;  // code bytes per 8-column slice
+  const int ng = D / g, spg = g / 8;  // groups per head vector, slices per group
+  const int c = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
+  const int len = min(p.lens[b], p.s_max);
+  const int c0 = c * DEC_CHUNK;
+  const int kv0 = first_visible_key(p, len);
+  if (c0 >= len || c0 + DEC_CHUNK <= kv0) return;
+  const int lo = max(c0, kv0 & ~(DEC_TILE - 1));
+  const int end = min(len, c0 + DEC_CHUNK);
+  const int n_tiles = (end - lo + DEC_TILE - 1) / DEC_TILE;
+  const int n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK - kv0 / DEC_CHUNK;
+  const int G = p.G;
+  const bool alibi = p.slopes != nullptr;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 127) & ~uintptr_t(127));
+  const QDecSmem lay(Dc, ng, D, G);
+  float* sq = reinterpret_cast<float*>(smem + lay.q);
+  float* sqs = reinterpret_cast<float*>(smem + lay.qs);
+  float* ss = reinterpret_cast<float*>(smem + lay.s);
+  float* salpha = reinterpret_cast<float*>(smem + lay.ml);
+  float* sm = salpha + G;
+  float* sl = sm + G;
+  float* sred = reinterpret_cast<float*>(smem + lay.red);
+  const uint32_t bar0 = smem_u32(smem + lay.bar);
+  const int tile_bytes = 2 * (DEC_TILE * Dc + qdec_param_positions(ng) * ng * 8);
+
+  auto tile_start = [&](int j) { return min(lo + j * DEC_TILE, end - DEC_TILE); };
+  auto issue = [&](int j) {
+    const int st = j % DEC_STAGES;
+    const uint32_t bar = bar0 + 8 * st;
+    uint8_t* base = smem + st * lay.stage;
+    mbar_arrive_expect_tx(bar, tile_bytes);
+    tma_load_4d(smem_u32(base + lay.kc), &tmKc, bar, 0, hk, tile_start(j), b);
+    tma_load_4d(smem_u32(base + lay.vc), &tmVc, bar, 0, hk, tile_start(j), b);
+    const int p0 = ng == 1 ? tile_start(j) & ~1 : tile_start(j);  // a 16-byte aligned first coordinate
+    tma_load_3d(smem_u32(base + lay.kp), &tmKp, bar, p0 * ng * 2, hk, b);
+    tma_load_3d(smem_u32(base + lay.vp), &tmVp, bar, p0 * ng * 2, hk, b);
+  };
+
+  if (tid == 0) {
+    for (int s = 0; s < DEC_STAGES; ++s) mbar_init(bar0 + 8 * s, 1);
+    fence_mbar_init();
+    tma_prefetch_desc(&tmKc);
+    tma_prefetch_desc(&tmVc);
+    tma_prefetch_desc(&tmKp);
+    tma_prefetch_desc(&tmVp);
+  }
+  __syncthreads();
+  if (tid == 0)
+    for (int j = 0; j < min(n_tiles, DEC_STAGES); ++j) issue(j);
+
+  const T* qb = reinterpret_cast<const T*>(p.q) + ((long long)b * p.H + (long long)hk * G) * D;
+  for (int i = tid; i < G * L; i += DEC_THREADS) {
+    float f[8];
+    ld8(qb + i * 8, f);
+    float sum = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      sq[i * 8 + e] = f[e] * p.scale_log2;
+      sum += f[e] * p.scale_log2;
+    }
+    sqs[i] = sum;
+  }
+  for (int h = tid; h < G; h += DEC_THREADS) {
+    sm[h] = -INFINITY;
+    sl[h] = 0.f;
+    if (alibi) sred[h] = __ldg(p.slopes + hk * G + h) * kLog2e;
+  }
+
+  const int items = G * L;
+  const int ks_n = items <= DEC_THREADS ? DEC_THREADS / items : 1;
+  int my_item[DEC_MAX_ITEMS], my_ks;
+  if (items <= DEC_THREADS) {
+    my_ks = tid / items;
+    my_item[0] = my_ks < ks_n ? tid % items : -1;
+    my_item[1] = -1;
+  } else {
+    my_ks = 0;
+    my_item[0] = tid;
+    my_item[1] = tid + DEC_THREADS < items ? tid + DEC_THREADS : -1;
+  }
+  float acc[DEC_MAX_ITEMS][8], accb[DEC_MAX_ITEMS];
+#pragma unroll
+  for (int r = 0; r < DEC_MAX_ITEMS; ++r) {
+    accb[r] = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[r][e] = 0.f;
+  }
+  __syncthreads();
+
+  for (int j = 0; j < n_tiles; ++j) {
+    const int st = j % DEC_STAGES;
+    mbar_wait(bar0 + 8 * st, (j / DEC_STAGES) & 1);
+    const uint8_t* base = smem + st * lay.stage;
+    const uint8_t* tKc = base + lay.kc;
+    const uint8_t* tVc = base + lay.vc;
+    const int start = tile_start(j);
+    const int poff = ng == 1 ? (start & 1) * 2 : 0;  // floats before the tile's first parameter pair
+    const float* tKp = reinterpret_cast<const float*>(base + lay.kp) + poff;
+    const float* tVp = reinterpret_cast<const float*>(base + lay.vp) + poff;
+    const int first_valid = max(lo + j * DEC_TILE, kv0);
+
+    {
+      const int kl = tid % L;
+      for (int key = tid / L; key < DEC_TILE; key += DEC_THREADS / L) {
+        float kf[8];
+        codes8<BITS>(tKc + key * Dc + kl * SB, kf);
+        const float2 sb = *reinterpret_cast<const float2*>(tKp + (key * ng + kl / spg) * 2);
+        const bool valid = start + key >= first_valid;
+        for (int h = 0; h < G; ++h) {
+          const float4 qa = *reinterpret_cast<const float4*>(sq + h * D + kl * 8);
+          const float4 qc = *reinterpret_cast<const float4*>(sq + h * D + kl * 8 + 4);
+          float d = qa.x * kf[0];
+          d = fmaf(qa.y, kf[1], d);
+          d = fmaf(qa.z, kf[2], d);
+          d = fmaf(qa.w, kf[3], d);
+          d = fmaf(qc.x, kf[4], d);
+          d = fmaf(qc.y, kf[5], d);
+          d = fmaf(qc.z, kf[6], d);
+          d = fmaf(qc.w, kf[7], d);
+          d = fmaf(sb.x, d, sb.y * sqs[h * L + kl]);
+#pragma unroll
+          for (int off = L / 2; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+          if (kl == 0) ss[h * DEC_TILE + key] = valid ? d : -INFINITY;
+        }
+      }
+    }
+    __syncthreads();
+
+    const float kd = (float)(start + lane - (len - 1));
+    for (int h = warp; h < G; h += DEC_THREADS / 32) {
+      float x = ss[h * DEC_TILE + lane];
+      if (alibi) x = x + sred[h] * kd;
+      const float m_old = sm[h];
+      const float m_new = fmaxf(m_old, warp_max(x));
+      const float pe = exp2f(x - m_new);
+      const float sum = warp_sum(pe);
+      ss[h * DEC_TILE + lane] = pe;
+      __syncwarp();
+      if (lane == 0) {
+        const float alpha = exp2f(m_old - m_new);
+        salpha[h] = alpha;
+        sl[h] = sl[h] * alpha + sum;
+        sm[h] = m_new;
+      }
+    }
+    __syncthreads();
+
+#pragma unroll
+    for (int r = 0; r < DEC_MAX_ITEMS; ++r) {
+      if (my_item[r] < 0) continue;
+      const int h = my_item[r] / L, sc = my_item[r] % L;
+      const float a = salpha[h];
+      accb[r] *= a;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[r][e] *= a;
+      const int gp = (sc / spg) * 2;
+      for (int key = my_ks; key < DEC_TILE; key += ks_n) {
+        const float pe = ss[h * DEC_TILE + key];
+        const float2 sb = *reinterpret_cast<const float2*>(tVp + key * ng * 2 + gp);
+        float vf[8];
+        codes8<BITS>(tVc + key * Dc + sc * SB, vf);
+        const float ps = pe * sb.x;
+        accb[r] = fmaf(pe, sb.y, accb[r]);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[r][e] = fmaf(ps, vf[e], acc[r][e]);
+      }
+    }
+    __syncthreads();
+    if (tid == 0 && j + DEC_STAGES < n_tiles) issue(j + DEC_STAGES);
+  }
+
+#pragma unroll
+  for (int r = 0; r < DEC_MAX_ITEMS; ++r)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc[r][e] += accb[r];
+
+  if (ks_n > 1) {
+    if (my_item[0] >= 0)
+#pragma unroll
+      for (int e = 0; e < 8; ++e) sred[(my_ks * items + my_item[0]) * 8 + e] = acc[0][e];
+    __syncthreads();
+    if (tid < items) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) acc[0][e] = sred[tid * 8 + e];
+      for (int k = 1; k < ks_n; ++k)
+#pragma unroll
+        for (int e = 0; e < 8; ++e) acc[0][e] += sred[(k * items + tid) * 8 + e];
+      my_item[0] = tid;
+    } else {
+      my_item[0] = -1;
+    }
+  }
+
+#pragma unroll
+  for (int r = 0; r < DEC_MAX_ITEMS; ++r) {
+    if (my_item[r] < 0) continue;
+    const int h = my_item[r] / L, sc = my_item[r] % L;
+    const long long bh = (long long)b * p.H + hk * G + h;
+    const float m = sm[h], l = sl[h];
+    if (n_chunks == 1) {
+      const float inv = 1.0f / l;
+      float f[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) f[e] = acc[r][e] * inv;
+      st8(reinterpret_cast<T*>(p.o) + bh * D + sc * 8, f);
+      if (p.lse != nullptr && sc == 0) p.lse[bh] = (m + log2f(l)) / kLog2e;
+    } else {
+      st8(p.part_acc + (bh * p.max_chunks + c) * D + sc * 8, acc[r]);
+      if (sc == 0) {
+        p.part_ml[(bh * p.max_chunks + c) * 2] = m;
+        p.part_ml[(bh * p.max_chunks + c) * 2 + 1] = l;
+      }
+    }
+  }
+}
+
+template <typename T, int D, int BITS>
+int launch_decode_quant(const CUtensorMap* tm, const DecArgs& a, int g, int B, int Hk, cudaStream_t stream) {
+  auto kern = attn_decode_quant_kernel<T, D, BITS>;
+  const QDecSmem lay(D * BITS / 8, D / g, D, a.G);
+  static int attr_bytes = 0;
+  if (lay.total > 48 * 1024 && lay.total > attr_bytes) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+    attr_bytes = lay.total;
+  }
+  kern<<<dim3(a.max_chunks, Hk, B), DEC_THREADS, lay.total, stream>>>(tm[0], tm[1], tm[2], tm[3], a, g);
+  B200_CHECK_LAUNCH();
+  if (a.max_chunks > 1) {
+    attn_decode_combine_kernel<T, D><<<dim3(a.H, B), D, 0, stream>>>(a);
+    B200_CHECK_LAUNCH();
+  }
+  return B200_OK;
+}
+
+template <typename T, int BITS>
+int launch_decode_quant_d(int D, const CUtensorMap* tm, const DecArgs& a, int g, int B, int Hk, cudaStream_t stream) {
+  switch (D) {
+    case 32: return launch_decode_quant<T, 32, BITS>(tm, a, g, B, Hk, stream);
+    case 64: return launch_decode_quant<T, 64, BITS>(tm, a, g, B, Hk, stream);
+    default: return launch_decode_quant<T, 128, BITS>(tm, a, g, B, Hk, stream);
+  }
+}
+
+// the format's argument checks shared by the three quantized-cache entries
+int check_quant_format(const char* what, int B, int s_max, int Hk, int D, int bits, int g) {
+  B200_CHECK_ARG(bits == 4 || bits == 8, "%s: kv_bits=%d unsupported (4 or 8)", what, bits);
+  B200_CHECK_ARG(g == 32 || g == 64 || g == 128, "%s: group size %d unsupported (32, 64 or 128)", what, g);
+  B200_CHECK_ARG(D == 32 || D == 64 || D == 128, "%s: head_dim %d unsupported (32, 64 or 128)", what, D);
+  B200_CHECK_ARG(D % g == 0, "%s: the group size %d must divide head_dim %d", what, g, D);
+  B200_CHECK_ARG(B > 0 && Hk > 0 && s_max > 0 && s_max % 2 == 0, "%s: bad shape B=%d s_max=%d (even) Hk=%d", what, B,
+                 s_max, Hk);
+  return B200_OK;
 }
 
 // window < 0 means none; slopes selects ALiBi
@@ -590,6 +1040,146 @@ int b200_kv_append_half(void* q, const void* k, const void* v, void* k_cache, vo
                                                              sin_t, nslice, s_max, H, Hk, D);
   B200_CHECK_LAUNCH();
   return B200_OK;
+}
+
+// The quantized KV cache of the reference's generator (core/generation_lite.py:75-90, :100-108, :190-195): the
+// conversion maybe_quantize_kv_cache makes, as codes and parameters written in place (DESIGN §4.2.1).
+int b200_kv_quantize(const void* k, const void* v, int n, int S, void* k_codes, void* v_codes, float* k_params,
+                     float* v_params, int B, int s_max, int Hk, int D, int bits, int group_size, int is_bf16,
+                     void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  if ((rc = check_quant_format("kv_quantize", B, s_max, Hk, D, bits, group_size))) return rc;
+  B200_CHECK_ARG(n >= 0 && n <= S && n <= s_max, "kv_quantize: n=%d must lie in [0, min(S=%d, s_max=%d)]", n, S, s_max);
+  B200_CHECK_ARG(al16(k) && al16(v) && al16(k_codes) && al16(v_codes) && al16(k_params) && al16(v_params),
+                 "kv_quantize: every pointer must be 16-byte aligned");
+  if (n == 0) return B200_OK;
+  const long long slices = 2LL * B * n * Hk * (D / 8);
+  long long blocks = (slices + 255) / 256;
+  if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+  auto* kc = static_cast<uint8_t*>(k_codes);
+  auto* vc = static_cast<uint8_t*>(v_codes);
+  if (is_bf16) {
+    auto* kk = static_cast<const __nv_bfloat16*>(k);
+    auto* vv = static_cast<const __nv_bfloat16*>(v);
+    if (bits == 8)
+      kv_quantize_kernel<__nv_bfloat16, 8><<<(int)blocks, 256, 0, s>>>(kk, vv, kc, vc, k_params, v_params, n, S, B,
+                                                                       s_max, Hk, D, group_size);
+    else
+      kv_quantize_kernel<__nv_bfloat16, 4><<<(int)blocks, 256, 0, s>>>(kk, vv, kc, vc, k_params, v_params, n, S, B,
+                                                                       s_max, Hk, D, group_size);
+  } else {
+    auto* kk = static_cast<const float*>(k);
+    auto* vv = static_cast<const float*>(v);
+    if (bits == 8)
+      kv_quantize_kernel<float, 8><<<(int)blocks, 256, 0, s>>>(kk, vv, kc, vc, k_params, v_params, n, S, B, s_max, Hk,
+                                                               D, group_size);
+    else
+      kv_quantize_kernel<float, 4><<<(int)blocks, 256, 0, s>>>(kk, vv, kc, vc, k_params, v_params, n, S, B, s_max, Hk,
+                                                               D, group_size);
+  }
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// b200_kv_append / b200_kv_append_half (half != 0) into the quantized cache (core/generation_lite.py:139, :149: the
+// decode steps after conversion)
+int b200_kv_append_quant(void* q, const void* k, const void* v, void* k_codes, void* v_codes, float* k_params,
+                         float* v_params, const int* lens, const float* cos_t, const float* sin_t, int half, int B,
+                         int s_max, int H, int Hk, int D, int bits, int group_size, int is_bf16, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc;
+  if ((rc = check_quant_format("kv_append_quant", B, s_max, Hk, D, bits, group_size))) return rc;
+  B200_CHECK_ARG(H > 0 && H % Hk == 0, "kv_append_quant: H=%d must be a multiple of Hk=%d", H, Hk);
+  B200_CHECK_ARG((cos_t == nullptr) == (sin_t == nullptr), "kv_append_quant: give both RoPE tables or neither");
+  B200_CHECK_ARG(!half || cos_t != nullptr, "kv_append_quant: the half layout needs the RoPE tables");
+  B200_CHECK_ARG(lens != nullptr && al16(q) && al16(k) && al16(v) && al16(k_codes) && al16(v_codes) &&
+                     al16(k_params) && al16(v_params) && (cos_t == nullptr || (al16(cos_t) && al16(sin_t))),
+                 "kv_append_quant: alignment (16 bytes) or null lens");
+  const dim3 grid(Hk, B);
+  auto* kc = static_cast<uint8_t*>(k_codes);
+  auto* vc = static_cast<uint8_t*>(v_codes);
+  if (is_bf16) {
+    auto* qq = static_cast<__nv_bfloat16*>(q);
+    auto* kk = static_cast<const __nv_bfloat16*>(k);
+    auto* vv = static_cast<const __nv_bfloat16*>(v);
+    if (bits == 8)
+      kv_append_quant_kernel<__nv_bfloat16, 8><<<grid, 128, 0, s>>>(qq, kk, vv, kc, vc, k_params, v_params, lens,
+                                                                    cos_t, sin_t, half, s_max, H, Hk, D, group_size);
+    else
+      kv_append_quant_kernel<__nv_bfloat16, 4><<<grid, 128, 0, s>>>(qq, kk, vv, kc, vc, k_params, v_params, lens,
+                                                                    cos_t, sin_t, half, s_max, H, Hk, D, group_size);
+  } else {
+    auto* qq = static_cast<float*>(q);
+    auto* kk = static_cast<const float*>(k);
+    auto* vv = static_cast<const float*>(v);
+    if (bits == 8)
+      kv_append_quant_kernel<float, 8><<<grid, 128, 0, s>>>(qq, kk, vv, kc, vc, k_params, v_params, lens, cos_t,
+                                                            sin_t, half, s_max, H, Hk, D, group_size);
+    else
+      kv_append_quant_kernel<float, 4><<<grid, 128, 0, s>>>(qq, kk, vv, kc, vc, k_params, v_params, lens, cos_t,
+                                                            sin_t, half, s_max, H, Hk, D, group_size);
+  }
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// b200_attn_decode_alibi (window < 0: none, slopes null: no ALiBi) over the quantized cache (the attention the
+// reference's decode steps run once the cache is a QuantizedKVCache, core/generation_lite.py:139)
+int b200_attn_decode_quant(const void* q, const void* k_codes, const void* v_codes, const float* k_params,
+                           const float* v_params, const int* lens, void* o, float* lse, int window,
+                           const float* slopes, int B, int s_max, int H, int Hk, int D, int bits, int group_size,
+                           float scale, int is_bf16, void* ws, size_t ws_bytes, void* stream) {
+  int rc;
+  if ((rc = check_quant_format("attn_decode_quant", B, s_max, Hk, D, bits, group_size))) return rc;
+  B200_CHECK_ARG(H > 0 && H % Hk == 0, "attn_decode_quant: H=%d must be a multiple of Hk=%d", H, Hk);
+  B200_CHECK_ARG(s_max >= DEC_TILE, "attn_decode_quant: s_max=%d must be >= %d", s_max, DEC_TILE);
+  const int G = H / Hk;
+  B200_CHECK_ARG(G * D <= DEC_MAX_ITEMS * DEC_THREADS * 8, "attn_decode_quant: (H/Hk) * D = %d exceeds %d", G * D,
+                 DEC_MAX_ITEMS * DEC_THREADS * 8);
+  B200_CHECK_ARG(al16(q) && al16(o) && lens != nullptr, "attn_decode_quant: q / o must be 16-byte aligned, lens non-null");
+  B200_CHECK_ARG(slopes == nullptr || (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
+                 "attn_decode_quant: slopes must be a 4-byte aligned fp32 [H] array");
+  const size_t need = b200_attn_decode_workspace_bytes(B, H, s_max, D);
+  if (ws_bytes < need || (need > 0 && ws == nullptr)) {
+    set_error("attn_decode_quant: workspace of %zu bytes, %zu needed", ws_bytes, need);
+    return B200_ERR_WORKSPACE;
+  }
+  const int Dc = D * bits / 8, ng = D / group_size;
+  const uint64_t cdims[4] = {(uint64_t)Dc, (uint64_t)Hk, (uint64_t)s_max, (uint64_t)B};
+  const uint64_t cstrides[3] = {(uint64_t)Dc, (uint64_t)Hk * Dc, (uint64_t)s_max * Hk * Dc};
+  const uint32_t cbox[4] = {(uint32_t)Dc, 1, (uint32_t)DEC_TILE, 1};
+  // parameters as [B, Hk, s_max * ng * 2] floats: a tile's block is one box (qdec_param_positions)
+  const uint64_t pdims[3] = {(uint64_t)s_max * ng * 2, (uint64_t)Hk, (uint64_t)B};
+  const uint64_t pstrides[2] = {(uint64_t)s_max * ng * 8, (uint64_t)Hk * s_max * ng * 8};
+  const uint32_t pbox[3] = {(uint32_t)(qdec_param_positions(ng) * ng * 2), 1, 1};
+  CUtensorMap tm[4];
+  if ((rc = make_tensor_map(&tm[0], k_codes, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 4, cdims, cstrides, cbox, false))) return rc;
+  if ((rc = make_tensor_map(&tm[1], v_codes, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, 4, cdims, cstrides, cbox, false))) return rc;
+  if ((rc = make_tensor_map(&tm[2], k_params, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 3, pdims, pstrides, pbox, false)))
+    return rc;
+  if ((rc = make_tensor_map(&tm[3], v_params, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, 3, pdims, pstrides, pbox, false)))
+    return rc;
+  DecArgs a;
+  a.q = q;
+  a.o = o;
+  a.lse = lse;
+  a.lens = lens;
+  a.max_chunks = (s_max + DEC_CHUNK - 1) / DEC_CHUNK;
+  a.part_acc = reinterpret_cast<float*>(ws);
+  a.part_ml = a.part_acc + (size_t)B * H * a.max_chunks * D;
+  a.H = H;
+  a.G = G;
+  a.s_max = s_max;
+  a.scale_log2 = scale * kLog2e;
+  a.window = window < 0 || window > s_max ? s_max : window;
+  a.slopes = slopes;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (is_bf16)
+    return bits == 8 ? launch_decode_quant_d<__nv_bfloat16, 8>(D, tm, a, group_size, B, Hk, s)
+                     : launch_decode_quant_d<__nv_bfloat16, 4>(D, tm, a, group_size, B, Hk, s);
+  return bits == 8 ? launch_decode_quant_d<float, 8>(D, tm, a, group_size, B, Hk, s)
+                   : launch_decode_quant_d<float, 4>(D, tm, a, group_size, B, Hk, s);
 }
 
 }  // extern "C"

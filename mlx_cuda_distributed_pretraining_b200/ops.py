@@ -1107,6 +1107,162 @@ def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.
 
 
 # ------------------------------------------------------------------------------------------------
+# the quantized KV cache (the reference's kv_bits / kv_group_size; DESIGN §4.2.1): per layer, codes uint8
+# [B, s_max, Hk, D * bits / 8] and parameters fp32 [B, Hk, s_max, D / group_size, 2] for each of K and V
+# ------------------------------------------------------------------------------------------------
+KV_BITS = (4, 8)
+KV_GROUP_SIZES = (32, 64, 128)
+
+
+def check_kv_quant(bits, group_size, head_dim: Optional[int] = None, what: str = "kv cache") -> None:
+    """Raises ValueError unless bits is 4 or 8, group_size is 32, 64 or 128 and (given head_dim) it divides head_dim,
+    which must then be 32, 64 or 128."""
+    if isinstance(bits, bool) or bits not in KV_BITS:
+        raise ValueError(f"{what}: kv_bits must be 4 or 8, got {bits!r}")
+    if isinstance(group_size, bool) or group_size not in KV_GROUP_SIZES:
+        raise ValueError(f"{what}: kv_group_size must be 32, 64 or 128, got {group_size!r}")
+    if head_dim is not None and (head_dim not in (32, 64, 128) or head_dim % group_size):
+        raise ValueError(f"{what}: a quantized KV cache needs head_dim in (32, 64, 128) divisible by kv_group_size "
+                         f"{group_size}, got head_dim {head_dim}")
+
+
+def kv_quant_shapes(B: int, s_max: int, Hk: int, D: int, bits: int, group_size: int):
+    """(codes shape, parameters shape) of one K or V buffer of the quantized cache."""
+    return (B, s_max, Hk, D * bits // 8), (B, Hk, s_max, D // group_size, 2)
+
+
+def _check_quant_cache(k_codes, v_codes, k_params, v_params, B: int, Hk: int, D: int, bits: int, group_size: int,
+                       device, what: str) -> int:
+    """The four buffers of one layer's quantized cache; returns s_max."""
+    check_kv_quant(bits, group_size, D, what)
+    if k_codes.dim() != 4:
+        raise ValueError(f"{what}: k_codes must be [B, s_max, Hk, D * bits / 8], got {tuple(k_codes.shape)}")
+    s_max = k_codes.shape[1]
+    cshape, pshape = kv_quant_shapes(B, s_max, Hk, D, bits, group_size)
+    bufs = ((k_codes, "k_codes", torch.uint8, cshape), (v_codes, "v_codes", torch.uint8, cshape),
+            (k_params, "k_params", torch.float32, pshape), (v_params, "v_params", torch.float32, pshape))
+    for t, nm, dt, shp in bufs:
+        if t.dtype != dt or tuple(t.shape) != shp:
+            raise ValueError(f"{what}: {nm} must be {dt} {list(shp)}, got {t.dtype} {list(t.shape)}")
+    for t, nm, dt, _ in bufs:
+        _need(t, dt, f"{what}: {nm}")
+        if t.device != device or t.data_ptr() % 16:
+            raise ValueError(f"{what}: {nm} must be 16-byte aligned on {device}")
+    if s_max % 2:
+        raise ValueError(f"{what}: s_max {s_max} must be even")
+    return s_max
+
+
+def kv_quantize(k: torch.Tensor, v: torch.Tensor, k_codes: torch.Tensor, v_codes: torch.Tensor,
+                k_params: torch.Tensor, v_params: torch.Tensor, bits: int, group_size: int,
+                n: Optional[int] = None) -> None:
+    """Quantizes positions [0, n) (default: all S) of k, v [B, S, Hk, D] (bf16 or fp32) into the cache buffers
+    (b200_kv_quantize).  Positions at or past n are not written."""
+    _is_bf16(k, "kv_quantize: k")
+    if k.dim() != 4 or v.shape != k.shape or v.dtype != k.dtype:
+        raise ValueError(f"kv_quantize: k and v must both be [B, S, Hk, D] of one dtype, got {k.dtype} "
+                         f"{tuple(k.shape)}, {v.dtype} {tuple(v.shape)}")
+    B, S, Hk, D = k.shape
+    s_max = _check_quant_cache(k_codes, v_codes, k_params, v_params, B, Hk, D, bits, group_size, k.device,
+                               "kv_quantize")
+    _need(k, k.dtype, "kv_quantize: k")
+    _need(v, k.dtype, "kv_quantize: v")
+    n = S if n is None else n
+    if isinstance(n, bool) or not isinstance(n, int) or not 0 <= n <= min(S, s_max):
+        raise ValueError(f"kv_quantize: n must be an int in [0, min(S={S}, s_max={s_max})], got {n!r}")
+    if k.data_ptr() % 16 or v.data_ptr() % 16:
+        raise ValueError("kv_quantize: k and v must be 16-byte aligned")
+    check(lib().b200_kv_quantize(k.data_ptr(), v.data_ptr(), n, S, k_codes.data_ptr(), v_codes.data_ptr(),
+                                 k_params.data_ptr(), v_params.data_ptr(), B, s_max, Hk, D, bits, group_size,
+                                 _is_bf16(k, "k"), _stream()), "b200_kv_quantize")
+
+
+def kv_append_quant(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_codes: torch.Tensor, v_codes: torch.Tensor,
+                    k_params: torch.Tensor, v_params: torch.Tensor, lens: torch.Tensor, bits: int, group_size: int,
+                    rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                    layout: str = "interleaved") -> None:
+    """kv_append into the quantized cache (b200_kv_append_quant): q [B,H,D] is rotated in place exactly as
+    kv_append rotates it, and the rotated k [B,Hk,D] and v, rounded to q's dtype, are quantized into position
+    lens[b] - 1."""
+    _check_choice(layout, ROPE_LAYOUTS, "kv_append_quant: layout")
+    _is_bf16(q, "kv_append_quant: q")
+    for t, nm in ((q, "q"), (k, "k"), (v, "v")):
+        if t.dim() != 3 or t.dtype != q.dtype:
+            raise ValueError(f"kv_append_quant: {nm} must be a [B, heads, D] {q.dtype} tensor, got {t.dtype} "
+                             f"{tuple(t.shape)}")
+    B, H, D = q.shape
+    if k.shape != v.shape or k.shape[0] != B or k.shape[2] != D or H % k.shape[1]:
+        raise ValueError(f"kv_append_quant: k, v must be [{B}, Hk, {D}] with H % Hk == 0, got {tuple(k.shape)}, "
+                         f"{tuple(v.shape)}")
+    Hk = k.shape[1]
+    s_max = _check_quant_cache(k_codes, v_codes, k_params, v_params, B, Hk, D, bits, group_size, q.device,
+                               "kv_append_quant")
+    for t, nm in ((q, "q"), (k, "k"), (v, "v")):
+        _need(t, q.dtype, f"kv_append_quant: {nm}")
+        if t.data_ptr() % 16:
+            raise ValueError(f"kv_append_quant: {nm} must be 16-byte aligned")
+    if lens.dtype != torch.int32 or lens.device != q.device or lens.shape != (B,) or not lens.is_contiguous():
+        raise ValueError(f"kv_append_quant: lens must be a contiguous int32 [B] tensor on {q.device}")
+    cos_t = sin_t = None
+    if rope_tables is not None:
+        cos_t, sin_t = rope_tables
+        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
+            _need(t, torch.float32, f"kv_append_quant: {nm}")
+            if t.dim() != 2 or t.shape[1] != D // 2:
+                raise ValueError(f"kv_append_quant: RoPE tables must be [positions, {D // 2}]")
+    half = int(layout == "half" and cos_t is not None)
+    check(lib().b200_kv_append_quant(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_codes.data_ptr(), v_codes.data_ptr(),
+                                     k_params.data_ptr(), v_params.data_ptr(), lens.data_ptr(), _ptr(cos_t),
+                                     _ptr(sin_t), half, B, s_max, H, Hk, D, bits, group_size, _is_bf16(q, "q"),
+                                     _stream()), "b200_kv_append_quant")
+
+
+def attention_decode_quant(q: torch.Tensor, k_codes: torch.Tensor, v_codes: torch.Tensor, k_params: torch.Tensor,
+                           v_params: torch.Tensor, lens: torch.Tensor, bits: int, group_size: int,
+                           scale: Optional[float] = None, workspace: Optional[torch.Tensor] = None,
+                           return_lse: bool = False, window: Optional[int] = None,
+                           alibi: Optional[torch.Tensor] = None):
+    """attention_decode over the quantized cache (b200_attn_decode_quant): the same result over the dequantised keys
+    and values s q + b, with the same lens, window, alibi, workspace and return_lse semantics.  q [B,H,D] bf16 or
+    fp32, D in {32, 64, 128}."""
+    _is_bf16(q, "attention_decode_quant: q")
+    if q.dim() != 3 or k_codes.dim() != 4:
+        raise ValueError(f"attention_decode_quant: expected q [B,H,D] and k_codes [B,s_max,Hk,Dc], got "
+                         f"{tuple(q.shape)}, {tuple(k_codes.shape)}")
+    B, H, D = q.shape
+    Hk = k_codes.shape[2]
+    check_kv_quant(bits, group_size, D, "attention_decode_quant")
+    if H % Hk:
+        raise ValueError(f"attention_decode_quant: H={H} must be a multiple of Hk={Hk}")
+    s_max = _check_quant_cache(k_codes, v_codes, k_params, v_params, B, Hk, D, bits, group_size, q.device,
+                               "attention_decode_quant")
+    _need(q, q.dtype, "attention_decode_quant: q")
+    if lens.dtype != torch.int32 or lens.device != q.device or lens.shape != (B,) or not lens.is_contiguous():
+        raise ValueError(f"attention_decode_quant: lens must be a contiguous int32 [B] tensor on {q.device}")
+    if window is not None:
+        window = _check_window(window, "attention_decode_quant")
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, True, "attention_decode_quant")
+    if scale is None:
+        scale = D ** -0.5
+    need = attention_decode_workspace_bytes(B, H, s_max, D)
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
+    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need:
+        raise ValueError(f"attention_decode_quant: workspace must be uint8 on {q.device} with >= {need} bytes")
+    o = torch.empty_like(q)
+    lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
+    tok = _t0("attn_decode")
+    check(lib().b200_attn_decode_quant(q.data_ptr(), k_codes.data_ptr(), v_codes.data_ptr(), k_params.data_ptr(),
+                                       v_params.data_ptr(), lens.data_ptr(), o.data_ptr(), _ptr(lse),
+                                       -1 if window is None else min(int(window), s_max), _ptr(alibi), B, s_max, H,
+                                       Hk, D, bits, group_size, float(scale), _is_bf16(q, "q"), workspace.data_ptr(),
+                                       workspace.numel(), _stream()), "b200_attn_decode_quant")
+    _t1(tok)
+    return (o, lse) if return_lse else o
+
+
+# ------------------------------------------------------------------------------------------------
 # raw strided GEMM + Shampoo elementwise helpers
 # ------------------------------------------------------------------------------------------------
 def gemm_raw(a_mn: bool, b_mn: bool, M: int, N: int, K: int, batch: int,
