@@ -430,6 +430,19 @@ int b200_attn_bwd_dropout(const void* q, const void* k, const void* v, const voi
                           int H, int Hk, int D, float scale, int causal, float p, unsigned long long seed,
                           int dkv_row_heads, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- generation: a chunk of queries against a KV cache (core/generation_lite.py:104-105, :119-122, :144-154: the
+ * prompt_cache and prefill_step_size of the reference's generate_step) ------------------------------------------
+ * q, o: bf16 [B, L, H, D]; k_cache, v_cache: bf16 [B, s_max, Hk, D] already holding the chunk's own keys; start,
+ * end: device int32 [B].  Query i of row b sits at position p = start[b] + i and sees cached key k iff
+ * max(0, p - window) <= k <= p (window < 0: no window), for i < end[b] - start[b]; later rows are padding, their
+ * outputs finite but unspecified.  Cache positions at or past end[b] may hold anything (NaN included) and never
+ * reach the result.  slopes (device fp32 [H], or NULL) adds ALiBi's slopes[h] * (k - p) to every score.  lse: f32
+ * [B, H, L] natural-log sum-exp of the scaled scores, or NULL.  D in {64, 128}.  One CTA per (128 queries, head,
+ * row) with no split over keys, so a row's output is bit-identical alone or in any batch; no host synchronisation. */
+int b200_attn_fwd_cached(const void* q, const void* k_cache, const void* v_cache, const int* start, const int* end,
+                         void* o, float* lse, int window, const float* slopes, int B, int L, int s_max, int H, int Hk,
+                         int D, float scale, void* stream);
+
 /* ---- generation: decode attention over a KV cache (arch/flash_attention.py:97-156, last query row) ------------
  * One new query per sequence against its cached keys, causal by construction (every cached key precedes it):
  *   q, o: [B,H,D]; k_cache, v_cache: [B,s_max,Hk,D] (the training layout [B,S,Hk,D]); q head h reads kv head
@@ -488,6 +501,12 @@ int b200_kv_quantize(const void* k, const void* v, int n, int S, void* k_codes, 
 int b200_kv_append_quant(void* q, const void* k, const void* v, void* k_codes, void* v_codes, float* k_params,
                          float* v_params, const int* lens, const float* cos_t, const float* sin_t, int half, int B,
                          int s_max, int H, int Hk, int D, int bits, int group_size, int is_bf16, void* stream);
+/* b200_kv_dequantize: positions [0, min(end[b], S)) of row b of the codes and parameters into bf16 k, v
+ *   [B, S, Hk, D], each value s q + b in f32 (product and sum rounded separately) rounded once to bf16; nothing at
+ *   or past end[b] is written.  end: device int32 [B]; 1 <= S <= s_max. */
+int b200_kv_dequantize(const void* k_codes, const void* v_codes, const float* k_params, const float* v_params,
+                       const int* end, void* k, void* v, int S, int B, int s_max, int Hk, int D, int bits,
+                       int group_size, void* stream);
 /* b200_attn_decode_alibi over a quantized cache: window < 0 is no window, slopes NULL is no ALiBi.  q and o bf16 or
  *   f32 [B, H, D]; same chunking, workspace (b200_attn_decode_workspace_bytes) and merge order, so a row's output is
  *   bit-identical alone or in any batch. */

@@ -277,3 +277,43 @@ class FlashAttention(nn.Module):
         ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace, window=window,
                                    alibi=self.alibi_slopes(q.device))
         return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
+
+    def forward_extend(self, x: torch.Tensor, k_cache, v_cache: Optional[torch.Tensor], chunk,
+                       window: Optional[int] = None, rope_layout: str = "interleaved") -> torch.Tensor:
+        """A chunk of new tokens per row, x [B, L, hidden] right-padded, appended at each row's current cache length
+        (chunk: the llama.CacheChunk of the call).  Token i of row b sits at position p = chunk.start[b] + i: its q
+        and k are rotated there (ops.rope at absolute positions), its k and v are written to that cache position
+        (quantized first when k_cache is a QuantizedKV, v_cache None), and its query attends over the row's cached
+        keys max(0, p - window) .. p (ops.attention_cached), over the cache's dequantised values once it is
+        quantized."""
+        B, L, _ = x.shape
+        q, k, v = self._project(x)
+        q = q.reshape(B, L, self.num_heads, self.head_dim)
+        k = k.reshape(B, L, self.num_kv_heads, self.head_dim)
+        v = v.reshape(B, L, self.num_kv_heads, self.head_dim)
+        if self.rope_tables is not None:
+            cos_t, sin_t = self.rope_tables
+            q = ops.rope(q, cos_t, sin_t, chunk.pos, rope_layout)
+            k = ops.rope(k, cos_t, sin_t, chunk.pos, rope_layout)
+        q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
+        r, src, dst = chunk.rows, chunk.src, chunk.dst
+        if isinstance(k_cache, QuantizedKV):
+            bits, g = k_cache.bits, k_cache.group_size
+            tmp = QuantizedKV(B, L + L % 2, self.num_kv_heads, self.head_dim, bits, g, x.device)
+            ops.kv_quantize(k, v, *tmp.buffers(), bits, g)
+            for t, u in zip(k_cache.buffers()[:2], tmp.buffers()[:2]):
+                t[r, dst] = u[r, src]
+            for t, u in zip(k_cache.buffers()[2:], tmp.buffers()[2:]):
+                t[r, :, dst] = u[r, :, src]
+            if chunk.scratch is None:  # one layer's bf16 K / V, reused by every layer of the call
+                shape = (B, chunk.max_end, self.num_kv_heads, self.head_dim)
+                chunk.scratch = (torch.empty(shape, device=x.device, dtype=torch.bfloat16),
+                                 torch.empty(shape, device=x.device, dtype=torch.bfloat16))
+            k_att, v_att = ops.kv_dequantize(*k_cache.buffers(), chunk.end, bits, g, out=chunk.scratch)
+        else:
+            k_cache[r, dst] = k[r, src]
+            v_cache[r, dst] = v[r, src]
+            k_att, v_att = k_cache, v_cache
+        ctx = ops.attention_cached(q, k_att, v_att, chunk.start, chunk.end, self.scale, window=window,
+                                   alibi=self.alibi_slopes(q.device))
+        return self._out(ctx.reshape(B, L, self.num_heads * self.head_dim))

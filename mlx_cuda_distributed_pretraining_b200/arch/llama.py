@@ -166,12 +166,15 @@ class AttentionModule(nn.Module):
         return self.attn(x, mask=mask, rope_layout=self.rope_layout, dropout_seed=dropout_seed)
 
     def cached(self, x: torch.Tensor, cache: "KVCache", layer: int, window: Optional[int] = None,
-               prefix: Optional[torch.Tensor] = None) -> torch.Tensor:
+               prefix: Optional[torch.Tensor] = None, chunk: Optional["CacheChunk"] = None) -> torch.Tensor:
         """This layer's attention against the KV cache: prefill when x is [B, S, hidden], one decode step when x is
-        [B, hidden].  window: the model's sliding window (None: causal).  prefix (int32 [B], prefill only): the
-        prefix-LM mask's prefix lengths."""
+        [B, hidden], a chunk appended at the cache's current lengths when chunk is given (x [B, L, hidden]).
+        window: the model's sliding window (None: causal).  prefix (int32 [B], prefill only): the prefix-LM mask's
+        prefix lengths."""
         if self.apply_rope and self.attn.rope_tables is None:
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
+        if chunk is not None:
+            return self.attn.forward_extend(x, *cache.layer(layer), chunk, window, self.rope_layout)
         if x.dim() == 3:
             mask = CausalMask(x.shape[1], window) if prefix is None else PrefixCausalMask(prefix, x.shape[1])
             return self.attn.forward_prefill(x, mask, *cache.layer(layer), self.rope_layout)
@@ -232,14 +235,14 @@ class TransformerBlock(nn.Module):
         return h, self._ffn(y, token_mask, aux)
 
     def forward_cached(self, h: torch.Tensor, pending, cache: "KVCache", layer: int, window: Optional[int] = None,
-                       prefix: Optional[torch.Tensor] = None):
+                       prefix: Optional[torch.Tensor] = None, chunk: Optional["CacheChunk"] = None):
         """forward_fused with the attention run against the KV cache (AttentionModule.cached)."""
         n1, n2 = self.input_layernorm, self.post_attention_layernorm
         if pending is None:
             y = n1(h)
         else:
             h, y = ops.add_rmsnorm(h, pending, n1.weight, n1.eps)
-        a = self.self_attn.cached(y, cache, layer, window, prefix)
+        a = self.self_attn.cached(y, cache, layer, window, prefix, chunk)
         h, y = ops.add_rmsnorm(h, a, n2.weight, n2.eps)
         return h, self._ffn(y)
 
@@ -307,6 +310,37 @@ class KVCache:
             else:
                 self._allocate(min(self.s_max, -(-(self.quantized_kv_start + 1) // 256) * 256))
 
+    def extend_lengths(self, counts) -> None:
+        """counts[b] >= 0 more positions for row b (one Model.extend chunk): host_start keeps the lengths before it.
+        Until the cache is quantized, the unquantized buffers grow (copied into larger ones, at most s_max positions)
+        when the chunk needs room; a kv_bits cache that holds nothing yet starts unquantized, because the reference
+        attends a chunk over the unquantized cache and converts afterwards (maybe_quantize)."""
+        counts = [int(n) for n in counts]
+        if len(counts) != self._batch or any(n < 0 for n in counts):
+            raise ValueError(f"counts must be {self._batch} non-negative ints, got {counts}")
+        ends = [n + c for n, c in zip(self.host_lens, counts)]
+        if max(ends) > self.s_max:
+            raise ValueError(f"KV cache full: rows would hold {max(ends)} positions, the cache has {self.s_max}")
+        if self.quant is None:
+            have = 0 if self.k is None else self.k[0].shape[1]
+            if max(ends) > have:
+                old_k, old_v = self.k, self.v
+                self._allocate(min(self.s_max, -(-max(ends) // 256) * 256))
+                if old_k is not None:
+                    for new, old in zip(self.k + self.v, old_k + old_v):
+                        new[:, :have].copy_(old)
+        self.host_start = list(self.host_lens)
+        self.host_lens = ends
+        self.lens.copy_(torch.tensor(ends, dtype=torch.int32))
+
+    def truncate(self, lengths) -> None:
+        """Shortens row b to lengths[b] <= its current length: later positions are left as they are and never read."""
+        lengths = [int(n) for n in lengths]
+        if len(lengths) != self._batch or any(not 0 <= n <= m for n, m in zip(lengths, self.host_lens)):
+            raise ValueError(f"truncate: lengths must lie in [0, current lengths {self.host_lens}], got {lengths}")
+        self.host_lens = lengths
+        self.lens.copy_(torch.tensor(lengths, dtype=torch.int32))
+
     def advance(self) -> None:
         """One more position per row (the token a decode step is about to append)."""
         if max(self.host_lens) + 1 > self.s_max:
@@ -330,6 +364,29 @@ class KVCache:
         if self.quant is not None:
             return sum(q.nbytes() for q in self.quant)
         return 0 if self.k is None else sum(t.numel() * t.element_size() for t in self.k + self.v)
+
+
+class CacheChunk:
+    """The positions one Model.extend call appends, as the layers read them: row b's tokens i < n_b of the chunk
+    [B, L] go to cache positions start[b] + i.  start / end: int32 [B] on the device (the lengths before and after);
+    pos: int32 [B, L] rotation positions (padding tokens take their row's last position, so that no rotation reads
+    past the tables); rows / src / dst: int64 indices of the valid tokens (row, index in the chunk, cache position);
+    scratch: a quantized cache's bf16 K / V for the call, made by its first layer."""
+
+    def __init__(self, start, counts, L: int, device):
+        ends = [a + n for a, n in zip(start, counts)]
+        self.start = torch.tensor(start, dtype=torch.int32).to(device)
+        self.end = torch.tensor(ends, dtype=torch.int32).to(device)
+        self.max_end = max(ends)
+        rows = [b for b, n in enumerate(counts) for _ in range(n)]
+        src = [i for n in counts for i in range(n)]
+        self.rows = torch.tensor(rows, dtype=torch.int64).to(device)
+        self.src = torch.tensor(src, dtype=torch.int64).to(device)
+        self.dst = torch.tensor([start[b] + i for b, i in zip(rows, src)], dtype=torch.int64).to(device)
+        last = torch.tensor([max(e - 1, 0) for e in ends], dtype=torch.int64)
+        pos = torch.minimum(torch.tensor(start, dtype=torch.int64)[:, None] + torch.arange(L)[None], last[:, None])
+        self.pos = pos.to(torch.int32).to(device)
+        self.scratch = None
 
 
 class Model(nn.Module):
@@ -469,6 +526,44 @@ class Model(nn.Module):
         cache.maybe_quantize()
         rows = torch.arange(B, device=tokens.device)
         last = torch.tensor([n - 1 for n in lengths], device=tokens.device)
+        return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])
+
+    def check_extend(self, cache: KVCache, counts=None) -> None:
+        """Raises ValueError when Model.extend cannot serve this model and cache (counts: the tokens per row)."""
+        attn = self.layers[0].self_attn
+        if self.embed_tokens.weight.dtype != torch.bfloat16:
+            raise ValueError(f"chunked prefill needs a bf16 model and cache, got {self.embed_tokens.weight.dtype} "
+                             "(the one-shot prefill serves other dtypes)")
+        if attn.head_dim not in (64, 128):
+            raise ValueError(f"chunked prefill needs head_dim 64 or 128, got {attn.head_dim} (the one-shot prefill "
+                             "serves other head dims)")
+        if self.args.prefix_lm and counts is not None \
+                and any(n > 0 and m == 0 for n, m in zip(counts, cache.host_lens)):
+            raise ValueError("a prefix-LM model's first prompt cannot be split into chunks: its prefix attends to the "
+                             "keys of later chunks (give it whole to Model.prefill)")
+
+    @torch.no_grad()
+    def extend(self, tokens: torch.Tensor, lengths, cache: KVCache) -> torch.Tensor:
+        """Appends the right-padded tokens [B, L] (row b valid in [0, lengths[b]), lengths[b] may be 0) at each row's
+        current cache length, each token attending over its row's cache as in decoding, and returns the fp32 logits
+        [B, V] after each row's last new token (a row with no new token gets its padding's logits).  The quantized
+        cache converts afterwards, as after a prefill (maybe_quantize)."""
+        B, L = tokens.shape
+        counts = [int(n) for n in lengths]
+        if B != cache._batch:
+            raise ValueError(f"tokens have {B} rows, the cache {cache._batch}")
+        if len(counts) != B or any(not 0 <= n <= L for n in counts) or max(counts) < 1:
+            raise ValueError(f"lengths must be {B} ints in [0, {L}], at least one positive, got {counts}")
+        self.check_extend(cache, counts)
+        cache.extend_lengths(counts)
+        chunk = CacheChunk(cache.host_start, counts, L, tokens.device)
+        h = ops.embedding(tokens, self.embed_tokens.weight)
+        pending = None
+        for i, layer in enumerate(self.layers):
+            h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window, chunk=chunk)
+        cache.maybe_quantize()
+        rows = torch.arange(B, device=tokens.device)
+        last = torch.tensor([max(n - 1, 0) for n in counts], device=tokens.device)
         return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])
 
     @torch.no_grad()

@@ -4,6 +4,7 @@
                               --repetition-penalty 1.1 --repetition-context-size 20]
                               [--top-p P --seed N --num-samples N --checkpoint step_N --runs-dir runs]
                               [--kv-bits {4,8} --kv-group-size {32,64,128} --quantized-kv-start N]
+                              [--prefill-step-size N]
 
 The run's config.yaml (written by the trainer) rebuilds the model through Trainer(cfg, for_training=False), the
 checkpoint's weights are loaded into it, and `generate` prefills [BOS] + tokenize(prompt) once and then decodes one
@@ -124,29 +125,89 @@ def position_limit(args) -> Optional[int]:
     return args.max_position_embeddings
 
 
+def prefill_chunks(prompts: Sequence[Sequence[int]], step: int) -> List[List[List[int]]]:
+    """The chunks of prefill_step_size = step: chunk c holds tokens [c step, (c + 1) step) of every prompt (empty for
+    a prompt already done), until the longest prompt is used up."""
+    longest = max(len(p) for p in prompts)
+    return [[list(p[c0:c0 + step]) for p in prompts] for c0 in range(0, longest, step)]
+
+
+def _prefill(model, prompts: List[List[int]], cache, step: Optional[int]) -> torch.Tensor:
+    """The fp32 logits [B, V] after each prompt's last token, the prompts appended to what the cache holds: in chunks
+    of `step` tokens (None: one chunk), each through Model.extend, except that the first chunk of an empty cache goes
+    through Model.prefill.  A row's logits come from the chunk that holds its last token."""
+    device = model.embed_tokens.weight.device
+    empty = all(n == 0 for n in cache.host_lens)
+    logits = None
+    for c, chunk in enumerate(prefill_chunks(prompts, step or max(len(p) for p in prompts))):
+        counts = [len(t) for t in chunk]
+        tokens = torch.zeros((len(chunk), max(counts)), dtype=torch.int64)
+        for b, t in enumerate(chunk):
+            tokens[b, :len(t)] = torch.tensor(t, dtype=torch.int64)
+        run = model.prefill if empty and c == 0 else model.extend
+        lg = run(tokens.to(device), counts, cache)
+        if logits is None:
+            logits = lg
+        else:
+            fresh = torch.tensor([n > 0 for n in counts], device=device)
+            logits = torch.where(fresh[:, None], lg, logits)
+    return logits
+
+
 def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature: float = 1.0,
              min_p: Optional[float] = 0.05, top_p: Optional[float] = None, repetition_penalty: float = 1.1,
              repetition_context_size: int = 20, eos_token: Optional[int] = None, seed: Optional[int] = None,
              on_step: Optional[Callable[[List[int]], None]] = None, kv_bits: Optional[int] = None,
-             kv_group_size: int = 64, quantized_kv_start: int = 0) -> List[List[int]]:
+             kv_group_size: int = 64, quantized_kv_start: int = 0, prefill_step_size: Optional[int] = None,
+             prompt_cache=None) -> List[List[int]]:
     """Generates up to max_tokens tokens for each of the ragged prompts in one batch.  A row stops at EOS, which is
     included in its output.  Returns the generated tokens per row (prompt excluded).  Per step, the sampled tokens
     are the one value read back from the device.  kv_bits (4 or 8; None: no quantization), kv_group_size and
-    quantized_kv_start select the reference's quantized KV cache (arch.llama.KVCache)."""
+    quantized_kv_start select the reference's quantized KV cache (arch.llama.KVCache).
+
+    prefill_step_size (int >= 1): the prompts go through the model in chunks of that many tokens (Model.extend), each
+    attending over the cache the earlier chunks filled, so prefill holds B x step activations rather than
+    B x prompt.  prompt_cache: a KVCache of batch len(prompts) that the caller built and keeps (its kv settings
+    apply; a different kv_bits is an error).  The prompts are appended to what it holds, and it is updated in place
+    so that it ends holding prompt + output of every row, ready for the next turn.  Without both, the prompts go
+    through Model.prefill in one piece."""
     from .. import ops
     from ..arch.llama import KVCache
 
     if not prompts or any(len(p) == 0 for p in prompts):
         raise ValueError("every prompt needs at least one token")
-    if kv_bits is not None:
+    if prefill_step_size is not None and (isinstance(prefill_step_size, bool) or not isinstance(prefill_step_size, int)
+                                          or prefill_step_size < 1):
+        raise ValueError(f"generate: prefill_step_size must be None or an int >= 1, got {prefill_step_size!r}")
+    if prompt_cache is not None:
+        if not isinstance(prompt_cache, KVCache):
+            raise ValueError(f"generate: prompt_cache must be an arch.llama.KVCache, got {type(prompt_cache).__name__}")
+        if kv_bits is not None and kv_bits != prompt_cache.kv_bits:
+            raise ValueError(f"generate: kv_bits={kv_bits!r} conflicts with the prompt_cache's kv_bits "
+                             f"{prompt_cache.kv_bits!r} (the cache's settings apply)")
+        if prompt_cache._batch != len(prompts):
+            raise ValueError(f"generate: prompt_cache holds {prompt_cache._batch} rows, {len(prompts)} prompts given")
+    elif kv_bits is not None:
         ops.check_kv_quant(kv_bits, kv_group_size, what="generate")
         if isinstance(quantized_kv_start, bool) or not isinstance(quantized_kv_start, int) or quantized_kv_start < 0:
             raise ValueError(f"generate: quantized_kv_start must be a non-negative int, got {quantized_kv_start!r}")
+    start = [0] * len(prompts) if prompt_cache is None else list(prompt_cache.host_lens)
     limit = position_limit(model.args)
     longest = max(len(p) for p in prompts)
-    if limit is not None and longest + max_tokens > limit:
-        raise ValueError(f"prompt ({longest} tokens) + max_tokens ({max_tokens}) exceeds max_position_embeddings "
-                         f"({limit}): training truncates there and the RoPE tables end there")
+    reach = max(s + len(p) for s, p in zip(start, prompts)) + max_tokens
+    if limit is not None and reach > limit:
+        raise ValueError(f"cached ({max(start)}) + prompt ({longest} tokens) + max_tokens ({max_tokens}) exceeds "
+                         f"max_position_embeddings ({limit}): training truncates there and the RoPE tables end there")
+    if prompt_cache is not None and reach > prompt_cache.s_max:
+        raise ValueError(f"generate: prompt_cache holds {prompt_cache.s_max} positions, {reach} needed (cached + prompt "
+                         f"+ max_tokens)")
+    chunked = prefill_step_size is not None or any(start)
+    if chunked:
+        if prefill_step_size is not None and model.args.prefix_lm and not any(start) and longest > prefill_step_size:
+            raise ValueError("generate: a prefix-LM model's first prompt cannot be split into chunks (its prefix "
+                             f"attends to keys of later chunks): prompt of {longest} tokens, prefill_step_size "
+                             f"{prefill_step_size}")
+        model.check_extend(prompt_cache)
     device = model.embed_tokens.weight.device
     gen = None
     if temperature != 0:
@@ -156,8 +217,13 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     tokens = torch.zeros((B, longest), dtype=torch.int64)
     for b, p in enumerate(prompts):
         tokens[b, :len(p)] = torch.tensor(p, dtype=torch.int64)
-    cache = KVCache(model, B, longest + max_tokens, kv_bits, kv_group_size, quantized_kv_start)
-    logits = model.prefill(tokens.to(device), [len(p) for p in prompts], cache)
+    cache = prompt_cache
+    if cache is None:
+        cache = KVCache(model, B, longest + max_tokens, kv_bits, kv_group_size, quantized_kv_start)
+    if chunked:
+        logits = _prefill(model, prompts, cache, prefill_step_size)
+    else:
+        logits = model.prefill(tokens.to(device), [len(p) for p in prompts], cache)
     history = [list(p) for p in prompts]
     out: List[List[int]] = [[] for _ in prompts]
     done = [False] * B
@@ -179,6 +245,11 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
         if all(done) or step + 1 == max_tokens:
             break
         logits = model.decode_step(nxt, cache)
+    if prompt_cache is not None:
+        # the reference feeds every token it yields: feed the last ones, then drop what finished rows were fed past EOS
+        if max_tokens > 0:
+            model.decode_step(nxt, cache)
+        cache.truncate([s + len(p) + len(o) for s, p, o in zip(start, prompts, out)])
     return out
 
 
@@ -206,11 +277,15 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
                     help="Group size of the KV cache quantization")
     ap.add_argument("--quantized-kv-start", type=int, default=0,
                     help="Quantize the KV cache once it holds more than this many tokens")
+    ap.add_argument("--prefill-step-size", type=int, default=None,
+                    help="Prefill the prompt in chunks of this many tokens (default: the whole prompt at once)")
     a = ap.parse_args(argv)
     if a.num_samples < 1:
         ap.error("--num-samples must be >= 1")
     if a.quantized_kv_start < 0:
         ap.error("--quantized-kv-start must be >= 0")
+    if a.prefill_step_size is not None and a.prefill_step_size < 1:
+        ap.error("--prefill-step-size must be >= 1")
     return a
 
 
@@ -267,7 +342,8 @@ def main(argv: Optional[List[str]] = None) -> None:
     outs = generate(trainer.model, [prompt] * a.num_samples, max_tokens=a.max_tokens, temperature=a.temperature,
                     min_p=a.min_p, top_p=a.top_p, repetition_penalty=a.repetition_penalty,
                     repetition_context_size=a.repetition_context_size, eos_token=tok.EOS_TOKEN, seed=seed,
-                    kv_bits=a.kv_bits, kv_group_size=a.kv_group_size, quantized_kv_start=a.quantized_kv_start)
+                    kv_bits=a.kv_bits, kv_group_size=a.kv_group_size, quantized_kv_start=a.quantized_kv_start,
+                    prefill_step_size=a.prefill_step_size)
     for o in outs:
         print(f"Greedy Output: {tok.detokenize(o)}")
     sys.stdout.flush()

@@ -548,6 +548,38 @@ kv_quantize_kernel(const T* __restrict__ k, const T* __restrict__ v, uint8_t* __
   }
 }
 
+// The inverse for a chunk that attends over a quantized cache: positions [0, end[b]) of row b (and below S) of the
+// codes and parameters into bf16 [B, S, Hk, D] K and V, one thread per 8-element slice.  The value is s q + b in fp32
+// with the product and the sum rounded separately (no fma, so the bits are those of the format's definition), then
+// rounded once to bf16.  Nothing at or past end[b] is written.
+template <int BITS>
+__global__ void __launch_bounds__(256)
+kv_dequantize_kernel(const uint8_t* __restrict__ kc, const uint8_t* __restrict__ vc, const float* __restrict__ kp,
+                     const float* __restrict__ vp, const int* __restrict__ end, __nv_bfloat16* __restrict__ k,
+                     __nv_bfloat16* __restrict__ v, int S, int B, int s_max, int Hk, int D, int g) {
+  const int L = D / 8, ng = D / g, Dc = D * BITS / 8;
+  const long long per = (long long)B * S * Hk * L;  // slices of K (then as many of V)
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < 2 * per; i += stride) {
+    const int which = i >= per;
+    const long long r = i - which * per;
+    const int sl = (int)(r % L);
+    const int h = (int)(r / L % Hk);
+    const int pos = (int)(r / L / Hk % S);
+    const int b = (int)(r / L / Hk / S);
+    if (pos >= __ldg(end + b)) continue;
+    float f[8];
+    codes8<BITS>((which ? vc : kc) + (((long long)b * s_max + pos) * Hk + h) * Dc + sl * BITS, f);
+    const float2 sb = *reinterpret_cast<const float2*>(
+        (which ? vp : kp) + ((((long long)b * Hk + h) * s_max + pos) * ng + sl / (g / 8)) * 2);
+    uint32_t w[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e)
+      w[e] = pack_bf16x2(__fadd_rn(__fmul_rn(sb.x, f[2 * e]), sb.y), __fadd_rn(__fmul_rn(sb.x, f[2 * e + 1]), sb.y));
+    stg128((which ? v : k) + (((long long)b * S + pos) * Hk + h) * D + sl * 8, make_uint4(w[0], w[1], w[2], w[3]));
+  }
+}
+
 // kv_append for the quantized cache: one CTA per (kv head, row).  Its G query heads are rotated in place and its k
 // and v heads rotated / copied exactly as kv_append_kernel (interleaved) or kv_append_half_kernel (half) do, the k and
 // v results rounded to T through shared memory; then warp 0 quantizes both into position lens[b] - 1.
@@ -1120,6 +1152,37 @@ int b200_kv_append_quant(void* q, const void* k, const void* v, void* k_codes, v
       kv_append_quant_kernel<float, 4><<<grid, 128, 0, s>>>(qq, kk, vv, kc, vc, k_params, v_params, lens, cos_t,
                                                             sin_t, half, s_max, H, Hk, D, group_size);
   }
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// Positions [0, end[b]) of the quantized cache as bf16 K and V [B, S, Hk, D]: the keys and values a chunk of queries
+// attends over once the cache is quantized (QuantizedKVCache.update_and_fetch of the reference quantizes the chunk
+// first, core/generation_lite.py:144-154)
+int b200_kv_dequantize(const void* k_codes, const void* v_codes, const float* k_params, const float* v_params,
+                       const int* end, void* k, void* v, int S, int B, int s_max, int Hk, int D, int bits,
+                       int group_size, void* stream) {
+  int rc;
+  if ((rc = check_quant_format("kv_dequantize", B, s_max, Hk, D, bits, group_size))) return rc;
+  B200_CHECK_ARG(S > 0 && S <= s_max, "kv_dequantize: S=%d must lie in [1, s_max=%d]", S, s_max);
+  B200_CHECK_ARG(end != nullptr && (reinterpret_cast<uintptr_t>(end) & 3u) == 0,
+                 "kv_dequantize: end must be a non-null, 4-byte aligned int32 [B] array");
+  B200_CHECK_ARG(al16(k_codes) && al16(v_codes) && al16(k_params) && al16(v_params) && al16(k) && al16(v),
+                 "kv_dequantize: every buffer must be 16-byte aligned");
+  const long long slices = 2LL * B * S * Hk * (D / 8);
+  long long blocks = (slices + 255) / 256;
+  if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  auto* kc = static_cast<const uint8_t*>(k_codes);
+  auto* vc = static_cast<const uint8_t*>(v_codes);
+  auto* kk = static_cast<__nv_bfloat16*>(k);
+  auto* vv = static_cast<__nv_bfloat16*>(v);
+  if (bits == 8)
+    kv_dequantize_kernel<8><<<(int)blocks, 256, 0, s>>>(kc, vc, k_params, v_params, end, kk, vv, S, B, s_max, Hk, D,
+                                                        group_size);
+  else
+    kv_dequantize_kernel<4><<<(int)blocks, 256, 0, s>>>(kc, vc, k_params, v_params, end, kk, vv, S, B, s_max, Hk, D,
+                                                        group_size);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

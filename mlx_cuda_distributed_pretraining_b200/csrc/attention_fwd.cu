@@ -48,6 +48,18 @@
 // 32 calls (both rows, chunks nc = 4 m + l) and the quad exchanges the 8-bit results with 4 shuffles per row.  Bit
 // 2 nc + c of keep[r] is this thread's key 8 nc + 2 l + c of row r.  DROP = false compiles to the kernels above
 // unchanged.
+//
+// Cached queries (CACHED = true, on the causal DOC = false kernels, with or without ALiBi): a chunk of L queries per
+// row attends over a KV cache [B, s_max, Hk, D] that already holds its own keys.  Query row i of batch row b sits at
+// position p = start[b] + i and sees key k iff max(0, p - W) <= k <= p, for the rows i < n_b = end[b] - start[b];
+// rows i >= n_b are padding.  Each CTA reads start[b] and end[b] itself.  A CTA with only padding rows writes zeros
+// and returns.  Otherwise its key tiles are anchored at kend, one past its last valid row's position (kend <= end[b]):
+// tile j holds keys kend - 128 (n_kv - j) .., so no cache position at or past kend is ever loaded (those may hold
+// anything, and 0 * NaN would reach O through the P V MMA); keys below 0 are TMA's zero fill and masked.  The element
+// mask `key > p || key < max(0, p - W)` runs, per thread, on the tiles its rows' diagonal crosses (at most two, as
+// the tiles are not aligned to the queries) and on those reaching below its rows' window start.  Padding rows take the last valid
+// row's position and their Q rows are zeroed in shared memory, so their outputs are finite whatever Q holds there.
+// CACHED = false compiles to the kernels above unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -85,6 +97,9 @@ struct FwdArgs {
   uint32_t drop_t;      // DROP: keep threshold t = round(p 65536) on the 16-bit Philox values
   float drop_inv;       // DROP: 1 / (1 - t / 65536)
   unsigned long long drop_seed;  // DROP: Philox key
+  const int* start;     // CACHED: [B] int32 position of each row's first query; S is the chunk length L
+  const int* end;       // CACHED: [B] int32 cached positions once the chunk is in (its last query's position + 1)
+  int s_max;            // CACHED: positions of the K / V cache
 };
 
 // first key query `row` of batch row b may see: its document start, or its window start when that is later
@@ -120,12 +135,13 @@ __device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db)
   else wgmma_m64n64k16_rs<1>(o, a, db);
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false, bool CACHED = false>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdArgs p) {
   static_assert(!PREFIX || (!DOC && !ALIBI), "the prefix mask is built on the causal kernel");
   static_assert(!PREFIX || !DROP, "dropout is not built on the prefix kernels");
+  static_assert(!CACHED || (!DOC && !PREFIX && !DROP), "cached queries are built on the causal kernel");
   using Cfg = FwdCfg<D>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -147,6 +163,24 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   // first key tile: the first query's document / window start (0 without documents)
   int j0 = 0;
   if constexpr (DOC) j0 = max(0, key_start(p, b, q0)) / ATT_BKV;
+  // CACHED: the row's first query position and valid rows, and the first key of tile 0
+  int c_st = 0, c_nv = 0, kbase = 0;
+  if constexpr (CACHED) {
+    c_st = max(__ldg(p.start + b), 0);
+    c_nv = min(min(__ldg(p.end + b), p.s_max) - c_st, p.S);
+    if (q0 >= c_nv) {  // padding rows only
+      const int rows = min(ATT_BQ, p.S - q0);
+      for (int i = threadIdx.x; i < rows * (D / 8); i += FWD_THREADS) {
+        const long long row = (long long)b * p.S + q0 + i / (D / 8);
+        stg128(p.o + (row * p.H + h) * D + (i % (D / 8)) * 8, make_uint4(0u, 0u, 0u, 0u));
+        if (i % (D / 8) == 0 && p.lse != nullptr) p.lse[((long long)b * p.H + h) * p.S + q0 + i / (D / 8)] = 0.f;
+      }
+      return;
+    }
+    const int kend = c_st + min(q0 + ATT_BQ, c_nv);
+    n_kv = (kend - max(0, c_st + q0 - p.window) + ATT_BKV - 1) / ATT_BKV;
+    kbase = kend - n_kv * ATT_BKV;
+  }
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
@@ -171,8 +205,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const uint32_t full = kv_full0 + 8 * s;
         mbar_arrive_expect_tx(full, 2 * Cfg::KV_BYTES);
         for (int nb = 0; nb < Cfg::NB; ++nb) {
-          tma_load_4d(sK + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmK, full, nb * 64, hk, j * ATT_BKV, b);
-          tma_load_4d(sV + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmV, full, nb * 64, hk, j * ATT_BKV, b);
+          tma_load_4d(sK + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmK, full, nb * 64, hk, kbase + j * ATT_BKV, b);
+          tma_load_4d(sV + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmV, full, nb * 64, hk, kbase + j * ATT_BKV, b);
         }
       }
     }
@@ -199,13 +233,33 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
   float ml2 = 0.f;  // ALIBI: this head's slope in log2 units
   if constexpr (ALIBI) ml2 = __ldg(p.slopes + h) * kLog2e;
+  // CACHED: the position of each of this thread's rows (a padding row takes the last valid row's)
+  int prow[2] = {0, 0};
+  if constexpr (CACHED) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) prow[r] = c_st + min(row_a + 8 * r, c_nv - 1);
+  }
   mbar_wait(q_full, 0);
+  if constexpr (CACHED) {
+    // padding rows of Q may hold anything: zero this warpgroup's (each 128-byte row of a 64-column block is one
+    // swizzled line) before its S MMAs read them
+    const int r0 = q0 + wg * 64;
+    if (r0 + 64 > c_nv) {
+      for (int i = threadIdx.x & 127; i < Cfg::NB * 64 * 8; i += 128) {
+        const int rr = (i >> 3) & 63;
+        if (r0 + rr >= c_nv)
+          sts128(sQ + (i >> 9) * ATT_BQ * 128 + (wg * 64 + rr) * 128 + (i & 7) * 16, make_uint4(0u, 0u, 0u, 0u));
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1 + wg, 128);
+    }
+  }
 
   for (int j = j0; j < n_kv; ++j) {
     const int s = (j - j0) & 1;
     mbar_wait(kv_full0 + 8 * s, ((j - j0) >> 1) & 1);
     const uint32_t tK = sK + s * Cfg::KV_BYTES, tV = sV + s * Cfg::KV_BYTES;
-    const int k0 = j * ATT_BKV;
+    const int k0 = kbase + j * ATT_BKV;
 
     // S = Q K^T: 64 rows x 128 keys per warpgroup, both operands K-major (head dim contiguous)
     float sc[64];
@@ -236,7 +290,30 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
     // scale (log2 domain), mask, online softmax; accumulator chunk nc holds keys 8 nc + 2 (lane % 4) + {0, 1}
     float mx[2] = {-INFINITY, -INFINITY};
-    if constexpr (ALIBI) {
+    if constexpr (CACHED) {
+      // keys k_lane + c, c = 8 nc + (e & 1); ALiBi's bias m log2e (key - p) is fmaf(m log2e, c, abase[r]) as below.
+      // The rows' window starts are formed per tile: kept across the loop they push D = 128 into spills.
+      const int plo[2] = {max(0, prow[0] - p.window), max(0, prow[1] - p.window)};
+      const bool edge = k0 + ATT_BKV - 1 > prow[0] || k0 < plo[1];  // prow[0] <= prow[1]
+      const int k_lane = k0 + (lane & 3) * 2;
+      float abase[2] = {0.f, 0.f};
+      if constexpr (ALIBI) {
+#pragma unroll
+        for (int r = 0; r < 2; ++r) abase[r] = ml2 * (float)(k_lane - prow[r]);
+      }
+#pragma unroll
+      for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int c = nc * 8 + (e & 1);
+          float x = sc[4 * nc + e] * sl2;
+          if constexpr (ALIBI) x += fmaf(ml2, (float)c, abase[e >> 1]);
+          if (edge && (k_lane + c > prow[e >> 1] || k_lane + c < plo[e >> 1])) x = -INFINITY;
+          sc[4 * nc + e] = x;
+          mx[e >> 1] = fmaxf(mx[e >> 1], x);
+        }
+      }
+    } else if constexpr (ALIBI) {
       // keys k0 + 2 (lane % 4) + c with the compile-time column c = 8 nc + (e & 1): row r sees c <= c_hi[r] (causal,
       // in bounds), and its bias is fmaf(m log2e, c, abase[r]) with abase[r] = m log2e (k0 + 2 (lane % 4) - row)
       const int k_lane = k0 + (lane & 3) * 2;
@@ -368,15 +445,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     for (int dc = 0; dc < D / 8; ++dc)
       *reinterpret_cast<uint32_t*>(orow + dc * 8 + (lane & 3) * 2) =
           pack_bf16x2(o[4 * dc + 2 * r] * inv[r], o[4 * dc + 2 * r + 1] * inv[r]);
-    if ((lane & 3) == 0) p.lse[((long long)b * p.H + h) * p.S + row] = (m_r[r] + log2f(l_r[r])) / kLog2e;
+    if ((lane & 3) == 0 && (!CACHED || p.lse != nullptr))
+      p.lse[((long long)b * p.H + h) * p.S + row] = (m_r[r] + log2f(l_r[r])) / kLog2e;
   }
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false, bool CACHED = false>
 int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
                cudaStream_t stream) {
   using Cfg = FwdCfg<D>;
-  auto kern = attn_fwd_kernel<D, DOC, ALIBI, PREFIX, DROP>;
+  auto kern = attn_fwd_kernel<D, DOC, ALIBI, PREFIX, DROP, CACHED>;
   static bool attr_set = false;
   if (!attr_set) {
     B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -431,6 +509,8 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   a.drop_t = drop_t;
   a.drop_inv = drop_inv;
   a.drop_seed = drop_seed;
+  a.start = a.end = nullptr;
+  a.s_max = 0;
   if (drop) {
     if (slopes)
       return D == 64 ? launch_fwd<64, true, true, false, true>(tmQ, tmK, tmV, a, stream)
@@ -513,6 +593,48 @@ int b200_attn_fwd_dropout(const void* q, const void* k, const void* v, void* o, 
   const uint32_t t = dropout_threshold(p);
   return attn_fwd_impl(q, k, v, o, lse, doc, pos, window, B, S, H, Hk, D, scale, doc ? 1 : causal, s, slopes,
                        nullptr, true, t, dropout_scale(t), seed);
+}
+
+// cached queries: query i of row b sits at position start[b] + i and sees cached key k iff
+// max(0, p - window) <= k <= p for i < end[b] - start[b]; the later rows are padding (finite, unspecified)
+int b200_attn_fwd_cached(const void* q, const void* k_cache, const void* v_cache, const int* start, const int* end,
+                         void* o, float* lse, int window, const float* slopes, int B, int L, int s_max, int H, int Hk,
+                         int D, float scale, void* stream) {
+  B200_CHECK_ARG(B > 0 && L > 0 && s_max > 0 && H > 0 && Hk > 0 && H % Hk == 0,
+                 "attn_fwd_cached: bad shape B=%d L=%d s_max=%d H=%d Hk=%d", B, L, s_max, H, Hk);
+  B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd_cached: head_dim %d unsupported (64 or 128)", D);
+  B200_CHECK_ARG(start != nullptr && end != nullptr && (reinterpret_cast<uintptr_t>(start) & 3u) == 0 &&
+                     (reinterpret_cast<uintptr_t>(end) & 3u) == 0,
+                 "attn_fwd_cached: start and end must be non-null, 4-byte aligned int32 [B] arrays");
+  B200_CHECK_ARG(al16(q) && al16(k_cache) && al16(v_cache) && al16(o),
+                 "attn_fwd_cached: q, k_cache, v_cache and o must be 16-byte aligned");
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0 && (reinterpret_cast<uintptr_t>(lse) & 3u) == 0,
+                 "attn_fwd_cached: slopes and lse must be 4-byte aligned");
+  CUtensorMap tmQ, tmK, tmV;
+  int rc;
+  if ((rc = make_bshd_map(&tmQ, q, B, L, H, D, ATT_BQ))) return rc;
+  if ((rc = make_bshd_map(&tmK, k_cache, B, s_max, Hk, D, ATT_BKV))) return rc;
+  if ((rc = make_bshd_map(&tmV, v_cache, B, s_max, Hk, D, ATT_BKV))) return rc;
+  FwdArgs a{};
+  a.o = reinterpret_cast<__nv_bfloat16*>(o);
+  a.lse = lse;
+  a.B = B;
+  a.S = L;
+  a.H = H;
+  a.Hk = Hk;
+  a.scale = scale;
+  a.causal = 1;
+  a.window = window < 0 || window > s_max ? s_max : window;
+  a.slopes = slopes;
+  a.start = start;
+  a.end = end;
+  a.s_max = s_max;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (slopes)
+    return D == 64 ? launch_fwd<64, false, true, false, false, true>(tmQ, tmK, tmV, a, s)
+                   : launch_fwd<128, false, true, false, false, true>(tmQ, tmK, tmV, a, s);
+  return D == 64 ? launch_fwd<64, false, false, false, false, true>(tmQ, tmK, tmV, a, s)
+                 : launch_fwd<128, false, false, false, false, true>(tmQ, tmK, tmV, a, s);
 }
 
 }  // extern "C"

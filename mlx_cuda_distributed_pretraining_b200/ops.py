@@ -1106,6 +1106,58 @@ def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.
                                _stream()), "b200_kv_append")
 
 
+def _check_rows(t, B: int, device, what: str, nm: str) -> None:
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or tuple(t.shape) != (B,) or t.device != device \
+            or not t.is_contiguous():
+        raise ValueError(f"{what}: {nm} must be a contiguous int32 [{B}] tensor on {device}, got "
+                         f"{getattr(t, 'dtype', type(t))} {list(getattr(t, 'shape', []))}")
+
+
+def attention_cached(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, start: torch.Tensor,
+                     end: torch.Tensor, scale: Optional[float] = None, window: Optional[int] = None,
+                     alibi: Optional[torch.Tensor] = None, return_lse: bool = False):
+    """A chunk of L new queries per row against the KV cache that already holds their keys (b200_attn_fwd_cached).
+
+    q [B,L,H,D]; k_cache, v_cache [B,s_max,Hk,D]; all bf16, D in {64, 128}.  start, end: int32 [B] on the device.
+    Query i of row b sits at position start[b] + i and sees the cached keys max(0, p - window) .. p (window None: from
+    0), with ALiBi's bias alibi[h] * (k - p) when alibi (fp32 [H] slopes) is given.  Rows i >= end[b] - start[b] are
+    padding: finite, unspecified.  Cache positions at or past end[b] are never read into the result.  The values of
+    start and end are not checked here (that would read the device): 0 <= start[b] <= end[b] <= s_max.  Returns o
+    [B,L,H,D] bf16, and the natural-log LSE [B,H,L] fp32 with return_lse."""
+    what = "attention_cached"
+    for t, nm in ((q, "q"), (k_cache, "k_cache"), (v_cache, "v_cache")):
+        if t.dtype != torch.bfloat16:
+            raise ValueError(f"{what}: {nm} must be bf16 (an fp32 cache is served by the one-shot prefill only), "
+                             f"got {t.dtype}")
+        _need(t, torch.bfloat16, f"{what}: {nm}")
+    if q.dim() != 4 or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
+        raise ValueError(f"{what}: expected q [B,L,H,D] and k_cache == v_cache [B,s_max,Hk,D], got "
+                         f"{tuple(q.shape)}, {tuple(k_cache.shape)}, {tuple(v_cache.shape)}")
+    B, L, H, D = q.shape
+    Bc, s_max, Hk, Dc = k_cache.shape
+    if Bc != B or Dc != D or H % Hk != 0:
+        raise ValueError(f"{what}: q {tuple(q.shape)} does not match cache {tuple(k_cache.shape)}")
+    if D not in (64, 128):
+        raise ValueError(f"{what}: head_dim {D} unsupported (64 or 128)")
+    _check_rows(start, B, q.device, what, "start")
+    _check_rows(end, B, q.device, what, "end")
+    if window is not None:
+        window = _check_window(window, what)
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, True, what)
+    if scale is None:
+        scale = D ** -0.5
+    o = torch.empty_like(q)
+    lse = torch.empty((B, H, L), device=q.device, dtype=torch.float32) if return_lse else None
+    tok = _t0("attn_cached")
+    check(lib().b200_attn_fwd_cached(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), start.data_ptr(),
+                                     end.data_ptr(), o.data_ptr(), _ptr(lse),
+                                     -1 if window is None else min(int(window), s_max), _ptr(alibi), B, L, s_max, H,
+                                     Hk, D, float(scale), _stream()), "b200_attn_fwd_cached")
+    _t1(tok)
+    return (o, lse) if return_lse else o
+
+
 # ------------------------------------------------------------------------------------------------
 # the quantized KV cache (the reference's kv_bits / kv_group_size; DESIGN §4.2.1): per layer, codes uint8
 # [B, s_max, Hk, D * bits / 8] and parameters fp32 [B, Hk, s_max, D / group_size, 2] for each of K and V
@@ -1175,6 +1227,40 @@ def kv_quantize(k: torch.Tensor, v: torch.Tensor, k_codes: torch.Tensor, v_codes
     check(lib().b200_kv_quantize(k.data_ptr(), v.data_ptr(), n, S, k_codes.data_ptr(), v_codes.data_ptr(),
                                  k_params.data_ptr(), v_params.data_ptr(), B, s_max, Hk, D, bits, group_size,
                                  _is_bf16(k, "k"), _stream()), "b200_kv_quantize")
+
+
+def kv_dequantize(k_codes: torch.Tensor, v_codes: torch.Tensor, k_params: torch.Tensor, v_params: torch.Tensor,
+                  end: torch.Tensor, bits: int, group_size: int, out: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                  S: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Positions [0, end[b]) of row b of a quantized cache as bf16 k, v [B, S, Hk, D] (b200_kv_dequantize): s q + b in
+    fp32, rounded once to bf16.  out: bf16 [B, S, Hk, D] buffers to write (else allocated with S positions, default
+    s_max).  Positions at or past end[b] are not written."""
+    what = "kv_dequantize"
+    if k_codes.dim() != 4:
+        raise ValueError(f"{what}: k_codes must be [B, s_max, Hk, D * bits / 8], got {tuple(k_codes.shape)}")
+    B, _, Hk, Dc = k_codes.shape
+    check_kv_quant(bits, group_size, what=what)
+    D = Dc * 8 // bits
+    s_max = _check_quant_cache(k_codes, v_codes, k_params, v_params, B, Hk, D, bits, group_size, k_codes.device, what)
+    _check_rows(end, B, k_codes.device, what, "end")
+    if out is None:
+        S = s_max if S is None else S
+        if isinstance(S, bool) or not isinstance(S, int) or not 1 <= S <= s_max:
+            raise ValueError(f"{what}: S must be an int in [1, {s_max}], got {S!r}")
+        shape = (B, S, Hk, D)
+        out = (torch.empty(shape, device=k_codes.device, dtype=torch.bfloat16),
+               torch.empty(shape, device=k_codes.device, dtype=torch.bfloat16))
+    k, v = out
+    for t, nm in ((k, "k"), (v, "v")):
+        _need(t, torch.bfloat16, f"{what}: {nm}")
+        if t.dim() != 4 or t.shape[0] != B or t.shape[2:] != (Hk, D) or not 1 <= t.shape[1] <= s_max \
+                or t.shape != k.shape or t.data_ptr() % 16:
+            raise ValueError(f"{what}: {nm} must be a 16-byte aligned bf16 [{B}, S <= {s_max}, {Hk}, {D}] tensor, "
+                             f"got {tuple(t.shape)}")
+    check(lib().b200_kv_dequantize(k_codes.data_ptr(), v_codes.data_ptr(), k_params.data_ptr(), v_params.data_ptr(),
+                                   end.data_ptr(), k.data_ptr(), v.data_ptr(), k.shape[1], B, s_max, Hk, D, bits,
+                                   group_size, _stream()), "b200_kv_dequantize")
+    return k, v
 
 
 def kv_append_quant(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_codes: torch.Tensor, v_codes: torch.Tensor,
