@@ -515,6 +515,37 @@ int b200_attn_decode_quant(const void* q, const void* k_codes, const void* v_cod
                            const float* slopes, int B, int s_max, int H, int Hk, int D, int bits, int group_size,
                            float scale, int is_bf16, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- rotating KV cache (the reference's max_kv_size, core/generation_lite.py:103, :120) ----------------------
+ * Each row keeps C slots, k_ring / v_ring bf16 [B, C, Hk, D].  Slot map: position t lives in slot
+ *     slot(t) = t                        for t < 4 (the sinks)
+ *     slot(t) = 4 + (t - 4) mod (C - 4)  otherwise.
+ * With M = max_kv_size (>= 5), query position q sees key position k iff
+ *     k <= q  and  (k < 4  or  q - k <= M - 5)  [and q - k <= window]
+ * and ALiBi's bias slopes[h] * (k - q) uses true positions.  end[b] is the number of positions row b holds; a slot
+ * whose position under the map was never written (slot >= end[b] before the first wrap) is never read into a result.
+ * C >= M (decode) or C >= M + L - 1 (a chunk of L queries), so no key a query sees has been overwritten.
+ *
+ * b200_attn_decode_ring: b200_attn_decode_alibi over a ring (window < 0: none, slopes NULL: no ALiBi), the query at
+ *   position end[b] - 1.  The visible slots are at most three ranges (the sinks and one arc, which may wrap); 256-slot
+ *   chunks holding none are not read.  Chunk boundaries and merge order depend on (end[b], M, C, window) alone, so a
+ *   row's output is bit-identical alone or in any batch.  Workspace: b200_attn_decode_workspace_bytes(B, H, C, D). */
+int b200_attn_decode_ring(const void* q, const void* k_ring, const void* v_ring, const int* end, void* o, float* lse,
+                          int max_kv, int window, const float* slopes, int B, int C, int H, int Hk, int D, float scale,
+                          void* workspace, size_t workspace_bytes, void* stream);
+/* b200_attn_fwd_cached over a ring: query i < end[b] - start[b] of row b sits at position start[b] + i, the ring
+ *   already holding the chunk's keys; later query rows are padding (finite, unspecified).  Masking follows the rule
+ *   above.  One CTA per (128 queries, head, row), no split over keys: a row is bit-identical alone or in any batch.
+ *   Key tiles with no visible key are skipped: a sink tile plus the arc, about M + 128 keys per query tile. */
+int b200_attn_fwd_ring(const void* q, const void* k_ring, const void* v_ring, const int* start, const int* end,
+                       void* o, float* lse, int max_kv, int window, const float* slopes, int B, int L, int C, int H,
+                       int Hk, int D, float scale, void* stream);
+/* b200_kv_append (half == 0) or b200_kv_append_half (half != 0, tables required) into a ring: q and k rotated by
+ *   position end[b] - 1 with those kernels' own statements, k and v written to slot(end[b] - 1).  live: device int32
+ *   [B] or NULL (all live); a row with live[b] == 0 writes nothing, q included. */
+int b200_kv_append_ring(void* q, const void* k, const void* v, void* k_ring, void* v_ring, const int* end,
+                        const int* live, const float* cos_t, const float* sin_t, int half, int B, int C, int H,
+                        int Hk, int D, void* stream);
+
 /* ---- mixture-of-experts MLP (Mixtral's sparse MoE block, model.misc.num_local_experts) -------------------------
  * T tokens, E experts (2..64), k experts per token (1..min(E, 8)), hidden H, per-expert intermediate I (H, I % 8 == 0).
  * Everything stays on the device and nothing uses atomics: the same inputs give the same bits on every run.

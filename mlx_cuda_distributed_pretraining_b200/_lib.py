@@ -109,6 +109,9 @@ SIGNATURES = {
                                   _i, _vp]),
     "b200_attn_fwd_cached": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
     "b200_kv_dequantize": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "b200_attn_decode_ring": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _f, _vp, _sz, _vp]),
+    "b200_attn_fwd_ring": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _vp]),
+    "b200_kv_append_ring": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_attn_decode_quant": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _f,
                                     _i, _vp, _sz, _vp]),
     "b200_moe_route_workspace_bytes": (_sz, [_i, _i, _i]),

@@ -125,6 +125,15 @@ class QuantizedKV:
         return sum(t.numel() * t.element_size() for t in self.buffers())
 
 
+class RingKV:
+    """One layer's rotating KV cache (mlx_lm's RotatingKVCache; DESIGN §4.2.3): K and V rings bf16 [B, C, Hk, D],
+    position t in slot ops.ring_slot(t, C), read under max_kv_size.  live: the cache's int32 [B] mask of rows a decode
+    step appends to (None: all)."""
+
+    def __init__(self, k: torch.Tensor, v: torch.Tensor, max_kv_size: int, live: Optional[torch.Tensor] = None):
+        self.k, self.v, self.max_kv_size, self.live = k, v, max_kv_size, live
+
+
 class FlashAttention(nn.Module):
     """alibi: add ALiBi's bias alibi_slopes(num_heads)[h] * (k - q) to every causal score (the slopes are not
     parameters: a device tensor made on first use, like rope_tables).  dropout: the probability p of dropping an
@@ -267,6 +276,11 @@ class FlashAttention(nn.Module):
         q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
         k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
+        if isinstance(k_cache, RingKV):
+            ops.kv_append_ring(q, k, v, k_cache.k, k_cache.v, lens, k_cache.live, self.rope_tables, rope_layout)
+            ctx = ops.attention_decode_ring(q, k_cache.k, k_cache.v, lens, k_cache.max_kv_size, self.scale, workspace,
+                                            window=window, alibi=self.alibi_slopes(q.device))
+            return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
         if isinstance(k_cache, QuantizedKV):
             bits, g = k_cache.bits, k_cache.group_size
             ops.kv_append_quant(q, k, v, *k_cache.buffers(), lens, bits, g, self.rope_tables, layout=rope_layout)
@@ -285,7 +299,8 @@ class FlashAttention(nn.Module):
         and k are rotated there (ops.rope at absolute positions), its k and v are written to that cache position
         (quantized first when k_cache is a QuantizedKV, v_cache None), and its query attends over the row's cached
         keys max(0, p - window) .. p (ops.attention_cached), over the cache's dequantised values once it is
-        quantized."""
+        quantized.  For a RingKV (v_cache None) chunk.dst are ring slots and the keys are those of
+        ops.attention_ring."""
         B, L, _ = x.shape
         q, k, v = self._project(x)
         q = q.reshape(B, L, self.num_heads, self.head_dim)
@@ -297,6 +312,12 @@ class FlashAttention(nn.Module):
             k = ops.rope(k, cos_t, sin_t, chunk.pos, rope_layout)
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
         r, src, dst = chunk.rows, chunk.src, chunk.dst
+        if isinstance(k_cache, RingKV):
+            k_cache.k[r, dst] = k[r, src]
+            k_cache.v[r, dst] = v[r, src]
+            ctx = ops.attention_ring(q, k_cache.k, k_cache.v, chunk.start, chunk.end, k_cache.max_kv_size, self.scale,
+                                     window=window, alibi=self.alibi_slopes(q.device))
+            return self._out(ctx.reshape(B, L, self.num_heads * self.head_dim))
         if isinstance(k_cache, QuantizedKV):
             bits, g = k_cache.bits, k_cache.group_size
             tmp = QuantizedKV(B, L + L % 2, self.num_kv_heads, self.head_dim, bits, g, x.device)

@@ -26,7 +26,7 @@ import torch
 from torch import nn
 
 from .. import ops
-from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask, QuantizedKV
+from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask, QuantizedKV, RingKV
 
 VARIANTS = (None, "reference", "mlx_lm")
 
@@ -257,12 +257,42 @@ class KVCache:
     after prefill or after a decode step, every layer converts to a QuantizedKV and the unquantized buffers are
     released.  When the prompt already passes the start, prefill writes the quantized cache directly and no
     unquantized buffer is ever allocated; otherwise those buffers hold quantized_kv_start + 1 positions (rounded up to
-    256), all they can hold before conversion.  The buffers are allocated by the first set_lengths (prefill)."""
+    256), all they can hold before conversion.  The buffers are allocated by the first set_lengths (prefill).
+
+    max_kv_size = M (an int >= 5) makes the cache rotate, as the reference's make_prompt_cache(model, max_kv_size)
+    (core/generation_lite.py:103, :120) gives every layer mlx_lm's RotatingKVCache(max_size=M, keep=4): each row keeps
+    C = M + max_chunk - 1 slots (rounded up to 256; s_max is then C), position t in slot ops.ring_slot(t, C), and a
+    query at position q sees key k iff k <= q and (k < 4 or q - k <= M - 5) (DESIGN §2).  A row's length is then
+    unbounded.  max_chunk (default 512) is the longest chunk Model.extend may append; the cache is filled by
+    Model.extend only, cannot be truncated (overwritten slots cannot be restored) and is bf16 with head_dim 64 or
+    128, not quantized and not for prefix-LM models."""
+
+    max_kv_size: Optional[int] = None
+    max_chunk: Optional[int] = None
+    live: Optional[torch.Tensor] = None  # rotating: the rows the current decode step appends to (None: all)
+    _rings = None  # rotating: the layers' RingKV views
 
     def __init__(self, model: "Model", batch: int, s_max: int, kv_bits: Optional[int] = None,
-                 kv_group_size: int = 64, quantized_kv_start: int = 0):
+                 kv_group_size: int = 64, quantized_kv_start: int = 0, max_kv_size: Optional[int] = None,
+                 max_chunk: Optional[int] = None):
         a = model.args
         attn = model.layers[0].self_attn
+        self.max_kv_size = max_kv_size
+        self.max_chunk = max_chunk
+        if max_kv_size is not None:
+            ops.check_max_kv_size(max_kv_size, "KVCache")
+            if kv_bits is not None:
+                raise ValueError("KVCache: max_kv_size does not combine with kv_bits (mlx_lm's rotating cache does "
+                                 "not quantize)")
+            if a.prefix_lm:
+                raise ValueError("KVCache: a prefix-LM model cannot use a rotating cache (its prompt is one prefix)")
+            model.check_extend(None)
+            self.max_chunk = 512 if max_chunk is None else max_chunk
+            if isinstance(self.max_chunk, bool) or not isinstance(self.max_chunk, int) or self.max_chunk < 1:
+                raise ValueError(f"KVCache: max_chunk must be an int >= 1, got {max_chunk!r}")
+            s_max = max_kv_size + self.max_chunk - 1
+        elif max_chunk is not None:
+            raise ValueError("KVCache: max_chunk is for a rotating cache (max_kv_size)")
         if kv_bits is not None:
             ops.check_kv_quant(kv_bits, kv_group_size, attn.head_dim, "KVCache")
             if isinstance(quantized_kv_start, bool) or not isinstance(quantized_kv_start, int) \
@@ -295,11 +325,23 @@ class KVCache:
     def quantized(self) -> bool:
         return self.quant is not None
 
+    @property
+    def rotating(self) -> bool:
+        return self.max_kv_size is not None
+
     def layer(self, i: int):
-        """(k, v) buffers of layer i, or (QuantizedKV, None) once the cache is quantized."""
+        """(k, v) buffers of layer i, (QuantizedKV, None) once the cache is quantized, or (RingKV, None) when it
+        rotates."""
+        if self.rotating:
+            if self._rings is None:  # made once: a decode step calls layer() for every layer
+                self._rings = [RingKV(k, v, self.max_kv_size) for k, v in zip(self.k, self.v)]
+            self._rings[i].live = self.live
+            return self._rings[i], None
         return (self.quant[i], None) if self.quant is not None else (self.k[i], self.v[i])
 
     def set_lengths(self, lengths) -> None:
+        if self.rotating:
+            raise ValueError("a rotating KV cache is filled in chunks by Model.extend, not by Model.prefill")
         if any(n < 1 or n > self.s_max for n in lengths):
             raise ValueError(f"lengths must lie in [1, {self.s_max}], got {list(lengths)}")
         self.host_lens = [int(n) for n in lengths]
@@ -319,9 +361,12 @@ class KVCache:
         if len(counts) != self._batch or any(n < 0 for n in counts):
             raise ValueError(f"counts must be {self._batch} non-negative ints, got {counts}")
         ends = [n + c for n, c in zip(self.host_lens, counts)]
-        if max(ends) > self.s_max:
+        if self.rotating and max(counts) > self.max_chunk:
+            raise ValueError(f"a chunk of {max(counts)} tokens exceeds the rotating cache's max_chunk "
+                             f"({self.max_chunk}): its keys would overwrite keys its queries see")
+        if not self.rotating and max(ends) > self.s_max:
             raise ValueError(f"KV cache full: rows would hold {max(ends)} positions, the cache has {self.s_max}")
-        if self.quant is None:
+        if self.quant is None and not self.rotating:  # a ring is allocated whole by __init__
             have = 0 if self.k is None else self.k[0].shape[1]
             if max(ends) > have:
                 old_k, old_v = self.k, self.v
@@ -335,18 +380,33 @@ class KVCache:
 
     def truncate(self, lengths) -> None:
         """Shortens row b to lengths[b] <= its current length: later positions are left as they are and never read."""
+        if self.rotating:
+            raise ValueError("a rotating KV cache cannot be truncated: the slots of dropped positions may hold keys "
+                             "that are already overwritten")
         lengths = [int(n) for n in lengths]
         if len(lengths) != self._batch or any(not 0 <= n <= m for n, m in zip(lengths, self.host_lens)):
             raise ValueError(f"truncate: lengths must lie in [0, current lengths {self.host_lens}], got {lengths}")
         self.host_lens = lengths
         self.lens.copy_(torch.tensor(lengths, dtype=torch.int32))
 
-    def advance(self) -> None:
-        """One more position per row (the token a decode step is about to append)."""
-        if max(self.host_lens) + 1 > self.s_max:
+    def advance(self, live=None) -> None:
+        """One more position per row (the token a decode step is about to append).  live (rotating caches; a bool
+        per row): only those rows advance, and the decode step writes nothing into the others (self.live)."""
+        if live is not None:
+            if not self.rotating:
+                raise ValueError("advance: live is for a rotating cache (an unbounded one is truncated instead)")
+            live = [bool(x) for x in live]
+            if len(live) != self._batch:
+                raise ValueError(f"advance: live must have {self._batch} entries, got {len(live)}")
+            self.host_lens = [n + int(x) for n, x in zip(self.host_lens, live)]
+            self.live = torch.tensor(live, dtype=torch.int32).to(self._device)
+            self.lens.add_(self.live)
+            return
+        if not self.rotating and max(self.host_lens) + 1 > self.s_max:
             raise ValueError(f"KV cache full ({self.s_max} positions)")
         self.host_lens = [n + 1 for n in self.host_lens]
         self.lens.add_(1)
+        self.live = None
 
     def maybe_quantize(self) -> None:
         """maybe_quantize_kv_cache (core/generation_lite.py:75-90): with kv_bits, the first time the longest row
@@ -371,9 +431,10 @@ class CacheChunk:
     [B, L] go to cache positions start[b] + i.  start / end: int32 [B] on the device (the lengths before and after);
     pos: int32 [B, L] rotation positions (padding tokens take their row's last position, so that no rotation reads
     past the tables); rows / src / dst: int64 indices of the valid tokens (row, index in the chunk, cache position);
-    scratch: a quantized cache's bf16 K / V for the call, made by its first layer."""
+    scratch: a quantized cache's bf16 K / V for the call, made by its first layer.  slots (a rotating cache's C): dst
+    are the ring slots ops.ring_slot(start[b] + i, C)."""
 
-    def __init__(self, start, counts, L: int, device):
+    def __init__(self, start, counts, L: int, device, slots: Optional[int] = None):
         ends = [a + n for a, n in zip(start, counts)]
         self.start = torch.tensor(start, dtype=torch.int32).to(device)
         self.end = torch.tensor(ends, dtype=torch.int32).to(device)
@@ -382,7 +443,10 @@ class CacheChunk:
         src = [i for n in counts for i in range(n)]
         self.rows = torch.tensor(rows, dtype=torch.int64).to(device)
         self.src = torch.tensor(src, dtype=torch.int64).to(device)
-        self.dst = torch.tensor([start[b] + i for b, i in zip(rows, src)], dtype=torch.int64).to(device)
+        dst = [start[b] + i for b, i in zip(rows, src)]
+        if slots is not None:
+            dst = [ops.ring_slot(t, slots) for t in dst]
+        self.dst = torch.tensor(dst, dtype=torch.int64).to(device)
         last = torch.tensor([max(e - 1, 0) for e in ends], dtype=torch.int64)
         pos = torch.minimum(torch.tensor(start, dtype=torch.int64)[:, None] + torch.arange(L)[None], last[:, None])
         self.pos = pos.to(torch.int32).to(device)
@@ -556,7 +620,7 @@ class Model(nn.Module):
             raise ValueError(f"lengths must be {B} ints in [0, {L}], at least one positive, got {counts}")
         self.check_extend(cache, counts)
         cache.extend_lengths(counts)
-        chunk = CacheChunk(cache.host_start, counts, L, tokens.device)
+        chunk = CacheChunk(cache.host_start, counts, L, tokens.device, cache.s_max if cache.rotating else None)
         h = ops.embedding(tokens, self.embed_tokens.weight)
         pending = None
         for i, layer in enumerate(self.layers):
@@ -567,10 +631,11 @@ class Model(nn.Module):
         return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])
 
     @torch.no_grad()
-    def decode_step(self, tokens: torch.Tensor, cache: KVCache) -> torch.Tensor:
+    def decode_step(self, tokens: torch.Tensor, cache: KVCache, live=None) -> torch.Tensor:
         """Appends one token per row (tokens [B]) at position cache.host_lens[b] and returns the fp32 logits [B, V]
-        that follow it."""
-        cache.advance()
+        that follow it.  live (a rotating cache only; a bool per row): rows with False neither advance nor write, and
+        their logits are unspecified."""
+        cache.advance(live)
         h = ops.embedding(tokens, self.embed_tokens.weight)
         pending = None
         for i, layer in enumerate(self.layers):

@@ -135,7 +135,7 @@ def prefill_chunks(prompts: Sequence[Sequence[int]], step: int) -> List[List[Lis
 def _prefill(model, prompts: List[List[int]], cache, step: Optional[int]) -> torch.Tensor:
     """The fp32 logits [B, V] after each prompt's last token, the prompts appended to what the cache holds: in chunks
     of `step` tokens (None: one chunk), each through Model.extend, except that the first chunk of an empty cache goes
-    through Model.prefill.  A row's logits come from the chunk that holds its last token."""
+    through Model.prefill unless the cache rotates.  A row's logits come from the chunk that holds its last token."""
     device = model.embed_tokens.weight.device
     empty = all(n == 0 for n in cache.host_lens)
     logits = None
@@ -144,7 +144,7 @@ def _prefill(model, prompts: List[List[int]], cache, step: Optional[int]) -> tor
         tokens = torch.zeros((len(chunk), max(counts)), dtype=torch.int64)
         for b, t in enumerate(chunk):
             tokens[b, :len(t)] = torch.tensor(t, dtype=torch.int64)
-        run = model.prefill if empty and c == 0 else model.extend
+        run = model.prefill if empty and c == 0 and not cache.rotating else model.extend
         lg = run(tokens.to(device), counts, cache)
         if logits is None:
             logits = lg
@@ -159,7 +159,7 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
              repetition_context_size: int = 20, eos_token: Optional[int] = None, seed: Optional[int] = None,
              on_step: Optional[Callable[[List[int]], None]] = None, kv_bits: Optional[int] = None,
              kv_group_size: int = 64, quantized_kv_start: int = 0, prefill_step_size: Optional[int] = None,
-             prompt_cache=None) -> List[List[int]]:
+             prompt_cache=None, max_kv_size: Optional[int] = None) -> List[List[int]]:
     """Generates up to max_tokens tokens for each of the ragged prompts in one batch.  A row stops at EOS, which is
     included in its output.  Returns the generated tokens per row (prompt excluded).  Per step, the sampled tokens
     are the one value read back from the device.  kv_bits (4 or 8; None: no quantization), kv_group_size and
@@ -170,7 +170,14 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     B x prompt.  prompt_cache: a KVCache of batch len(prompts) that the caller built and keeps (its kv settings
     apply; a different kv_bits is an error).  The prompts are appended to what it holds, and it is updated in place
     so that it ends holding prompt + output of every row, ready for the next turn.  Without both, the prompts go
-    through Model.prefill in one piece."""
+    through Model.prefill in one piece.
+
+    max_kv_size (an int >= 5): a rotating KV cache (arch.llama.KVCache(max_kv_size=...)), as the reference's
+    make_prompt_cache(model, max_kv_size) (core/generation_lite.py:103, :120): each query sees the first 4 positions
+    of its row and its most recent max_kv_size - 4, and the cache holds a constant number of slots whatever the
+    length.  The prompts then always go through Model.extend, in chunks of prefill_step_size (default 512).  A
+    rotating prompt_cache brings its own max_kv_size (a different one is an error).  A row that stops at EOS neither
+    advances nor writes afterwards, as a ring cannot be truncated."""
     from .. import ops
     from ..arch.llama import KVCache
 
@@ -179,9 +186,23 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     if prefill_step_size is not None and (isinstance(prefill_step_size, bool) or not isinstance(prefill_step_size, int)
                                           or prefill_step_size < 1):
         raise ValueError(f"generate: prefill_step_size must be None or an int >= 1, got {prefill_step_size!r}")
+    if max_kv_size is not None:
+        ops.check_max_kv_size(max_kv_size, "generate")
+        if kv_bits is not None:
+            raise ValueError("generate: max_kv_size does not combine with kv_bits (mlx_lm's rotating cache does not "
+                             "quantize)")
+        if model.args.prefix_lm:
+            raise ValueError("generate: a prefix-LM model cannot use a rotating cache (max_kv_size)")
+        model.check_extend(None)
     if prompt_cache is not None:
         if not isinstance(prompt_cache, KVCache):
             raise ValueError(f"generate: prompt_cache must be an arch.llama.KVCache, got {type(prompt_cache).__name__}")
+        if max_kv_size is not None and max_kv_size != prompt_cache.max_kv_size:
+            raise ValueError(f"generate: max_kv_size={max_kv_size!r} conflicts with the prompt_cache's max_kv_size "
+                             f"{prompt_cache.max_kv_size!r} (the cache's settings apply)")
+        if prompt_cache.rotating and prefill_step_size is not None and prefill_step_size > prompt_cache.max_chunk:
+            raise ValueError(f"generate: prefill_step_size {prefill_step_size} exceeds the rotating prompt_cache's "
+                             f"max_chunk {prompt_cache.max_chunk}")
         if kv_bits is not None and kv_bits != prompt_cache.kv_bits:
             raise ValueError(f"generate: kv_bits={kv_bits!r} conflicts with the prompt_cache's kv_bits "
                              f"{prompt_cache.kv_bits!r} (the cache's settings apply)")
@@ -198,7 +219,10 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     if limit is not None and reach > limit:
         raise ValueError(f"cached ({max(start)}) + prompt ({longest} tokens) + max_tokens ({max_tokens}) exceeds "
                          f"max_position_embeddings ({limit}): training truncates there and the RoPE tables end there")
-    if prompt_cache is not None and reach > prompt_cache.s_max:
+    rotating = max_kv_size is not None or (prompt_cache is not None and prompt_cache.rotating)
+    if rotating and prefill_step_size is None:
+        prefill_step_size = 512 if prompt_cache is None else min(512, prompt_cache.max_chunk)
+    if prompt_cache is not None and not rotating and reach > prompt_cache.s_max:
         raise ValueError(f"generate: prompt_cache holds {prompt_cache.s_max} positions, {reach} needed (cached + prompt "
                          f"+ max_tokens)")
     chunked = prefill_step_size is not None or any(start)
@@ -218,7 +242,9 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     for b, p in enumerate(prompts):
         tokens[b, :len(p)] = torch.tensor(p, dtype=torch.int64)
     cache = prompt_cache
-    if cache is None:
+    if cache is None and rotating:
+        cache = KVCache(model, B, longest + max_tokens, max_kv_size=max_kv_size, max_chunk=prefill_step_size)
+    elif cache is None:
         cache = KVCache(model, B, longest + max_tokens, kv_bits, kv_group_size, quantized_kv_start)
     if chunked:
         logits = _prefill(model, prompts, cache, prefill_step_size)
@@ -227,12 +253,15 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     history = [list(p) for p in prompts]
     out: List[List[int]] = [[] for _ in prompts]
     done = [False] * B
+    live = None  # rotating: the rows that took a token this step (the others must not write into the ring)
     for step in range(max_tokens):
         if repetition_penalty != 1.0 and repetition_context_size > 0:
             logits = apply_repetition_penalty(logits, [repetition_window(h, repetition_context_size) for h in history],
                                               repetition_penalty)
         nxt = sample(logits, temperature, min_p, top_p, gen)
         picked = nxt.tolist()
+        if rotating:
+            live = None if not any(done) else [not d for d in done]
         for b, t in enumerate(picked):
             if done[b]:
                 continue
@@ -244,8 +273,12 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
             on_step(picked)
         if all(done) or step + 1 == max_tokens:
             break
-        logits = model.decode_step(nxt, cache)
-    if prompt_cache is not None:
+        logits = model.decode_step(nxt, cache, live)
+    if prompt_cache is not None and rotating:
+        # the last tokens, fed only to the rows that took one: the ring then holds prompt + output of every row
+        if max_tokens > 0:
+            model.decode_step(nxt, cache, live)
+    elif prompt_cache is not None:
         # the reference feeds every token it yields: feed the last ones, then drop what finished rows were fed past EOS
         if max_tokens > 0:
             model.decode_step(nxt, cache)
@@ -279,6 +312,9 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
                     help="Quantize the KV cache once it holds more than this many tokens")
     ap.add_argument("--prefill-step-size", type=int, default=None,
                     help="Prefill the prompt in chunks of this many tokens (default: the whole prompt at once)")
+    ap.add_argument("--max-kv-size", type=int, default=None,
+                    help="Keep a rotating KV cache: each token attends to the first 4 and the most recent "
+                         "max-kv-size - 4 tokens (default: an unbounded cache)")
     a = ap.parse_args(argv)
     if a.num_samples < 1:
         ap.error("--num-samples must be >= 1")
@@ -286,6 +322,8 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
         ap.error("--quantized-kv-start must be >= 0")
     if a.prefill_step_size is not None and a.prefill_step_size < 1:
         ap.error("--prefill-step-size must be >= 1")
+    if a.max_kv_size is not None and a.max_kv_size < 5:
+        ap.error("--max-kv-size must be >= 5")
     return a
 
 
@@ -343,7 +381,7 @@ def main(argv: Optional[List[str]] = None) -> None:
                     min_p=a.min_p, top_p=a.top_p, repetition_penalty=a.repetition_penalty,
                     repetition_context_size=a.repetition_context_size, eos_token=tok.EOS_TOKEN, seed=seed,
                     kv_bits=a.kv_bits, kv_group_size=a.kv_group_size, quantized_kv_start=a.quantized_kv_start,
-                    prefill_step_size=a.prefill_step_size)
+                    prefill_step_size=a.prefill_step_size, max_kv_size=a.max_kv_size)
     for o in outs:
         print(f"Greedy Output: {tok.detokenize(o)}")
     sys.stdout.flush()

@@ -96,28 +96,115 @@ struct DecArgs {
   float scale_log2;   // scale * log2 e
   int window;         // keys len - 1 - window .. len - 1 are visible; s_max without a window
   const float* slopes;  // ALIBI: [H] fp32 per-query-head slopes
+  int ring_m;           // RING: max_kv_size M (s_max is the ring's C slots, window has no s_max bound)
 };
 
 // kv0: the first cached key the row's query sees
 __device__ __forceinline__ int first_visible_key(const DecArgs& p, int len) { return max(0, len - 1 - p.window); }
 
+// RING: the slots the query at position n = end - 1 sees, in ascending slot order: [lo[i], hi[i]) holds positions
+// slot + off[i] (empty ranges have lo == hi).  Range 0 is the sinks max(0, n - W) .. min(3, n); the arc
+// A = max(4, n - min(M - 5, W)) .. n is range 1 when its slots do not wrap, else ranges 1 = [4, slot(n)] and
+// 2 = [slot(A), C).
+struct RingRow {
+  int lo[3], hi[3], off[3];
+};
+__device__ __forceinline__ RingRow ring_row(int end, int M, int C, int W) {
+  RingRow r;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) r.lo[i] = r.hi[i] = r.off[i] = 0;
+  const int n = end - 1;
+  if (max(0, n - W) < min(RING_SINKS, end)) {
+    r.lo[0] = max(0, n - W);
+    r.hi[0] = min(RING_SINKS, end);
+  }
+  const int A = max(RING_SINKS, n - min(M - 5, W));
+  if (A <= n) {
+    const int sa = ring_slot(A, C), sn = ring_slot(n, C);
+    r.lo[1] = sa <= sn ? sa : RING_SINKS;
+    r.hi[1] = sn + 1;
+    r.off[1] = n - sn;
+    if (sa > sn) {
+      r.lo[2] = sa;
+      r.hi[2] = C;
+      r.off[2] = A - sa;
+    }
+  }
+  return r;
+}
+// the hull [lo, hi) of the visible slots in the 256-slot chunk from c0; false when it holds none
+__device__ __forceinline__ bool ring_chunk(const RingRow& r, int c0, int& lo, int& hi) {
+  lo = INT_MAX;
+  hi = INT_MIN;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const int l = max(r.lo[i], c0), h = min(r.hi[i], c0 + DEC_CHUNK);
+    if (l < h) {
+      lo = min(lo, l);
+      hi = max(hi, h);
+    }
+  }
+  return lo < hi;
+}
+// chunks holding a visible slot (the ranges are ascending and disjoint)
+__device__ __forceinline__ int ring_live_chunks(const RingRow& r) {
+  int n = 0, last = -1;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    if (r.lo[i] >= r.hi[i]) continue;
+    const int c_hi = (r.hi[i] - 1) / DEC_CHUNK;
+    n += max(0, c_hi - max(r.lo[i] / DEC_CHUNK, last + 1) + 1);
+    last = max(last, c_hi);
+  }
+  return n;
+}
+// whether slot s is visible, and its position's offset from s
+__device__ __forceinline__ bool ring_visible(const RingRow& r, int s, int& off) {
+  off = 0;
+  bool in = false;
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+    if (s >= r.lo[i] && s < r.hi[i]) {
+      in = true;
+      off = r.off[i];
+    }
+  return in;
+}
+
 // ALIBI: at least 4 CTAs per SM (<= 128 registers); left to itself ptxas keeps the ALiBi kernels at 64 registers and
-// spills the bf16 D = 32 / 128 ones.  ALIBI = false keeps the plain bound (0 = none).
-template <typename T, int D, bool ALIBI = false>
-__global__ void __launch_bounds__(DEC_THREADS, ALIBI ? 4 : 0)
+// spills the bf16 D = 32 / 128 ones.  RING takes the same bound (without it the ring kernels spill too).
+// ALIBI = RING = false keeps the plain bound (0 = none).
+//
+// RING (attn_decode_ring): s_max is the ring's C slots and lens[b] the positions the row holds.  The chunks are
+// 256-slot chunks of the ring; one holding no visible slot (ring_row) exits at once, and one holding some reads the
+// hull of its visible slots, from the 32-slot tile holding the first, with the slots outside the ranges masked.  The
+// ALiBi distance is the slot's position (slot + its range's offset) minus the query's.
+template <typename T, int D, bool ALIBI = false, bool RING = false>
+__global__ void __launch_bounds__(DEC_THREADS, ALIBI || RING ? 4 : 0)
 attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const DecArgs p) {
   constexpr int L = D / 8;                        // 8-column slices per row
   constexpr int TILE_ELEMS = DEC_TILE * D;
   constexpr int TILE_BYTES = TILE_ELEMS * (int)sizeof(T);
   const int c = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
-  const int len = min(p.lens[b], p.s_max);
   const int c0 = c * DEC_CHUNK;
-  const int kv0 = first_visible_key(p, len);
-  if (c0 >= len || c0 + DEC_CHUNK <= kv0) return;
-  const int lo = max(c0, kv0 & ~(DEC_TILE - 1));  // the first live chunk starts at the tile holding kv0
-  const int end = min(len, c0 + DEC_CHUNK);
+  int len, kv0, lo, end, n_chunks;
+  RingRow rr;
+  if constexpr (RING) {
+    len = p.lens[b];
+    if (len < 1) return;
+    rr = ring_row(len, p.ring_m, p.s_max, p.window);
+    if (!ring_chunk(rr, c0, kv0, end)) return;
+    lo = kv0 & ~(DEC_TILE - 1);
+    n_chunks = ring_live_chunks(rr);
+  } else {
+    len = min(p.lens[b], p.s_max);
+    kv0 = first_visible_key(p, len);
+    if (c0 >= len || c0 + DEC_CHUNK <= kv0) return;
+    lo = max(c0, kv0 & ~(DEC_TILE - 1));  // the first live chunk starts at the tile holding kv0
+    end = min(len, c0 + DEC_CHUNK);
+    n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK - kv0 / DEC_CHUNK;  // live chunks of the row
+  }
   const int n_tiles = (end - lo + DEC_TILE - 1) / DEC_TILE;
-  const int n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK - kv0 / DEC_CHUNK;  // live chunks of the row
   const int G = p.G;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
@@ -201,7 +288,11 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
       for (int key = tid / L; key < DEC_TILE; key += DEC_THREADS / L) {
         float kf[8];
         ld8(tK + key * D + kl * 8, kf);
-        const bool valid = start + key >= first_valid;
+        bool valid = start + key >= first_valid;
+        if constexpr (RING) {
+          int off;
+          valid = valid && ring_visible(rr, start + key, off);
+        }
         for (int g = 0; g < G; ++g) {
           const float4 qa = *reinterpret_cast<const float4*>(sq + g * D + kl * 8);
           const float4 qc = *reinterpret_cast<const float4*>(sq + g * D + kl * 8 + 4);
@@ -224,7 +315,11 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     // online softmax (log2 domain): one warp per head, one lane per key; every tile holds at least one valid key
     // (kv0 < end, and kv0 lies in the first tile).  ALIBI: kd = this lane's key distance, converted once per tile
     float kd = 0.f;
-    if constexpr (ALIBI) kd = (float)(start + lane - (len - 1));
+    if constexpr (ALIBI) {
+      int off = 0;
+      if constexpr (RING) ring_visible(rr, start + lane, off);
+      kd = (float)(start + lane + off - (len - 1));
+    }
     for (int g = warp; g < G; g += DEC_THREADS / 32) {
       float x = ss[g * DEC_TILE + lane];
       if constexpr (ALIBI) x = x + sred[g] * kd;
@@ -307,21 +402,38 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
 
 // o = sum_c exp2(m_c - M) acc_c / sum_c exp2(m_c - M) l_c over a row's live chunks, in chunk order; one thread per
 // column
-template <typename T, int D>
+// (RING: over the chunks ring_chunk finds live, the others skipped)
+template <typename T, int D, bool RING = false>
 __global__ void __launch_bounds__(D)
 attn_decode_combine_kernel(const DecArgs p) {
   const int h = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
-  const int len = min(p.lens[b], p.s_max);
-  const int c_lo = first_visible_key(p, len) / DEC_CHUNK;
-  const int n = (len + DEC_CHUNK - 1) / DEC_CHUNK;
-  if (n - c_lo <= 1) return;  // finished by attn_decode_kernel
+  int c_lo, n;
+  RingRow rr;
+  if constexpr (RING) {
+    if (p.lens[b] < 1) return;
+    rr = ring_row(p.lens[b], p.ring_m, p.s_max, p.window);
+    if (ring_live_chunks(rr) <= 1) return;  // finished by attn_decode_kernel
+    c_lo = 0;
+    n = p.max_chunks;
+  } else {
+    const int len = min(p.lens[b], p.s_max);
+    c_lo = first_visible_key(p, len) / DEC_CHUNK;
+    n = (len + DEC_CHUNK - 1) / DEC_CHUNK;
+    if (n - c_lo <= 1) return;  // finished by attn_decode_kernel
+  }
+  auto live = [&](int c) {
+    int lo, hi;
+    return !RING || ring_chunk(rr, c * DEC_CHUNK, lo, hi);
+  };
   const long long bh = (long long)b * p.H + h;
   const float* ml = p.part_ml + bh * p.max_chunks * 2;
   const float* pa = p.part_acc + bh * p.max_chunks * D + d;
   float M = -INFINITY;
-  for (int c = c_lo; c < n; ++c) M = fmaxf(M, ml[2 * c]);
+  for (int c = c_lo; c < n; ++c)
+    if (live(c)) M = fmaxf(M, ml[2 * c]);
   float l = 0.f, acc = 0.f;
   for (int c = c_lo; c < n; ++c) {
+    if (!live(c)) continue;
     const float w = exp2f(ml[2 * c] - M);
     l = fmaf(ml[2 * c + 1], w, l);
     acc = fmaf(pa[(long long)c * D], w, acc);
@@ -332,10 +444,10 @@ attn_decode_combine_kernel(const DecArgs p) {
   if (p.lse != nullptr && d == 0) p.lse[bh] = (M + log2f(l)) / kLog2e;
 }
 
-template <typename T, int D, bool ALIBI = false>
+template <typename T, int D, bool ALIBI = false, bool RING = false>
 int launch_decode(const CUtensorMap& tmK, const CUtensorMap& tmV, const DecArgs& a, int B, int Hk,
                   cudaStream_t stream) {
-  auto kern = attn_decode_kernel<T, D, ALIBI>;
+  auto kern = attn_decode_kernel<T, D, ALIBI, RING>;
   const DecSmem lay(D, (int)sizeof(T), a.G);
   static int attr_bytes = 0;
   if (lay.total > 48 * 1024 && lay.total > attr_bytes) {
@@ -345,7 +457,7 @@ int launch_decode(const CUtensorMap& tmK, const CUtensorMap& tmV, const DecArgs&
   kern<<<dim3(a.max_chunks, Hk, B), DEC_THREADS, lay.total, stream>>>(tmK, tmV, a);
   B200_CHECK_LAUNCH();
   if (a.max_chunks > 1) {
-    attn_decode_combine_kernel<T, D><<<dim3(a.H, B), D, 0, stream>>>(a);
+    attn_decode_combine_kernel<T, D, RING><<<dim3(a.H, B), D, 0, stream>>>(a);
     B200_CHECK_LAUNCH();
   }
   return B200_OK;
@@ -375,11 +487,14 @@ __device__ __forceinline__ void rope_pairs8(const float* xv, const float* cos4, 
 // One thread per 8-column vector: q heads (rotated in place, RoPE only), then k heads (rotated when RoPE is on) and
 // v heads, both written to cache row pos = lens[b] - 1.  The rotation is b200_rope's arithmetic, statement for
 // statement, so a token rotated here equals the same token rotated by the prefill.
-template <typename T>
+// RING (kv_append_ring): s_max is the ring's C slots; the cache row is slot(pos), pos itself unbounded, and a row
+// with live[b] == 0 (live non-null) is skipped whole.
+template <typename T, bool RING = false>
 __global__ void __launch_bounds__(256)
 kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v, T* __restrict__ k_cache,
                  T* __restrict__ v_cache, const int* __restrict__ lens, const float* __restrict__ cos_t,
-                 const float* __restrict__ sin_t, long long nvec, int s_max, int H, int Hk, int D) {
+                 const float* __restrict__ sin_t, long long nvec, int s_max, int H, int Hk, int D,
+                 const int* __restrict__ live = nullptr) {
   const int L = D / 8;
   const int q_heads = cos_t != nullptr ? H : 0;
   const int heads = q_heads + 2 * Hk;
@@ -388,7 +503,13 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
     const int hh = (int)(i / L % heads);
     const int b = (int)(i / L / heads);
     const int pos = lens[b] - 1;
-    if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
+    int row = pos;  // the cache row
+    if constexpr (RING) {
+      if (pos < 0 || (live != nullptr && live[b] == 0)) continue;
+      row = ring_slot(pos, s_max);
+    } else {
+      if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
+    }
     const T* src;
     T* dst;
     bool rotate = cos_t != nullptr;
@@ -397,11 +518,11 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
     } else if (hh < q_heads + Hk) {
       const int h = hh - q_heads;
       src = k + ((long long)b * Hk + h) * D + dv * 8;
-      dst = k_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+      dst = k_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
     } else {
       const int h = hh - q_heads - Hk;
       src = v + ((long long)b * Hk + h) * D + dv * 8;
-      dst = v_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+      dst = v_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
       rotate = false;
     }
     float xv[8], o[8];
@@ -417,11 +538,12 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
 
 // kv_append_kernel for the half-split layout: one thread per 8-column slice pair (columns [8 dv, 8 dv + 8) and the
 // same D/2 later) of a q, k or v head.  q and k are rotated by rope_half8, b200_rope_half's own rotation.
-template <typename T>
+template <typename T, bool RING = false>
 __global__ void __launch_bounds__(256)
 kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v, T* __restrict__ k_cache,
                       T* __restrict__ v_cache, const int* __restrict__ lens, const float* __restrict__ cos_t,
-                      const float* __restrict__ sin_t, long long nslice, int s_max, int H, int Hk, int D) {
+                      const float* __restrict__ sin_t, long long nslice, int s_max, int H, int Hk, int D,
+                      const int* __restrict__ live = nullptr) {
   const int L = D / 16;
   const int heads = H + 2 * Hk;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nslice; i += (long long)gridDim.x * blockDim.x) {
@@ -429,7 +551,13 @@ kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __res
     const int hh = (int)(i / L % heads);
     const int b = (int)(i / L / heads);
     const int pos = lens[b] - 1;
-    if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
+    int row = pos;  // the cache row
+    if constexpr (RING) {
+      if (pos < 0 || (live != nullptr && live[b] == 0)) continue;
+      row = ring_slot(pos, s_max);
+    } else {
+      if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
+    }
     const T* src;
     T* dst;
     bool rotate = true;
@@ -438,11 +566,11 @@ kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __res
     } else if (hh < H + Hk) {
       const int h = hh - H;
       src = k + ((long long)b * Hk + h) * D + dv * 8;
-      dst = k_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+      dst = k_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
     } else {
       const int h = hh - H - Hk;
       src = v + ((long long)b * Hk + h) * D + dv * 8;
-      dst = v_cache + (((long long)b * s_max + pos) * Hk + h) * D + dv * 8;
+      dst = v_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
       rotate = false;
     }
     float xl[8], xh[8];
@@ -940,9 +1068,10 @@ int check_quant_format(const char* what, int B, int s_max, int Hk, int D, int bi
 }
 
 // window < 0 means none; slopes selects ALiBi
+// ring_m > 0: a ring of s_max slots (bf16, D 64 / 128) with max_kv_size ring_m
 int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                      int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
-                     size_t ws_bytes, cudaStream_t stream, const float* slopes = nullptr) {
+                     size_t ws_bytes, cudaStream_t stream, const float* slopes = nullptr, int ring_m = 0) {
   B200_CHECK_ARG(B > 0 && H > 0 && Hk > 0 && H % Hk == 0, "attn_decode: bad shape B=%d H=%d Hk=%d", B, H, Hk);
   B200_CHECK_ARG(D == 16 || D == 32 || D == 64 || D == 128, "attn_decode: head_dim %d unsupported (16/32/64/128)", D);
   B200_CHECK_ARG(s_max >= DEC_TILE, "attn_decode: s_max=%d must be >= %d", s_max, DEC_TILE);
@@ -978,6 +1107,15 @@ int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, co
   a.scale_log2 = scale * kLog2e;
   a.window = window < 0 || window > s_max ? s_max : window;
   a.slopes = slopes;
+  a.ring_m = ring_m;
+  if (ring_m > 0) {
+    a.window = window < 0 ? INT_MAX : window;
+    if (slopes)
+      return D == 64 ? launch_decode<__nv_bfloat16, 64, true, true>(tmK, tmV, a, B, Hk, stream)
+                     : launch_decode<__nv_bfloat16, 128, true, true>(tmK, tmV, a, B, Hk, stream);
+    return D == 64 ? launch_decode<__nv_bfloat16, 64, false, true>(tmK, tmV, a, B, Hk, stream)
+                   : launch_decode<__nv_bfloat16, 128, false, true>(tmK, tmV, a, B, Hk, stream);
+  }
   if (slopes)
     return is_bf16 ? launch_decode_d<__nv_bfloat16, true>(D, tmK, tmV, a, B, Hk, stream)
                    : launch_decode_d<float, true>(D, tmK, tmV, a, B, Hk, stream);
@@ -1070,6 +1208,57 @@ int b200_kv_append_half(void* q, const void* k, const void* v, void* k_cache, vo
     kv_append_half_kernel<float><<<(int)blocks, 256, 0, s>>>((float*)q, (const float*)k, (const float*)v,
                                                              (float*)k_cache, (float*)v_cache, lens, cos_t,
                                                              sin_t, nslice, s_max, H, Hk, D);
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// The rotating KV cache of the reference's generator (core/generation_lite.py:103, :120: max_kv_size makes every
+// layer's cache an mlx_lm RotatingKVCache): decode attention over a ring of C slots (include/b200_hotpath.h)
+int b200_attn_decode_ring(const void* q, const void* k_ring, const void* v_ring, const int* end, void* o, float* lse,
+                          int max_kv, int window, const float* slopes, int B, int C, int H, int Hk, int D, float scale,
+                          void* ws, size_t ws_bytes, void* stream) {
+  B200_CHECK_ARG(max_kv >= 5 && C >= max_kv, "attn_decode_ring: max_kv=%d must be >= 5 and <= C=%d", max_kv, C);
+  B200_CHECK_ARG(D == 64 || D == 128, "attn_decode_ring: head_dim %d unsupported (64 or 128)", D);
+  B200_CHECK_ARG(al16(k_ring) && al16(v_ring), "attn_decode_ring: k_ring and v_ring must be 16-byte aligned");
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0, "attn_decode_ring: slopes must be 4-byte aligned");
+  return attn_decode_impl(q, k_ring, v_ring, end, o, lse, window, B, C, H, Hk, D, scale, 1, ws, ws_bytes,
+                          static_cast<cudaStream_t>(stream), slopes, max_kv);
+}
+
+// The token a decode step appends to a ring (core/generation_lite.py:103, :120): rotated at position end[b] - 1,
+// stored in slot(end[b] - 1); rows with live[b] == 0 are left alone
+int b200_kv_append_ring(void* q, const void* k, const void* v, void* k_ring, void* v_ring, const int* end,
+                        const int* live, const float* cos_t, const float* sin_t, int half, int B, int C, int H,
+                        int Hk, int D, void* stream) {
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  B200_CHECK_ARG(B > 0 && C > RING_SINKS && H > 0 && Hk > 0 && H % Hk == 0 && (D == 64 || D == 128),
+                 "kv_append_ring: bad shape B=%d C=%d H=%d Hk=%d D=%d (D 64 or 128)", B, C, H, Hk, D);
+  B200_CHECK_ARG(end != nullptr && (reinterpret_cast<uintptr_t>(end) & 3u) == 0 &&
+                     (reinterpret_cast<uintptr_t>(live) & 3u) == 0,
+                 "kv_append_ring: end (non-null) and live must be 4-byte aligned int32 [B] arrays");
+  B200_CHECK_ARG((cos_t == nullptr) == (sin_t == nullptr) && (!half || cos_t != nullptr),
+                 "kv_append_ring: give both RoPE tables or neither (the half layout needs them)");
+  B200_CHECK_ARG(al16(q) && al16(k) && al16(v) && al16(k_ring) && al16(v_ring) &&
+                     (cos_t == nullptr || (al16(cos_t) && al16(sin_t))),
+                 "kv_append_ring: alignment");
+  auto* qq = static_cast<__nv_bfloat16*>(q);
+  auto* kk = static_cast<const __nv_bfloat16*>(k);
+  auto* vv = static_cast<const __nv_bfloat16*>(v);
+  auto* kr = static_cast<__nv_bfloat16*>(k_ring);
+  auto* vr = static_cast<__nv_bfloat16*>(v_ring);
+  if (half) {
+    const long long nslice = (long long)B * (H + 2 * Hk) * (D / 16);
+    long long blocks = (nslice + 255) / 256;
+    if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+    kv_append_half_kernel<__nv_bfloat16, true><<<(int)blocks, 256, 0, s>>>(qq, kk, vv, kr, vr, end, cos_t, sin_t,
+                                                                           nslice, C, H, Hk, D, live);
+  } else {
+    const long long nvec = (long long)B * ((cos_t != nullptr ? H : 0) + 2 * Hk) * (D / 8);
+    long long blocks = (nvec + 255) / 256;
+    if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+    kv_append_kernel<__nv_bfloat16, true><<<(int)blocks, 256, 0, s>>>(qq, kk, vv, kr, vr, end, cos_t, sin_t, nvec,
+                                                                      C, H, Hk, D, live);
+  }
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

@@ -60,6 +60,16 @@
 // the tiles are not aligned to the queries) and on those reaching below its rows' window start.  Padding rows take the last valid
 // row's position and their Q rows are zeroed in shared memory, so their outputs are finite whatever Q holds there.
 // CACHED = false compiles to the kernels above unchanged.
+//
+// Rotating cache (RING = true, on the CACHED kernels): the cache is a ring of C = s_max slots holding position t in
+// slot(t) (common.cuh, ring_slot), and query position q sees key position k iff k <= q, q - k <= W and (k < 4 or
+// q - k <= M - 5).  The CTA's queries q_lo .. q_hi see the sinks and the arc A = max(4, q_lo - min(M - 5, W)) .. q_hi,
+// whose slots form at most two ranges (the arc wraps at most once, as C >= M + L - 1).  Thread 0 writes a table of
+// three slot ranges into shared memory: the sink tile (ending at slot min(4, q_hi + 1)), then the arc's ranges, each
+// tiled by 128-slot tiles anchored at the range's end.  Inside a range position = slot + off, and the keys below its
+// first position are masked like those below a window start, so the loop, its masks and ALiBi run on positions as in
+// the cached kernel.  No slot at or past end[b] is loaded before the ring first wraps; after it every slot holds a
+// written key.  RING = false compiles to the kernels above unchanged.
 #include "common.cuh"
 #include "host.h"
 
@@ -99,8 +109,50 @@ struct FwdArgs {
   unsigned long long drop_seed;  // DROP: Philox key
   const int* start;     // CACHED: [B] int32 position of each row's first query; S is the chunk length L
   const int* end;       // CACHED: [B] int32 cached positions once the chunk is in (its last query's position + 1)
-  int s_max;            // CACHED: positions of the K / V cache
+  int s_max;            // CACHED: positions of the K / V cache (RING: its slots C)
+  int ring_m;           // RING: max_kv_size M
 };
+
+// RING: the table of slot ranges (see the head of this file), 4 ints per range: the running tile count at its end,
+// the slot of its first tile, the offset from slot to position and its first visible position
+constexpr int RING_TAB_BYTES = 64;
+__device__ __forceinline__ void ring_table(int* tab, int qlo, int qhi, int C, int M, int W) {
+  int n = qlo - W <= RING_SINKS - 1 ? 1 : 0;  // some sink is in some query's window
+  tab[0] = n;
+  tab[1] = min(RING_SINKS, qhi + 1) - ATT_BKV;
+  tab[2] = tab[3] = 0;
+  const int A = max(RING_SINKS, qlo - min(M - 5, W));
+  int lo[2] = {0, 0}, hi[2] = {0, 0}, off[2] = {0, 0};
+  if (A <= qhi) {
+    const int sa = ring_slot(A, C), sh = ring_slot(qhi, C);
+    lo[0] = sa;
+    if (sa <= sh) {
+      hi[0] = sh + 1;
+      off[0] = qhi - sh;
+    } else {  // the older positions up to slot C - 1, then the newer ones from slot 4
+      hi[0] = C;
+      off[0] = A - sa;
+      lo[1] = RING_SINKS;
+      hi[1] = sh + 1;
+      off[1] = qhi - sh;
+    }
+  }
+  for (int r = 0; r < 2; ++r) {
+    const int nt = (hi[r] - lo[r] + ATT_BKV - 1) / ATT_BKV;
+    n += nt;
+    tab[4 * r + 4] = n;
+    tab[4 * r + 5] = hi[r] - nt * ATT_BKV;
+    tab[4 * r + 6] = off[r];
+    tab[4 * r + 7] = lo[r] + off[r];
+  }
+}
+// RING: tile j's first slot, its range (0: the sinks), the range's offset and first visible position
+__device__ __forceinline__ int ring_tile(const int* tab, int j, int& r, int& off, int& rlo) {
+  r = (j >= tab[0]) + (j >= tab[4]);
+  off = tab[4 * r + 2];
+  rlo = tab[4 * r + 3];
+  return tab[4 * r + 1] + (j - (r == 0 ? 0 : tab[4 * r - 4])) * ATT_BKV;
+}
 
 // first key query `row` of batch row b may see: its document start, or its window start when that is later
 __device__ __forceinline__ int key_start(const FwdArgs& p, int b, int row) {
@@ -135,10 +187,12 @@ __device__ __forceinline__ void pv_mma(float* o, const uint32_t* a, uint64_t db)
   else wgmma_m64n64k16_rs<1>(o, a, db);
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false, bool CACHED = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false, bool CACHED = false,
+          bool RING = false>
 __global__ void __launch_bounds__(FWD_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const FwdArgs p) {
+  static_assert(!RING || CACHED, "the ring is built on the cached kernel");
   static_assert(!PREFIX || (!DOC && !ALIBI), "the prefix mask is built on the causal kernel");
   static_assert(!PREFIX || !DROP, "dropout is not built on the prefix kernels");
   static_assert(!CACHED || (!DOC && !PREFIX && !DROP), "cached queries are built on the causal kernel");
@@ -148,6 +202,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const uint32_t s0 = smem_u32(smem);
   const uint32_t sQ = s0 + Cfg::OFF_Q, sK = s0 + Cfg::OFF_K, sV = s0 + Cfg::OFF_V;
   const uint32_t q_full = s0 + Cfg::OFF_BAR, kv_full0 = q_full + 8, kv_empty0 = q_full + 24;
+  int* ring_tab = reinterpret_cast<int*>(smem + Cfg::OFF_BAR + 64);  // RING only
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int hk = h / (p.H / p.Hk);
   const int q0 = qt * ATT_BQ;
@@ -167,7 +222,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   int c_st = 0, c_nv = 0, kbase = 0;
   if constexpr (CACHED) {
     c_st = max(__ldg(p.start + b), 0);
-    c_nv = min(min(__ldg(p.end + b), p.s_max) - c_st, p.S);
+    c_nv = min((RING ? __ldg(p.end + b) : min(__ldg(p.end + b), p.s_max)) - c_st, p.S);
     if (q0 >= c_nv) {  // padding rows only
       const int rows = min(ATT_BQ, p.S - q0);
       for (int i = threadIdx.x; i < rows * (D / 8); i += FWD_THREADS) {
@@ -178,8 +233,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       return;
     }
     const int kend = c_st + min(q0 + ATT_BQ, c_nv);
-    n_kv = (kend - max(0, c_st + q0 - p.window) + ATT_BKV - 1) / ATT_BKV;
-    kbase = kend - n_kv * ATT_BKV;
+    if constexpr (RING) {
+      if (threadIdx.x == 0) ring_table(ring_tab, c_st + q0, kend - 1, p.s_max, p.ring_m, p.window);
+    } else {
+      n_kv = (kend - max(0, c_st + q0 - p.window) + ATT_BKV - 1) / ATT_BKV;
+      kbase = kend - n_kv * ATT_BKV;
+    }
   }
 
   if (threadIdx.x == 0) {
@@ -191,6 +250,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     fence_mbar_init();
   }
   __syncthreads();
+  if constexpr (RING) n_kv = ring_tab[8];
 
   if (warp == 8) {
     if (lane == 0) {
@@ -204,9 +264,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mbar_wait(kv_empty0 + 8 * s, (((j - j0) >> 1) & 1) ^ 1u);
         const uint32_t full = kv_full0 + 8 * s;
         mbar_arrive_expect_tx(full, 2 * Cfg::KV_BYTES);
+        int slot = kbase + j * ATT_BKV;
+        if constexpr (RING) {
+          int r, off, rlo;
+          slot = ring_tile(ring_tab, j, r, off, rlo);
+        }
         for (int nb = 0; nb < Cfg::NB; ++nb) {
-          tma_load_4d(sK + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmK, full, nb * 64, hk, kbase + j * ATT_BKV, b);
-          tma_load_4d(sV + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmV, full, nb * 64, hk, kbase + j * ATT_BKV, b);
+          tma_load_4d(sK + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmK, full, nb * 64, hk, slot, b);
+          tma_load_4d(sV + s * Cfg::KV_BYTES + nb * ATT_BKV * 128, &tmV, full, nb * 64, hk, slot, b);
         }
       }
     }
@@ -259,7 +324,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const int s = (j - j0) & 1;
     mbar_wait(kv_full0 + 8 * s, ((j - j0) >> 1) & 1);
     const uint32_t tK = sK + s * Cfg::KV_BYTES, tV = sV + s * Cfg::KV_BYTES;
-    const int k0 = kbase + j * ATT_BKV;
+    int k0 = kbase + j * ATT_BKV;
 
     // S = Q K^T: 64 rows x 128 keys per warpgroup, both operands K-major (head dim contiguous)
     float sc[64];
@@ -293,7 +358,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     if constexpr (CACHED) {
       // keys k_lane + c, c = 8 nc + (e & 1); ALiBi's bias m log2e (key - p) is fmaf(m log2e, c, abase[r]) as below.
       // The rows' window starts are formed per tile: kept across the loop they push D = 128 into spills.
-      const int plo[2] = {max(0, prow[0] - p.window), max(0, prow[1] - p.window)};
+      // RING: the tile's position and its range's bounds are read here, after the S MMAs, for the same reason.
+      int ring_lo = 0, ring_w = 0;
+      if constexpr (RING) {
+        int r, off;
+        k0 = ring_tile(ring_tab, j, r, off, ring_lo) + off;
+        ring_w = r == 0 ? p.window : min(p.ring_m - 5, p.window);
+      }
+      const int plo[2] = {RING ? max(ring_lo, prow[0] - ring_w) : max(0, prow[0] - p.window),
+                          RING ? max(ring_lo, prow[1] - ring_w) : max(0, prow[1] - p.window)};
       const bool edge = k0 + ATT_BKV - 1 > prow[0] || k0 < plo[1];  // prow[0] <= prow[1]
       const int k_lane = k0 + (lane & 3) * 2;
       float abase[2] = {0.f, 0.f};
@@ -450,18 +523,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   }
 }
 
-template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false, bool CACHED = false>
+template <int D, bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false, bool CACHED = false,
+          bool RING = false>
 int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
                cudaStream_t stream) {
   using Cfg = FwdCfg<D>;
-  auto kern = attn_fwd_kernel<D, DOC, ALIBI, PREFIX, DROP, CACHED>;
+  auto kern = attn_fwd_kernel<D, DOC, ALIBI, PREFIX, DROP, CACHED, RING>;
+  constexpr int smem_bytes = Cfg::SMEM_BYTES + (RING ? RING_TAB_BYTES : 0);
   static bool attr_set = false;
   if (!attr_set) {
-    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     attr_set = true;
   }
   dim3 grid((a.S + ATT_BQ - 1) / ATT_BQ, a.H, a.B);
-  kern<<<grid, FWD_THREADS, Cfg::SMEM_BYTES, stream>>>(tmQ, tmK, tmV, a);
+  kern<<<grid, FWD_THREADS, smem_bytes, stream>>>(tmQ, tmK, tmV, a);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }
@@ -635,6 +710,51 @@ int b200_attn_fwd_cached(const void* q, const void* k_cache, const void* v_cache
                    : launch_fwd<128, false, true, false, false, true>(tmQ, tmK, tmV, a, s);
   return D == 64 ? launch_fwd<64, false, false, false, false, true>(tmQ, tmK, tmV, a, s)
                  : launch_fwd<128, false, false, false, false, true>(tmQ, tmK, tmV, a, s);
+}
+
+// The rotating KV cache of the reference's generator (core/generation_lite.py:103, :120): a chunk of queries at
+// positions start[b] + i over a ring of C slots that already holds their keys (include/b200_hotpath.h)
+int b200_attn_fwd_ring(const void* q, const void* k_ring, const void* v_ring, const int* start, const int* end,
+                       void* o, float* lse, int max_kv, int window, const float* slopes, int B, int L, int C, int H,
+                       int Hk, int D, float scale, void* stream) {
+  B200_CHECK_ARG(B > 0 && L > 0 && H > 0 && Hk > 0 && H % Hk == 0, "attn_fwd_ring: bad shape B=%d L=%d H=%d Hk=%d",
+                 B, L, H, Hk);
+  B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd_ring: head_dim %d unsupported (64 or 128)", D);
+  B200_CHECK_ARG(max_kv >= 5 && (long long)C >= (long long)max_kv + L - 1,
+                 "attn_fwd_ring: max_kv=%d must be >= 5 and C=%d >= max_kv + L - 1 (L=%d)", max_kv, C, L);
+  B200_CHECK_ARG(start != nullptr && end != nullptr && (reinterpret_cast<uintptr_t>(start) & 3u) == 0 &&
+                     (reinterpret_cast<uintptr_t>(end) & 3u) == 0,
+                 "attn_fwd_ring: start and end must be non-null, 4-byte aligned int32 [B] arrays");
+  B200_CHECK_ARG(al16(q) && al16(k_ring) && al16(v_ring) && al16(o),
+                 "attn_fwd_ring: q, k_ring, v_ring and o must be 16-byte aligned");
+  B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0 && (reinterpret_cast<uintptr_t>(lse) & 3u) == 0,
+                 "attn_fwd_ring: slopes and lse must be 4-byte aligned");
+  CUtensorMap tmQ, tmK, tmV;
+  int rc;
+  if ((rc = make_bshd_map(&tmQ, q, B, L, H, D, ATT_BQ))) return rc;
+  if ((rc = make_bshd_map(&tmK, k_ring, B, C, Hk, D, ATT_BKV))) return rc;
+  if ((rc = make_bshd_map(&tmV, v_ring, B, C, Hk, D, ATT_BKV))) return rc;
+  FwdArgs a{};
+  a.o = reinterpret_cast<__nv_bfloat16*>(o);
+  a.lse = lse;
+  a.B = B;
+  a.S = L;
+  a.H = H;
+  a.Hk = Hk;
+  a.scale = scale;
+  a.causal = 1;
+  a.window = window < 0 ? INT_MAX : window;
+  a.slopes = slopes;
+  a.start = start;
+  a.end = end;
+  a.s_max = C;
+  a.ring_m = max_kv;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (slopes)
+    return D == 64 ? launch_fwd<64, false, true, false, false, true, true>(tmQ, tmK, tmV, a, s)
+                   : launch_fwd<128, false, true, false, false, true, true>(tmQ, tmK, tmV, a, s);
+  return D == 64 ? launch_fwd<64, false, false, false, false, true, true>(tmQ, tmK, tmV, a, s)
+                 : launch_fwd<128, false, false, false, false, true, true>(tmQ, tmK, tmV, a, s);
 }
 
 }  // extern "C"

@@ -29,6 +29,12 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t u) {
   return __bfloat1622float2(v);
 }
 
+// The rotating KV cache's slot map (include/b200_hotpath.h, ops.ring_slot): position t of a ring of C slots
+constexpr int RING_SINKS = 4;
+__device__ __forceinline__ int ring_slot(int t, int C) {
+  return t < RING_SINKS ? t : RING_SINKS + (t - RING_SINKS) % (C - RING_SINKS);
+}
+
 // Attention dropout's keep bits: Philox4x32-10 (Salmon et al., SC'11) of counter (k >> 3, q, h, b) and key
 // (seed lo, seed hi) gives 8 uniform 16-bit values r, one per key 8 (k >> 3) + i, r_i = (w[i >> 1] >> 16 (i & 1)) &
 // 0xffff.  Key i is kept iff r_i >= t; bit i of the result.

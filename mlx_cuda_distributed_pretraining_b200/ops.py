@@ -1159,6 +1159,142 @@ def attention_cached(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
 
 
 # ------------------------------------------------------------------------------------------------
+# the rotating KV cache (the reference's max_kv_size; DESIGN §4.2.3): per layer, K and V rings bf16 [B, C, Hk, D]
+# ------------------------------------------------------------------------------------------------
+RING_SINKS = 4
+
+
+def ring_slot(pos, slots: int):
+    """The slot of position pos in a ring of `slots` slots (include/b200_hotpath.h): pos itself for the sinks
+    pos < 4, else 4 + (pos - 4) mod (slots - 4).  pos: an int or an integer tensor."""
+    if isinstance(pos, torch.Tensor):
+        return torch.where(pos < RING_SINKS, pos, RING_SINKS + (pos - RING_SINKS) % (slots - RING_SINKS))
+    return pos if pos < RING_SINKS else RING_SINKS + (pos - RING_SINKS) % (slots - RING_SINKS)
+
+
+def check_max_kv_size(max_kv_size, what: str = "max_kv_size") -> int:
+    if isinstance(max_kv_size, bool) or not isinstance(max_kv_size, int) or max_kv_size < RING_SINKS + 1:
+        raise ValueError(f"{what}: max_kv_size must be an int >= {RING_SINKS + 1}, got {max_kv_size!r}")
+    return max_kv_size
+
+
+def _check_ring(q: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.Tensor, max_kv_size, what: str, qdim: int):
+    for t, nm in ((q, "q"), (k_ring, "k_ring"), (v_ring, "v_ring")):
+        if t.dtype != torch.bfloat16:
+            raise ValueError(f"{what}: {nm} must be bf16 (the rotating cache is bf16 only), got {t.dtype}")
+        _need(t, torch.bfloat16, f"{what}: {nm}")
+    if q.dim() != qdim or k_ring.dim() != 4 or k_ring.shape != v_ring.shape:
+        raise ValueError(f"{what}: expected q with {qdim} dims and k_ring == v_ring [B,C,Hk,D], got "
+                         f"{tuple(q.shape)}, {tuple(k_ring.shape)}, {tuple(v_ring.shape)}")
+    B, H, D = q.shape[0], q.shape[-2], q.shape[-1]
+    Bc, C, Hk, Dc = k_ring.shape
+    if Bc != B or Dc != D or H % Hk != 0:
+        raise ValueError(f"{what}: q {tuple(q.shape)} does not match the ring {tuple(k_ring.shape)}")
+    if D not in (64, 128):
+        raise ValueError(f"{what}: head_dim {D} unsupported (64 or 128)")
+    check_max_kv_size(max_kv_size, what)
+    return B, H, D, C, Hk
+
+
+def attention_decode_ring(q: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.Tensor, end: torch.Tensor,
+                          max_kv_size: int, scale: Optional[float] = None, workspace: Optional[torch.Tensor] = None,
+                          return_lse: bool = False, window: Optional[int] = None,
+                          alibi: Optional[torch.Tensor] = None):
+    """attention_decode over a ring of C slots (b200_attn_decode_ring): the query at position p = end[b] - 1 sees
+    key positions k <= p with k < 4 or p - k <= max_kv_size - 5 (and p - k <= window), read from slot ring_slot(k, C),
+    with ALiBi's bias alibi[h] * (k - p).  q [B,H,D]; k_ring, v_ring [B,C,Hk,D]; all bf16, D in {64, 128};
+    C >= max_kv_size; end int32 [B] on the device, end[b] >= 1 (not checked: that would read the device)."""
+    what = "attention_decode_ring"
+    B, H, D, C, Hk = _check_ring(q, k_ring, v_ring, max_kv_size, what, 3)
+    _check_rows(end, B, q.device, what, "end")
+    if C < max_kv_size:
+        raise ValueError(f"{what}: the ring's {C} slots cannot hold max_kv_size={max_kv_size} keys")
+    if window is not None:
+        window = _check_window(window, what)
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, True, what)
+    if scale is None:
+        scale = D ** -0.5
+    need = attention_decode_workspace_bytes(B, H, C, D)
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
+    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need:
+        raise ValueError(f"{what}: workspace must be uint8 on {q.device} with >= {need} bytes")
+    o = torch.empty_like(q)
+    lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
+    tok = _t0("attn_decode_ring")
+    check(lib().b200_attn_decode_ring(q.data_ptr(), k_ring.data_ptr(), v_ring.data_ptr(), end.data_ptr(),
+                                      o.data_ptr(), _ptr(lse), int(max_kv_size), -1 if window is None else int(window),
+                                      _ptr(alibi), B, C, H, Hk, D, float(scale), workspace.data_ptr(),
+                                      workspace.numel(), _stream()), "b200_attn_decode_ring")
+    _t1(tok)
+    return (o, lse) if return_lse else o
+
+
+def attention_ring(q: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.Tensor, start: torch.Tensor,
+                   end: torch.Tensor, max_kv_size: int, scale: Optional[float] = None, window: Optional[int] = None,
+                   alibi: Optional[torch.Tensor] = None, return_lse: bool = False):
+    """attention_cached over a ring of C slots that already holds the chunk's keys (b200_attn_fwd_ring): query i of
+    row b sits at position p = start[b] + i and sees key positions k <= p with k < 4 or p - k <= max_kv_size - 5
+    (and p - k <= window), with ALiBi's bias on positions.  q [B,L,H,D]; k_ring, v_ring [B,C,Hk,D] bf16; D in {64,
+    128}; C >= max_kv_size + L - 1.  Rows i >= end[b] - start[b] are padding: finite, unspecified.  The values of
+    start and end are not checked (0 <= end[b] - start[b] <= L)."""
+    what = "attention_ring"
+    B, H, D, C, Hk = _check_ring(q, k_ring, v_ring, max_kv_size, what, 4)
+    L = q.shape[1]
+    if C < max_kv_size + L - 1:
+        raise ValueError(f"{what}: the ring's {C} slots are fewer than max_kv_size + L - 1 = "
+                         f"{max_kv_size + L - 1}: writing the chunk would overwrite keys its queries see")
+    _check_rows(start, B, q.device, what, "start")
+    _check_rows(end, B, q.device, what, "end")
+    if window is not None:
+        window = _check_window(window, what)
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, True, what)
+    if scale is None:
+        scale = D ** -0.5
+    o = torch.empty_like(q)
+    lse = torch.empty((B, H, L), device=q.device, dtype=torch.float32) if return_lse else None
+    tok = _t0("attn_ring")
+    check(lib().b200_attn_fwd_ring(q.data_ptr(), k_ring.data_ptr(), v_ring.data_ptr(), start.data_ptr(),
+                                   end.data_ptr(), o.data_ptr(), _ptr(lse), int(max_kv_size),
+                                   -1 if window is None else int(window), _ptr(alibi), B, L, C, H, Hk, D,
+                                   float(scale), _stream()), "b200_attn_fwd_ring")
+    _t1(tok)
+    return (o, lse) if return_lse else o
+
+
+def kv_append_ring(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.Tensor,
+                   end: torch.Tensor, live: Optional[torch.Tensor] = None,
+                   rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                   layout: str = "interleaved") -> None:
+    """kv_append into a ring (b200_kv_append_ring): k (rotated at position end[b] - 1 with rope_tables, as is q in
+    place) and v go to slot ring_slot(end[b] - 1, C).  live (int32 [B] on the device, optional): rows with live[b]
+    == 0 are left alone, q included.  bf16, D in {64, 128}."""
+    what = "kv_append_ring"
+    _check_choice(layout, ROPE_LAYOUTS, f"{what}: layout")
+    B, H, D, C, Hk = _check_ring(q, k_ring, v_ring, RING_SINKS + 1, what, 3)
+    _check_rows(end, B, q.device, what, "end")
+    if live is not None:
+        _check_rows(live, B, q.device, what, "live")
+    for t, nm in ((k, "k"), (v, "v")):
+        _need(t, torch.bfloat16, f"{what}: {nm}")
+        if t.shape != (B, Hk, D):
+            raise ValueError(f"{what}: {nm} must be [{B},{Hk},{D}], got {tuple(t.shape)}")
+    cos_t = sin_t = None
+    if rope_tables is not None:
+        cos_t, sin_t = rope_tables
+        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
+            _need(t, torch.float32, f"{what}: {nm}")
+            if t.dim() != 2 or t.shape[1] != D // 2:
+                raise ValueError(f"{what}: RoPE tables must be [positions, {D // 2}]")
+    half = int(layout == "half" and cos_t is not None)
+    check(lib().b200_kv_append_ring(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_ring.data_ptr(), v_ring.data_ptr(),
+                                    end.data_ptr(), _ptr(live), _ptr(cos_t), _ptr(sin_t), half, B, C, H, Hk, D,
+                                    _stream()), "b200_kv_append_ring")
+
+
+# ------------------------------------------------------------------------------------------------
 # the quantized KV cache (the reference's kv_bits / kv_group_size; DESIGN §4.2.1): per layer, codes uint8
 # [B, s_max, Hk, D * bits / 8] and parameters fp32 [B, Hk, s_max, D / group_size, 2] for each of K and V
 # ------------------------------------------------------------------------------------------------
