@@ -546,6 +546,43 @@ int b200_kv_append_ring(void* q, const void* k, const void* v, void* k_ring, voi
                         const int* live, const float* cos_t, const float* sin_t, int half, int B, int C, int H,
                         int Hk, int D, void* stream);
 
+/* ---- beam search over a shared-prompt cache (the reference's beam_search, generate_lite.py:400-484) -------------
+ * R beam rows in n_groups groups (one per prompt), described by one device int32 array
+ *     tables = [row_group (R) | row_slot (R) | grp_t0 (n_groups) | grp_row0 (n_groups) | grp_rows (n_groups)].
+ * A group's rows are contiguous (grp_row0[g], grp_rows[g] of them) and have the same length lens[b] (positions held,
+ * the new token included).  Positions t < T0 = grp_t0[g] (a multiple of 256) live in the group's prefix cache
+ * k_prefix / v_prefix [n_groups, s_prefix, Hk, D]; positions t >= T0 of row b at index t - T0 of its tail slot
+ * row_slot[b] in k_tail / v_tail [n_slots, tail_cap, Hk, D].
+ * Prefix positions >= T0, tail indices >= lens[b] - T0 and slots no row uses are never read.
+ *
+ * b200_attn_decode_beam: b200_attn_decode_alibi (window < 0: none, slopes NULL: no ALiBi) for each row's query at
+ *   position lens[b] - 1 over that layout.  Chunks are 256 positions from 0, as b200_attn_decode's.  A prefix chunk is
+ *   read once for each pack of b200_attn_decode_beam_pack(H, Hk, D) consecutive rows of a group, whose query heads
+ *   run together; a tail chunk once per row.  Merge order depends on (lens[b], T0, window) alone, so a row's output is
+ *   bit-identical in any batch and, with one row per group, equal to b200_attn_decode(_alibi) over the materialised
+ *   row.  q and o bf16 or f32 [R, H, D], D in 16/32/64/128.  s_prefix and tail_cap are multiples of 256.
+ *   Workspace: b200_attn_decode_beam_workspace_bytes, 128-byte aligned; the call writes the tails' tensor maps to its
+ *   start (an asynchronous copy on the stream) and the partials after them. */
+int b200_attn_decode_beam(const void* q, const void* k_prefix, const void* v_prefix, const void* k_tail,
+                          const void* v_tail, const int* lens, const int* tables, void* o, float* lse, int window,
+                          const float* slopes, int R, int n_groups, int s_prefix, int n_slots, int tail_cap, int H,
+                          int Hk, int D, float scale, int is_bf16, void* workspace, size_t workspace_bytes,
+                          void* stream);
+size_t b200_attn_decode_beam_workspace_bytes(int R, int H, int s_prefix, int tail_cap, int D);
+/* Beam rows that share one read of a prefix chunk: max(1, 2048 / (H / Hk * D)); 0 for a bad shape. */
+int b200_attn_decode_beam_pack(int H, int Hk, int D);
+/* b200_kv_append (half == 0) or b200_kv_append_half (half != 0, tables required) into the tails: q and k rotated at
+ *   position lens[b] - 1 with those kernels' own statements, k and v written to index lens[b] - 1 - T0 of slot
+ *   row_slot[b] (T0 = grp_t0[row_group[b]], tables as above; only its first 2 R + n_groups entries are read). */
+int b200_kv_append_beam(void* q, const void* k, const void* v, void* k_tail, void* v_tail, const int* lens,
+                        const int* tables, const float* cos_t, const float* sin_t, int half, int R, int tail_cap, int H,
+                        int Hk, int D, int is_bf16, void* stream);
+/* Copy-on-fork: copies int32 [n_copies, 3] = (src slot, dst slot, n) copies tail indices [0, n <= max_len) from slot
+ *   src to slot dst in each of the n_bufs tails bufs (a device array of pointers, every layer's K and V), one launch.
+ *   row_bytes = Hk * D * element size, a multiple of 16.  No destination may be a source.  n_copies == 0: nothing. */
+int b200_kv_beam_fork(void* const* bufs, int n_bufs, const int* copies, int n_copies, int max_len, int tail_cap,
+                      int row_bytes, void* stream);
+
 /* ---- mixture-of-experts MLP (Mixtral's sparse MoE block, model.misc.num_local_experts) -------------------------
  * T tokens, E experts (2..64), k experts per token (1..min(E, 8)), hidden H, per-expert intermediate I (H, I % 8 == 0).
  * Everything stays on the device and nothing uses atomics: the same inputs give the same bits on every run.

@@ -134,6 +134,15 @@ class RingKV:
         self.k, self.v, self.max_kv_size, self.live = k, v, max_kv_size, live
 
 
+class BeamKV:
+    """One layer of a beam search's cache (llama.BeamKVCache; DESIGN §4.2.4): the groups' prefix K / V [G, s_prefix,
+    Hk, D], the beam tails [S, tail_cap, Hk, D] and the cache's int32 device tables (ops.attention_decode_beam)."""
+
+    def __init__(self, k_prefix, v_prefix, k_tail, v_tail, tables: torch.Tensor, n_groups: int):
+        self.k_prefix, self.v_prefix, self.k_tail, self.v_tail = k_prefix, v_prefix, k_tail, v_tail
+        self.tables, self.n_groups = tables, n_groups
+
+
 class FlashAttention(nn.Module):
     """alibi: add ALiBi's bias alibi_slopes(num_heads)[h] * (k - q) to every causal score (the slopes are not
     parameters: a device tensor made on first use, like rope_tables).  dropout: the probability p of dropping an
@@ -270,12 +279,18 @@ class FlashAttention(nn.Module):
         """One new token per row, x [B, hidden]: its k and v go to cache position lens[b] - 1 (rotated there when
         RoPE is on), then its query attends over the row's first lens[b] cached keys (the last window + 1 of them
         with a sliding window), with the ALiBi bias when the module has it.  k_cache is a QuantizedKV (v_cache None)
-        for a quantized cache."""
+        for a quantized cache, a BeamKV (v_cache None) for a beam search's rows."""
         B = x.shape[0]
         q, k, v = self._project(x)
         q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
         k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
         v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
+        if isinstance(k_cache, BeamKV):
+            c = k_cache
+            ops.kv_append_beam(q, k, v, c.k_tail, c.v_tail, lens, c.tables, c.n_groups, self.rope_tables, rope_layout)
+            ctx = ops.attention_decode_beam(q, c.k_prefix, c.v_prefix, c.k_tail, c.v_tail, lens, c.tables, self.scale,
+                                            workspace, window=window, alibi=self.alibi_slopes(q.device))
+            return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
         if isinstance(k_cache, RingKV):
             ops.kv_append_ring(q, k, v, k_cache.k, k_cache.v, lens, k_cache.live, self.rope_tables, rope_layout)
             ctx = ops.attention_decode_ring(q, k_cache.k, k_cache.v, lens, k_cache.max_kv_size, self.scale, workspace,

@@ -26,7 +26,8 @@ import torch
 from torch import nn
 
 from .. import ops
-from .flash_attention import CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask, QuantizedKV, RingKV
+from .flash_attention import (BeamKV, CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask, QuantizedKV,
+                              RingKV)
 
 VARIANTS = (None, "reference", "mlx_lm")
 
@@ -424,6 +425,89 @@ class KVCache:
         if self.quant is not None:
             return sum(q.nbytes() for q in self.quant)
         return 0 if self.k is None else sum(t.numel() * t.element_size() for t in self.k + self.v)
+
+
+class BeamKVCache:
+    """The cache of a beam search (core.generation.beam_search; DESIGN §4.2.4).  `prefix` is an ordinary KVCache of
+    batch G that Model.prefill filled with the G prompts (the groups), stored and read once per group.  Group g's fork
+    point is T0_g = 256 floor(P_g / 256) for its prompt length P_g: positions below it are read from the prefix, and a
+    beam's positions t >= T0_g live at index t - T0_g of the beam's tail slot, per layer K and V tails
+    [S = G n_beams, tail_cap, Hk, D] with tail_cap = 255 + max_tokens rounded up to 256.  Group g owns slots
+    [g n_beams, (g + 1) n_beams); prompt positions [T0_g, P_g) start in slot g n_beams.
+
+    The decode batch is the live beam rows, set by set_rows (group, slot and length per row; a group's rows are
+    contiguous and equally long).  fork copies tails between slots.  Model.decode_step runs on it unchanged."""
+
+    def __init__(self, model: "Model", prefix: KVCache, n_beams: int, max_tokens: int):
+        if prefix.quantized or prefix.rotating or prefix.kv_bits is not None or prefix.k is None:
+            raise ValueError("BeamKVCache: the prefix must be an unquantized, non-rotating KVCache filled by prefill")
+        attn = model.layers[0].self_attn
+        self.prefix, self.n_beams = prefix, n_beams
+        self.n_groups = prefix._batch
+        self.t0 = [256 * (n // 256) for n in prefix.host_lens]
+        self.tail_cap = -(-(255 + max_tokens) // 256) * 256
+        S = self.n_groups * n_beams
+        shape = (S, self.tail_cap, attn.num_kv_heads, attn.head_dim)
+        dev, dt = prefix._device, prefix._dtype
+        self.k = [torch.zeros(shape, device=dev, dtype=dt) for _ in range(prefix._layers)]
+        self.v = [torch.zeros(shape, device=dev, dtype=dt) for _ in range(prefix._layers)]
+        for g, (t0, n) in enumerate(zip(self.t0, prefix.host_lens)):  # the prompts' last positions, once
+            for tail, pre in zip(self.k + self.v, prefix.k + prefix.v):
+                tail[g * n_beams, :n - t0].copy_(pre[g, t0:n])
+        tails = self.k + self.v
+        self._buffers = torch.tensor([t.data_ptr() for t in tails], dtype=torch.int64).to(dev)
+        nbytes = ops.attention_decode_beam_workspace_bytes(S, attn.num_heads, prefix.s_max, self.tail_cap,
+                                                           attn.head_dim)
+        self.workspace = torch.empty(max(nbytes, 16), device=dev, dtype=torch.uint8)
+        self._views = None
+        self.set_rows(list(range(self.n_groups)), [g * n_beams for g in range(self.n_groups)], prefix.host_lens)
+
+    def set_rows(self, groups, slots, lengths) -> None:
+        """The decode batch: row b belongs to group groups[b] (ascending), holds lengths[b] positions and keeps its
+        tail in slot slots[b].  One host-to-device copy."""
+        groups, slots, lengths = [int(g) for g in groups], [int(s) for s in slots], [int(n) for n in lengths]
+        R, G = len(groups), self.n_groups
+        if R < 1 or len(slots) != R or len(lengths) != R or any(b < a for a, b in zip(groups, groups[1:])):
+            raise ValueError("set_rows: one group, slot and length per row, groups ascending, at least one row")
+        row0, rows = [0] * G, [0] * G
+        for b, g in enumerate(groups):
+            if rows[g] == 0:
+                row0[g] = b
+            rows[g] += 1
+        t = torch.tensor(lengths + groups + slots + self.t0 + row0 + rows, dtype=torch.int32).to(self.prefix._device)
+        self.host_lens, self.groups, self.slots = lengths, groups, slots
+        self.lens, self.tables = t[:R], t[R:]
+        self._views = None
+
+    def fork(self, copies) -> None:
+        """copies: (src slot, dst slot, positions) triples: tail indices [0, positions) of every layer's K and V tail
+        go from src to dst, in one launch.  No destination may be a source."""
+        if not copies:
+            return
+        c = torch.tensor(copies, dtype=torch.int32).to(self.prefix._device)
+        ops.kv_beam_fork(self._buffers, c, max(n for _, _, n in copies), self.k + self.v)
+
+    def layer(self, i: int):
+        if self._views is None:  # made once per decode step: it calls layer() for every layer
+            p = self.prefix
+            self._views = [BeamKV(pk, pv, k, v, self.tables, self.n_groups)
+                           for pk, pv, k, v in zip(p.k, p.v, self.k, self.v)]
+        return self._views[i], None
+
+    def advance(self, live=None) -> None:
+        if live is not None:
+            raise ValueError("advance: live is for a rotating cache")
+        if any(n + 1 - self.t0[g] > self.tail_cap for n, g in zip(self.host_lens, self.groups)):
+            raise ValueError(f"beam cache full: the tails hold {self.tail_cap} positions past the fork point")
+        self.host_lens = [n + 1 for n in self.host_lens]
+        self.lens.add_(1)
+
+    def maybe_quantize(self) -> None:
+        pass
+
+    def nbytes(self) -> int:
+        """Bytes held by the prefix and the tails."""
+        return self.prefix.nbytes() + sum(t.numel() * t.element_size() for t in self.k + self.v)
 
 
 class CacheChunk:

@@ -4,7 +4,7 @@
                               --repetition-penalty 1.1 --repetition-context-size 20]
                               [--top-p P --seed N --num-samples N --checkpoint step_N --runs-dir runs]
                               [--kv-bits {4,8} --kv-group-size {32,64,128} --quantized-kv-start N]
-                              [--prefill-step-size N]
+                              [--prefill-step-size N] [--num-beams N]
 
 The run's config.yaml (written by the trainer) rebuilds the model through Trainer(cfg, for_training=False), the
 checkpoint's weights are loaded into it, and `generate` prefills [BOS] + tokenize(prompt) once and then decodes one
@@ -18,11 +18,12 @@ argmax.  The filters below are device-agnostic torch over [..., V] fp32 logits.
 from __future__ import annotations
 
 import argparse
+import math
 import random
 import sys
 import time
 from pathlib import Path
-from typing import Callable, List, Optional, Sequence
+from typing import Callable, List, Optional, Sequence, Tuple
 
 import torch
 
@@ -287,6 +288,140 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
 
 
 # ------------------------------------------------------------------------------------------------
+# beam search (generate_lite.py:400-484 of the reference; DESIGN §2 records each rule)
+# ------------------------------------------------------------------------------------------------
+Beam = Tuple[List[int], float]
+
+
+def select_beams(beams: Sequence[Beam], top_tokens, top_logprobs, n: int, stop_tokens=None):
+    """One step of the reference's selection for one group.  beams: the live beams (generated tokens, score) in order;
+    top_tokens / top_logprobs: per beam, its top candidates in rank order (at least n).  Candidates are scored
+    parent + log-probability (Python floats), ordered beam-major then by rank, stably sorted by score descending and
+    popped until n are chosen; one ending in a stop token is finished instead (its token stripped, score -inf when it
+    is the first generated token) and n drops by one.  Returns (chosen (parent index, token, score) in order, finished
+    beams, the new n)."""
+    stops = set(stop_tokens) if stop_tokens is not None else None
+    cands = [(i, int(top_tokens[i][k]), score + float(top_logprobs[i][k]))
+             for i, (_, score) in enumerate(beams) for k in range(n)]
+    cands.sort(key=lambda c: c[2], reverse=True)
+    chosen, finished = [], []
+    for i, t, score in cands:
+        if len(chosen) >= n:
+            break
+        if stops is not None and t in stops:
+            finished.append((list(beams[i][0]), -math.inf if not beams[i][0] else score))
+            n -= 1
+        else:
+            chosen.append((i, t, score))
+    return chosen, finished, n
+
+
+def plan_slots(slots: Sequence[int], free: Sequence[int], parents: Sequence[int]):
+    """Copy-on-fork for one group.  slots[i]: the tail slot of live beam i; free: the group's unused slots; parents:
+    the parent of each chosen child, in row order.  A parent's first child keeps its slot; each further child takes a
+    free slot (those unused, then those of beams without children) that receives a copy of the parent's tail.
+    Returns (the children's slots, (src, dst) copies, the slots left free)."""
+    has_child = set(parents)
+    pool = list(free) + [s for i, s in enumerate(slots) if i not in has_child]
+    kept, out, copies = set(), [], []
+    for p in parents:
+        if p not in kept:
+            kept.add(p)
+            out.append(slots[p])
+        else:
+            d = pool.pop(0)
+            copies.append((slots[p], d))
+            out.append(d)
+    return out, copies, pool
+
+
+def beam_result(live: Sequence[Beam], finished: Sequence[Beam]) -> List[Beam]:
+    """The reference's result: the live beams when nothing finished, else the finished beams and the live beams that
+    generated a token; sorted by score descending (stable)."""
+    res = list(live) if not finished else list(finished) + [b for b in live if len(b[0]) > 0]
+    res.sort(key=lambda b: b[1], reverse=True)
+    return [(list(t), s) for t, s in res]
+
+
+def beam_search(model, prompts: List[List[int]], n_beams: int = 4, max_tokens: int = 512,
+                stop_tokens: Optional[Sequence[int]] = None, *, kv_bits: Optional[int] = None,
+                max_kv_size: Optional[int] = None, prompt_cache=None,
+                on_step: Optional[Callable[[List[List[int]], torch.Tensor], None]] = None) -> List[List[Beam]]:
+    """The reference's beam_search for each prompt, the prompts searched independently in one batch.  Returns per
+    prompt the list of (generated tokens, score), best first (beam_result).  The model's logits go through
+    log_softmax; there is no temperature, sampler or repetition penalty.  Each prompt is prefilled once and its cache
+    shared by its beams (arch.llama.BeamKVCache); a beam step reads back the [rows, n] candidates once, selects on the
+    host (select_beams), forks the tails (plan_slots) and runs Model.decode_step over the live beams.  A quantized or
+    rotating cache and continuing from a prompt_cache are not supported.  on_step(rows, logits), if given, sees each
+    step's decode rows (prompt + generated tokens, in row order) and their fp32 logits [rows, V] before selection."""
+    from ..arch.llama import BeamKVCache, KVCache
+
+    if isinstance(n_beams, bool) or not isinstance(n_beams, int) or n_beams < 1:
+        raise ValueError(f"beam_search: n_beams must be an int >= 1, got {n_beams!r}")
+    if kv_bits is not None or max_kv_size is not None or prompt_cache is not None:
+        raise ValueError("beam_search: kv_bits, max_kv_size and prompt_cache are not supported (the beams share one "
+                         "unquantized, unbounded prompt cache)")
+    if not prompts or any(len(p) == 0 for p in prompts):
+        raise ValueError("beam_search: every prompt needs at least one token")
+    if isinstance(max_tokens, bool) or not isinstance(max_tokens, int) or max_tokens < 0:
+        raise ValueError(f"beam_search: max_tokens must be an int >= 0, got {max_tokens!r}")
+    limit = position_limit(model.args)
+    longest = max(len(p) for p in prompts)
+    if limit is not None and longest + max_tokens > limit:
+        raise ValueError(f"prompt ({longest} tokens) + max_tokens ({max_tokens}) exceeds max_position_embeddings "
+                         f"({limit}): training truncates there and the RoPE tables end there")
+    G = len(prompts)
+    if max_tokens == 0:
+        return [[([], 0.0) for _ in range(n_beams)] for _ in prompts]
+    device = model.embed_tokens.weight.device
+    tokens = torch.zeros((G, longest), dtype=torch.int64)
+    for g, p in enumerate(prompts):
+        tokens[g, :len(p)] = torch.tensor(p, dtype=torch.int64)
+    prefix = KVCache(model, G, longest)
+    logits = model.prefill(tokens.to(device), [len(p) for p in prompts], prefix)
+    cache = BeamKVCache(model, prefix, n_beams, max_tokens)
+    # per group: live beams, their slots, the free slots, n, finished beams (step 0 starts from one beam per prompt:
+    # the reference's n identical copies give the same candidates once duplicates are dropped)
+    beams: List[List[Beam]] = [[([], 0.0)] for _ in prompts]
+    slots = [[g * n_beams] for g in range(G)]
+    free = [list(range(g * n_beams + 1, (g + 1) * n_beams)) for g in range(G)]
+    n = [n_beams] * G
+    finished: List[List[Beam]] = [[] for _ in prompts]
+    for step in range(max_tokens):
+        alive = [g for g in range(G) if beams[g]]
+        if on_step is not None:
+            on_step([list(prompts[g]) + b[0] for g in alive for b in beams[g]], logits)
+        width = max(n[g] for g in alive)
+        logprobs = torch.log_softmax(logits, dim=-1)
+        top = _sorted_desc(logprobs)[:, :width]
+        host = torch.cat([top.double(), torch.gather(logprobs, -1, top).double()], dim=1).cpu().tolist()
+        r = 0
+        rows_g, rows_slot, rows_len, next_tokens, copies = [], [], [], [], []
+        for g in alive:
+            rows = host[r:r + len(beams[g])]
+            r += len(beams[g])
+            chosen, done, n[g] = select_beams(beams[g], [x[:width] for x in rows], [x[width:] for x in rows], n[g],
+                                              stop_tokens)
+            finished[g] += done
+            parents = [c[0] for c in chosen]
+            new_slots, pairs, free[g] = plan_slots(slots[g], free[g], parents)
+            held = len(prompts[g]) + step - cache.t0[g]  # tail positions each parent holds
+            copies += [(s, d, held) for s, d in pairs]
+            beams[g] = [(beams[g][i][0] + [t], score) for i, t, score in chosen]
+            slots[g] = new_slots
+            rows_g += [g] * len(chosen)
+            rows_slot += new_slots
+            rows_len += [len(prompts[g]) + step] * len(chosen)
+            next_tokens += [t for _, t, _ in chosen]
+        if step + 1 == max_tokens or not next_tokens:
+            break
+        cache.set_rows(rows_g, rows_slot, rows_len)
+        cache.fork(copies)
+        logits = model.decode_step(torch.tensor(next_tokens, dtype=torch.int64).to(device), cache)
+    return [beam_result(beams[g], finished[g]) for g in range(G)]
+
+
+# ------------------------------------------------------------------------------------------------
 # CLI (core/generation.py:10-78 of the reference)
 # ------------------------------------------------------------------------------------------------
 def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
@@ -315,7 +450,19 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
     ap.add_argument("--max-kv-size", type=int, default=None,
                     help="Keep a rotating KV cache: each token attends to the first 4 and the most recent "
                          "max-kv-size - 4 tokens (default: an unbounded cache)")
+    ap.add_argument("--num-beams", type=int, default=None,
+                    help="Beam search with this many beams, printing every returned beam with its score (default: "
+                         "sampling).  The sampling flags (temperature, min-p, top-p, repetition penalty, seed) do not "
+                         "apply to it, as in the reference")
     a = ap.parse_args(argv)
+    if a.num_beams is not None:
+        if a.num_beams < 1:
+            ap.error("--num-beams must be >= 1")
+        for flag, given in (("--num-samples > 1", a.num_samples > 1), ("--kv-bits", a.kv_bits is not None),
+                            ("--max-kv-size", a.max_kv_size is not None),
+                            ("--prefill-step-size", a.prefill_step_size is not None)):
+            if given:
+                ap.error(f"--num-beams does not combine with {flag}")
     if a.num_samples < 1:
         ap.error("--num-samples must be >= 1")
     if a.quantized_kv_start < 0:
@@ -376,6 +523,12 @@ def main(argv: Optional[List[str]] = None) -> None:
     trainer = load_run(a.run, a.runs_dir, a.checkpoint)
     tok = trainer.tokenizer
     prompt = [tok.BOS_TOKEN] + tok.tokenize(a.prompt)
+    if a.num_beams is not None:
+        for toks, score in beam_search(trainer.model, [prompt], n_beams=a.num_beams, max_tokens=a.max_tokens,
+                                       stop_tokens=[tok.EOS_TOKEN])[0]:
+            print(f"Beam Output (Score: {score:.3f}): {tok.detokenize(toks)}")
+        sys.stdout.flush()
+        return
     seed = a.seed if a.seed is not None else random.SystemRandom().randrange(1 << 62)
     outs = generate(trainer.model, [prompt] * a.num_samples, max_tokens=a.max_tokens, temperature=a.temperature,
                     min_p=a.min_p, top_p=a.top_p, repetition_penalty=a.repetition_penalty,

@@ -96,7 +96,10 @@ struct DecArgs {
   float scale_log2;   // scale * log2 e
   int window;         // keys len - 1 - window .. len - 1 are visible; s_max without a window
   const float* slopes;  // ALIBI: [H] fp32 per-query-head slopes
-  int ring_m;           // RING: max_kv_size M (s_max is the ring's C slots, window has no s_max bound)
+  union {  // the struct's size and every field's offset stay those of the kernels without BEAM
+    int ring_m;                   // RING: max_kv_size M (s_max is the ring's C slots, window has no s_max bound)
+    const struct BeamMaps* beam;  // BEAM: the tails' tensor maps and the tables, in global memory
+  };
 };
 
 // kv0: the first cached key the row's query sees
@@ -171,6 +174,26 @@ __device__ __forceinline__ bool ring_visible(const RingRow& r, int s, int& off) 
   return in;
 }
 
+// BEAM (attn_decode_beam): the beam rows of a group share the group's prefix cache [n_groups, s_prefix, Hk, D] below
+// its fork point T0 (a multiple of DEC_CHUNK) and keep positions t >= T0 at index t - T0 of their own tail slot
+// [n_slots, tail_cap, Hk, D].  A group's rows are contiguous and have the same length.
+struct BeamArgs {
+  const int* row_group;  // [R] the row's group
+  const int* row_slot;   // [R] the row's tail slot
+  const int* grp_t0;     // [n_groups] fork point
+  const int* grp_row0;   // [n_groups] first row
+  const int* grp_rows;   // [n_groups] live rows
+  int pack;              // beams per prefix CTA: pack * G * D <= DEC_MAX_ITEMS * DEC_THREADS * 8
+};
+// BEAM: the tails' tensor maps and the tables, written by the host to the start of the workspace so that the kernel
+// keeps attn_decode_kernel's parameters; BEAM_HDR bytes, the partials follow
+struct BeamMaps {
+  CUtensorMap k_tail, v_tail;
+  BeamArgs args;
+};
+constexpr int BEAM_HDR = 384;
+static_assert(sizeof(BeamMaps) <= BEAM_HDR, "BeamMaps exceeds its workspace header");
+
 // ALIBI: at least 4 CTAs per SM (<= 128 registers); left to itself ptxas keeps the ALiBi kernels at 64 registers and
 // spills the bf16 D = 32 / 128 ones.  RING takes the same bound (without it the ring kernels spill too).
 // ALIBI = RING = false keeps the plain bound (0 = none).
@@ -179,9 +202,16 @@ __device__ __forceinline__ bool ring_visible(const RingRow& r, int s, int& off) 
 // 256-slot chunks of the ring; one holding no visible slot (ring_row) exits at once, and one holding some reads the
 // hull of its visible slots, from the 32-slot tile holding the first, with the slots outside the ranges masked.  The
 // ALiBi distance is the slot's position (slot + its range's offset) minus the query's.
-template <typename T, int D, bool ALIBI = false, bool RING = false>
-__global__ void __launch_bounds__(DEC_THREADS, ALIBI || RING ? 4 : 0)
+//
+// BEAM: blockIdx.z is a beam row and the chunks are the unwindowed kernel's.  A tail chunk (c0 >= T0) reads the row's
+// slot at index pos - T0 (an end-anchored tile below T0 reads TMA's zero fill, masked as below position 0).  A prefix
+// chunk is run by the first row of each pack of `pack` consecutive rows of the group only: it reads the prefix tile
+// once for the nb <= pack rows, whose nb * G query heads act as the CTA's heads (head e = row e / G, q head e % G).
+template <typename T, int D, bool ALIBI = false, bool RING = false, bool BEAM = false>
+__global__ void __launch_bounds__(DEC_THREADS, ALIBI || RING || BEAM ? 4 : 0)
 attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const DecArgs p) {
+  const BeamMaps* bm = BEAM ? p.beam : nullptr;  // BEAM: tmK / tmV are the prefix caches
+  const BeamArgs* bp = BEAM ? &bm->args : nullptr;
   constexpr int L = D / 8;                        // 8-column slices per row
   constexpr int TILE_ELEMS = DEC_TILE * D;
   constexpr int TILE_BYTES = TILE_ELEMS * (int)sizeof(T);
@@ -189,6 +219,8 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   const int c0 = c * DEC_CHUNK;
   int len, kv0, lo, end, n_chunks;
   RingRow rr;
+  int nb = 1, grp = 0, t0 = 0, slot = 0;  // BEAM: rows in this CTA, the row's group, fork point and tail slot
+  bool tail = false;
   if constexpr (RING) {
     len = p.lens[b];
     if (len < 1) return;
@@ -200,12 +232,23 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     len = min(p.lens[b], p.s_max);
     kv0 = first_visible_key(p, len);
     if (c0 >= len || c0 + DEC_CHUNK <= kv0) return;
+    if constexpr (BEAM) {
+      grp = bp->row_group[b];
+      t0 = bp->grp_t0[grp];
+      slot = bp->row_slot[b];
+      tail = c0 >= t0;
+      if (!tail) {
+        const int j = b - bp->grp_row0[grp];
+        if (j % bp->pack != 0) return;
+        nb = min(bp->pack, bp->grp_rows[grp] - j);
+      }
+    }
     lo = max(c0, kv0 & ~(DEC_TILE - 1));  // the first live chunk starts at the tile holding kv0
     end = min(len, c0 + DEC_CHUNK);
     n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK - kv0 / DEC_CHUNK;  // live chunks of the row
   }
   const int n_tiles = (end - lo + DEC_TILE - 1) / DEC_TILE;
-  const int G = p.G;
+  const int G = BEAM ? nb * p.G : p.G;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   extern __shared__ uint8_t smem_raw[];
@@ -225,32 +268,54 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     const int st = j % DEC_STAGES;
     const uint32_t bar = bar0 + 8 * st;
     mbar_arrive_expect_tx(bar, 2 * TILE_BYTES);
-    tma_load_4d(smem_u32(ring + (2 * st) * TILE_ELEMS), &tmK, bar, 0, hk, tile_start(j), b);
-    tma_load_4d(smem_u32(ring + (2 * st + 1) * TILE_ELEMS), &tmV, bar, 0, hk, tile_start(j), b);
+    if (BEAM && tail) {
+      tma_load_4d(smem_u32(ring + (2 * st) * TILE_ELEMS), &bm->k_tail, bar, 0, hk, tile_start(j) - t0, slot);
+      tma_load_4d(smem_u32(ring + (2 * st + 1) * TILE_ELEMS), &bm->v_tail, bar, 0, hk, tile_start(j) - t0, slot);
+    } else {
+      tma_load_4d(smem_u32(ring + (2 * st) * TILE_ELEMS), &tmK, bar, 0, hk, tile_start(j), BEAM ? grp : b);
+      tma_load_4d(smem_u32(ring + (2 * st + 1) * TILE_ELEMS), &tmV, bar, 0, hk, tile_start(j), BEAM ? grp : b);
+    }
   };
 
   if (tid == 0) {
     for (int s = 0; s < DEC_STAGES; ++s) mbar_init(bar0 + 8 * s, 1);
     fence_mbar_init();
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
+    if constexpr (BEAM) {  // the tail maps were written through the generic proxy, possibly over older maps
+      asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(&bm->k_tail) : "memory");
+      asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(&bm->v_tail) : "memory");
+    }
+    tma_prefetch_desc(BEAM && tail ? &bm->k_tail : &tmK);
+    tma_prefetch_desc(BEAM && tail ? &bm->v_tail : &tmV);
   }
   __syncthreads();
   if (tid == 0)
     for (int j = 0; j < min(n_tiles, DEC_STAGES); ++j) issue(j);
 
-  // the G query heads of this kv head are contiguous in [B, H, D]
-  const T* qb = reinterpret_cast<const T*>(p.q) + ((long long)b * p.H + (long long)hk * G) * D;
-  for (int i = tid; i < G * L; i += DEC_THREADS) {
-    float f[8];
-    ld8(qb + i * 8, f);
+  if constexpr (BEAM) {
+    // head e of the CTA is q head hk * p.G + e % p.G of row b + e / p.G
+    for (int i = tid; i < G * L; i += DEC_THREADS) {
+      const int e = i / L;
+      float f[8];
+      ld8(reinterpret_cast<const T*>(p.q) + ((long long)(b + e / p.G) * p.H + hk * p.G + e % p.G) * D + (i % L) * 8,
+          f);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) sq[i * 8 + e] = f[e] * p.scale_log2;
+      for (int x = 0; x < 8; ++x) sq[i * 8 + x] = f[x] * p.scale_log2;
+    }
+  } else {
+    // the G query heads of this kv head are contiguous in [B, H, D]
+    const T* qb = reinterpret_cast<const T*>(p.q) + ((long long)b * p.H + (long long)hk * G) * D;
+    for (int i = tid; i < G * L; i += DEC_THREADS) {
+      float f[8];
+      ld8(qb + i * 8, f);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) sq[i * 8 + e] = f[e] * p.scale_log2;
+    }
   }
   for (int g = tid; g < G; g += DEC_THREADS) {
     sm[g] = -INFINITY;
     sl[g] = 0.f;
-    if constexpr (ALIBI) sred[g] = __ldg(p.slopes + hk * G + g) * kLog2e;  // G <= DEC_THREADS * 8
+    if constexpr (ALIBI && !BEAM) sred[g] = __ldg(p.slopes + hk * G + g) * kLog2e;  // G <= DEC_THREADS * 8
+    if constexpr (ALIBI && BEAM) sred[g] = __ldg(p.slopes + hk * p.G + g % p.G) * kLog2e;
   }
 
   // accumulator ownership: item = (head g, slice) with g = item / L; keys my_ks, my_ks + ks_n, ... of every tile
@@ -380,8 +445,8 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   for (int r = 0; r < DEC_MAX_ITEMS; ++r) {
     if (my_item[r] < 0) continue;
     const int g = my_item[r] / L, sc = my_item[r] % L;
-    const int h = hk * G + g;
-    const long long bh = (long long)b * p.H + h;
+    const int h = BEAM ? hk * p.G + g % p.G : hk * G + g;
+    const long long bh = (long long)(BEAM ? b + g / p.G : b) * p.H + h;
     const float m = sm[g], l = sl[g];
     if (n_chunks == 1) {
       const float inv = 1.0f / l;
@@ -474,6 +539,35 @@ int launch_decode_d(int D, const CUtensorMap& tmK, const CUtensorMap& tmV, const
   }
 }
 
+template <typename T, int D, bool ALIBI>
+int launch_decode_beam(const CUtensorMap* tm, const DecArgs& a, int pack, int R, int Hk, cudaStream_t stream) {
+  auto kern = attn_decode_kernel<T, D, ALIBI, false, true>;
+  const DecSmem lay(D, (int)sizeof(T), a.G * pack);
+  static int attr_bytes = 0;
+  if (lay.total > 48 * 1024 && lay.total > attr_bytes) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+    attr_bytes = lay.total;
+  }
+  kern<<<dim3(a.max_chunks, Hk, R), DEC_THREADS, lay.total, stream>>>(tm[0], tm[1], a);
+  B200_CHECK_LAUNCH();
+  if (a.max_chunks > 1) {
+    attn_decode_combine_kernel<T, D><<<dim3(a.H, R), D, 0, stream>>>(a);
+    B200_CHECK_LAUNCH();
+  }
+  return B200_OK;
+}
+
+template <typename T, bool ALIBI>
+int launch_decode_beam_d(int D, const CUtensorMap* tm, const DecArgs& a, int bp, int R, int Hk,
+                         cudaStream_t stream) {
+  switch (D) {
+    case 16: return launch_decode_beam<T, 16, ALIBI>(tm, a, bp, R, Hk, stream);
+    case 32: return launch_decode_beam<T, 32, ALIBI>(tm, a, bp, R, Hk, stream);
+    case 64: return launch_decode_beam<T, 64, ALIBI>(tm, a, bp, R, Hk, stream);
+    default: return launch_decode_beam<T, 128, ALIBI>(tm, a, bp, R, Hk, stream);
+  }
+}
+
 // b200_rope's interleaved-pair rotation of one 8-column vector, c / sn = the vector's 4 table entries
 __device__ __forceinline__ void rope_pairs8(const float* xv, const float* cos4, const float* sin4, float* o) {
   const float4 c = *reinterpret_cast<const float4*>(cos4);
@@ -489,7 +583,9 @@ __device__ __forceinline__ void rope_pairs8(const float* xv, const float* cos4, 
 // statement, so a token rotated here equals the same token rotated by the prefill.
 // RING (kv_append_ring): s_max is the ring's C slots; the cache row is slot(pos), pos itself unbounded, and a row
 // with live[b] == 0 (live non-null) is skipped whole.
-template <typename T, bool RING = false>
+// BEAM (kv_append_beam): the caches are the tails [n_slots, s_max = tail_cap, Hk, D]; row b writes index pos - T0 of
+// its slot, T0 its group's fork point, and `live` holds the tables [row_group (B) | row_slot (B) | grp_t0].
+template <typename T, bool RING = false, bool BEAM = false>
 __global__ void __launch_bounds__(256)
 kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v, T* __restrict__ k_cache,
                  T* __restrict__ v_cache, const int* __restrict__ lens, const float* __restrict__ cos_t,
@@ -504,9 +600,15 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
     const int b = (int)(i / L / heads);
     const int pos = lens[b] - 1;
     int row = pos;  // the cache row
+    int cb = b;     // the cache's batch index
     if constexpr (RING) {
       if (pos < 0 || (live != nullptr && live[b] == 0)) continue;
       row = ring_slot(pos, s_max);
+    } else if constexpr (BEAM) {
+      const int R = (int)(nvec / L / heads);  // live: the tables [row_group (R) | row_slot (R) | grp_t0]
+      row = pos - live[2 * R + live[b]];
+      cb = live[R + b];
+      if (row < 0 || row >= s_max) continue;
     } else {
       if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
     }
@@ -518,11 +620,11 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
     } else if (hh < q_heads + Hk) {
       const int h = hh - q_heads;
       src = k + ((long long)b * Hk + h) * D + dv * 8;
-      dst = k_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
+      dst = k_cache + (((long long)cb * s_max + row) * Hk + h) * D + dv * 8;
     } else {
       const int h = hh - q_heads - Hk;
       src = v + ((long long)b * Hk + h) * D + dv * 8;
-      dst = v_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
+      dst = v_cache + (((long long)cb * s_max + row) * Hk + h) * D + dv * 8;
       rotate = false;
     }
     float xv[8], o[8];
@@ -538,7 +640,7 @@ kv_append_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict
 
 // kv_append_kernel for the half-split layout: one thread per 8-column slice pair (columns [8 dv, 8 dv + 8) and the
 // same D/2 later) of a q, k or v head.  q and k are rotated by rope_half8, b200_rope_half's own rotation.
-template <typename T, bool RING = false>
+template <typename T, bool RING = false, bool BEAM = false>
 __global__ void __launch_bounds__(256)
 kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __restrict__ v, T* __restrict__ k_cache,
                       T* __restrict__ v_cache, const int* __restrict__ lens, const float* __restrict__ cos_t,
@@ -552,9 +654,15 @@ kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __res
     const int b = (int)(i / L / heads);
     const int pos = lens[b] - 1;
     int row = pos;  // the cache row
+    int cb = b;     // the cache's batch index
     if constexpr (RING) {
       if (pos < 0 || (live != nullptr && live[b] == 0)) continue;
       row = ring_slot(pos, s_max);
+    } else if constexpr (BEAM) {
+      const int R = (int)(nslice / L / heads);  // live: the tables [row_group (R) | row_slot (R) | grp_t0]
+      row = pos - live[2 * R + live[b]];
+      cb = live[R + b];
+      if (row < 0 || row >= s_max) continue;
     } else {
       if (pos < 0 || pos >= s_max) continue;  // outside the documented 1 <= lens[b] <= s_max: write nothing
     }
@@ -566,11 +674,11 @@ kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __res
     } else if (hh < H + Hk) {
       const int h = hh - H;
       src = k + ((long long)b * Hk + h) * D + dv * 8;
-      dst = k_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
+      dst = k_cache + (((long long)cb * s_max + row) * Hk + h) * D + dv * 8;
     } else {
       const int h = hh - H - Hk;
       src = v + ((long long)b * Hk + h) * D + dv * 8;
-      dst = v_cache + (((long long)b * s_max + row) * Hk + h) * D + dv * 8;
+      dst = v_cache + (((long long)cb * s_max + row) * Hk + h) * D + dv * 8;
       rotate = false;
     }
     float xl[8], xh[8];
@@ -588,6 +696,21 @@ kv_append_half_kernel(T* __restrict__ q, const T* __restrict__ k, const T* __res
       st8(dst + D / 2, xh);
     }
   }
+}
+
+// Copy-on-fork: copies[3 i .. 3 i + 2] = (src slot, dst slot, n) copies tail indices [0, n) of slot src to slot dst
+// in each of the n_bufs tails bufs[z] [n_slots, tail_cap, row_vec x 16 bytes].  One CTA row per (copy, buffer); the
+// host makes copies only from live slots to free ones, so no copy reads what another writes.
+__global__ void __launch_bounds__(256)
+kv_beam_fork_kernel(void* const* __restrict__ bufs, const int* __restrict__ copies, int tail_cap, int row_vec) {
+  const int i = blockIdx.y;
+  const int src = copies[3 * i], dst = copies[3 * i + 1], n = copies[3 * i + 2];
+  uint4* base = static_cast<uint4*>(bufs[blockIdx.z]);
+  const uint4* s = base + (long long)src * tail_cap * row_vec;
+  uint4* d = base + (long long)dst * tail_cap * row_vec;
+  const long long total = (long long)n * row_vec;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x)
+    d[e] = s[e];
 }
 
 // ---- quantized KV cache (DESIGN §4.2.1) --------------------------------------------------------------------------
@@ -1259,6 +1382,154 @@ int b200_kv_append_ring(void* q, const void* k, const void* v, void* k_ring, voi
     kv_append_kernel<__nv_bfloat16, true><<<(int)blocks, 256, 0, s>>>(qq, kk, vv, kr, vr, end, cos_t, sin_t, nvec,
                                                                       C, H, Hk, D, live);
   }
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// Beam search over a shared-prompt cache (generate_lite.py:400-484 of the reference runs n_beams full sequences per
+// prompt; here each prompt's cache is stored and read once for its beams, include/b200_hotpath.h)
+int b200_attn_decode_beam(const void* q, const void* k_prefix, const void* v_prefix, const void* k_tail,
+                          const void* v_tail, const int* lens, const int* tables, void* o, float* lse, int window,
+                          const float* slopes, int R, int n_groups, int s_prefix, int n_slots, int tail_cap, int H,
+                          int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes, void* stream) {
+  B200_CHECK_ARG(R > 0 && n_groups > 0 && n_slots > 0 && H > 0 && Hk > 0 && H % Hk == 0,
+                 "attn_decode_beam: bad shape R=%d n_groups=%d n_slots=%d H=%d Hk=%d", R, n_groups, n_slots, H, Hk);
+  B200_CHECK_ARG(D == 16 || D == 32 || D == 64 || D == 128, "attn_decode_beam: head_dim %d unsupported (16/32/64/128)",
+                 D);
+  B200_CHECK_ARG(s_prefix >= DEC_CHUNK && s_prefix % DEC_CHUNK == 0 && tail_cap >= DEC_CHUNK &&
+                     tail_cap % DEC_CHUNK == 0,
+                 "attn_decode_beam: s_prefix=%d and tail_cap=%d must be positive multiples of %d", s_prefix, tail_cap,
+                 DEC_CHUNK);
+  const int G = H / Hk;
+  B200_CHECK_ARG(G * D <= DEC_MAX_ITEMS * DEC_THREADS * 8, "attn_decode_beam: (H/Hk) * D = %d exceeds %d", G * D,
+                 DEC_MAX_ITEMS * DEC_THREADS * 8);
+  B200_CHECK_ARG(al16(q) && al16(o) && al16(k_prefix) && al16(v_prefix) && al16(k_tail) && al16(v_tail),
+                 "attn_decode_beam: q, o and the caches must be 16-byte aligned");
+  B200_CHECK_ARG(lens != nullptr && tables != nullptr && (reinterpret_cast<uintptr_t>(tables) & 3u) == 0,
+                 "attn_decode_beam: lens and tables must be non-null int32 arrays");
+  B200_CHECK_ARG(slopes == nullptr || (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
+                 "attn_decode_beam: slopes must be a 4-byte aligned fp32 [H] array");
+  const size_t need = b200_attn_decode_beam_workspace_bytes(R, H, s_prefix, tail_cap, D);
+  if (ws_bytes < need || ws == nullptr || (reinterpret_cast<uintptr_t>(ws) & 127u) != 0) {
+    set_error("attn_decode_beam: workspace of %zu bytes (128-byte aligned), %zu needed", ws_bytes, need);
+    return B200_ERR_WORKSPACE;
+  }
+  const int s_max = s_prefix + tail_cap;
+  const int elem = is_bf16 ? 2 : 4;
+  const CUtensorMapDataType dt = is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  const uint32_t box[4] = {(uint32_t)D, 1, (uint32_t)DEC_TILE, 1};
+  const uint64_t strides[3] = {(uint64_t)D * elem, (uint64_t)Hk * D * elem, (uint64_t)s_prefix * Hk * D * elem};
+  const uint64_t dims[4] = {(uint64_t)D, (uint64_t)Hk, (uint64_t)s_prefix, (uint64_t)n_groups};
+  const uint64_t tstrides[3] = {(uint64_t)D * elem, (uint64_t)Hk * D * elem, (uint64_t)tail_cap * Hk * D * elem};
+  const uint64_t tdims[4] = {(uint64_t)D, (uint64_t)Hk, (uint64_t)tail_cap, (uint64_t)n_slots};
+  CUtensorMap tm[2];
+  BeamMaps hdr;
+  int rc;
+  if ((rc = make_tensor_map(&tm[0], k_prefix, dt, elem, 4, dims, strides, box, false))) return rc;
+  if ((rc = make_tensor_map(&tm[1], v_prefix, dt, elem, 4, dims, strides, box, false))) return rc;
+  if ((rc = make_tensor_map(&hdr.k_tail, k_tail, dt, elem, 4, tdims, tstrides, box, false))) return rc;
+  if ((rc = make_tensor_map(&hdr.v_tail, v_tail, dt, elem, 4, tdims, tstrides, box, false))) return rc;
+  const int pack = b200_attn_decode_beam_pack(H, Hk, D);
+  hdr.args = BeamArgs{tables, tables + R, tables + 2 * R, tables + 2 * R + n_groups, tables + 2 * R + 2 * n_groups,
+                      pack};
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  B200_CHECK_CUDA(cudaMemcpyAsync(ws, &hdr, sizeof(hdr), cudaMemcpyHostToDevice, s));
+  DecArgs a;
+  a.q = q;
+  a.o = o;
+  a.lse = lse;
+  a.lens = lens;
+  a.max_chunks = s_max / DEC_CHUNK;
+  a.part_acc = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + BEAM_HDR);
+  a.part_ml = a.part_acc + (size_t)R * H * a.max_chunks * D;
+  a.H = H;
+  a.G = G;
+  a.s_max = s_max;
+  a.scale_log2 = scale * kLog2e;
+  a.window = window < 0 || window > s_max ? s_max : window;
+  a.slopes = slopes;
+  a.beam = static_cast<const BeamMaps*>(ws);
+  if (slopes)
+    return is_bf16 ? launch_decode_beam_d<__nv_bfloat16, true>(D, tm, a, pack, R, Hk, s)
+                   : launch_decode_beam_d<float, true>(D, tm, a, pack, R, Hk, s);
+  return is_bf16 ? launch_decode_beam_d<__nv_bfloat16, false>(D, tm, a, pack, R, Hk, s)
+                 : launch_decode_beam_d<float, false>(D, tm, a, pack, R, Hk, s);
+}
+
+size_t b200_attn_decode_beam_workspace_bytes(int R, int H, int s_prefix, int tail_cap, int D) {
+  if (R <= 0 || H <= 0 || s_prefix <= 0 || tail_cap <= 0 || D <= 0) return 0;
+  return BEAM_HDR + b200_attn_decode_workspace_bytes(R, H, s_prefix + tail_cap, D);
+}
+
+int b200_attn_decode_beam_pack(int H, int Hk, int D) {
+  if (H <= 0 || Hk <= 0 || D <= 0 || H % Hk != 0) return 0;
+  return max(1, DEC_MAX_ITEMS * DEC_THREADS * 8 / (H / Hk * D));
+}
+
+// The token a beam step appends: b200_kv_append (half == 0) or b200_kv_append_half (half != 0) rotated at position
+// lens[b] - 1 and written to index lens[b] - 1 - T0 of row b's tail slot
+int b200_kv_append_beam(void* q, const void* k, const void* v, void* k_tail, void* v_tail, const int* lens,
+                        const int* tables, const float* cos_t, const float* sin_t, int half, int R, int tail_cap, int H,
+                        int Hk, int D, int is_bf16, void* stream) {
+  B200_CHECK_ARG(R > 0 && tail_cap > 0 && H > 0 && Hk > 0 && D > 0 && D % (half ? 16 : 8) == 0,
+                 "kv_append_beam: bad shape R=%d tail_cap=%d H=%d Hk=%d D=%d (D %% %d == 0)", R, tail_cap, H, Hk, D,
+                 half ? 16 : 8);
+  B200_CHECK_ARG((cos_t == nullptr) == (sin_t == nullptr) && (!half || cos_t != nullptr),
+                 "kv_append_beam: give both RoPE tables or neither (the half layout needs them)");
+  B200_CHECK_ARG(lens != nullptr && tables != nullptr, "kv_append_beam: lens and tables must be non-null");
+  B200_CHECK_ARG(al16(k) && al16(v) && al16(k_tail) && al16(v_tail) &&
+                     (cos_t == nullptr || (al16(q) && al16(cos_t) && al16(sin_t))),
+                 "kv_append_beam: alignment");
+  const long long n = half ? (long long)R * (H + 2 * Hk) * (D / 16)
+                           : (long long)R * ((cos_t != nullptr ? H : 0) + 2 * Hk) * (D / 8);
+  long long blocks = (n + 255) / 256;
+  if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (is_bf16) {
+    auto* qq = static_cast<__nv_bfloat16*>(q);
+    auto* kk = static_cast<const __nv_bfloat16*>(k);
+    auto* vv = static_cast<const __nv_bfloat16*>(v);
+    auto* kt = static_cast<__nv_bfloat16*>(k_tail);
+    auto* vt = static_cast<__nv_bfloat16*>(v_tail);
+    if (half)
+      kv_append_half_kernel<__nv_bfloat16, false, true><<<(int)blocks, 256, 0, s>>>(
+          qq, kk, vv, kt, vt, lens, cos_t, sin_t, n, tail_cap, H, Hk, D, tables);
+    else
+      kv_append_kernel<__nv_bfloat16, false, true><<<(int)blocks, 256, 0, s>>>(
+          qq, kk, vv, kt, vt, lens, cos_t, sin_t, n, tail_cap, H, Hk, D, tables);
+  } else {
+    auto* qq = static_cast<float*>(q);
+    auto* kk = static_cast<const float*>(k);
+    auto* vv = static_cast<const float*>(v);
+    auto* kt = static_cast<float*>(k_tail);
+    auto* vt = static_cast<float*>(v_tail);
+    if (half)
+      kv_append_half_kernel<float, false, true><<<(int)blocks, 256, 0, s>>>(
+          qq, kk, vv, kt, vt, lens, cos_t, sin_t, n, tail_cap, H, Hk, D, tables);
+    else
+      kv_append_kernel<float, false, true><<<(int)blocks, 256, 0, s>>>(qq, kk, vv, kt, vt, lens, cos_t, sin_t, n,
+                                                                       tail_cap, H, Hk, D, tables);
+  }
+  B200_CHECK_LAUNCH();
+  return B200_OK;
+}
+
+// The copies of one beam step's fork, for every layer's K and V tail in one launch
+int b200_kv_beam_fork(void* const* bufs, int n_bufs, const int* copies, int n_copies, int max_len, int tail_cap,
+                      int row_bytes, void* stream) {
+  if (n_copies == 0) return B200_OK;
+  B200_CHECK_ARG(bufs != nullptr && copies != nullptr && n_bufs > 0 && n_bufs <= 65535 && n_copies > 0 &&
+                     n_copies <= 65535,
+                 "kv_beam_fork: bad table n_bufs=%d n_copies=%d", n_bufs, n_copies);
+  B200_CHECK_ARG(max_len >= 0 && max_len <= tail_cap && row_bytes > 0 && row_bytes % 16 == 0,
+                 "kv_beam_fork: max_len=%d must lie in [0, tail_cap=%d], row_bytes=%d a multiple of 16", max_len,
+                 tail_cap, row_bytes);
+  if (max_len == 0) return B200_OK;
+  const int row_vec = row_bytes / 16;
+  const long long per = (long long)max_len * row_vec;
+  const int bx = (int)(per < 64 * 256 ? (per + 255) / 256 : 64);
+  kv_beam_fork_kernel<<<dim3(bx, n_copies, n_bufs), 256, 0, static_cast<cudaStream_t>(stream)>>>(bufs, copies,
+                                                                                               tail_cap, row_vec);
   B200_CHECK_LAUNCH();
   return B200_OK;
 }

@@ -1295,6 +1295,126 @@ def kv_append_ring(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_ring: to
 
 
 # ------------------------------------------------------------------------------------------------
+# beam search over a shared-prompt cache (DESIGN §4.2.4): per layer, the groups' prefix caches [G, s_prefix, Hk, D]
+# and the beam tails [S, tail_cap, Hk, D]; `tables` is one int32 device tensor holding, for R rows and G groups,
+# [row_group (R) | row_slot (R) | grp_t0 (G) | grp_row0 (G) | grp_rows (G)]
+# ------------------------------------------------------------------------------------------------
+def attention_decode_beam_workspace_bytes(R: int, H: int, s_prefix: int, tail_cap: int, D: int) -> int:
+    return int(lib().b200_attn_decode_beam_workspace_bytes(R, H, s_prefix, tail_cap, D))
+
+
+def attention_decode_beam_pack(H: int, Hk: int, D: int) -> int:
+    """Beam rows of a group that share one read of a prefix chunk."""
+    return int(lib().b200_attn_decode_beam_pack(H, Hk, D))
+
+
+def _check_beam_tables(tables: torch.Tensor, R: int, G: int, device, what: str) -> None:
+    if not isinstance(tables, torch.Tensor) or tables.dtype != torch.int32 or tables.device != device \
+            or not tables.is_contiguous() or tables.numel() != 2 * R + 3 * G:
+        raise ValueError(f"{what}: tables must be a contiguous int32 [2 R + 3 G] = [{2 * R + 3 * G}] tensor on {device}")
+
+
+def attention_decode_beam(q: torch.Tensor, k_prefix: torch.Tensor, v_prefix: torch.Tensor, k_tail: torch.Tensor,
+                          v_tail: torch.Tensor, lens: torch.Tensor, tables: torch.Tensor,
+                          scale: Optional[float] = None, workspace: Optional[torch.Tensor] = None,
+                          return_lse: bool = False, window: Optional[int] = None,
+                          alibi: Optional[torch.Tensor] = None):
+    """attention_decode for beam rows over a shared-prompt cache (b200_attn_decode_beam): row b's query at position
+    p = lens[b] - 1 sees keys t < T0 from its group's prefix cache and keys T0 <= t <= p from index t - T0 of its tail
+    slot (tables above).  q [R,H,D]; k_prefix, v_prefix [G,s_prefix,Hk,D]; k_tail, v_tail [S,tail_cap,Hk,D]; all bf16
+    or all fp32, D in {16, 32, 64, 128}, s_prefix and tail_cap multiples of 256.  window and alibi as in
+    attention_decode.  The table values are not checked here (that would read the device)."""
+    what = "attention_decode_beam"
+    _is_bf16(q, "q")
+    for t, nm in ((q, "q"), (k_prefix, "k_prefix"), (v_prefix, "v_prefix"), (k_tail, "k_tail"), (v_tail, "v_tail")):
+        _need(t, q.dtype, f"{what}: {nm}")
+    if q.dim() != 3 or k_prefix.dim() != 4 or k_prefix.shape != v_prefix.shape or k_tail.dim() != 4 \
+            or k_tail.shape != v_tail.shape or k_prefix.shape[2:] != k_tail.shape[2:]:
+        raise ValueError(f"{what}: expected q [R,H,D], prefix [G,s_prefix,Hk,D] and tails [S,tail_cap,Hk,D], got "
+                         f"{tuple(q.shape)}, {tuple(k_prefix.shape)}, {tuple(k_tail.shape)}")
+    R, H, D = q.shape
+    G, s_prefix, Hk, Dc = k_prefix.shape
+    S, tail_cap = k_tail.shape[:2]
+    if Dc != D or H % Hk != 0 or D not in (16, 32, 64, 128):
+        raise ValueError(f"{what}: q {tuple(q.shape)} does not match the caches {tuple(k_prefix.shape)} "
+                         f"(head_dim 16, 32, 64 or 128)")
+    _check_rows(lens, R, q.device, what, "lens")
+    _check_beam_tables(tables, R, G, q.device, what)
+    if window is not None:
+        window = _check_window(window, what)
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, True, what)
+    if scale is None:
+        scale = D ** -0.5
+    need = attention_decode_beam_workspace_bytes(R, H, s_prefix, tail_cap, D)
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
+    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need \
+            or workspace.data_ptr() % 128:
+        raise ValueError(f"{what}: workspace must be 128-byte aligned uint8 on {q.device} with >= {need} bytes")
+    o = torch.empty_like(q)
+    lse = torch.empty((R, H), device=q.device, dtype=torch.float32) if return_lse else None
+    tok = _t0("attn_decode_beam")
+    check(lib().b200_attn_decode_beam(q.data_ptr(), k_prefix.data_ptr(), v_prefix.data_ptr(), k_tail.data_ptr(),
+                                      v_tail.data_ptr(), lens.data_ptr(), tables.data_ptr(), o.data_ptr(), _ptr(lse),
+                                      -1 if window is None else int(window), _ptr(alibi), R, G, s_prefix, S, tail_cap,
+                                      H, Hk, D, float(scale), _is_bf16(q, "q"), workspace.data_ptr(),
+                                      workspace.numel(), _stream()), "b200_attn_decode_beam")
+    _t1(tok)
+    return (o, lse) if return_lse else o
+
+
+def kv_append_beam(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_tail: torch.Tensor, v_tail: torch.Tensor,
+                   lens: torch.Tensor, tables: torch.Tensor, n_groups: int,
+                   rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                   layout: str = "interleaved") -> None:
+    """kv_append into the beam tails (b200_kv_append_beam): k (rotated at position lens[b] - 1 with rope_tables, as
+    is q in place) and v go to index lens[b] - 1 - T0 of row b's tail slot."""
+    what = "kv_append_beam"
+    _check_choice(layout, ROPE_LAYOUTS, f"{what}: layout")
+    _is_bf16(q, "q")
+    for t, nm in ((q, "q"), (k, "k"), (v, "v"), (k_tail, "k_tail"), (v_tail, "v_tail")):
+        _need(t, q.dtype, f"{what}: {nm}")
+    R, H, D = q.shape
+    if k_tail.dim() != 4 or k_tail.shape != v_tail.shape or k_tail.shape[3] != D or H % k_tail.shape[2]:
+        raise ValueError(f"{what}: tails {tuple(k_tail.shape)} do not match q {tuple(q.shape)}")
+    tail_cap, Hk = k_tail.shape[1], k_tail.shape[2]
+    for t, nm in ((k, "k"), (v, "v")):
+        if t.shape != (R, Hk, D):
+            raise ValueError(f"{what}: {nm} must be [{R},{Hk},{D}], got {tuple(t.shape)}")
+    _check_rows(lens, R, q.device, what, "lens")
+    _check_beam_tables(tables, R, n_groups, q.device, what)
+    cos_t = sin_t = None
+    if rope_tables is not None:
+        cos_t, sin_t = rope_tables
+        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
+            _need(t, torch.float32, f"{what}: {nm}")
+            if t.dim() != 2 or t.shape[1] != D // 2:
+                raise ValueError(f"{what}: RoPE tables must be [positions, {D // 2}]")
+    half = int(layout == "half" and cos_t is not None)
+    check(lib().b200_kv_append_beam(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_tail.data_ptr(), v_tail.data_ptr(),
+                                    lens.data_ptr(), tables.data_ptr(), _ptr(cos_t), _ptr(sin_t), half, R,
+                                    tail_cap, H, Hk, D, _is_bf16(q, "q"), _stream()), "b200_kv_append_beam")
+
+
+def kv_beam_fork(buffers: torch.Tensor, copies: torch.Tensor, max_len: int, tails: Sequence[torch.Tensor]) -> None:
+    """Copy-on-fork (b200_kv_beam_fork): copies int32 [n, 3] on the device = (src slot, dst slot, positions) copies
+    tail indices [0, positions) from slot src to slot dst in every tail of `tails` (each [S, tail_cap, Hk, D]);
+    buffers: int64 device tensor of their data pointers.  max_len >= every copy's positions.  No copies: nothing."""
+    n = copies.shape[0] if copies.dim() == 2 else 0
+    if n == 0:
+        return
+    t0 = tails[0]
+    if copies.dtype != torch.int32 or copies.shape[1] != 3 or not copies.is_contiguous() or copies.device != t0.device:
+        raise ValueError("kv_beam_fork: copies must be a contiguous int32 [n, 3] tensor on the tails' device")
+    if buffers.dtype != torch.int64 or buffers.numel() != len(tails) or buffers.device != t0.device:
+        raise ValueError("kv_beam_fork: buffers must be an int64 device tensor of the tails' pointers")
+    row_bytes = t0.shape[2] * t0.shape[3] * t0.element_size()
+    check(lib().b200_kv_beam_fork(buffers.data_ptr(), len(tails), copies.data_ptr(), n, int(max_len), t0.shape[1],
+                                  row_bytes, _stream()), "b200_kv_beam_fork")
+
+
+# ------------------------------------------------------------------------------------------------
 # the quantized KV cache (the reference's kv_bits / kv_group_size; DESIGN §4.2.1): per layer, codes uint8
 # [B, s_max, Hk, D * bits / 8] and parameters fp32 [B, Hk, s_max, D / group_size, 2] for each of K and V
 # ------------------------------------------------------------------------------------------------
