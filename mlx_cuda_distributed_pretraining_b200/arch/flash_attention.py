@@ -104,6 +104,47 @@ class PrefixCausalMask:
         return m[:, None]
 
 
+# -- one layer's KV cache, one class per format --------------------------------------------------------------------
+# Each format owns its buffers and the ops calls that write and read them, for the generation phases it serves:
+#   store(k, v)                                       prefill: k, v [B, S, Hk, D] into positions [0, S)
+#   decode(q, k, v, step, attn, window, rope_layout)  q [B, H, D], k, v [B, Hk, D] appended at step.lens - 1 (rotated
+#                                                     there with attn.rope_tables), then attended -> ctx [B, H, D]
+#   extend(q, k, v, chunk, attn, window)              a llama.CacheChunk's rotated q [B, L, H, D], k, v [B, L, Hk, D]
+#                                                     written, then attended -> ctx [B, L, H, D]
+# step is the model-wide cache (llama.KVCache / BeamKVCache), which holds the per-step state: lens, workspace and,
+# per format, the ring's live mask or the beam tables.  attn is the FlashAttention module: scale, rope_tables and
+# alibi_slopes().
+def _nbytes(*tensors) -> int:
+    return sum(t.numel() * t.element_size() for t in tensors)
+
+
+class DenseKV:
+    """One layer's K and V [B, s_max, Hk, D] in the model's activation dtype."""
+
+    def __init__(self, k: torch.Tensor, v: torch.Tensor):
+        self.k, self.v = k, v
+
+    def nbytes(self) -> int:
+        return _nbytes(self.k, self.v)
+
+    def store(self, k: torch.Tensor, v: torch.Tensor) -> None:
+        S = k.shape[1]
+        self.k[:, :S].copy_(k)
+        self.v[:, :S].copy_(v)
+
+    def decode(self, q, k, v, step, attn, window, rope_layout):
+        ops.kv_append(q, k, v, self.k, self.v, step.lens, attn.rope_tables, layout=rope_layout)
+        return ops.attention_decode(q, self.k, self.v, step.lens, attn.scale, step.workspace, window=window,
+                                    alibi=attn.alibi_slopes(q.device))
+
+    def extend(self, q, k, v, chunk, attn, window):
+        r, src, dst = chunk.rows, chunk.src, chunk.dst
+        self.k[r, dst] = k[r, src]
+        self.v[r, dst] = v[r, src]
+        return ops.attention_cached(q, self.k, self.v, chunk.start, chunk.end, attn.scale, window=window,
+                                    alibi=attn.alibi_slopes(q.device))
+
+
 class QuantizedKV:
     """One layer's quantized KV cache (the reference's QuantizedKVCache; DESIGN §4.2.1): for K and for V, codes uint8
     [B, s_max, Hk, D * bits / 8] and fp32 (scale, bias) parameters [B, Hk, s_max, D / group_size, 2]."""
@@ -122,25 +163,90 @@ class QuantizedKV:
         return self.k_codes, self.v_codes, self.k_params, self.v_params
 
     def nbytes(self) -> int:
-        return sum(t.numel() * t.element_size() for t in self.buffers())
+        return _nbytes(*self.buffers())
+
+    def store(self, k: torch.Tensor, v: torch.Tensor, n: Optional[int] = None) -> None:
+        """Quantizes positions [0, n) (default: all) of k, v [B, S, Hk, D]: a prefill, or the conversion of a
+        DenseKV's buffers."""
+        ops.kv_quantize(k.contiguous(), v.contiguous(), *self.buffers(), self.bits, self.group_size, n=n)
+
+    def decode(self, q, k, v, step, attn, window, rope_layout):
+        bits, g = self.bits, self.group_size
+        ops.kv_append_quant(q, k, v, *self.buffers(), step.lens, bits, g, attn.rope_tables, layout=rope_layout)
+        return ops.attention_decode_quant(q, *self.buffers(), step.lens, bits, g, attn.scale, step.workspace,
+                                          window=window, alibi=attn.alibi_slopes(q.device))
+
+    def extend(self, q, k, v, chunk, attn, window):
+        """The chunk is quantized into a temporary cache and its valid positions copied in; the queries then attend
+        over the cache's dequantised [0, end) in chunk.scratch (bf16 K / V made by the call's first layer)."""
+        B, L, Hk, D = k.shape
+        bits, g = self.bits, self.group_size
+        r, src, dst = chunk.rows, chunk.src, chunk.dst
+        tmp = QuantizedKV(B, L + L % 2, Hk, D, bits, g, k.device)
+        ops.kv_quantize(k, v, *tmp.buffers(), bits, g)
+        for t, u in zip(self.buffers()[:2], tmp.buffers()[:2]):
+            t[r, dst] = u[r, src]
+        for t, u in zip(self.buffers()[2:], tmp.buffers()[2:]):
+            t[r, :, dst] = u[r, :, src]
+        if chunk.scratch is None:
+            shape = (B, chunk.max_end, Hk, D)
+            chunk.scratch = (torch.empty(shape, device=k.device, dtype=torch.bfloat16),
+                             torch.empty(shape, device=k.device, dtype=torch.bfloat16))
+        k_att, v_att = ops.kv_dequantize(*self.buffers(), chunk.end, bits, g, out=chunk.scratch)
+        return ops.attention_cached(q, k_att, v_att, chunk.start, chunk.end, attn.scale, window=window,
+                                    alibi=attn.alibi_slopes(q.device))
 
 
 class RingKV:
     """One layer's rotating KV cache (mlx_lm's RotatingKVCache; DESIGN §4.2.3): K and V rings bf16 [B, C, Hk, D],
-    position t in slot ops.ring_slot(t, C), read under max_kv_size.  live: the cache's int32 [B] mask of rows a decode
-    step appends to (None: all)."""
+    position t in slot ops.ring_slot(t, C), read under max_kv_size.  Filled by extend only (chunk.dst are ring
+    slots); a decode step appends to the rows of step.live (int32 [B], None: all)."""
 
-    def __init__(self, k: torch.Tensor, v: torch.Tensor, max_kv_size: int, live: Optional[torch.Tensor] = None):
-        self.k, self.v, self.max_kv_size, self.live = k, v, max_kv_size, live
+    def __init__(self, k: torch.Tensor, v: torch.Tensor, max_kv_size: int):
+        self.k, self.v, self.max_kv_size = k, v, max_kv_size
+
+    def nbytes(self) -> int:
+        return _nbytes(self.k, self.v)
+
+    def decode(self, q, k, v, step, attn, window, rope_layout):
+        ops.kv_append_ring(q, k, v, self.k, self.v, step.lens, step.live, attn.rope_tables, rope_layout)
+        return ops.attention_decode_ring(q, self.k, self.v, step.lens, self.max_kv_size, attn.scale, step.workspace,
+                                         window=window, alibi=attn.alibi_slopes(q.device))
+
+    def extend(self, q, k, v, chunk, attn, window):
+        r, src, dst = chunk.rows, chunk.src, chunk.dst
+        self.k[r, dst] = k[r, src]
+        self.v[r, dst] = v[r, src]
+        return ops.attention_ring(q, self.k, self.v, chunk.start, chunk.end, self.max_kv_size, attn.scale,
+                                  window=window, alibi=attn.alibi_slopes(q.device))
 
 
 class BeamKV:
-    """One layer of a beam search's cache (llama.BeamKVCache; DESIGN §4.2.4): the groups' prefix K / V [G, s_prefix,
-    Hk, D], the beam tails [S, tail_cap, Hk, D] and the cache's int32 device tables (ops.attention_decode_beam)."""
+    """One layer of a beam search's cache (llama.BeamKVCache; DESIGN §4.2.4): the DenseKV `prefix` [G, s_prefix, Hk,
+    D] holding the G prompts, and beam tails k_tail, v_tail [G n_beams, tail_cap, Hk, D].  Group g's positions
+    [t0[g], lens[g]) start at index 0 of slot g n_beams.  Decode only; step.tables are the cache's int32 device
+    tables (ops.attention_decode_beam)."""
 
-    def __init__(self, k_prefix, v_prefix, k_tail, v_tail, tables: torch.Tensor, n_groups: int):
-        self.k_prefix, self.v_prefix, self.k_tail, self.v_tail = k_prefix, v_prefix, k_tail, v_tail
-        self.tables, self.n_groups = tables, n_groups
+    def __init__(self, prefix: DenseKV, n_beams: int, tail_cap: int, t0, lens):
+        self.prefix, self.n_groups = prefix, len(t0)
+        p = prefix.k
+        shape = (self.n_groups * n_beams, tail_cap) + tuple(p.shape[2:])
+        self.k_tail = torch.zeros(shape, device=p.device, dtype=p.dtype)
+        self.v_tail = torch.zeros(shape, device=p.device, dtype=p.dtype)
+        for g, (s, n) in enumerate(zip(t0, lens)):
+            self.k_tail[g * n_beams, :n - s].copy_(prefix.k[g, s:n])
+            self.v_tail[g * n_beams, :n - s].copy_(prefix.v[g, s:n])
+
+    def nbytes(self) -> int:
+        """Bytes of the tails (the prefix belongs to its own cache)."""
+        return _nbytes(self.k_tail, self.v_tail)
+
+    def decode(self, q, k, v, step, attn, window, rope_layout):
+        ops.kv_append_beam(q, k, v, self.k_tail, self.v_tail, step.lens, step.tables, self.n_groups,
+                           attn.rope_tables, rope_layout)
+        return ops.attention_decode_beam(q, self.prefix.k, self.prefix.v, self.k_tail, self.v_tail, step.lens,
+                                         step.tables, attn.scale, step.workspace, window=window,
+                                         alibi=attn.alibi_slopes(q.device))
 
 
 class FlashAttention(nn.Module):
@@ -218,18 +324,27 @@ class FlashAttention(nn.Module):
                           dropout=p, seed=seed)
         return o if dt == torch.bfloat16 else o.to(dt)
 
-    def forward(self, x: torch.Tensor, mask=None, rope_layout: str = "interleaved",
-                dropout_seed: Optional[int] = None) -> torch.Tensor:
-        """rope_layout: ops.rope's pair layout when RoPE is on ("interleaved" or mlx_lm's "half").  dropout_seed: the
-        model's per-step dropout base (see drops() for when it applies)."""
-        B, S, _ = x.shape
+    def _qkv(self, x: torch.Tensor):
+        """q [..., H, D] and k, v [..., Hk, D] projected from x [..., hidden]."""
+        lead = x.shape[:-1]
         if self.q_proj.bias is None and self.k_proj.bias is None and self.v_proj.bias is None:
             q, k, v = ops.multi_linear(x, (self.q_proj.weight, self.k_proj.weight, self.v_proj.weight))
         else:
             q, k, v = self.q_proj(x), self.k_proj(x), self.v_proj(x)
-        q = q.reshape(B, S, self.num_heads, self.head_dim)
-        k = k.reshape(B, S, self.num_kv_heads, self.head_dim)
-        v = v.reshape(B, S, self.num_kv_heads, self.head_dim)
+        return (q.reshape(*lead, self.num_heads, self.head_dim), k.reshape(*lead, self.num_kv_heads, self.head_dim),
+                v.reshape(*lead, self.num_kv_heads, self.head_dim))
+
+    def _out(self, ctx: torch.Tensor) -> torch.Tensor:
+        """o_proj of ctx [..., H, D]."""
+        ctx = ctx.reshape(*ctx.shape[:-2], self.num_heads * self.head_dim)
+        return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
+
+    def forward(self, x: torch.Tensor, mask=None, rope_layout: str = "interleaved",
+                dropout_seed: Optional[int] = None) -> torch.Tensor:
+        """rope_layout: ops.rope's pair layout when RoPE is on ("interleaved" or mlx_lm's "half").  dropout_seed: the
+        model's per-step dropout base (see drops() for when it applies)."""
+        S = x.shape[1]
+        q, k, v = self._qkv(x)
         if self.rope_tables is not None:
             cos_t, sin_t = self.rope_tables
             pos = mask.pos if isinstance(mask, DocumentCausalMask) else None  # packed rows: position in document
@@ -238,118 +353,40 @@ class FlashAttention(nn.Module):
         # the dropout arguments go only to dropping calls: without them the call is exactly the dropout-free one
         ctx = (self._flash_attention(q, k, v, mask, dropout_seed, True) if self.drops()
                else self._flash_attention(q, k, v, mask))
-        ctx = ctx.reshape(B, S, self.num_heads * self.head_dim)
-        return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
+        return self._out(ctx)
 
-    # -- generation: the same layer against a KV cache ([B, s_max, Hk, D] K and V buffers) ----------------------
-    def _project(self, x: torch.Tensor):
-        if self.q_proj.bias is None and self.k_proj.bias is None and self.v_proj.bias is None:
-            return ops.multi_linear(x, (self.q_proj.weight, self.k_proj.weight, self.v_proj.weight))
-        return self.q_proj(x), self.k_proj(x), self.v_proj(x)
-
-    def _out(self, ctx: torch.Tensor) -> torch.Tensor:
-        return ops.linear(ctx, self.o_proj.weight) if self.o_proj.bias is None else self.o_proj(ctx)
-
-    def forward_prefill(self, x: torch.Tensor, mask, k_cache, v_cache: Optional[torch.Tensor],
-                        rope_layout: str = "interleaved") -> torch.Tensor:
+    # -- generation: the same layer against one layer of a KV cache (a DenseKV, QuantizedKV, RingKV or BeamKV) ------
+    def forward_prefill(self, x: torch.Tensor, mask, kv, rope_layout: str = "interleaved") -> torch.Tensor:
         """forward(x, mask) over a right-padded prompt batch x [B, S, hidden] that also stores the (rotated) keys and
-        values in cache positions [0, S): in the k_cache and v_cache tensors, or quantized into k_cache when it is a
-        QuantizedKV (v_cache None).  Attention runs through _flash_attention on the unquantized k and v, so the
-        numerics are the training forward's."""
-        B, S, _ = x.shape
-        q, k, v = self._project(x)
-        q = q.reshape(B, S, self.num_heads, self.head_dim)
-        k = k.reshape(B, S, self.num_kv_heads, self.head_dim)
-        v = v.reshape(B, S, self.num_kv_heads, self.head_dim)
+        values in positions [0, S) of kv (kv.store).  Attention runs through _flash_attention on the unquantized k and
+        v, so the numerics are the training forward's."""
+        S = x.shape[1]
+        q, k, v = self._qkv(x)
         if self.rope_tables is not None:
             cos_t, sin_t = self.rope_tables
             q = ops.rope(q, cos_t[:S], sin_t[:S], layout=rope_layout)
             k = ops.rope(k, cos_t[:S], sin_t[:S], layout=rope_layout)
-        if isinstance(k_cache, QuantizedKV):
-            ops.kv_quantize(k.contiguous(), v.contiguous(), *k_cache.buffers(), k_cache.bits, k_cache.group_size)
-        else:
-            k_cache[:, :S].copy_(k)
-            v_cache[:, :S].copy_(v)
-        ctx = self._flash_attention(q, k, v, mask)
-        return self._out(ctx.reshape(B, S, self.num_heads * self.head_dim))
+        kv.store(k, v)
+        return self._out(self._flash_attention(q, k, v, mask))
 
-    def forward_decode(self, x: torch.Tensor, k_cache, v_cache: Optional[torch.Tensor], lens: torch.Tensor,
-                       workspace: torch.Tensor, window: Optional[int] = None,
+    def forward_decode(self, x: torch.Tensor, kv, step, window: Optional[int] = None,
                        rope_layout: str = "interleaved") -> torch.Tensor:
-        """One new token per row, x [B, hidden]: its k and v go to cache position lens[b] - 1 (rotated there when
-        RoPE is on), then its query attends over the row's first lens[b] cached keys (the last window + 1 of them
-        with a sliding window), with the ALiBi bias when the module has it.  k_cache is a QuantizedKV (v_cache None)
-        for a quantized cache, a BeamKV (v_cache None) for a beam search's rows."""
-        B = x.shape[0]
-        q, k, v = self._project(x)
-        q = q.reshape(B, self.num_heads, self.head_dim).contiguous()
-        k = k.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
-        v = v.reshape(B, self.num_kv_heads, self.head_dim).contiguous()
-        if isinstance(k_cache, BeamKV):
-            c = k_cache
-            ops.kv_append_beam(q, k, v, c.k_tail, c.v_tail, lens, c.tables, c.n_groups, self.rope_tables, rope_layout)
-            ctx = ops.attention_decode_beam(q, c.k_prefix, c.v_prefix, c.k_tail, c.v_tail, lens, c.tables, self.scale,
-                                            workspace, window=window, alibi=self.alibi_slopes(q.device))
-            return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
-        if isinstance(k_cache, RingKV):
-            ops.kv_append_ring(q, k, v, k_cache.k, k_cache.v, lens, k_cache.live, self.rope_tables, rope_layout)
-            ctx = ops.attention_decode_ring(q, k_cache.k, k_cache.v, lens, k_cache.max_kv_size, self.scale, workspace,
-                                            window=window, alibi=self.alibi_slopes(q.device))
-            return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
-        if isinstance(k_cache, QuantizedKV):
-            bits, g = k_cache.bits, k_cache.group_size
-            ops.kv_append_quant(q, k, v, *k_cache.buffers(), lens, bits, g, self.rope_tables, layout=rope_layout)
-            ctx = ops.attention_decode_quant(q, *k_cache.buffers(), lens, bits, g, self.scale, workspace,
-                                             window=window, alibi=self.alibi_slopes(q.device))
-            return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
-        ops.kv_append(q, k, v, k_cache, v_cache, lens, self.rope_tables, layout=rope_layout)
-        ctx = ops.attention_decode(q, k_cache, v_cache, lens, self.scale, workspace, window=window,
-                                   alibi=self.alibi_slopes(q.device))
-        return self._out(ctx.reshape(B, self.num_heads * self.head_dim))
+        """One new token per row, x [B, hidden]: its k and v go to cache position step.lens[b] - 1 (rotated there
+        when RoPE is on), then its query attends over the row's first lens[b] cached keys (the last window + 1 of them
+        with a sliding window), with the ALiBi bias when the module has it (kv.decode; step: the model-wide cache)."""
+        q, k, v = (t.contiguous() for t in self._qkv(x))
+        return self._out(kv.decode(q, k, v, step, self, window, rope_layout))
 
-    def forward_extend(self, x: torch.Tensor, k_cache, v_cache: Optional[torch.Tensor], chunk,
-                       window: Optional[int] = None, rope_layout: str = "interleaved") -> torch.Tensor:
+    def forward_extend(self, x: torch.Tensor, kv, chunk, window: Optional[int] = None,
+                       rope_layout: str = "interleaved") -> torch.Tensor:
         """A chunk of new tokens per row, x [B, L, hidden] right-padded, appended at each row's current cache length
         (chunk: the llama.CacheChunk of the call).  Token i of row b sits at position p = chunk.start[b] + i: its q
-        and k are rotated there (ops.rope at absolute positions), its k and v are written to that cache position
-        (quantized first when k_cache is a QuantizedKV, v_cache None), and its query attends over the row's cached
-        keys max(0, p - window) .. p (ops.attention_cached), over the cache's dequantised values once it is
-        quantized.  For a RingKV (v_cache None) chunk.dst are ring slots and the keys are those of
-        ops.attention_ring."""
-        B, L, _ = x.shape
-        q, k, v = self._project(x)
-        q = q.reshape(B, L, self.num_heads, self.head_dim)
-        k = k.reshape(B, L, self.num_kv_heads, self.head_dim)
-        v = v.reshape(B, L, self.num_kv_heads, self.head_dim)
+        and k are rotated there (ops.rope at absolute positions), then kv.extend writes its k and v to the cache and
+        its query attends over the row's cached keys up to p (max(0, p - window) .. p with a sliding window)."""
+        q, k, v = self._qkv(x)
         if self.rope_tables is not None:
             cos_t, sin_t = self.rope_tables
             q = ops.rope(q, cos_t, sin_t, chunk.pos, rope_layout)
             k = ops.rope(k, cos_t, sin_t, chunk.pos, rope_layout)
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        r, src, dst = chunk.rows, chunk.src, chunk.dst
-        if isinstance(k_cache, RingKV):
-            k_cache.k[r, dst] = k[r, src]
-            k_cache.v[r, dst] = v[r, src]
-            ctx = ops.attention_ring(q, k_cache.k, k_cache.v, chunk.start, chunk.end, k_cache.max_kv_size, self.scale,
-                                     window=window, alibi=self.alibi_slopes(q.device))
-            return self._out(ctx.reshape(B, L, self.num_heads * self.head_dim))
-        if isinstance(k_cache, QuantizedKV):
-            bits, g = k_cache.bits, k_cache.group_size
-            tmp = QuantizedKV(B, L + L % 2, self.num_kv_heads, self.head_dim, bits, g, x.device)
-            ops.kv_quantize(k, v, *tmp.buffers(), bits, g)
-            for t, u in zip(k_cache.buffers()[:2], tmp.buffers()[:2]):
-                t[r, dst] = u[r, src]
-            for t, u in zip(k_cache.buffers()[2:], tmp.buffers()[2:]):
-                t[r, :, dst] = u[r, :, src]
-            if chunk.scratch is None:  # one layer's bf16 K / V, reused by every layer of the call
-                shape = (B, chunk.max_end, self.num_kv_heads, self.head_dim)
-                chunk.scratch = (torch.empty(shape, device=x.device, dtype=torch.bfloat16),
-                                 torch.empty(shape, device=x.device, dtype=torch.bfloat16))
-            k_att, v_att = ops.kv_dequantize(*k_cache.buffers(), chunk.end, bits, g, out=chunk.scratch)
-        else:
-            k_cache[r, dst] = k[r, src]
-            v_cache[r, dst] = v[r, src]
-            k_att, v_att = k_cache, v_cache
-        ctx = ops.attention_cached(q, k_att, v_att, chunk.start, chunk.end, self.scale, window=window,
-                                   alibi=self.alibi_slopes(q.device))
-        return self._out(ctx.reshape(B, L, self.num_heads * self.head_dim))
+        return self._out(kv.extend(q, k, v, chunk, self, window))

@@ -26,8 +26,8 @@ import torch
 from torch import nn
 
 from .. import ops
-from .flash_attention import (BeamKV, CausalMask, DocumentCausalMask, FlashAttention, PrefixCausalMask, QuantizedKV,
-                              RingKV)
+from .flash_attention import (BeamKV, CausalMask, DenseKV, DocumentCausalMask, FlashAttention, PrefixCausalMask,
+                              QuantizedKV, RingKV)
 
 VARIANTS = (None, "reference", "mlx_lm")
 
@@ -174,13 +174,13 @@ class AttentionModule(nn.Module):
         prefix lengths."""
         if self.apply_rope and self.attn.rope_tables is None:
             self.attn.rope_tables = ops.rope_tables(self.max_positions, self.head_dim, self.rope_theta, x.device)
+        kv = cache.layer(layer)
         if chunk is not None:
-            return self.attn.forward_extend(x, *cache.layer(layer), chunk, window, self.rope_layout)
+            return self.attn.forward_extend(x, kv, chunk, window, self.rope_layout)
         if x.dim() == 3:
             mask = CausalMask(x.shape[1], window) if prefix is None else PrefixCausalMask(prefix, x.shape[1])
-            return self.attn.forward_prefill(x, mask, *cache.layer(layer), self.rope_layout)
-        return self.attn.forward_decode(x, *cache.layer(layer), cache.lens, cache.workspace, window,
-                                        self.rope_layout)
+            return self.attn.forward_prefill(x, mask, kv, self.rope_layout)
+        return self.attn.forward_decode(x, kv, cache, window, self.rope_layout)
 
 
 class TransformerBlock(nn.Module):
@@ -248,17 +248,40 @@ class TransformerBlock(nn.Module):
         return h, self._ffn(y)
 
 
+def check_cache_options(model: "Model", kv_bits: Optional[int] = None, kv_group_size: int = 64,
+                        quantized_kv_start: int = 0, max_kv_size: Optional[int] = None, what: str = "KVCache",
+                        head_dim: Optional[int] = None) -> None:
+    """Raises ValueError, naming `what`, for KV-cache options KVCache cannot serve: a bad max_kv_size, a rotating cache
+    with kv_bits, for a prefix-LM model or for a model Model.extend cannot serve, and bad kv_bits / kv_group_size
+    (given head_dim, one that does not divide it) or quantized_kv_start.  The model is read only for a rotating
+    cache."""
+    if max_kv_size is not None:
+        ops.check_max_kv_size(max_kv_size, what)
+        if kv_bits is not None:
+            raise ValueError(f"{what}: max_kv_size does not combine with kv_bits (mlx_lm's rotating cache does not "
+                             "quantize)")
+        if model.args.prefix_lm:
+            raise ValueError(f"{what}: a prefix-LM model cannot use a rotating cache (max_kv_size): its prompt is one "
+                             "prefix")
+        model.check_extend(None)
+    if kv_bits is not None:
+        ops.check_kv_quant(kv_bits, kv_group_size, head_dim, what)
+        if isinstance(quantized_kv_start, bool) or not isinstance(quantized_kv_start, int) or quantized_kv_start < 0:
+            raise ValueError(f"{what}: quantized_kv_start must be a non-negative int, got {quantized_kv_start!r}")
+
+
 class KVCache:
-    """Per-layer K and V buffers [B, s_max, Hk, D] in the model's activation dtype, and the number of valid positions
-    per row: `lens` on the device (read by the kernels) and `host_lens` (so sizing a launch never reads the device).
-    s_max is rounded up to a multiple of 256, the decode kernel's chunk.
+    """Per-layer KV caches (`layers`, one DenseKV, QuantizedKV or RingKV per layer; flash_attention) and the number of
+    valid positions per row: `lens` on the device (read by the kernels) and `host_lens` (so sizing a launch never
+    reads the device).  A DenseKV holds K and V [B, s_max, Hk, D] in the model's activation dtype.  s_max is rounded
+    up to a multiple of 256, the decode kernel's chunk.
 
     kv_bits (4 or 8), kv_group_size (32, 64 or 128) and quantized_kv_start are the reference's quantized cache
     (core/generation_lite.py:75-90, :100-108): once the longest row holds more than quantized_kv_start positions,
     after prefill or after a decode step, every layer converts to a QuantizedKV and the unquantized buffers are
     released.  When the prompt already passes the start, prefill writes the quantized cache directly and no
     unquantized buffer is ever allocated; otherwise those buffers hold quantized_kv_start + 1 positions (rounded up to
-    256), all they can hold before conversion.  The buffers are allocated by the first set_lengths (prefill).
+    256), all they can hold before conversion.  The layers are allocated by the first set_lengths (prefill).
 
     max_kv_size = M (an int >= 5) makes the cache rotate, as the reference's make_prompt_cache(model, max_kv_size)
     (core/generation_lite.py:103, :120) gives every layer mlx_lm's RotatingKVCache(max_size=M, keep=4): each row keeps
@@ -271,41 +294,29 @@ class KVCache:
     max_kv_size: Optional[int] = None
     max_chunk: Optional[int] = None
     live: Optional[torch.Tensor] = None  # rotating: the rows the current decode step appends to (None: all)
-    _rings = None  # rotating: the layers' RingKV views
 
     def __init__(self, model: "Model", batch: int, s_max: int, kv_bits: Optional[int] = None,
                  kv_group_size: int = 64, quantized_kv_start: int = 0, max_kv_size: Optional[int] = None,
                  max_chunk: Optional[int] = None):
         a = model.args
         attn = model.layers[0].self_attn
+        check_cache_options(model, kv_bits, kv_group_size, quantized_kv_start, max_kv_size, "KVCache", attn.head_dim)
         self.max_kv_size = max_kv_size
         self.max_chunk = max_chunk
         if max_kv_size is not None:
-            ops.check_max_kv_size(max_kv_size, "KVCache")
-            if kv_bits is not None:
-                raise ValueError("KVCache: max_kv_size does not combine with kv_bits (mlx_lm's rotating cache does "
-                                 "not quantize)")
-            if a.prefix_lm:
-                raise ValueError("KVCache: a prefix-LM model cannot use a rotating cache (its prompt is one prefix)")
-            model.check_extend(None)
             self.max_chunk = 512 if max_chunk is None else max_chunk
             if isinstance(self.max_chunk, bool) or not isinstance(self.max_chunk, int) or self.max_chunk < 1:
                 raise ValueError(f"KVCache: max_chunk must be an int >= 1, got {max_chunk!r}")
             s_max = max_kv_size + self.max_chunk - 1
         elif max_chunk is not None:
             raise ValueError("KVCache: max_chunk is for a rotating cache (max_kv_size)")
-        if kv_bits is not None:
-            ops.check_kv_quant(kv_bits, kv_group_size, attn.head_dim, "KVCache")
-            if isinstance(quantized_kv_start, bool) or not isinstance(quantized_kv_start, int) \
-                    or quantized_kv_start < 0:
-                raise ValueError(f"quantized_kv_start must be a non-negative int, got {quantized_kv_start!r}")
         self.kv_bits, self.kv_group_size, self.quantized_kv_start = kv_bits, kv_group_size, quantized_kv_start
         w = model.embed_tokens.weight
         self._layers, self._device, self._dtype = a.num_hidden_layers, w.device, w.dtype
         self._batch, self._heads = batch, (attn.num_kv_heads, attn.head_dim)
         self.s_max = max(256, -(-s_max // 256) * 256)
-        self.k = self.v = None  # unquantized buffers, one per layer
-        self.quant = None       # QuantizedKV per layer once quantized
+        self.layers = None
+        self.quantized = False
         if kv_bits is None:
             self._allocate(self.s_max)
         self.lens = torch.zeros(batch, device=w.device, dtype=torch.int32)
@@ -314,31 +325,29 @@ class KVCache:
         self.workspace = torch.empty(max(nbytes, 16), device=w.device, dtype=torch.uint8)
 
     def _allocate(self, positions: int) -> None:
+        """Unquantized layers of `positions` positions: RingKV when the cache rotates, else DenseKV."""
         shape = (self._batch, positions) + self._heads
-        self.k = [torch.zeros(shape, device=self._device, dtype=self._dtype) for _ in range(self._layers)]
-        self.v = [torch.zeros(shape, device=self._device, dtype=self._dtype) for _ in range(self._layers)]
+
+        def zeros():
+            return torch.zeros(shape, device=self._device, dtype=self._dtype)
+
+        if self.rotating:
+            self.layers = [RingKV(zeros(), zeros(), self.max_kv_size) for _ in range(self._layers)]
+        else:
+            self.layers = [DenseKV(zeros(), zeros()) for _ in range(self._layers)]
 
     def _allocate_quantized(self) -> None:
-        self.quant = [QuantizedKV(self._batch, self.s_max, *self._heads, self.kv_bits, self.kv_group_size,
-                                  self._device) for _ in range(self._layers)]
-
-    @property
-    def quantized(self) -> bool:
-        return self.quant is not None
+        self.layers = [QuantizedKV(self._batch, self.s_max, *self._heads, self.kv_bits, self.kv_group_size,
+                                   self._device) for _ in range(self._layers)]
+        self.quantized = True
 
     @property
     def rotating(self) -> bool:
         return self.max_kv_size is not None
 
     def layer(self, i: int):
-        """(k, v) buffers of layer i, (QuantizedKV, None) once the cache is quantized, or (RingKV, None) when it
-        rotates."""
-        if self.rotating:
-            if self._rings is None:  # made once: a decode step calls layer() for every layer
-                self._rings = [RingKV(k, v, self.max_kv_size) for k, v in zip(self.k, self.v)]
-            self._rings[i].live = self.live
-            return self._rings[i], None
-        return (self.quant[i], None) if self.quant is not None else (self.k[i], self.v[i])
+        """Layer i's cache object (DenseKV, QuantizedKV or RingKV)."""
+        return self.layers[i]
 
     def set_lengths(self, lengths) -> None:
         if self.rotating:
@@ -347,7 +356,7 @@ class KVCache:
             raise ValueError(f"lengths must lie in [1, {self.s_max}], got {list(lengths)}")
         self.host_lens = [int(n) for n in lengths]
         self.lens.copy_(torch.tensor(self.host_lens, dtype=torch.int32))
-        if self.k is None and self.quant is None:  # kv_bits: the prefill decides the first format
+        if self.layers is None:  # kv_bits: the prefill decides the first format
             if max(self.host_lens) > self.quantized_kv_start:
                 self._allocate_quantized()
             else:
@@ -367,14 +376,15 @@ class KVCache:
                              f"({self.max_chunk}): its keys would overwrite keys its queries see")
         if not self.rotating and max(ends) > self.s_max:
             raise ValueError(f"KV cache full: rows would hold {max(ends)} positions, the cache has {self.s_max}")
-        if self.quant is None and not self.rotating:  # a ring is allocated whole by __init__
-            have = 0 if self.k is None else self.k[0].shape[1]
+        if not self.quantized and not self.rotating:  # a ring is allocated whole by __init__
+            have = 0 if self.layers is None else self.layers[0].k.shape[1]
             if max(ends) > have:
-                old_k, old_v = self.k, self.v
+                old = self.layers
                 self._allocate(min(self.s_max, -(-max(ends) // 256) * 256))
-                if old_k is not None:
-                    for new, old in zip(self.k + self.v, old_k + old_v):
-                        new[:, :have].copy_(old)
+                if old is not None:
+                    for new, o in zip(self.layers, old):
+                        new.k[:, :have].copy_(o.k)
+                        new.v[:, :have].copy_(o.v)
         self.host_start = list(self.host_lens)
         self.host_lens = ends
         self.lens.copy_(torch.tensor(ends, dtype=torch.int32))
@@ -412,54 +422,45 @@ class KVCache:
     def maybe_quantize(self) -> None:
         """maybe_quantize_kv_cache (core/generation_lite.py:75-90): with kv_bits, the first time the longest row
         holds more than quantized_kv_start positions, convert every layer and release the unquantized buffers."""
-        if self.kv_bits is None or self.quant is not None or max(self.host_lens) <= self.quantized_kv_start:
+        if self.kv_bits is None or self.quantized or max(self.host_lens) <= self.quantized_kv_start:
             return
         n = max(self.host_lens)
+        dense = self.layers
         self._allocate_quantized()
-        for k, v, qkv in zip(self.k, self.v, self.quant):
-            ops.kv_quantize(k, v, *qkv.buffers(), self.kv_bits, self.kv_group_size, n=n)
-        self.k = self.v = None
+        for d, qkv in zip(dense, self.layers):
+            qkv.store(d.k, d.v, n)
 
     def nbytes(self) -> int:
-        """Bytes held by the K/V buffers."""
-        if self.quant is not None:
-            return sum(q.nbytes() for q in self.quant)
-        return 0 if self.k is None else sum(t.numel() * t.element_size() for t in self.k + self.v)
+        """Bytes held by the layers' buffers."""
+        return 0 if self.layers is None else sum(kv.nbytes() for kv in self.layers)
 
 
 class BeamKVCache:
     """The cache of a beam search (core.generation.beam_search; DESIGN §4.2.4).  `prefix` is an ordinary KVCache of
     batch G that Model.prefill filled with the G prompts (the groups), stored and read once per group.  Group g's fork
     point is T0_g = 256 floor(P_g / 256) for its prompt length P_g: positions below it are read from the prefix, and a
-    beam's positions t >= T0_g live at index t - T0_g of the beam's tail slot, per layer K and V tails
-    [S = G n_beams, tail_cap, Hk, D] with tail_cap = 255 + max_tokens rounded up to 256.  Group g owns slots
-    [g n_beams, (g + 1) n_beams); prompt positions [T0_g, P_g) start in slot g n_beams.
+    beam's positions t >= T0_g live at index t - T0_g of the beam's tail slot, per layer (a BeamKV over the prefix
+    layer's DenseKV) K and V tails [S = G n_beams, tail_cap, Hk, D] with tail_cap = 255 + max_tokens rounded up to
+    256.  Group g owns slots [g n_beams, (g + 1) n_beams); prompt positions [T0_g, P_g) start in slot g n_beams.
 
     The decode batch is the live beam rows, set by set_rows (group, slot and length per row; a group's rows are
     contiguous and equally long).  fork copies tails between slots.  Model.decode_step runs on it unchanged."""
 
     def __init__(self, model: "Model", prefix: KVCache, n_beams: int, max_tokens: int):
-        if prefix.quantized or prefix.rotating or prefix.kv_bits is not None or prefix.k is None:
+        if prefix.quantized or prefix.rotating or prefix.kv_bits is not None:
             raise ValueError("BeamKVCache: the prefix must be an unquantized, non-rotating KVCache filled by prefill")
         attn = model.layers[0].self_attn
         self.prefix, self.n_beams = prefix, n_beams
         self.n_groups = prefix._batch
         self.t0 = [256 * (n // 256) for n in prefix.host_lens]
         self.tail_cap = -(-(255 + max_tokens) // 256) * 256
-        S = self.n_groups * n_beams
-        shape = (S, self.tail_cap, attn.num_kv_heads, attn.head_dim)
-        dev, dt = prefix._device, prefix._dtype
-        self.k = [torch.zeros(shape, device=dev, dtype=dt) for _ in range(prefix._layers)]
-        self.v = [torch.zeros(shape, device=dev, dtype=dt) for _ in range(prefix._layers)]
-        for g, (t0, n) in enumerate(zip(self.t0, prefix.host_lens)):  # the prompts' last positions, once
-            for tail, pre in zip(self.k + self.v, prefix.k + prefix.v):
-                tail[g * n_beams, :n - t0].copy_(pre[g, t0:n])
-        tails = self.k + self.v
-        self._buffers = torch.tensor([t.data_ptr() for t in tails], dtype=torch.int64).to(dev)
-        nbytes = ops.attention_decode_beam_workspace_bytes(S, attn.num_heads, prefix.s_max, self.tail_cap,
-                                                           attn.head_dim)
+        self.layers = [BeamKV(kv, n_beams, self.tail_cap, self.t0, prefix.host_lens) for kv in prefix.layers]
+        self._tails = [kv.k_tail for kv in self.layers] + [kv.v_tail for kv in self.layers]
+        dev = prefix._device
+        self._buffers = torch.tensor([t.data_ptr() for t in self._tails], dtype=torch.int64).to(dev)
+        nbytes = ops.attention_decode_beam_workspace_bytes(self.n_groups * n_beams, attn.num_heads, prefix.s_max,
+                                                           self.tail_cap, attn.head_dim)
         self.workspace = torch.empty(max(nbytes, 16), device=dev, dtype=torch.uint8)
-        self._views = None
         self.set_rows(list(range(self.n_groups)), [g * n_beams for g in range(self.n_groups)], prefix.host_lens)
 
     def set_rows(self, groups, slots, lengths) -> None:
@@ -477,7 +478,6 @@ class BeamKVCache:
         t = torch.tensor(lengths + groups + slots + self.t0 + row0 + rows, dtype=torch.int32).to(self.prefix._device)
         self.host_lens, self.groups, self.slots = lengths, groups, slots
         self.lens, self.tables = t[:R], t[R:]
-        self._views = None
 
     def fork(self, copies) -> None:
         """copies: (src slot, dst slot, positions) triples: tail indices [0, positions) of every layer's K and V tail
@@ -485,14 +485,11 @@ class BeamKVCache:
         if not copies:
             return
         c = torch.tensor(copies, dtype=torch.int32).to(self.prefix._device)
-        ops.kv_beam_fork(self._buffers, c, max(n for _, _, n in copies), self.k + self.v)
+        ops.kv_beam_fork(self._buffers, c, max(n for _, _, n in copies), self._tails)
 
     def layer(self, i: int):
-        if self._views is None:  # made once per decode step: it calls layer() for every layer
-            p = self.prefix
-            self._views = [BeamKV(pk, pv, k, v, self.tables, self.n_groups)
-                           for pk, pv, k, v in zip(p.k, p.v, self.k, self.v)]
-        return self._views[i], None
+        """Layer i's BeamKV."""
+        return self.layers[i]
 
     def advance(self, live=None) -> None:
         if live is not None:
@@ -507,7 +504,7 @@ class BeamKVCache:
 
     def nbytes(self) -> int:
         """Bytes held by the prefix and the tails."""
-        return self.prefix.nbytes() + sum(t.numel() * t.element_size() for t in self.k + self.v)
+        return self.prefix.nbytes() + sum(kv.nbytes() for kv in self.layers)
 
 
 class CacheChunk:

@@ -179,22 +179,14 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     length.  The prompts then always go through Model.extend, in chunks of prefill_step_size (default 512).  A
     rotating prompt_cache brings its own max_kv_size (a different one is an error).  A row that stops at EOS neither
     advances nor writes afterwards, as a ring cannot be truncated."""
-    from .. import ops
-    from ..arch.llama import KVCache
+    from ..arch.llama import KVCache, check_cache_options
 
     if not prompts or any(len(p) == 0 for p in prompts):
         raise ValueError("every prompt needs at least one token")
     if prefill_step_size is not None and (isinstance(prefill_step_size, bool) or not isinstance(prefill_step_size, int)
                                           or prefill_step_size < 1):
         raise ValueError(f"generate: prefill_step_size must be None or an int >= 1, got {prefill_step_size!r}")
-    if max_kv_size is not None:
-        ops.check_max_kv_size(max_kv_size, "generate")
-        if kv_bits is not None:
-            raise ValueError("generate: max_kv_size does not combine with kv_bits (mlx_lm's rotating cache does not "
-                             "quantize)")
-        if model.args.prefix_lm:
-            raise ValueError("generate: a prefix-LM model cannot use a rotating cache (max_kv_size)")
-        model.check_extend(None)
+    check_cache_options(model, kv_bits, kv_group_size, quantized_kv_start, max_kv_size, "generate")
     if prompt_cache is not None:
         if not isinstance(prompt_cache, KVCache):
             raise ValueError(f"generate: prompt_cache must be an arch.llama.KVCache, got {type(prompt_cache).__name__}")
@@ -209,10 +201,6 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
                              f"{prompt_cache.kv_bits!r} (the cache's settings apply)")
         if prompt_cache._batch != len(prompts):
             raise ValueError(f"generate: prompt_cache holds {prompt_cache._batch} rows, {len(prompts)} prompts given")
-    elif kv_bits is not None:
-        ops.check_kv_quant(kv_bits, kv_group_size, what="generate")
-        if isinstance(quantized_kv_start, bool) or not isinstance(quantized_kv_start, int) or quantized_kv_start < 0:
-            raise ValueError(f"generate: quantized_kv_start must be a non-negative int, got {quantized_kv_start!r}")
     start = [0] * len(prompts) if prompt_cache is None else list(prompt_cache.host_lens)
     limit = position_limit(model.args)
     longest = max(len(p) for p in prompts)

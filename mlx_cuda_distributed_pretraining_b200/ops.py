@@ -1007,6 +1007,48 @@ def attention_decode_workspace_bytes(B: int, H: int, s_max: int, D: int) -> int:
     return int(lib().b200_attn_decode_workspace_bytes(B, H, s_max, D))
 
 
+def _check_rows(t, B: int, device, what: str, nm: str) -> None:
+    if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or tuple(t.shape) != (B,) or t.device != device \
+            or not t.is_contiguous():
+        raise ValueError(f"{what}: {nm} must be a contiguous int32 [{B}] tensor on {device}, got "
+                         f"{getattr(t, 'dtype', type(t))} {list(getattr(t, 'shape', []))}")
+
+
+def _check_scores(q: torch.Tensor, scale, window, alibi, what: str):
+    """(window, alibi, scale) of an attention-over-a-cache wrapper: window and ALiBi slopes checked, scale defaulting
+    to head_dim ** -0.5."""
+    if window is not None:
+        window = _check_window(window, what)
+    if alibi is not None:
+        alibi = _check_alibi(alibi, q, True, what)
+    return window, alibi, q.shape[-1] ** -0.5 if scale is None else scale
+
+
+def _check_workspace(workspace: Optional[torch.Tensor], need: int, device, what: str, align: int = 1) -> torch.Tensor:
+    """The decode workspace: allocated when None, else checked to be uint8 on `device`, align-byte aligned, with at
+    least `need` bytes."""
+    if workspace is None:
+        return torch.empty(max(need, 16), device=device, dtype=torch.uint8)
+    if workspace.dtype != torch.uint8 or workspace.device != device or workspace.numel() < need \
+            or workspace.data_ptr() % align:
+        aligned = f"{align}-byte aligned " if align > 1 else ""
+        raise ValueError(f"{what}: workspace must be {aligned}uint8 on {device} with >= {need} bytes")
+    return workspace
+
+
+def _check_rope_tables(rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]], D: int, layout: str, what: str):
+    """(cos, sin, half) of a cache-append wrapper: the fp32 [positions, D / 2] tables of rope_tables() (None, None
+    without RoPE) and the flag of the half layout (0 without RoPE)."""
+    if rope_tables is None:
+        return None, None, 0
+    cos_t, sin_t = rope_tables
+    for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
+        _need(t, torch.float32, f"{what}: {nm}")
+        if t.dim() != 2 or t.shape[1] != D // 2:
+            raise ValueError(f"{what}: RoPE tables must be [positions, {D // 2}]")
+    return cos_t, sin_t, int(layout == "half")
+
+
 def _check_cache(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor, what: str):
     _is_bf16(q, "q")
     for t, nm in ((q, "q"), (k_cache, "k_cache"), (v_cache, "v_cache")):
@@ -1018,9 +1060,7 @@ def _check_cache(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, 
     Bc, s_max, Hk, Dc = k_cache.shape
     if Bc != B or Dc != D or H % Hk != 0:
         raise ValueError(f"{what}: q {tuple(q.shape)} does not match cache {tuple(k_cache.shape)}")
-    if lens.dtype != torch.int32 or lens.device != q.device or lens.shape != (B,) or not lens.is_contiguous():
-        raise ValueError(f"{what}: lens must be a contiguous int32 [B] tensor on {q.device}, got {lens.dtype} "
-                         f"{tuple(lens.shape)} on {lens.device}")
+    _check_rows(lens, B, q.device, what, "lens")
     return B, H, D, s_max, Hk
 
 
@@ -1038,17 +1078,9 @@ def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     B, H, D, s_max, Hk = _check_cache(q, k_cache, v_cache, lens, "attention_decode")
     if D not in (16, 32, 64, 128):
         raise ValueError(f"attention_decode: head_dim {D} unsupported (16, 32, 64 or 128)")
-    if window is not None:
-        window = _check_window(window, "attention_decode")
-    if alibi is not None:
-        alibi = _check_alibi(alibi, q, True, "attention_decode")
-    if scale is None:
-        scale = D ** -0.5
-    need = attention_decode_workspace_bytes(B, H, s_max, D)
-    if workspace is None:
-        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
-    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need:
-        raise ValueError(f"attention_decode: workspace must be uint8 on {q.device} with >= {need} bytes")
+    window, alibi, scale = _check_scores(q, scale, window, alibi, "attention_decode")
+    workspace = _check_workspace(workspace, attention_decode_workspace_bytes(B, H, s_max, D), q.device,
+                                 "attention_decode")
     o = torch.empty_like(q)
     lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_decode")
@@ -1087,14 +1119,8 @@ def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.
             raise ValueError(f"kv_append: {nm} must be [{B},{Hk},{D}], got {tuple(t.shape)}")
     if D % 8 != 0:
         raise ValueError(f"kv_append: head_dim {D} must be a multiple of 8")
-    cos_t = sin_t = None
-    if rope_tables is not None:
-        cos_t, sin_t = rope_tables
-        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
-            _need(t, torch.float32, f"kv_append: {nm}")
-            if t.dim() != 2 or t.shape[1] != D // 2:
-                raise ValueError(f"kv_append: RoPE tables must be [positions, {D // 2}]")
-    if layout == "half" and cos_t is not None:
+    cos_t, sin_t, half = _check_rope_tables(rope_tables, D, layout, "kv_append")
+    if half:
         if D % 16 != 0:
             raise ValueError(f"kv_append: the half layout needs head_dim % 16 == 0, got {D}")
         check(lib().b200_kv_append_half(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(),
@@ -1104,13 +1130,6 @@ def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.
     check(lib().b200_kv_append(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                lens.data_ptr(), _ptr(cos_t), _ptr(sin_t), B, s_max, H, Hk, D, _is_bf16(q, "q"),
                                _stream()), "b200_kv_append")
-
-
-def _check_rows(t, B: int, device, what: str, nm: str) -> None:
-    if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or tuple(t.shape) != (B,) or t.device != device \
-            or not t.is_contiguous():
-        raise ValueError(f"{what}: {nm} must be a contiguous int32 [{B}] tensor on {device}, got "
-                         f"{getattr(t, 'dtype', type(t))} {list(getattr(t, 'shape', []))}")
 
 
 def attention_cached(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, start: torch.Tensor,
@@ -1141,12 +1160,7 @@ def attention_cached(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
         raise ValueError(f"{what}: head_dim {D} unsupported (64 or 128)")
     _check_rows(start, B, q.device, what, "start")
     _check_rows(end, B, q.device, what, "end")
-    if window is not None:
-        window = _check_window(window, what)
-    if alibi is not None:
-        alibi = _check_alibi(alibi, q, True, what)
-    if scale is None:
-        scale = D ** -0.5
+    window, alibi, scale = _check_scores(q, scale, window, alibi, what)
     o = torch.empty_like(q)
     lse = torch.empty((B, H, L), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_cached")
@@ -1209,17 +1223,8 @@ def attention_decode_ring(q: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.T
     _check_rows(end, B, q.device, what, "end")
     if C < max_kv_size:
         raise ValueError(f"{what}: the ring's {C} slots cannot hold max_kv_size={max_kv_size} keys")
-    if window is not None:
-        window = _check_window(window, what)
-    if alibi is not None:
-        alibi = _check_alibi(alibi, q, True, what)
-    if scale is None:
-        scale = D ** -0.5
-    need = attention_decode_workspace_bytes(B, H, C, D)
-    if workspace is None:
-        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
-    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need:
-        raise ValueError(f"{what}: workspace must be uint8 on {q.device} with >= {need} bytes")
+    window, alibi, scale = _check_scores(q, scale, window, alibi, what)
+    workspace = _check_workspace(workspace, attention_decode_workspace_bytes(B, H, C, D), q.device, what)
     o = torch.empty_like(q)
     lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_decode_ring")
@@ -1247,12 +1252,7 @@ def attention_ring(q: torch.Tensor, k_ring: torch.Tensor, v_ring: torch.Tensor, 
                          f"{max_kv_size + L - 1}: writing the chunk would overwrite keys its queries see")
     _check_rows(start, B, q.device, what, "start")
     _check_rows(end, B, q.device, what, "end")
-    if window is not None:
-        window = _check_window(window, what)
-    if alibi is not None:
-        alibi = _check_alibi(alibi, q, True, what)
-    if scale is None:
-        scale = D ** -0.5
+    window, alibi, scale = _check_scores(q, scale, window, alibi, what)
     o = torch.empty_like(q)
     lse = torch.empty((B, H, L), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_ring")
@@ -1281,14 +1281,7 @@ def kv_append_ring(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_ring: to
         _need(t, torch.bfloat16, f"{what}: {nm}")
         if t.shape != (B, Hk, D):
             raise ValueError(f"{what}: {nm} must be [{B},{Hk},{D}], got {tuple(t.shape)}")
-    cos_t = sin_t = None
-    if rope_tables is not None:
-        cos_t, sin_t = rope_tables
-        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
-            _need(t, torch.float32, f"{what}: {nm}")
-            if t.dim() != 2 or t.shape[1] != D // 2:
-                raise ValueError(f"{what}: RoPE tables must be [positions, {D // 2}]")
-    half = int(layout == "half" and cos_t is not None)
+    cos_t, sin_t, half = _check_rope_tables(rope_tables, D, layout, what)
     check(lib().b200_kv_append_ring(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_ring.data_ptr(), v_ring.data_ptr(),
                                     end.data_ptr(), _ptr(live), _ptr(cos_t), _ptr(sin_t), half, B, C, H, Hk, D,
                                     _stream()), "b200_kv_append_ring")
@@ -1340,18 +1333,9 @@ def attention_decode_beam(q: torch.Tensor, k_prefix: torch.Tensor, v_prefix: tor
                          f"(head_dim 16, 32, 64 or 128)")
     _check_rows(lens, R, q.device, what, "lens")
     _check_beam_tables(tables, R, G, q.device, what)
-    if window is not None:
-        window = _check_window(window, what)
-    if alibi is not None:
-        alibi = _check_alibi(alibi, q, True, what)
-    if scale is None:
-        scale = D ** -0.5
-    need = attention_decode_beam_workspace_bytes(R, H, s_prefix, tail_cap, D)
-    if workspace is None:
-        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
-    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need \
-            or workspace.data_ptr() % 128:
-        raise ValueError(f"{what}: workspace must be 128-byte aligned uint8 on {q.device} with >= {need} bytes")
+    window, alibi, scale = _check_scores(q, scale, window, alibi, what)
+    workspace = _check_workspace(workspace, attention_decode_beam_workspace_bytes(R, H, s_prefix, tail_cap, D),
+                                 q.device, what, align=128)
     o = torch.empty_like(q)
     lse = torch.empty((R, H), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_decode_beam")
@@ -1384,14 +1368,7 @@ def kv_append_beam(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_tail: to
             raise ValueError(f"{what}: {nm} must be [{R},{Hk},{D}], got {tuple(t.shape)}")
     _check_rows(lens, R, q.device, what, "lens")
     _check_beam_tables(tables, R, n_groups, q.device, what)
-    cos_t = sin_t = None
-    if rope_tables is not None:
-        cos_t, sin_t = rope_tables
-        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
-            _need(t, torch.float32, f"{what}: {nm}")
-            if t.dim() != 2 or t.shape[1] != D // 2:
-                raise ValueError(f"{what}: RoPE tables must be [positions, {D // 2}]")
-    half = int(layout == "half" and cos_t is not None)
+    cos_t, sin_t, half = _check_rope_tables(rope_tables, D, layout, what)
     check(lib().b200_kv_append_beam(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_tail.data_ptr(), v_tail.data_ptr(),
                                     lens.data_ptr(), tables.data_ptr(), _ptr(cos_t), _ptr(sin_t), half, R,
                                     tail_cap, H, Hk, D, _is_bf16(q, "q"), _stream()), "b200_kv_append_beam")
@@ -1543,16 +1520,8 @@ def kv_append_quant(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_codes: 
         _need(t, q.dtype, f"kv_append_quant: {nm}")
         if t.data_ptr() % 16:
             raise ValueError(f"kv_append_quant: {nm} must be 16-byte aligned")
-    if lens.dtype != torch.int32 or lens.device != q.device or lens.shape != (B,) or not lens.is_contiguous():
-        raise ValueError(f"kv_append_quant: lens must be a contiguous int32 [B] tensor on {q.device}")
-    cos_t = sin_t = None
-    if rope_tables is not None:
-        cos_t, sin_t = rope_tables
-        for t, nm in ((cos_t, "cos"), (sin_t, "sin")):
-            _need(t, torch.float32, f"kv_append_quant: {nm}")
-            if t.dim() != 2 or t.shape[1] != D // 2:
-                raise ValueError(f"kv_append_quant: RoPE tables must be [positions, {D // 2}]")
-    half = int(layout == "half" and cos_t is not None)
+    _check_rows(lens, B, q.device, "kv_append_quant", "lens")
+    cos_t, sin_t, half = _check_rope_tables(rope_tables, D, layout, "kv_append_quant")
     check(lib().b200_kv_append_quant(q.data_ptr(), k.data_ptr(), v.data_ptr(), k_codes.data_ptr(), v_codes.data_ptr(),
                                      k_params.data_ptr(), v_params.data_ptr(), lens.data_ptr(), _ptr(cos_t),
                                      _ptr(sin_t), half, B, s_max, H, Hk, D, bits, group_size, _is_bf16(q, "q"),
@@ -1579,19 +1548,10 @@ def attention_decode_quant(q: torch.Tensor, k_codes: torch.Tensor, v_codes: torc
     s_max = _check_quant_cache(k_codes, v_codes, k_params, v_params, B, Hk, D, bits, group_size, q.device,
                                "attention_decode_quant")
     _need(q, q.dtype, "attention_decode_quant: q")
-    if lens.dtype != torch.int32 or lens.device != q.device or lens.shape != (B,) or not lens.is_contiguous():
-        raise ValueError(f"attention_decode_quant: lens must be a contiguous int32 [B] tensor on {q.device}")
-    if window is not None:
-        window = _check_window(window, "attention_decode_quant")
-    if alibi is not None:
-        alibi = _check_alibi(alibi, q, True, "attention_decode_quant")
-    if scale is None:
-        scale = D ** -0.5
-    need = attention_decode_workspace_bytes(B, H, s_max, D)
-    if workspace is None:
-        workspace = torch.empty(max(need, 16), device=q.device, dtype=torch.uint8)
-    elif workspace.dtype != torch.uint8 or workspace.device != q.device or workspace.numel() < need:
-        raise ValueError(f"attention_decode_quant: workspace must be uint8 on {q.device} with >= {need} bytes")
+    _check_rows(lens, B, q.device, "attention_decode_quant", "lens")
+    window, alibi, scale = _check_scores(q, scale, window, alibi, "attention_decode_quant")
+    workspace = _check_workspace(workspace, attention_decode_workspace_bytes(B, H, s_max, D), q.device,
+                                 "attention_decode_quant")
     o = torch.empty_like(q)
     lse = torch.empty((B, H), device=q.device, dtype=torch.float32) if return_lse else None
     tok = _t0("attn_decode")

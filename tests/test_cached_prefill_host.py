@@ -40,7 +40,7 @@ def _cache(batch=2, s_max=512, positions=None, kv_bits=None):
     c = KVCache.__new__(KVCache)
     c._layers, c._device, c._dtype, c._batch, c._heads = 2, torch.device("cpu"), torch.bfloat16, batch, (2, 64)
     c.s_max, c.kv_bits, c.kv_group_size, c.quantized_kv_start = s_max, kv_bits, 64, 0
-    c.k = c.v = c.quant = None
+    c.layers, c.quantized = None, False
     if positions:
         c._allocate(positions)
     c.lens = torch.zeros(batch, dtype=torch.int32)
@@ -48,17 +48,21 @@ def _cache(batch=2, s_max=512, positions=None, kv_bits=None):
     return c
 
 
-def test_kv_cache_extend_truncate_and_grow():
+def test_kv_cache_layers_extend_truncate_and_grow():
     c = _cache()
     c.extend_lengths([3, 0])
     assert c.host_start == [0, 0] and c.host_lens == [3, 0] and c.lens.tolist() == [3, 0]
-    assert c.k[0].shape[1] == 256  # allocated on first use, rounded up to 256
-    c.k[1][0, :3] = 1.5
+    assert c.layers[0].k.shape[1] == 256  # allocated on first use, rounded up to 256
+    c.layers[1].k[0, :3] = 1.5
+    c.layers[1].v[1, :2] = -2.0
     c.extend_lengths([300, 2])
     assert c.host_start == [3, 0] and c.host_lens == [303, 2]
-    assert c.k[0].shape[1] == 512 and bool((c.k[1][0, :3] == 1.5).all()), "growth keeps the cached positions"
+    assert c.layers[0].k.shape[1] == 512 and c.layers[0].v.shape[1] == 512
+    assert bool((c.layers[1].k[0, :3] == 1.5).all()) and bool((c.layers[1].v[1, :2] == -2.0).all()), \
+        "growth keeps the cached positions"
     c.truncate([100, 2])
     assert c.host_lens == [100, 2] and c.lens.tolist() == [100, 2]
+    layers = c.layers
     with pytest.raises(ValueError, match="truncate"):
         c.truncate([101, 2])
     with pytest.raises(ValueError, match="KV cache full"):
@@ -67,7 +71,7 @@ def test_kv_cache_extend_truncate_and_grow():
         c.extend_lengths([1, -1])
     with pytest.raises(ValueError):
         c.extend_lengths([1])
-    assert c.host_lens == [100, 2], "a refused extend changes nothing"
+    assert c.host_lens == [100, 2] and c.layers is layers, "a refused extend changes nothing"
 
 
 # -- refusals ---------------------------------------------------------------------------------------------------------

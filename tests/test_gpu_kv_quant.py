@@ -281,8 +281,9 @@ def _quant_tol(kind, bits):
 
 @pytest.mark.parametrize("bits", [4, 8])
 @pytest.mark.parametrize("kind", ["bf16_gqa", "bf16_rope"])
-def test_prefill_decode_quantized_cache(kind, bits):
+def test_prefill_decode_quantized_layers(kind, bits):
     from mlx_cuda_distributed_pretraining_b200.arch.llama import KVCache
+    from mlx_cuda_distributed_pretraining_b200.arch.flash_attention import QuantizedKV
     from tests.test_gpu_generation import _rel_rows
     model = _trainer(kind).model
     T, t0 = 300, 260
@@ -299,7 +300,7 @@ def test_prefill_decode_quantized_cache(kind, bits):
 
     dense, _ = run()
     quant, cache = run(kv_bits=bits)
-    assert cache.quantized and cache.k is None
+    assert cache.quantized and all(isinstance(kv, QuantizedKV) for kv in cache.layers)
     e_dense, e_full = _rel_rows(quant, dense), _rel_rows(quant, full)
     tol = _quant_tol(kind, bits)
     print(f"{kind} {bits}-bit cache: vs bf16 cache {e_dense:.2e}, vs forward {e_full:.2e} (tolerance {tol:.2e})")
@@ -307,8 +308,9 @@ def test_prefill_decode_quantized_cache(kind, bits):
 
 
 @pytest.mark.parametrize("kind", ["bf16_rope", "c1_fp32_d32"])
-def test_conversion_equals_direct_quantization(kind):
+def test_conversion_equals_direct_quantized_layers(kind):
     from mlx_cuda_distributed_pretraining_b200.arch.llama import KVCache
+    from mlx_cuda_distributed_pretraining_b200.arch.flash_attention import QuantizedKV
     if kind == "c1_fp32_d32":  # fp32 activations, head_dim 32
         from mlx_cuda_distributed_pretraining_b200.core.training import Config, Trainer
         from tests.test_gpu_generation import _cfg
@@ -322,16 +324,16 @@ def test_conversion_equals_direct_quantization(kind):
     tokens = torch.randint(0, 256, (2, t0 + 8), generator=torch.Generator().manual_seed(2)).cuda()
     direct = KVCache(model, 2, t0 + 8, kv_bits=4, kv_group_size=32)
     model.prefill(tokens[:, :t0], [t0, t0 - 9], direct)
-    assert direct.quantized and direct.k is None
+    assert direct.quantized and all(isinstance(kv, QuantizedKV) for kv in direct.layers)
     late = KVCache(model, 2, t0 + 8, kv_bits=4, kv_group_size=32, quantized_kv_start=start)
     model.prefill(tokens[:, :t0], [t0, t0 - 9], late)
-    assert not late.quantized and late.k[0].shape[1] == 256  # start + 1 rounded up to 256
+    assert not late.quantized and late.layers[0].k.shape[1] == 256  # start + 1 rounded up to 256
     steps = 0
     while not late.quantized:
         model.decode_step(tokens[:, t0 + steps], late)
         steps += 1
-    assert steps == start + 1 - t0 and late.k is None and late.v is None
-    for a, b in zip(direct.quant, late.quant):  # each row's prompt positions (the decode steps wrote past them)
+    assert steps == start + 1 - t0 and all(isinstance(kv, QuantizedKV) for kv in late.layers)
+    for a, b in zip(direct.layers, late.layers):  # each row's prompt positions (the decode steps wrote past them)
         for x, y in zip(a.buffers(), b.buffers()):
             for row, n in enumerate((t0, t0 - 9)):
                 if x.dtype == torch.uint8:

@@ -115,7 +115,7 @@ def _ring_cache(max_kv_size=64, max_chunk=128):
     from mlx_cuda_distributed_pretraining_b200.arch.llama import KVCache
     c = KVCache.__new__(KVCache)
     c._layers, c._device, c._dtype, c._batch, c._heads = 1, torch.device("cpu"), torch.bfloat16, 2, (2, 64)
-    c.kv_bits, c.quant, c.max_kv_size, c.max_chunk = None, None, max_kv_size, max_chunk
+    c.kv_bits, c.quantized, c.max_kv_size, c.max_chunk = None, False, max_kv_size, max_chunk
     c.s_max = -(-(max_kv_size + max_chunk - 1) // 256) * 256
     c._allocate(c.s_max)
     c.lens = torch.zeros(2, dtype=torch.int32)
@@ -123,15 +123,15 @@ def _ring_cache(max_kv_size=64, max_chunk=128):
     return c
 
 
-def test_ring_cache_bookkeeping_and_refusals():
+def test_ring_cache_layers_bookkeeping_and_refusals():
     c = _ring_cache()
     nbytes = c.nbytes()
     assert nbytes == 2 * 2 * 256 * 2 * 64 * 2
-    rings = [c.layer(0)[0].k]
+    rings = [c.layer(0).k, c.layer(0).v]
     for _ in range(5):
         c.extend_lengths([128, 100])  # rows grow past the ring's slots
     assert c.host_lens == [640, 500] and c.nbytes() == nbytes
-    assert c.layer(0)[0].k is rings[0] and c.layer(0)[1] is None, "the ring is never reallocated"
+    assert c.layer(0).k is rings[0] and c.layer(0).v is rings[1], "the ring is never reallocated"
     with pytest.raises(ValueError, match="max_chunk"):
         c.extend_lengths([129, 0])
     with pytest.raises(ValueError, match="truncated"):
