@@ -470,6 +470,19 @@ int b200_attn_decode_window(const void* q, const void* k_cache, const void* v_ca
 int b200_attn_decode_alibi(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o,
                            float* lse, int window, const float* slopes, int B, int s_max, int H, int Hk, int D,
                            float scale, int is_bf16, void* workspace, size_t workspace_bytes, void* stream);
+/* A short chunk of new queries over the dense cache that already holds their keys (speculative decoding's verify
+ * step): q, o [B, n_q, H, D], 1 <= n_q <= 16; query i of row b sits at position p = start[b] + i and is valid iff
+ * i < end[b] - start[b]; it sees keys max(0, p - window) .. p (window < 0: none), with slopes[h] * (k - p) added when
+ * slopes is non-null.  lse: f32 [B, H, n_q] or NULL.  Invalid queries' o and lse are not written; no position at or
+ * past end[b] is read.  Dtypes, D and (H/Hk) * D as b200_attn_decode.  The chunks, the merge order and the tiles
+ * depend on (start[b], end[b], window) alone, so a row is bit-identical alone or in any batch, and with n_q = 1 it
+ * is bit-equal to b200_attn_decode(_window / _alibi) with lens = end.  0 <= start[b] <= end[b] <= s_max (device
+ * values, not checked); B * n_q <= 65535.  Workspace: b200_attn_decode_multi_workspace_bytes(B, n_q, H, s_max, D). */
+size_t b200_attn_decode_multi_workspace_bytes(int B, int n_q, int H, int s_max, int D);
+int b200_attn_decode_multi(const void* q, const void* k_cache, const void* v_cache, const int* start, const int* end,
+                           void* o, float* lse, int window, const float* slopes, int B, int n_q, int s_max, int H,
+                           int Hk, int D, float scale, int is_bf16, void* workspace, size_t workspace_bytes,
+                           void* stream);
 /* Appends one token per row at pos = lens[b] - 1: k_cache[b,pos] = rot(k[b]), v_cache[b,pos] = v[b] (k, v:
  * [B,Hk,D]).  With cos_t/sin_t (f32 [>= max pos + 1, D/2], ops.rope_tables) the interleaved-pair rotation of
  * b200_rope (arch/llama_standard.py:90-131) is applied to k and, in place, to q [B,H,D], with b200_rope's exact

@@ -118,6 +118,9 @@ SIGNATURES = {
                                    _i, _f, _i, _vp, _sz, _vp]),
     "b200_attn_decode_beam_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "b200_attn_decode_beam_pack": (_i, [_i, _i, _i]),
+    "b200_attn_decode_multi": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _f, _i, _vp,
+                                    _sz, _vp]),
+    "b200_attn_decode_multi_workspace_bytes": (_sz, [_i, _i, _i, _i, _i]),
     "b200_kv_append_beam": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
     "b200_kv_beam_fork": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _vp]),
     "b200_moe_route_workspace_bytes": (_sz, [_i, _i, _i]),

@@ -111,6 +111,8 @@ class PrefixCausalMask:
 #                                                     there with attn.rope_tables), then attended -> ctx [B, H, D]
 #   extend(q, k, v, chunk, attn, window)              a llama.CacheChunk's rotated q [B, L, H, D], k, v [B, L, Hk, D]
 #                                                     written, then attended -> ctx [B, L, H, D]
+#   verify(q, k, v, chunk, attn, window)              extend for a short chunk (chunk.verify, L <= 16: speculative
+#                                                     decoding), attended split over keys (DenseKV only)
 # step is the model-wide cache (llama.KVCache / BeamKVCache), which holds the per-step state: lens, workspace and,
 # per format, the ring's live mask or the beam tables.  attn is the FlashAttention module: scale, rope_tables and
 # alibi_slopes().
@@ -143,6 +145,13 @@ class DenseKV:
         self.v[r, dst] = v[r, src]
         return ops.attention_cached(q, self.k, self.v, chunk.start, chunk.end, attn.scale, window=window,
                                     alibi=attn.alibi_slopes(q.device))
+
+    def verify(self, q, k, v, chunk, attn, window):
+        r, src, dst = chunk.rows, chunk.src, chunk.dst
+        self.k[r, dst] = k[r, src]
+        self.v[r, dst] = v[r, src]
+        return ops.attention_decode_multi(q, self.k, self.v, chunk.start, chunk.end, attn.scale, chunk.workspace,
+                                          window=window, alibi=attn.alibi_slopes(q.device))
 
 
 class QuantizedKV:
@@ -382,11 +391,13 @@ class FlashAttention(nn.Module):
         """A chunk of new tokens per row, x [B, L, hidden] right-padded, appended at each row's current cache length
         (chunk: the llama.CacheChunk of the call).  Token i of row b sits at position p = chunk.start[b] + i: its q
         and k are rotated there (ops.rope at absolute positions), then kv.extend writes its k and v to the cache and
-        its query attends over the row's cached keys up to p (max(0, p - window) .. p with a sliding window)."""
+        its query attends over the row's cached keys up to p (max(0, p - window) .. p with a sliding window).  A
+        chunk made for Model.verify (chunk.verify) goes through kv.verify instead."""
         q, k, v = self._qkv(x)
         if self.rope_tables is not None:
             cos_t, sin_t = self.rope_tables
             q = ops.rope(q, cos_t, sin_t, chunk.pos, rope_layout)
             k = ops.rope(k, cos_t, sin_t, chunk.pos, rope_layout)
         q, k, v = q.contiguous(), k.contiguous(), v.contiguous()
-        return self._out(kv.extend(q, k, v, chunk, self, window))
+        attend = kv.verify if chunk.verify else kv.extend
+        return self._out(attend(q, k, v, chunk, self, window))

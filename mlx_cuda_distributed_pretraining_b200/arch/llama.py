@@ -513,7 +513,11 @@ class CacheChunk:
     pos: int32 [B, L] rotation positions (padding tokens take their row's last position, so that no rotation reads
     past the tables); rows / src / dst: int64 indices of the valid tokens (row, index in the chunk, cache position);
     scratch: a quantized cache's bf16 K / V for the call, made by its first layer.  slots (a rotating cache's C): dst
-    are the ring slots ops.ring_slot(start[b] + i, C)."""
+    are the ring slots ops.ring_slot(start[b] + i, C).  verify / workspace: set by Model.verify, whose chunks the
+    layers attend with DenseKV.verify over that decode workspace."""
+
+    verify = False
+    workspace: Optional[torch.Tensor] = None
 
     def __init__(self, start, counts, L: int, device, slots: Optional[int] = None):
         ends = [a + n for a, n in zip(start, counts)]
@@ -710,6 +714,38 @@ class Model(nn.Module):
         rows = torch.arange(B, device=tokens.device)
         last = torch.tensor([max(n - 1, 0) for n in counts], device=tokens.device)
         return self._row_logits(h[rows, last], None if pending is None else pending[rows, last])
+
+    @torch.no_grad()
+    def verify(self, tokens: torch.Tensor, lengths, cache: KVCache) -> torch.Tensor:
+        """Model.extend for a short chunk, tokens [B, L] with L <= 16 (speculative decoding's verify step and the
+        draft's catch-up): the same appends, absolute-position RoPE, window, ALiBi and MoE, with the chunk attended by
+        the split-KV multi-query decode kernel (DenseKV.verify), so any dtype and head dim the decode step serves.
+        Returns the fp32 logits [B, L, V] after every token of the chunk (a row's padding positions get unspecified
+        logits).  The cache must be an unquantized, non-rotating KVCache holding at least one position per row with
+        new tokens (a prefix-LM model's decoded queries are causal)."""
+        B, L = tokens.shape
+        counts = [int(n) for n in lengths]
+        if B != cache._batch:
+            raise ValueError(f"tokens have {B} rows, the cache {cache._batch}")
+        if not 1 <= L <= ops.MULTI_MAX_QUERIES:
+            raise ValueError(f"verify: chunks of 1 to {ops.MULTI_MAX_QUERIES} tokens per row, got {L}")
+        if len(counts) != B or any(not 0 <= n <= L for n in counts) or max(counts) < 1:
+            raise ValueError(f"lengths must be {B} ints in [0, {L}], at least one positive, got {counts}")
+        if cache.rotating or cache.kv_bits is not None or cache.layers is None:
+            raise ValueError("verify needs an unquantized, non-rotating KV cache that a prefill has filled")
+        if any(n > 0 and m == 0 for n, m in zip(counts, cache.host_lens)):
+            raise ValueError("verify appends to a prefilled cache: a row with new tokens holds no position")
+        cache.extend_lengths(counts)
+        chunk = CacheChunk(cache.host_start, counts, L, tokens.device)
+        attn = self.layers[0].self_attn
+        chunk.verify = True
+        chunk.workspace = torch.empty(max(16, ops.attention_decode_multi_workspace_bytes(
+            B, L, attn.num_heads, cache.s_max, attn.head_dim)), device=tokens.device, dtype=torch.uint8)
+        h = ops.embedding(tokens, self.embed_tokens.weight)
+        pending = None
+        for i, layer in enumerate(self.layers):
+            h, pending = layer.forward_cached(h, pending, cache, i, self.args.sliding_window, chunk=chunk)
+        return self._row_logits(h, pending)
 
     @torch.no_grad()
     def decode_step(self, tokens: torch.Tensor, cache: KVCache, live=None) -> torch.Tensor:

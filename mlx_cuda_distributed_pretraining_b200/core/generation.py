@@ -5,6 +5,7 @@
                               [--top-p P --seed N --num-samples N --checkpoint step_N --runs-dir runs]
                               [--kv-bits {4,8} --kv-group-size {32,64,128} --quantized-kv-start N]
                               [--prefill-step-size N] [--num-beams N]
+                              [--draft-run NAME --draft-checkpoint step_N --num-draft-tokens K]
 
 The run's config.yaml (written by the trainer) rebuilds the model through Trainer(cfg, for_training=False), the
 checkpoint's weights are loaded into it, and `generate` prefills [BOS] + tokenize(prompt) once and then decodes one
@@ -102,15 +103,19 @@ def sampling_distribution(logits: torch.Tensor, temp: float, min_p: Optional[flo
     return temperature_distribution(logits, temp)
 
 
+def token_probs(logits: torch.Tensor, temp: float, min_p: Optional[float], top_p: Optional[float]) -> torch.Tensor:
+    """The distribution sample() draws from (temp > 0): the sampler over log-probabilities (logits - logsumexp)."""
+    logprobs = logits - torch.logsumexp(logits, dim=-1, keepdim=True)
+    return sampling_distribution(logprobs, temp, min_p, top_p)
+
+
 def sample(logits: torch.Tensor, temp: float, min_p: Optional[float], top_p: Optional[float],
            generator: Optional[torch.Generator]) -> torch.Tensor:
     """Next tokens [B] from fp32 logits [B, V], on the logits' device.  Like the reference, the sampler sees
     log-probabilities (logits - logsumexp); temperature 0 is argmax."""
-    logprobs = logits - torch.logsumexp(logits, dim=-1, keepdim=True)
     if temp == 0:
-        return torch.argmax(logprobs, dim=-1)
-    probs = sampling_distribution(logprobs, temp, min_p, top_p)
-    return torch.multinomial(probs, 1, generator=generator).squeeze(-1)
+        return torch.argmax(logits - torch.logsumexp(logits, dim=-1, keepdim=True), dim=-1)
+    return torch.multinomial(token_probs(logits, temp, min_p, top_p), 1, generator=generator).squeeze(-1)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -160,7 +165,8 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
              repetition_context_size: int = 20, eos_token: Optional[int] = None, seed: Optional[int] = None,
              on_step: Optional[Callable[[List[int]], None]] = None, kv_bits: Optional[int] = None,
              kv_group_size: int = 64, quantized_kv_start: int = 0, prefill_step_size: Optional[int] = None,
-             prompt_cache=None, max_kv_size: Optional[int] = None) -> List[List[int]]:
+             prompt_cache=None, max_kv_size: Optional[int] = None, draft_model=None, num_draft_tokens: int = 3,
+             on_round: Optional[Callable[[List[List[int]], List[List[int]]], None]] = None) -> List[List[int]]:
     """Generates up to max_tokens tokens for each of the ragged prompts in one batch.  A row stops at EOS, which is
     included in its output.  Returns the generated tokens per row (prompt excluded).  Per step, the sampled tokens
     are the one value read back from the device.  kv_bits (4 or 8; None: no quantization), kv_group_size and
@@ -178,11 +184,21 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
     of its row and its most recent max_kv_size - 4, and the cache holds a constant number of slots whatever the
     length.  The prompts then always go through Model.extend, in chunks of prefill_step_size (default 512).  A
     rotating prompt_cache brings its own max_kv_size (a different one is an error).  A row that stops at EOS neither
-    advances nor writes afterwards, as a ring cannot be truncated."""
+    advances nor writes afterwards, as a ring cannot be truncated.
+
+    draft_model (a Model with the same vocabulary): speculative decoding, as mlx_lm's generate(..., draft_model=...)
+    (DESIGN §2).  Each round the draft proposes up to num_draft_tokens (1 to 15, default 3) tokens and the target
+    scores them all in one Model.verify call; the output is still a sample of the target, with plain generation's
+    distribution.  on_round(emitted, drafted), if given, sees each round's tokens emitted and drafted per row.  It
+    does not combine with kv_bits, max_kv_size, prompt_cache or on_step.  With prefill_step_size the draft is
+    prefilled in the same chunks when Model.extend serves it, else in one piece (draft_prefill_step)."""
     from ..arch.llama import KVCache, check_cache_options
 
     if not prompts or any(len(p) == 0 for p in prompts):
         raise ValueError("every prompt needs at least one token")
+    if draft_model is not None:
+        check_draft(model, draft_model, num_draft_tokens, max(len(p) for p in prompts) + max_tokens, kv_bits=kv_bits,
+                    max_kv_size=max_kv_size, prompt_cache=prompt_cache, on_step=on_step)
     if prefill_step_size is not None and (isinstance(prefill_step_size, bool) or not isinstance(prefill_step_size, int)
                                           or prefill_step_size < 1):
         raise ValueError(f"generate: prefill_step_size must be None or an int >= 1, got {prefill_step_size!r}")
@@ -239,6 +255,16 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
         logits = _prefill(model, prompts, cache, prefill_step_size)
     else:
         logits = model.prefill(tokens.to(device), [len(p) for p in prompts], cache)
+    if draft_model is not None:
+        draft_cache = KVCache(draft_model, B, longest + max_tokens)
+        draft_step = draft_prefill_step(draft_model, prefill_step_size, longest)
+        if draft_step is not None:
+            _prefill(draft_model, prompts, draft_cache, draft_step)
+        else:
+            draft_model.prefill(tokens.to(device), [len(p) for p in prompts], draft_cache)
+        sampler = (temperature, min_p, top_p, repetition_penalty, repetition_context_size, gen)
+        return _speculative(model, draft_model, prompts, logits, cache, draft_cache, max_tokens, num_draft_tokens,
+                            eos_token, sampler, on_round)
     history = [list(p) for p in prompts]
     out: List[List[int]] = [[] for _ in prompts]
     done = [False] * B
@@ -272,6 +298,191 @@ def generate(model, prompts: List[List[int]], max_tokens: int = 256, temperature
         if max_tokens > 0:
             model.decode_step(nxt, cache)
         cache.truncate([s + len(p) + len(o) for s, p, o in zip(start, prompts, out)])
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# speculative decoding (mlx_lm's generate with a draft_model; DESIGN §2 records each rule)
+# ------------------------------------------------------------------------------------------------
+MAX_DRAFT_TOKENS = 15  # the target verifies K + 1 <= 16 positions per row (ops.attention_decode_multi)
+
+
+def check_draft(model, draft_model, num_draft_tokens, reach: int, kv_bits=None, max_kv_size=None, prompt_cache=None,
+                on_step=None, num_beams=None) -> None:
+    """Raises ValueError for a draft generate cannot run: a different vocabulary size, K outside 1..15, options a
+    draft does not combine with, or a draft whose position limit is below reach = prompt + max_tokens."""
+    if draft_model.vocab_size != model.vocab_size:
+        raise ValueError(f"draft_model: vocabulary of {draft_model.vocab_size} tokens, the model has "
+                         f"{model.vocab_size}: the draft must share the target's tokenizer")
+    if isinstance(num_draft_tokens, bool) or not isinstance(num_draft_tokens, int) \
+            or not 1 <= num_draft_tokens <= MAX_DRAFT_TOKENS:
+        raise ValueError(f"num_draft_tokens must be an int in [1, {MAX_DRAFT_TOKENS}], got {num_draft_tokens!r}")
+    for name, given in (("kv_bits", kv_bits is not None), ("max_kv_size (a ring cannot be rewound)",
+                                                             max_kv_size is not None),
+                        ("prompt_cache", prompt_cache is not None), ("num_beams", num_beams is not None),
+                        ("on_step (use on_round)", on_step is not None)):
+        if given:
+            raise ValueError(f"draft_model does not combine with {name}")
+    limit = position_limit(draft_model.args)
+    if limit is not None and reach > limit:
+        raise ValueError(f"draft_model: prompt + max_tokens ({reach}) exceeds the draft's max_position_embeddings "
+                         f"({limit})")
+
+
+def draft_prefill_step(draft_model, prefill_step_size: Optional[int], longest: int) -> Optional[int]:
+    """The draft's prefill chunk: prefill_step_size when Model.extend serves the draft, else None (one piece).
+    Model.extend needs a bf16 model with head_dim 64 or 128, and a prefix-LM prompt cannot be split; a draft outside
+    that (C1: fp32, head_dim 16) is prefilled whole, as such drafts are small."""
+    if prefill_step_size is None:
+        return None
+    try:
+        draft_model.check_extend(None)
+    except ValueError:
+        return None
+    if draft_model.args.prefix_lm and longest > prefill_step_size:
+        return None
+    return prefill_step_size
+
+
+def check_draft_tokenizer(tokenizer, draft_tokenizer) -> None:
+    """Raises ValueError when two runs' tokenizers differ: the byte-level vocabulary size, or the tokenizer file's
+    contents."""
+    def ident(t):  # a core.training.TokenizerManager
+        path = t.config.tokenizer_path if t.external_tokenizer is not None else None
+        data = (Path(path) / "tokenizer.json").read_bytes() if path is not None else None
+        byte_level = t.config.tokenizer.get("normal_vocab_size") if path is None else None
+        return t.VOCAB_SIZE, t.EOS_TOKEN, byte_level, data
+
+    if ident(tokenizer) != ident(draft_tokenizer):
+        raise ValueError("the draft run's tokenizer differs from the target run's (vocabulary or tokenizer file)")
+
+
+def repetition_windows(history: Sequence[int], drafted: Sequence[int], context_size: int) -> List[List[int]]:
+    """The repetition window of each of the k + 1 positions a round samples at, drafted = d_1 .. d_k: position i
+    follows history + drafted[:i] (history ends with the round's input token), repetition_window's rule."""
+    h = list(history)
+    return [repetition_window(h + list(drafted[:i]), context_size) for i in range(len(drafted) + 1)]
+
+
+def draft_counts(emitted: Sequence[int], done: Sequence[bool], K: int, max_tokens: int) -> List[int]:
+    """Tokens each row drafts this round: min(K, max_tokens - emitted[b]) for a live row, 0 for a finished one."""
+    return [0 if d else min(K, max_tokens - n) for n, d in zip(emitted, done)]
+
+
+def accept_drafts(drafted: Sequence[int], sampled: Sequence[int], room: int, eos_token: Optional[int] = None):
+    """One row's accept step.  drafted = d_1 .. d_k (k >= 1), sampled = the target's t_0 .. t_k, t_i sampled after
+    the round's input token and d_1 .. d_i; room >= 1 tokens the row may still emit.  Drafts are accepted while
+    t_i == d_{i+1}; the row emits them and then t_n, the target's token at the first mismatch or its bonus token t_k,
+    cut after the first EOS and at room.  Returns (emitted, n accepted, stopped)."""
+    n = 0
+    while n < len(drafted) and sampled[n] == drafted[n]:
+        n += 1
+    emitted = list(drafted[:n]) + [int(sampled[n])]
+    if eos_token is not None and eos_token in emitted:
+        emitted = emitted[:emitted.index(eos_token) + 1]
+    emitted = emitted[:room]
+    stopped = len(emitted) == room or (eos_token is not None and emitted[-1] == eos_token)
+    return emitted, n, stopped
+
+
+def rewind(base: int, k: int, emitted: Sequence[int], drafted: Sequence[int]):
+    """The caches after a round that started with the target holding base positions (its input token unfed at
+    position base) and drafted k tokens: the target was fed the input and d_1 .. d_k, the draft the input (after any
+    catch-up) and d_1 .. d_{k-1}.  Returns (target length, draft length, the draft's next input): both keep the input
+    and the emitted tokens but the last, which is the next round's input; when all k drafts were accepted the draft
+    never saw d_k, so its next input is [d_k, last]."""
+    keep = base + len(emitted)
+    draft_keep = min(keep, base + k)
+    nxt = [int(emitted[-1])] if draft_keep == keep else [int(drafted[k - 1]), int(emitted[-1])]
+    return keep, draft_keep, nxt
+
+
+def _padded(rows: Sequence[Sequence[int]], device) -> torch.Tensor:
+    t = torch.zeros((len(rows), max(1, max(len(r) for r in rows))), dtype=torch.int64)
+    for b, r in enumerate(rows):
+        t[b, :len(r)] = torch.tensor(list(r), dtype=torch.int64)
+    return t.to(device)
+
+
+def _feed(model, rows: Sequence[Sequence[int]], cache) -> torch.Tensor:
+    """Appends rows[b] (0 to 16 tokens) to row b of the cache; returns the fp32 logits [B, V] after each row's last
+    token (unspecified for an empty row).  One token for every row is a decode step, anything else Model.verify."""
+    device = model.embed_tokens.weight.device
+    counts = [len(r) for r in rows]
+    if all(n == 1 for n in counts):
+        return model.decode_step(_padded(rows, device)[:, 0], cache)
+    logits = model.verify(_padded(rows, device), counts, cache)
+    last = torch.tensor([max(n - 1, 0) for n in counts], device=device)
+    return logits[torch.arange(len(rows), device=device), last]
+
+
+def _speculative(model, draft_model, prompts, logits, cache, draft_cache, max_tokens, K, eos_token, sampler,
+                 on_round):
+    temperature, min_p, top_p, penalty, ctx, gen = sampler
+    penalize = penalty != 1.0 and ctx > 0
+    B = len(prompts)
+
+    def pick(lg: torch.Tensor, idx: List[int], windows) -> List[int]:
+        """Tokens sampled from rows idx of lg only (the others, a finished row's or a padding position's, hold
+        unspecified logits), with windows[i] the repetition window of row idx[i]."""
+        lg = lg[torch.tensor(idx, dtype=torch.int64, device=lg.device)]
+        if penalize:
+            lg = apply_repetition_penalty(lg, windows, penalty)
+        return sample(lg, temperature, min_p, top_p, gen).tolist()
+
+    device = model.embed_tokens.weight.device
+    history = [list(p) for p in prompts]
+    out: List[List[int]] = [[] for _ in prompts]
+    done = [False] * B
+    if max_tokens <= 0:
+        return out
+    # the first token is the target's sample after the prompt, as in plain generation
+    for b, t in enumerate(pick(logits, list(range(B)), [repetition_window(h, ctx) for h in history])):
+        out[b].append(t)
+        history[b].append(t)
+        done[b] = max_tokens == 1 or (eos_token is not None and t == eos_token)
+    base = [len(p) for p in prompts]  # target positions held; the input token out[b][-1] sits at base[b]
+    pending = [[out[b][-1]] for b in range(B)]  # the draft's next input
+    while not all(done):
+        k = draft_counts([len(o) for o in out], done, K, max_tokens)
+        drafted: List[List[int]] = [[] for _ in prompts]
+        dl = _feed(draft_model, [[] if done[b] else pending[b] for b in range(B)], draft_cache)
+        for j in range(max(k)):
+            need = [b for b in range(B) if j < k[b]]  # rows fed this step: the others' logits are unspecified
+            d = dict(zip(need, pick(dl, need, [repetition_window(history[b] + drafted[b], ctx) for b in need])))
+            for b in need:
+                drafted[b].append(d[b])
+            if j + 1 < max(k):
+                dl = _feed(draft_model, [[d[b]] if j + 1 < k[b] else [] for b in range(B)], draft_cache)
+        rows = [[] if done[b] else [out[b][-1]] + drafted[b] for b in range(B)]
+        tl = model.verify(_padded(rows, device), [len(r) for r in rows], cache)  # [B, max k + 1, V]
+        L = tl.shape[1]
+        idx, windows = [], []  # the valid (row, position) pairs: k[b] + 1 per live row
+        for b in range(B):
+            if not done[b]:
+                idx += [b * L + i for i in range(k[b] + 1)]
+                windows += repetition_windows(history[b], drafted[b], ctx)
+        flat = pick(tl.reshape(B * L, -1), idx, windows)
+        t = {}
+        for b in range(B):
+            if not done[b]:
+                t[b], flat = flat[:k[b] + 1], flat[k[b] + 1:]
+        emitted_all: List[List[int]] = [[] for _ in prompts]
+        keep, draft_keep = list(cache.host_lens), list(draft_cache.host_lens)
+        for b in range(B):
+            if done[b]:
+                continue
+            emitted, _, stopped = accept_drafts(drafted[b], t[b], max_tokens - len(out[b]), eos_token)
+            keep[b], draft_keep[b], pending[b] = rewind(base[b], k[b], emitted, drafted[b])
+            base[b] = keep[b]
+            out[b] += emitted
+            history[b] += emitted
+            emitted_all[b] = emitted
+            done[b] = stopped
+        cache.truncate(keep)
+        draft_cache.truncate(draft_keep)
+        if on_round is not None:
+            on_round(emitted_all, drafted)
     return out
 
 
@@ -442,7 +653,22 @@ def parse_args(argv: Optional[List[str]] = None) -> argparse.Namespace:
                     help="Beam search with this many beams, printing every returned beam with its score (default: "
                          "sampling).  The sampling flags (temperature, min-p, top-p, repetition penalty, seed) do not "
                          "apply to it, as in the reference")
+    ap.add_argument("--draft-run", type=str, default=None,
+                    help="Speculative decoding: a run with the same tokenizer whose model drafts tokens for this one")
+    ap.add_argument("--draft-checkpoint", type=str, default=None,
+                    help="Checkpoint of the draft run (default: its final checkpoint)")
+    ap.add_argument("--num-draft-tokens", type=int, default=3,
+                    help="Tokens the draft proposes per round, 1 to 15 (with --draft-run)")
     a = ap.parse_args(argv)
+    if a.draft_run is not None:
+        if not 1 <= a.num_draft_tokens <= MAX_DRAFT_TOKENS:
+            ap.error(f"--num-draft-tokens must lie in [1, {MAX_DRAFT_TOKENS}]")
+        for flag, given in (("--num-beams", a.num_beams is not None), ("--kv-bits", a.kv_bits is not None),
+                            ("--max-kv-size", a.max_kv_size is not None)):
+            if given:
+                ap.error(f"--draft-run does not combine with {flag}")
+    elif a.draft_checkpoint is not None:
+        ap.error("--draft-checkpoint needs --draft-run")
     if a.num_beams is not None:
         if a.num_beams < 1:
             ap.error("--num-beams must be >= 1")
@@ -518,11 +744,29 @@ def main(argv: Optional[List[str]] = None) -> None:
         sys.stdout.flush()
         return
     seed = a.seed if a.seed is not None else random.SystemRandom().randrange(1 << 62)
+    draft, counts = None, [0, 0]
+    if a.draft_run is not None:
+        draft_trainer = load_run(a.draft_run, a.runs_dir, a.draft_checkpoint)
+        check_draft_tokenizer(tok, draft_trainer.tokenizer)
+        draft = draft_trainer.model
+
+    def on_round(emitted, drafted):
+        for e, d in zip(emitted, drafted):
+            n = 0
+            while n < min(len(e), len(d)) and e[n] == d[n]:
+                n += 1
+            counts[0] += n
+            counts[1] += len(d)
+
     outs = generate(trainer.model, [prompt] * a.num_samples, max_tokens=a.max_tokens, temperature=a.temperature,
                     min_p=a.min_p, top_p=a.top_p, repetition_penalty=a.repetition_penalty,
                     repetition_context_size=a.repetition_context_size, eos_token=tok.EOS_TOKEN, seed=seed,
                     kv_bits=a.kv_bits, kv_group_size=a.kv_group_size, quantized_kv_start=a.quantized_kv_start,
-                    prefill_step_size=a.prefill_step_size, max_kv_size=a.max_kv_size)
+                    prefill_step_size=a.prefill_step_size, max_kv_size=a.max_kv_size, draft_model=draft,
+                    num_draft_tokens=a.num_draft_tokens, on_round=on_round if draft is not None else None)
+    if draft is not None:
+        rate = counts[0] / counts[1] if counts[1] else 0.0
+        sys.stderr.write(f"[speculative] {counts[0]} of {counts[1]} draft tokens accepted ({rate:.1%})\n")
     for o in outs:
         print(f"Greedy Output: {tok.detokenize(o)}")
     sys.stdout.flush()

@@ -31,6 +31,8 @@
 // into the reduction buffer, which is free until the key subsets merge.  Per tile each lane converts its key's distance
 // start + lane - (len - 1) once for all G heads, and the online-softmax step adds slope * distance to the score; keys
 // below the tile start or the window stay -inf.  With zero slopes the scores are the window kernel's.
+#include <type_traits>
+
 #include "common.cuh"
 #include "host.h"
 
@@ -101,6 +103,20 @@ struct DecArgs {
     const struct BeamMaps* beam;  // BEAM: the tails' tensor maps and the tables, in global memory
   };
 };
+
+// MULTI (attn_decode_multi): n_q new queries per row, query i of row b at position start[b] + i and valid iff
+// i < lens[b] - start[b] (lens is each row's end).  q / o are [B, n_q, H, D], lse [B, H, n_q], and the partials are
+// those of B * n_q decode rows.  A separate type, so the kernels without MULTI keep their parameters.
+struct DecMultiArgs : DecArgs {
+  const int* start;  // [B]
+  int n_q;
+};
+// MULTI: queries per CTA, so that their (query, q head) pairs fit the accumulators: pack * G * D <= 2048
+__host__ __device__ __forceinline__ int multi_pack(int G, int D) {
+  return max(1, DEC_MAX_ITEMS * DEC_THREADS * 8 / (G * D));
+}
+template <bool MULTI>
+using DecArgsT = std::conditional_t<MULTI, DecMultiArgs, DecArgs>;
 
 // kv0: the first cached key the row's query sees
 __device__ __forceinline__ int first_visible_key(const DecArgs& p, int len) { return max(0, len - 1 - p.window); }
@@ -207,21 +223,48 @@ static_assert(sizeof(BeamMaps) <= BEAM_HDR, "BeamMaps exceeds its workspace head
 // slot at index pos - T0 (an end-anchored tile below T0 reads TMA's zero fill, masked as below position 0).  A prefix
 // chunk is run by the first row of each pack of `pack` consecutive rows of the group only: it reads the prefix tile
 // once for the nb <= pack rows, whose nb * G query heads act as the CTA's heads (head e = row e / G, q head e % G).
-template <typename T, int D, bool ALIBI = false, bool RING = false, bool BEAM = false>
-__global__ void __launch_bounds__(DEC_THREADS, ALIBI || RING || BEAM ? 4 : 0)
-attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV, const DecArgs p) {
+//
+// MULTI: blockIdx.z is (row, pack of multi_pack(G, D) consecutive queries); the CTA's heads are the pack's nb valid
+// queries' G q heads (head e = query qi0 + e / G, q head e % G).  The chunks are the unwindowed kernel's, the CTA reads
+// the hull from the tile holding its first query's kv0 to the chunk's end as seen by the row's last valid query
+// (min(end, c0 + 256), so no position at or past end is read), and each head masks the keys outside its own query's
+// view max(0, pos - W) .. pos.  A tile may hold no visible key for some head: its max stays -inf, and the softmax
+// step then adds nothing.  A query writes only for the chunks its own view touches, finishing itself when that is one.
+template <typename T, int D, bool ALIBI = false, bool RING = false, bool BEAM = false, bool MULTI = false>
+__global__ void __launch_bounds__(DEC_THREADS, ALIBI || RING || BEAM || MULTI ? 4 : 0)
+attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                   const DecArgsT<MULTI> p) {
   const BeamMaps* bm = BEAM ? p.beam : nullptr;  // BEAM: tmK / tmV are the prefix caches
   const BeamArgs* bp = BEAM ? &bm->args : nullptr;
   constexpr int L = D / 8;                        // 8-column slices per row
   constexpr int TILE_ELEMS = DEC_TILE * D;
   constexpr int TILE_BYTES = TILE_ELEMS * (int)sizeof(T);
-  const int c = blockIdx.x, hk = blockIdx.y, b = blockIdx.z;
+  int n_q = 1, qp = 1, n_packs = 1;  // MULTI: queries per row, per CTA, and query packs per row
+  if constexpr (MULTI) {
+    n_q = p.n_q;
+    qp = multi_pack(p.G, D);
+    n_packs = (n_q + qp - 1) / qp;
+  }
+  const int c = blockIdx.x, hk = blockIdx.y, b = MULTI ? blockIdx.z / n_packs : blockIdx.z;
   const int c0 = c * DEC_CHUNK;
   int len, kv0, lo, end, n_chunks;
   RingRow rr;
   int nb = 1, grp = 0, t0 = 0, slot = 0;  // BEAM: rows in this CTA, the row's group, fork point and tail slot
   bool tail = false;
-  if constexpr (RING) {
+  int qi0 = 0, qpos0 = 0;  // MULTI: the CTA's first query and its position
+  if constexpr (MULTI) {
+    len = min(p.lens[b], p.s_max);
+    const int s0 = p.start[b];
+    qi0 = blockIdx.z % n_packs * qp;
+    if (s0 < 0 || qi0 >= min(len - s0, n_q)) return;
+    nb = min(qp, min(len - s0, n_q) - qi0);
+    qpos0 = s0 + qi0;
+    kv0 = max(0, qpos0 - p.window);
+    if (c0 > qpos0 + nb - 1 || c0 + DEC_CHUNK <= kv0) return;
+    lo = max(c0, kv0 & ~(DEC_TILE - 1));
+    end = min(len, c0 + DEC_CHUNK);
+    n_chunks = 0;  // per query, below
+  } else if constexpr (RING) {
     len = p.lens[b];
     if (len < 1) return;
     rr = ring_row(len, p.ring_m, p.s_max, p.window);
@@ -248,7 +291,7 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     n_chunks = (len + DEC_CHUNK - 1) / DEC_CHUNK - kv0 / DEC_CHUNK;  // live chunks of the row
   }
   const int n_tiles = (end - lo + DEC_TILE - 1) / DEC_TILE;
-  const int G = BEAM ? nb * p.G : p.G;
+  const int G = BEAM || MULTI ? nb * p.G : p.G;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   extern __shared__ uint8_t smem_raw[];
@@ -291,13 +334,13 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   if (tid == 0)
     for (int j = 0; j < min(n_tiles, DEC_STAGES); ++j) issue(j);
 
-  if constexpr (BEAM) {
-    // head e of the CTA is q head hk * p.G + e % p.G of row b + e / p.G
+  if constexpr (BEAM || MULTI) {
+    // head e of the CTA is q head hk * p.G + e % p.G of row b + e / p.G (MULTI: of query qi0 + e / p.G of row b)
     for (int i = tid; i < G * L; i += DEC_THREADS) {
       const int e = i / L;
+      const long long row = MULTI ? (long long)b * n_q + qi0 + e / p.G : b + e / p.G;
       float f[8];
-      ld8(reinterpret_cast<const T*>(p.q) + ((long long)(b + e / p.G) * p.H + hk * p.G + e % p.G) * D + (i % L) * 8,
-          f);
+      ld8(reinterpret_cast<const T*>(p.q) + (row * p.H + hk * p.G + e % p.G) * D + (i % L) * 8, f);
 #pragma unroll
       for (int x = 0; x < 8; ++x) sq[i * 8 + x] = f[x] * p.scale_log2;
     }
@@ -314,8 +357,8 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   for (int g = tid; g < G; g += DEC_THREADS) {
     sm[g] = -INFINITY;
     sl[g] = 0.f;
-    if constexpr (ALIBI && !BEAM) sred[g] = __ldg(p.slopes + hk * G + g) * kLog2e;  // G <= DEC_THREADS * 8
-    if constexpr (ALIBI && BEAM) sred[g] = __ldg(p.slopes + hk * p.G + g % p.G) * kLog2e;
+    if constexpr (ALIBI && !BEAM && !MULTI) sred[g] = __ldg(p.slopes + hk * G + g) * kLog2e;  // G <= DEC_THREADS * 8
+    if constexpr (ALIBI && (BEAM || MULTI)) sred[g] = __ldg(p.slopes + hk * p.G + g % p.G) * kLog2e;
   }
 
   // accumulator ownership: item = (head g, slice) with g = item / L; keys my_ks, my_ks + ks_n, ... of every tile
@@ -371,6 +414,10 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
           d = fmaf(qc.w, kf[7], d);
 #pragma unroll
           for (int off = L / 2; off > 0; off >>= 1) d += __shfl_xor_sync(0xffffffffu, d, off);
+          if constexpr (MULTI) {  // the view of head g's query at position qpos
+            const int qpos = qpos0 + g / p.G;
+            valid = start + key <= qpos && start + key >= max(lo + j * DEC_TILE, qpos - p.window);
+          }
           if (kl == 0) ss[g * DEC_TILE + key] = valid ? d : -INFINITY;
         }
       }
@@ -378,24 +425,27 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
     __syncthreads();
 
     // online softmax (log2 domain): one warp per head, one lane per key; every tile holds at least one valid key
-    // (kv0 < end, and kv0 lies in the first tile).  ALIBI: kd = this lane's key distance, converted once per tile
+    // (kv0 < end, and kv0 lies in the first tile), except under MULTI.  ALIBI: kd = this lane's key distance,
+    // converted once per tile (MULTI: per head, from the head's query)
     float kd = 0.f;
-    if constexpr (ALIBI) {
+    if constexpr (ALIBI && !MULTI) {
       int off = 0;
       if constexpr (RING) ring_visible(rr, start + lane, off);
       kd = (float)(start + lane + off - (len - 1));
     }
     for (int g = warp; g < G; g += DEC_THREADS / 32) {
       float x = ss[g * DEC_TILE + lane];
+      if constexpr (ALIBI && MULTI) kd = (float)(start + lane - (qpos0 + g / p.G));
       if constexpr (ALIBI) x = x + sred[g] * kd;
       const float m_old = sm[g];
       const float m_new = fmaxf(m_old, warp_max(x));
-      const float pe = exp2f(x - m_new);
+      const float m_use = MULTI && m_new == -INFINITY ? 0.f : m_new;  // no visible key yet: p = 0, alpha = 0
+      const float pe = exp2f(x - m_use);
       const float sum = warp_sum(pe);
       ss[g * DEC_TILE + lane] = pe;
       __syncwarp();
       if (lane == 0) {
-        const float alpha = exp2f(m_old - m_new);
+        const float alpha = exp2f(m_old - m_use);
         salpha[g] = alpha;
         sl[g] = sl[g] * alpha + sum;
         sm[g] = m_new;
@@ -445,16 +495,24 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
   for (int r = 0; r < DEC_MAX_ITEMS; ++r) {
     if (my_item[r] < 0) continue;
     const int g = my_item[r] / L, sc = my_item[r] % L;
-    const int h = BEAM ? hk * p.G + g % p.G : hk * G + g;
-    const long long bh = (long long)(BEAM ? b + g / p.G : b) * p.H + h;
+    const int h = BEAM || MULTI ? hk * p.G + g % p.G : hk * G + g;
+    const int qi = qi0 + g / p.G;  // MULTI: the head's query
+    const long long bh = (MULTI ? (long long)b * n_q + qi : (long long)(BEAM ? b + g / p.G : b)) * p.H + h;
     const float m = sm[g], l = sl[g];
-    if (n_chunks == 1) {
+    int nc = n_chunks;
+    if constexpr (MULTI) {  // the chunks the query's view touches
+      const int qpos = qpos0 + g / p.G;
+      const int c_first = max(0, qpos - p.window) / DEC_CHUNK, c_last = qpos / DEC_CHUNK;
+      if (c < c_first || c > c_last) continue;
+      nc = c_last - c_first + 1;
+    }
+    if (nc == 1) {
       const float inv = 1.0f / l;
       float f[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) f[e] = acc[r][e] * inv;
       st8(reinterpret_cast<T*>(p.o) + bh * D + sc * 8, f);
-      if (p.lse != nullptr && sc == 0) p.lse[bh] = (m + log2f(l)) / kLog2e;
+      if (p.lse != nullptr && sc == 0) p.lse[MULTI ? ((long long)b * p.H + h) * n_q + qi : bh] = (m + log2f(l)) / kLog2e;
     } else {
       st8(p.part_acc + (bh * p.max_chunks + c) * D + sc * 8, acc[r]);
       if (sc == 0) {
@@ -467,14 +525,25 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constan
 
 // o = sum_c exp2(m_c - M) acc_c / sum_c exp2(m_c - M) l_c over a row's live chunks, in chunk order; one thread per
 // column
-// (RING: over the chunks ring_chunk finds live, the others skipped)
-template <typename T, int D, bool RING = false>
+// (RING: over the chunks ring_chunk finds live, the others skipped; MULTI: blockIdx.y is (row, query), a query's
+// live chunks those of its own view)
+template <typename T, int D, bool RING = false, bool MULTI = false>
 __global__ void __launch_bounds__(D)
-attn_decode_combine_kernel(const DecArgs p) {
+attn_decode_combine_kernel(const DecArgsT<MULTI> p) {
   const int h = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
   int c_lo, n;
   RingRow rr;
-  if constexpr (RING) {
+  long long lse_i = 0;  // MULTI: the query's LSE in [B, H, n_q]
+  if constexpr (MULTI) {
+    const int rb = b / p.n_q, qi = b % p.n_q;
+    const int s0 = p.start[rb];
+    if (s0 < 0 || qi >= min(p.lens[rb], p.s_max) - s0) return;
+    const int len = s0 + qi + 1;
+    c_lo = max(0, len - 1 - p.window) / DEC_CHUNK;
+    n = (len + DEC_CHUNK - 1) / DEC_CHUNK;
+    if (n - c_lo <= 1) return;  // finished by attn_decode_kernel
+    lse_i = ((long long)rb * p.H + h) * p.n_q + qi;
+  } else if constexpr (RING) {
     if (p.lens[b] < 1) return;
     rr = ring_row(p.lens[b], p.ring_m, p.s_max, p.window);
     if (ring_live_chunks(rr) <= 1) return;  // finished by attn_decode_kernel
@@ -506,7 +575,7 @@ attn_decode_combine_kernel(const DecArgs p) {
   const float out = acc / l;
   if constexpr (sizeof(T) == 2) reinterpret_cast<__nv_bfloat16*>(p.o)[bh * D + d] = __float2bfloat16(out);
   else reinterpret_cast<float*>(p.o)[bh * D + d] = out;
-  if (p.lse != nullptr && d == 0) p.lse[bh] = (M + log2f(l)) / kLog2e;
+  if (p.lse != nullptr && d == 0) p.lse[MULTI ? lse_i : bh] = (M + log2f(l)) / kLog2e;
 }
 
 template <typename T, int D, bool ALIBI = false, bool RING = false>
@@ -536,6 +605,38 @@ int launch_decode_d(int D, const CUtensorMap& tmK, const CUtensorMap& tmV, const
     case 32: return launch_decode<T, 32, ALIBI>(tmK, tmV, a, B, Hk, stream);
     case 64: return launch_decode<T, 64, ALIBI>(tmK, tmV, a, B, Hk, stream);
     default: return launch_decode<T, 128, ALIBI>(tmK, tmV, a, B, Hk, stream);
+  }
+}
+
+// MULTI: grid z is (row, query pack), the combine's y (row, query)
+template <typename T, int D, bool ALIBI>
+int launch_decode_multi(const CUtensorMap& tmK, const CUtensorMap& tmV, const DecMultiArgs& a, int B, int Hk,
+                        cudaStream_t stream) {
+  auto kern = attn_decode_kernel<T, D, ALIBI, false, false, true>;
+  const int qp = min(multi_pack(a.G, D), a.n_q);
+  const DecSmem lay(D, (int)sizeof(T), a.G * qp);
+  static int attr_bytes = 0;
+  if (lay.total > 48 * 1024 && lay.total > attr_bytes) {
+    B200_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, lay.total));
+    attr_bytes = lay.total;
+  }
+  kern<<<dim3(a.max_chunks, Hk, B * ((a.n_q + qp - 1) / qp)), DEC_THREADS, lay.total, stream>>>(tmK, tmV, a);
+  B200_CHECK_LAUNCH();
+  if (a.max_chunks > 1) {
+    attn_decode_combine_kernel<T, D, false, true><<<dim3(a.H, B * a.n_q), D, 0, stream>>>(a);
+    B200_CHECK_LAUNCH();
+  }
+  return B200_OK;
+}
+
+template <typename T, bool ALIBI>
+int launch_decode_multi_d(int D, const CUtensorMap& tmK, const CUtensorMap& tmV, const DecMultiArgs& a, int B, int Hk,
+                          cudaStream_t stream) {
+  switch (D) {
+    case 16: return launch_decode_multi<T, 16, ALIBI>(tmK, tmV, a, B, Hk, stream);
+    case 32: return launch_decode_multi<T, 32, ALIBI>(tmK, tmV, a, B, Hk, stream);
+    case 64: return launch_decode_multi<T, 64, ALIBI>(tmK, tmV, a, B, Hk, stream);
+    default: return launch_decode_multi<T, 128, ALIBI>(tmK, tmV, a, B, Hk, stream);
   }
 }
 
@@ -1192,9 +1293,11 @@ int check_quant_format(const char* what, int B, int s_max, int Hk, int D, int bi
 
 // window < 0 means none; slopes selects ALiBi
 // ring_m > 0: a ring of s_max slots (bf16, D 64 / 128) with max_kv_size ring_m
+// start non-null: n_q queries per row from position start[b], lens the rows' ends (attn_decode_multi)
 int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, const int* lens, void* o, float* lse,
                      int window, int B, int s_max, int H, int Hk, int D, float scale, int is_bf16, void* ws,
-                     size_t ws_bytes, cudaStream_t stream, const float* slopes = nullptr, int ring_m = 0) {
+                     size_t ws_bytes, cudaStream_t stream, const float* slopes = nullptr, int ring_m = 0,
+                     const int* start = nullptr, int n_q = 1) {
   B200_CHECK_ARG(B > 0 && H > 0 && Hk > 0 && H % Hk == 0, "attn_decode: bad shape B=%d H=%d Hk=%d", B, H, Hk);
   B200_CHECK_ARG(D == 16 || D == 32 || D == 64 || D == 128, "attn_decode: head_dim %d unsupported (16/32/64/128)", D);
   B200_CHECK_ARG(s_max >= DEC_TILE, "attn_decode: s_max=%d must be >= %d", s_max, DEC_TILE);
@@ -1202,7 +1305,7 @@ int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, co
   B200_CHECK_ARG(G * D <= DEC_MAX_ITEMS * DEC_THREADS * 8, "attn_decode: (H/Hk) * D = %d exceeds %d", G * D,
                  DEC_MAX_ITEMS * DEC_THREADS * 8);
   B200_CHECK_ARG(al16(q) && al16(o) && lens != nullptr, "attn_decode: q / o must be 16-byte aligned, lens non-null");
-  const size_t need = b200_attn_decode_workspace_bytes(B, H, s_max, D);
+  const size_t need = b200_attn_decode_workspace_bytes(B * n_q, H, s_max, D);
   if (ws_bytes < need || (need > 0 && ws == nullptr)) {
     set_error("attn_decode: workspace of %zu bytes, %zu needed", ws_bytes, need);
     return B200_ERR_WORKSPACE;
@@ -1216,14 +1319,14 @@ int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, co
   int rc;
   if ((rc = make_tensor_map(&tmK, k_cache, dt, elem, 4, dims, strides, box, false))) return rc;
   if ((rc = make_tensor_map(&tmV, v_cache, dt, elem, 4, dims, strides, box, false))) return rc;
-  DecArgs a;
+  DecMultiArgs a;
   a.q = q;
   a.o = o;
   a.lse = lse;
   a.lens = lens;
   a.max_chunks = (s_max + DEC_CHUNK - 1) / DEC_CHUNK;
   a.part_acc = reinterpret_cast<float*>(ws);
-  a.part_ml = a.part_acc + (size_t)B * H * a.max_chunks * D;
+  a.part_ml = a.part_acc + (size_t)B * n_q * H * a.max_chunks * D;
   a.H = H;
   a.G = G;
   a.s_max = s_max;
@@ -1231,6 +1334,15 @@ int attn_decode_impl(const void* q, const void* k_cache, const void* v_cache, co
   a.window = window < 0 || window > s_max ? s_max : window;
   a.slopes = slopes;
   a.ring_m = ring_m;
+  a.start = start;
+  a.n_q = n_q;
+  if (start != nullptr) {
+    if (slopes)
+      return is_bf16 ? launch_decode_multi_d<__nv_bfloat16, true>(D, tmK, tmV, a, B, Hk, stream)
+                     : launch_decode_multi_d<float, true>(D, tmK, tmV, a, B, Hk, stream);
+    return is_bf16 ? launch_decode_multi_d<__nv_bfloat16, false>(D, tmK, tmV, a, B, Hk, stream)
+                   : launch_decode_multi_d<float, false>(D, tmK, tmV, a, B, Hk, stream);
+  }
   if (ring_m > 0) {
     a.window = window < 0 ? INT_MAX : window;
     if (slopes)
@@ -1346,6 +1458,29 @@ int b200_attn_decode_ring(const void* q, const void* k_ring, const void* v_ring,
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0, "attn_decode_ring: slopes must be 4-byte aligned");
   return attn_decode_impl(q, k_ring, v_ring, end, o, lse, window, B, C, H, Hk, D, scale, 1, ws, ws_bytes,
                           static_cast<cudaStream_t>(stream), slopes, max_kv);
+}
+
+// Speculative decoding's verify step (the reference's mlx_lm generate with a draft_model): n_q <= 16 new queries per
+// row over its dense cache, query i at position start[b] + i valid iff i < end[b] - start[b] (include/b200_hotpath.h)
+int b200_attn_decode_multi(const void* q, const void* k_cache, const void* v_cache, const int* start, const int* end,
+                           void* o, float* lse, int window, const float* slopes, int B, int n_q, int s_max, int H,
+                           int Hk, int D, float scale, int is_bf16, void* ws, size_t ws_bytes, void* stream) {
+  B200_CHECK_ARG(n_q >= 1 && n_q <= 16, "attn_decode_multi: n_q=%d must lie in [1, 16]", n_q);
+  // grid z is (row, query pack) and the combine's grid y (row, query): both at most B * n_q
+  B200_CHECK_ARG(B > 0 && (long long)B * n_q <= 65535, "attn_decode_multi: B * n_q = %lld exceeds the grid's 65535",
+                 (long long)B * n_q);
+  B200_CHECK_ARG(start != nullptr && end != nullptr && (reinterpret_cast<uintptr_t>(start) & 3u) == 0 &&
+                     (reinterpret_cast<uintptr_t>(end) & 3u) == 0,
+                 "attn_decode_multi: start and end must be non-null, 4-byte aligned int32 [B] arrays");
+  B200_CHECK_ARG(slopes == nullptr || (reinterpret_cast<uintptr_t>(slopes) & 3u) == 0,
+                 "attn_decode_multi: slopes must be a 4-byte aligned fp32 [H] array");
+  return attn_decode_impl(q, k_cache, v_cache, end, o, lse, window, B, s_max, H, Hk, D, scale, is_bf16, ws, ws_bytes,
+                          static_cast<cudaStream_t>(stream), slopes, 0, start, n_q);
+}
+
+size_t b200_attn_decode_multi_workspace_bytes(int B, int n_q, int H, int s_max, int D) {
+  if (n_q <= 0) return 0;
+  return b200_attn_decode_workspace_bytes(B * n_q, H, s_max, D);
 }
 
 // The token a decode step appends to a ring (core/generation_lite.py:103, :120): rotated at position end[b] - 1,

@@ -1104,6 +1104,59 @@ def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     return (o, lse) if return_lse else o
 
 
+MULTI_MAX_QUERIES = 16  # queries per row of attention_decode_multi
+
+
+def attention_decode_multi_workspace_bytes(B: int, L: int, H: int, s_max: int, D: int) -> int:
+    return int(lib().b200_attn_decode_multi_workspace_bytes(B, L, H, s_max, D))
+
+
+def attention_decode_multi(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, start: torch.Tensor,
+                           end: torch.Tensor, scale: Optional[float] = None, workspace: Optional[torch.Tensor] = None,
+                           window: Optional[int] = None, alibi: Optional[torch.Tensor] = None,
+                           return_lse: bool = False):
+    """A short chunk of L <= 16 new queries per row against the dense KV cache that already holds their keys
+    (b200_attn_decode_multi): speculative decoding's verify step, split over keys as attention_decode is.
+
+    q [B,L,H,D]; k_cache, v_cache [B,s_max,Hk,D]; all bf16 or all fp32, D in {16, 32, 64, 128}.  start, end: int32
+    [B] on the device.  Query i of row b sits at position p = start[b] + i and sees the cached keys max(0, p - window)
+    .. p (window None: from 0), with ALiBi's bias alibi[h] * (k - p) when alibi (fp32 [H] slopes) is given.  Rows
+    i >= end[b] - start[b] are padding: the kernel does not write them, and o and lse hold 0 there.  Cache positions at or past end[b] are never read.  The values of
+    start and end are not checked here (that would read the device): 0 <= start[b] <= end[b] <= s_max.  `workspace`
+    (uint8, at least attention_decode_multi_workspace_bytes(B, L, H, s_max, D)) is allocated when not given.  With
+    L = 1 the result is bit-equal to attention_decode with lens = end.  Returns o [B,L,H,D] in q's dtype, and the
+    natural-log LSE [B,H,L] fp32 with return_lse."""
+    what = "attention_decode_multi"
+    _is_bf16(q, "q")
+    for t, nm in ((q, "q"), (k_cache, "k_cache"), (v_cache, "v_cache")):
+        _need(t, q.dtype, f"{what}: {nm}")
+    if q.dim() != 4 or k_cache.dim() != 4 or k_cache.shape != v_cache.shape:
+        raise ValueError(f"{what}: expected q [B,L,H,D] and k_cache == v_cache [B,s_max,Hk,D], got "
+                         f"{tuple(q.shape)}, {tuple(k_cache.shape)}, {tuple(v_cache.shape)}")
+    B, L, H, D = q.shape
+    Bc, s_max, Hk, Dc = k_cache.shape
+    if Bc != B or Dc != D or H % Hk != 0:
+        raise ValueError(f"{what}: q {tuple(q.shape)} does not match cache {tuple(k_cache.shape)}")
+    if D not in (16, 32, 64, 128):
+        raise ValueError(f"{what}: head_dim {D} unsupported (16, 32, 64 or 128)")
+    if not 1 <= L <= MULTI_MAX_QUERIES:
+        raise ValueError(f"{what}: {L} queries per row, 1 to {MULTI_MAX_QUERIES} supported")
+    _check_rows(start, B, q.device, what, "start")
+    _check_rows(end, B, q.device, what, "end")
+    window, alibi, scale = _check_scores(q, scale, window, alibi, what)
+    workspace = _check_workspace(workspace, attention_decode_multi_workspace_bytes(B, L, H, s_max, D), q.device, what)
+    o = torch.zeros_like(q)
+    lse = torch.zeros((B, H, L), device=q.device, dtype=torch.float32) if return_lse else None
+    tok = _t0("attn_decode_multi")
+    check(lib().b200_attn_decode_multi(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), start.data_ptr(),
+                                       end.data_ptr(), o.data_ptr(), _ptr(lse),
+                                       -1 if window is None else min(int(window), s_max), _ptr(alibi), B, L, s_max, H,
+                                       Hk, D, float(scale), _is_bf16(q, "q"), workspace.data_ptr(), workspace.numel(),
+                                       _stream()), "b200_attn_decode_multi")
+    _t1(tok)
+    return (o, lse) if return_lse else o
+
+
 def kv_append(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor,
               lens: torch.Tensor, rope_tables: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
               layout: str = "interleaved") -> None:
