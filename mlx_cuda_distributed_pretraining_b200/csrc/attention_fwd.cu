@@ -12,31 +12,19 @@
 //                   online softmax on the fp32 accumulators in registers, then O += P V as wgmma with P as the
 //                   register A operand (the accumulator fragment packed to bf16) and V read MN-major from smem.
 //
-// Document variant (DOC = true, packed sequences): pos[b, s] is token s's position within its document, so query q
-// sees keys q - pos[q] .. q.  The key loop starts at the tile of the CTA's first query's document start (doc starts
-// are monotone in q, so that is the lowest start of the CTA's rows) and the extra `key < q - pos[q]` mask runs only
-// on tiles below the CTA's highest document start.  Rows with no visible key in a tile pass through the online
-// softmax as the causal rows do (m_use).  DOC = false compiles to the causal / non-causal kernel unchanged.
-//
-// Sliding window (same DOC instantiation): query q sees keys q - min(pos[q], W) .. q, i.e. the document mask with pos
-// clamped at W, which keeps the starts monotone in q.  pos == nullptr reads as pos[q] = q (one document per row), so
-// an unpacked windowed launch needs no [B, S] buffer.  Without a window W = S, and min(pos[q], S) = pos[q].
-//
-// ALiBi (ALIBI = true, DOC kernels only): every score gets the bias m_h (k - q) <= 0 of the query head's slope
-// m_h = slopes[h], added to the scaled score before the mask and the softmax, on every tile.  In log2 units the bias is
-// b = m_h log2e (k - q).  A thread's keys in a tile are k0 + 2 (lane % 4) + c with the compile-time column c = 8 nc +
-// {0, 1}, so each tile converts one integer per row, base = m log2e (k0 + 2 (lane % 4) - row), and the element's bias
-// is fmaf(m log2e, c, base): no int -> float conversion per element (that pipe is the one exp2 already fills).  With
-// m = 0 the bias is exactly 0 and the scores are the DOC kernel's.  k - q is also the distance within a document, so
-// packed rows need nothing more.  ALIBI = false compiles to the kernels above unchanged.
-//
-// Prefix-LM (PREFIX = true, causal DOC = false kernels only): row b has a prefix length P_b = prefix[b], clamped to
-// [0, S] in the kernel so that no value can send the key loop past the sequence.  Query q sees key k iff k <= q or
-// k < P_b: the prefix attends bidirectionally within itself and later queries are causal over everything before them.
-// The visible keys of a query are still 0 .. max(q, P_b - 1), monotone in q, so the key loop ends at
-// max(causal end, ceil(P_b / 128)) and the element mask `key >= S || (key > row && key >= P_b)` runs only on tiles
-// whose last key exceeds max(q0, P_b - 1) or that cross S.  P_b <= 1 is the causal mask (the same tiles, the same
-// values); P_b = S is the non-causal one.  PREFIX = false compiles to the kernels above unchanged.
+// Masks.  In every variant the keys query row r (at position q) sees are one interval [lo, hi] (row_keys):
+//   causal / non-causal         [0, min(r, S - 1)] / [0, S - 1]
+//   DOC (documents, window)     [r - min(pos[r], W), min(r, S - 1)]   (pos == nullptr reads as pos[r] = r)
+//   PREFIX                      [0, min(max(r, P_b - 1), S - 1)],  P_b = prefix[b] clamped to [0, S]
+//   CACHED                      [max(0, q - W), q],  q = start[b] + min(r, n_b - 1)
+//   RING                        [max(lo_t, q - W_t), q],  lo_t / W_t of the tile's slot range (below)
+// Both ends rise with r, so a CTA's key tiles run from its first row's lo to its last row's hi, and a tile is masked
+// only when it reaches past a thread's first row's hi or below its second row's lo.  Each score is scaled into the
+// log2 domain, gets the ALiBi bias m_h log2e (k - q) (ALIBI), is set to -inf outside its row's interval and then
+// enters the online softmax; a row with no visible key in a tile passes through as m_use shows.  ALiBi's bias is
+// fmaf(m log2e, c, base) of the compile-time column c, one int -> float conversion per row and tile.  The intervals
+// are formed per tile from the rows' positions: CACHED's window starts, held across the key loop, pushed D = 128 into
+// spills, and RING's depend on the tile's slot range.
 //
 // Dropout (DROP = true, on the causal / non-causal and the DOC / ALiBi kernels): O = (P o Z / (1 - p_eff)) V as
 // arch/flash_attention.py:146-148 of the reference applies mx.dropout after the softmax.  The softmax P, its row sums
@@ -46,30 +34,26 @@
 // mask depends on positions only, never on the tiling.  A quad's rows are one (row, 8-key chunk) Philox call per
 // chunk nc, whose word w[l] holds exactly lane l's keys 8 nc + 2 l + {0, 1}; so each lane computes 8 of the tile's
 // 32 calls (both rows, chunks nc = 4 m + l) and the quad exchanges the 8-bit results with 4 shuffles per row.  Bit
-// 2 nc + c of keep[r] is this thread's key 8 nc + 2 l + c of row r.  DROP = false compiles to the kernels above
-// unchanged.
+// 2 nc + c of keep[r] is this thread's key 8 nc + 2 l + c of row r.
 //
-// Cached queries (CACHED = true, on the causal DOC = false kernels, with or without ALiBi): a chunk of L queries per
-// row attends over a KV cache [B, s_max, Hk, D] that already holds its own keys.  Query row i of batch row b sits at
-// position p = start[b] + i and sees key k iff max(0, p - W) <= k <= p, for the rows i < n_b = end[b] - start[b];
-// rows i >= n_b are padding.  Each CTA reads start[b] and end[b] itself.  A CTA with only padding rows writes zeros
-// and returns.  Otherwise its key tiles are anchored at kend, one past its last valid row's position (kend <= end[b]):
-// tile j holds keys kend - 128 (n_kv - j) .., so no cache position at or past kend is ever loaded (those may hold
-// anything, and 0 * NaN would reach O through the P V MMA); keys below 0 are TMA's zero fill and masked.  The element
-// mask `key > p || key < max(0, p - W)` runs, per thread, on the tiles its rows' diagonal crosses (at most two, as
-// the tiles are not aligned to the queries) and on those reaching below its rows' window start.  Padding rows take the last valid
-// row's position and their Q rows are zeroed in shared memory, so their outputs are finite whatever Q holds there.
-// CACHED = false compiles to the kernels above unchanged.
+// Cached queries (CACHED = true, on the causal kernels, with or without ALiBi): a chunk of L queries per row attends
+// over a KV cache [B, s_max, Hk, D] that already holds its own keys; query row i of batch row b sits at position
+// start[b] + i, and rows i >= n_b = end[b] - start[b] are padding.  A CTA with only padding rows writes zeros and
+// returns.  Otherwise its key tiles are anchored at one past its last valid row's position (<= end[b]), so no cache
+// position at or past it is ever loaded (those may hold anything, and 0 * NaN would reach O through the P V MMA);
+// keys below 0 are TMA's zero fill and masked.  Padding rows take the last valid row's position and their Q rows are
+// zeroed in shared memory, so their outputs are finite whatever Q holds there.
 //
 // Rotating cache (RING = true, on the CACHED kernels): the cache is a ring of C = s_max slots holding position t in
 // slot(t) (common.cuh, ring_slot), and query position q sees key position k iff k <= q, q - k <= W and (k < 4 or
 // q - k <= M - 5).  The CTA's queries q_lo .. q_hi see the sinks and the arc A = max(4, q_lo - min(M - 5, W)) .. q_hi,
 // whose slots form at most two ranges (the arc wraps at most once, as C >= M + L - 1).  Thread 0 writes a table of
 // three slot ranges into shared memory: the sink tile (ending at slot min(4, q_hi + 1)), then the arc's ranges, each
-// tiled by 128-slot tiles anchored at the range's end.  Inside a range position = slot + off, and the keys below its
-// first position are masked like those below a window start, so the loop, its masks and ALiBi run on positions as in
-// the cached kernel.  No slot at or past end[b] is loaded before the ring first wraps; after it every slot holds a
-// written key.  RING = false compiles to the kernels above unchanged.
+// tiled by 128-slot tiles anchored at the range's end.  Inside a range position = slot + off, and a range's keys are
+// masked below its first position lo_t, with W_t = W for the sinks and min(M - 5, W) for the arc.  No slot at or past
+// end[b] is loaded before the ring first wraps; after it every slot holds a written key.
+//
+// Each flag set to false compiles to the kernels without it.
 #include "common.cuh"
 #include "host.h"
 
@@ -101,7 +85,7 @@ struct FwdArgs {
   float scale;
   int causal;
   const int* pos;  // [B, S] positions within documents (DOC kernels only; null: pos[q] = q)
-  int window;      // DOC: query q sees keys from q - min(pos[q], window); S when there is no window
+  int window;      // query q sees keys from q - min(pos[q], window) (CACHED: q - window); INT_MAX for none
   const float* slopes;  // ALIBI: [H] fp32 per-query-head slopes
   const int* prefix;    // PREFIX: [B] int32 prefix lengths (clamped to [0, S])
   uint32_t drop_t;      // DROP: keep threshold t = round(p 65536) on the 16-bit Philox values
@@ -161,6 +145,27 @@ __device__ __forceinline__ int key_start(const FwdArgs& p, int b, int row) {
   return p.pos ? row - min(__ldg(p.pos + (long long)b * p.S + row), p.window) : max(0, row - p.window);
 }
 
+// The position of query row `row`, from which ALiBi measures k - q: the row itself, or for CACHED start[b] + row
+// (c_st, c_nv: the batch row's first position and valid rows), where a padding row takes the last valid row's
+template <bool CACHED>
+__device__ __forceinline__ int row_pos(int row, int c_st, int c_nv) {
+  return CACHED ? c_st + min(row, c_nv - 1) : row;
+}
+
+// The keys [lo, hi] that the query at position q (row_pos) sees, as in the table at the head of this file.  dstart:
+// DOC, the row's key_start; pfx: PREFIX, the batch row's prefix length; ring_lo / ring_w: RING, the first position
+// and the window of the tile's slot range (ring_tile).
+struct RowKeys {
+  int lo, hi;
+};
+template <bool DOC, bool PREFIX, bool CACHED, bool RING>
+__device__ __forceinline__ RowKeys row_keys(const FwdArgs& p, int q, int dstart, int pfx, int ring_lo = 0,
+                                            int ring_w = 0) {
+  if constexpr (CACHED) return {RING ? max(ring_lo, q - ring_w) : max(0, q - p.window), q};
+  const int last = p.S - 1;
+  return {DOC ? dstart : 0, PREFIX ? min(max(q, pfx - 1), last) : p.causal ? min(q, last) : last};
+}
+
 // DROP: keep bits of a thread's 2 x 32 scores in the key tile from k0 (rows row_a, row_a + 8).  Byte m of lane L's
 // `own` is chunk 4 m + L of row r; this lane takes bits 2 (lane % 4) + {0, 1} of every byte.
 __device__ __forceinline__ void drop_keep_bits(const FwdArgs& p, int k0, int row_a, int h, int b, int lane,
@@ -207,19 +212,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int hk = h / (p.H / p.Hk);
   const int q0 = qt * ATT_BQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_kv_all = (p.S + ATT_BKV - 1) / ATT_BKV;
-  int n_kv = p.causal ? min(n_kv_all, (q0 + ATT_BQ - 1) / ATT_BKV + 1) : n_kv_all;
-  // PREFIX: this row's prefix length, and the key loop extended to the last tile holding a prefix key
-  int pfx = 0;
-  if constexpr (PREFIX) {
-    pfx = min(max(__ldg(p.prefix + b), 0), p.S);
-    n_kv = max(n_kv, (pfx + ATT_BKV - 1) / ATT_BKV);
-  }
-  // first key tile: the first query's document / window start (0 without documents)
-  int j0 = 0;
-  if constexpr (DOC) j0 = max(0, key_start(p, b, q0)) / ATT_BKV;
-  // CACHED: the row's first query position and valid rows, and the first key of tile 0
-  int c_st = 0, c_nv = 0, kbase = 0;
+  const int pfx = PREFIX ? min(max(__ldg(p.prefix + b), 0), p.S) : 0;
+  // CACHED: the row's first query position and valid rows
+  int c_st = 0, c_nv = 0;
   if constexpr (CACHED) {
     c_st = max(__ldg(p.start + b), 0);
     c_nv = min((RING ? __ldg(p.end + b) : min(__ldg(p.end + b), p.s_max)) - c_st, p.S);
@@ -232,13 +227,22 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       }
       return;
     }
-    const int kend = c_st + min(q0 + ATT_BQ, c_nv);
-    if constexpr (RING) {
-      if (threadIdx.x == 0) ring_table(ring_tab, c_st + q0, kend - 1, p.s_max, p.ring_m, p.window);
-    } else {
-      n_kv = (kend - max(0, c_st + q0 - p.window) + ATT_BKV - 1) / ATT_BKV;
-      kbase = kend - n_kv * ATT_BKV;
-    }
+  }
+  // key tiles from the CTA's first row's first key to its last row's last; CACHED: tile j holds keys
+  // kbase + 128 j .., anchored at the last one
+  const int q_first = row_pos<CACHED>(q0, c_st, c_nv);
+  const int q_last = row_pos<CACHED>(min(q0 + ATT_BQ, p.S) - 1, c_st, c_nv);
+  const RowKeys first = row_keys<DOC, PREFIX, CACHED, RING>(p, q_first, DOC ? key_start(p, b, q0) : 0, pfx);
+  const RowKeys last = row_keys<DOC, PREFIX, CACHED, RING>(p, q_last, 0, pfx);
+  int j0 = 0, n_kv = 0, kbase = 0;
+  if constexpr (RING) {
+    if (threadIdx.x == 0) ring_table(ring_tab, q_first, q_last, p.s_max, p.ring_m, p.window);
+  } else if constexpr (CACHED) {
+    n_kv = (last.hi + 1 - first.lo + ATT_BKV - 1) / ATT_BKV;
+    kbase = last.hi + 1 - n_kv * ATT_BKV;
+  } else {
+    j0 = max(0, first.lo) / ATT_BKV;
+    n_kv = last.hi / ATT_BKV + 1;
   }
 
   if (threadIdx.x == 0) {
@@ -285,25 +289,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   float m_r[2] = {-INFINITY, -INFINITY}, l_r[2] = {0.f, 0.f};
   const float sl2 = p.scale * kLog2e;
   const int row_a = q0 + wg * 64 + wq * 16 + (lane >> 2);  // this thread's rows: row_a, row_a + 8
-  // DOC: document / window start of each of this thread's rows, and the highest start of the CTA's rows (its last
-  // row's)
-  int dstart[2] = {0, 0}, dstart_hi = 0;
+  // DOC: document / window start of each of this thread's rows; a row past S takes the last row's, which keeps the
+  // starts rising with the row as the edge-tile test needs
+  int dstart[2] = {0, 0};
   if constexpr (DOC) {
-    dstart_hi = key_start(p, b, min(q0 + ATT_BQ, p.S) - 1);
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int row = row_a + 8 * r;
-      dstart[r] = row < p.S ? key_start(p, b, row) : 0;
-    }
+    for (int r = 0; r < 2; ++r) dstart[r] = key_start(p, b, min(row_a + 8 * r, p.S - 1));
   }
+  // CACHED: the positions of this thread's rows, held across the key loop (elsewhere a row's position is the row)
+  const int qpos[2] = {row_pos<CACHED>(row_a, c_st, c_nv), row_pos<CACHED>(row_a + 8, c_st, c_nv)};
   float ml2 = 0.f;  // ALIBI: this head's slope in log2 units
   if constexpr (ALIBI) ml2 = __ldg(p.slopes + h) * kLog2e;
-  // CACHED: the position of each of this thread's rows (a padding row takes the last valid row's)
-  int prow[2] = {0, 0};
-  if constexpr (CACHED) {
-#pragma unroll
-    for (int r = 0; r < 2; ++r) prow[r] = c_st + min(row_a + 8 * r, c_nv - 1);
-  }
   mbar_wait(q_full, 0);
   if constexpr (CACHED) {
     // padding rows of Q may hold anything: zero this warpgroup's (each 128-byte row of a 64-column block is one
@@ -326,6 +322,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const uint32_t tK = sK + s * Cfg::KV_BYTES, tV = sV + s * Cfg::KV_BYTES;
     int k0 = kbase + j * ATT_BKV;
 
+    int ring_lo = 0, ring_w = 0;
+    if constexpr (RING) {  // the tile's first position and its slot range's bounds
+      int r, off;
+      k0 = ring_tile(ring_tab, j, r, off, ring_lo) + off;
+      ring_w = r == 0 ? p.window : min(p.ring_m - 5, p.window);
+    }
     // S = Q K^T: 64 rows x 128 keys per warpgroup, both operands K-major (head dim contiguous)
     float sc[64];
 #pragma unroll
@@ -340,104 +342,46 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_commit();
     wgmma_wait<0>();
 
-    if constexpr (DOC) {
-      if (k0 < dstart_hi) {  // the tile reaches below some row's document start
+    // scale (log2 domain), bias, mask, online softmax.  Accumulator chunk nc holds keys k_lane + c, c = 8 nc + {0, 1};
+    // row r sees the columns c_lo[r] .. c_hi[r].  Only a tile that some row's range does not cover is masked (edge);
+    // both ends of the ranges rise with the row.  The bias gets a pass of its own: in the mask's pass, with the
+    // bounds, it pushed the D = 128 ALiBi kernels into spills.
+    RowKeys rk[2];
 #pragma unroll
-        for (int nc = 0; nc < 16; ++nc) {
+    for (int r = 0; r < 2; ++r)
+      rk[r] = row_keys<DOC, PREFIX, CACHED, RING>(p, CACHED ? qpos[r] : (row_a + 8 * r), dstart[r], pfx, ring_lo,
+                                                  ring_w);
+    const bool edge = k0 + ATT_BKV - 1 > rk[0].hi || k0 < rk[1].lo;
+    const int k_lane = k0 + (lane & 3) * 2;
+    float abase[2] = {0.f, 0.f};  // ALIBI: the bias m log2e (key - q) of column c is fmaf(m log2e, c, abase[r])
+    int c_lo[2], c_hi[2];
 #pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
-            if (key < dstart[e >> 1]) sc[4 * nc + e] = -INFINITY;
-          }
-        }
-      }
+    for (int r = 0; r < 2; ++r) {
+      c_lo[r] = rk[r].lo - k_lane;
+      c_hi[r] = rk[r].hi - k_lane;
+      if constexpr (ALIBI) abase[r] = ml2 * (float)(k_lane - (CACHED ? qpos[r] : (row_a + 8 * r)));
     }
-
-    // scale (log2 domain), mask, online softmax; accumulator chunk nc holds keys 8 nc + 2 (lane % 4) + {0, 1}
     float mx[2] = {-INFINITY, -INFINITY};
-    if constexpr (CACHED) {
-      // keys k_lane + c, c = 8 nc + (e & 1); ALiBi's bias m log2e (key - p) is fmaf(m log2e, c, abase[r]) as below.
-      // The rows' window starts are formed per tile: kept across the loop they push D = 128 into spills.
-      // RING: the tile's position and its range's bounds are read here, after the S MMAs, for the same reason.
-      int ring_lo = 0, ring_w = 0;
-      if constexpr (RING) {
-        int r, off;
-        k0 = ring_tile(ring_tab, j, r, off, ring_lo) + off;
-        ring_w = r == 0 ? p.window : min(p.ring_m - 5, p.window);
-      }
-      const int plo[2] = {RING ? max(ring_lo, prow[0] - ring_w) : max(0, prow[0] - p.window),
-                          RING ? max(ring_lo, prow[1] - ring_w) : max(0, prow[1] - p.window)};
-      const bool edge = k0 + ATT_BKV - 1 > prow[0] || k0 < plo[1];  // prow[0] <= prow[1]
-      const int k_lane = k0 + (lane & 3) * 2;
-      float abase[2] = {0.f, 0.f};
-      if constexpr (ALIBI) {
 #pragma unroll
-        for (int r = 0; r < 2; ++r) abase[r] = ml2 * (float)(k_lane - prow[r]);
-      }
+    for (int nc = 0; nc < 16; ++nc) {
 #pragma unroll
-      for (int nc = 0; nc < 16; ++nc) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int c = nc * 8 + (e & 1);
-          float x = sc[4 * nc + e] * sl2;
-          if constexpr (ALIBI) x += fmaf(ml2, (float)c, abase[e >> 1]);
-          if (edge && (k_lane + c > prow[e >> 1] || k_lane + c < plo[e >> 1])) x = -INFINITY;
-          sc[4 * nc + e] = x;
-          mx[e >> 1] = fmaxf(mx[e >> 1], x);
-        }
-      }
-    } else if constexpr (ALIBI) {
-      // keys k0 + 2 (lane % 4) + c with the compile-time column c = 8 nc + (e & 1): row r sees c <= c_hi[r] (causal,
-      // in bounds), and its bias is fmaf(m log2e, c, abase[r]) with abase[r] = m log2e (k0 + 2 (lane % 4) - row)
-      const int k_lane = k0 + (lane & 3) * 2;
-      int c_hi[2];
-      float abase[2];
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int row = row_a + 8 * r;
-        c_hi[r] = min(row, p.S - 1) - k_lane;
-        abase[r] = ml2 * (float)(k_lane - row);
-      }
-#pragma unroll
-      for (int nc = 0; nc < 16; ++nc) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int c = nc * 8 + (e & 1);
-          float x = sc[4 * nc + e] * sl2 + fmaf(ml2, (float)c, abase[e >> 1]);
-          if (c > c_hi[e >> 1]) x = -INFINITY;
-          sc[4 * nc + e] = x;
-          mx[e >> 1] = fmaxf(mx[e >> 1], x);
-        }
-      }
-    } else if constexpr (PREFIX) {
-      // tiles wholly inside the prefix or at or below every row's diagonal, and inside S, are visible throughout
-      const bool edge = k0 + ATT_BKV - 1 > max(q0, pfx - 1) || k0 + ATT_BKV > p.S;
-#pragma unroll
-      for (int nc = 0; nc < 16; ++nc) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
-          const int row = row_a + ((e >> 1) << 3);
-          float x = sc[4 * nc + e] * sl2;
-          if (edge && (key >= p.S || (key > row && key >= pfx))) x = -INFINITY;
-          sc[4 * nc + e] = x;
-          mx[e >> 1] = fmaxf(mx[e >> 1], x);
-        }
-      }
-    } else {
-#pragma unroll
-      for (int nc = 0; nc < 16; ++nc) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int key = k0 + nc * 8 + (lane & 3) * 2 + (e & 1);
-          const int row = row_a + ((e >> 1) << 3);
-          float x = sc[4 * nc + e] * sl2;
-          if (key >= p.S || (p.causal && key > row)) x = -INFINITY;
-          sc[4 * nc + e] = x;
-          mx[e >> 1] = fmaxf(mx[e >> 1], x);
-        }
+      for (int e = 0; e < 4; ++e) {
+        const int c = nc * 8 + (e & 1);
+        float x = sc[4 * nc + e] * sl2;
+        if constexpr (ALIBI) x += fmaf(ml2, (float)c, abase[e >> 1]);
+        sc[4 * nc + e] = x;
       }
     }
+#pragma unroll
+    for (int nc = 0; nc < 16; ++nc) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int c = nc * 8 + (e & 1);
+        sc[4 * nc + e] = edge && (c < c_lo[e >> 1] || c > c_hi[e >> 1]) ? -INFINITY : sc[4 * nc + e];
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sc[i]);
     float alpha[2], m_use[2];
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -541,6 +485,13 @@ int launch_fwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap
   return B200_OK;
 }
 
+template <bool DOC, bool ALIBI = false, bool PREFIX = false, bool DROP = false, bool CACHED = false, bool RING = false>
+int launch_fwd_d(int D, const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const FwdArgs& a,
+                 cudaStream_t stream) {
+  return D == 64 ? launch_fwd<64, DOC, ALIBI, PREFIX, DROP, CACHED, RING>(tmQ, tmK, tmV, a, stream)
+                 : launch_fwd<128, DOC, ALIBI, PREFIX, DROP, CACHED, RING>(tmQ, tmK, tmV, a, stream);
+}
+
 }  // namespace
 
 // [B, S, heads, D] bf16 tensor -> 4-D tensor map {D, heads, S, B}, box {64, 1, rows, 1}, 128B swizzle
@@ -553,12 +504,14 @@ int make_bshd_map(CUtensorMap* tm, const void* base, int B, int S, int heads, in
 
 namespace {
 
-// doc selects the document / window instantiation; window < 0 means none; slopes (doc only) selects ALiBi; prefix
-// (causal, not doc) selects the prefix-LM kernels; drop selects the dropout kernels (not with prefix)
+// doc selects the document / window instantiation; window < 0 means none; slopes selects ALiBi; prefix (causal, not
+// doc) the prefix-LM kernels; drop the dropout kernels (not with prefix); start the cached queries (not doc), over a
+// K / V cache of s_max positions, and ring_m > 0 their rotating cache of s_max slots
 int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* lse, bool doc, const int* pos,
                   int window, int B, int S, int H, int Hk, int D, float scale, int causal, cudaStream_t stream,
                   const float* slopes = nullptr, const int* prefix = nullptr, bool drop = false,
-                  uint32_t drop_t = 0, float drop_inv = 1.f, unsigned long long drop_seed = 0) {
+                  uint32_t drop_t = 0, float drop_inv = 1.f, unsigned long long drop_seed = 0,
+                  const int* start = nullptr, const int* end = nullptr, int s_max = 0, int ring_m = 0) {
   B200_CHECK_ARG(B > 0 && S > 0 && H > 0 && Hk > 0 && H % Hk == 0,
                  "attn_fwd: bad shape B=%d S=%d H=%d Hk=%d", B, S, H, Hk);
   B200_CHECK_ARG(D == 64 || D == 128, "attn_fwd: head_dim %d unsupported (64 or 128; pad smaller dims)", D);
@@ -566,8 +519,8 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   CUtensorMap tmQ, tmK, tmV;
   int rc;
   if ((rc = make_bshd_map(&tmQ, q, B, S, H, D, ATT_BQ))) return rc;
-  if ((rc = make_bshd_map(&tmK, k, B, S, Hk, D, ATT_BKV))) return rc;
-  if ((rc = make_bshd_map(&tmV, v, B, S, Hk, D, ATT_BKV))) return rc;
+  if ((rc = make_bshd_map(&tmK, k, B, start ? s_max : S, Hk, D, ATT_BKV))) return rc;
+  if ((rc = make_bshd_map(&tmV, v, B, start ? s_max : S, Hk, D, ATT_BKV))) return rc;
   FwdArgs a;
   a.o = reinterpret_cast<__nv_bfloat16*>(o);
   a.lse = lse;
@@ -578,32 +531,31 @@ int attn_fwd_impl(const void* q, const void* k, const void* v, void* o, float* l
   a.scale = scale;
   a.causal = causal;
   a.pos = pos;
-  a.window = window < 0 || window > S ? S : window;
+  a.window = window < 0 ? INT_MAX : window;
   a.slopes = slopes;
   a.prefix = prefix;
   a.drop_t = drop_t;
   a.drop_inv = drop_inv;
   a.drop_seed = drop_seed;
-  a.start = a.end = nullptr;
-  a.s_max = 0;
+  a.start = start;
+  a.end = end;
+  a.s_max = s_max;
+  a.ring_m = ring_m;
+  if (start && ring_m > 0)
+    return slopes ? launch_fwd_d<false, true, false, false, true, true>(D, tmQ, tmK, tmV, a, stream)
+                  : launch_fwd_d<false, false, false, false, true, true>(D, tmQ, tmK, tmV, a, stream);
+  if (start)
+    return slopes ? launch_fwd_d<false, true, false, false, true>(D, tmQ, tmK, tmV, a, stream)
+                  : launch_fwd_d<false, false, false, false, true>(D, tmQ, tmK, tmV, a, stream);
   if (drop) {
-    if (slopes)
-      return D == 64 ? launch_fwd<64, true, true, false, true>(tmQ, tmK, tmV, a, stream)
-                     : launch_fwd<128, true, true, false, true>(tmQ, tmK, tmV, a, stream);
-    if (doc)
-      return D == 64 ? launch_fwd<64, true, false, false, true>(tmQ, tmK, tmV, a, stream)
-                     : launch_fwd<128, true, false, false, true>(tmQ, tmK, tmV, a, stream);
-    return D == 64 ? launch_fwd<64, false, false, false, true>(tmQ, tmK, tmV, a, stream)
-                   : launch_fwd<128, false, false, false, true>(tmQ, tmK, tmV, a, stream);
+    if (slopes) return launch_fwd_d<true, true, false, true>(D, tmQ, tmK, tmV, a, stream);
+    if (doc) return launch_fwd_d<true, false, false, true>(D, tmQ, tmK, tmV, a, stream);
+    return launch_fwd_d<false, false, false, true>(D, tmQ, tmK, tmV, a, stream);
   }
-  if (prefix)
-    return D == 64 ? launch_fwd<64, false, false, true>(tmQ, tmK, tmV, a, stream)
-                   : launch_fwd<128, false, false, true>(tmQ, tmK, tmV, a, stream);
-  if (slopes)
-    return D == 64 ? launch_fwd<64, true, true>(tmQ, tmK, tmV, a, stream)
-                   : launch_fwd<128, true, true>(tmQ, tmK, tmV, a, stream);
-  if (doc) return D == 64 ? launch_fwd<64, true>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, true>(tmQ, tmK, tmV, a, stream);
-  return D == 64 ? launch_fwd<64, false>(tmQ, tmK, tmV, a, stream) : launch_fwd<128, false>(tmQ, tmK, tmV, a, stream);
+  if (prefix) return launch_fwd_d<false, false, true>(D, tmQ, tmK, tmV, a, stream);
+  if (slopes) return launch_fwd_d<true, true>(D, tmQ, tmK, tmV, a, stream);
+  if (doc) return launch_fwd_d<true>(D, tmQ, tmK, tmV, a, stream);
+  return launch_fwd_d<false>(D, tmQ, tmK, tmV, a, stream);
 }
 
 }  // namespace
@@ -685,31 +637,8 @@ int b200_attn_fwd_cached(const void* q, const void* k_cache, const void* v_cache
                  "attn_fwd_cached: q, k_cache, v_cache and o must be 16-byte aligned");
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0 && (reinterpret_cast<uintptr_t>(lse) & 3u) == 0,
                  "attn_fwd_cached: slopes and lse must be 4-byte aligned");
-  CUtensorMap tmQ, tmK, tmV;
-  int rc;
-  if ((rc = make_bshd_map(&tmQ, q, B, L, H, D, ATT_BQ))) return rc;
-  if ((rc = make_bshd_map(&tmK, k_cache, B, s_max, Hk, D, ATT_BKV))) return rc;
-  if ((rc = make_bshd_map(&tmV, v_cache, B, s_max, Hk, D, ATT_BKV))) return rc;
-  FwdArgs a{};
-  a.o = reinterpret_cast<__nv_bfloat16*>(o);
-  a.lse = lse;
-  a.B = B;
-  a.S = L;
-  a.H = H;
-  a.Hk = Hk;
-  a.scale = scale;
-  a.causal = 1;
-  a.window = window < 0 || window > s_max ? s_max : window;
-  a.slopes = slopes;
-  a.start = start;
-  a.end = end;
-  a.s_max = s_max;
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (slopes)
-    return D == 64 ? launch_fwd<64, false, true, false, false, true>(tmQ, tmK, tmV, a, s)
-                   : launch_fwd<128, false, true, false, false, true>(tmQ, tmK, tmV, a, s);
-  return D == 64 ? launch_fwd<64, false, false, false, false, true>(tmQ, tmK, tmV, a, s)
-                 : launch_fwd<128, false, false, false, false, true>(tmQ, tmK, tmV, a, s);
+  return attn_fwd_impl(q, k_cache, v_cache, o, lse, false, nullptr, window, B, L, H, Hk, D, scale, 1,
+                       static_cast<cudaStream_t>(stream), slopes, nullptr, false, 0, 1.f, 0, start, end, s_max);
 }
 
 // The rotating KV cache of the reference's generator (core/generation_lite.py:103, :120): a chunk of queries at
@@ -729,32 +658,8 @@ int b200_attn_fwd_ring(const void* q, const void* k_ring, const void* v_ring, co
                  "attn_fwd_ring: q, k_ring, v_ring and o must be 16-byte aligned");
   B200_CHECK_ARG((reinterpret_cast<uintptr_t>(slopes) & 3u) == 0 && (reinterpret_cast<uintptr_t>(lse) & 3u) == 0,
                  "attn_fwd_ring: slopes and lse must be 4-byte aligned");
-  CUtensorMap tmQ, tmK, tmV;
-  int rc;
-  if ((rc = make_bshd_map(&tmQ, q, B, L, H, D, ATT_BQ))) return rc;
-  if ((rc = make_bshd_map(&tmK, k_ring, B, C, Hk, D, ATT_BKV))) return rc;
-  if ((rc = make_bshd_map(&tmV, v_ring, B, C, Hk, D, ATT_BKV))) return rc;
-  FwdArgs a{};
-  a.o = reinterpret_cast<__nv_bfloat16*>(o);
-  a.lse = lse;
-  a.B = B;
-  a.S = L;
-  a.H = H;
-  a.Hk = Hk;
-  a.scale = scale;
-  a.causal = 1;
-  a.window = window < 0 ? INT_MAX : window;
-  a.slopes = slopes;
-  a.start = start;
-  a.end = end;
-  a.s_max = C;
-  a.ring_m = max_kv;
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (slopes)
-    return D == 64 ? launch_fwd<64, false, true, false, false, true, true>(tmQ, tmK, tmV, a, s)
-                   : launch_fwd<128, false, true, false, false, true, true>(tmQ, tmK, tmV, a, s);
-  return D == 64 ? launch_fwd<64, false, false, false, false, true, true>(tmQ, tmK, tmV, a, s)
-                 : launch_fwd<128, false, false, false, false, true, true>(tmQ, tmK, tmV, a, s);
+  return attn_fwd_impl(q, k_ring, v_ring, o, lse, false, nullptr, window, B, L, H, Hk, D, scale, 1,
+                       static_cast<cudaStream_t>(stream), slopes, nullptr, false, 0, 1.f, 0, start, end, C, max_kv);
 }
 
 }  // extern "C"
